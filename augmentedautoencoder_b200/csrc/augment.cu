@@ -134,7 +134,7 @@ __global__ void aug_blur_lut_kernel(const uint8_t* __restrict__ in, int B, int H
 
 inline unsigned aug_grid(long long n) {
   long long b = (n + 255) / 256;
-  return (unsigned)(b < 1 ? 1 : (b > 148 * 32 ? 148 * 32 : b));
+  return (unsigned)(b < 1 ? 1 : (b > 132 * 32 ? 132 * 32 : b));
 }
 
 }  // namespace

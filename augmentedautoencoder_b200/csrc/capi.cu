@@ -65,11 +65,11 @@ void tf_same_pad(int in, int k, int stride, int* before) {
   *before = total / 2;  // TF: pad_before = total // 2, remainder goes after (asymmetric for stride 2)
 }
 
-// Pick a split-K factor so that small-M GEMMs still fill the 148 SMs.
+// Pick a split-K factor so that small-M GEMMs still fill the 132 SMs.
 int choose_splits(int64_t M, int64_t N, int64_t K, size_t partial_cap_floats) {
   const int64_t tiles = ceil_div(M, 128) * ceil_div(N, 128);
   const int64_t chunks = ceil_div(K, 16);
-  if (tiles >= 148 || chunks < 8) return 1;
+  if (tiles >= 132 || chunks < 8) return 1;
   int64_t s = std::min<int64_t>(ceil_div(296, tiles), chunks / 4);
   if (partial_cap_floats > 0) s = std::min<int64_t>(s, (int64_t)(partial_cap_floats / (size_t)(M * N)));
   return (int)std::max<int64_t>(s, 1);
@@ -276,7 +276,7 @@ extern "C" const char* aae_last_error_string(void) { return g_err; }
 extern "C" int aae_device_supported(int device) {
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { cudaGetLastError(); return 0; }
-  return prop.major == 10 ? 1 : 0;
+  return (prop.major == 9 && prop.minor == 0) ? 1 : 0;
 }
 
 static int check_device(int device) {
@@ -974,7 +974,7 @@ static int encoder_dense_backward(aae_trainer* h, const float* flat, int B, floa
 }
 
 // Training step on the tensor cores: forward through the split-fp16 plans (their (hi, lo) activations double as the ReLU
-// masks and the wgrad operands), conv backward as tcgen05 GEMMs (tc_train.cu), the two dense layers, conv1's wgrad (K = 75)
+// masks and the wgrad operands), conv backward as wgmma GEMMs (tc_train.cu), the two dense layers, conv1's wgrad (K = 75)
 // and the elementwise pieces on the fp32 kernels.
 static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, int B, float* loss_out, cudaStream_t s) {
   aae_encoder* E = h->enc;

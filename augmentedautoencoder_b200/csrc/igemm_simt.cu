@@ -1,7 +1,7 @@
 // SIMT fp32 implicit-GEMM: the exact-order (IEEE FMA chain) path for every dense contraction of the
 // AAE hot path -- conv forward (auto_pose/ae/encoder.py:43-50, decoder.py:56-62), dense layers
 // (encoder.py:62-66, decoder.py:44-51) and their backward passes (TF autodiff behind
-// auto_pose/ae/ae_factory.py:86-88).  It is the correctness anchor for the tcgen05 kernels and the
+// auto_pose/ae/ae_factory.py:86-88).  It is the correctness anchor for the tensor-core kernels and the
 // arithmetic of AAE_PREC_FP32_SIMT.
 //
 // One kernel, three gather modes (common.cuh):  C[M,N] = sum_k A[m,k] * Bm[k,n]

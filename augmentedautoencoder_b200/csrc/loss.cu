@@ -3,7 +3,7 @@
 // and its gradient wrt x: 2 (x - target) / (B k) on the selected elements, 0 elsewhere.
 //
 // One CTA per sample keeps the whole squared-error row in shared memory (49 152 floats = 192 KB of the
-// 227 KB a B200 SM offers) and finds the k-th largest value with a 4-pass 8-bit radix select on the
+// 227 KB an H100 SM offers) and finds the k-th largest value with a 4-pass 8-bit radix select on the
 // float bit patterns (non-negative floats order like unsigned integers) -- no sort, one HBM read of x
 // and target, one HBM write of the gradient.  tf.nn.top_k is stable: among equal values the lower index
 // wins, so ties at the threshold are admitted in index order.

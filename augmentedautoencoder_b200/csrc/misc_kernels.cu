@@ -402,7 +402,7 @@ __global__ void l2_normalize_kernel(const float* __restrict__ z, int B, int J, f
   for (int j = lane; j < J; j += 32) out[(long long)row * J + j] = z[(long long)row * J + j] * inv;
 }
 
-inline unsigned grid_for(long long n, int threads, int cap = 148 * 16) {
+inline unsigned grid_for(long long n, int threads, int cap = 132 * 16) {
   long long b = (n + threads - 1) / threads;
   if (b > cap) b = cap;
   if (b < 1) b = 1;
@@ -487,7 +487,7 @@ int launch_conv1_wgrad(const float* x, const float* dy, int B, int H, int W, int
   const int PW = 2 * OW + 3, PH = 2 * C1W_RB + 3;
   const size_t smem = ((size_t)((PH * PW * 3 + 3) & ~3) + 2 * C1W_CH * C1W_N) * sizeof(float);
   const int tiles = B * (OH / C1W_RB);
-  int grid = std::min(tiles, 2 * 148);
+  int grid = std::min(tiles, 2 * 132);
   grid = (int)std::min<size_t>((size_t)grid, partial_floats / (C1W_K * C1W_N));
   AAE_REQUIRE(grid >= 1, "conv1 wgrad: partial scratch too small");
   AAE_CUDA_OK(cudaFuncSetAttribute(conv1_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05 / TMEM / TMA) execution plans behind AAE_PREC_TC_SPLIT.  Internal to the library.
+// Tensor-core (wgmma / TMA) execution plans behind AAE_PREC_TC_SPLIT.  Internal to the library.
 #pragma once
 #include "common.cuh"
 

@@ -1,4 +1,4 @@
-// First encoder layer on tcgen05 (AAE_PREC_TC_SPLIT): conv 5x5 / stride 2 / TF-SAME(1,2), Cin = 3 -> Cout = 128, + bias +
+// First encoder layer on wgmma (AAE_PREC_TC_SPLIT): conv 5x5 / stride 2 / TF-SAME(1,2), Cin = 3 -> Cout = 128, + bias +
 // ReLU  (auto_pose/ae/encoder.py:43-50, first loop iteration), fused with the x/255. of auto_pose/ae/codebook.py:58-59.
 //
 // K = 25*3 = 75 is far too small and too ragged for TMA (patches overlap, 3-byte pixels), so the A operand is built in
@@ -7,8 +7,8 @@
 // the kernel, so the fused path is bit-identical to the reference's float feed), and the row is written in the
 // 128-byte-swizzle K-major canonical layout.  K is padded to 80 = 5 MMA K-steps.  The packed weights ([128][128] K-major,
 // zero beyond k = 75) are TMA-loaded once per CTA and stay resident.  Persistent CTAs loop over 128-pixel tiles with a
-// single-stage A buffer and a double-buffered TMEM accumulator: builders (warps 0-3), epilogue (warps 4-11, two per TMEM
-// lane quadrant) and the MMA issuer (warp 12) all overlap.  The epilogue writes conv2's input directly: (hi, lo) fp16, space-to-depth layout.
+// single-stage A buffer: builders (warps 0-3) run a tile ahead of the two MMA + epilogue warpgroups (warps 4-11); warp 12
+// loads the weights.  The epilogue writes conv2's input directly: (hi, lo) fp16, space-to-depth layout.
 #include <stdlib.h>
 
 #include <algorithm>
@@ -27,7 +27,7 @@ constexpr int C1_STAGE = 4 * C1_ATOM;              // hi k[0,64), hi k[64,128), 
 constexpr int C1_STAGES = 1;                       // the build (~0.4k cycles) is short next to the MMAs + epilogue; smem goes to the output staging
 constexpr int C1_OUT_LD = 1040;                    // staged output: 32 blocks of 1 KB (one space-to-depth position each), padded against bank conflicts
 constexpr int C1_KPAD = 80;
-constexpr int C1_EPI_WARPS = 8;                    // two per TMEM lane quadrant (each takes every other 32-channel chunk)
+constexpr int C1_EPI_WARPS = 8;                    // two warpgroups: wgmma for 64 pixels of the tile each, then their epilogue
 constexpr int C1_MMA_WARP = 4 + C1_EPI_WARPS;
 constexpr int C1_THREADS = 32 * (C1_MMA_WARP + 1);
 constexpr int C1_PIX_ROWS = 7;                     // input rows feeding two output rows: 2*2 + 3
@@ -45,7 +45,6 @@ struct Conv1Params {
   __half* out_hi;
   __half* out_lo;
   unsigned* range_flag;    // run-time range guard (tc_plan.cuh): bit 0 = this layer's activation overflowed fp16 at out_scale
-  long long* trace;        // AAE_C1_TRACE: clock64 stamps of CTA 0 (first 12 tiles): [i*8 + 0..2] builder start / stage free / tile built, +3,4 MMA issuer got accumulator / operands, +5,6 epilogue warp 4 start / end
 };
 
 template <int N>
@@ -83,13 +82,9 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
   uint64_t* w_full = reinterpret_cast<uint64_t*>(raw_smem + S::RAW_BYTES);
   uint64_t* a_full = w_full + 1;
   uint64_t* a_empty = a_full + C1_STAGES;
-  uint64_t* acc_full = a_empty + C1_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_empty + 2);
   __shared__ float bias_s[N];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr int TMEM_COLS = 2 * N < 32 ? 32 : 2 * N;
   if (threadIdx.x < N) bias_s[threadIdx.x] = p.bias[threadIdx.x];
 
   if (threadIdx.x < 256) {
@@ -103,15 +98,10 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
   if (warp == C1_MMA_WARP && lane == 0) {
     prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_w_lo);
     mbar_init(w_full, 1);
-    for (int s = 0; s < C1_STAGES; ++s) { mbar_init(&a_full[s], 128); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], C1_EPI_WARPS); }
+    for (int s = 0; s < C1_STAGES; ++s) { mbar_init(&a_full[s], 128); mbar_init(&a_empty[s], 2); }
     fence_barrier_init();
   }
-  if (warp == C1_MMA_WARP) tmem_alloc<TMEM_COLS>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const int my_tiles = (p.num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
   const int hw = p.OH * p.OW;
 
@@ -208,53 +198,69 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
       asm volatile("bar.sync 1, 128;" ::: "memory");       // staged rows of tile i+1 visible to all builders
     }
   } else if (warp < C1_MMA_WARP) {
-    // ===================== epilogue =====================
+    // ===================== wgmma + epilogue (two warpgroups, pixels [0,64) and [64,128) of the tile) =====================
     // The 128 pixels x 128 channels of a tile (two output rows of one image) are exactly ONE contiguous 32 KB slab of the
-    // consumer's space-to-depth tensor (row oh/2, all 32 column pairs, all four parities) -- per (hi, lo).  Each thread
-    // (= pixel) writes its 256 B into a padded shared-memory image of that slab; one thread then ships it with 1 KB bulk
+    // consumer's space-to-depth tensor (row oh/2, all 32 column pairs, all four parities) -- per (hi, lo).  Each thread writes
+    // its accumulator fragment into a padded shared-memory image of that slab; one thread then ships it with 1 KB bulk
     // stores, i.e. full-line HBM writes instead of 16-byte scattered ones.
-    const int q = warp & 3, half = (warp - 4) >> 2, r = q * 32 + lane;
-    const int ow = r % p.OW, dr = r / p.OW;
-    // blocks are grouped G at a time (contiguous, one bulk store per group); 16 bytes of padding after every group
+    const int wg = (warp - 4) >> 2;
     const int G = p.out_group, grp_ld = G * 8 * N + 16;
-    uint8_t* my_hi = out_smem + ((ow >> 1) / G) * grp_ld + ((ow >> 1) % G) * (8 * N) + (((dr & 1) << 1) | (ow & 1)) * (2 * N);
-    uint8_t* my_lo = my_hi + 32 * C1_OUT_LD;
+    uint8_t* my_hi[2];
+#pragma unroll
+    for (int h2 = 0; h2 < 2; ++h2) {                 // the thread's two fragment rows
+      const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h2;
+      const int ow = r % p.OW, dr = r / p.OW;
+      // blocks are grouped G at a time (contiguous, one bulk store per group); 16 bytes of padding after every group
+      my_hi[h2] = out_smem + ((ow >> 1) / G) * grp_ld + ((ow >> 1) % G) * (8 * N) + (((dr & 1) << 1) | (ow & 1)) * (2 * N);
+    }
+    mbar_wait(w_full, 0);
+    const uint32_t wst = smem_u32(w_smem);
+    float acc[N / 2];
     for (int i = 0; i < my_tiles; ++i) {
-      const int as = i & 1;
+      const int s = i % C1_STAGES;
       const int m_first = ((int)blockIdx.x + i * (int)gridDim.x) * 128;
       const int b = m_first / hw, oh0 = (m_first - b * hw) / p.OW;
-      mbar_wait(&acc_full[as], (uint32_t)(i >> 1) & 1u);
-      tc_fence_after();
+      mbar_wait(&a_full[s], (uint32_t)(i / C1_STAGES) & 1u);
+      const uint32_t ast = smem_u32(a_smem + s * C1_STAGE) + (uint32_t)(wg * 64 * 128);
+      wgmma_fence_regs(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < C1_KPAD / 16; ++k) {
+        const int atom = k >> 2, kk = k & 3;
+        const uint64_t a_hi = desc_advance_k(make_sw128_kmajor_desc(ast + atom * C1_ATOM), kk);
+        const uint64_t a_lo = desc_advance_k(make_sw128_kmajor_desc(ast + (2 + atom) * C1_ATOM), kk);
+        const uint64_t w_hi = desc_advance_k(make_sw128_kmajor_desc(wst + atom * N * 128), kk);
+        const uint64_t w_lo = desc_advance_k(make_sw128_kmajor_desc(wst + (2 + atom) * N * 128), kk);
+        Wgmma<N>::template ss<0, 0>(acc, a_lo, w_hi, k > 0 ? 1u : 0u);
+        Wgmma<N>::template ss<0, 0>(acc, a_hi, w_lo, 1u);
+        Wgmma<N>::template ss<0, 0>(acc, a_hi, w_hi, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if ((warp & 3) == 0 && lane == 0) mbar_arrive(&a_empty[s]);
       if (i > 0) {                                   // the previous tile's bulk stores must have finished reading the staging
         if (warp == 4) bulk_wait_read_all();
-        asm volatile("bar.sync 2, %0;" ::"n"(32 * C1_EPI_WARPS) : "memory");
+        named_bar_sync(2, 32 * C1_EPI_WARPS);
       }
-#pragma unroll 1
-      for (int c = half; c < N / 32; c += C1_EPI_WARPS / 4) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * N + c * 32), v);
-        tmem_ld_wait();
-        uint32_t hi[16], lo[16];
-        float amax = 0.f;
+      float amax = 0.f;
 #pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          const float a = fmaxf(__uint_as_float(v[j]) * p.unscale + bias_s[c * 32 + j], 0.f) * p.out_scale;
-          const float bb = fmaxf(__uint_as_float(v[j + 1]) * p.unscale + bias_s[c * 32 + j + 1], 0.f) * p.out_scale;
+      for (int j = 0; j < N / 8; ++j) {
+        const int c = 8 * j + 2 * (lane & 3);
+#pragma unroll
+        for (int h2 = 0; h2 < 2; ++h2) {
+          const float a = fmaxf(acc[4 * j + 2 * h2] * p.unscale + bias_s[c], 0.f) * p.out_scale;
+          const float bb = fmaxf(acc[4 * j + 2 * h2 + 1] * p.unscale + bias_s[c + 1], 0.f) * p.out_scale;
           amax = fmaxf(amax, fmaxf(a, bb));
-          split_f16x2(a, bb, hi[j >> 1], lo[j >> 1]);
-        }
-        if (p.range_flag != nullptr && !(amax < 65520.f)) atomicOr(p.range_flag, 1u);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          *reinterpret_cast<uint4*>(my_hi + c * 64 + j * 16) = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-          *reinterpret_cast<uint4*>(my_lo + c * 64 + j * 16) = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
+          uint32_t hi, lo;
+          split_f16x2(a, bb, hi, lo);
+          *reinterpret_cast<uint32_t*>(my_hi[h2] + c * 2) = hi;
+          *reinterpret_cast<uint32_t*>(my_hi[h2] + 32 * C1_OUT_LD + c * 2) = lo;
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[as]);
+      if (p.range_flag != nullptr && !(amax < 65520.f)) atomicOr(p.range_flag, 1u);
       fence_proxy_async_smem();                      // generic-proxy writes -> visible to the bulk-copy engine
-      asm volatile("bar.sync 2, %0;" ::"n"(32 * C1_EPI_WARPS) : "memory");
+      named_bar_sync(2, 32 * C1_EPI_WARPS);
       if (warp == 4 && b < p.B) {                    // lane j ships group j (G KB) of the hi and of the lo slab
         const long long slab = ((long long)(b * (p.OH >> 1) + (oh0 >> 1)) * (p.OW >> 1)) * (4LL * N);   // elements
         if (lane < 32 / G) {
@@ -266,44 +272,14 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
     }
     if (warp == 4) bulk_wait_all();                    // all stores landed before the CTA exits
   } else {
-    // ===================== weight TMA + MMA issuer (last warp) =====================
+    // ===================== weight TMA (last warp) =====================
     if (lane == 0) {
       mbar_arrive_expect_tx(w_full, S::W_BYTES);
       tma_load_2d(w_smem, &tm_w_hi, w_full, 0, 0);
       tma_load_2d(w_smem + N * 128, &tm_w_hi, w_full, 64, 0);
       tma_load_2d(w_smem + 2 * N * 128, &tm_w_lo, w_full, 0, 0);
       tma_load_2d(w_smem + 3 * N * 128, &tm_w_lo, w_full, 64, 0);
-      mbar_wait(w_full, 0);
-      constexpr uint32_t idesc = make_idesc_f16(128, N, 0);
-      const uint32_t wst = smem_u32(w_smem);
-      for (int i = 0; i < my_tiles; ++i) {
-        const int s = i % C1_STAGES, as = i & 1;
-        mbar_wait(&acc_empty[as], ((uint32_t)(i >> 1) & 1u) ^ 1u);
-        mbar_wait(&a_full[s], (uint32_t)(i / C1_STAGES) & 1u);
-        tc_fence_after();
-        const uint32_t ast = smem_u32(a_smem + s * C1_STAGE);
-        const uint32_t d = tmem_base + (uint32_t)(as * N);
-#pragma unroll
-        for (int k = 0; k < C1_KPAD / 16; ++k) {
-          const int atom = k >> 2, kk = k & 3;
-          const uint64_t a_hi = desc_advance_k(make_sw128_kmajor_desc(ast + atom * C1_ATOM), kk);
-          const uint64_t a_lo = desc_advance_k(make_sw128_kmajor_desc(ast + (2 + atom) * C1_ATOM), kk);
-          const uint64_t w_hi = desc_advance_k(make_sw128_kmajor_desc(wst + atom * N * 128), kk);
-          const uint64_t w_lo = desc_advance_k(make_sw128_kmajor_desc(wst + (2 + atom) * N * 128), kk);
-          umma_f16(d, a_lo, w_hi, idesc, k > 0 ? 1u : 0u);
-          umma_f16(d, a_hi, w_lo, idesc, 1u);
-          umma_f16(d, a_hi, w_hi, idesc, 1u);
-        }
-        umma_commit(&a_empty[s]);
-        umma_commit(&acc_full[as]);
-      }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == C1_MMA_WARP) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
   }
 }
 
@@ -319,10 +295,9 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
 //     10 STS.128 per builder thread and tile (before: 80 + 20), bank-conflict free (lane -> pixel order below, 800-byte rows);
 //   * the staged input rows are fp16 written straight from the 16-byte global loads (byte -> fp16 is two PRMT + two HSUB2
 //     per four bytes), double buffered; the A tile is double buffered too, so builders run a tile ahead of the MMAs;
-//   * TMEM lane r is output "slot" r of the tile's 32 KB slab of conv2's space-to-depth input (slot = (ow/2)*4 + (oh%2)*2 +
-//     ow%2), so the staged output tile is the slab in order; it is written in the 128-byte-swizzle layout (conflict-free
-//     STS.128) and leaves through eight 8 KB TMA tensor stores per tile, issued in two phases so that the staging double-buffers
-//     itself (instead of 32 bulk copies behind a full stop).
+//   * accumulator row r is output "slot" r of the tile's 32 KB slab of conv2's space-to-depth input (slot = (ow/2)*4 + (oh%2)*2 +
+//     ow%2), so the staged output tile is the slab in order; every warp stages its 16 slots in the 64-byte-swizzle layout and
+//     ships them with its own TMA tensor stores (instead of 32 bulk copies behind a full stop).
 constexpr int U8_A_STAGES = 2;
 constexpr int U8_A_STAGE = 2 * C1_ATOM;           // K slots [0,64) and [64,80): two 128-row x 128-byte atoms
 constexpr int U8_PIX_LD = 400;                    // fp16 elements per staged input row: 8 lead-in + 384 data + 8 tail
@@ -330,8 +305,6 @@ constexpr int U8_PIX_BUF = C1_PIX_ROWS * U8_PIX_LD * 2;   // bytes
 constexpr int U8_W_BYTES = 4 * C1_ATOM;
 constexpr int U8_OUT_BYTES = 4 * C1_ATOM;         // hi ch[0,64), hi ch[64,128), lo ch[0,64), lo ch[64,128): 128 slots x 128 B each
 constexpr int U8_SMEM_TOTAL = U8_W_BYTES + U8_A_STAGES * U8_A_STAGE + U8_OUT_BYTES + 2 * U8_PIX_BUF + 1024 /*align*/ + 256 /*barriers*/;
-
-__device__ __forceinline__ void bulk_wait_read_1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
 
 // four bytes -> four fp16 (exact): 0x6400 | b is the fp16 1024 + b, minus 1024
 __device__ __forceinline__ void bytes_to_half4(uint32_t x, uint32_t& lo2, uint32_t& hi2) {
@@ -342,13 +315,11 @@ __device__ __forceinline__ void bytes_to_half4(uint32_t x, uint32_t& lo2, uint32
   hi2 = *reinterpret_cast<const uint32_t*>(&hb);
 }
 
-// Epilogue warps of the uint8 kernel: 16 (four per TMEM lane quadrant, one 32-channel chunk of the tile each) or 8 (two chunks each).
-// In-kernel trace (profiles/r02_conv1_trace.txt): the epilogue paces the kernel -- one chunk costs a warp ~1.7 k cycles of mostly
-// latency (TMEM load, split, proxy fence, tensor-store issue), the builders and the MMAs are far ahead.
-constexpr int U8_MAX_EPI_WARPS = 16;
-constexpr int U8_MAX_THREADS = 32 * (4 + U8_MAX_EPI_WARPS + 1);
+// The uint8 kernel's MMA + epilogue warps: two warpgroups, 64 slots of the tile each.
+constexpr int U8_EPI_WARPS = 8;
+constexpr int U8_THREADS = 32 * (4 + U8_EPI_WARPS + 1);
 
-__global__ void __launch_bounds__(U8_MAX_THREADS, 1)
+__global__ void __launch_bounds__(U8_THREADS, 1)
 tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo,
                    const __grid_constant__ CUtensorMap tm_out_hi, const __grid_constant__ CUtensorMap tm_out_lo, const Conv1Params p) {
   constexpr int N = 128, CIN = 3;
@@ -361,28 +332,19 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
   uint64_t* w_full = reinterpret_cast<uint64_t*>(pix + 2 * U8_PIX_BUF);
   uint64_t* a_full = w_full + 1;
   uint64_t* a_empty = a_full + U8_A_STAGES;
-  uint64_t* acc_full = a_empty + U8_A_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_empty + 2);
   __shared__ float bias_s[N];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_epi = ((int)blockDim.x >> 5) - 5, mma_warp = 4 + n_epi;      // 8 or 16 epilogue warps, then the issuer warp
-  constexpr int TMEM_COLS = 2 * N;
+  constexpr int mma_warp = 4 + U8_EPI_WARPS;                  // the weight loader
   if (threadIdx.x < N) bias_s[threadIdx.x] = p.bias[threadIdx.x] * p.out_scale;     // relu(x) * s == relu(x * s) for s > 0
   for (int i = threadIdx.x; i < 2 * U8_PIX_BUF / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(pix)[i] = 0u;   // lead-in / tail stay zero
   if (warp == mma_warp && lane == 0) {
     prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_w_lo); prefetch_tmap(&tm_out_hi); prefetch_tmap(&tm_out_lo);
     mbar_init(w_full, 1);
-    for (int s = 0; s < U8_A_STAGES; ++s) { mbar_init(&a_full[s], 128); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], n_epi); }
+    for (int s = 0; s < U8_A_STAGES; ++s) { mbar_init(&a_full[s], 128); mbar_init(&a_empty[s], 2); }
     fence_barrier_init();
   }
-  if (warp == mma_warp) tmem_alloc<TMEM_COLS>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const int my_tiles = (p.num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
   const int hw = p.OH * p.OW;
 
@@ -431,15 +393,12 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
     for (int i = 0; i < my_tiles; ++i) {
       const int s = i % U8_A_STAGES;
       const bool more = i + 1 < my_tiles;
-      const bool tr = p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 0 && i < 12;
-      if (tr) p.trace[i * 8 + 0] = clock64();
       if (more) fetch((int)blockIdx.x + (i + 1) * (int)gridDim.x);
       // kernel row kh of this pixel's patch = elements [4 + 6*ow, +16) of staged row 2*dr + kh: slot 0 is the element before the
       // patch (zero weight), slots 1..15 the 5 x 3 taps
       const uint8_t* src = pix + (i & 1) * U8_PIX_BUF + (2 * dr) * (U8_PIX_LD * 2) + (4 + 6 * ow) * 2;
       mbar_wait(&a_empty[s], ((uint32_t)(i / U8_A_STAGES) & 1u) ^ 1u);
       uint8_t* st = a_smem + s * U8_A_STAGE;
-      if (tr) p.trace[i * 8 + 1] = clock64();
 #pragma unroll
       for (int kh = 0; kh < 5; ++kh) {
         const uint32_t* q = reinterpret_cast<const uint32_t*>(src + kh * (U8_PIX_LD * 2));
@@ -451,111 +410,86 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
       }
       fence_proxy_async_smem();
       mbar_arrive(&a_full[s]);
-      if (tr) p.trace[i * 8 + 2] = clock64();
       if (more) stage(pix + ((i + 1) & 1) * U8_PIX_BUF);    // that buffer's last readers (tile i-1) passed the barrier below an iteration ago
       asm volatile("bar.sync 1, 128;" ::: "memory");
     }
   } else if (warp < mma_warp) {
-    // ===================== epilogue: TMEM -> bias + ReLU + (hi, lo) split -> swizzled staging -> TMA tensor stores =====================
-    // Warp (q, g) owns the tile's slots [32 q, 32 q + 32) and the 32-channel chunks g, g + groups, ... (groups = n_epi / 4: one
-    // chunk per tile with sixteen warps, two with eight).  A chunk goes through 4 KB of the warp's own staging (hi 2 KB, lo 2 KB,
-    // 64-byte rows, 64-byte swizzle: conflict-free STS.128 from a thread-per-slot warp) and is shipped by the warp's own lane 0, so
-    // the tile's tensor stores are issued by n_epi lanes in parallel and no barrier couples the warps.  Sixteen warps: one buffer,
-    // reused a whole tile later; eight warps: one buffer per chunk, the stores of one drain under the math of the other.
-    const int q = warp & 3, g = (warp - 4) >> 2, groups = n_epi >> 2, per_warp = 4 / groups;
+    // ===================== wgmma + epilogue -> bias + ReLU + (hi, lo) split -> swizzled staging -> TMA tensor stores =====================
+    // Warpgroup wg computes slots [64 wg, 64 wg + 64) of the tile; warp (wg, w) holds slots [64 wg + 16 w, +16) x 128 channels in
+    // registers.  Each of its four 32-channel chunks goes through 2 KB of the warp's own staging (hi 1 KB, lo 1 KB, 64-byte rows,
+    // 64-byte swizzle) and is shipped by the warp's own lane 0 as a 16-slot x 32-channel tensor store, so no barrier couples the
+    // warps; the buffer is reused a tile later, once the engine has read it.
+    const int wg = (warp - 4) >> 2, w4 = warp & 3;
     const float us = p.unscale * p.out_scale;
-    const int rsw = (lane >> 1) & 3;
-    uint8_t* wbuf = out_smem + (warp - 4) * (U8_OUT_BYTES / n_epi);
-    int ph = 0;
+    uint8_t* wbuf = out_smem + (warp - 4) * (U8_OUT_BYTES / U8_EPI_WARPS);
+    mbar_wait(w_full, 0);
+    const uint32_t wst = smem_u32(w_smem);
+    float acc[N / 2];
     for (int i = 0; i < my_tiles; ++i) {
-      const int as = i & 1;
+      const int s = i % U8_A_STAGES;
       const int tile = (int)blockIdx.x + i * (int)gridDim.x;
-      mbar_wait(&acc_full[as], (uint32_t)(i >> 1) & 1u);
-      tc_fence_after();
-      const bool tr = p.trace != nullptr && blockIdx.x == 0 && threadIdx.x == 128 && i < 12;
-      if (tr) p.trace[i * 8 + 5] = clock64();
-#pragma unroll 1
-      for (int cc = 0; cc < per_warp; ++cc, ++ph) {
-        const int c0 = (g + cc * groups) * 32;           // first channel of this chunk
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * N + c0), v);
-        tmem_ld_wait();
-        if (cc == per_warp - 1) {                        // this warp's TMEM columns have been read: the accumulator may be overwritten
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_empty[as]);
-        }
-        uint32_t hi[16], lo[16];
-        float amax = 0.f;
+      mbar_wait(&a_full[s], (uint32_t)(i / U8_A_STAGES) & 1u);
+      const uint32_t ast = smem_u32(a_smem + s * U8_A_STAGE) + (uint32_t)(wg * 64 * 128);
+      wgmma_fence_regs(acc);
+      wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          const float a = fmaxf(fmaf(__uint_as_float(v[j]), us, bias_s[c0 + j]), 0.f);
-          const float bb = fmaxf(fmaf(__uint_as_float(v[j + 1]), us, bias_s[c0 + j + 1]), 0.f);
-          amax = fmaxf(amax, fmaxf(a, bb));
-          split_f16x2(a, bb, hi[j >> 1], lo[j >> 1]);
-        }
-        if (p.range_flag != nullptr && !(amax < 65520.f)) atomicOr(p.range_flag, 1u);
-        if (ph >= per_warp) {                            // the buffer was shipped per_warp chunks ago: only newer groups may still be unread
-          if (lane == 0) { if (per_warp == 2) bulk_wait_read_1(); else bulk_wait_read_all(); }
-          __syncwarp();
-        }
-        uint8_t* sb = wbuf + cc * 4096;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int ch = (j ^ rsw) << 4;
-          *reinterpret_cast<uint4*>(sb + lane * 64 + ch) = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-          *reinterpret_cast<uint4*>(sb + 2048 + lane * 64 + ch) = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
-        }
-        fence_proxy_async_smem();                        // generic-proxy writes -> visible to the TMA engine
+      for (int k = 0; k < C1_KPAD / 16; ++k) {
+        const int atom = k >> 2, kk = k & 3;
+        const uint64_t a = desc_advance_k(make_sw128_kmajor_desc(ast + atom * C1_ATOM), kk);
+        const uint64_t w_hi = desc_advance_k(make_sw128_kmajor_desc(wst + atom * C1_ATOM), kk);
+        const uint64_t w_lo = desc_advance_k(make_sw128_kmajor_desc(wst + (2 + atom) * C1_ATOM), kk);
+        Wgmma<N>::template ss<0, 0>(acc, a, w_lo, k > 0 ? 1u : 0u);
+        Wgmma<N>::template ss<0, 0>(acc, a, w_hi, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (w4 == 0 && lane == 0) mbar_arrive(&a_empty[s]);
+      if (i > 0) {                                       // the previous tile's stores have read this warp's staging
+        if (lane == 0) bulk_wait_read_all();
         __syncwarp();
-        if (lane == 0) {
-          tma_store_2d(&tm_out_hi, sb, c0, tile * 128 + q * 32);
-          tma_store_2d(&tm_out_lo, sb + 2048, c0, tile * 128 + q * 32);
-          bulk_commit_group();
+      }
+      float amax = 0.f;
+#pragma unroll
+      for (int j = 0; j < N / 8; ++j) {
+        const int c = 8 * j + 2 * (lane & 3);
+        uint8_t* sb = wbuf + (j >> 2) * 2048;            // chunk j / 4
+#pragma unroll
+        for (int h2 = 0; h2 < 2; ++h2) {
+          const int rr = (lane >> 2) + 8 * h2;           // slot within the warp's 16
+          const float a = fmaxf(fmaf(acc[4 * j + 2 * h2], us, bias_s[c]), 0.f);
+          const float bb = fmaxf(fmaf(acc[4 * j + 2 * h2 + 1], us, bias_s[c + 1]), 0.f);
+          amax = fmaxf(amax, fmaxf(a, bb));
+          uint32_t hi, lo;
+          split_f16x2(a, bb, hi, lo);
+          const int off = rr * 64 + (((j & 3) ^ ((rr >> 1) & 3)) << 4) + 4 * (lane & 3);
+          *reinterpret_cast<uint32_t*>(sb + off) = hi;
+          *reinterpret_cast<uint32_t*>(sb + 1024 + off) = lo;
         }
       }
-      if (tr) p.trace[i * 8 + 6] = clock64();
+      if (p.range_flag != nullptr && !(amax < 65520.f)) atomicOr(p.range_flag, 1u);
+      fence_proxy_async_smem();                          // generic-proxy writes -> visible to the TMA engine
+      __syncwarp();
+      if (lane == 0) {
+        const int slot0 = tile * 128 + wg * 64 + w4 * 16;
+#pragma unroll
+        for (int cc = 0; cc < N / 32; ++cc) {
+          tma_store_2d(&tm_out_hi, wbuf + cc * 2048, cc * 32, slot0);
+          tma_store_2d(&tm_out_lo, wbuf + cc * 2048 + 1024, cc * 32, slot0);
+        }
+        bulk_commit_group();
+      }
     }
     if (lane == 0) bulk_wait_all();                      // all stores landed before the CTA exits
   } else {
-    // ===================== weight TMA + MMA issuer (last warp) =====================
+    // ===================== weight TMA (last warp) =====================
     if (lane == 0) {
       mbar_arrive_expect_tx(w_full, U8_W_BYTES);
       tma_load_2d(w_smem, &tm_w_hi, w_full, 0, 0);
       tma_load_2d(w_smem + C1_ATOM, &tm_w_hi, w_full, 64, 0);
       tma_load_2d(w_smem + 2 * C1_ATOM, &tm_w_lo, w_full, 0, 0);
       tma_load_2d(w_smem + 3 * C1_ATOM, &tm_w_lo, w_full, 64, 0);
-      mbar_wait(w_full, 0);
-      constexpr uint32_t idesc = make_idesc_f16(128, N, 0);
-      const uint32_t wst = smem_u32(w_smem);
-      for (int i = 0; i < my_tiles; ++i) {
-        const int s = i % U8_A_STAGES, as = i & 1;
-        mbar_wait(&acc_empty[as], ((uint32_t)(i >> 1) & 1u) ^ 1u);
-        if (p.trace != nullptr && blockIdx.x == 0 && i < 12) p.trace[i * 8 + 3] = clock64();
-        mbar_wait(&a_full[s], (uint32_t)(i / U8_A_STAGES) & 1u);
-        if (p.trace != nullptr && blockIdx.x == 0 && i < 12) p.trace[i * 8 + 4] = clock64();
-        tc_fence_after();
-        const uint32_t ast = smem_u32(a_smem + s * U8_A_STAGE);
-        const uint32_t d = tmem_base + (uint32_t)(as * N);
-#pragma unroll
-        for (int k = 0; k < C1_KPAD / 16; ++k) {
-          const int atom = k >> 2, kk = k & 3;
-          const uint64_t a = desc_advance_k(make_sw128_kmajor_desc(ast + atom * C1_ATOM), kk);
-          const uint64_t w_hi = desc_advance_k(make_sw128_kmajor_desc(wst + atom * C1_ATOM), kk);
-          const uint64_t w_lo = desc_advance_k(make_sw128_kmajor_desc(wst + (2 + atom) * C1_ATOM), kk);
-          umma_f16(d, a, w_lo, idesc, k > 0 ? 1u : 0u);
-          umma_f16(d, a, w_hi, idesc, 1u);
-        }
-        umma_commit(&a_empty[s]);
-        umma_commit(&acc_full[as]);
-      }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == mma_warp) {
-    tc_fence_after();
-    tmem_dealloc<TMEM_COLS>(tmem_base);
   }
 }
 
@@ -659,7 +593,6 @@ int tc_conv1_pack(TcConv1* h, const float* w_dev, int K, float w_scale, unsigned
 int tc_conv1_forward(TcConv1* h, const aae_net_cfg* cfg, const void* crops, int src_u8, int B, const float* bias, float act_scale,
                      float w_scale, __half* out_hi, __half* out_lo, unsigned* range_flag, cudaStream_t s) {
   Conv1Params p;
-  p.trace = nullptr;
   p.range_flag = range_flag;
   p.x = crops; p.B = B; p.H = cfg->in_h; p.W = cfg->in_w; p.C = cfg->in_c;
   p.OH = cfg->in_h / 2; p.OW = cfg->in_w / 2; p.N = h->N;
@@ -682,31 +615,13 @@ int tc_conv1_forward(TcConv1* h, const aae_net_cfg* cfg, const void* crops, int 
     if (h->bound_hi != out_hi || h->bound_lo != out_lo || h->slots != slots) {
       const uint64_t dims[2] = {128, (uint64_t)slots};
       const uint64_t strides[1] = {256};
-      const uint32_t box32[2] = {32, 32};                   // one warp's 32 slots x 32 channels, 64-byte swizzle
+      const uint32_t box32[2] = {32, 16};                   // one warp's 16 slots x 32 channels, 64-byte swizzle
       AAE_TRY(make_tmap_f16(&h->tm_out32_hi, out_hi, 2, dims, strides, box32, 64));
       AAE_TRY(make_tmap_f16(&h->tm_out32_lo, out_lo, 2, dims, strides, box32, 64));
       h->bound_hi = out_hi; h->bound_lo = out_lo; h->slots = slots;
     }
     p.unscale = 1.f / (w_scale * 256.f);              // accumulators hold sum u8 * (w * w_scale * 256 / 255)
-    const char* epi8 = getenv("AAE_C1_EPI8");               // read per launch (scripts/ab_inproc.py): "1" = eight epilogue warps
-    const int u8_threads = 32 * (4 + ((epi8 && epi8[0] == '1') ? 8 : U8_MAX_EPI_WARPS) + 1);
-    static long long* trace_dev = nullptr;
-    p.trace = nullptr;
-    if (getenv("AAE_C1_TRACE")) {
-      if (!trace_dev) cudaMalloc(&trace_dev, 96 * sizeof(long long));
-      cudaMemsetAsync(trace_dev, 0, 96 * sizeof(long long), s);
-      p.trace = trace_dev;
-    }
-    tc_conv1_u8_kernel<<<grid, u8_threads, U8_SMEM_TOTAL, s>>>(h->tm8_hi, h->tm8_lo, h->tm_out32_hi, h->tm_out32_lo, p);
-    if (p.trace) {
-      long long t[96];
-      cudaStreamSynchronize(s);
-      cudaMemcpy(t, p.trace, sizeof(t), cudaMemcpyDeviceToHost);
-      fprintf(stderr, "[conv1 trace, CTA 0, clocks from the first builder stamp] tile: builder start | stage free | built || issuer: accumulator free | operands ready || epilogue warp 4: start | end\n");
-      for (int i = 0; i < 12; ++i)
-        fprintf(stderr, "  tile %2d: %6lld | %6lld | %6lld || %6lld | %6lld || %6lld | %6lld\n", i, t[i * 8] - t[0], t[i * 8 + 1] - t[0], t[i * 8 + 2] - t[0],
-                t[i * 8 + 3] - t[0], t[i * 8 + 4] - t[0], t[i * 8 + 5] - t[0], t[i * 8 + 6] - t[0]);
-    }
+    tc_conv1_u8_kernel<<<grid, U8_THREADS, U8_SMEM_TOTAL, s>>>(h->tm8_hi, h->tm8_lo, h->tm_out32_hi, h->tm_out32_lo, p);
   } else if (src_u8) {
     AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel<128, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     tc_conv1_kernel<128, 3, true><<<grid, C1_THREADS, S::TOTAL, s>>>(h->tm_hi, h->tm_lo, p);

@@ -1,19 +1,14 @@
-// Fused codebook match on tcgen05 (AAE_PREC_TC_SPLIT): ONE kernel does
+// Fused codebook match on wgmma (AAE_PREC_TC_SPLIT): ONE kernel does
 //     zq = z * rsqrt(max(sum z^2, 1e-12))          (tf.nn.l2_normalize,  auto_pose/ae/codebook.py:27)
 //     cos = zq . E^T                                (tf.matmul,           codebook.py:50)
 //     idx = argmax(cos), lowest index on ties       (np.argmax,           codebook.py:63-68)
 // and never materialises the [B, N] cosine matrix.
 //
-// Layout: TMEM lanes = queries (M = 128 per block, up to two blocks for B <= 256), TMEM columns = codebook rows (128 per
-// tile), so the arg-max over rows is a per-thread scan of its own lane -- no cross-thread reduction.
-// The normalised queries are split into fp16 (hi, lo) in the kernel prologue and stay resident IN TENSOR MEMORY as the
-// MMA's A operand (tcgen05.mma with A from TMEM), which leaves all of shared memory to the codebook: pre-split into
-// (hi, lo) fp16 at create time -- the same 512 bytes per row as the fp32 table -- it streams through a 3-stage x 64 KB TMA
-// ring, each row read from HBM exactly once.  Per (tile, query block) the issuer thread fires  hi*hi + hi*lo + lo*hi  into
-// one fp32 accumulator (both operands pre-scaled by 64 so every lo term is a normal fp16; the 2^-12 unscale in the epilogue
-// is exact).  Two accumulator stages alternate, so the epilogue scan of one block overlaps the MMAs of the next.  Per-CTA winners are merged with one 64-bit atomicMax per query on a
-// (score, ~index) key -- max is order-independent, so the result is deterministic -- and the last CTA to finish writes
-// the [B] score / index outputs and re-arms the scratch for the next launch (steady state: a single launch, no memset).
+// MMA rows = queries (128 per launch, one 64-row warpgroup each half), MMA columns = codebook rows (128 per tile): the queries,
+// normalised and split into fp16 (hi, lo) in the prologue, stay in shared memory as the A operand; the codebook, pre-split at
+// create time, streams through a TMA ring, each row read from HBM once; per tile  hi*hi + hi*lo + lo*hi  go into one fp32
+// accumulator (operands pre-scaled by 64, exact unscale).  Per-CTA winners merge through a 64-bit atomicMax on (score, ~index)
+// (k = 1) or per-CTA lists merged by the last CTA (k <= 8), deterministically; the last CTA re-arms the scratch.
 #include <stdlib.h>
 
 #include "tc.cuh"
@@ -26,14 +21,15 @@ using namespace tc;
 namespace {
 
 constexpr int MT_ROWS = 128;                // codebook rows per tile (= MMA N)
-constexpr int MT_STAGES = 3;
+constexpr int MT_STAGES = 2;
+constexpr int MT_THREADS = 384;
 constexpr int MT_E_BYTES = MT_ROWS * 128;   // one K-half of one (hi|lo) array: 128 rows x 128 B
 constexpr int MT_STAGE_BYTES = 4 * MT_E_BYTES;  // hi k0, hi k1, lo k0, lo k1  = 64 KB
 constexpr float MT_SCALE = 64.f;
-constexpr int MT_SMEM_TOTAL = MT_STAGES * MT_STAGE_BYTES + 1024 + 256;
-// TMEM columns: per 128-query block mq: [mq*128, +64) Q_hi, [mq*128+64, +64) Q_lo  (fp16 pairs, K = 128 -> 64 columns);
-// accumulators: two stages of 128 fp32 columns at 256 and 384.
-constexpr int MT_TMEM_ACC0 = 256;
+constexpr int MT_Q_BYTES = 4 * MT_E_BYTES;      // the launch's 128 queries as (hi, lo) fp16, K = 128
+constexpr int MT_SMEM_TOTAL = MT_STAGES * MT_STAGE_BYTES + MT_Q_BYTES + 1024 + 256;
+constexpr int MT_MAX_GRID = 148;                // CTAs of one launch at most (sm_count is clamped to it)
+constexpr int MT_BATCH = 128;                   // queries per launch
 
 __device__ __forceinline__ unsigned long long pack_best(float s, int idx) {
   uint32_t b = __float_as_uint(s);
@@ -47,277 +43,6 @@ __device__ __forceinline__ void unpack_best(unsigned long long k, float& s, int&
   idx = (int)(0xFFFFFFFFu - (uint32_t)(k & 0xFFFFFFFFu));
 }
 
-template <int MQ>
-__global__ void __launch_bounds__(256, 1)
-tc_match_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_constant__ CUtensorMap tm_e_lo, const float* __restrict__ z,
-                int B, int n_rows, int n_tiles, long long row_offset, unsigned long long* __restrict__ best, unsigned int* __restrict__ counter,
-                float* __restrict__ scores_out, int* __restrict__ idx_out, long long* __restrict__ trace) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* e_smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* e_full = reinterpret_cast<uint64_t*>(e_smem + MT_STAGES * MT_STAGE_BYTES);
-  uint64_t* e_empty = e_full + MT_STAGES;
-  uint64_t* acc_full = e_empty + MT_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  __shared__ int s_is_last;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (trace != nullptr && threadIdx.x == 0) {
-    if (blockIdx.x == 0) trace[12] = clock64();
-    unsigned long long g;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
-    trace[256 + blockIdx.x] = (long long)g;
-  }
-
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tm_e_hi); prefetch_tmap(&tm_e_lo); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < MT_STAGES; ++s) { mbar_init(&e_full[s], 1); mbar_init(&e_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4); }
-    fence_barrier_init();
-  }
-  if (trace != nullptr && blockIdx.x == 0 && threadIdx.x == 64) { trace[13] = clock64(); }
-  if (warp == 2) tmem_alloc<512>(tmem_ptr);
-  if (trace != nullptr && blockIdx.x == 0 && threadIdx.x == 64) { trace[14] = clock64(); }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const bool tr = trace != nullptr && blockIdx.x == 0;
-  if (tr && threadIdx.x == 0) trace[0] = clock64();
-  const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  // kick off the first codebook tiles now: their HBM latency overlaps the query prologue below
-  if (warp == 0 && lane == 0) {
-    for (int i = 0; i < my_tiles && i < 1; ++i) {   // stages 1 and 2 serve as the query staging area until the prologue is done
-      const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * MT_ROWS;
-      uint8_t* st = e_smem + i * MT_STAGE_BYTES;
-      mbar_arrive_expect_tx(&e_full[i], MT_STAGE_BYTES);
-      tma_load_2d(st, &tm_e_hi, &e_full[i], 0, row0);
-      tma_load_2d(st + MT_E_BYTES, &tm_e_hi, &e_full[i], 64, row0);
-      tma_load_2d(st + 2 * MT_E_BYTES, &tm_e_lo, &e_full[i], 0, row0);
-      tma_load_2d(st + 3 * MT_E_BYTES, &tm_e_lo, &e_full[i], 64, row0);
-    }
-  }
-
-  // ---- prologue, phase A (all warps, coalesced): cp.async every query row into the not-yet-used ring stages 1.. as fp32
-  //      (512 B per row, 16-byte chunks XOR-swizzled by the row, so the row-wise writes here and the thread-per-row reads
-  //      of phase B are both bank-conflict free)
-#pragma unroll 4
-  for (int row = warp; row < MQ * 128; row += 8) {
-    const int mq = row >> 7, r = row & 127;
-    cp_async_16(e_smem + (1 + mq) * MT_STAGE_BYTES + r * 512 + ((lane ^ (r & 31)) << 4), z + (long long)(row < B ? row : 0) * 128 + lane * 4,
-                row < B);
-  }
-  if (tr && threadIdx.x == 0) trace[4] = clock64();
-  cp_async_wait_all();
-  if (tr && threadIdx.x == 0) trace[5] = clock64();
-  __syncthreads();
-  if (tr && threadIdx.x == 0) trace[7] = clock64();
-  // ---- phase B: thread (warp%4, lane) owns row r = 32*(warp%4) + lane of query block mq = warp/4 (warps 4-7 -> block 0,
-  //      warps 0-3 -> block 1): sum of squares, tf.nn.l2_normalize's rsqrt(max(ss, 1e-12)), scale by 64, split into fp16
-  //      (hi, lo) and park the row in TMEM as the MMA's A operand (lane = row, column c = K elements 2c, 2c+1) -- the
-  //      queries never occupy shared memory during the main loop.
-  {
-    const int mq = warp >= 4 ? 0 : 1;
-    if (mq < MQ) {
-      const int q = warp & 3, r = q * 32 + lane;
-      const uint8_t* src = e_smem + (1 + mq) * MT_STAGE_BYTES + r * 512;
-      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#pragma unroll 8
-      for (int c = 0; c < 32; ++c) {
-        const float4 v = *reinterpret_cast<const float4*>(src + ((c ^ (r & 31)) << 4));
-        s0 = fmaf(v.x, v.x, s0); s1 = fmaf(v.y, v.y, s1); s2 = fmaf(v.z, v.z, s2); s3 = fmaf(v.w, v.w, s3);
-      }
-      const float ss = fmaxf((s0 + s1) + (s2 + s3), 1e-12f);
-      float y = rsqrtf(ss);
-      y = y * (1.5f - 0.5f * ss * y * y);              // one Newton step: ~1 ulp
-      const float inv = MT_SCALE * y;
-      const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mq * 128);
-#pragma unroll 2
-      for (int g = 0; g < 8; ++g) {                    // 16 K elements -> 8 packed columns of Q_hi and of Q_lo
-        uint32_t hi[8], lo[8];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 v = *reinterpret_cast<const float4*>(src + (((g * 4 + j) ^ (r & 31)) << 4));
-          split_f16x2(v.x * inv, v.y * inv, hi[2 * j], lo[2 * j]);
-          split_f16x2(v.z * inv, v.w * inv, hi[2 * j + 1], lo[2 * j + 1]);
-        }
-        tmem_st_32x8(lane_base + (uint32_t)(g * 8), hi);
-        tmem_st_32x8(lane_base + (uint32_t)(64 + g * 8), lo);
-      }
-      tmem_st_wait();
-    }
-  }
-  if (tr && threadIdx.x == 0) trace[8] = clock64();
-  fence_proxy_async_smem();   // the staging area is about to be overwritten by TMA (async proxy)
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (tr && threadIdx.x == 0) trace[1] = clock64();
-
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int i = 1; i < my_tiles; ++i) {
-        const int s = i % MT_STAGES;
-        const uint32_t ph = (uint32_t)(i / MT_STAGES) & 1u;
-        mbar_wait(&e_empty[s], ph ^ 1u);
-        const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * MT_ROWS;
-        uint8_t* st = e_smem + s * MT_STAGE_BYTES;
-        mbar_arrive_expect_tx(&e_full[s], MT_STAGE_BYTES);
-        tma_load_2d(st, &tm_e_hi, &e_full[s], 0, row0);
-        tma_load_2d(st + MT_E_BYTES, &tm_e_hi, &e_full[s], 64, row0);
-        tma_load_2d(st + 2 * MT_E_BYTES, &tm_e_lo, &e_full[s], 0, row0);
-        tma_load_2d(st + 3 * MT_E_BYTES, &tm_e_lo, &e_full[s], 64, row0);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(128, MT_ROWS, 0);
-      for (int i = 0; i < my_tiles; ++i) {
-        const int s = i % MT_STAGES;
-        mbar_wait(&e_full[s], (uint32_t)(i / MT_STAGES) & 1u);
-        if (tr && i < 16) trace[16 + i * 8 + 0] = clock64();
-        const uint32_t est = smem_u32(e_smem + s * MT_STAGE_BYTES);
-#pragma unroll 1
-        for (int mq = 0; mq < MQ; ++mq) {
-          const int u = i * MQ + mq, as = u & 1;        // accumulator stage alternates per (tile, query block)
-          mbar_wait(&acc_empty[as], ((uint32_t)(u >> 1) & 1u) ^ 1u);
-          tc_fence_after();
-          if (tr && i < 16) trace[16 + i * 8 + 1 + mq * 2] = clock64();
-          const uint32_t d = tmem_base + (uint32_t)(MT_TMEM_ACC0 + as * MT_ROWS);
-          const uint32_t q_hi = tmem_base + (uint32_t)(mq * 128), q_lo = q_hi + 64;
-#pragma unroll 1
-          for (int kh = 0; kh < 2; ++kh) {
-            const uint64_t e_hi = make_sw128_kmajor_desc(est + kh * MT_E_BYTES);
-            const uint64_t e_lo = make_sw128_kmajor_desc(est + (2 + kh) * MT_E_BYTES);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint32_t kc = (uint32_t)((kh * 4 + k) * 8);   // 16 fp16 K elements = 8 packed columns
-              umma_f16_ts(d, q_lo + kc, desc_advance_k(e_hi, k), idesc, (kh > 0 || k > 0) ? 1u : 0u);
-              umma_f16_ts(d, q_hi + kc, desc_advance_k(e_lo, k), idesc, 1u);
-              umma_f16_ts(d, q_hi + kc, desc_advance_k(e_hi, k), idesc, 1u);
-            }
-          }
-          umma_commit(&acc_full[as]);
-          if (tr && i < 16) trace[16 + i * 8 + 2 + mq * 2] = clock64();
-        }
-        umma_commit(&e_empty[s]);
-      }
-    }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    float bs0 = -3.0e38f, bs1 = -3.0e38f;   // running best per query block (kept in named registers: the mq loop is rolled)
-    int bi0 = 0x7FFFFFFF, bi1 = 0x7FFFFFFF;
-    for (int i = 0; i < my_tiles; ++i) {
-      const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * MT_ROWS;
-      const int nvalid = min(MT_ROWS, n_rows - row0);
-#pragma unroll 1
-      for (int mq = 0; mq < MQ; ++mq) {
-        const int u = i * MQ + mq, as = u & 1;
-        float cbs = mq ? bs1 : bs0;
-        int cbi = mq ? bi1 : bi0;
-        mbar_wait(&acc_full[as], (uint32_t)(u >> 1) & 1u);
-        tc_fence_after();
-        if (tr && warp == 4 && lane == 0 && i < 16) trace[16 + i * 8 + 5 + mq] = clock64();
-#pragma unroll 1
-        for (int c = 0; c < MT_ROWS / 64; ++c) {
-          uint32_t v[32], w[32];
-          const uint32_t col = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(MT_TMEM_ACC0 + as * MT_ROWS + c * 64);
-          tmem_ld_32x32(col, v);
-          tmem_ld_32x32(col + 32, w);
-          tmem_ld_wait();
-          if (nvalid < MT_ROWS) {                       // last tile only: padding rows must never win
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              if (c * 64 + j >= nvalid) v[j] = 0xFF800000u;        // -inf
-              if (c * 64 + 32 + j >= nvalid) w[j] = 0xFF800000u;
-            }
-          }
-          // log-depth max of the 64 scores; the (rare) index search only runs when this chunk beats the running best
-          float m[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) m[j] = fmaxf(__uint_as_float(v[j]), __uint_as_float(w[j]));
-#pragma unroll
-          for (int st = 16; st >= 1; st >>= 1)
-#pragma unroll
-            for (int j = 0; j < st; ++j) m[j] = fmaxf(m[j], m[j + st]);
-          const float mx = m[0];
-          if (mx > cbs) {                               // strict >: an equal score later in the table never replaces an earlier row
-            int first = 63;
-#pragma unroll
-            for (int j = 31; j >= 0; --j)
-              if (__uint_as_float(w[j]) == mx) first = 32 + j;
-#pragma unroll
-            for (int j = 31; j >= 0; --j)
-              if (__uint_as_float(v[j]) == mx) first = j;          // lowest column holding the maximum
-            cbs = mx;
-            cbi = row0 + c * 64 + first;
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[as]);
-        if (mq) { bs1 = cbs; bi1 = cbi; } else { bs0 = cbs; bi0 = cbi; }
-      }
-    }
-#pragma unroll
-    for (int mq = 0; mq < MQ; ++mq) {
-      const int qi = mq * 128 + q * 32 + lane;
-      const float fs = mq ? bs1 : bs0;
-      const int fi = mq ? bi1 : bi0;
-      if (qi < B && fi != 0x7FFFFFFF) atomicMax(best + qi, pack_best(fs * (1.f / (MT_SCALE * MT_SCALE)), fi));
-    }
-  }
-  // ---- teardown + last-CTA finalisation ----
-  if (tr && threadIdx.x == 128) trace[2] = clock64();
-  tc_fence_before();
-  __threadfence();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
-  if (threadIdx.x == 0) {
-    const unsigned int ticket = atomicAdd(counter, 1u);
-    s_is_last = (ticket == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (s_is_last) {
-    __threadfence();
-    for (int qi = threadIdx.x; qi < B; qi += blockDim.x) {
-      const unsigned long long k = atomicExch(best + qi, 0ull);   // read + re-arm
-      float s;
-      int idx;
-      unpack_best(k, s, idx);
-      scores_out[qi] = s;
-      idx_out[qi] = (int)(idx + row_offset);
-    }
-    if (threadIdx.x == 0) *counter = 0u;
-  }
-  if (tr && threadIdx.x == 0) trace[3] = clock64();
-  if (trace != nullptr && threadIdx.x == 0) {
-    unsigned long long g;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
-    trace[512 + blockIdx.x] = (long long)g;
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------------
-// Second generation of the fused match (default; AAE_MATCH_V1=1 selects the kernel above for same-box A/B runs).
-// Same arithmetic, same operand layouts, same result.  What changed, each item aimed at the fixed costs that dominated the
-// first kernel (20.5 us at B = 1 against a 7.2 us HBM floor):
-//   * the codebook stream starts before anything else: thread 0 initialises the barriers, fences and issues the TMA loads
-//     of the first tiles while the TMEM allocation, the query staging and the normalise/split prologue are still to come
-//     (before: after the allocation and a block-wide barrier, and one tile only);
-//   * B <= 128 stages its queries in ONE ring stage, so TWO tiles (128 KB per SM, 19 MB chip-wide = 40 % of the table) are in
-//     flight during the prologue; B > 128 runs the prologue in two rounds of 128 queries and hands each staging stage to the
-//     TMA producer as soon as its round is done;
-//   * in every round all eight warps work: warps w and w+4 own the same 32 TMEM lanes (queries) and each converts one K
-//     half of the row -- the fp32 -> fp16x2 conversions (the slow pipe) are what the prologue is bound by;
-//   * top-k (k <= 8) and `upright` (codebook.py:64-71) run on this kernel too: a per-lane sorted list of K (score, index)
-//     pairs in registers replaces the running best, per-CTA lists go through a scratch table and the last CTA merges them
-//     ("score descending, ties to the lowest index" = the order of the packed 64-bit keys); upright is the same kernel on a
-//     tensor map whose row stride is num_cyclo rows.
 template <int K>
 struct TopList {
   float s[K];
@@ -328,7 +53,7 @@ struct TopList {
   }
   __device__ __forceinline__ float worst() const { return s[K - 1]; }
   // precondition: v > worst().  Replaces the worst entry and bubbles up past STRICTLY smaller scores only, so that among equal
-  // scores the entry inserted first (lower row index: a CTA visits its rows in increasing order) stays ahead.
+  // scores the entry inserted first (lower row index: a thread visits its rows in increasing order) stays ahead.
   __device__ __forceinline__ void insert(float v, int idx) {
     s[K - 1] = v; i[K - 1] = idx;
 #pragma unroll
@@ -341,250 +66,172 @@ struct TopList {
   }
 };
 
-template <int MQ, int K>
-__global__ void __launch_bounds__(256, 1)
-tc_match2_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_constant__ CUtensorMap tm_e_lo, const float* __restrict__ z,
-                 int B, int n_rows, int n_tiles, int idx_mul, long long row_offset, int k_out, unsigned long long* __restrict__ best,
-                 unsigned long long* __restrict__ lists, unsigned int* __restrict__ counter, float* __restrict__ scores_out,
-                 int* __restrict__ idx_out, long long* __restrict__ trace) {
+// The four threads of a quad hold the same query row (wgmma fragment layout): merge their sorted lists into the row's top K packed
+// keys (every thread of the quad ends up with the same keys).
+template <int K>
+__device__ __forceinline__ void quad_merge(const TopList<K>& l, float unscale, unsigned long long (&out)[K]) {
+  unsigned long long key[K];
+#pragma unroll
+  for (int j = 0; j < K; ++j) key[j] = l.i[j] != 0x7FFFFFFF ? pack_best(l.s[j] * unscale, l.i[j]) : 0ull;
+#pragma unroll
+  for (int j = 0; j < K; ++j) {
+    unsigned long long m = key[0];
+#pragma unroll
+    for (int off = 1; off <= 2; off <<= 1) {
+      const unsigned long long o = __shfl_xor_sync(0xFFFFFFFFu, m, off);
+      m = o > m ? o : m;
+    }
+    out[j] = m;
+    if (m != 0ull && key[0] == m) {                  // unique key: exactly one thread of the quad pops its head
+#pragma unroll
+      for (int t = 0; t + 1 < K; ++t) key[t] = key[t + 1];
+      key[K - 1] = 0ull;
+    }
+  }
+}
+
+// 384 threads: warp 0 streams the codebook through the TMA ring; warpgroups 1 and 2 (warps 4-11) normalise and split queries
+// [0,64) and [64,128) of the block into shared memory, then run wgmma (A = queries, B = a 128-row codebook tile) and scan their
+// accumulator fragments: thread (warp, lane) owns rows 16 (warp % 4) + lane / 4 (+8) of its warpgroup's 64 queries and 32 of
+// the 128 codebook rows of each tile.
+template <int K>
+__global__ void __launch_bounds__(MT_THREADS, 1)
+tc_match_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_constant__ CUtensorMap tm_e_lo, const float* __restrict__ z,
+                int B, int n_rows, int n_tiles, int idx_mul, long long row_offset, int k_out, unsigned long long* __restrict__ best,
+                unsigned long long* __restrict__ lists, unsigned int* __restrict__ counter, float* __restrict__ scores_out,
+                int* __restrict__ idx_out) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* e_smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* e_full = reinterpret_cast<uint64_t*>(e_smem + MT_STAGES * MT_STAGE_BYTES);
+  uint8_t* q_smem = e_smem + MT_STAGES * MT_STAGE_BYTES;   // Q_hi k0, Q_hi k1, Q_lo k0, Q_lo k1: 128 queries x 128 B each
+  uint64_t* e_full = reinterpret_cast<uint64_t*>(q_smem + MT_Q_BYTES);
   uint64_t* e_empty = e_full + MT_STAGES;
-  uint64_t* acc_full = e_empty + MT_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_empty + 2);
   __shared__ int s_is_last;
-  __shared__ float s_part[MQ][2][128];
+  __shared__ float s_part[2][128];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bool tr = trace != nullptr && blockIdx.x == 0;
-  if (tr && threadIdx.x == 0) trace[0] = clock64();
   const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  // ring stage of this CTA's i-th tile.  MQ = 2 swaps stages 1 and 2: stage 2 is the staging area of the FIRST prologue round
-  // and is free (and refilled) one round earlier than stage 1.
-  auto stage_of = [](int i) -> int { const int r = i % MT_STAGES; return MQ == 1 ? r : (r == 0 ? 0 : MT_STAGES - r); };
-  auto load_tile = [&](int i) {
-    const int s = stage_of(i);
-    const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * MT_ROWS;
-    uint8_t* st = e_smem + s * MT_STAGE_BYTES;
-    mbar_arrive_expect_tx(&e_full[s], MT_STAGE_BYTES);
-    tma_load_2d(st, &tm_e_hi, &e_full[s], 0, row0);
-    tma_load_2d(st + MT_E_BYTES, &tm_e_hi, &e_full[s], 64, row0);
-    tma_load_2d(st + 2 * MT_E_BYTES, &tm_e_lo, &e_full[s], 0, row0);
-    tma_load_2d(st + 3 * MT_E_BYTES, &tm_e_lo, &e_full[s], 64, row0);
-  };
-  constexpr int kPrefetch = MQ == 1 ? 2 : 1;   // tiles requested before the prologue
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < MT_STAGES; ++s) { mbar_init(&e_full[s], 1); mbar_init(&e_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4); }
+    for (int s = 0; s < MT_STAGES; ++s) { mbar_init(&e_full[s], 1); mbar_init(&e_empty[s], 2); }
     fence_barrier_init();
-    for (int i = 0; i < kPrefetch && i < my_tiles; ++i) load_tile(i);     // the codebook stream starts here
   }
-  if (warp == 2) tmem_alloc<512>(tmem_ptr);
-
-  // ---- prologue: 128 queries per round.  Phase A (all warps, coalesced): cp.async the round's rows as fp32 into a staging
-  //      stage (512 B per row, 16-byte chunks XOR-swizzled by the row: the row-wise writes here and the thread-per-row reads of
-  //      phase B are both bank-conflict free).  Round 0 -> stage 2, round 1 (MQ = 2) -> stage 1.
-#pragma unroll
-  for (int mq = 0; mq < MQ; ++mq) {
-    uint8_t* stg = e_smem + (2 - mq) * MT_STAGE_BYTES;
-#pragma unroll 4
-    for (int r = warp; r < 128; r += 8) {
-      const int row = mq * 128 + r;
-      cp_async_16(stg + r * 512 + ((lane ^ (r & 31)) << 4), z + (long long)(row < B ? row : 0) * 128 + lane * 4, row < B);
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");      // one group per round: round 1's rows keep arriving while round 0 is converted
-  }
-  if (MQ == 2) asm volatile("cp.async.wait_group 1;" ::: "memory"); else asm volatile("cp.async.wait_group 0;" ::: "memory");
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  if (tr && threadIdx.x == 0) trace[4] = clock64();
-  // ---- phase B: warps w and w+4 own TMEM lanes 32*(w%4).. = queries r = 32*(w%4) + lane of the round's block; both read
-  //      sum the squares of one K half each and exchange the partial sums (tf.nn.l2_normalize: z * rsqrt(max(sum z^2, 1e-12))),
-  //      warp w < 4 converts K elements 0..63, warp w + 4 elements 64..127: scale by 64, split into fp16 (hi, lo), park in TMEM as the MMA's A operand
-  //      (lane = query, column c = K elements 2c, 2c+1; Q_hi at columns [mq*128, +64), Q_lo at [mq*128+64, +64)).
-#pragma unroll
-  for (int mq = 0; mq < MQ; ++mq) {
-    if (mq == 1) {                                   // round 1's rows: this thread's copies have landed; the barrier makes everybody's visible
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
-      __syncthreads();
-    }
-    const int q = warp & 3, half = warp >> 2, r = q * 32 + lane;
-    const uint8_t* src = e_smem + (2 - mq) * MT_STAGE_BYTES + r * 512;
-    float4 mine[16];
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#pragma unroll
-    for (int c = 0; c < 16; ++c) {
-      const float4 v = *reinterpret_cast<const float4*>(src + (((half * 16 + c) ^ (r & 31)) << 4));
-      s0 = fmaf(v.x, v.x, s0); s1 = fmaf(v.y, v.y, s1); s2 = fmaf(v.z, v.z, s2); s3 = fmaf(v.w, v.w, s3);
-      mine[c] = v;
-    }
-    s_part[mq][half][r] = (s0 + s1) + (s2 + s3);       // each thread sums its K half; the two halves meet through shared memory
-    __syncthreads();
-    const float ss = fmaxf(s_part[mq][0][r] + s_part[mq][1][r], 1e-12f);
-    float y = rsqrtf(ss);
-    y = y * (1.5f - 0.5f * ss * y * y);              // one Newton step: ~1 ulp
-    const float inv = MT_SCALE * y;
-    const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mq * 128 + half * 32);
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {                    // 16 K elements -> 8 packed columns of Q_hi and of Q_lo
-      uint32_t hi[8], lo[8];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float4 v = mine[g * 4 + j];
-        split_f16x2(v.x * inv, v.y * inv, hi[2 * j], lo[2 * j]);
-        split_f16x2(v.z * inv, v.w * inv, hi[2 * j + 1], lo[2 * j + 1]);
-      }
-      tmem_st_32x8(lane_base + (uint32_t)(g * 8), hi);
-      tmem_st_32x8(lane_base + (uint32_t)(64 + g * 8), lo);
-    }
-    tmem_st_wait();
-    fence_proxy_async_smem();   // the staging stage is about to be overwritten by TMA (async proxy)
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    // the round's staging stage is free: request the tile that lives there (MQ = 1: tile 2 -> stage 2; MQ = 2: tile 1 -> stage 2,
-    // then tile 2 -> stage 1)
-    if (threadIdx.x == 0 && kPrefetch + mq < my_tiles) load_tile(kPrefetch + mq);
-  }
-  if (tr && threadIdx.x == 0) trace[1] = clock64();
-  constexpr int kIssued = kPrefetch + MQ;     // tiles requested so far (= MT_STAGES)
 
   if (warp == 0) {
-    if (lane == 0) {
-      for (int i = kIssued; i < my_tiles; ++i) {
-        const int s = stage_of(i);
-        mbar_wait(&e_empty[s], ((uint32_t)(i / MT_STAGES) & 1u) ^ 1u);
-        load_tile(i);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(128, MT_ROWS, 0);
+    if (lane == 0) {                                  // the codebook stream starts before the query prologue
       for (int i = 0; i < my_tiles; ++i) {
-        const int s = stage_of(i);
-        mbar_wait(&e_full[s], (uint32_t)(i / MT_STAGES) & 1u);
-        if (tr && i < 16) trace[16 + i * 8 + 0] = clock64();
-        const uint32_t est = smem_u32(e_smem + s * MT_STAGE_BYTES);
-#pragma unroll 1
-        for (int mq = 0; mq < MQ; ++mq) {
-          const int u = i * MQ + mq, as = u & 1;        // accumulator stage alternates per (tile, query block)
-          mbar_wait(&acc_empty[as], ((uint32_t)(u >> 1) & 1u) ^ 1u);
-          tc_fence_after();
-          if (tr && i < 16) trace[16 + i * 8 + 1 + mq * 2] = clock64();
-          const uint32_t d = tmem_base + (uint32_t)(MT_TMEM_ACC0 + as * MT_ROWS);
-          const uint32_t q_hi = tmem_base + (uint32_t)(mq * 128), q_lo = q_hi + 64;
-#pragma unroll 1
-          for (int kh = 0; kh < 2; ++kh) {
-            const uint64_t e_hi = make_sw128_kmajor_desc(est + kh * MT_E_BYTES);
-            const uint64_t e_lo = make_sw128_kmajor_desc(est + (2 + kh) * MT_E_BYTES);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint32_t kc = (uint32_t)((kh * 4 + k) * 8);   // 16 fp16 K elements = 8 packed columns
-              umma_f16_ts(d, q_lo + kc, desc_advance_k(e_hi, k), idesc, (kh > 0 || k > 0) ? 1u : 0u);
-              umma_f16_ts(d, q_hi + kc, desc_advance_k(e_lo, k), idesc, 1u);
-              umma_f16_ts(d, q_hi + kc, desc_advance_k(e_hi, k), idesc, 1u);
-            }
-          }
-          umma_commit(&acc_full[as]);
-          if (tr && i < 16) trace[16 + i * 8 + 2 + mq * 2] = clock64();
-        }
-        umma_commit(&e_empty[s]);
+        const int s = i % MT_STAGES;
+        mbar_wait(&e_empty[s], ((uint32_t)(i / MT_STAGES) & 1u) ^ 1u);
+        const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * MT_ROWS;
+        uint8_t* st = e_smem + s * MT_STAGE_BYTES;
+        mbar_arrive_expect_tx(&e_full[s], MT_STAGE_BYTES);
+        tma_load_2d(st, &tm_e_hi, &e_full[s], 0, row0);
+        tma_load_2d(st + MT_E_BYTES, &tm_e_hi, &e_full[s], 64, row0);
+        tma_load_2d(st + 2 * MT_E_BYTES, &tm_e_lo, &e_full[s], 0, row0);
+        tma_load_2d(st + 3 * MT_E_BYTES, &tm_e_lo, &e_full[s], 64, row0);
       }
     }
   } else if (warp >= 4) {
-    const int q = warp & 3;
-    TopList<K> l0, l1;                       // one list per query block (named objects: the mq loop is rolled)
-    l0.init(); l1.init();
+    // ---- prologue: thread t owns K half t / 128 of query r = t % 128: sum of squares (the halves meet through shared memory),
+    //      tf.nn.l2_normalize's z * rsqrt(max(sum z^2, 1e-12)), scale by 64, split into fp16 (hi, lo), store in the 128-byte-
+    //      swizzle K-major layout of the MMA's A operand.
+    {
+      const int t = (int)threadIdx.x - 128, r = t & 127, half = t >> 7;
+      float4 mine[16];
+      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+      const float4* src = reinterpret_cast<const float4*>(z + (long long)(r < B ? r : 0) * 128 + half * 64);
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+        const float4 v = r < B ? __ldg(src + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+        s0 = fmaf(v.x, v.x, s0); s1 = fmaf(v.y, v.y, s1); s2 = fmaf(v.z, v.z, s2); s3 = fmaf(v.w, v.w, s3);
+        mine[c] = v;
+      }
+      s_part[half][r] = (s0 + s1) + (s2 + s3);
+      named_bar_sync(1, 256);
+      const float ss = fmaxf(s_part[0][r] + s_part[1][r], 1e-12f);
+      float y = rsqrtf(ss);
+      y = y * (1.5f - 0.5f * ss * y * y);              // one Newton step: ~1 ulp
+      const float inv = MT_SCALE * y;
+      uint8_t* qh = q_smem + half * MT_E_BYTES + r * 128;
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {                    // 8 K elements = one 16-byte chunk of the row
+        uint32_t hi[4], lo[4];
+        const float4 a = mine[2 * g], b = mine[2 * g + 1];
+        split_f16x2(a.x * inv, a.y * inv, hi[0], lo[0]);
+        split_f16x2(a.z * inv, a.w * inv, hi[1], lo[1]);
+        split_f16x2(b.x * inv, b.y * inv, hi[2], lo[2]);
+        split_f16x2(b.z * inv, b.w * inv, hi[3], lo[3]);
+        const int off = (g ^ (r & 7)) << 4;
+        *reinterpret_cast<uint4*>(qh + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+        *reinterpret_cast<uint4*>(qh + 2 * MT_E_BYTES + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+      }
+      fence_proxy_async_smem();                        // generic-proxy writes -> visible to wgmma
+      named_bar_sync(1, 256);
+    }
+    const int wg = (warp - 4) >> 2;
+    const uint32_t q_base = smem_u32(q_smem) + (uint32_t)(wg * 64 * 128);
+    TopList<K> la, lb;                                 // rows 16 (warp % 4) + lane / 4 and that + 8 of the warpgroup's queries
+    la.init(); lb.init();
+    float acc[MT_ROWS / 2];
     for (int i = 0; i < my_tiles; ++i) {
+      const int s = i % MT_STAGES;
       const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * MT_ROWS;
       const int nvalid = min(MT_ROWS, n_rows - row0);
-#pragma unroll 1
-      for (int mq = 0; mq < MQ; ++mq) {
-        const int u = i * MQ + mq, as = u & 1;
-        TopList<K> cur = mq ? l1 : l0;
-        mbar_wait(&acc_full[as], (uint32_t)(u >> 1) & 1u);
-        tc_fence_after();
-        if (tr && warp == 4 && lane == 0 && i < 16) trace[16 + i * 8 + 5 + mq] = clock64();
-#pragma unroll 1
-        for (int c = 0; c < MT_ROWS / 64; ++c) {
-          uint32_t v[32], w[32];
-          const uint32_t col = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(MT_TMEM_ACC0 + as * MT_ROWS + c * 64);
-          tmem_ld_32x32(col, v);
-          tmem_ld_32x32(col + 32, w);
-          tmem_ld_wait();
-          if (nvalid < MT_ROWS) {                       // last tile only: padding rows must never win
+      mbar_wait(&e_full[s], (uint32_t)(i / MT_STAGES) & 1u);
+      const uint32_t est = smem_u32(e_smem + s * MT_STAGE_BYTES);
+      wgmma_fence_regs(acc);
+      wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              if (c * 64 + j >= nvalid) v[j] = 0xFF800000u;        // -inf
-              if (c * 64 + 32 + j >= nvalid) w[j] = 0xFF800000u;
-            }
-          }
-          // log-depth max of the 64 scores; the (rare) list update only runs when this chunk beats the list's worst entry
-          float m[32];
+      for (int kh = 0; kh < 2; ++kh) {
+        const uint64_t q_hi = make_sw128_kmajor_desc(q_base + kh * MT_E_BYTES);
+        const uint64_t q_lo = make_sw128_kmajor_desc(q_base + (2 + kh) * MT_E_BYTES);
+        const uint64_t e_hi = make_sw128_kmajor_desc(est + kh * MT_E_BYTES);
+        const uint64_t e_lo = make_sw128_kmajor_desc(est + (2 + kh) * MT_E_BYTES);
 #pragma unroll
-          for (int j = 0; j < 32; ++j) m[j] = fmaxf(__uint_as_float(v[j]), __uint_as_float(w[j]));
-#pragma unroll
-          for (int st = 16; st >= 1; st >>= 1)
-#pragma unroll
-            for (int j = 0; j < st; ++j) m[j] = fmaxf(m[j], m[j + st]);
-          const float mx = m[0];
-          if (mx > cur.worst()) {                       // strict >: an equal score later in the table never displaces an earlier row
-            if (K == 1) {
-              int first = 63;
-#pragma unroll
-              for (int j = 31; j >= 0; --j)
-                if (__uint_as_float(w[j]) == mx) first = 32 + j;
-#pragma unroll
-              for (int j = 31; j >= 0; --j)
-                if (__uint_as_float(v[j]) == mx) first = j;          // lowest column holding the maximum
-              cur.s[0] = mx;
-              cur.i[0] = row0 + c * 64 + first;
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (__uint_as_float(v[j]) > cur.worst()) cur.insert(__uint_as_float(v[j]), row0 + c * 64 + j);
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (__uint_as_float(w[j]) > cur.worst()) cur.insert(__uint_as_float(w[j]), row0 + c * 64 + 32 + j);
-            }
-          }
+        for (int k = 0; k < 4; ++k) {
+          Wgmma<MT_ROWS>::template ss<0, 0>(acc, desc_advance_k(q_lo, k), desc_advance_k(e_hi, k), (kh > 0 || k > 0) ? 1u : 0u);
+          Wgmma<MT_ROWS>::template ss<0, 0>(acc, desc_advance_k(q_hi, k), desc_advance_k(e_lo, k), 1u);
+          Wgmma<MT_ROWS>::template ss<0, 0>(acc, desc_advance_k(q_hi, k), desc_advance_k(e_hi, k), 1u);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[as]);
-        if (mq) l1 = cur; else l0 = cur;
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if ((warp & 3) == 0 && lane == 0) mbar_arrive(&e_empty[s]);
+      // strict >: an equal score later in the table never displaces an earlier row (columns are visited in increasing order)
+#pragma unroll
+      for (int j = 0; j < MT_ROWS / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = 8 * j + 2 * (lane & 3) + e;
+          const float va = col < nvalid ? acc[4 * j + e] : -INFINITY;       // padding rows must never win
+          const float vb = col < nvalid ? acc[4 * j + 2 + e] : -INFINITY;
+          if (va > la.worst()) la.insert(va, row0 + col);
+          if (vb > lb.worst()) lb.insert(vb, row0 + col);
+        }
       }
     }
     constexpr float kUnscale = 1.f / (MT_SCALE * MT_SCALE);
+    const int qa = wg * 64 + (warp & 3) * 16 + (lane >> 2), qb = qa + 8;
+    if (K == 1) {
+      if (qa < B && la.i[0] != 0x7FFFFFFF) atomicMax(best + qa, pack_best(la.s[0] * kUnscale, la.i[0]));
+      if (qb < B && lb.i[0] != 0x7FFFFFFF) atomicMax(best + qb, pack_best(lb.s[0] * kUnscale, lb.i[0]));
+    } else {
+      unsigned long long ka[K], kb[K];
+      quad_merge(la, kUnscale, ka);
+      quad_merge(lb, kUnscale, kb);
+      if ((lane & 3) == 0) {
 #pragma unroll
-    for (int mq = 0; mq < MQ; ++mq) {
-      const int qi = mq * 128 + q * 32 + lane;
-      const TopList<K>& fin = mq ? l1 : l0;
-      if (qi < B) {
-        if (K == 1) {
-          if (fin.i[0] != 0x7FFFFFFF) atomicMax(best + qi, pack_best(fin.s[0] * kUnscale, fin.i[0]));
-        } else {
-#pragma unroll
-          for (int j = 0; j < K; ++j)
-            lists[((size_t)blockIdx.x * B + qi) * K + j] = fin.i[j] != 0x7FFFFFFF ? pack_best(fin.s[j] * kUnscale, fin.i[j]) : 0ull;
+        for (int j = 0; j < K; ++j) {
+          if (qa < B) lists[((size_t)blockIdx.x * B + qa) * K + j] = ka[j];
+          if (qb < B) lists[((size_t)blockIdx.x * B + qb) * K + j] = kb[j];
         }
       }
     }
   }
   // ---- teardown + last-CTA finalisation ----
-  if (tr && threadIdx.x == 128) trace[2] = clock64();
-  tc_fence_before();
   __threadfence();
   __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
   if (threadIdx.x == 0) {
     const unsigned int ticket = atomicAdd(counter, 1u);
     s_is_last = (ticket == gridDim.x - 1);
@@ -603,9 +250,9 @@ tc_match2_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_const
       }
     } else {
       // one warp per query: the k_out largest of the gridDim.x * K packed keys (all distinct: the index is part of the key)
-      constexpr int kPerLane = (148 * K + 31) / 32;
+      constexpr int kPerLane = (MT_MAX_GRID * K + 31) / 32;
       const int total = (int)gridDim.x * K;
-      for (int qi = warp; qi < B; qi += 8) {
+      for (int qi = warp; qi < B; qi += MT_THREADS / 32) {
         unsigned long long key[kPerLane];
 #pragma unroll
         for (int t = 0; t < kPerLane; ++t) {
@@ -642,21 +289,12 @@ tc_match2_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_const
     }
     if (threadIdx.x == 0) *counter = 0u;
   }
-  if (tr && threadIdx.x == 0) trace[3] = clock64();
 }
 
-// Measurement aid (aae_launch_floor_probe): the fixed cost of launching a grid shaped like the match kernel -- one CTA per SM, the
-// same dynamic shared memory (forces the same L1/shared carveout), optionally the same 512-column TMEM allocation -- that does nothing.
-__global__ void __launch_bounds__(256, 1) launch_floor_kernel(int tmem, unsigned int* sink) {
+// Measurement aid (aae_launch_floor_probe): the fixed cost of launching a grid shaped like the match kernel -- one CTA per SM and
+// the same dynamic shared memory (forces the same L1/shared carveout) -- that does nothing.
+__global__ void __launch_bounds__(MT_THREADS, 1) launch_floor_kernel(unsigned int* sink) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint32_t tmem_ptr;
-  if (tmem) {
-    if (threadIdx.x < 32) tmem_alloc<512>(&tmem_ptr);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (threadIdx.x < 32) tmem_dealloc<512>(tmem_ptr);
-  }
   if (sink != nullptr && threadIdx.x == 0 && smem_raw[0] == 0xFF && blockIdx.x == 0xFFFFFFFFu) *sink = 1u;   // never true: keeps smem_raw referenced
 }
 
@@ -687,8 +325,6 @@ struct TcCodebook {
   unsigned long long* best = nullptr;
   unsigned long long* lists = nullptr;   // [grid][max_batch][8] packed keys of the per-CTA top-k lists (k > 1)
   unsigned int* counter = nullptr;
-  long long* trace = nullptr;   // optional clock64 trace of CTA 0 (AAE_MATCH_TRACE=1), diagnostics only
-  bool v1 = false;              // AAE_MATCH_V1=1: first-generation kernel (k = 1, no upright) for A/B runs
 };
 
 constexpr int MT_KMAX = 8;
@@ -696,6 +332,7 @@ constexpr int MT_KMAX = 8;
 int tc_codebook_max_k() { return MT_KMAX; }
 
 int tc_launch_floor_probe(int device, int with_tmem, cudaStream_t s) {
+  (void)with_tmem;                                      // there is no tensor-memory allocation to include on this architecture
   static bool attr_set = false;
   if (!attr_set) {
     AAE_CUDA_OK(cudaFuncSetAttribute(launch_floor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MT_SMEM_TOTAL));
@@ -703,14 +340,14 @@ int tc_launch_floor_probe(int device, int with_tmem, cudaStream_t s) {
   }
   static int sms = 0;                                   // (cudaGetDeviceProperties costs milliseconds: never on a timed path)
   if (sms == 0) AAE_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-  launch_floor_kernel<<<std::min(sms, 148), 256, MT_SMEM_TOTAL, s>>>(with_tmem, nullptr);
+  launch_floor_kernel<<<std::min(sms, MT_MAX_GRID), MT_THREADS, MT_SMEM_TOTAL, s>>>(nullptr);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
 
 int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int latent, int num_cyclo, int max_batch, TcCodebook** out) {
   *out = nullptr;
-  AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 10.x device (tcgen05/TMEM)");
+  AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   AAE_REQUIRE(latent == 128, "AAE_PREC_TC_SPLIT codebook match is built for latent = 128 (got %d)", latent);
   TcCodebook* h = new TcCodebook();
   h->device = device;
@@ -721,11 +358,10 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
   h->num_cyclo = std::max(1, num_cyclo);
   h->n_up = ceil_div(n_rows, (int64_t)h->num_cyclo);
   h->n_tiles_up = (int)ceil_div(h->n_up, (int64_t)MT_ROWS);
-  h->v1 = getenv("AAE_MATCH_V1") != nullptr;
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
-  h->sm_count = std::min(prop.multiProcessorCount, 148);
-  const int cap_b = std::min(256, std::max(1, max_batch));
+  h->sm_count = std::min(prop.multiProcessorCount, MT_MAX_GRID);
+  const int cap_b = std::min(MT_BATCH, std::max(1, max_batch));
   cudaError_t e = cudaMalloc(&h->e_hi, (size_t)h->n_pad * 128 * sizeof(__half));
   if (e == cudaSuccess) e = cudaMalloc(&h->e_lo, (size_t)h->n_pad * 128 * sizeof(__half));
   if (e == cudaSuccess) e = cudaMalloc(&h->best, 256 * sizeof(unsigned long long));
@@ -734,7 +370,6 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
   if (e != cudaSuccess) { set_error("tc codebook alloc failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_OOM; }
   cudaMemset(h->best, 0, 256 * sizeof(unsigned long long));
   cudaMemset(h->counter, 0, sizeof(unsigned int));
-  if (getenv("AAE_MATCH_TRACE")) { cudaMalloc(&h->trace, 768 * sizeof(long long)); cudaMemset(h->trace, 0, 768 * sizeof(long long)); }
   pack_codebook_kernel<<<1024, 256>>>(E_dev, n_rows, h->n_pad, h->e_hi, h->e_lo);
   g_launches.fetch_add(1);
   e = cudaDeviceSynchronize();
@@ -756,11 +391,7 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
   if (st != AAE_OK) { tc_codebook_destroy(h); return st; }
   auto attr = [&](const void* fn) { return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MT_SMEM_TOTAL); };
   e = attr((const void*)tc_match_kernel<1>);
-  if (e == cudaSuccess) e = attr((const void*)tc_match_kernel<2>);
-  if (e == cudaSuccess) e = attr((const void*)tc_match2_kernel<1, 1>);
-  if (e == cudaSuccess) e = attr((const void*)tc_match2_kernel<2, 1>);
-  if (e == cudaSuccess) e = attr((const void*)tc_match2_kernel<1, MT_KMAX>);
-  if (e == cudaSuccess) e = attr((const void*)tc_match2_kernel<2, MT_KMAX>);
+  if (e == cudaSuccess) e = attr((const void*)tc_match_kernel<MT_KMAX>);
   if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(match kernels) failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_CUDA; }
   *out = h;
   return AAE_OK;
@@ -768,28 +399,8 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
 
 void tc_codebook_destroy(TcCodebook* h) {
   if (!h) return;
-  cudaFree(h->e_hi); cudaFree(h->e_lo); cudaFree(h->best); cudaFree(h->lists); cudaFree(h->counter); cudaFree(h->trace);
+  cudaFree(h->e_hi); cudaFree(h->e_lo); cudaFree(h->best); cudaFree(h->lists); cudaFree(h->counter);
   delete h;
-}
-
-static void print_trace(TcCodebook* h, int grid, cudaStream_t s) {
-  long long t[768];
-  cudaStreamSynchronize(s);
-  cudaMemcpy(t, h->trace, sizeof(t), cudaMemcpyDeviceToHost);
-  if (h->v1) {
-    long long e0 = t[256], e1 = t[256], x0 = t[512], x1 = t[512];
-    for (int i = 0; i < grid; ++i) { e0 = std::min(e0, t[256 + i]); e1 = std::max(e1, t[256 + i]); x0 = std::min(x0, t[512 + i]); x1 = std::max(x1, t[512 + i]); }
-    fprintf(stderr, "[match trace] globaltimer ns: CTA entries span %lld, first exit +%lld, last exit +%lld; CTA0 entry +%lld exit +%lld\n", e1 - e0, x0 - e0, x1 - e0, t[256] - e0, t[512] - e0);
-    fprintf(stderr, "[match trace] entry->t0 %lld (alloc begin %lld end %lld) | ", t[0] - t[12], t[13] - t[12], t[14] - t[12]);
-    fprintf(stderr, "[match trace] start->prologue_done %lld  ->loops_done %lld  ->end %lld | cp issued %lld landed %lld synced %lld tmem written %lld\n", t[1] - t[0], t[2] - t[0], t[3] - t[0], t[4] - t[0], t[5] - t[0], t[7] - t[0], t[8] - t[0]);
-  } else {
-    fprintf(stderr, "[match2 trace, CTA 0, clocks from kernel entry] queries staged + TMEM allocated %lld | prologue done %lld | loops done %lld | end %lld\n",
-            t[4] - t[0], t[1] - t[0], t[2] - t[0], t[3] - t[0]);
-  }
-  for (int i = 0; i < 6; ++i)
-    fprintf(stderr, "  tile %d: e_full %lld | mq0 acc_empty %lld issued %lld | mq1 acc_empty %lld issued %lld | epi acc_full mq0 %lld mq1 %lld\n", i,
-            t[16 + i * 8] - t[0], t[16 + i * 8 + 1] - t[0], t[16 + i * 8 + 2] - t[0], t[16 + i * 8 + 3] - t[0], t[16 + i * 8 + 4] - t[0],
-            t[16 + i * 8 + 5] - t[0], t[16 + i * 8 + 6] - t[0]);
 }
 
 // k in [1, 8]; upright != 0 searches rows (row_offset + r * num_cyclo) only -- needs row_offset % num_cyclo == 0 (shard_bounds aligns shards so)
@@ -806,25 +417,15 @@ int tc_codebook_match(TcCodebook* h, const float* z_dev, int B, int64_t row_offs
   const CUtensorMap& th = up ? h->tm_hi_up : h->tm_hi;
   const CUtensorMap& tl = up ? h->tm_lo_up : h->tm_lo;
   const int grid = std::min(h->sm_count, n_tiles);
-  const bool v1 = h->v1 && k == 1 && !up;
-  for (int a = 0; a < B; a += 256) {
-    const int nb = std::min(256, B - a);
+  for (int a = 0; a < B; a += MT_BATCH) {
+    const int nb = std::min(MT_BATCH, B - a);
     const float* z = z_dev + (size_t)a * 128;
     float* so = scores_out + (size_t)a * k;
     int32_t* io = idx_out + (size_t)a * k;
-    if (v1) {
-      if (nb > 128) tc_match_kernel<2><<<grid, 256, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, (long long)row_offset, h->best, h->counter, so, io, h->trace);
-      else tc_match_kernel<1><<<grid, 256, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, (long long)row_offset, h->best, h->counter, so, io, h->trace);
-    } else if (k == 1) {
-      if (nb > 128) tc_match2_kernel<2, 1><<<grid, 256, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, 1, h->best, h->lists, h->counter, so, io, h->trace);
-      else tc_match2_kernel<1, 1><<<grid, 256, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, 1, h->best, h->lists, h->counter, so, io, h->trace);
-    } else {
-      if (nb > 128) tc_match2_kernel<2, MT_KMAX><<<grid, 256, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best, h->lists, h->counter, so, io, h->trace);
-      else tc_match2_kernel<1, MT_KMAX><<<grid, 256, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best, h->lists, h->counter, so, io, h->trace);
-    }
+    if (k == 1) tc_match_kernel<1><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, 1, h->best, h->lists, h->counter, so, io);
+    else tc_match_kernel<MT_KMAX><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best, h->lists, h->counter, so, io);
     AAE_LAUNCH_OK();
   }
-  if (h->trace) print_trace(h, grid, s);
   return AAE_OK;
 }
 

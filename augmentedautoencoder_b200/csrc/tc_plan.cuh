@@ -60,15 +60,7 @@ __device__ __forceinline__ float tc_dyn_unscale(unsigned amax_bits) { return __i
 constexpr float ACT_SCALE = 16.f;     // activations (and the [0,1] input) are stored as 16 * x
 constexpr float W_SCALE = 256.f;      // weights are stored as 256 * w
 constexpr int TC_STAGES = 2;
-constexpr int TC_THREADS = 512;       // warp 0 TMA, 1 MMA, 2 TMEM allocator, 3 idle, 4-15 epilogue (three per TMEM lane quadrant)
-// Threads actually launched: 512 by default.  Measured in one process (scripts/ab_inproc.py, +-0.1 %): twelve epilogue warps
-// instead of eight take conv2 / conv3 / conv4 from 1.029 / 0.886 / 0.458 to 1.000 / 0.871 / 0.452 ms (the exposed epilogue shrinks);
-// four warps: 1.170 / 0.941 / 0.468.  AAE_TC_EPI8=1 -> 384 threads, AAE_TC_EPI4=1 -> 256 (read per launch: "1" = on).
-inline int tc_block_threads() {
-  const char* e4 = getenv("AAE_TC_EPI4");
-  const char* e8 = getenv("AAE_TC_EPI8");
-  return (e4 && e4[0] == '1') ? 256 : ((e8 && e8[0] == '1') ? 384 : 512);
-}
+constexpr int TC_THREADS = 384;       // warp 0 TMA, 1-3 idle, warpgroups 1-2 (warps 4-11) wgmma + epilogue
 
 struct TcLayer {
   int in_h, in_w, in_c, out_h, out_w, out_c;   // conv geometry (input is the space-to-depth tensor [B, in_h/2, in_w/2, 4*in_c])
@@ -76,14 +68,9 @@ struct TcLayer {
   __half *in_hi = nullptr, *in_lo = nullptr;    // activations entering this layer
   __half *w_hi = nullptr, *w_lo = nullptr;      // packed weights [out_c][taps*in_c]
   CUtensorMap tm_a_hi, tm_a_lo, tm_w_hi, tm_w_lo;
-  CUtensorMap tm_w2_hi, tm_w2_lo;               // weight tile halves (128 rows) for the CTA-pair kernel
-  CUtensorMap tm_o_hi, tm_o_lo;                 // output (= next layer's input) as a store target: box = 32 pixels x 32 channels
-  bool tma_out = false;                         // the persistent pair kernel may ship its epilogue through tm_o_* (TMA tensor stores)
-  const float* tma_f32_base = nullptr;          // OUT_F32: tm_o_hi describes THIS buffer (fp32 [rows, N] seen as fp16 [rows, 2N]); other targets use plain stores
-  bool pair = false;
   TcGemmParams gp;
   int n_tile;
-  int kch;    // K chunk per pipeline stage: 64 (128-byte swizzle) or 32 (64-byte swizzle, 4 stages)
+  int kch;    // K chunk per pipeline stage: 64 (128-byte swizzle) or 32 (64-byte swizzle)
 };
 
 // bits of the range flag word: bit l = the activation written by conv layer l (0-based; the decoder counts dense_1 as 0)
@@ -209,66 +196,34 @@ __device__ __forceinline__ void tc_store_chunk(const TcGemmParams& p, const TcRo
 }
 
 
-// The same arithmetic as tc_store_chunk's (hi, lo) branch without its per-element mode tests, for the persistent kernel whose
-// epilogue is exposed (profiles/r02_conv_gemm_trace.txt): ReLU or identity, bias absent or 16-byte aligned, any of the three
-// (hi, lo) layouts.  v / x are the raw hh and cross-term accumulators.
-__device__ __forceinline__ bool tc_lean_epilogue_ok(const TcGemmParams& p) {
-  return (p.out_mode == OUT_S2D_SPLIT || p.out_mode == OUT_PLAIN_SPLIT || p.out_mode == OUT_D2S_SPLIT) && p.relu != 2 &&
-         (reinterpret_cast<uintptr_t>(p.bias) & 15) == 0;
-}
-// bias + activation + range guard + (hi, lo) split of one 32-column chunk: hi[k] / lo[k] = packed fp16 pair of columns 2k, 2k+1
-template <bool BIAS>
-__device__ __forceinline__ void tc_lean_chunk_t(const TcGemmParams& p, int n, const uint32_t (&v)[32], const uint32_t (&x)[32], float unscale,
-                                                float floor_v, uint32_t (&hi)[16], uint32_t (&lo)[16]) {
-  const float4* bp = reinterpret_cast<const float4*>(p.bias + n);
-  const float os = p.out_scale;
-  float amax = 0.f;
+// The two consumer warpgroups' accumulators (rows 64 wg .. 64 wg + 63, main and cross term) -> the fp32 image [128][ld]
+// that the row-per-thread epilogue reads (it takes the place of the stage ring once every MMA has completed).
+template <int R>
+__device__ __forceinline__ void tc_park_acc(float* img, int ld, int wg, int warp, int lane, const float (&acc)[R], const float (&crs)[R]) {
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = (lane & 3) * 2;
 #pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const float4 b = BIAS ? __ldg(bp + (j >> 2)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const float a0 = fmaxf(__fadd_rn(__fmul_rn(__fadd_rn(__uint_as_float(v[j]), __uint_as_float(x[j])), unscale), b.x), floor_v);
-    const float a1 = fmaxf(__fadd_rn(__fmul_rn(__fadd_rn(__uint_as_float(v[j + 1]), __uint_as_float(x[j + 1])), unscale), b.y), floor_v);
-    const float a2 = fmaxf(__fadd_rn(__fmul_rn(__fadd_rn(__uint_as_float(v[j + 2]), __uint_as_float(x[j + 2])), unscale), b.z), floor_v);
-    const float a3 = fmaxf(__fadd_rn(__fmul_rn(__fadd_rn(__uint_as_float(v[j + 3]), __uint_as_float(x[j + 3])), unscale), b.w), floor_v);
-    amax = fmaxf(fmaxf(amax, fmaxf(fabsf(a0), fabsf(a1))), fmaxf(fabsf(a2), fabsf(a3)));
-    tc::split_f16x2(a0 * os, a1 * os, hi[j >> 1], lo[j >> 1]);
-    tc::split_f16x2(a2 * os, a3 * os, hi[(j >> 1) + 1], lo[(j >> 1) + 1]);
+  for (int j = 0; j < R / 4; ++j) {
+    *reinterpret_cast<float2*>(img + r0 * ld + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(img + (r0 + 8) * ld + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    *reinterpret_cast<float2*>(img + r0 * ld + 2 * R + 8 * j + c0) = make_float2(crs[4 * j], crs[4 * j + 1]);
+    *reinterpret_cast<float2*>(img + (r0 + 8) * ld + 2 * R + 8 * j + c0) = make_float2(crs[4 * j + 2], crs[4 * j + 3]);
   }
-  if (p.range_flag != nullptr && !(amax * os < TC_F16_OVERFLOW)) atomicOr(p.range_flag, p.range_bit);
 }
-__device__ __forceinline__ void tc_lean_chunk(const TcGemmParams& p, int n, const uint32_t (&v)[32], const uint32_t (&x)[32], float unscale,
-                                              float floor_v, uint32_t (&hi)[16], uint32_t (&lo)[16]) {
-  if (p.bias != nullptr) tc_lean_chunk_t<true>(p, n, v, x, unscale, floor_v, hi, lo);
-  else tc_lean_chunk_t<false>(p, n, v, x, unscale, floor_v, hi, lo);
-}
-__device__ __forceinline__ void tc_store_chunk_lean(const TcGemmParams& p, const TcRow& r, int n, const uint32_t (&v)[32], const uint32_t (&x)[32],
-                                                    float unscale, float floor_v) {
-  uint32_t hi[16], lo[16];
-  tc_lean_chunk(p, n, v, x, unscale, floor_v, hi, lo);
-  long long off = r.row_off + n;
-  if (p.out_mode == OUT_D2S_SPLIT) {
-    const int cq = p.N >> 2, cls = n / cq, co = n - cls * cq;     // a 32-column chunk never straddles a parity class (cq % 32 == 0)
-    off = ((long long)(r.b * 2 * p.OH + 2 * r.i + (cls >> 1)) * (2 * p.OW) + 2 * r.j + (cls & 1)) * cq + co;
-  }
-  uint4* dh = reinterpret_cast<uint4*>(p.out_hi + off);
-  uint4* dl = reinterpret_cast<uint4*>(p.out_lo + off);
+__device__ __forceinline__ void tc_acc_ld32(const float* img, int ld, int row, int col, uint32_t (&v)[32]) {
+  const float4* src = reinterpret_cast<const float4*>(img + row * ld + col);
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    dh[j] = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-    dl[j] = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
+  for (int j = 0; j < 8; ++j) {
+    const float4 f = src[j];
+    v[4 * j] = __float_as_uint(f.x); v[4 * j + 1] = __float_as_uint(f.y); v[4 * j + 2] = __float_as_uint(f.z); v[4 * j + 3] = __float_as_uint(f.w);
   }
 }
 
-// launches the GEMM kernel instantiation that matches the layer's tile shape (CTA pair / single CTA, N tile, K chunk)
+// launches the GEMM kernel instantiation that matches the layer's tile shape (N tile, K chunk)
 int tc_launch_layer(const TcLayer& T, dim3 grid, cudaStream_t s);
 int tc_dev_alloc(void** p, size_t bytes);
 // Tensor maps + packed-weight storage of a layer whose A operand is a PLAIN NHWC (hi, lo) tensor [B_pad, in_h, in_w, in_c]
 // (taps = unit-stride boxes): fills tm_a_*, allocates w_hi/w_lo [ceil(N / n_tile) * n_tile][taps * in_c] and their maps.
 // T.{in_h,in_w,in_c,taps,BW,BH,BB,n_tile,kch,gp.N} must be set; with alloc_input = false T.in_hi/in_lo are the caller's.
-int tc_layer_setup_plain(TcLayer& T, int B, bool pair_ok, bool alloc_input);
-// Store-side tensor maps for the persistent pair kernel's epilogue (T.tma_out): the (hi, lo) output of a layer whose gp.out_mode
-// is OUT_S2D_SPLIT / OUT_PLAIN_SPLIT / OUT_D2S_SPLIT (out_rows_pad = images the destination buffers hold), or an fp32 [rows, N]
-// buffer for OUT_F32 (out_rows_pad = rows it holds).  Leaves T.tma_out false when the geometry has no 32-pixel box.
-int tc_layer_setup_out_maps(TcLayer& T, long long out_rows_pad);
+int tc_layer_setup_plain(TcLayer& T, int B, bool alloc_input);
 
 }  // namespace aae

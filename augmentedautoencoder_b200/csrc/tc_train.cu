@@ -10,7 +10,7 @@
 //                               encoder 5x5/s2 layer   : W'[(py,px,ci)][(tap', co)] = W[3 - 2ty + py][3 - 2tx + px][ci][co]  (0 outside 5x5)
 //                             i.e. the transposed stride-2 conv is a 3x3 conv producing the space-to-depth form of dX.
 //   wgrad  dW = X^T G         contraction over pixels: both operands are read straight from their NHWC tensors as
-//                             MN-major tcgen05 operands (channels contiguous), no transposed copies (tc_wgrad_kernel).
+//                             MN-major wgmma operands (channels contiguous), no transposed copies (tc_wgrad_kernel).
 //
 // Gradients have no a-priori range, so every G tensor is stored as (hi, lo) fp16 of  G * 2^k  with k chosen per tensor and
 // per step from its largest magnitude (tc_dyn_scale): dgrad/wgrad results are written as raw fp32, a small elementwise
@@ -38,7 +38,7 @@ struct TcWgradParams {
   int chunks_per_split;    // K chunks per blockIdx.z
   int8_t tap_di[32], tap_dj[32];
   int tap_ch[32];          // channel offset of the tap's parity plane in X
-  int m_tiles;             // taps * cin_blocks (the CTA-pair kernel pads an odd count with an idle CTA)
+  int m_tiles;             // taps * cin_blocks
   TcGemmParams ep;         // epilogue: OUT_F32 partials [splits][taps*Cin][N]
 };
 
@@ -48,33 +48,25 @@ struct WgSmem {
   static constexpr int X_BYTES = 128 * KP * 2;           // two 64-channel boxes of KP rows x 128 B
   static constexpr int G_BYTES = N_TILE * KP * 2;
   static constexpr int STAGE_BYTES = 2 * X_BYTES + 2 * G_BYTES;
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 + 256;
+  static constexpr int ACC_LD = 2 * N_TILE + 4;          // fp32 accumulator image [128][ACC_LD] (main | cross)
+  static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
+  static constexpr int BODY = STAGES * STAGE_BYTES > ACC_BYTES ? STAGES * STAGE_BYTES : ACC_BYTES;
+  static constexpr int TOTAL = BODY + 1024 + 256;
 };
 
-// MN-major operand in the 128-byte-swizzle canonical layout: K rows (pixels) of 128 B = 64 fp16 channels, 8-row groups SBO
-// apart, successive 64-channel atoms LBO apart (cute::UMMA canonical ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units).
-__device__ __forceinline__ uint64_t make_sw128_mnmajor_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(lbo_bytes >> 4) << 16;
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
+// Both operands are MN-major (channels contiguous, K = pixels): warpgroup wg takes the X box of channels [64 wg, 64 wg + 64) as
+// its 64 rows of A, and the whole G tile (N_TILE / 64 boxes, LBO apart) as B.
 template <int N_TILE, int STAGES>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_wgrad_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
                 const __grid_constant__ CUtensorMap tm_g_hi, const __grid_constant__ CUtensorMap tm_g_lo, const TcWgradParams p) {
   using S = WgSmem<N_TILE, STAGES>;
+  constexpr int R = N_TILE / 2;
   constexpr int BOX_BYTES = 64 * S::KP * 2;   // one TMA box: 64 channels x KP pixels
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::BODY);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tap = blockIdx.x / p.cin_blocks, cb = blockIdx.x - tap * p.cin_blocks;
@@ -83,17 +75,12 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_consta
   const int q_begin = blockIdx.z * p.chunks_per_split;
   const int q_end = min(p.total_chunks, q_begin + p.chunks_per_split);
 
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tm_x_hi); prefetch_tmap(&tm_x_lo); prefetch_tmap(&tm_g_hi); prefetch_tmap(&tm_g_lo); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(tmem_full_bar, 1);
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tm_x_hi); prefetch_tmap(&tm_x_lo); prefetch_tmap(&tm_g_hi); prefetch_tmap(&tm_g_lo);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<2 * N_TILE>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -119,182 +106,56 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(128, N_TILE, 0) | (1u << 15) | (1u << 16);   // both operands MN-major
-      for (int q = q_begin, i = 0; q < q_end; ++q, ++i) {
-        const int s = i % STAGES;
-        mbar_wait(&full_bar[s], ((uint32_t)(i / STAGES)) & 1u);
-        tc_fence_after();
-        const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
-#pragma unroll
-        for (int k = 0; k < S::KP / 16; ++k) {
-          const uint32_t ko = (uint32_t)k * 16u * 128u;   // 16 pixel rows of 128 B
-          const uint64_t x_hi = make_sw128_mnmajor_desc(st + ko, BOX_BYTES, 1024);
-          const uint64_t x_lo = make_sw128_mnmajor_desc(st + S::X_BYTES + ko, BOX_BYTES, 1024);
-          const uint64_t g_hi = make_sw128_mnmajor_desc(st + 2 * S::X_BYTES + ko, BOX_BYTES, 1024);
-          const uint64_t g_lo = make_sw128_mnmajor_desc(st + 2 * S::X_BYTES + S::G_BYTES + ko, BOX_BYTES, 1024);
-          const uint32_t first = (i > 0 || k > 0) ? 1u : 0u;
-          umma_f16(tmem_base, x_hi, g_hi, idesc, first);
-          umma_f16(tmem_base + N_TILE, x_lo, g_hi, idesc, first);
-          umma_f16(tmem_base + N_TILE, x_hi, g_lo, idesc, 1u);
-        }
-        umma_commit(&empty_bar[s]);
-      }
-      umma_commit(tmem_full_bar);
-    }
   } else if (warp >= 4) {
+    const int wg = (warp - 4) >> 2;
+    float acc[R], crs[R];
+#pragma unroll
+    for (int j = 0; j < R; ++j) { acc[j] = 0.f; crs[j] = 0.f; }
+    for (int q = q_begin, i = 0; q < q_end; ++q, ++i) {
+      const int s = i % STAGES;
+      mbar_wait(&full_bar[s], ((uint32_t)(i / STAGES)) & 1u);
+      const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
+      wgmma_fence_regs(acc); wgmma_fence_regs(crs);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < S::KP / 16; ++k) {
+        const uint32_t ko = (uint32_t)k * 16u * 128u;   // 16 pixel rows of 128 B
+        const uint64_t x_hi = make_sw128_mnmajor_desc(st + wg * BOX_BYTES + ko, BOX_BYTES, 1024);
+        const uint64_t x_lo = make_sw128_mnmajor_desc(st + S::X_BYTES + wg * BOX_BYTES + ko, BOX_BYTES, 1024);
+        const uint64_t g_hi = make_sw128_mnmajor_desc(st + 2 * S::X_BYTES + ko, BOX_BYTES, 1024);
+        const uint64_t g_lo = make_sw128_mnmajor_desc(st + 2 * S::X_BYTES + S::G_BYTES + ko, BOX_BYTES, 1024);
+        const uint32_t first = (i > 0 || k > 0) ? 1u : 0u;
+        Wgmma<N_TILE>::template ss<1, 1>(acc, x_hi, g_hi, first);
+        Wgmma<N_TILE>::template ss<1, 1>(crs, x_lo, g_hi, first);
+        Wgmma<N_TILE>::template ss<1, 1>(crs, x_hi, g_lo, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      wgmma_fence_regs(acc); wgmma_fence_regs(crs);
+      if (i > 0 && (warp & 3) == 0 && lane == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc); wgmma_fence_regs(crs);
+    named_bar_sync(1, 256);
+    float* img = reinterpret_cast<float*>(smem);
+    tc_park_acc(img, S::ACC_LD, wg, warp, lane, acc, crs);
+    named_bar_sync(1, 256);
     const int q4 = warp & 3, half = (warp - 4) >> 2;
-    const int epi_groups = ((int)blockDim.x >> 5) > 8 ? 2 : 1;
     const TcRow row = tc_decode_row(p.ep, m0 + q4 * 32 + lane);
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
     const bool has_work = q_end > q_begin;
     const float unscale = p.ep.amax_bits ? p.ep.unscale * tc_dyn_unscale(__ldg(p.ep.amax_bits)) : p.ep.unscale;
 #pragma unroll 1
-    for (int c = half; c < N_TILE / 32; c += epi_groups) {
-      uint32_t v[32], x[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(c * 32), v);
-      tmem_ld_32x32(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(N_TILE + c * 32), x);
-      tmem_ld_wait();
+    for (int c = half; c < N_TILE / 32; c += 2) {
       const int n = n0 + c * 32;
       if (!row.valid || n >= p.ep.N) continue;
+      uint32_t v[32], x[32];
+      tc_acc_ld32(img, S::ACC_LD, q4 * 32 + lane, c * 32, v);
+      tc_acc_ld32(img, S::ACC_LD, q4 * 32 + lane, N_TILE + c * 32, x);
       float f[32];
 #pragma unroll
       for (int j = 0; j < 32; ++j) f[j] = has_work ? (__uint_as_float(v[j]) + __uint_as_float(x[j])) * unscale : 0.f;
       tc_store_chunk(p.ep, row, n, f, (int)blockIdx.z);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<2 * N_TILE>(tmem_base);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------- wgrad on CTA pairs
-// Same contraction with cta_group::2: two M tiles (consecutive (tap, channel-block) pairs) share one 256-column G tile and
-// run as ONE M = 256 MMA; each CTA stages its own X tile and only HALF of the G tile (128 columns), i.e. 32 KB instead of
-// 48 KB per K chunk, which is what bounds the single-CTA kernel (shared-memory bandwidth, see tc_gemm2_kernel).
-template <int STAGES>
-struct WgSmem2 {
-  static constexpr int KP = 32;
-  static constexpr int T_BYTES = 128 * KP * 2;            // X tile and G half tile: 128 channels x KP pixels
-  static constexpr int STAGE_BYTES = 4 * T_BYTES;         // X_hi, X_lo, G_hi(half), G_lo(half)
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 + 256;
-};
-
-template <int STAGES>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1)
-tc_wgrad2_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
-                 const __grid_constant__ CUtensorMap tm_g_hi, const __grid_constant__ CUtensorMap tm_g_lo, const TcWgradParams p) {
-  using S = WgSmem2<STAGES>;
-  constexpr int N_TILE = 256;
-  constexpr int BOX_BYTES = 64 * S::KP * 2;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * S::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  // an odd number of M tiles is padded to whole pairs: the extra CTA repeats the last tile's loads and writes nothing
-  const int mt = min((int)blockIdx.x, p.m_tiles - 1);
-  const int tap = mt / p.cin_blocks, cb = mt - tap * p.cin_blocks;
-  const int m0 = blockIdx.x * 128;
-  const int n0 = blockIdx.y * N_TILE;
-  const int q_begin = blockIdx.z * p.chunks_per_split;
-  const int q_end = min(p.total_chunks, q_begin + p.chunks_per_split);
-
-  if (warp == 0 && lane == 0) { prefetch_tmap(&tm_x_hi); prefetch_tmap(&tm_x_lo); prefetch_tmap(&tm_g_hi); prefetch_tmap(&tm_g_lo); }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(tmem_full_bar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc_2sm<512>(tmem_ptr);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      const int cols = p.OW / p.BWk;
-      const int cx = p.tap_ch[tap] + cb * 128;
-      const int di = p.tap_di[tap], dj = p.tap_dj[tap];
-      const int gn = n0 + (int)rank * 128;
-      for (int q = q_begin, i = 0; q < q_end; ++q, ++i) {
-        const int s = i % STAGES;
-        mbar_wait(&empty_bar[s], (((uint32_t)(i / STAGES)) & 1u) ^ 1u);
-        const int b = q / p.chunks_per_image, r = q - b * p.chunks_per_image;
-        const int y0 = (r / cols) * p.BHk, x0 = (r - (r / cols) * cols) * p.BWk;
-        uint8_t* st = smem + s * S::STAGE_BYTES;
-        if (leader) mbar_arrive_expect_tx(&full_bar[s], 2 * S::STAGE_BYTES);
-        const uint32_t lb = leader_bar_addr(&full_bar[s]);
-#pragma unroll
-        for (int g = 0; g < 2; ++g) {
-          tma_load_4d_2sm(st + g * BOX_BYTES, &tm_x_hi, lb, cx + 64 * g, x0 + dj, y0 + di, b);
-          tma_load_4d_2sm(st + S::T_BYTES + g * BOX_BYTES, &tm_x_lo, lb, cx + 64 * g, x0 + dj, y0 + di, b);
-          tma_load_4d_2sm(st + 2 * S::T_BYTES + g * BOX_BYTES, &tm_g_hi, lb, gn + 64 * g, x0, y0, b);
-          tma_load_4d_2sm(st + 3 * S::T_BYTES + g * BOX_BYTES, &tm_g_lo, lb, gn + 64 * g, x0, y0, b);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(256, N_TILE, 0) | (1u << 15) | (1u << 16);
-      for (int q = q_begin, i = 0; q < q_end; ++q, ++i) {
-        const int s = i % STAGES;
-        mbar_wait(&full_bar[s], ((uint32_t)(i / STAGES)) & 1u);
-        tc_fence_after();
-        const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
-#pragma unroll
-        for (int k = 0; k < S::KP / 16; ++k) {
-          const uint32_t ko = (uint32_t)k * 16u * 128u;
-          const uint64_t x_hi = make_sw128_mnmajor_desc(st + ko, BOX_BYTES, 1024);
-          const uint64_t x_lo = make_sw128_mnmajor_desc(st + S::T_BYTES + ko, BOX_BYTES, 1024);
-          const uint64_t g_hi = make_sw128_mnmajor_desc(st + 2 * S::T_BYTES + ko, BOX_BYTES, 1024);
-          const uint64_t g_lo = make_sw128_mnmajor_desc(st + 3 * S::T_BYTES + ko, BOX_BYTES, 1024);
-          const uint32_t first = (i > 0 || k > 0) ? 1u : 0u;
-          umma_f16_2sm(tmem_base, x_hi, g_hi, idesc, first);
-          umma_f16_2sm(tmem_base + N_TILE, x_lo, g_hi, idesc, first);
-          umma_f16_2sm(tmem_base + N_TILE, x_hi, g_lo, idesc, 1u);
-        }
-        umma_commit_2sm(&empty_bar[s]);
-      }
-      umma_commit_2sm(tmem_full_bar);
-    }
-  } else if (warp >= 4) {
-    const int q4 = warp & 3, half = (warp - 4) >> 2;
-    const int epi_groups = ((int)blockDim.x >> 5) > 8 ? 2 : 1;
-    const TcRow row = tc_decode_row(p.ep, m0 + q4 * 32 + lane);
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    const float unscale = p.ep.amax_bits ? p.ep.unscale * tc_dyn_unscale(__ldg(p.ep.amax_bits)) : p.ep.unscale;
-#pragma unroll 1
-    for (int c = half; c < N_TILE / 32; c += epi_groups) {
-      uint32_t v[32], x[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(c * 32), v);
-      tmem_ld_32x32(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(N_TILE + c * 32), x);
-      tmem_ld_wait();
-      const int n = n0 + c * 32;
-      if (!row.valid || n >= p.ep.N) continue;
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = (__uint_as_float(v[j]) + __uint_as_float(x[j])) * unscale;
-      tc_store_chunk(p.ep, row, n, f, (int)blockIdx.z);
-    }
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2sm<512>(tmem_base);
   }
 }
 
@@ -603,7 +464,7 @@ __global__ void compact_cols_kernel(const float* __restrict__ in, long long rows
 
 inline unsigned ew_grid(long long n, int threads = 256) {
   long long b = (n + threads - 1) / threads;
-  return (unsigned)std::max<long long>(1, std::min<long long>(b, 148 * 16));
+  return (unsigned)std::max<long long>(1, std::min<long long>(b, 132 * 16));
 }
 
 // First encoder layer (Cin = 3, K = 75): its weight gradient is a 1x1 wgrad GEMM over the im2col matrix of the input image.
@@ -642,19 +503,7 @@ int launch_wgrad(const CUtensorMap& xh, const CUtensorMap& xl, const CUtensorMap
   using S = WgSmem<N_TILE, STAGES>;
   auto kern = tc_wgrad_kernel<N_TILE, STAGES>;
   AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-  kern<<<grid, tc_block_threads(), S::TOTAL, s>>>(xh, xl, gh, gl, p);
-  AAE_LAUNCH_OK();
-  return AAE_OK;
-}
-
-template <int STAGES>
-int launch_wgrad2(const CUtensorMap& xh, const CUtensorMap& xl, const CUtensorMap& gh, const CUtensorMap& gl, const TcWgradParams& p, dim3 grid,
-                  cudaStream_t s) {
-  using S = WgSmem2<STAGES>;
-  auto kern = tc_wgrad2_kernel<STAGES>;
-  AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-  grid.x = (grid.x + 1) & ~1u;
-  kern<<<grid, tc_block_threads(), S::TOTAL, s>>>(xh, xl, gh, gl, p);
+  kern<<<grid, TC_THREADS, S::TOTAL, s>>>(xh, xl, gh, gl, p);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -725,7 +574,7 @@ static int make_wgrad_maps(TcUnit& U, int x_c_total, int x_bpad, int g_bpad) {
   w.ep.OH = w.ep.OW = 1;
   w.ep.unscale = 1.f / ACT_SCALE;
   w.m_tiles = U.taps_w * w.cin_blocks;
-  U.wg_n_tile = U.gN >= 256 ? 256 : 64;
+  U.wg_n_tile = U.gN % 128 == 0 ? 128 : 64;
   return AAE_OK;
 }
 
@@ -746,8 +595,8 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     T.out_h = U.gh; T.out_w = U.gw; T.out_c = U.nd;
     T.taps = U.dg_taps;
     T.BW = U.gw; T.BH = std::min(U.gh, 128 / T.BW); T.BB = 128 / (T.BW * T.BH);
-    T.n_tile = U.nd >= 256 ? 256 : 128;
-    T.kch = T.n_tile == 256 ? 32 : 64;
+    T.n_tile = 128;
+    T.kch = 64;
     if (U.gw > 128 || (U.gw & (U.gw - 1)) || (U.gh & (U.gh - 1)) || U.gN % T.kch != 0 || U.nd % T.n_tile != 0 || U.cin % 128 != 0 ||
         U.gN % 64 != 0 || (U.gh * U.gw) % 32 != 0) {
       set_error("tensor-core trainer: layer geometry unsupported (G %dx%dx%d, dgrad N %d, Cin %d)", U.gh, U.gw, U.gN, U.nd, U.cin);
@@ -763,7 +612,7 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     }
     g.unscale = 1.f / W_SCALE;
     g.out_mode = OUT_F32;
-    AAE_TRY(tc_layer_setup_plain(T, B, /*pair_ok=*/true, /*alloc_input=*/true));
+    AAE_TRY(tc_layer_setup_plain(T, B, /*alloc_input=*/true));
     U.x_hi = F.in_hi; U.x_lo = F.in_lo;
     const int x_bpad = (int)ceil_div(B, F.BB) * F.BB, g_bpad = (int)ceil_div(B, T.BB) * T.BB;
     AAE_TRY(make_wgrad_maps(U, x_c_total, x_bpad, g_bpad));
@@ -824,13 +673,6 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
   if (st == AAE_OK) st = tc_dev_alloc((void**)&h->partials, part_max * sizeof(float));
   if (st == AAE_OK) st = tc_dev_alloc((void**)&h->wm, wm_max * sizeof(float));
   h->raw_floats = raw_max; h->partial_floats = part_max; h->wm_floats = wm_max;
-  // the persistent pair kernel ships unsplit dgrad results to `raw` with tensor stores
-  for (size_t u = 0; u < h->units.size() && st == AAE_OK; ++u) {
-    TcLayer& T = h->units[u].dg;
-    if (!T.pair) continue;
-    T.gp.out_f32 = h->raw;
-    st = tc_layer_setup_out_maps(T, (long long)(raw_max / (size_t)T.gp.N));
-  }
   if (st != AAE_OK) { tc_train_destroy(h); return st; }
   *out = h;
   return AAE_OK;
@@ -910,7 +752,7 @@ int tc_train_unit_wgrad(TcTrainPlan* h, int u, int B, float* dw_out, cudaStream_
   w.total_chunks = B * w.chunks_per_image;
   const int m_tiles = U.taps_w * w.cin_blocks, n_tiles = U.gN / U.wg_n_tile;
   const long long mn = (long long)w.ep.M * w.ep.N;
-  int splits = (int)std::max<long long>(1, (444 + (long long)m_tiles * n_tiles / 2) / ((long long)m_tiles * n_tiles));
+  int splits = (int)std::max<long long>(1, (396 + (long long)m_tiles * n_tiles / 2) / ((long long)m_tiles * n_tiles));
   splits = std::min(splits, std::max(1, w.total_chunks / 16));
   splits = (int)std::min<long long>(splits, (long long)(h->partial_floats / (size_t)mn));
   AAE_REQUIRE(splits >= 1, "tc trainer: wgrad partial scratch too small");
@@ -919,8 +761,7 @@ int tc_train_unit_wgrad(TcTrainPlan* h, int u, int B, float* dw_out, cudaStream_
   w.ep.amax_bits = h->amax + u;
   w.ep.out_f32 = h->partials;
   dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)splits);
-  if (U.wg_n_tile == 256 && getenv("AAE_WG_1CTA") == nullptr) AAE_TRY((launch_wgrad2<6>(U.tm_x_hi, U.tm_x_lo, U.tm_g_hi, U.tm_g_lo, w, grid, s)));
-  else if (U.wg_n_tile == 256) AAE_TRY((launch_wgrad<256, 4>(U.tm_x_hi, U.tm_x_lo, U.tm_g_hi, U.tm_g_lo, w, grid, s)));
+  if (U.wg_n_tile == 128) AAE_TRY((launch_wgrad<128, 6>(U.tm_x_hi, U.tm_x_lo, U.tm_g_hi, U.tm_g_lo, w, grid, s)));
   else AAE_TRY((launch_wgrad<64, 6>(U.tm_x_hi, U.tm_x_lo, U.tm_g_hi, U.tm_g_lo, w, grid, s)));
   if (U.gN == U.n_real) return launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, dw_out, s);
   AAE_REQUIRE((size_t)mn <= h->wm_floats, "tc trainer: merged-gradient scratch too small");
@@ -959,7 +800,7 @@ int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s) {
   const int m_tiles = (int)ceil_div(T.gp.M, 128), n_tiles = U.nd / T.n_tile;
   const int total_iters = T.gp.taps * T.gp.chunks_per_tap;
   // few output tiles and a long K (the 8x8 layers): split K so that the grid covers the SMs, fold the partials afterwards
-  int splits = std::max(1, 148 / std::max(1, ((m_tiles + 1) & ~1) * n_tiles));
+  int splits = std::max(1, 132 / std::max(1, m_tiles * n_tiles));
   splits = std::min(splits, std::max(1, total_iters / 64));
   const long long mn = (long long)T.gp.M * U.nd;
   if ((size_t)splits * (size_t)mn > h->partial_floats) splits = 1;
@@ -992,7 +833,7 @@ int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool want_f32, bool 
   const int C = U.enc ? U.cin : U.nd;
   const int gpr = U.nd / 8;                          // 8-column groups per raw row
   // with the fused column sums every block leaves one partial row: 4 blocks per SM keep the fold short
-  const unsigned grid = db_out ? std::min(ew_grid(groups), 148u * 4u) : ew_grid(groups);
+  const unsigned grid = db_out ? std::min(ew_grid(groups), 132u * 4u) : ew_grid(groups);
   float* colsum = nullptr;
   if (db_out) {
     AAE_REQUIRE(gpr <= 256 && 256 % gpr == 0, "tc trainer: %d columns unsupported by the fused bias gradient", U.nd);

@@ -2,7 +2,7 @@
 """bench.py -- pose queries/sec (encode + codebook NN) on 128x128 crops (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision simt|tc]
-                    [--workload infer|sharded|routed|train|process] [--batches-per-step M]
+                    [--workload infer|sharded|routed|train|process] [--batches-per-step M] [--dump-outputs DIR]
 
 infer (default, BASELINE.json configs[1]): one BATCH = 256 synthetic uint8 crops through the hot path: conv encoder -> latent
     -> fused L2-normalise + cosine match against the 92 232-row codebook -> (score, index) per crop.  One "step" = M (default
@@ -50,10 +50,6 @@ ROUTED_OBJECTS = 8
 ENC_FLOP_PER_CROP = 2 * 2140667904            # SURVEY.md section 8(d)
 LAYER_MAC_PER_CROP = [39321600, 838860800, 838860800, 419430400, 4194304]
 MATCH_BYTES = N_ROWS * LATENT * 4 + BATCH * LATENT * 4 + BATCH * 8
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the `ncu --set full` captures of this exact workload
-# (profiles/r02_ncu_*.txt, conv2 / conv3 from the re-capture r02b_ncu_*.txt; precision=tc, batch 256).  Algorithmic bytes beside them: conv1 = 12.6 MB crops + 537 MB (hi,lo)
-# output; conv2 = 537 MB (hi,lo) input + 3.3 MB weights + 268 MB output = 808 MB; match = 47.36 MB.
-NCU_TRAFFIC = {"tc": {"conv1": 12700160 + 482454784, "conv2": 559772160 + 239571968, "conv3": 619160064 + 117579264, "match": 47427584 + 0}}
 METRIC = "pose queries/sec (encode+codebook NN)"
 
 
@@ -63,7 +59,8 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "src": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- not reached figures
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler(threading.Thread):
@@ -121,6 +118,16 @@ def pin_to_gpu_numa(index):
     except Exception:  # noqa: BLE001
         pass
     return None
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes what the timed path returned in its last step as out_dir/<name>.npy: floating arrays as float32, integer
+    arrays as float64 (exact for indices below 2^53)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        a = a.astype(np.float32) if np.issubdtype(a.dtype, np.floating) else a.astype(np.float64)
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def pct(xs, q):
@@ -506,7 +513,7 @@ def run_ours(args, rank, world, local_rank):
     n_ring = 4
     host_crops = [torch.randint(0, 256, (BATCH, 128, 128, 3), dtype=torch.uint8, generator=g).pin_memory() for _ in range(n_ring)]
     dev_crops = [c.to(dev) for c in host_crops]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
     enc_h, cb_h = enc.handle(dev), cb.handle(dev)
     M = max(1, args.batches_per_step)
     n_batches = args.steps * M
@@ -531,10 +538,12 @@ def run_ours(args, rank, world, local_rank):
         flush.zero_()
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
-        batch_device(i)
+        last = batch_device(i)
         b.record()
         evs.append((a, b))
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"scores": last[0], "indices": last[1]})
     if world > 1:
         dist.barrier()
     launches = lib.aae_launch_count() - launches0
@@ -615,9 +624,8 @@ def run_ours(args, rank, world, local_rank):
         peak = pk["tf_burst"]
         names = ["conv1 (3->128)", "conv2 (128->256)", "conv3 (256->512)", "conv4 (512->512)", "dense (32768->128)"]
         products = 3 if args.precision == "tc" else 1
-        traffic = NCU_TRAFFIC.get(args.precision, {}).get(["conv1", "conv2", "conv3", "conv4", "dense"][dom])
         roof = {"kernel": "encoder " + names[dom], "bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
-                "traffic": traffic, "peak_source": pk["src"] + " bf16 burst", "stage_ms": stage_med,
+                "peak_source": pk["src"] + " bf16 burst", "stage_ms": stage_med,
                 "tensor_pipe": {"products_per_mac": products, "issued_tflops": ach * products, "issued_frac_of_peak": ach * products / peak,
                                 "why": "fp32-grade results need hi*hi + hi*lo + lo*hi on fp16 tensor cores; `achieved` counts each MAC once"},
                 "share_of_step": stage_med[dom] / ms_per_batch,
@@ -627,10 +635,10 @@ def run_ours(args, rank, world, local_rank):
     mm = statistics.median(match_ms) if match_ms else float("nan")
     ach_b = MATCH_BYTES / (mm * 1e-3) / 1e9
     roof_match = {"kernel": "fused codebook match (l2norm + scores + argmax)", "bound": "hbm", "achieved": ach_b, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                  "frac": ach_b / pk["hbm_gbs"], "traffic": NCU_TRAFFIC.get(args.precision, {}).get("match"), "ms": mm, "bytes": MATCH_BYTES,
+                  "frac": ach_b / pk["hbm_gbs"], "ms": mm, "bytes": MATCH_BYTES,
                   "peak_source": pk["src"],
-                  "regime": "B=256 with 3 split-fp16 products per MAC is tensor-bound (18.1 GFLOP issued ~= 10.7 us at the bf16 burst peak > 7.2 us HBM "
-                            "floor); B <= 128 is HBM-bound"}
+                  "regime": "B=256 with 3 split-fp16 products per MAC is tensor-bound on an H100 SXM (18.1 GFLOP issued ~= 18.3 us at the "
+                            "989 TFLOP/s data-sheet rate > 14.1 us HBM floor at 3.35 TB/s); B <= 128 is HBM-bound"}
     cpu = None
     if world == 1 and not args.no_cpu_baseline:
         arm = CpuArm()
@@ -877,7 +885,7 @@ def run_train(args, rank, world, local_rank):
         roof["frac"] = roof["achieved"] / roof["peak"]
     print(json.dumps({"metric": "AAE training steps/sec (batch 64, 128x128)", "value": 1e3 / ms, "unit": "steps/s", "n_gpus": 1, "steps": args.steps,
                       "warmup": warm, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                      "dtype": "f32 (split-fp16 x3 on tcgen05)" if tc else "f32",
+                      "dtype": "f32 (split-fp16 x3 on wgmma)" if tc else "f32",
                       "data": "synthetic", "images_per_s": B * 1e3 / ms,
                       "ms_per_step_stats": {"median": statistics.median(step_ms), "p10": pct(step_ms, 0.1), "p90": pct(step_ms, 0.9)},
                       "config": {"workload": "configs[2]: AAE training step, batch=64", "precision": "tc_split" if tc else "fp32_simt",
@@ -900,7 +908,12 @@ def main():
     ap.add_argument("--no-collective-workloads", action="store_true")
     ap.add_argument("--batches-per-step", type=int, default=16)
     ap.add_argument("--workload", default="infer", choices=["infer", "train", "sharded", "routed", "process"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the scores and codebook indices of the last timed batch as DIR/<name>.npy "
+                         "(infer workload; inputs are seeded, so two builds can be compared output for output)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload != "infer"):
+        ap.error("--dump-outputs is implemented for --impl ours --workload infer")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

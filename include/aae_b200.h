@@ -1,5 +1,5 @@
 /*
- * aae_b200.h -- C ABI of the B200-native Augmented-Autoencoder hot path.
+ * aae_b200.h -- C ABI of the GPU-native Augmented-Autoencoder hot path (NVIDIA H100, sm_90a).
  *
  * The reference (DLR-RM/AugmentedAutoencoder) has no FFI: its device boundary is
  * `tf.Session.run` on a TensorFlow graph (SURVEY.md section 8b).  Each entry point below
@@ -47,9 +47,9 @@ typedef enum {
 
 /* Arithmetic used for the dense contractions (convs, dense layers, codebook scores).
  *   AAE_PREC_FP32_SIMT : IEEE fp32 FMA chains on the CUDA cores (exact-order reference path)
- *   AAE_PREC_TC_SPLIT  : tcgen05 tensor cores, every fp32 operand split into two fp16 terms
+ *   AAE_PREC_TC_SPLIT  : wgmma tensor cores, every fp32 operand split into two fp16 terms
  *                        (hi + 2^-11 lo), three products hi*hi + hi*lo + lo*hi accumulated in
- *                        fp32 TMEM -- fp32-grade results at tensor-core rate. */
+ *                        fp32 registers -- fp32-grade results at tensor-core rate. */
 typedef enum { AAE_PREC_FP32_SIMT = 0, AAE_PREC_TC_SPLIT = 1 } aae_precision;
 
 #define AAE_MAX_LAYERS 8
@@ -74,7 +74,7 @@ typedef struct aae_trainer aae_trainer;
 
 AAE_API int aae_version(void);
 AAE_API const char* aae_last_error_string(void);
-/* 1 if a tcgen05-capable device (compute capability 10.x) is present on `device`, else 0. */
+/* 1 if a wgmma-capable device (compute capability 9.0, H100) is present on `device`, else 0. */
 AAE_API int aae_device_supported(int device);
 /* Total number of CUDA kernels this library has launched in the process (for launch accounting in benchmarks). */
 AAE_API int64_t aae_launch_count(void);
@@ -147,9 +147,9 @@ AAE_API int aae_topk_merge(const float* scores_dev, const int32_t* idx_dev, int 
 AAE_API int aae_topk_merge_packed(const void* packed_dev, int n_shards, int batch, int k,
                                   float* scores_out_dev, int32_t* idx_out_dev, void* stream);
 AAE_API int64_t aae_codebook_rows(const aae_codebook* h);
-/* Measurement aid: launches a kernel shaped like the fused match (one CTA per SM, the same 193 KB of dynamic shared memory, with
- * with_tmem != 0 the same 512-column TMEM allocation) that does no work -- the fixed launch / carveout / allocation cost that every
- * event-timed or ncu-timed figure of that kernel contains (scripts/match_bench.py --floor). */
+/* Measurement aid: launches a kernel shaped like the fused match (one CTA per SM, the same dynamic shared memory) that does no
+ * work -- the fixed launch / carveout cost that every event-timed figure of that kernel contains.  with_tmem is accepted for ABI
+ * compatibility and ignored. */
 AAE_API int aae_launch_floor_probe(int device, int with_tmem, void* stream);
 /* Same contract as aae_encoder_profile; one stage: the whole fused match (k = 1). */
 AAE_API int aae_codebook_profile(aae_codebook* h, int enable, float* stage_ms_out, int capacity);
@@ -193,7 +193,7 @@ AAE_API int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, con
  * The arithmetic follows the handles: encoder and decoder must have been created with the same
  * aae_precision.  AAE_PREC_FP32_SIMT runs every contraction as fp32 FMA chains; AAE_PREC_TC_SPLIT
  * runs the forward pass, the data gradients and the weight gradients of all convs with Cin >= 128
- * as tcgen05 GEMMs (split-fp16 x3, gradients re-scaled per tensor and per step by a power of two),
+ * as wgmma GEMMs (split-fp16 x3, gradients re-scaled per tensor and per step by a power of two),
  * the two dense layers and conv1's weight gradient as fp32 kernels; parameters, Adam state and
  * the gradients returned by aae_trainer_get_grads are fp32 in the reference layouts either way. */
 AAE_API int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate,

@@ -1,5 +1,5 @@
 """In-process A/B of a switch that is read when an encoder plan is CREATED: builds one encoder without and one with the variable,
-alternates them batch by batch and compares the stage times.   python scripts/ab_two_encoders.py AAE_TC_KCH64 1"""
+alternates them batch by batch and compares the stage times.   python scripts/ab_two_encoders.py AAE_C1_V1 1"""
 import ctypes as C
 import os
 import statistics

@@ -1,4 +1,4 @@
-"""GPU parity tests of the tensor-core path (AAE_PREC_TC_SPLIT: tcgen05 + TMA + TMEM, split-fp16 operands) against the
+"""GPU parity tests of the tensor-core path (AAE_PREC_TC_SPLIT: wgmma + TMA, split-fp16 operands) against the
 float64 oracle, layer by layer and end to end.  Same tolerances as the fp32 SIMT path: this path must be fp32-grade."""
 import numpy as np
 import pytest
@@ -130,48 +130,6 @@ def test_tc_path_agrees_with_fp32_path_for_ragged_batches(sess, batch):
         assert abs(cos[j, i0[b]] - cos[j, i1[b]]) < 2e-6, (b, i0[b], i1[b])
 
 
-def test_tma_store_epilogue_is_bit_identical_to_the_plain_store_epilogue(sess, monkeypatch):
-    """The persistent pair GEMM ships its epilogue with TMA tensor stores (space-to-depth, plain, depth-to-space and fp32 dgrad
-    targets); AAE_TC_NO_TMA_OUT=1 (read per launch) selects per-thread row stores.  Same arithmetic, so latents, the decoder's
-    reconstruction and the weights after a training step must agree bit for bit — including a batch that leaves the last
-    pixel tile and the last CTA pair partly empty."""
-    from augmentedautoencoder_b200.ae.decoder import Decoder
-    from augmentedautoencoder_b200.ae.session import placeholder
-    p = O.make_encoder_params(42, bias_scale=0.05)
-    dp = O.make_decoder_params(43, bias_scale=0.05)
-    enc = _enc(1, 64, p)
-    zin = placeholder(np.float32, [None, 128])
-    dec = Decoder(placeholder(np.float32, [None, 128, 128, 3]), zin, list(reversed(O.NUM_FILTER)), 5, list(reversed(O.STRIDES)), "L2", 4,
-                  False, False, max_batch=64, precision=1)
-    dec.load_weights(dp)
-    got = {}
-    for mode in ("0", "1"):
-        monkeypatch.setenv("AAE_TC_NO_TMA_OUT", mode)
-        for batch in (3, 37, 64):
-            xu8 = O.make_crops_u8(900 + batch, batch)
-            z = sess.run(enc.z, {enc.x: xu8})
-            acts = [enc.activation_device(layer, sess.device).cpu().numpy().copy() for layer in range(1, 4)]
-            rec = dec.decode_device(torch.from_numpy(z).cuda()).cpu().numpy()
-            got[(mode, batch)] = (z, acts, rec)
-        enc_t, dec_t, op, _, _ = _train_pair(1, 8)
-        rs = np.random.RandomState(5)
-        x = (rs.rand(8, 128, 128, 3).astype(np.float32), rs.rand(8, 128, 128, 3).astype(np.float32))
-        loss = op.step_device(torch.from_numpy(x[0]).cuda(), torch.from_numpy(x[1]).cuda())
-        got[(mode, "train")] = (float(loss), enc_t.get_weights(), dec_t.get_weights())
-    for batch in (3, 37, 64):
-        z0, a0, r0 = got[("0", batch)]
-        z1, a1, r1 = got[("1", batch)]
-        assert np.array_equal(z0, z1) and np.array_equal(r0, r1), batch
-        for u, v in zip(a0, a1):
-            assert np.array_equal(u, v), batch
-    l0, we0, wd0 = got[("0", "train")]
-    l1, we1, wd1 = got[("1", "train")]
-    assert l0 == l1
-    for w0, w1 in ((we0, we1), (wd0, wd1)):
-        for k in w0:
-            assert np.array_equal(w0[k], w1[k]), k
-
-
 def test_c_abi_rejects_bad_calls_without_crashing(sess):
     import ctypes as C
     from augmentedautoencoder_b200 import _lib
@@ -240,7 +198,7 @@ def _train_pair(prec, B):
 
 
 def test_tc_training_gradients_match_float64_oracle(sess):
-    """Tensor-core trainer (tcgen05 forward, dgrad and wgrad GEMMs): loss and all 20 gradients of one forward/backward vs the
+    """Tensor-core trainer (wgmma forward, dgrad and wgrad GEMMs): loss and all 20 gradients of one forward/backward vs the
     float64 oracle.  Compared in relative L2 norm: a ReLU unit whose pre-activation is within the split-fp16 rounding of zero
     may fall on either side (as in any finite-precision implementation), which perturbs a few entries discretely."""
     enc, dec, top, ep, dp = _train_pair(1, 2)
@@ -319,7 +277,7 @@ def test_range_guard_reports_overflow_instead_of_garbage(sess):
     enc = _enc(1, 4, bad_w)
     with pytest.raises(AaeError, match=r"weight.*layer\(s\) 2"):
         sess.run(enc.z, {enc.x: crops})
-    # (2) activations: a large bias pushes conv1's (bit 0, tcgen05 conv1 kernel) / conv2's (bit 1, GEMM epilogue) output past 4094
+    # (2) activations: a large bias pushes conv1's (bit 0, tensor-core conv1 kernel) / conv2's (bit 1, GEMM epilogue) output past 4094
     for name, layer in (("conv2d/bias", 0), ("conv2d_1/bias", 1)):
         bad_a = dict(p)
         bad_a[name] = p[name].copy()
