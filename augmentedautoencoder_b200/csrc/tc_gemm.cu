@@ -72,6 +72,7 @@ struct TcSmem {
 
 // Warp roles (384 threads): warp 0 TMA producer (warps 1-3 idle), warpgroups 1 and 2 (warps 4-11) issue the wgmma for pixel rows
 // [0,64) and [64,128) of the tile and then run the epilogue, two warps per 32-row quadrant.
+// Grid: x = N tile, y = M tile, z = K split (see launch_tc_gemm).
 template <int N_TILE, int STAGES, int KCH>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
@@ -85,8 +86,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int m0 = blockIdx.x * 128;
-  const int n0 = blockIdx.y * N_TILE;
+  const int m0 = blockIdx.y * 128;
+  const int n0 = blockIdx.x * N_TILE;
   const int total_iters = p.taps * p.chunks_per_tap;
   const int it_begin = blockIdx.z * p.iters_per_split;
   const int it_end = min(total_iters, it_begin + p.iters_per_split);
@@ -257,12 +258,16 @@ __global__ void __launch_bounds__(256) splitk_forward_finish_kernel(const float*
   }
 }
 
+// tiles = (m_tiles, n_tiles, splits).  The kernel runs the N tiles on grid.x, so the N tiles of an M tile are adjacent in launch
+// order and read the activation tile (and its 5 x 5 tap re-reads) while it is in L2; M first would put all resident CTAs on one
+// weight column and stream every activation tile from HBM once per N tile.
 template <int N_TILE, int STAGES, int KCH>
-int launch_tc_gemm(const TcLayer& L, dim3 grid, cudaStream_t s) {
+int launch_tc_gemm(const TcLayer& L, dim3 tiles, cudaStream_t s) {
   using S = TcSmem<N_TILE, STAGES, KCH>;
   auto kern = tc_gemm_kernel<N_TILE, STAGES, KCH>;
+  AAE_REQUIRE(tiles.x <= 65535u, "tc_gemm: %u row tiles exceed the grid's y limit", tiles.x);
   AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-  kern<<<grid, TC_THREADS, S::TOTAL, s>>>(L.tm_a_hi, L.tm_a_lo, L.tm_w_hi, L.tm_w_lo, L.gp);
+  kern<<<dim3(tiles.y, tiles.x, tiles.z), TC_THREADS, S::TOTAL, s>>>(L.tm_a_hi, L.tm_a_lo, L.tm_w_hi, L.tm_w_lo, L.gp);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
