@@ -974,8 +974,8 @@ static int encoder_dense_backward(aae_trainer* h, const float* flat, int B, floa
 }
 
 // Training step on the tensor cores: forward through the split-fp16 plans (their (hi, lo) activations double as the ReLU
-// masks and the wgrad operands), conv backward as wgmma GEMMs (tc_train.cu), the two dense layers, conv1's wgrad (K = 75)
-// and the elementwise pieces on the fp32 kernels.
+// masks and the wgrad operands), conv backward as wgmma GEMMs (tc_train.cu) -- conv1's wgrad (K = 75) as a 1x1 wgrad GEMM over
+// the im2col of the input -- and the two dense layers and the elementwise pieces on the fp32 kernels.
 static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, int B, float* loss_out, cudaStream_t s) {
   aae_encoder* E = h->enc;
   aae_decoder* D = h->dec;
@@ -1032,7 +1032,7 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
     pt.mark(4, s);
     // masks with the ReLU of the producing layer (conv l-1, or dense_1) and folds that layer's bias gradient into the same pass;
     // dense_1's fp32 backward reads the masked gradient itself
-    AAE_TRY(tc_train_finish(P, u, u + 1 < n_dec ? u + 1 : -1, B, false, /*keep_masked=*/l == 1, l > 1 ? h->dec_b[l - 1].g.p : nullptr, s));
+    AAE_TRY(tc_train_finish(P, u, u + 1 < n_dec ? u + 1 : -1, B, /*keep_masked=*/l == 1, l > 1 ? h->dec_b[l - 1].g.p : nullptr, s));
   }
   pt.mark(5, s);
   AAE_TRY(decoder_dense_backward(h, raw, B, s));
@@ -1057,19 +1057,12 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
     AAE_TRY(tc_train_unit_dgrad(P, u, B, s));
     pt.mark(4, s);
     const bool last = u + 1 == n_units;
-    const int c1 = tc_train_conv1_unit(P);
     // masked gradient of conv i-1's output (space-to-depth order, columns (cls, cin)); its column sums are conv i-1's bias gradient.
-    // The last unit's result is conv1's output gradient: (hi, lo) operand of the tensor-core conv1 wgrad, or fp32 for the SIMT one
-    AAE_TRY(tc_train_finish(P, u, last ? c1 : u + 1, B, last && c1 < 0, false, h->enc_b[i - 1].g.p, s));
+    // The last unit's result is conv1's output gradient: the (hi, lo) operand of the conv1 wgrad
+    AAE_TRY(tc_train_finish(P, u, last ? tc_train_conv1_unit(P) : u + 1, B, false, h->enc_b[i - 1].g.p, s));
   }
-  if (tc_train_conv1_unit(P) >= 0) {
-    pt.mark(2, s);
-    AAE_TRY(tc_train_conv1_wgrad(P, x, B, h->enc_k[0].g.p, s));
-  } else {
-    // conv1 (Cin = 3, K = 75): fp32 wgrad from the plain-layout gradient the last unit wrote
-    pt.mark(5, s);
-    AAE_TRY(conv_wgrad(h, E->conv[0], x, B, tc_train_f32_out(P), h->enc_k[0].g.p, s));
-  }
+  pt.mark(2, s);
+  AAE_TRY(tc_train_conv1_wgrad(P, x, B, h->enc_k[0].g.p, s));
   pt.mark(6, s);   // closes the last phase; aae_train_step charges Adam to phase 6 and closes it with one more mark
   return AAE_OK;
 }

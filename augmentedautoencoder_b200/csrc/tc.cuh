@@ -43,11 +43,10 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
 void tc_train_destroy(TcTrainPlan* h);
 int tc_train_num_units(const TcTrainPlan* h);
 int tc_train_num_decoder_units(const TcTrainPlan* h);
-int tc_train_conv1_unit(const TcTrainPlan* h);   // index of the wgrad-only conv1 unit (target of the last tc_train_finish), or -1
+int tc_train_conv1_unit(const TcTrainPlan* h);   // index of the wgrad-only conv1 unit (target of the last tc_train_finish)
 int tc_train_conv1_wgrad(TcTrainPlan* h, const float* x_dev, int B, float* dw_out, cudaStream_t s);
 void tc_train_unit_info(const TcTrainPlan* h, int u, int* is_enc, int* cin, int* cout, int* gh, int* gw, int* nd);
 float* tc_train_raw(TcTrainPlan* h);
-float* tc_train_f32_out(TcTrainPlan* h);
 int tc_train_begin_step(TcTrainPlan* h, cudaStream_t s);
 int tc_train_pack_weights(TcTrainPlan* h, int u, const float* w_dev, cudaStream_t s);
 int tc_train_pack_weights_merged(TcTrainPlan* h, int u, const float* wm_dev, cudaStream_t s);
@@ -55,7 +54,7 @@ int tc_train_set_loss_grad(TcTrainPlan* h, const float* g_dev, int B, cudaStream
 int tc_train_set_unit_grad(TcTrainPlan* h, int u, const float* g_dev, int B, cudaStream_t s);
 int tc_train_unit_wgrad(TcTrainPlan* h, int u, int B, float* dw_out, cudaStream_t s);
 int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s);
-int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool want_f32, bool keep_masked, float* db_out, cudaStream_t s);
+int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, float* db_out, cudaStream_t s);
 int tc_train_unpack_flat(TcTrainPlan* h, int B, float* out, cudaStream_t s);
 
 int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int latent, int num_cyclo, int max_batch, TcCodebook** out);

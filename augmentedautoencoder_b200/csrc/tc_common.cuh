@@ -99,18 +99,6 @@ template <int N>
 struct Wgmma;
 #define AAE_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
 template <>
-struct Wgmma<32> {
-  template <int TA, int TB>
-  static __device__ __forceinline__ void ss(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n\t}\n"
-        : AAE_D8(0), AAE_D8(8)
-        : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB));
-  }
-};
-
-template <>
 struct Wgmma<64> {
   template <int TA, int TB>
   static __device__ __forceinline__ void ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -163,15 +151,6 @@ __device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
   d |= (uint64_t)1 << 62;
-  return d;
-}
-// Same for the 64-byte-swizzle layout: rows of 32 fp16 (64 B), 8-row groups 512 B apart, CU_TENSOR_MAP_SWIZZLE_64B.
-__device__ __forceinline__ uint64_t make_sw64_kmajor_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(512 >> 4) << 32;
-  d |= (uint64_t)2 << 62;
   return d;
 }
 // MN-major operand in the 128-byte-swizzle layout: K rows of 128 B = 64 fp16 along M/N, 8-row groups SBO apart, successive

@@ -1,16 +1,14 @@
 // First encoder layer on wgmma (AAE_PREC_TC_SPLIT): conv 5x5 / stride 2 / TF-SAME(1,2), Cin = 3 -> Cout = 128, + bias +
-// ReLU  (auto_pose/ae/encoder.py:43-50, first loop iteration), fused with the x/255. of auto_pose/ae/codebook.py:58-59.
+// ReLU  (auto_pose/ae/encoder.py:43-50, first loop iteration).  tc_conv1_kernel takes float crops (the training feed),
+// tc_conv1_u8_kernel uint8 crops with the x/255. of auto_pose/ae/codebook.py:58-59 fused.
 //
 // K = 25*3 = 75 is far too small and too ragged for TMA (patches overlap, 3-byte pixels), so the A operand is built in
-// shared memory by 128 "builder" threads -- one output pixel (one im2col row) each -- straight from the uint8 crop:
-// a 256-entry lookup table maps a byte to the fp16 (hi, lo) pair of 16 * (u8 / 255) (exact IEEE divide on the host of
-// the kernel, so the fused path is bit-identical to the reference's float feed), and the row is written in the
+// shared memory by 128 "builder" threads -- one output pixel (one im2col row) each -- straight from the float crop:
+// every value is scaled to 16 * x and split into its fp16 (hi, lo) pair, and the row is written in the
 // 128-byte-swizzle K-major canonical layout.  K is padded to 80 = 5 MMA K-steps.  The packed weights ([128][128] K-major,
 // zero beyond k = 75) are TMA-loaded once per CTA and stay resident.  Persistent CTAs loop over 128-pixel tiles with a
 // single-stage A buffer: builders (warps 0-3) run a tile ahead of the two MMA + epilogue warpgroups (warps 4-11); warp 12
 // loads the weights.  The epilogue writes conv2's input directly: (hi, lo) fp16, space-to-depth layout.
-#include <stdlib.h>
-
 #include <algorithm>
 
 #include "tc.cuh"
@@ -32,6 +30,8 @@ constexpr int C1_MMA_WARP = 4 + C1_EPI_WARPS;
 constexpr int C1_THREADS = 32 * (C1_MMA_WARP + 1);
 constexpr int C1_PIX_ROWS = 7;                     // input rows feeding two output rows: 2*2 + 3
 constexpr int C1_PIX_LD = 400;                     // (128 + 3 padding pixels) * 3 channels = 393 words, rounded up
+// consecutive 1 KB output blocks shipped by one bulk store: fewer, larger copies vs bank conflicts
+constexpr int C1_OUT_GROUP = 2;                    // measured: 0.25 / 0.22 / 0.28 / 0.28 ms for 1 / 2 / 4 / 8
 
 struct Conv1Params {
   const void* x;           // crops NHWC, uint8 or float32
@@ -39,7 +39,6 @@ struct Conv1Params {
   int OH, OW, N;           // output dims, N = Cout (<= 128)
   int pad_t, pad_l;
   int num_tiles;
-  int out_group;           // consecutive 1 KB output blocks shipped by one bulk store (1, 2, 4, 8): fewer, larger copies vs bank conflicts
   const float* bias;
   float unscale, out_scale, in_scale;
   __half* out_hi;
@@ -47,38 +46,25 @@ struct Conv1Params {
   unsigned* range_flag;    // run-time range guard (tc_plan.cuh): bit 0 = this layer's activation overflowed fp16 at out_scale
 };
 
-template <int N>
 struct Conv1Smem {
-  static constexpr int W_BYTES = 4 * N * 128;
+  static constexpr int W_BYTES = 4 * C1_ATOM;                         // hi k0, hi k1, lo k0, lo k1 (128 rows x 128 B each)
   static constexpr int PIX_BYTES = C1_PIX_ROWS * C1_PIX_LD * 4;       // staged input rows of one tile, (hi|lo) words
   static constexpr int OUT_BYTES = 2 * 32 * C1_OUT_LD;                // (hi, lo) output tile staged for bulk stores
-  static constexpr int RAW_BYTES = ((C1_PIX_ROWS * 128 * 3 * (int)sizeof(float) + 127) / 128) * 128;   // fp32 worst case
-  static constexpr int TOTAL = W_BYTES + C1_STAGES * C1_STAGE + PIX_BYTES + OUT_BYTES + RAW_BYTES + 1024 /*lut*/ + 1024 /*align*/ + 256;
+  static constexpr int RAW_BYTES = ((C1_PIX_ROWS * 128 * 3 * (int)sizeof(float) + 127) / 128) * 128;   // fp32 input rows
+  static constexpr int TOTAL = W_BYTES + C1_STAGES * C1_STAGE + PIX_BYTES + OUT_BYTES + RAW_BYTES + 1024 /*align*/ + 256;
 };
 
-template <bool U8>
-__device__ __forceinline__ uint32_t conv1_fetch(const Conv1Params& p, const uint32_t* lut, long long idx, bool ok) {
-  // returns (hi fp16 bits) | (lo fp16 bits << 16) of in_scale * pixel
-  if (!ok) return 0u;
-  if (U8) return lut[reinterpret_cast<const uint8_t*>(p.x)[idx]];
-  const float v = __ldg(reinterpret_cast<const float*>(p.x) + idx) * p.in_scale;
-  __half h, l;
-  split_f16(v, h, l);
-  return (uint32_t)__half_as_ushort(h) | ((uint32_t)__half_as_ushort(l) << 16);
-}
-
-template <int N, int CIN, bool U8>
 __global__ void __launch_bounds__(C1_THREADS, 1)
 tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, const Conv1Params p) {
-  using S = Conv1Smem<N>;
+  using S = Conv1Smem;
+  constexpr int N = 128, CIN = 3;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* w_smem = smem;                                   // hi k0, hi k1, lo k0, lo k1 (N rows x 128 B each)
   uint8_t* a_smem = smem + S::W_BYTES;
   uint32_t* pix = reinterpret_cast<uint32_t*>(a_smem + C1_STAGES * C1_STAGE);   // [C1_PIX_ROWS][C1_PIX_LD]
   uint8_t* out_smem = reinterpret_cast<uint8_t*>(pix + C1_PIX_ROWS * C1_PIX_LD);   // [2 (hi,lo)][32][C1_OUT_LD]
-  uint32_t* lut = reinterpret_cast<uint32_t*>(out_smem + S::OUT_BYTES);
-  uint8_t* raw_smem = reinterpret_cast<uint8_t*>(lut + 256);                    // raw input rows of the tile being staged
+  uint8_t* raw_smem = out_smem + S::OUT_BYTES;                                  // raw input rows of the tile being staged
   uint64_t* w_full = reinterpret_cast<uint64_t*>(raw_smem + S::RAW_BYTES);
   uint64_t* a_full = w_full + 1;
   uint64_t* a_empty = a_full + C1_STAGES;
@@ -87,13 +73,6 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x < N) bias_s[threadIdx.x] = p.bias[threadIdx.x];
 
-  if (threadIdx.x < 256) {
-    // byte -> (hi, lo) of in_scale * (u8 / 255): the divide is the IEEE fp32 divide the reference's feed amounts to
-    const float v = ((float)threadIdx.x / 255.0f) * p.in_scale;
-    __half h, l;
-    split_f16(v, h, l);
-    lut[threadIdx.x] = (uint32_t)__half_as_ushort(h) | ((uint32_t)__half_as_ushort(l) << 16);
-  }
   for (int i = threadIdx.x; i < C1_PIX_ROWS * C1_PIX_LD; i += blockDim.x) pix[i] = 0u;   // left/right padding pixels stay zero
   if (warp == C1_MMA_WARP && lane == 0) {
     prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_w_lo);
@@ -114,7 +93,7 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
     const int r = threadIdx.x;
     constexpr int run = 5 * CIN;                             // words per kernel row (kw, c)
     constexpr int ROWW = 128 * CIN;                          // words per staged input row (image width 128)
-    constexpr int NV = U8 ? (C1_PIX_ROWS * ROWW / 16 + 127) / 128 : (C1_PIX_ROWS * ROWW / 4 + 127) / 128;
+    constexpr int NV = (C1_PIX_ROWS * ROWW / 4 + 127) / 128;
     uint4 raw[NV];
     auto fetch = [&](int tile) {                             // global -> registers
       const int m_first = tile * 128;
@@ -123,17 +102,10 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
       for (int v = 0; v < NV; ++v) {
         const int u = r + v * 128;
         raw[v] = make_uint4(0u, 0u, 0u, 0u);
-        if (U8) {
-          const int row = u / (ROWW / 16), c16 = u - row * (ROWW / 16);
-          const int ih = 2 * oh0 - p.pad_t + row;
-          if (row < C1_PIX_ROWS && b < p.B && ih >= 0 && ih < p.H)
-            raw[v] = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const uint8_t*>(p.x) + ((long long)(b * p.H + ih) * p.W) * CIN) + c16);
-        } else {
-          const int row = u / (ROWW / 4), c4 = u - row * (ROWW / 4);
-          const int ih = 2 * oh0 - p.pad_t + row;
-          if (row < C1_PIX_ROWS && b < p.B && ih >= 0 && ih < p.H)
-            raw[v] = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(p.x) + ((long long)(b * p.H + ih) * p.W) * CIN) + c4);
-        }
+        const int row = u / (ROWW / 4), c4 = u - row * (ROWW / 4);
+        const int ih = 2 * oh0 - p.pad_t + row;
+        if (row < C1_PIX_ROWS && b < p.B && ih >= 0 && ih < p.H)
+          raw[v] = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(p.x) + ((long long)(b * p.H + ih) * p.W) * CIN) + c4);
       }
     };
     uint8_t* rawbuf = raw_smem;
@@ -144,20 +116,14 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
 #pragma unroll
       for (int v = 0; v < NV; ++v) {
         const int u = r + v * 128;
-        if (u < C1_PIX_ROWS * ROWW / (U8 ? 16 : 4)) reinterpret_cast<uint4*>(rawbuf)[u] = raw[v];
+        if (u < C1_PIX_ROWS * ROWW / 4) reinterpret_cast<uint4*>(rawbuf)[u] = raw[v];
       }
       asm volatile("bar.sync 1, 128;" ::: "memory");
       for (int e = r; e < C1_PIX_ROWS * ROWW; e += 128) {
         const int row = e / ROWW, col = e - row * ROWW;
-        uint32_t w;
-        if (U8) {
-          w = lut[rawbuf[e]];
-        } else {
-          __half h, l;
-          split_f16(reinterpret_cast<const float*>(rawbuf)[e] * p.in_scale, h, l);
-          w = (uint32_t)__half_as_ushort(h) | ((uint32_t)__half_as_ushort(l) << 16);
-        }
-        dst[row * C1_PIX_LD + p.pad_l * CIN + col] = w;
+        __half h, l;
+        split_f16(reinterpret_cast<const float*>(rawbuf)[e] * p.in_scale, h, l);
+        dst[row * C1_PIX_LD + p.pad_l * CIN + col] = (uint32_t)__half_as_ushort(h) | ((uint32_t)__half_as_ushort(l) << 16);
       }
     };
     if (my_tiles > 0) {
@@ -204,7 +170,7 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
     // its accumulator fragment into a padded shared-memory image of that slab; one thread then ships it with 1 KB bulk
     // stores, i.e. full-line HBM writes instead of 16-byte scattered ones.
     const int wg = (warp - 4) >> 2;
-    const int G = p.out_group, grp_ld = G * 8 * N + 16;
+    constexpr int G = C1_OUT_GROUP, grp_ld = G * 8 * N + 16;
     uint8_t* my_hi[2];
 #pragma unroll
     for (int h2 = 0; h2 < 2; ++h2) {                 // the thread's two fragment rows
@@ -285,9 +251,8 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
 
 
 // =====================================================================================================================
-// uint8 feed, second generation (default for uint8 crops; AAE_C1_V1=1 selects the kernel above for same-box A/B runs).
-// The first kernel ran at 0.35 of the HBM write roofline: 3.9 k shared-memory wavefronts per 128-pixel tile against an HBM
-// budget of 2.8 k cycles per tile.  What changed:
+// uint8 feed.  The kernel above, fed bytes through a byte -> (hi, lo) lookup table, ran at 0.35 of the HBM write roofline:
+// 3.9 k shared-memory wavefronts per 128-pixel tile against an HBM budget of 2.8 k cycles per tile.  This one differs in:
 //   * 1/255 is folded into the packed weights, so the A operand is the BYTE ITSELF as fp16 -- exact, no lo plane: two
 //     products per K step (A*W_hi + A*W_lo) instead of three, half the A-tile bytes, and no lookup table;
 //   * K is laid out as 5 kernel rows x 16 slots (slot 0 of every row meets a zero weight, slots 1..15 are the 15 (kw, c)
@@ -534,7 +499,6 @@ struct TcConv1 {
   CUtensorMap tm8_hi, tm8_lo, tm_out32_hi, tm_out32_lo;   // output maps: one box = a warp's 32 slots x 32 channels
   const __half *bound_hi = nullptr, *bound_lo = nullptr;
   long long slots = 0;            // 256-byte output slots the tensor maps cover ((b, oh/2, ow/2, parity) positions)
-  bool u8_ok = false;
 };
 
 bool tc_conv1_supported(const aae_net_cfg* cfg) {
@@ -558,14 +522,13 @@ int tc_conv1_create(int device, const aae_net_cfg* cfg, TcConv1** out) {
   const uint32_t box[2] = {64, (uint32_t)h->N};
   int st = make_tmap_f16(&h->tm_hi, h->w_hi, 2, dims, strides, box);
   if (st == AAE_OK) st = make_tmap_f16(&h->tm_lo, h->w_lo, 2, dims, strides, box);
-  if (st == AAE_OK && h->N == 128 && getenv("AAE_C1_V1") == nullptr) {
+  if (st == AAE_OK) {
     e = cudaMalloc(&h->w8_hi, (size_t)h->N * 128 * sizeof(__half));
     if (e == cudaSuccess) e = cudaMalloc(&h->w8_lo, (size_t)h->N * 128 * sizeof(__half));
     if (e != cudaSuccess) { set_error("tc conv1 alloc failed: %s", cudaGetErrorString(e)); tc_conv1_destroy(h); return AAE_ERR_OOM; }
     st = make_tmap_f16(&h->tm8_hi, h->w8_hi, 2, dims, strides, box);
     if (st == AAE_OK) st = make_tmap_f16(&h->tm8_lo, h->w8_lo, 2, dims, strides, box);
     if (st == AAE_OK) st = cudaFuncSetAttribute(tc_conv1_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, U8_SMEM_TOTAL) == cudaSuccess ? AAE_OK : AAE_ERR_CUDA;
-    h->u8_ok = st == AAE_OK;
   }
   if (st != AAE_OK) { tc_conv1_destroy(h); return st; }
   *out = h;
@@ -581,17 +544,18 @@ void tc_conv1_destroy(TcConv1* h) {
 int tc_conv1_pack(TcConv1* h, const float* w_dev, int K, float w_scale, unsigned* range_flag, unsigned range_bit, cudaStream_t s) {
   pack_conv1_weights_kernel<<<(unsigned)ceil_div(h->N * 128, 256), 256, 0, s>>>(w_dev, K, h->N, w_scale, h->w_hi, h->w_lo, range_flag, range_bit);
   AAE_LAUNCH_OK();
-  if (h->u8_ok) {
-    AAE_REQUIRE(K == 75, "tc conv1 (uint8 kernel): K = %d, expected 75", K);
-    pack_conv1_u8_weights_kernel<<<(unsigned)ceil_div(h->N * 128, 256), 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8_hi, h->w8_lo, range_flag,
-                                                                                    range_bit);
-    AAE_LAUNCH_OK();
-  }
+  AAE_REQUIRE(K == 75, "tc conv1 (uint8 kernel): K = %d, expected 75", K);
+  pack_conv1_u8_weights_kernel<<<(unsigned)ceil_div(h->N * 128, 256), 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8_hi, h->w8_lo, range_flag,
+                                                                                  range_bit);
+  AAE_LAUNCH_OK();
   return AAE_OK;
 }
 
 int tc_conv1_forward(TcConv1* h, const aae_net_cfg* cfg, const void* crops, int src_u8, int B, const float* bias, float act_scale,
                      float w_scale, __half* out_hi, __half* out_lo, unsigned* range_flag, cudaStream_t s) {
+  // both kernels load the crop rows in 16-byte pieces
+  AAE_REQUIRE((reinterpret_cast<uintptr_t>(crops) & 15u) == 0,
+              "AAE_PREC_TC_SPLIT: the crops pointer must be 16-byte aligned (AAE_PREC_FP32_SIMT accepts any alignment)");
   Conv1Params p;
   p.range_flag = range_flag;
   p.x = crops; p.B = B; p.H = cfg->in_h; p.W = cfg->in_w; p.C = cfg->in_c;
@@ -599,16 +563,11 @@ int tc_conv1_forward(TcConv1* h, const aae_net_cfg* cfg, const void* crops, int 
   p.pad_t = std::max((p.OH - 1) * 2 + 5 - p.H, 0) / 2;
   p.pad_l = std::max((p.OW - 1) * 2 + 5 - p.W, 0) / 2;
   p.num_tiles = (int)ceil_div((int64_t)B * p.OH * p.OW, 128);
-  {
-    static const int group = [] { const char* e = getenv("AAE_C1_GROUP"); const int g = e ? atoi(e) : 2; return (g == 1 || g == 2 || g == 4 || g == 8) ? g : 2; }();   // measured: 0.25 / 0.22 / 0.28 / 0.28 ms for 1 / 2 / 4 / 8
-    p.out_group = group;
-  }
   p.bias = bias;
   p.in_scale = act_scale; p.out_scale = act_scale; p.unscale = 1.f / (act_scale * w_scale);
   p.out_hi = out_hi; p.out_lo = out_lo;
   const int grid = std::min(h->sm_count, p.num_tiles);
-  using S = Conv1Smem<128>;
-  if (src_u8 && h->u8_ok && (reinterpret_cast<uintptr_t>(crops) & 15u) == 0) {   // 16-byte row pieces are loaded as uint4
+  if (src_u8) {
     // output tensor maps: [slot][128 channels] views of conv2's (hi, lo) input; the buffers hold max_batch crops, this call
     // may be shorter -- the maps cover exactly the slots this call writes
     const long long slots = (long long)p.num_tiles * 128;
@@ -622,12 +581,9 @@ int tc_conv1_forward(TcConv1* h, const aae_net_cfg* cfg, const void* crops, int 
     }
     p.unscale = 1.f / (w_scale * 256.f);              // accumulators hold sum u8 * (w * w_scale * 256 / 255)
     tc_conv1_u8_kernel<<<grid, U8_THREADS, U8_SMEM_TOTAL, s>>>(h->tm8_hi, h->tm8_lo, h->tm_out32_hi, h->tm_out32_lo, p);
-  } else if (src_u8) {
-    AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel<128, 3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    tc_conv1_kernel<128, 3, true><<<grid, C1_THREADS, S::TOTAL, s>>>(h->tm_hi, h->tm_lo, p);
   } else {
-    AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel<128, 3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    tc_conv1_kernel<128, 3, false><<<grid, C1_THREADS, S::TOTAL, s>>>(h->tm_hi, h->tm_lo, p);
+    AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Conv1Smem::TOTAL));
+    tc_conv1_kernel<<<grid, C1_THREADS, Conv1Smem::TOTAL, s>>>(h->tm_hi, h->tm_lo, p);
   }
   AAE_LAUNCH_OK();
   return AAE_OK;

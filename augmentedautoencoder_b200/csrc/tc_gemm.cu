@@ -17,8 +17,6 @@
 //
 // Warp roles (384 threads): warp 0 TMA producer, warpgroups 1-2 wgmma consumers and then epilogue (registers -> shared-memory
 // accumulator image -> bias/ReLU -> hi/lo split -> global, in the next layer's space-to-depth layout).
-#include <stdlib.h>
-
 #include <algorithm>
 #include <vector>
 
@@ -59,10 +57,10 @@ int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* 
 }
 
 // ------------------------------------------------------------------------------------------------- kernel
-template <int N_TILE, int STAGES, int KCH = 64>
+template <int N_TILE, int STAGES>
 struct TcSmem {
-  static constexpr int A_BYTES = 128 * KCH * 2;        // 128 rows x KCH fp16
-  static constexpr int W_BYTES = N_TILE * KCH * 2;
+  static constexpr int A_BYTES = 128 * TC_KCH * 2;     // 128 rows x TC_KCH fp16
+  static constexpr int W_BYTES = N_TILE * TC_KCH * 2;
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
   static constexpr int ACC_LD = 2 * N_TILE + 4;        // fp32 accumulator image [128][ACC_LD] (main | cross), padded
   static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
@@ -72,12 +70,12 @@ struct TcSmem {
 
 // Warp roles (384 threads): warp 0 TMA producer (warps 1-3 idle), warpgroups 1 and 2 (warps 4-11) issue the wgmma for pixel rows
 // [0,64) and [64,128) of the tile and then run the epilogue, two warps per 32-row quadrant.
-// Grid: x = N tile, y = M tile, z = K split (see launch_tc_gemm).
-template <int N_TILE, int STAGES, int KCH>
+// Grid: x = N tile, y = M tile, z = K split (see tc_launch_layer).
+template <int N_TILE, int STAGES>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, const TcGemmParams p) {
-  using S = TcSmem<N_TILE, STAGES, KCH>;
+  using S = TcSmem<N_TILE, STAGES>;
   constexpr int R = N_TILE / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -112,11 +110,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
         const int tap = it / p.chunks_per_tap, cc = it - tap * p.chunks_per_tap;
         uint8_t* st = smem + s * S::STAGE_BYTES;
         mbar_arrive_expect_tx(&full_bar[s], S::STAGE_BYTES);
-        const int c0 = p.tap_ch[tap] + cc * KCH;
+        const int c0 = p.tap_ch[tap] + cc * TC_KCH;
         const int x = ow0 + p.tap_dj[tap], y = oh0 + p.tap_di[tap];
         tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
         tma_load_4d(st + S::A_BYTES, &tm_a_lo, &full_bar[s], c0, x, y, b0);
-        const int kcol = it * KCH;
+        const int kcol = it * TC_KCH;
         tma_load_2d(st + 2 * S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, n0);
         tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tm_w_lo, &full_bar[s], kcol, n0);
       }
@@ -131,15 +129,15 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
       const int s = i % STAGES;
       mbar_wait(&full_bar[s], (uint32_t)(i / STAGES) & 1u);
       const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
-      const uint32_t a_off = (uint32_t)(wg * 64 * KCH * 2);
-      const uint64_t a_hi = KCH == 64 ? make_sw128_kmajor_desc(st + a_off) : make_sw64_kmajor_desc(st + a_off);
-      const uint64_t a_lo = KCH == 64 ? make_sw128_kmajor_desc(st + S::A_BYTES + a_off) : make_sw64_kmajor_desc(st + S::A_BYTES + a_off);
-      const uint64_t w_hi = KCH == 64 ? make_sw128_kmajor_desc(st + 2 * S::A_BYTES) : make_sw64_kmajor_desc(st + 2 * S::A_BYTES);
-      const uint64_t w_lo = KCH == 64 ? make_sw128_kmajor_desc(st + 2 * S::A_BYTES + S::W_BYTES) : make_sw64_kmajor_desc(st + 2 * S::A_BYTES + S::W_BYTES);
+      const uint32_t a_off = (uint32_t)(wg * 64 * TC_KCH * 2);
+      const uint64_t a_hi = make_sw128_kmajor_desc(st + a_off);
+      const uint64_t a_lo = make_sw128_kmajor_desc(st + S::A_BYTES + a_off);
+      const uint64_t w_hi = make_sw128_kmajor_desc(st + 2 * S::A_BYTES);
+      const uint64_t w_lo = make_sw128_kmajor_desc(st + 2 * S::A_BYTES + S::W_BYTES);
       wgmma_fence_regs(acc); wgmma_fence_regs(crs);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < KCH / 16; ++k) {
+      for (int k = 0; k < TC_KCH / 16; ++k) {
         // The tensor core truncates when it adds into a large fp32 accumulator, so the 2^-11-sized cross terms get an
         // accumulator of their own (small magnitude -> negligible truncation) and are folded in by the epilogue in RN fp32.
         const uint32_t first = (i > 0 || k > 0) ? 1u : 0u;
@@ -258,20 +256,6 @@ __global__ void __launch_bounds__(256) splitk_forward_finish_kernel(const float*
   }
 }
 
-// tiles = (m_tiles, n_tiles, splits).  The kernel runs the N tiles on grid.x, so the N tiles of an M tile are adjacent in launch
-// order and read the activation tile (and its 5 x 5 tap re-reads) while it is in L2; M first would put all resident CTAs on one
-// weight column and stream every activation tile from HBM once per N tile.
-template <int N_TILE, int STAGES, int KCH>
-int launch_tc_gemm(const TcLayer& L, dim3 tiles, cudaStream_t s) {
-  using S = TcSmem<N_TILE, STAGES, KCH>;
-  auto kern = tc_gemm_kernel<N_TILE, STAGES, KCH>;
-  AAE_REQUIRE(tiles.x <= 65535u, "tc_gemm: %u row tiles exceed the grid's y limit", tiles.x);
-  AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-  kern<<<dim3(tiles.y, tiles.x, tiles.z), TC_THREADS, S::TOTAL, s>>>(L.tm_a_hi, L.tm_a_lo, L.tm_w_hi, L.tm_w_lo, L.gp);
-  AAE_LAUNCH_OK();
-  return AAE_OK;
-}
-
 int dev_alloc(void** p, size_t bytes) { return tc_dev_alloc(p, bytes); }
 
 bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
@@ -285,11 +269,17 @@ int tc_dev_alloc(void** p, size_t bytes) {
   return AAE_OK;
 }
 
-int tc_launch_layer(const TcLayer& T, dim3 grid, cudaStream_t s) {
-  if (T.n_tile == 128 && T.kch == 64) return launch_tc_gemm<128, 3, 64>(T, grid, s);
-  if (T.n_tile == 32 && T.kch == 32) return launch_tc_gemm<32, 6, 32>(T, grid, s);
-  set_error("tc_launch_layer: no kernel for n_tile=%d kch=%d", T.n_tile, T.kch);
-  return AAE_ERR_UNSUPPORTED;
+// tiles = (m_tiles, n_tiles, splits).  The kernel runs the N tiles on grid.x, so the N tiles of an M tile are adjacent in launch
+// order and read the activation tile (and its 5 x 5 tap re-reads) while it is in L2; M first would put all resident CTAs on one
+// weight column and stream every activation tile from HBM once per N tile.
+int tc_launch_layer(const TcLayer& T, dim3 tiles, cudaStream_t s) {
+  using S = TcSmem<TC_N_TILE, 3>;
+  auto kern = tc_gemm_kernel<TC_N_TILE, 3>;
+  AAE_REQUIRE(tiles.x <= 65535u, "tc_gemm: %u row tiles exceed the grid's y limit", tiles.x);
+  AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+  kern<<<dim3(tiles.y, tiles.x, tiles.z), TC_THREADS, S::TOTAL, s>>>(T.tm_a_hi, T.tm_a_lo, T.tm_w_hi, T.tm_w_lo, T.gp);
+  AAE_LAUNCH_OK();
+  return AAE_OK;
 }
 
 int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
@@ -327,8 +317,6 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
       h->flat = T.in_c;
       if (T.in_c % 64 != 0 || T.out_c % 32 != 0) { set_error("AAE_PREC_TC_SPLIT: dense layer needs flat %% 64 == 0 and latent %% 32 == 0"); st = AAE_ERR_UNSUPPORTED; break; }
     }
-    T.n_tile = 128;
-    T.kch = 64;
     // batch dimension padded to a whole number of TMA boxes, so a tile never addresses rows outside the tensor map
     const int B_pad = (int)ceil_div(B, T.BB) * T.BB;
     const size_t act_alloc = (size_t)B_pad * T.in_h * T.in_w * T.in_c;
@@ -342,29 +330,28 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
       const uint64_t C4 = 4ull * T.in_c, W2 = T.in_w / 2, H2 = T.in_h / 2;
       const uint64_t dims[4] = {C4, W2, H2, (uint64_t)B_pad};
       const uint64_t strides[3] = {C4 * 2, W2 * C4 * 2, H2 * W2 * C4 * 2};
-      const uint32_t box[4] = {(uint32_t)T.kch, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
-      const int swz = 2 * T.kch;
-      if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box, swz)) != AAE_OK) break;
-      if ((st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box, swz)) != AAE_OK) break;
+      const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
+      if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box)) != AAE_OK) break;
+      if ((st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) break;
     } else {
       const uint64_t dims[4] = {(uint64_t)T.in_c, 1, 1, (uint64_t)B_pad};
       const uint64_t strides[3] = {(uint64_t)T.in_c * 2, (uint64_t)T.in_c * 2, (uint64_t)T.in_c * 2};
-      const uint32_t box[4] = {(uint32_t)T.kch, 1, 1, 128};
-      if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box, 2 * T.kch)) != AAE_OK) break;
-      if ((st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box, 2 * T.kch)) != AAE_OK) break;
+      const uint32_t box[4] = {(uint32_t)TC_KCH, 1, 1, 128};
+      if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box)) != AAE_OK) break;
+      if ((st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) break;
     }
     {
       const uint64_t K = (uint64_t)T.taps * T.in_c;
       const uint64_t dims[2] = {K, (uint64_t)T.out_c};
       const uint64_t strides[1] = {K * 2};
-      const uint32_t box[2] = {(uint32_t)T.kch, (uint32_t)std::min(T.n_tile, T.out_c)};
-      if ((st = make_tmap_f16(&T.tm_w_hi, T.w_hi, 2, dims, strides, box, 2 * T.kch)) != AAE_OK) break;
-      if ((st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box, 2 * T.kch)) != AAE_OK) break;
+      const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)std::min(TC_N_TILE, T.out_c)};
+      if ((st = make_tmap_f16(&T.tm_w_hi, T.w_hi, 2, dims, strides, box)) != AAE_OK) break;
+      if ((st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box)) != AAE_OK) break;
     }
     // ---- static GEMM parameters ----
     TcGemmParams& g = T.gp;
     g.N = T.out_c; g.OH = T.out_h; g.OW = T.out_w; g.BW = T.BW; g.BH = T.BH;
-    g.taps = T.taps; g.chunks_per_tap = T.in_c / T.kch;
+    g.taps = T.taps; g.chunks_per_tap = T.in_c / TC_KCH;
     g.iters_per_split = g.taps * g.chunks_per_tap;
     for (int t = 0; t < T.taps; ++t) {
       if (dense) { g.tap_di[t] = 0; g.tap_dj[t] = 0; g.tap_ch[t] = 0; continue; }
@@ -481,12 +468,11 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
     TcLayer& T = h->layers[i];
     const bool dense = (i + 1 == h->layers.size());
     T.gp.M = dense ? B : B * T.out_h * T.out_w;
-    dim3 grid((unsigned)ceil_div(T.gp.M, 128), (unsigned)ceil_div(T.out_c, T.n_tile), dense ? (unsigned)h->dense_splits : 1u);
+    dim3 grid((unsigned)ceil_div(T.gp.M, 128), (unsigned)ceil_div(T.out_c, TC_N_TILE), dense ? (unsigned)h->dense_splits : 1u);
     // Small batches leave most SMs idle (conv4 at 32 crops: 16 tiles of 400 K iterations for 132 SMs): split K so that the
     // grid covers the GPU, fold the fp32 partials and apply the real epilogue in splitk_forward_finish_kernel.
     int splits = 1;
-    static const bool fwd_splitk = getenv("AAE_TC_NO_FWD_SPLITK") == nullptr;     // (A/B switch, read once)
-    if (!dense && T.gp.out_mode != OUT_F32 && fwd_splitk) {
+    if (!dense && T.gp.out_mode != OUT_F32) {
       const int tiles = (int)(grid.x * grid.y), total_iters = T.gp.taps * T.gp.chunks_per_tap;
       if (tiles * 2 <= 132) {
         splits = std::min(132 / tiles, std::max(1, total_iters / 24));
@@ -559,7 +545,8 @@ int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int
 // every "nearest x2 upsample + conv5x5 (+ReLU)" as ONE GEMM  [B*h*w pixels] x [9*Cin] x [4*Cout]  over the LOW-resolution
 // activation (plain NHWC (hi, lo) fp16, 3x3 taps as unit-stride TMA boxes) with the taps of the 5x5 kernel pre-summed per
 // output parity; the epilogue scatters column (parity, co) of pixel (i, j) to pixel (2i+py, 2j+px) of the next layer's input
-// (depth-to-space).  The output layer (Cout = 3 -> N = 12, padded to 32) applies the sigmoid and writes fp32 NHWC.
+// (depth-to-space).  The output layer (Cout <= 3) is tap-separable: a 1x1 GEMM into fp32 P with N = 9 taps x 4 parities x Cout
+// (padded to 128), then outlayer_gather_kernel sums the 3x3 neighbourhood, adds the bias, applies the sigmoid and writes fp32 NHWC.
 namespace {
 
 __global__ void split_scale_kernel(const float* __restrict__ x, long long n, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
@@ -617,9 +604,9 @@ __global__ void outlayer_gather_kernel(const float* __restrict__ P, const float*
   }
 }
 
-__global__ void tile_bias_kernel(const float* __restrict__ b, int cout, int n_pad, float* __restrict__ out) {
+__global__ void tile_bias_kernel(const float* __restrict__ b, int cout, float* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n_pad) out[i] = i < 4 * cout ? b[i % cout] : 0.f;
+  if (i < 4 * cout) out[i] = b[i % cout];
 }
 
 }  // namespace
@@ -633,22 +620,22 @@ int tc_layer_setup_plain(TcLayer& T, int B, bool alloc_input) {
     if ((st = dev_alloc((void**)&T.in_lo, act * sizeof(__half))) != AAE_OK) return st;
   }
   const uint64_t K = (uint64_t)T.taps * T.in_c;
-  const int rows = (int)ceil_div(T.gp.N, T.n_tile) * T.n_tile;
+  const int rows = (int)ceil_div(T.gp.N, TC_N_TILE) * TC_N_TILE;
   if ((st = dev_alloc((void**)&T.w_hi, (size_t)rows * K * sizeof(__half))) != AAE_OK) return st;
   if ((st = dev_alloc((void**)&T.w_lo, (size_t)rows * K * sizeof(__half))) != AAE_OK) return st;
   {
     const uint64_t dims[4] = {(uint64_t)T.in_c, (uint64_t)T.in_w, (uint64_t)T.in_h, (uint64_t)B_pad};
     const uint64_t strides[3] = {(uint64_t)T.in_c * 2, (uint64_t)T.in_w * T.in_c * 2, (uint64_t)T.in_h * T.in_w * T.in_c * 2};
-    const uint32_t box[4] = {(uint32_t)T.kch, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
-    if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box, 2 * T.kch)) != AAE_OK) return st;
-    if ((st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box, 2 * T.kch)) != AAE_OK) return st;
+    const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
+    if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box)) != AAE_OK) return st;
+    if ((st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) return st;
   }
   {
     const uint64_t dims[2] = {K, (uint64_t)rows};
     const uint64_t strides[1] = {K * 2};
-    const uint32_t box[2] = {(uint32_t)T.kch, (uint32_t)T.n_tile};
-    if ((st = make_tmap_f16(&T.tm_w_hi, T.w_hi, 2, dims, strides, box, 2 * T.kch)) != AAE_OK) return st;
-    if ((st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box, 2 * T.kch)) != AAE_OK) return st;
+    const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)TC_N_TILE};
+    if ((st = make_tmap_f16(&T.tm_w_hi, T.w_hi, 2, dims, strides, box)) != AAE_OK) return st;
+    if ((st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box)) != AAE_OK) return st;
   }
   return AAE_OK;
 }
@@ -671,10 +658,9 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
     TcLayer T;
     memset(&T.gp, 0, sizeof(T.gp));
     TcGemmParams& g = T.gp;
-    T.kch = 64;
     if (l == 0) {                                   // dense_1: [B, latent] x [latent, h0*h0*f0]
       T.in_h = T.in_w = 1; T.in_c = cfg->latent; T.out_h = T.out_w = 1; T.out_c = h0 * h0 * nf[0];
-      T.taps = 1; T.BW = 1; T.BH = 1; T.BB = 128; T.n_tile = 128;
+      T.taps = 1; T.BW = 1; T.BH = 1; T.BB = 128;
       g.N = T.out_c; g.OH = g.OW = 1; g.relu = 1; g.out_mode = OUT_PLAIN_SPLIT;
       if (cfg->latent % 64 != 0 || T.out_c % 128 != 0) { set_error("tc decoder: latent %% 64 and dense width %% 128 required"); st = AAE_ERR_UNSUPPORTED; break; }
     } else {                                        // sub-pixel conv on the (h x w x C) low-resolution activation
@@ -688,16 +674,18 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
       }
       T.BW = hh; T.BH = std::min(hh, 128 / T.BW); T.BB = 128 / (T.BW * T.BH);
       g.OH = g.OW = hh;
-      if (l < L) { g.N = 4 * cout; T.n_tile = 128; g.relu = 1; g.out_mode = OUT_D2S_SPLIT; }
-      else if (36 * cout <= 128 && T.in_c % 64 == 0 && getenv("AAE_TC_OUT9") == nullptr) {
-        h->sep_out = true;                          // 1x1 GEMM into P, neighbourhood sum in outlayer_gather_kernel
-        T.taps = 1; T.kch = 64; g.N = 128; T.n_tile = 128; g.relu = 0; g.out_mode = OUT_F32; g.cout_real = cout;
+      if (l < L) { g.N = 4 * cout; g.relu = 1; g.out_mode = OUT_D2S_SPLIT; }
+      else {                                        // 1x1 GEMM into P, neighbourhood sum in outlayer_gather_kernel
+        if (36 * cout > 128) {
+          set_error("tc decoder: %d output channels, the tensor-core output layer takes at most 3 (AAE_PREC_FP32_SIMT takes any count)", cout);
+          st = AAE_ERR_UNSUPPORTED; break;
+        }
+        T.taps = 1; g.N = 128; g.relu = 0; g.out_mode = OUT_F32;
         st = dev_alloc((void**)&h->out_p, (size_t)ceil_div((int64_t)B * hh * hh, 128) * 128 * 128 * sizeof(float));
         if (st != AAE_OK) break;
-      } else { g.N = 32; T.n_tile = 32; T.kch = 32; g.relu = 2; g.out_mode = OUT_D2S_F32; g.cout_real = cout;
-             if (4 * cout > 32) { set_error("tc decoder: output channels > 8 unsupported"); st = AAE_ERR_UNSUPPORTED; break; } }
+      }
     }
-    g.BW = T.BW; g.BH = T.BH; g.taps = T.taps; g.chunks_per_tap = T.in_c / T.kch;
+    g.BW = T.BW; g.BH = T.BH; g.taps = T.taps; g.chunks_per_tap = T.in_c / TC_KCH;
     g.iters_per_split = g.taps * g.chunks_per_tap;
     for (int t = 0; t < T.taps; ++t) {
       g.tap_di[t] = (int8_t)(T.taps == 1 ? 0 : t / 3 - 1);
@@ -709,7 +697,7 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
     if ((st = tc_layer_setup_plain(T, B, /*alloc_input=*/true)) != AAE_OK) { h->layers.push_back(T); break; }
     h->layers.push_back(T);
     float* bz = nullptr;
-    if (l > 0) st = dev_alloc((void**)&bz, (size_t)std::max(g.N, 32) * sizeof(float));
+    if (l > 0 && l < L) st = dev_alloc((void**)&bz, (size_t)g.N * sizeof(float));
     h->bias_dev.push_back(bz);
     h->wm_floats = std::max(h->wm_floats, (size_t)9 * T.in_c * 4 * T.out_c);
   }
@@ -752,10 +740,10 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
     if (b_dev) T.gp.bias = b_dev;      // device pointer owned by the decoder handle
     return AAE_OK;
   }
-  const bool sep = h->sep_out && layer + 1 == (int)h->layers.size();
+  const bool out_layer = layer + 1 == (int)h->layers.size();
   if (w_dev) {
     AAE_TRY(launch_merge_subpixel_weights(w_dev, T.in_c, T.out_c, h->wm_tmp, s));
-    if (sep) {
+    if (out_layer) {
       pack_out_sep_kernel<<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, 1u << (16 + layer));
     } else {
       dim3 grid((unsigned)ceil_div(4 * T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), 9);
@@ -763,13 +751,12 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
     }
     AAE_LAUNCH_OK();
   }
-  if (sep) {
+  if (out_layer) {
     if (b_dev) h->out_bias = b_dev;
     return AAE_OK;
   }
   if (b_dev) {
-    const int n_pad = std::max(T.gp.N, 32);
-    tile_bias_kernel<<<(unsigned)ceil_div(n_pad, 128), 128, 0, s>>>(b_dev, T.out_c, n_pad, h->bias_dev[layer]);
+    tile_bias_kernel<<<(unsigned)ceil_div(T.gp.N, 128), 128, 0, s>>>(b_dev, T.out_c, h->bias_dev[layer]);
     AAE_LAUNCH_OK();
     T.gp.bias = h->bias_dev[layer];
   }
@@ -787,13 +774,13 @@ int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, cu
     TcLayer& T = h->layers[i];
     T.gp.M = i == 0 ? B : B * T.in_h * T.in_w;
     const bool last = i + 1 == h->layers.size();
-    if (last) T.gp.out_f32 = h->sep_out ? h->out_p : x_out;
-    dim3 grid((unsigned)ceil_div(T.gp.M, 128), (unsigned)ceil_div(T.gp.N, T.n_tile), 1u);
+    if (last) T.gp.out_f32 = h->out_p;
+    dim3 grid((unsigned)ceil_div(T.gp.M, 128), (unsigned)ceil_div(T.gp.N, TC_N_TILE), 1u);
     AAE_TRY(tc_launch_layer(T, grid, s));
-    if (last && h->sep_out) {
-      const long long total = (long long)T.gp.M * 4 * T.gp.cout_real;
+    if (last) {
+      const long long total = (long long)T.gp.M * 4 * T.out_c;
       outlayer_gather_kernel<<<(unsigned)std::min<long long>(132 * 16, ceil_div(total, 256)), 256, 0, s>>>(h->out_p, h->out_bias, B, T.in_h, T.in_w,
-                                                                                                         T.gp.cout_real, x_out);
+                                                                                                         T.out_c, x_out);
       AAE_LAUNCH_OK();
     }
   }

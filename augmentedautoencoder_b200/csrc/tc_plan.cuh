@@ -14,8 +14,7 @@ enum TcOutMode : int {
   OUT_S2D_SPLIT = 0,      // (hi, lo) fp16, space-to-depth layout of the next stride-2 conv
   OUT_PLAIN_SPLIT = 1,    // (hi, lo) fp16, plain [M, N]
   OUT_F32 = 2,            // fp32 [splits, M, N] raw accumulators (split-K partials)
-  OUT_D2S_SPLIT = 3,      // (hi, lo) fp16, depth-to-space: column (cls, co) of pixel (b,i,j) -> pixel (2i+py, 2j+px) of [B,2OH,2OW,N/4]
-  OUT_D2S_F32 = 4         // fp32, depth-to-space with `cout_real` channels per parity (decoder output layer, N padded)
+  OUT_D2S_SPLIT = 3       // (hi, lo) fp16, depth-to-space: column (cls, co) of pixel (b,i,j) -> pixel (2i+py, 2j+px) of [B,2OH,2OW,N/4]
 };
 
 struct TcGemmParams {
@@ -32,8 +31,7 @@ struct TcGemmParams {
   const unsigned* amax_bits;  // optional: the A operand was scaled by tc_dyn_scale(*amax_bits) (training gradients); folded into unscale
   float out_scale;       // scale applied before the hi/lo split of the output (next layer's scale_A)
   const float* bias;
-  int relu;              // activation: 0 none, 1 ReLU, 2 sigmoid
-  int cout_real;         // OUT_D2S_F32: real channels per parity class (columns >= 4*cout_real are padding)
+  int relu;              // activation: 0 none, 1 ReLU
   int out_mode;
   __half* out_hi;
   __half* out_lo;
@@ -61,6 +59,8 @@ constexpr float ACT_SCALE = 16.f;     // activations (and the [0,1] input) are s
 constexpr float W_SCALE = 256.f;      // weights are stored as 256 * w
 constexpr int TC_STAGES = 2;
 constexpr int TC_THREADS = 384;       // warp 0 TMA, 1-3 idle, warpgroups 1-2 (warps 4-11) wgmma + epilogue
+constexpr int TC_N_TILE = 128;        // output channels per GEMM tile
+constexpr int TC_KCH = 64;            // K chunk per pipeline stage: 64 fp16 = one 128-byte swizzle row
 
 struct TcLayer {
   int in_h, in_w, in_c, out_h, out_w, out_c;   // conv geometry (input is the space-to-depth tensor [B, in_h/2, in_w/2, 4*in_c])
@@ -69,8 +69,6 @@ struct TcLayer {
   __half *w_hi = nullptr, *w_lo = nullptr;      // packed weights [out_c][taps*in_c]
   CUtensorMap tm_a_hi, tm_a_lo, tm_w_hi, tm_w_lo;
   TcGemmParams gp;
-  int n_tile;
-  int kch;    // K chunk per pipeline stage: 64 (128-byte swizzle) or 32 (64-byte swizzle)
 };
 
 // bits of the range flag word: bit l = the activation written by conv layer l (0-based; the decoder counts dense_1 as 0)
@@ -99,12 +97,11 @@ struct TcDecoder {
   aae_net_cfg cfg;
   unsigned* range_flag = nullptr;
   std::vector<TcLayer> layers;     // [0] dense_1, [1..L-1] sub-pixel convs, [L] sub-pixel output layer
-  std::vector<float*> bias_dev;    // per layer: bias in GEMM-column order (dense: the caller's; convs: tiled 4x, padded)
+  std::vector<float*> bias_dev;    // per sub-pixel conv: bias tiled 4x in GEMM-column order (nullptr for dense_1 and the output layer)
   float* wm_tmp = nullptr;         // fp32 merged-weight scratch
-  // Output layer with 36 * Cout <= 128 (Cout = 3): "tap-separable" form.  P[pixel, (tap, cls, co)] = X[pixel, :] . Wm[tap, :, (cls, co)]
+  // Output layer (Cout <= 3, so that 36 * Cout <= 128) in "tap-separable" form.  P[pixel, (tap, cls, co)] = X[pixel, :] . Wm[tap, :, (cls, co)]
   // is ONE 1x1 GEMM (K = Cin, N = 128) that reads the activation once instead of once per tap; the 3x3 neighbourhood sum,
   // bias, sigmoid and depth-to-space scatter happen in a small gather kernel over P.
-  bool sep_out = false;
   float* out_p = nullptr;          // [B*h*w (padded to 128 rows)][128] fp32
   const float* out_bias = nullptr; // the caller's bias [Cout] (device)
   size_t wm_floats = 0;
@@ -154,25 +151,9 @@ __device__ __forceinline__ void tc_store_chunk(const TcGemmParams& p, const TcRo
 #pragma unroll
     for (int j = 0; j < 32; ++j) b[j] = 0.f;
   }
-  if (p.relu == 2) {
+  const float floor_v = p.relu == 1 ? 0.f : -INFINITY;       // fmaxf(a, -inf) = a
 #pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = 1.f / (1.f + expf(-(f[j] + b[j])));
-  } else {
-    const float floor_v = p.relu == 1 ? 0.f : -INFINITY;       // fmaxf(a, -inf) = a
-#pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j] + b[j], floor_v);
-  }
-  if (p.out_mode == OUT_D2S_F32) {
-    const int cr = p.cout_real;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const int nn = n + j;
-      if (nn >= 4 * cr) continue;
-      const int cls = nn / cr, co = nn - cls * cr;
-      p.out_f32[((long long)(r.b * 2 * p.OH + 2 * r.i + (cls >> 1)) * (2 * p.OW) + 2 * r.j + (cls & 1)) * cr + co] = f[j];
-    }
-    return;
-  }
+  for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j] + b[j], floor_v);
   long long off = r.row_off + n;
   if (p.out_mode == OUT_D2S_SPLIT) {
     const int cq = p.N >> 2, cls = n / cq, co = n - cls * cq;     // a 32-column chunk never straddles a parity class (cq % 32 == 0)
@@ -218,12 +199,12 @@ __device__ __forceinline__ void tc_acc_ld32(const float* img, int ld, int row, i
   }
 }
 
-// launches the GEMM kernel instantiation that matches the layer's tile shape (N tile, K chunk)
+// launches tc_gemm_kernel over grid = (M tiles, N tiles, K splits)
 int tc_launch_layer(const TcLayer& T, dim3 grid, cudaStream_t s);
 int tc_dev_alloc(void** p, size_t bytes);
 // Tensor maps + packed-weight storage of a layer whose A operand is a PLAIN NHWC (hi, lo) tensor [B_pad, in_h, in_w, in_c]
-// (taps = unit-stride boxes): fills tm_a_*, allocates w_hi/w_lo [ceil(N / n_tile) * n_tile][taps * in_c] and their maps.
-// T.{in_h,in_w,in_c,taps,BW,BH,BB,n_tile,kch,gp.N} must be set; with alloc_input = false T.in_hi/in_lo are the caller's.
+// (taps = unit-stride boxes): fills tm_a_*, allocates w_hi/w_lo [ceil(N / TC_N_TILE) * TC_N_TILE][taps * in_c] and their maps.
+// T.{in_h,in_w,in_c,taps,BW,BH,BB,gp.N} must be set; with alloc_input = false T.in_hi/in_lo are the caller's.
 int tc_layer_setup_plain(TcLayer& T, int B, bool alloc_input);
 
 }  // namespace aae

@@ -15,8 +15,6 @@
 // Gradients have no a-priori range, so every G tensor is stored as (hi, lo) fp16 of  G * 2^k  with k chosen per tensor and
 // per step from its largest magnitude (tc_dyn_scale): dgrad/wgrad results are written as raw fp32, a small elementwise
 // pass applies the ReLU mask of the forward activation, finds the maximum and re-splits into the next unit's layout.
-#include <stdlib.h>
-
 #include <algorithm>
 #include <vector>
 
@@ -226,12 +224,12 @@ __global__ void amax_kernel(const float* __restrict__ x, const __half* __restric
 }
 
 // raw (fp32 dgrad result, source layout) -> ReLU mask of the forward activation (same layout as raw) -> (hi, lo) fp16 of
-// value * tc_dyn_scale(amax) and/or fp32 in the remapped layout; optionally the masked fp32 back in place (fp32 consumers)
+// value * tc_dyn_scale(amax) in the remapped layout; optionally the masked fp32 back in place (fp32 consumers)
 // and the per-column sums of the masked values (bias gradient): a thread always meets the same 8-column group because
 // 256 % groups_per_row == 0, so it sums in registers and the block folds the threads of a group in fixed order.
 __global__ void __launch_bounds__(256) finish_kernel(float* __restrict__ raw, const __half* __restrict__ mask, long long groups, int mode, int h, int w,
                                                      int C, const unsigned* __restrict__ amax, __half* __restrict__ hi, __half* __restrict__ lo,
-                                                     float* __restrict__ out_f32, int write_masked, float* __restrict__ colsum, int groups_per_row) {
+                                                     int write_masked, float* __restrict__ colsum, int groups_per_row) {
   __shared__ float red[256 * 8];
   const float scale = amax ? tc_dyn_scale(__ldg(amax)) : 1.f;
   float cs[8];
@@ -248,7 +246,6 @@ __global__ void __launch_bounds__(256) finish_kernel(float* __restrict__ raw, co
 #pragma unroll
     for (int j = 0; j < 8; ++j) cs[j] += v[j];
     const long long j = remap_offset(i, mode, h, w, C);
-    if (out_f32) store8(out_f32 + j, v);
     if (hi) {
       uint32_t hh[4], ll[4];
 #pragma unroll
@@ -304,27 +301,6 @@ __global__ void amax_scalar_kernel(const float* __restrict__ x, long long n, uns
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(x[i]));
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(slot, __float_as_uint(m));
-}
-
-// pre-sigmoid gradient g [B, 2h, 2w, c] (c <= 4) -> G of the output layer's GEMM: [B, h, w, gN] with channel (cls * c + co), rest zero
-__global__ void pack_loss_grad_kernel(const float* __restrict__ g, int B, int h, int w, int c, int gN, const unsigned* __restrict__ amax,
-                                      __half* __restrict__ hi, __half* __restrict__ lo) {
-  const float scale = tc_dyn_scale(__ldg(amax));
-  const long long total = (long long)B * h * w * 4 * c;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int n = (int)(i % (4 * c));
-    long long r = i / (4 * c);
-    const int x = (int)(r % w); r /= w;
-    const int y = (int)(r % h);
-    const long long b = r / h;
-    const int cls = n / c, co = n - cls * c;
-    const float v = g[((b * 2 * h + 2 * y + (cls >> 1)) * (2LL * w) + 2 * x + (cls & 1)) * c + co] * scale;
-    __half a, d;
-    split_f16(v, a, d);
-    const long long o = ((b * h + y) * w + x) * gN + n;
-    hi[o] = a;
-    lo[o] = d;
-  }
 }
 
 // tap-separable output layer: G[pixel (b,y,x)][tap * n4 + m] = gs[(b, y - (ty-1), x - (tx-1))][m], gs = space-to-depth of the
@@ -394,35 +370,20 @@ __device__ __forceinline__ void split_store8(const float (&v)[8], float scale, _
   *reinterpret_cast<uint4*>(lo) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
 }
 
-// decoder unit: merged weights Wm [9][cin][n4] -> dgrad operand [cin][9 * gN] with the taps flipped, columns >= n4 zero.
-// One thread per 8 consecutive columns (n4 % 8 == 0) or per column (the padded output layer).
-__global__ void pack_dec_dgrad_kernel(const float* __restrict__ wm, int cin, int n4, int gN, float scale, __half* __restrict__ hi,
+// decoder sub-pixel unit: merged weights Wm [9][cin][n4] -> dgrad operand [cin][9 * n4] with the taps flipped.
+// One thread per 8 consecutive columns (n4 % 8 == 0).
+__global__ void pack_dec_dgrad_kernel(const float* __restrict__ wm, int cin, int n4, float scale, __half* __restrict__ hi,
                                       __half* __restrict__ lo) {
-  if (n4 % 8 == 0 && gN == n4) {
-    const int g8 = gN / 8;
-    const long long total = (long long)cin * 9 * g8;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-      const int n = (int)(i % g8) * 8;
-      long long r = i / g8;
-      const int t = (int)(r % 9);
-      const int ci = (int)(r / 9);
-      float v[8];
-      load8(wm + ((long long)(8 - t) * cin + ci) * n4 + n, v);
-      split_store8(v, scale, hi + i * 8, lo + i * 8);
-    }
-    return;
-  }
-  const long long total = (long long)cin * 9 * gN;
+  const int g8 = n4 / 8;
+  const long long total = (long long)cin * 9 * g8;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int n = (int)(i % gN);
-    long long r = i / gN;
+    const int n = (int)(i % g8) * 8;
+    long long r = i / g8;
     const int t = (int)(r % 9);
     const int ci = (int)(r / 9);
-    const float v = n < n4 ? wm[((long long)(8 - t) * cin + ci) * n4 + n] * scale : 0.f;
-    __half a, d;
-    split_f16(v, a, d);
-    hi[i] = a;
-    lo[i] = d;
+    float v[8];
+    load8(wm + ((long long)(8 - t) * cin + ci) * n4 + n, v);
+    split_store8(v, scale, hi + i * 8, lo + i * 8);
   }
 }
 
@@ -454,12 +415,6 @@ __global__ void unpack_plain_kernel(const __half* __restrict__ hi, const __half*
                                     float* __restrict__ out) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     out[i] = (__half2float(hi[i]) + __half2float(lo[i])) * inv_scale;
-}
-
-__global__ void compact_cols_kernel(const float* __restrict__ in, long long rows, int ld, int n, float* __restrict__ out) {
-  const long long total = rows * n;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
-    out[i] = in[(i / n) * ld + (i % n)];
 }
 
 inline unsigned ew_grid(long long n, int threads = 256) {
@@ -515,7 +470,6 @@ struct TcUnit {
   bool enc;                 // encoder 5x5/s2 layer (X in space-to-depth form) or decoder sub-pixel layer
   int cin, cout;            // the layer's real channel counts
   int gh, gw, gN;           // G = pre-activation gradient of the layer's GEMM output: plain [B, gh, gw, gN]
-  int n_real;               // real columns of G (4*cout for the decoder output layer whose gN is padded)
   int taps_w;               // taps of the wgrad (25 / 9; 1 for the tap-separable output layer)
   int dg_taps;              // taps of the dgrad conv over G (9; 1 for the tap-separable output layer)
   bool sep;                 // decoder output layer in tap-separable form: G is the im2col [pixel][(tap, cls, co)] of the loss gradient
@@ -537,12 +491,11 @@ struct TcTrainPlan {
   unsigned* amax = nullptr;       // one slot per unit (largest |G|, fp32 bits)
   float* raw = nullptr;           // fp32 dgrad result of the current unit
   size_t raw_floats = 0;
-  float* f32_out = nullptr;       // fp32 gradient handed to the SIMT conv1 wgrad (plain NHWC)
   float* partials = nullptr;      // split-K partials of the wgrad GEMMs
   size_t partial_floats = 0;
   float* wm = nullptr;            // fp32 merged sub-pixel weights / padded merged gradient scratch
   size_t wm_floats = 0;
-  // conv1 (Cin = 3): wgrad-only unit appended after the encoder units (index c1, -1 = SIMT wgrad): X = im2col of the input image
+  // conv1 (Cin = 3): wgrad-only unit appended after the encoder units (index c1): X = im2col of the input image
   int c1 = -1;
   __half *c1_x_hi = nullptr, *c1_x_lo = nullptr;
 };
@@ -595,16 +548,14 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     T.out_h = U.gh; T.out_w = U.gw; T.out_c = U.nd;
     T.taps = U.dg_taps;
     T.BW = U.gw; T.BH = std::min(U.gh, 128 / T.BW); T.BB = 128 / (T.BW * T.BH);
-    T.n_tile = 128;
-    T.kch = 64;
-    if (U.gw > 128 || (U.gw & (U.gw - 1)) || (U.gh & (U.gh - 1)) || U.gN % T.kch != 0 || U.nd % T.n_tile != 0 || U.cin % 128 != 0 ||
+    if (U.gw > 128 || (U.gw & (U.gw - 1)) || (U.gh & (U.gh - 1)) || U.gN % TC_KCH != 0 || U.nd % TC_N_TILE != 0 || U.cin % 128 != 0 ||
         U.gN % 64 != 0 || (U.gh * U.gw) % 32 != 0) {
       set_error("tensor-core trainer: layer geometry unsupported (G %dx%dx%d, dgrad N %d, Cin %d)", U.gh, U.gw, U.gN, U.nd, U.cin);
       return AAE_ERR_UNSUPPORTED;
     }
     TcGemmParams& g = T.gp;
     g.N = U.nd; g.OH = U.gh; g.OW = U.gw; g.BW = T.BW; g.BH = T.BH;
-    g.taps = T.taps; g.chunks_per_tap = U.gN / T.kch; g.iters_per_split = g.taps * g.chunks_per_tap;
+    g.taps = T.taps; g.chunks_per_tap = U.gN / TC_KCH; g.iters_per_split = g.taps * g.chunks_per_tap;
     for (int t = 0; t < T.taps; ++t) {
       g.tap_di[t] = (int8_t)(T.taps == 1 ? 0 : t / 3 - 1);
       g.tap_dj[t] = (int8_t)(T.taps == 1 ? 0 : t % 3 - 1);
@@ -626,12 +577,10 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     TcUnit U;
     U.enc = false; U.cin = F.in_c; U.cout = F.out_c;
     U.gh = F.in_h; U.gw = F.in_w;
-    U.sep = l == Ld && dec->sep_out;
-    U.n_real = U.sep ? 36 * F.out_c : 4 * F.out_c;
-    U.gN = U.sep ? 128 : (l == Ld ? 64 : 4 * F.out_c);
+    U.sep = l == Ld;
+    U.gN = U.sep ? 128 : 4 * F.out_c;
     U.taps_w = U.sep ? 1 : 9; U.dg_taps = U.sep ? 1 : 9; U.nd = F.in_c;
     U.mask_hi = F.in_hi;                                   // dgrad result = gradient wrt this layer's input activation
-    if (l == Ld && U.n_real > U.gN) { set_error("tensor-core trainer: output channels > 16 unsupported"); st = AAE_ERR_UNSUPPORTED; break; }
     h->units.push_back(U);
     st = add_unit(h->units.back(), F, F.in_c);
   }
@@ -640,13 +589,13 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     const TcLayer& F = enc->layers[i];
     TcUnit U;
     U.enc = true; U.cin = F.in_c; U.cout = F.out_c;
-    U.gh = F.out_h; U.gw = F.out_w; U.gN = F.out_c; U.n_real = F.out_c;
+    U.gh = F.out_h; U.gw = F.out_w; U.gN = F.out_c;
     U.taps_w = 25; U.dg_taps = 9; U.sep = false; U.nd = 4 * F.in_c;
     U.mask_hi = F.in_hi;                                   // space-to-depth activation, same layout as the dgrad result
     h->units.push_back(U);
     st = add_unit(h->units.back(), F, 4 * F.in_c);
   }
-  if (st == AAE_OK && Le >= 1 && enc->cfg.in_c == 3 && enc->cfg.kernel_size == 5 && enc->layers[0].in_c == 128 && getenv("AAE_C1_WGRAD_SIMT") == nullptr) {
+  if (st == AAE_OK) {
     // dW1[75, 128] = sum over pixels of im2col(x)[pixel, :75]^T G1[pixel, :]: the same 1x1 wgrad GEMM as the tap-separable output layer
     const TcLayer& F2 = enc->layers[0];                    // conv2: in_h x in_w x in_c are the dims of conv1's output (stored space-to-depth)
     const size_t n = (size_t)B * F2.in_h * F2.in_w * 128;
@@ -658,7 +607,7 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
       Fx.in_hi = h->c1_x_hi; Fx.in_lo = h->c1_x_lo; Fx.BB = 1;
       TcUnit U;
       U.enc = true; U.cin = 128; U.cout = F2.in_c;
-      U.gh = F2.in_h; U.gw = F2.in_w; U.gN = F2.in_c; U.n_real = F2.in_c;
+      U.gh = F2.in_h; U.gw = F2.in_w; U.gN = F2.in_c;
       U.taps_w = 1; U.dg_taps = 1; U.sep = false; U.nd = 128;   // (no dgrad is ever run for this unit: the input image needs no gradient)
       U.mask_hi = nullptr;
       h->units.push_back(U);
@@ -669,7 +618,6 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
   part_max = (size_t)40 << 20;   // 160 MB of fp32 partials; wgrad split counts are clamped to fit
   if (st == AAE_OK) st = tc_dev_alloc((void**)&h->amax, 64 * sizeof(unsigned));
   if (st == AAE_OK) st = tc_dev_alloc((void**)&h->raw, raw_max * sizeof(float));
-  if (st == AAE_OK) st = tc_dev_alloc((void**)&h->f32_out, raw_max * sizeof(float));
   if (st == AAE_OK) st = tc_dev_alloc((void**)&h->partials, part_max * sizeof(float));
   if (st == AAE_OK) st = tc_dev_alloc((void**)&h->wm, wm_max * sizeof(float));
   h->raw_floats = raw_max; h->partial_floats = part_max; h->wm_floats = wm_max;
@@ -681,16 +629,15 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
 void tc_train_destroy(TcTrainPlan* h) {
   if (!h) return;
   for (auto& U : h->units) { cudaFree(U.dg.in_hi); cudaFree(U.dg.in_lo); cudaFree(U.dg.w_hi); cudaFree(U.dg.w_lo); }
-  cudaFree(h->amax); cudaFree(h->raw); cudaFree(h->f32_out); cudaFree(h->partials); cudaFree(h->wm);
+  cudaFree(h->amax); cudaFree(h->raw); cudaFree(h->partials); cudaFree(h->wm);
   cudaFree(h->c1_x_hi); cudaFree(h->c1_x_lo);
   delete h;
 }
 
-int tc_train_num_units(const TcTrainPlan* h) { return (int)h->units.size() - (h->c1 >= 0 ? 1 : 0); }   // conv units with a dgrad
+int tc_train_num_units(const TcTrainPlan* h) { return (int)h->units.size() - 1; }   // conv units with a dgrad: all but conv1's
 int tc_train_conv1_unit(const TcTrainPlan* h) { return h->c1; }
 int tc_train_num_decoder_units(const TcTrainPlan* h) { return h->n_dec; }
 float* tc_train_raw(TcTrainPlan* h) { return h->raw; }
-float* tc_train_f32_out(TcTrainPlan* h) { return h->f32_out; }
 
 int tc_train_begin_step(TcTrainPlan* h, cudaStream_t s) {
   AAE_CUDA_OK(cudaMemsetAsync(h->amax, 0, 64 * sizeof(unsigned), s));
@@ -715,7 +662,7 @@ int tc_train_pack_weights_merged(TcTrainPlan* h, int u, const float* wm_dev, cud
   AAE_REQUIRE(u >= 0 && u < h->n_dec, "tc trainer: unit %d is not a decoder unit", u);
   TcUnit& U = h->units[u];
   if (U.sep) pack_dec_dgrad_sep_kernel<<<ew_grid((long long)U.cin * 128), 256, 0, s>>>(wm_dev, U.cin, 4 * U.cout, W_SCALE, U.dg.w_hi, U.dg.w_lo);
-  else pack_dec_dgrad_kernel<<<ew_grid((long long)U.cin * 9 * U.gN), 256, 0, s>>>(wm_dev, U.cin, U.n_real, U.gN, W_SCALE, U.dg.w_hi, U.dg.w_lo);
+  else pack_dec_dgrad_kernel<<<ew_grid((long long)U.cin * 9 * U.gN), 256, 0, s>>>(wm_dev, U.cin, U.gN, W_SCALE, U.dg.w_hi, U.dg.w_lo);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -727,8 +674,7 @@ int tc_train_set_loss_grad(TcTrainPlan* h, const float* g_dev, int B, cudaStream
   const long long n = (long long)B * U.gh * U.gw * 4 * c;
   amax_scalar_kernel<<<ew_grid(n), 256, 0, s>>>(g_dev, n, h->amax + 0);
   AAE_LAUNCH_OK();
-  if (U.sep) pack_loss_grad_sep_kernel<<<ew_grid((long long)B * U.gh * U.gw * 9), 256, 0, s>>>(g_dev, B, U.gh, U.gw, c, h->amax + 0, U.dg.in_hi, U.dg.in_lo);
-  else pack_loss_grad_kernel<<<ew_grid(n), 256, 0, s>>>(g_dev, B, U.gh, U.gw, c, U.gN, h->amax + 0, U.dg.in_hi, U.dg.in_lo);
+  pack_loss_grad_sep_kernel<<<ew_grid((long long)B * U.gh * U.gw * 9), 256, 0, s>>>(g_dev, B, U.gh, U.gw, c, h->amax + 0, U.dg.in_hi, U.dg.in_lo);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -740,7 +686,7 @@ int tc_train_set_unit_grad(TcTrainPlan* h, int u, const float* g_dev, int B, cud
   amax_kernel<<<ew_grid(groups), 256, 0, s>>>(g_dev, nullptr, groups, h->amax + u);
   AAE_LAUNCH_OK();
   finish_kernel<<<ew_grid(groups), 256, 0, s>>>(const_cast<float*>(g_dev), nullptr, groups, REMAP_SAME, U.gh, U.gw, U.gN, h->amax + u, U.dg.in_hi,
-                                                U.dg.in_lo, nullptr, 0, nullptr, 1);
+                                                U.dg.in_lo, 0, nullptr, 1);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -763,22 +709,16 @@ int tc_train_unit_wgrad(TcTrainPlan* h, int u, int B, float* dw_out, cudaStream_
   dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)splits);
   if (U.wg_n_tile == 128) AAE_TRY((launch_wgrad<128, 6>(U.tm_x_hi, U.tm_x_lo, U.tm_g_hi, U.tm_g_lo, w, grid, s)));
   else AAE_TRY((launch_wgrad<64, 6>(U.tm_x_hi, U.tm_x_lo, U.tm_g_hi, U.tm_g_lo, w, grid, s)));
-  if (U.gN == U.n_real) return launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, dw_out, s);
+  if (!U.sep) return launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, dw_out, s);
   AAE_REQUIRE((size_t)mn <= h->wm_floats, "tc trainer: merged-gradient scratch too small");
   AAE_TRY(launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, h->wm, s));
-  if (U.sep) {
-    rearrange_sep_wgrad_kernel<<<ew_grid(9LL * U.cin * 4 * U.cout), 256, 0, s>>>(h->wm, U.cin, 4 * U.cout, dw_out);
-    AAE_LAUNCH_OK();
-    return AAE_OK;
-  }
-  compact_cols_kernel<<<ew_grid((long long)w.ep.M * U.n_real), 256, 0, s>>>(h->wm, w.ep.M, U.gN, U.n_real, dw_out);
+  rearrange_sep_wgrad_kernel<<<ew_grid(9LL * U.cin * 4 * U.cout), 256, 0, s>>>(h->wm, U.cin, 4 * U.cout, dw_out);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
 
 // dW of conv1 [75][cout] from the fp32 input image x [B, H, W, 3] and the unit's G (written by tc_train_finish(..., next = conv1 unit))
 int tc_train_conv1_wgrad(TcTrainPlan* h, const float* x_dev, int B, float* dw_out, cudaStream_t s) {
-  AAE_REQUIRE(h->c1 >= 0, "tc trainer: no tensor-core conv1 wgrad unit");
   TcUnit& U = h->units[h->c1];
   const aae_net_cfg& cfg = h->enc->cfg;
   const long long pixels = (long long)B * U.gh * U.gw;
@@ -797,7 +737,7 @@ int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s) {
   TcLayer& T = U.dg;
   T.gp.M = B * U.gh * U.gw;
   T.gp.amax_bits = h->amax + u;
-  const int m_tiles = (int)ceil_div(T.gp.M, 128), n_tiles = U.nd / T.n_tile;
+  const int m_tiles = (int)ceil_div(T.gp.M, 128), n_tiles = U.nd / TC_N_TILE;
   const int total_iters = T.gp.taps * T.gp.chunks_per_tap;
   // few output tiles and a long K (the 8x8 layers): split K so that the grid covers the SMs, fold the partials afterwards
   int splits = std::max(1, 132 / std::max(1, m_tiles * n_tiles));
@@ -813,10 +753,10 @@ int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s) {
   return AAE_OK;
 }
 
-// raw of unit u -> ReLU mask -> G of unit `next` (when next >= 0) and/or fp32 in the remapped layout (want_f32), the masked
-// fp32 back in place (keep_masked) and its per-channel sums db_out (bias gradient of the layer that produced the masked
-// activation).  Layout change: decoder plain -> space-to-depth (the producing layer's GEMM columns), encoder the reverse.
-int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool want_f32, bool keep_masked, float* db_out, cudaStream_t s) {
+// raw of unit u -> ReLU mask -> G of unit `next` (when next >= 0), the masked fp32 back in place (keep_masked) and its
+// per-channel sums db_out (bias gradient of the layer that produced the masked activation).  Layout change: decoder
+// plain -> space-to-depth (the producing layer's GEMM columns), encoder the reverse.
+int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, float* db_out, cudaStream_t s) {
   TcUnit& U = h->units[u];
   const long long groups = (long long)B * U.gh * U.gw * U.nd / 8;
   __half *hi = nullptr, *lo = nullptr;
@@ -840,8 +780,8 @@ int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool want_f32, bool 
     AAE_REQUIRE((size_t)grid * U.nd <= h->partial_floats, "tc trainer: column-sum scratch too small");
     colsum = h->partials;
   }
-  finish_kernel<<<grid, 256, 0, s>>>(h->raw, U.mask_hi, groups, mode, U.gh, U.gw, C, slot, hi, lo, want_f32 ? h->f32_out : nullptr,
-                                     keep_masked ? 1 : 0, colsum, std::max(gpr, 1));
+  finish_kernel<<<grid, 256, 0, s>>>(h->raw, U.mask_hi, groups, mode, U.gh, U.gw, C, slot, hi, lo, keep_masked ? 1 : 0, colsum,
+                                     std::max(gpr, 1));
   AAE_LAUNCH_OK();
   if (db_out) {
     colsum_final_kernel<<<(unsigned)ceil_div(C, 32), dim3(32, 32), 0, s>>>(colsum, (int)grid, U.nd / C, C, db_out);

@@ -143,6 +143,11 @@ def test_c_abi_rejects_bad_calls_without_crashing(sess):
     assert b"max_batch" in lib.aae_last_error_string()
     assert lib.aae_encoder_forward_u8(h, None, 4, _lib.ptr(z), None) == -1
     assert lib.aae_encoder_forward_u8(h, _lib.ptr(x), 0, _lib.ptr(z), None) == -1
+    assert lib.aae_encoder_forward_u8(h, x.data_ptr() + 1, 4, _lib.ptr(z), None) == -1             # crops not 16-byte aligned
+    assert b"align" in lib.aae_last_error_string()
+    xf = torch.zeros((5, 128, 128, 3), device="cuda")
+    assert lib.aae_encoder_forward_f32(h, xf.data_ptr() + 4, 4, _lib.ptr(z), None) == -1
+    assert b"align" in lib.aae_last_error_string()
     cbh = C.c_void_p()
     E = O.make_codebook(1, n=100, num_cyclo=1, duplicate_cyclo_endpoints=False)
     assert lib.aae_codebook_create(0, _lib.ptr(E), 100, 96, 1, 0, 8, 1, C.byref(cbh)) != 0     # TC match is built for latent 128
@@ -178,6 +183,18 @@ def test_tc_decoder_forward_matches_oracle(sess, batch):
     e_simt, e_tc = np.max(np.abs(outs[0] - ref)), np.max(np.abs(outs[1] - ref))
     print("decoder forward max abs error vs float64: simt %.2e  tc %.2e" % (e_simt, e_tc))
     assert e_simt < 2e-6 and e_tc < 5e-6
+    # the tensor-core output layer takes at most 3 channels; the fp32 path runs a 4-channel decoder
+    from augmentedautoencoder_b200._lib import AaeError
+    for prec in (1, 0):
+        dec4 = Decoder(placeholder(np.float32, [None, 128, 128, 4]), placeholder(np.float32, [None, 128]), list(reversed(O.NUM_FILTER)), 5,
+                       list(reversed(O.STRIDES)), "L2", 4, False, False, max_batch=64, precision=prec)
+        dec4.load_weights(O.make_decoder_params(43, out_ch=4, bias_scale=0.05))
+        if prec == 1:
+            with pytest.raises(AaeError, match="at most 3"):
+                dec4.decode_device(torch.from_numpy(z).cuda())
+        else:
+            x4 = dec4.decode_device(torch.from_numpy(z).cuda()).cpu().numpy()
+            assert x4.shape == (batch, 128, 128, 4) and np.all((x4 >= 0) & (x4 <= 1))
 
 
 def _train_pair(prec, B):
