@@ -46,17 +46,32 @@ struct DevBuf {
   }
 };
 
+// Geometry and fp32 master weights of one conv layer; every precision needs these.
 struct ConvLayer {
   int in_h, in_w, in_c;     // stored input dims
   int out_h, out_w, out_c;
   int ksize, stride, pad_t, pad_l, ups, act;
   DevBuf w, b;              // HWIO kernel, bias
-  DevBuf out;               // activation [max_batch, out_h, out_w, out_c]
-  // sub-pixel form of (x2 nearest upsample + conv5x5): merged 3x3 weights [3,3,in_c,(py,px,out_c)] and the bias tiled 4x
-  bool subpixel = false;
-  bool wm_dirty = true;
-  DevBuf wm, bias4;
   size_t w_count() const { return (size_t)ksize * ksize * in_c * out_c; }
+  size_t out_count(size_t B) const { return B * out_h * out_w * out_c; }
+  // sub-pixel form of (x2 nearest upsample + conv5x5): merged 3x3 weights [3,3,in_c,(py,px,out_c)]
+  bool subpixel() const { return ups == 1 && ksize == 5 && out_c % 4 == 0; }
+  size_t wm_count() const { return subpixel() ? (size_t)9 * in_c * 4 * out_c : 0; }
+};
+
+// Workspace of the fp32 CUDA-core path (AAE_PREC_FP32_SIMT), allocated for that precision only.
+struct SimtEncoder {
+  std::vector<DevBuf> out;  // activation of conv i [max_batch, out_h, out_w, out_c]
+  DevBuf partials;          // split-K scratch
+  ~SimtEncoder() { for (auto& o : out) o.release(); partials.release(); }
+};
+
+struct SimtDecoder {
+  DevBuf dense_out;         // [max_batch, h0, w0, f0]  (post ReLU)
+  std::vector<DevBuf> out, wm, bias4;  // per conv: activation; sub-pixel convs: merged weights and the bias tiled 4x
+  uint64_t wm_version = 0;             // w_version the merged weights were built from
+  DevBuf partials;
+  ~SimtDecoder() { for (auto* v : {&out, &wm, &bias4}) for (auto& d : *v) d.release(); dense_out.release(); partials.release(); }
 };
 
 void tf_same_pad(int in, int k, int stride, int* before) {
@@ -114,28 +129,6 @@ IGemmParams dense_params(const float* src, int B, int in_features, const float* 
   p.Bm = w; p.N = out_features; p.M = B; p.K = in_features;
   return p;
 }
-
-// Optional per-stage device timing (cudaEvents on the launching stream), read back by bench.py for the roofline lines.
-struct StageTimer {
-  bool enabled = false;
-  std::vector<cudaEvent_t> ev;   // stage i is bracketed by ev[i], ev[i+1]
-  int used = 0;
-  void mark(cudaStream_t s) {
-    if (!enabled) return;
-    if (used == (int)ev.size()) { cudaEvent_t e; if (cudaEventCreate(&e) != cudaSuccess) return; ev.push_back(e); }
-    cudaEventRecord(ev[used++], s);
-  }
-  void reset() { used = 0; }
-  int read(float* ms, int cap) {
-    int n = 0;
-    if (used >= 2) {
-      cudaEventSynchronize(ev[used - 1]);
-      for (int i = 0; i + 1 < used && n < cap; ++i, ++n) cudaEventElapsedTime(&ms[n], ev[i], ev[i + 1]);
-    }
-    return n;
-  }
-  void release() { for (auto e : ev) cudaEventDestroy(e); ev.clear(); used = 0; }
-};
 
 // Per-phase device timing of the training step: every mark opens a phase; the time until the next mark is charged to it.
 struct PhaseTimer {
@@ -203,15 +196,14 @@ struct aae_encoder {
   std::vector<ConvLayer> conv;
   int flat;                 // features entering the dense layer
   DevBuf dense_w, dense_b;  // [flat, latent], [latent]
-  DevBuf partials;          // split-K scratch
+  SimtEncoder* simt = nullptr;  // fp32 CUDA-core workspace (AAE_PREC_FP32_SIMT)
   TcEncoder* tc = nullptr;  // tensor-core execution plan (AAE_PREC_TC_SPLIT)
   int last_batch = 0;
-  bool last_was_tc = false;
-  // the fp32 tensors above are the master copy; the tensor-core plan holds packed (hi, lo) fp16 operands derived from them.
-  // w_version counts changes of the master copy (set_weights, Adam); tc_stale = the plan's operands are older than the masters
-  // (set by the optimizer step, which updates the masters in place; cleared by the lazy repack in the forward entry points).
+  // the fp32 tensors above are the master copy.  w_version counts its changes (set_weights, Adam); every copy derived from it
+  // (the tensor-core plan's packed (hi, lo) fp16 operands, the fp32 decoder's merged sub-pixel weights, the trainer's dgrad
+  // operands) records the w_version it was built from and is rebuilt just before its next use when the two differ.
   uint64_t w_version = 1;
-  bool tc_stale = false;
+  uint64_t tc_version = 1;  // the plan's operands start as zeros, like the masters
   StageTimer timer;
 };
 
@@ -220,13 +212,10 @@ struct aae_decoder {
   aae_net_cfg cfg;
   int h0, w0, f0;           // spatial size / filters after the dense layer
   DevBuf dense_w, dense_b;  // [latent, h0*w0*f0]
-  DevBuf dense_out;         // [max_batch, h0, w0, f0]  (post ReLU)
   std::vector<ConvLayer> conv;  // forward order; conv.back() is the sigmoid output layer
-  DevBuf partials;
+  SimtDecoder* simt = nullptr;  // fp32 CUDA-core workspace (AAE_PREC_FP32_SIMT)
   TcDecoder* tc = nullptr;      // tensor-core execution plan (AAE_PREC_TC_SPLIT, forward only)
-  int last_batch = 0;
-  uint64_t w_version = 1;       // see aae_encoder
-  bool tc_stale = false;
+  uint64_t w_version = 1, tc_version = 1;   // see aae_encoder
 };
 
 struct aae_codebook {
@@ -256,8 +245,9 @@ struct aae_trainer {
   // gradients / Adam state: enc conv kernels+biases, enc dense, dec dense, dec convs (same order as *_set_weights)
   std::vector<ParamGrad> enc_k, enc_b, dec_k, dec_b;
   DevBuf dx_out;        // dLoss/d(decoder output) then pre-sigmoid grad  [B, H, W, C]
-  DevBuf grad_a, grad_b;  // ping-pong pre-activation gradients
-  DevBuf dxup;          // full-resolution dgrad scratch (before 2x2 sum pooling)
+  DevBuf grad_a;        // fp32 trainer: ping-pong pre-activation gradients with grad_b; tensor-core trainer: gradient wrt `flat`
+  DevBuf grad_b, dxup;  // fp32 trainer only; dxup: full-resolution dgrad scratch (before 2x2 sum pooling)
+  DevBuf flat;          // tensor-core trainer only: fp32 copy of the encoder's last conv activation [B, flat]
   DevBuf wt;            // transposed-weight scratch
   DevBuf partials;      // split-K / small-N partials
   DevBuf bias_scratch;  // 256 * max(out_c)
@@ -304,6 +294,14 @@ static int check_cfg(const aae_net_cfg* cfg) {
 }
 
 // ============================================================================ encoder
+static int simt_encoder_create(aae_encoder* h) {
+  SimtEncoder* S = h->simt = new (std::nothrow) SimtEncoder();
+  AAE_REQUIRE(S != nullptr, "host allocation failed");
+  for (auto& L : h->conv) { S->out.emplace_back(); AAE_TRY(S->out.back().alloc(L.out_count(h->cfg.max_batch))); }
+  // split-K scratch for the skinny dense layer: up to 296 splits of [max_batch, latent]
+  return S->partials.alloc((size_t)320 * std::max(h->cfg.max_batch, 128) * h->cfg.latent);
+}
+
 extern "C" int aae_encoder_create(int device, const aae_net_cfg* cfg, aae_encoder** out) {
   AAE_REQUIRE(out != nullptr, "out is null");
   *out = nullptr;
@@ -316,7 +314,6 @@ extern "C" int aae_encoder_create(int device, const aae_net_cfg* cfg, aae_encode
   h->cfg = *cfg;
   int ih = cfg->in_h, iw = cfg->in_w, ic = cfg->in_c;
   int st = AAE_OK;
-  size_t max_partial = 0;
   for (int i = 0; i < cfg->num_layers && st == AAE_OK; ++i) {
     ConvLayer L;
     L.in_h = ih; L.in_w = iw; L.in_c = ic;
@@ -328,7 +325,6 @@ extern "C" int aae_encoder_create(int device, const aae_net_cfg* cfg, aae_encode
     ConvLayer& R = h->conv.back();
     if ((st = R.w.alloc(R.w_count())) != AAE_OK) break;
     if ((st = R.b.alloc(R.out_c)) != AAE_OK) break;
-    if ((st = R.out.alloc((size_t)cfg->max_batch * R.out_h * R.out_w * R.out_c)) != AAE_OK) break;
     cudaMemset(R.w.p, 0, R.w.n * sizeof(float));
     cudaMemset(R.b.p, 0, R.b.n * sizeof(float));
     ih = R.out_h; iw = R.out_w; ic = R.out_c;
@@ -340,12 +336,9 @@ extern "C" int aae_encoder_create(int device, const aae_net_cfg* cfg, aae_encode
     if (st == AAE_OK) {
       cudaMemset(h->dense_w.p, 0, h->dense_w.n * sizeof(float));
       cudaMemset(h->dense_b.p, 0, h->dense_b.n * sizeof(float));
-      // split-K scratch for the skinny dense layer: up to 296 splits of [max_batch, latent]
-      max_partial = (size_t)320 * std::max(cfg->max_batch, 128) * cfg->latent;
-      st = h->partials.alloc(max_partial);
     }
   }
-  if (st == AAE_OK && cfg->precision == AAE_PREC_TC_SPLIT) st = tc_encoder_create(device, cfg, &h->tc);
+  if (st == AAE_OK) st = cfg->precision == AAE_PREC_TC_SPLIT ? tc_encoder_create(device, cfg, &h->tc) : simt_encoder_create(h);
   if (st != AAE_OK) { aae_encoder_destroy(h); return st; }
   *out = h;
   return AAE_OK;
@@ -354,8 +347,9 @@ extern "C" int aae_encoder_create(int device, const aae_net_cfg* cfg, aae_encode
 extern "C" int aae_encoder_destroy(aae_encoder* h) {
   if (!h) return AAE_OK;
   DeviceGuard g(h->device);
-  for (auto& L : h->conv) { L.w.release(); L.b.release(); L.out.release(); }
-  h->dense_w.release(); h->dense_b.release(); h->partials.release();
+  for (auto& L : h->conv) { L.w.release(); L.b.release(); }
+  h->dense_w.release(); h->dense_b.release();
+  delete h->simt;
   if (h->tc) tc_encoder_destroy(h->tc);
   h->timer.release();
   delete h;
@@ -371,9 +365,11 @@ extern "C" int aae_encoder_set_weights(aae_encoder* h, int layer, const float* k
   DevBuf& b = layer < (int)h->conv.size() ? h->conv[layer].b : h->dense_b;
   if (kernel_any) AAE_TRY(copy_any(w.p, kernel_any, w.n * sizeof(float), s));
   if (bias_any) AAE_TRY(copy_any(b.p, bias_any, b.n * sizeof(float), s));
+  const bool tc_current = h->tc_version == h->w_version;
   h->w_version += 1;
   if (h->tc && kernel_any) AAE_TRY(tc_encoder_pack_weights(h->tc, layer, w.p, s));
   if (h->tc) AAE_TRY(tc_encoder_set_bias(h->tc, layer, b.p));
+  if (tc_current) h->tc_version = h->w_version;   // this layer is packed again; a plan behind by an Adam step stays behind
   AAE_CUDA_OK(cudaStreamSynchronize(s));  // host source buffers may be freed by the caller on return
   if (h->tc) AAE_TRY(range_peek(tc_encoder_range_flag(h->tc), "encoder set_weights", 0, s));
   return AAE_OK;
@@ -407,28 +403,30 @@ extern "C" int aae_encoder_get_weights(aae_encoder* h, int layer, float* kernel_
 // Re-derive the tensor-core plan's packed operands from the fp32 master weights after an optimizer step changed them in place
 // (inference in the training process -- Codebook.update_embedding, decoder.x -- must see the weights get_weights() returns).
 static int encoder_sync_tc(aae_encoder* h, cudaStream_t s) {
-  if (!h->tc || !h->tc_stale) return AAE_OK;
+  if (!h->tc || h->tc_version == h->w_version) return AAE_OK;
   const int nl = (int)h->conv.size();
   for (int i = 0; i < nl; ++i) AAE_TRY(tc_encoder_pack_weights(h->tc, i, h->conv[i].w.p, s));
   AAE_TRY(tc_encoder_pack_weights(h->tc, nl, h->dense_w.p, s));
-  h->tc_stale = false;
+  h->tc_version = h->w_version;
   return AAE_OK;
 }
 
 static int encoder_forward_simt(aae_encoder* h, const void* crops, int src_u8, int B, float* z_out, cudaStream_t s) {
+  SimtEncoder& S = *h->simt;
   const void* src = crops;
   int u8 = src_u8;
   h->timer.reset();
   h->timer.mark(s);
-  for (auto& L : h->conv) {
+  for (size_t i = 0; i < h->conv.size(); ++i) {
+    const ConvLayer& L = h->conv[i];
     IGemmParams p = conv_params(L, src, u8, B);
-    AAE_TRY(run_igemm(p, GATHER_FWD, h->partials, L.out.p, L.b.p, L.act, nullptr, s));
+    AAE_TRY(run_igemm(p, GATHER_FWD, S.partials, S.out[i].p, L.b.p, L.act, nullptr, s));
     h->timer.mark(s);
-    src = L.out.p;
+    src = S.out[i].p;
     u8 = 0;
   }
   IGemmParams p = dense_params((const float*)src, B, h->flat, h->dense_w.p, h->cfg.latent);
-  AAE_TRY(run_igemm(p, GATHER_FWD, h->partials, z_out, h->dense_b.p, ACT_NONE, nullptr, s));
+  AAE_TRY(run_igemm(p, GATHER_FWD, S.partials, z_out, h->dense_b.p, ACT_NONE, nullptr, s));
   h->timer.mark(s);
   return AAE_OK;
 }
@@ -440,11 +438,9 @@ static int encoder_forward(aae_encoder* h, const void* crops, int src_u8, int B,
   DeviceGuard g(h->device);
   h->last_batch = B;
   if (h->tc) {
-    h->last_was_tc = true;
     AAE_TRY(encoder_sync_tc(h, (cudaStream_t)stream));
-    return tc_encoder_forward(h->tc, crops, src_u8, B, h->conv[0].w.p, h->conv[0].b.p, h->dense_b.p, z_out, (cudaStream_t)stream);
+    return tc_encoder_forward(h->tc, crops, src_u8, B, h->conv[0].w.p, h->conv[0].b.p, h->dense_b.p, z_out, &h->timer, (cudaStream_t)stream);
   }
-  h->last_was_tc = false;
   return encoder_forward_simt(h, crops, src_u8, B, z_out, (cudaStream_t)stream);
 }
 
@@ -458,13 +454,11 @@ extern "C" int aae_encoder_forward_f32(aae_encoder* h, const float* crops_dev, i
 extern "C" int aae_encoder_activation(aae_encoder* h, int layer, const float** ptr_dev, int64_t* count) {
   AAE_REQUIRE(h != nullptr && ptr_dev != nullptr && count != nullptr, "null argument");
   AAE_REQUIRE(layer >= 0 && layer <= (int)h->conv.size(), "layer %d out of range", layer);
-  if (h->last_was_tc) {
-    DeviceGuard g(h->device);
-    return tc_encoder_activation(h->tc, std::min(layer, (int)h->conv.size() - 1), h->last_batch, ptr_dev, count, nullptr);
-  }
-  const ConvLayer& L = h->conv[std::min(layer, (int)h->conv.size() - 1)];
-  *ptr_dev = L.out.p;
-  *count = (int64_t)h->last_batch * L.out_h * L.out_w * L.out_c;
+  const int l = std::min(layer, (int)h->conv.size() - 1);
+  DeviceGuard g(h->device);
+  if (h->tc) return tc_encoder_activation(h->tc, l, h->last_batch, ptr_dev, count, nullptr);
+  *ptr_dev = h->simt->out[l].p;
+  *count = (int64_t)h->conv[l].out_count(h->last_batch);
   return AAE_OK;
 }
 
@@ -472,9 +466,8 @@ extern "C" int aae_encoder_profile(aae_encoder* h, int enable, float* stage_ms_o
   AAE_REQUIRE(h != nullptr, "encoder handle is null");
   DeviceGuard g(h->device);
   int n = 0;
-  if (stage_ms_out && capacity > 0) n = h->tc ? tc_encoder_read_timer(h->tc, stage_ms_out, capacity) : h->timer.read(stage_ms_out, capacity);
+  if (stage_ms_out && capacity > 0) n = h->timer.read(stage_ms_out, capacity);
   h->timer.enabled = enable != 0;
-  if (h->tc) tc_encoder_enable_timer(h->tc, enable != 0);
   return n;
 }
 
@@ -617,6 +610,20 @@ extern "C" int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, 
 }
 
 // ============================================================================ decoder
+static int simt_decoder_create(aae_decoder* h) {
+  SimtDecoder* S = h->simt = new (std::nothrow) SimtDecoder();
+  AAE_REQUIRE(S != nullptr, "host allocation failed");
+  const size_t B = h->cfg.max_batch;
+  AAE_TRY(S->dense_out.alloc(B * h->dense_b.n));
+  for (auto& L : h->conv) {
+    S->out.emplace_back(); S->wm.emplace_back(); S->bias4.emplace_back();
+    AAE_TRY(S->out.back().alloc(L.out_count(B)));
+    AAE_TRY(S->wm.back().alloc(L.wm_count()));
+    AAE_TRY(S->bias4.back().alloc(L.subpixel() ? (size_t)4 * L.out_c : 0));
+  }
+  return S->partials.alloc((size_t)4 << 20);
+}
+
 extern "C" int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decoder** out) {
   AAE_REQUIRE(out != nullptr, "out is null");
   *out = nullptr;
@@ -645,7 +652,6 @@ extern "C" int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decode
     const size_t dense_out = (size_t)h->h0 * h->w0 * h->f0;
     status = h->dense_w.alloc((size_t)cfg->latent * dense_out);
     if (status == AAE_OK) status = h->dense_b.alloc(dense_out);
-    if (status == AAE_OK) status = h->dense_out.alloc((size_t)cfg->max_batch * dense_out);
     if (status == AAE_OK) { cudaMemset(h->dense_w.p, 0, h->dense_w.n * 4); cudaMemset(h->dense_b.p, 0, h->dense_b.n * 4); }
   }
   int ih = dims[0], ic = nf[0];
@@ -661,17 +667,10 @@ extern "C" int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decode
     ConvLayer& R = h->conv.back();
     if ((status = R.w.alloc(R.w_count())) != AAE_OK) break;
     if ((status = R.b.alloc(R.out_c)) != AAE_OK) break;
-    if ((status = R.out.alloc((size_t)cfg->max_batch * R.out_h * R.out_w * R.out_c)) != AAE_OK) break;
     cudaMemset(R.w.p, 0, R.w.n * 4); cudaMemset(R.b.p, 0, R.b.n * 4);
-    R.subpixel = R.ksize == 5 && R.out_c % 4 == 0;
-    if (R.subpixel) {
-      if ((status = R.wm.alloc((size_t)9 * R.in_c * 4 * R.out_c)) != AAE_OK) break;
-      if ((status = R.bias4.alloc((size_t)4 * R.out_c)) != AAE_OK) break;
-    }
     ih = R.out_h; ic = R.out_c;
   }
-  if (status == AAE_OK) status = h->partials.alloc((size_t)4 << 20);
-  if (status == AAE_OK && cfg->precision == AAE_PREC_TC_SPLIT) status = tc_decoder_create(device, cfg, &h->tc);
+  if (status == AAE_OK) status = cfg->precision == AAE_PREC_TC_SPLIT ? tc_decoder_create(device, cfg, &h->tc) : simt_decoder_create(h);
   if (status != AAE_OK) { aae_decoder_destroy(h); return status; }
   *out = h;
   return AAE_OK;
@@ -680,8 +679,9 @@ extern "C" int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decode
 extern "C" int aae_decoder_destroy(aae_decoder* h) {
   if (!h) return AAE_OK;
   DeviceGuard g(h->device);
-  h->dense_w.release(); h->dense_b.release(); h->dense_out.release(); h->partials.release();
-  for (auto& L : h->conv) { L.w.release(); L.b.release(); L.out.release(); L.wm.release(); L.bias4.release(); }
+  h->dense_w.release(); h->dense_b.release();
+  for (auto& L : h->conv) { L.w.release(); L.b.release(); }
+  delete h->simt;
   if (h->tc) tc_decoder_destroy(h->tc);
   delete h;
   return AAE_OK;
@@ -696,9 +696,10 @@ extern "C" int aae_decoder_set_weights(aae_decoder* h, int layer, const float* k
   DevBuf& b = layer == 0 ? h->dense_b : h->conv[layer - 1].b;
   if (kernel_any) AAE_TRY(copy_any(w.p, kernel_any, w.n * sizeof(float), s));
   if (bias_any) AAE_TRY(copy_any(b.p, bias_any, b.n * sizeof(float), s));
-  if (layer > 0) h->conv[layer - 1].wm_dirty = true;
-  h->w_version += 1;
+  const bool tc_current = h->tc_version == h->w_version;
+  h->w_version += 1;   // the fp32 path's merged sub-pixel weights are rebuilt by the next forward
   if (h->tc) AAE_TRY(tc_decoder_pack_weights(h->tc, layer, kernel_any ? w.p : nullptr, bias_any ? b.p : nullptr, s));
+  if (tc_current) h->tc_version = h->w_version;   // see aae_encoder_set_weights
   AAE_CUDA_OK(cudaStreamSynchronize(s));
   if (h->tc) AAE_TRY(range_peek(tc_decoder_range_flag(h->tc), "decoder set_weights", 0, s));
   return AAE_OK;
@@ -724,35 +725,36 @@ extern "C" int aae_decoder_get_weights(aae_decoder* h, int layer, float* kernel_
 }
 
 static int decoder_sync_tc(aae_decoder* h, cudaStream_t s) {   // see encoder_sync_tc
-  if (!h->tc || !h->tc_stale) return AAE_OK;
+  if (!h->tc || h->tc_version == h->w_version) return AAE_OK;
   AAE_TRY(tc_decoder_pack_weights(h->tc, 0, h->dense_w.p, h->dense_b.p, s));
   for (int l = 1; l <= (int)h->conv.size(); ++l) AAE_TRY(tc_decoder_pack_weights(h->tc, l, h->conv[l - 1].w.p, h->conv[l - 1].b.p, s));
-  h->tc_stale = false;
+  h->tc_version = h->w_version;
   return AAE_OK;
 }
 
 static int decoder_forward_impl(aae_decoder* h, const float* z, int B, float* x_out, cudaStream_t s) {
+  SimtDecoder& S = *h->simt;
   const int dense_out = h->h0 * h->w0 * h->f0;
   IGemmParams p = dense_params(z, B, h->cfg.latent, h->dense_w.p, dense_out);
-  AAE_TRY(run_igemm(p, GATHER_FWD, h->partials, h->dense_out.p, h->dense_b.p, ACT_RELU, nullptr, s));
-  const float* src = h->dense_out.p;
+  AAE_TRY(run_igemm(p, GATHER_FWD, S.partials, S.dense_out.p, h->dense_b.p, ACT_RELU, nullptr, s));
+  const float* src = S.dense_out.p;
+  const bool remerge = S.wm_version != h->w_version;
   for (size_t i = 0; i < h->conv.size(); ++i) {
     ConvLayer& L = h->conv[i];
-    float* dst = (i + 1 == h->conv.size() && x_out) ? x_out : L.out.p;
-    if (L.subpixel) {
+    float* dst = (i + 1 == h->conv.size() && x_out) ? x_out : S.out[i].p;
+    if (L.subpixel()) {
       // upsample x2 + conv5x5 == four 3x3 convs of the low-res input with merged taps: one GEMM, N = 4*Cout, 9/25 of the MACs
-      if (L.wm_dirty) {
-        AAE_TRY(launch_merge_subpixel_weights(L.w.p, L.in_c, L.out_c, L.wm.p, s));
-        for (int c = 0; c < 4; ++c) AAE_CUDA_OK(cudaMemcpyAsync(L.bias4.p + c * L.out_c, L.b.p, L.out_c * sizeof(float), cudaMemcpyDeviceToDevice, s));
-        L.wm_dirty = false;
+      if (remerge) {
+        AAE_TRY(launch_merge_subpixel_weights(L.w.p, L.in_c, L.out_c, S.wm[i].p, s));
+        for (int c = 0; c < 4; ++c) AAE_CUDA_OK(cudaMemcpyAsync(S.bias4[i].p + c * L.out_c, L.b.p, L.out_c * sizeof(float), cudaMemcpyDeviceToDevice, s));
       }
       IGemmParams q;
       memset(&q, 0, sizeof(q));
       q.src = src; q.B = B; q.SH = L.in_h; q.SW = L.in_w; q.SC = L.in_c;
       q.PH = L.in_h; q.PW = L.in_w; q.KH = q.KW = 3; q.stride = 1; q.pad_t = q.pad_l = 1;
-      q.Bm = L.wm.p; q.N = 4 * L.out_c; q.M = B * L.in_h * L.in_w; q.K = 9 * L.in_c;
+      q.Bm = S.wm[i].p; q.N = 4 * L.out_c; q.M = B * L.in_h * L.in_w; q.K = 9 * L.in_c;
       q.d2s_out = 1;
-      AAE_TRY(run_igemm(q, GATHER_FWD, h->partials, dst, L.bias4.p, L.act, nullptr, s, /*allow_split=*/false));
+      AAE_TRY(run_igemm(q, GATHER_FWD, S.partials, dst, S.bias4[i].p, L.act, nullptr, s, /*allow_split=*/false));
       src = dst;
       continue;
     }
@@ -761,10 +763,11 @@ static int decoder_forward_impl(aae_decoder* h, const float* z, int B, float* x_
       q.C = dst; q.bias = L.b.p; q.act = L.act;
       AAE_TRY(launch_conv_small_n(q, s));
     } else {
-      AAE_TRY(run_igemm(q, GATHER_FWD, h->partials, dst, L.b.p, L.act, nullptr, s));
+      AAE_TRY(run_igemm(q, GATHER_FWD, S.partials, dst, L.b.p, L.act, nullptr, s));
     }
     src = dst;
   }
+  S.wm_version = h->w_version;
   return AAE_OK;
 }
 
@@ -772,7 +775,6 @@ extern "C" int aae_decoder_forward(aae_decoder* h, const float* z_dev, int batch
   AAE_REQUIRE(h != nullptr && z_dev != nullptr && x_out_dev != nullptr, "null argument");
   AAE_REQUIRE(batch >= 1 && batch <= h->cfg.max_batch, "batch %d outside [1, max_batch=%d]", batch, h->cfg.max_batch);
   DeviceGuard g(h->device);
-  h->last_batch = batch;
   if (h->tc) {
     AAE_TRY(decoder_sync_tc(h, (cudaStream_t)stream));
     return tc_decoder_forward(h->tc, z_dev, batch, x_out_dev, (cudaStream_t)stream);
@@ -825,26 +827,29 @@ extern "C" int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootst
   if (st == AAE_OK) st = make_pg(h->dec_k, dec->dense_w);
   if (st == AAE_OK) st = make_pg(h->dec_b, dec->dense_b);
   for (auto& L : dec->conv) { if (st == AAE_OK) st = make_pg(h->dec_k, L.w); if (st == AAE_OK) st = make_pg(h->dec_b, L.b); }
-  const size_t B = enc->cfg.max_batch;
-  size_t max_act = 0, max_up = 0, max_w = std::max(enc->dense_w.n, dec->dense_w.n), max_c = 0;
-  for (auto& L : enc->conv) { max_act = std::max(max_act, L.out.n); max_w = std::max(max_w, L.w.n); max_c = std::max<size_t>(max_c, L.out_c); }
+  const size_t B = enc->cfg.max_batch, max_dense_w = std::max(enc->dense_w.n, dec->dense_w.n);
+  size_t max_act = 0, max_up = 0, max_w = max_dense_w, max_c = 0;
+  for (auto& L : enc->conv) { max_act = std::max(max_act, L.out_count(B)); max_w = std::max(max_w, L.w_count()); max_c = std::max<size_t>(max_c, L.out_c); }
   size_t max_wm = 0;
   for (auto& L : dec->conv) {
-    max_act = std::max(max_act, L.out.n);
+    max_act = std::max(max_act, L.out_count(B));
     max_up = std::max(max_up, B * L.out_h * L.out_w * (size_t)std::max(L.in_c, L.out_c));
-    max_w = std::max(max_w, std::max(L.w.n, L.wm.n));
-    max_wm = std::max(max_wm, L.wm.n);
+    max_w = std::max(max_w, std::max(L.w_count(), L.wm_count()));
+    max_wm = std::max(max_wm, L.wm_count());
     max_c = std::max<size_t>(max_c, L.out_c);
   }
-  max_act = std::max(max_act, dec->dense_out.n);
+  max_act = std::max(max_act, B * dec->dense_b.n);
   max_c = std::max<size_t>(max_c, dec->dense_b.n);
   const size_t out_elems = B * enc->cfg.in_h * enc->cfg.in_w * enc->cfg.in_c;
+  // the tensor-core trainer runs only the two dense layers' backward on fp32 buffers: a [B, flat] gradient and the dense kernels
+  const bool simt = enc->tc == nullptr;
   if (st == AAE_OK) st = h->dx_out.alloc(out_elems);
   if (st == AAE_OK) st = h->rec.alloc(out_elems);
-  if (st == AAE_OK) st = h->grad_a.alloc(max_act);
-  if (st == AAE_OK) st = h->grad_b.alloc(max_act);
-  if (st == AAE_OK) st = h->dxup.alloc(max_up);
-  if (st == AAE_OK) st = h->wt.alloc(max_w);
+  if (st == AAE_OK) st = h->grad_a.alloc(simt ? max_act : B * enc->flat);
+  if (st == AAE_OK) st = h->grad_b.alloc(simt ? max_act : 0);
+  if (st == AAE_OK) st = h->dxup.alloc(simt ? max_up : 0);
+  if (st == AAE_OK) st = h->flat.alloc(simt ? 0 : B * enc->flat);
+  if (st == AAE_OK) st = h->wt.alloc(simt ? max_w : max_dense_w);
   if (st == AAE_OK) st = h->partials.alloc((size_t)48 << 20);
   if (st == AAE_OK) st = h->bias_scratch.alloc(256 * max_c);
   if (st == AAE_OK) st = h->sample_sums.alloc(B);
@@ -862,7 +867,7 @@ extern "C" int aae_trainer_destroy(aae_trainer* h) {
   DeviceGuard g(h->enc->device);
   for (auto* v : {&h->enc_k, &h->enc_b, &h->dec_k, &h->dec_b})
     for (auto& pg : *v) { pg.g.release(); pg.m.release(); pg.v.release(); }
-  h->dx_out.release(); h->grad_a.release(); h->grad_b.release(); h->dxup.release(); h->wt.release(); h->partials.release();
+  h->dx_out.release(); h->grad_a.release(); h->grad_b.release(); h->dxup.release(); h->flat.release(); h->wt.release(); h->partials.release();
   h->bias_scratch.release(); h->sample_sums.release(); h->z.release(); h->dz.release(); h->rec.release(); h->dwm.release();
   tc_train_destroy(h->tc);
   h->ptimer.release();
@@ -990,15 +995,14 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
   pt.mark(0, s);
   // ---- operands follow the fp32 master weights (Adam and set_weights change those) ----
   AAE_TRY(encoder_sync_tc(E, s));
-  if (h->packed_dec_version != D->w_version || D->tc_stale) {
+  if (h->packed_dec_version != D->w_version || D->tc_version != D->w_version) {
     // forward and dgrad operands of a decoder layer share one merge of its 5x5 taps
     AAE_TRY(tc_decoder_pack_weights(D->tc, 0, D->dense_w.p, D->dense_b.p, s));
     for (int l = 1; l <= nd; ++l) {
       AAE_TRY(tc_decoder_pack_weights(D->tc, l, D->conv[l - 1].w.p, D->conv[l - 1].b.p, s));
       AAE_TRY(tc_train_pack_weights_merged(P, nd - l, tc_decoder_merged_weights(D->tc), s));
     }
-    D->tc_stale = false;
-    h->packed_dec_version = D->w_version;
+    D->tc_version = h->packed_dec_version = D->w_version;
   }
   if (h->packed_enc_version != E->w_version) {
     for (int u = n_dec; u < n_units; ++u) AAE_TRY(tc_train_pack_weights(P, u, E->conv[nl - 1 - (u - n_dec)].w.p, s));
@@ -1007,9 +1011,8 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
   pt.mark(1, s);
   AAE_TRY(tc_train_begin_step(P, s));
   // ---- forward ----
-  E->last_batch = B; E->last_was_tc = true;
-  AAE_TRY(tc_encoder_forward(E->tc, x, 0, B, E->conv[0].w.p, E->conv[0].b.p, E->dense_b.p, h->z.p, s));
-  D->last_batch = B;
+  E->last_batch = B;
+  AAE_TRY(tc_encoder_forward(E->tc, x, 0, B, E->conv[0].w.p, E->conv[0].b.p, E->dense_b.p, h->z.p, &E->timer, s));
   AAE_TRY(tc_decoder_forward(D->tc, h->z.p, B, h->rec.p, s));
   const int k = h->bootstrap_ratio > 1 ? numel / h->bootstrap_ratio : numel;
   AAE_TRY(launch_bootstrap_l2(h->rec.p, y, B, numel, k, h->sample_sums.p, loss_out, h->dx_out.p, s));
@@ -1037,7 +1040,7 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
   pt.mark(5, s);
   AAE_TRY(decoder_dense_backward(h, raw, B, s));
   // ---- encoder backward ----
-  float* flat = E->conv.back().out.p;            // fp32 view of the last conv activation for the fp32 dense backward
+  float* flat = h->flat.p;                       // fp32 view of the last conv activation for the fp32 dense backward
   pt.mark(4, s);
   AAE_TRY(tc_train_unpack_flat(P, B, flat, s));
   float* da = h->grad_a.p;
@@ -1074,9 +1077,9 @@ static int trainer_fwd_bwd(aae_trainer* h, const float* x, const float* y, int B
   const int H = E->cfg.in_h, W = E->cfg.in_w, C = E->cfg.in_c;
   const int numel = H * W * C;
   // ---- forward ----
-  E->last_batch = B; E->last_was_tc = false;
+  const SimtEncoder& SE = *E->simt; const SimtDecoder& SD = *D->simt;
+  E->last_batch = B;
   AAE_TRY(encoder_forward_simt(E, x, 0, B, h->z.p, s));
-  D->last_batch = B;
   AAE_TRY(decoder_forward_impl(D, h->z.p, B, h->rec.p, s));
   const int k = h->bootstrap_ratio > 1 ? numel / h->bootstrap_ratio : numel;
   AAE_TRY(launch_bootstrap_l2(h->rec.p, y, B, numel, k, h->sample_sums.p, loss_out, h->dx_out.p, s));
@@ -1087,10 +1090,10 @@ static int trainer_fwd_bwd(aae_trainer* h, const float* x, const float* y, int B
   float* pong = h->grad_b.p;
   for (int i = (int)D->conv.size() - 1; i >= 0; --i) {
     ConvLayer& L = D->conv[i];
-    const float* in_act = i == 0 ? D->dense_out.p : D->conv[i - 1].out.p;
+    const float* in_act = i == 0 ? SD.dense_out.p : SD.out[i - 1].p;
     const int64_t rows = (int64_t)B * L.out_h * L.out_w;
     AAE_TRY(launch_bias_grad(dy, rows, L.out_c, h->dec_b[i + 1].g.p, h->bias_scratch.p, s));
-    if (L.subpixel) {
+    if (L.subpixel()) {
       // backward of the sub-pixel GEMM  Ys[b,i,j,(cls,co)] = sum_{dy,dx,ci} a[b,i+dy,j+dx,ci] Wm[dy,dx,ci,(cls,co)]
       float* dys = h->dxup.p;                                              // dY in space-to-depth form [B*h*w, 4*Cout]
       AAE_TRY(launch_space_to_depth(dy, dys, B, L.in_h, L.in_w, L.out_c, s));
@@ -1102,7 +1105,7 @@ static int trainer_fwd_bwd(aae_trainer* h, const float* x, const float* y, int B
       AAE_TRY(run_igemm(w, GATHER_WGRAD, h->partials, h->dwm.p, nullptr, ACT_NONE, nullptr, s));
       AAE_TRY(launch_unmerge_subpixel_grads(h->dwm.p, L.in_c, L.out_c, h->dec_k[i + 1].g.p, s));
       // dgrad: dA[pix, ci] = sum_{tap,(cls,co)} dYs[pix - tap, (cls,co)] Wm[tap, ci, (cls,co)], fused with the ReLU mask of a
-      AAE_TRY(launch_transpose_last2(L.wm.p, h->wt.p, 9, L.in_c, 4 * L.out_c, s));
+      AAE_TRY(launch_transpose_last2(SD.wm[i].p, h->wt.p, 9, L.in_c, 4 * L.out_c, s));
       IGemmParams d;
       memset(&d, 0, sizeof(d));
       d.src = dys; d.B = B; d.SH = L.in_h; d.SW = L.in_w; d.SC = 4 * L.out_c;
@@ -1124,12 +1127,12 @@ static int trainer_fwd_bwd(aae_trainer* h, const float* x, const float* y, int B
   // ---- encoder backward ----
   {
     const int nl = (int)E->conv.size();
-    AAE_TRY(encoder_dense_backward(h, E->conv.back().out.p, B, ping, s));
+    AAE_TRY(encoder_dense_backward(h, SE.out.back().p, B, ping, s));
     dy = ping;
     std::swap(ping, pong);
     for (int i = nl - 1; i >= 0; --i) {
       ConvLayer& L = E->conv[i];
-      const void* in_act = i == 0 ? (const void*)x : (const void*)E->conv[i - 1].out.p;
+      const void* in_act = i == 0 ? (const void*)x : (const void*)SE.out[i - 1].p;
       const int64_t rows = (int64_t)B * L.out_h * L.out_w;
       AAE_TRY(launch_bias_grad(dy, rows, L.out_c, h->enc_b[i].g.p, h->bias_scratch.p, s));
       AAE_TRY(conv_wgrad(h, L, in_act, B, dy, h->enc_k[i].g.p, s));
@@ -1173,12 +1176,10 @@ extern "C" int aae_train_step(aae_trainer* h, const float* x_dev, const float* y
       ab.p[t] = pg.p; ab.g[t] = pg.g.p; ab.m[t] = pg.m.p; ab.v[t] = pg.v.p; ab.n[t] = (long long)pg.n;
     }
   if (ab.count) AAE_TRY(launch_adam_multi(ab, lr_t, h->b1, h->b2, h->eps, s));
-  for (auto& L : h->dec->conv) L.wm_dirty = true;   // the merged sub-pixel weights follow the updated taps
   h->ptimer.mark(6, s);
-  // the masters changed in place: every packed copy (inference plans, trainer dgrad operands) is now one step behind
+  // the masters changed in place: every derived copy (merged sub-pixel weights, inference plans, trainer dgrad operands) is now
+  // one step behind
   h->enc->w_version += 1; h->dec->w_version += 1;
-  h->enc->tc_stale = h->enc->tc != nullptr;
-  h->dec->tc_stale = h->dec->tc != nullptr;
   return AAE_OK;
 }
 

@@ -7,6 +7,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <vector>
 
 #include "../../include/aae_b200.h"
 
@@ -57,6 +58,28 @@ struct DeviceGuard {
 };
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// Optional per-stage device timing (cudaEvents on the launching stream), read back by bench.py for the roofline lines.
+struct StageTimer {
+  bool enabled = false;
+  std::vector<cudaEvent_t> ev;   // stage i is bracketed by ev[i], ev[i+1]
+  int used = 0;
+  void mark(cudaStream_t s) {
+    if (!enabled) return;
+    if (used == (int)ev.size()) { cudaEvent_t e; if (cudaEventCreate(&e) != cudaSuccess) return; ev.push_back(e); }
+    cudaEventRecord(ev[used++], s);
+  }
+  void reset() { used = 0; }
+  int read(float* ms, int cap) {
+    int n = 0;
+    if (used >= 2) {
+      cudaEventSynchronize(ev[used - 1]);
+      for (int i = 0; i + 1 < used && n < cap; ++i, ++n) cudaEventElapsedTime(&ms[n], ev[i], ev[i + 1]);
+    }
+    return n;
+  }
+  void release() { for (auto e : ev) cudaEventDestroy(e); ev.clear(); used = 0; }
+};
 
 // ---- generic implicit-GEMM (SIMT fp32) -----------------------------------------------------
 // C[M,N] = sum_k A[m,k] * Bm[k,n] where A is gathered from an NHWC tensor.

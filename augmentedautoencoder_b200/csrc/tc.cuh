@@ -20,14 +20,12 @@ void tc_encoder_destroy(TcEncoder* h);
 // (re)pack the fp32 weights of `layer` (device pointer, reference layout) into the split-fp16 operand layout
 int tc_encoder_pack_weights(TcEncoder* h, int layer, const float* w_dev, cudaStream_t s);
 int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const float* w0, const float* b0, const float* dense_b,
-                       float* z_out, cudaStream_t s);
+                       float* z_out, StageTimer* timer, cudaStream_t s);
 
 int tc_encoder_set_bias(TcEncoder* h, int layer, const float* bias_dev);
 // device word of the run-time range guard (tc_plan.cuh): bit l = activation of layer l overflowed fp16, bit 16 + l = a weight did
 unsigned* tc_encoder_range_flag(TcEncoder* h);
 int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int64_t* count, cudaStream_t s);
-void tc_encoder_enable_timer(TcEncoder* h, bool on);
-int tc_encoder_read_timer(TcEncoder* h, float* ms, int cap);
 
 struct TcDecoder;
 int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out);

@@ -404,7 +404,6 @@ void tc_encoder_destroy(TcEncoder* h) {
   cudaFree(h->dbg);
   cudaFree(h->range_flag);
   tc_conv1_destroy(h->conv1);
-  for (auto e : h->ev) cudaEventDestroy(e);
   delete h;
 }
 
@@ -424,28 +423,11 @@ int tc_encoder_pack_weights(TcEncoder* h, int layer, const float* w_dev, cudaStr
 unsigned* tc_encoder_range_flag(TcEncoder* h) { return h->range_flag; }
 unsigned* tc_decoder_range_flag(TcDecoder* h) { return h->range_flag; }
 
-void tc_encoder_enable_timer(TcEncoder* h, bool on) { h->timer_on = on; }
-
-static void tc_mark(TcEncoder* h, cudaStream_t s) {
-  if (!h->timer_on) return;
-  if (h->ev_used == (int)h->ev.size()) { cudaEvent_t e; if (cudaEventCreate(&e) != cudaSuccess) return; h->ev.push_back(e); }
-  cudaEventRecord(h->ev[h->ev_used++], s);
-}
-
-int tc_encoder_read_timer(TcEncoder* h, float* ms, int cap) {
-  int n = 0;
-  if (h->ev_used >= 2) {
-    cudaEventSynchronize(h->ev[h->ev_used - 1]);
-    for (int i = 0; i + 1 < h->ev_used && n < cap; ++i, ++n) cudaEventElapsedTime(&ms[n], h->ev[i], h->ev[i + 1]);
-  }
-  return n;
-}
-
 int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const float* w0, const float* b0, const float* dense_b,
-                       float* z_out, cudaStream_t s) {
+                       float* z_out, StageTimer* timer, cudaStream_t s) {
   const aae_net_cfg& cfg = h->cfg;
-  h->ev_used = 0;
-  tc_mark(h, s);
+  timer->reset();
+  timer->mark(s);
   if (h->conv1) {
     AAE_TRY(tc_conv1_forward(h->conv1, &cfg, crops, src_u8, B, b0, ACT_SCALE, W_SCALE, h->layers[0].in_hi, h->layers[0].in_lo, h->range_flag, s));
   } else {  // conv1 (Cin = 3, K = 75): fp32 SIMT implicit GEMM, epilogue writes conv2's space-to-depth (hi, lo) input directly
@@ -463,7 +445,7 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
     p.split_hi = h->layers[0].in_hi; p.split_lo = h->layers[0].in_lo; p.split_scale = ACT_SCALE; p.split_s2d = 1;
     AAE_TRY(launch_igemm(p, GATHER_FWD, s));
   }
-  tc_mark(h, s);
+  timer->mark(s);
   for (size_t i = 0; i < h->layers.size(); ++i) {
     TcLayer& T = h->layers[i];
     const bool dense = (i + 1 == h->layers.size());
@@ -506,7 +488,7 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
       AAE_TRY(tc_launch_layer(T, grid, s));
     }
     if (dense) AAE_TRY(launch_splitk_reduce(h->partials, h->dense_splits, (int64_t)B * cfg.latent, cfg.latent, dense_b, ACT_NONE, z_out, s));
-    tc_mark(h, s);
+    timer->mark(s);
   }
   return AAE_OK;
 }

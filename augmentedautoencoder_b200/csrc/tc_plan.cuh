@@ -86,9 +86,6 @@ struct TcEncoder {
   TcConv1* conv1 = nullptr;      // tensor-core first layer (when the geometry allows), else the fp32 SIMT kernel
   float* dbg = nullptr;          // fp32 view of an activation (tests)
   size_t dbg_floats = 0;
-  bool timer_on = false;
-  std::vector<cudaEvent_t> ev;
-  int ev_used = 0;
 };
 
 

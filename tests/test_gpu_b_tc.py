@@ -251,10 +251,28 @@ def test_inference_after_a_training_step_uses_the_updated_weights(sess):
     """Adam updates the fp32 master weights in place; the tensor-core plans keep packed (hi, lo) copies.  In-process inference
     after training (Codebook.update_embedding, decoder.x: ae_embed.py:84-91 run after ae_train.py) must use the step-N
     weights that get_weights() / the checkpoint hold -- i.e. equal a fresh handle loaded from get_weights()."""
+    _check_inference_after_training(sess, 1)
+
+
+def test_inference_after_a_training_step_uses_the_updated_weights_fp32(sess):
+    """The same at the fp32 precision, whose decoder keeps merged sub-pixel weights derived from the masters."""
+    _check_inference_after_training(sess, 0)
+
+
+def _check_inference_after_training(sess, prec):
+    from augmentedautoencoder_b200 import _lib
     from augmentedautoencoder_b200.ae.decoder import Decoder
     from augmentedautoencoder_b200.ae.encoder import Encoder
     from augmentedautoencoder_b200.ae.session import placeholder
-    enc, dec, top, ep, dp = _train_pair(1, 4)
+    enc, dec, top, ep, dp = _train_pair(prec, 4)
+
+    def fresh_pair():                                   # new handles loaded from what get_weights() returns now
+        e = Encoder(placeholder(np.float32, [None, 128, 128, 3]), 128, list(O.NUM_FILTER), 5, list(O.STRIDES), False, max_batch=4, precision=prec)
+        d = Decoder(placeholder(np.float32, [None, 128, 128, 3]), e.z, list(reversed(O.NUM_FILTER)), 5, list(reversed(O.STRIDES)), "L2", 4,
+                    False, False, max_batch=4, precision=prec)
+        e.load_weights(enc.get_weights())
+        d.load_weights(dec.get_weights())
+        return e, d
     xb = torch.from_numpy(np.random.RandomState(11).rand(3, 128, 128, 3).astype(np.float32)).cuda()
     yb = torch.from_numpy(np.random.RandomState(12).rand(3, 128, 128, 3).astype(np.float32)).cuda()
     z_before = enc.encode_device(xb).clone()
@@ -263,19 +281,27 @@ def test_inference_after_a_training_step_uses_the_updated_weights(sess):
     z_after = enc.encode_device(xb).clone()
     rec_after = dec.decode_device(z_after).clone()
     assert float((z_after - z_before).abs().max()) > 1e-4           # the step did move the weights
-    enc2 = Encoder(placeholder(np.float32, [None, 128, 128, 3]), 128, list(O.NUM_FILTER), 5, list(O.STRIDES), False, max_batch=4, precision=1)
-    dec2 = Decoder(placeholder(np.float32, [None, 128, 128, 3]), enc2.z, list(reversed(O.NUM_FILTER)), 5, list(reversed(O.STRIDES)), "L2", 4,
-                   False, False, max_batch=4, precision=1)
-    enc2.load_weights(enc.get_weights())
-    dec2.load_weights(dec.get_weights())
+    enc2, dec2 = fresh_pair()
     z_fresh = enc2.encode_device(xb)
     assert torch.equal(z_after, z_fresh), float((z_after - z_fresh).abs().max())
     assert torch.equal(rec_after, dec2.decode_device(z_fresh))
     # ... and training continues from the same state after the inference calls (the trainer's operands follow too)
     l3 = float(top.step_device(xb, yb, update=True))
-    enc3, dec3, top3, _, _ = _train_pair(1, 4)
+    enc3, dec3, top3, _, _ = _train_pair(prec, 4)
     ref = [float(top3.step_device(xb, yb, update=True)) for _ in range(3)]
     assert abs(l3 - ref[2]) < 1e-6, (l3, ref)
+    # set_weights of a single layer right after an Adam step packs that layer only: every other layer's derived copy is
+    # still one step behind and must be rebuilt by the next forward
+    lib = _lib.lib()
+    for set_weights, mod, layer, name in ((lib.aae_encoder_set_weights, enc, 1, "conv2d_1"), (lib.aae_decoder_set_weights, dec, 2, "conv2d_5")):
+        w = mod.get_weights(short_names=True)
+        k, b = np.ascontiguousarray(w[name + "/kernel"] * 0.5), np.ascontiguousarray(w[name + "/bias"] * 0.5)
+        _lib.check(set_weights(mod.handle(sess.device), layer, _lib.ptr(k), _lib.ptr(b), None), "set_weights")
+    z_set = enc.encode_device(xb).clone()
+    rec_set = dec.decode_device(z_set).clone()
+    enc4, dec4 = fresh_pair()
+    assert torch.equal(z_set, enc4.encode_device(xb))
+    assert torch.equal(rec_set, dec4.decode_device(z_set))
 
 
 def test_range_guard_reports_overflow_instead_of_garbage(sess):
