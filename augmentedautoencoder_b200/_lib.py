@@ -9,6 +9,7 @@ HEADER_PATH = os.path.join(_HERE, "..", "include", "aae_b200.h")
 AAE_MAX_LAYERS = 8
 PREC_FP32_SIMT = 0
 PREC_TC_SPLIT = 1
+PREC_TC_FP16 = 2      # inference only (encoder + codebook match): one fp16 product per K step, see include/aae_b200.h
 
 
 class AaeError(RuntimeError):

@@ -114,6 +114,10 @@ class TrainOp(Tensor):
             enc, dec = self._ae._encoder, self._ae._decoder
             if self._ae._norm_regularize > 0:
                 raise NotImplementedError("NORM_REGULARIZE > 0 is not part of the fused training step")
+            if _lib.PREC_TC_FP16 in (enc.precision, dec.precision):
+                # never switch a precision the caller chose: the fp16 mode has no backward pass
+                raise _lib.AaeError("training needs precision PREC_TC_SPLIT or PREC_FP32_SIMT; PREC_TC_FP16 is inference-only "
+                                    "(create the encoder with another precision for training)")
             h = C.c_void_p()
             with torch.cuda.device(dev):
                 eh, dh = enc.handle(device), dec.handle(device)       # settles automatic precisions

@@ -178,7 +178,8 @@ class Encoder(_DeviceModule):
         self._in_shape = (h, w, c)
         self.max_batch = int(max_batch)
         # default: tensor cores (fp32-grade split-fp16 arithmetic) for inference and training; precision=_lib.PREC_FP32_SIMT
-        # selects the fp32 CUDA-core path (exact fp32 operation order; ~10x slower)
+        # selects the fp32 CUDA-core path (exact fp32 operation order; ~10x slower), precision=_lib.PREC_TC_FP16 the inference-only
+        # single-pass fp16 path (TF32-class rounding; never chosen automatically, and never replaced by another precision)
         self._auto_precision = precision is None
         if precision is None:
             precision = _lib.PREC_TC_SPLIT

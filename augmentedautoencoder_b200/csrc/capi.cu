@@ -166,7 +166,7 @@ int copy_any(void* dst, const void* src, size_t bytes, cudaStream_t s) {
 // Run-time range guard of the tensor-core path's static fp16 scaling (DESIGN.md section 3): kernels set bits in a device word
 // instead of producing inf silently.  `peek` reads the word (the caller has synchronised the stream the work ran on), names
 // the offending layers in the error string, clears it and returns AAE_ERR_UNSUPPORTED; 0 bits -> AAE_OK.
-int range_peek(unsigned* flag_dev, const char* what, int act_layer_base, cudaStream_t s) {
+int range_peek(unsigned* flag_dev, const char* what, int act_layer_base, cudaStream_t s, int precision = AAE_PREC_TC_SPLIT) {
   if (!flag_dev) return AAE_OK;
   unsigned bits = 0;
   AAE_CUDA_OK(cudaMemcpyAsync(&bits, flag_dev, sizeof(bits), cudaMemcpyDeviceToHost, s));
@@ -178,8 +178,9 @@ int range_peek(unsigned* flag_dev, const char* what, int act_layer_base, cudaStr
     if (bits & (1u << l)) snprintf(acts + strlen(acts), sizeof(acts) - strlen(acts), " %d", l + act_layer_base);
     if (bits & (1u << (16 + l))) snprintf(wts + strlen(wts), sizeof(wts) - strlen(wts), " %d", l);
   }
-  set_error("%s: values outside the range of the split-fp16 tensor-core arithmetic (AAE_PREC_TC_SPLIT)%s%s%s%s%s -- use AAE_PREC_FP32_SIMT for "
-            "this model", what, acts[0] ? "; |activation| >= 4094 written by layer(s)" : "", acts, wts[0] ? "; |weight| >= 255.9 in layer(s)" : "", wts,
+  set_error("%s: values outside the range of the %s tensor-core arithmetic (%s)%s%s%s%s%s -- use AAE_PREC_FP32_SIMT for "
+            "this model", what, precision == AAE_PREC_TC_FP16 ? "fp16" : "split-fp16", precision == AAE_PREC_TC_FP16 ? "AAE_PREC_TC_FP16" : "AAE_PREC_TC_SPLIT",
+            acts[0] ? "; |activation| >= 4094 written by layer(s)" : "", acts, wts[0] ? "; |weight| >= 255.9 in layer(s)" : "", wts,
             (bits & (1u << 15)) ? "; |latent| >= 4094 at the decoder input" : "");
   return AAE_ERR_UNSUPPORTED;
 }
@@ -197,7 +198,7 @@ struct aae_encoder {
   int flat;                 // features entering the dense layer
   DevBuf dense_w, dense_b;  // [flat, latent], [latent]
   SimtEncoder* simt = nullptr;  // fp32 CUDA-core workspace (AAE_PREC_FP32_SIMT)
-  TcEncoder* tc = nullptr;  // tensor-core execution plan (AAE_PREC_TC_SPLIT)
+  TcEncoder* tc = nullptr;  // tensor-core execution plan (AAE_PREC_TC_SPLIT or AAE_PREC_TC_FP16)
   int last_batch = 0;
   // the fp32 tensors above are the master copy.  w_version counts its changes (set_weights, Adam); every copy derived from it
   // (the tensor-core plan's packed (hi, lo) fp16 operands, the fp32 decoder's merged sub-pixel weights, the trainer's dgrad
@@ -286,6 +287,8 @@ static int check_cfg(const aae_net_cfg* cfg) {
   AAE_REQUIRE(cfg->in_h > 0 && cfg->in_w > 0 && cfg->in_c > 0 && cfg->latent > 0 && cfg->max_batch > 0, "bad geometry");
   AAE_REQUIRE(cfg->kernel_size >= 1 && cfg->kernel_size <= 7, "kernel_size=%d unsupported", cfg->kernel_size);
   AAE_REQUIRE(cfg->latent % 4 == 0, "latent=%d must be a multiple of 4", cfg->latent);
+  AAE_REQUIRE(cfg->precision == AAE_PREC_FP32_SIMT || cfg->precision == AAE_PREC_TC_SPLIT || cfg->precision == AAE_PREC_TC_FP16,
+              "precision=%d is not an aae_precision (0, 1 or 2)", cfg->precision);
   for (int i = 0; i < cfg->num_layers; ++i) {
     AAE_REQUIRE(cfg->strides[i] == 1 || cfg->strides[i] == 2, "stride[%d]=%d unsupported (1 or 2)", i, cfg->strides[i]);
     AAE_REQUIRE(cfg->filters[i] > 0 && cfg->filters[i] % 4 == 0, "filters[%d]=%d must be a positive multiple of 4", i, cfg->filters[i]);
@@ -338,7 +341,7 @@ extern "C" int aae_encoder_create(int device, const aae_net_cfg* cfg, aae_encode
       cudaMemset(h->dense_b.p, 0, h->dense_b.n * sizeof(float));
     }
   }
-  if (st == AAE_OK) st = cfg->precision == AAE_PREC_TC_SPLIT ? tc_encoder_create(device, cfg, &h->tc) : simt_encoder_create(h);
+  if (st == AAE_OK) st = cfg->precision != AAE_PREC_FP32_SIMT ? tc_encoder_create(device, cfg, &h->tc) : simt_encoder_create(h);
   if (st != AAE_OK) { aae_encoder_destroy(h); return st; }
   *out = h;
   return AAE_OK;
@@ -371,7 +374,7 @@ extern "C" int aae_encoder_set_weights(aae_encoder* h, int layer, const float* k
   if (h->tc) AAE_TRY(tc_encoder_set_bias(h->tc, layer, b.p));
   if (tc_current) h->tc_version = h->w_version;   // this layer is packed again; a plan behind by an Adam step stays behind
   AAE_CUDA_OK(cudaStreamSynchronize(s));  // host source buffers may be freed by the caller on return
-  if (h->tc) AAE_TRY(range_peek(tc_encoder_range_flag(h->tc), "encoder set_weights", 0, s));
+  if (h->tc) AAE_TRY(range_peek(tc_encoder_range_flag(h->tc), "encoder set_weights", 0, s, h->cfg.precision));
   return AAE_OK;
 }
 
@@ -384,7 +387,7 @@ extern "C" int aae_encoder_range_word(aae_encoder* h, const uint32_t** word_dev)
 extern "C" int aae_encoder_range_status(aae_encoder* h, void* stream) {
   AAE_REQUIRE(h != nullptr, "encoder handle is null");
   DeviceGuard g(h->device);
-  return h->tc ? range_peek(tc_encoder_range_flag(h->tc), "encoder", 0, (cudaStream_t)stream) : AAE_OK;
+  return h->tc ? range_peek(tc_encoder_range_flag(h->tc), "encoder", 0, (cudaStream_t)stream, h->cfg.precision) : AAE_OK;
 }
 
 extern "C" int aae_encoder_get_weights(aae_encoder* h, int layer, float* kernel_any, float* bias_any, void* stream) {
@@ -489,6 +492,8 @@ extern "C" int aae_codebook_create(int device, const float* embedding_any, int64
   AAE_REQUIRE(n_rows >= 1 && n_rows + row_offset < (int64_t)INT32_MAX, "n_rows=%lld (+offset) must fit int32", (long long)n_rows);
   AAE_REQUIRE(latent >= 4 && latent % 4 == 0 && latent <= 256, "latent=%d must be a multiple of 4 in [4,256]", latent);
   AAE_REQUIRE(num_cyclo >= 1 && max_batch >= 1 && row_offset >= 0, "bad num_cyclo/max_batch/row_offset");
+  AAE_REQUIRE(precision == AAE_PREC_FP32_SIMT || precision == AAE_PREC_TC_SPLIT || precision == AAE_PREC_TC_FP16,
+              "precision=%d is not an aae_precision (0, 1 or 2)", precision);
   AAE_TRY(check_device(device));
   DeviceGuard g(device);
   aae_codebook* h = new (std::nothrow) aae_codebook();
@@ -504,7 +509,8 @@ extern "C" int aae_codebook_create(int device, const float* embedding_any, int64
     cudaError_t e = cudaMemcpy(h->E.p, embedding_any, (size_t)n_rows * latent * sizeof(float), cudaMemcpyDefault);
     if (e != cudaSuccess) { set_error("codebook upload failed: %s", cudaGetErrorString(e)); st = AAE_ERR_CUDA; }
   }
-  if (st == AAE_OK && precision == AAE_PREC_TC_SPLIT) st = tc_codebook_create(device, h->E.p, n_rows, latent, num_cyclo, max_batch, &h->tc);
+  if (st == AAE_OK && precision != AAE_PREC_FP32_SIMT)
+    st = tc_codebook_create(device, h->E.p, n_rows, latent, num_cyclo, max_batch, precision == AAE_PREC_TC_FP16 ? 1 : 2, &h->tc);
   if (st != AAE_OK) { aae_codebook_destroy(h); return st; }
   *out = h;
   return AAE_OK;
@@ -628,6 +634,10 @@ extern "C" int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decode
   AAE_REQUIRE(out != nullptr, "out is null");
   *out = nullptr;
   AAE_TRY(check_cfg(cfg));
+  if (cfg->precision == AAE_PREC_TC_FP16) {
+    set_error("AAE_PREC_TC_FP16 is inference-only (encoder and codebook match): create the decoder with AAE_PREC_TC_SPLIT or AAE_PREC_FP32_SIMT");
+    return AAE_ERR_UNSUPPORTED;
+  }
   AAE_TRY(check_device(device));
   DeviceGuard g(device);
   aae_decoder* h = new (std::nothrow) aae_decoder();
@@ -813,6 +823,12 @@ extern "C" int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootst
   *out = nullptr;
   AAE_REQUIRE(enc && dec, "null handle");
   AAE_REQUIRE(enc->device == dec->device, "encoder and decoder live on different devices");
+  if ((enc->cfg.precision != AAE_PREC_FP32_SIMT && enc->cfg.precision != AAE_PREC_TC_SPLIT) ||
+      (dec->cfg.precision != AAE_PREC_FP32_SIMT && dec->cfg.precision != AAE_PREC_TC_SPLIT)) {
+    set_error("training needs AAE_PREC_FP32_SIMT or AAE_PREC_TC_SPLIT handles (encoder precision %d, decoder precision %d; AAE_PREC_TC_FP16 is "
+              "inference-only)", enc->cfg.precision, dec->cfg.precision);
+    return AAE_ERR_UNSUPPORTED;
+  }
   AAE_REQUIRE((enc->tc == nullptr) == (dec->tc == nullptr), "encoder and decoder must use the same aae_precision for training");
   AAE_REQUIRE(enc->cfg.max_batch == dec->cfg.max_batch && enc->cfg.in_h == dec->cfg.in_h, "encoder/decoder geometry mismatch");
   DeviceGuard g(enc->device);

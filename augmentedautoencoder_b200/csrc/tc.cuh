@@ -1,4 +1,5 @@
-// Tensor-core (wgmma / TMA) execution plans behind AAE_PREC_TC_SPLIT.  Internal to the library.
+// Tensor-core (wgmma / TMA) execution plans behind AAE_PREC_TC_SPLIT and, for inference, AAE_PREC_TC_FP16 (cfg->precision
+// selects the plan's operand planes).  Internal to the library.
 #pragma once
 #include "common.cuh"
 
@@ -55,7 +56,9 @@ int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s);
 int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, float* db_out, cudaStream_t s);
 int tc_train_unpack_flat(TcTrainPlan* h, int B, float* out, cudaStream_t s);
 
-int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int latent, int num_cyclo, int max_batch, TcCodebook** out);
+// planes: 2 = (hi, lo) codebook and three products per k-step (AAE_PREC_TC_SPLIT), 1 = hi only, one product (AAE_PREC_TC_FP16)
+int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int latent, int num_cyclo, int max_batch, int planes,
+                       TcCodebook** out);
 void tc_codebook_destroy(TcCodebook* h);
 int tc_codebook_max_k();
 int tc_launch_floor_probe(int device, int with_tmem, cudaStream_t s);

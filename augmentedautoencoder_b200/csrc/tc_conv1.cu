@@ -9,6 +9,9 @@
 // zero beyond k = 75) are TMA-loaded once per CTA and stay resident.  Persistent CTAs loop over 128-pixel tiles with a
 // single-stage A buffer: builders (warps 0-3) run a tile ahead of the two MMA + epilogue warpgroups (warps 4-11); warp 12
 // loads the weights.  The epilogue writes conv2's input directly: (hi, lo) fp16, space-to-depth layout.
+//
+// Both kernels have a single-pass instantiation (PLANES = 1, AAE_PREC_TC_FP16): operands and output are the hi terms alone,
+// one product per K step, and only the hi slab is written.
 #include <algorithm>
 
 #include "tc.cuh"
@@ -54,6 +57,7 @@ struct Conv1Smem {
   static constexpr int TOTAL = W_BYTES + C1_STAGES * C1_STAGE + PIX_BYTES + OUT_BYTES + RAW_BYTES + 1024 /*align*/ + 256;
 };
 
+template <int PLANES = 2>
 __global__ void __launch_bounds__(C1_THREADS, 1)
 tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, const Conv1Params p) {
   using S = Conv1Smem;
@@ -75,7 +79,8 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
 
   for (int i = threadIdx.x; i < C1_PIX_ROWS * C1_PIX_LD; i += blockDim.x) pix[i] = 0u;   // left/right padding pixels stay zero
   if (warp == C1_MMA_WARP && lane == 0) {
-    prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_w_lo);
+    prefetch_tmap(&tm_w_hi);
+    if constexpr (PLANES == 2) prefetch_tmap(&tm_w_lo);
     mbar_init(w_full, 1);
     for (int s = 0; s < C1_STAGES; ++s) { mbar_init(&a_full[s], 128); mbar_init(&a_empty[s], 2); }
     fence_barrier_init();
@@ -121,9 +126,13 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
       asm volatile("bar.sync 1, 128;" ::: "memory");
       for (int e = r; e < C1_PIX_ROWS * ROWW; e += 128) {
         const int row = e / ROWW, col = e - row * ROWW;
-        __half h, l;
-        split_f16(reinterpret_cast<const float*>(rawbuf)[e] * p.in_scale, h, l);
-        dst[row * C1_PIX_LD + p.pad_l * CIN + col] = (uint32_t)__half_as_ushort(h) | ((uint32_t)__half_as_ushort(l) << 16);
+        if constexpr (PLANES == 1) {                       // hi only: the upper half of the word stays zero
+          dst[row * C1_PIX_LD + p.pad_l * CIN + col] = (uint32_t)__half_as_ushort(__float2half_rn(reinterpret_cast<const float*>(rawbuf)[e] * p.in_scale));
+        } else {
+          __half h, l;
+          split_f16(reinterpret_cast<const float*>(rawbuf)[e] * p.in_scale, h, l);
+          dst[row * C1_PIX_LD + p.pad_l * CIN + col] = (uint32_t)__half_as_ushort(h) | ((uint32_t)__half_as_ushort(l) << 16);
+        }
       }
     };
     if (my_tiles > 0) {
@@ -156,7 +165,7 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
         const int atom = ci >> 3, chunk = ci & 7;
         const uint32_t off = (uint32_t)(atom * C1_ATOM + r * 128 + ((chunk ^ (r & 7)) << 4));
         *reinterpret_cast<uint4*>(st + off) = hv;
-        *reinterpret_cast<uint4*>(st + 2 * C1_ATOM + off) = lv;
+        if constexpr (PLANES == 2) *reinterpret_cast<uint4*>(st + 2 * C1_ATOM + off) = lv;
       }
       fence_proxy_async_smem();
       mbar_arrive(&a_full[s]);
@@ -194,12 +203,16 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
       for (int k = 0; k < C1_KPAD / 16; ++k) {
         const int atom = k >> 2, kk = k & 3;
         const uint64_t a_hi = desc_advance_k(make_sw128_kmajor_desc(ast + atom * C1_ATOM), kk);
-        const uint64_t a_lo = desc_advance_k(make_sw128_kmajor_desc(ast + (2 + atom) * C1_ATOM), kk);
         const uint64_t w_hi = desc_advance_k(make_sw128_kmajor_desc(wst + atom * N * 128), kk);
-        const uint64_t w_lo = desc_advance_k(make_sw128_kmajor_desc(wst + (2 + atom) * N * 128), kk);
-        Wgmma<N>::template ss<0, 0>(acc, a_lo, w_hi, k > 0 ? 1u : 0u);
-        Wgmma<N>::template ss<0, 0>(acc, a_hi, w_lo, 1u);
-        Wgmma<N>::template ss<0, 0>(acc, a_hi, w_hi, 1u);
+        if constexpr (PLANES == 1) {
+          Wgmma<N>::template ss<0, 0>(acc, a_hi, w_hi, k > 0 ? 1u : 0u);
+        } else {
+          const uint64_t a_lo = desc_advance_k(make_sw128_kmajor_desc(ast + (2 + atom) * C1_ATOM), kk);
+          const uint64_t w_lo = desc_advance_k(make_sw128_kmajor_desc(wst + (2 + atom) * N * 128), kk);
+          Wgmma<N>::template ss<0, 0>(acc, a_lo, w_hi, k > 0 ? 1u : 0u);
+          Wgmma<N>::template ss<0, 0>(acc, a_hi, w_lo, 1u);
+          Wgmma<N>::template ss<0, 0>(acc, a_hi, w_hi, 1u);
+        }
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -218,10 +231,15 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
           const float a = fmaxf(acc[4 * j + 2 * h2] * p.unscale + bias_s[c], 0.f) * p.out_scale;
           const float bb = fmaxf(acc[4 * j + 2 * h2 + 1] * p.unscale + bias_s[c + 1], 0.f) * p.out_scale;
           amax = fmaxf(amax, fmaxf(a, bb));
-          uint32_t hi, lo;
-          split_f16x2(a, bb, hi, lo);
-          *reinterpret_cast<uint32_t*>(my_hi[h2] + c * 2) = hi;
-          *reinterpret_cast<uint32_t*>(my_hi[h2] + 32 * C1_OUT_LD + c * 2) = lo;
+          if constexpr (PLANES == 1) {
+            const __half2 hh = __floats2half2_rn(a, bb);
+            *reinterpret_cast<uint32_t*>(my_hi[h2] + c * 2) = *reinterpret_cast<const uint32_t*>(&hh);
+          } else {
+            uint32_t hi, lo;
+            split_f16x2(a, bb, hi, lo);
+            *reinterpret_cast<uint32_t*>(my_hi[h2] + c * 2) = hi;
+            *reinterpret_cast<uint32_t*>(my_hi[h2] + 32 * C1_OUT_LD + c * 2) = lo;
+          }
         }
       }
       if (p.range_flag != nullptr && !(amax < 65520.f)) atomicOr(p.range_flag, 1u);
@@ -231,7 +249,8 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
         const long long slab = ((long long)(b * (p.OH >> 1) + (oh0 >> 1)) * (p.OW >> 1)) * (4LL * N);   // elements
         if (lane < 32 / G) {
           bulk_store_1d(p.out_hi + slab + (long long)lane * G * 4 * N, out_smem + lane * grp_ld, (uint32_t)(G * 8 * N));
-          bulk_store_1d(p.out_lo + slab + (long long)lane * G * 4 * N, out_smem + 32 * C1_OUT_LD + lane * grp_ld, (uint32_t)(G * 8 * N));
+          if constexpr (PLANES == 2)
+            bulk_store_1d(p.out_lo + slab + (long long)lane * G * 4 * N, out_smem + 32 * C1_OUT_LD + lane * grp_ld, (uint32_t)(G * 8 * N));
         }
         bulk_commit_group();
       }
@@ -240,11 +259,13 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
   } else {
     // ===================== weight TMA (last warp) =====================
     if (lane == 0) {
-      mbar_arrive_expect_tx(w_full, S::W_BYTES);
+      mbar_arrive_expect_tx(w_full, PLANES * S::W_BYTES / 2);
       tma_load_2d(w_smem, &tm_w_hi, w_full, 0, 0);
       tma_load_2d(w_smem + N * 128, &tm_w_hi, w_full, 64, 0);
-      tma_load_2d(w_smem + 2 * N * 128, &tm_w_lo, w_full, 0, 0);
-      tma_load_2d(w_smem + 3 * N * 128, &tm_w_lo, w_full, 64, 0);
+      if constexpr (PLANES == 2) {
+        tma_load_2d(w_smem + 2 * N * 128, &tm_w_lo, w_full, 0, 0);
+        tma_load_2d(w_smem + 3 * N * 128, &tm_w_lo, w_full, 64, 0);
+      }
     }
   }
 }
@@ -284,6 +305,7 @@ __device__ __forceinline__ void bytes_to_half4(uint32_t x, uint32_t& lo2, uint32
 constexpr int U8_EPI_WARPS = 8;
 constexpr int U8_THREADS = 32 * (4 + U8_EPI_WARPS + 1);
 
+template <int PLANES = 2>
 __global__ void __launch_bounds__(U8_THREADS, 1)
 tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo,
                    const __grid_constant__ CUtensorMap tm_out_hi, const __grid_constant__ CUtensorMap tm_out_lo, const Conv1Params p) {
@@ -304,7 +326,11 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
   if (threadIdx.x < N) bias_s[threadIdx.x] = p.bias[threadIdx.x] * p.out_scale;     // relu(x) * s == relu(x * s) for s > 0
   for (int i = threadIdx.x; i < 2 * U8_PIX_BUF / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(pix)[i] = 0u;   // lead-in / tail stay zero
   if (warp == mma_warp && lane == 0) {
-    prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_w_lo); prefetch_tmap(&tm_out_hi); prefetch_tmap(&tm_out_lo);
+    if constexpr (PLANES == 1) {
+      prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_out_hi);
+    } else {
+      prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_w_lo); prefetch_tmap(&tm_out_hi); prefetch_tmap(&tm_out_lo);
+    }
     mbar_init(w_full, 1);
     for (int s = 0; s < U8_A_STAGES; ++s) { mbar_init(&a_full[s], 128); mbar_init(&a_empty[s], 2); }
     fence_barrier_init();
@@ -402,9 +428,13 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
         const int atom = k >> 2, kk = k & 3;
         const uint64_t a = desc_advance_k(make_sw128_kmajor_desc(ast + atom * C1_ATOM), kk);
         const uint64_t w_hi = desc_advance_k(make_sw128_kmajor_desc(wst + atom * C1_ATOM), kk);
-        const uint64_t w_lo = desc_advance_k(make_sw128_kmajor_desc(wst + (2 + atom) * C1_ATOM), kk);
-        Wgmma<N>::template ss<0, 0>(acc, a, w_lo, k > 0 ? 1u : 0u);
-        Wgmma<N>::template ss<0, 0>(acc, a, w_hi, 1u);
+        if constexpr (PLANES == 1) {
+          Wgmma<N>::template ss<0, 0>(acc, a, w_hi, k > 0 ? 1u : 0u);
+        } else {
+          const uint64_t w_lo = desc_advance_k(make_sw128_kmajor_desc(wst + (2 + atom) * C1_ATOM), kk);
+          Wgmma<N>::template ss<0, 0>(acc, a, w_lo, k > 0 ? 1u : 0u);
+          Wgmma<N>::template ss<0, 0>(acc, a, w_hi, 1u);
+        }
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -425,11 +455,16 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
           const float a = fmaxf(fmaf(acc[4 * j + 2 * h2], us, bias_s[c]), 0.f);
           const float bb = fmaxf(fmaf(acc[4 * j + 2 * h2 + 1], us, bias_s[c + 1]), 0.f);
           amax = fmaxf(amax, fmaxf(a, bb));
-          uint32_t hi, lo;
-          split_f16x2(a, bb, hi, lo);
           const int off = rr * 64 + (((j & 3) ^ ((rr >> 1) & 3)) << 4) + 4 * (lane & 3);
-          *reinterpret_cast<uint32_t*>(sb + off) = hi;
-          *reinterpret_cast<uint32_t*>(sb + 1024 + off) = lo;
+          if constexpr (PLANES == 1) {
+            const __half2 hh = __floats2half2_rn(a, bb);
+            *reinterpret_cast<uint32_t*>(sb + off) = *reinterpret_cast<const uint32_t*>(&hh);
+          } else {
+            uint32_t hi, lo;
+            split_f16x2(a, bb, hi, lo);
+            *reinterpret_cast<uint32_t*>(sb + off) = hi;
+            *reinterpret_cast<uint32_t*>(sb + 1024 + off) = lo;
+          }
         }
       }
       if (p.range_flag != nullptr && !(amax < 65520.f)) atomicOr(p.range_flag, 1u);
@@ -440,7 +475,7 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
 #pragma unroll
         for (int cc = 0; cc < N / 32; ++cc) {
           tma_store_2d(&tm_out_hi, wbuf + cc * 2048, cc * 32, slot0);
-          tma_store_2d(&tm_out_lo, wbuf + cc * 2048 + 1024, cc * 32, slot0);
+          if constexpr (PLANES == 2) tma_store_2d(&tm_out_lo, wbuf + cc * 2048 + 1024, cc * 32, slot0);
         }
         bulk_commit_group();
       }
@@ -449,17 +484,21 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
   } else {
     // ===================== weight TMA (last warp) =====================
     if (lane == 0) {
-      mbar_arrive_expect_tx(w_full, U8_W_BYTES);
+      mbar_arrive_expect_tx(w_full, PLANES * U8_W_BYTES / 2);
       tma_load_2d(w_smem, &tm_w_hi, w_full, 0, 0);
       tma_load_2d(w_smem + C1_ATOM, &tm_w_hi, w_full, 64, 0);
-      tma_load_2d(w_smem + 2 * C1_ATOM, &tm_w_lo, w_full, 0, 0);
-      tma_load_2d(w_smem + 3 * C1_ATOM, &tm_w_lo, w_full, 64, 0);
+      if constexpr (PLANES == 2) {
+        tma_load_2d(w_smem + 2 * C1_ATOM, &tm_w_lo, w_full, 0, 0);
+        tma_load_2d(w_smem + 3 * C1_ATOM, &tm_w_lo, w_full, 64, 0);
+      }
     }
   }
 }
 
 // W fp32 [75][N] (HWIO flattened) -> (hi, lo) fp16 [N][128] in the 5 x 16 slot order of the uint8 kernel: slot kh*16 + 1 + (kw*3 + c)
-// holds scale * W[kh][kw][c][n] (scale = 2^16 / 255: the x/255 of codebook.py:58-59 lives here), every other slot is zero
+// holds scale * W[kh][kw][c][n] (scale = 2^16 / 255: the x/255 of codebook.py:58-59 lives here), every other slot is zero.
+// PLANES = 1 writes hi only.
+template <int PLANES = 2>
 __global__ void pack_conv1_u8_weights_kernel(const float* __restrict__ w, int N, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
                                              unsigned* __restrict__ range_flag, unsigned range_bit) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -471,10 +510,11 @@ __global__ void pack_conv1_u8_weights_kernel(const float* __restrict__ w, int N,
   __half h, l;
   split_f16(v, h, l);
   hi[i] = h;
-  lo[i] = l;
+  if constexpr (PLANES == 2) lo[i] = l;
 }
 
-// W fp32 [75][N] (HWIO flattened) -> (hi, lo) fp16 [N][128] K-major, scaled, zero for k >= K
+// W fp32 [75][N] (HWIO flattened) -> (hi, lo) fp16 [N][128] K-major, scaled, zero for k >= K; PLANES = 1 writes hi only
+template <int PLANES = 2>
 __global__ void pack_conv1_weights_kernel(const float* __restrict__ w, int K, int N, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
                                           unsigned* __restrict__ range_flag, unsigned range_bit) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -485,13 +525,14 @@ __global__ void pack_conv1_weights_kernel(const float* __restrict__ w, int K, in
   __half h, l;
   split_f16(v, h, l);
   hi[i] = h;
-  lo[i] = l;
+  if constexpr (PLANES == 2) lo[i] = l;
 }
 
 }  // namespace
 
 struct TcConv1 {
   int N, sm_count;
+  int planes;                     // 2: (hi, lo) operands and output (AAE_PREC_TC_SPLIT); 1: hi only (AAE_PREC_TC_FP16), no lo buffers
   __half *w_hi = nullptr, *w_lo = nullptr;
   CUtensorMap tm_hi, tm_lo;
   // uint8 kernel: weights with 1/255 folded in, 5 x 16 slot order; output tensor maps over conv2's (hi, lo) input
@@ -511,24 +552,27 @@ int tc_conv1_create(int device, const aae_net_cfg* cfg, TcConv1** out) {
   *out = nullptr;
   TcConv1* h = new TcConv1();
   h->N = cfg->filters[0];
+  h->planes = cfg->precision == AAE_PREC_TC_FP16 ? 1 : 2;
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
   h->sm_count = prop.multiProcessorCount;
   cudaError_t e = cudaMalloc(&h->w_hi, (size_t)h->N * 128 * sizeof(__half));
-  if (e == cudaSuccess) e = cudaMalloc(&h->w_lo, (size_t)h->N * 128 * sizeof(__half));
+  if (e == cudaSuccess && h->planes == 2) e = cudaMalloc(&h->w_lo, (size_t)h->N * 128 * sizeof(__half));
   if (e != cudaSuccess) { set_error("tc conv1 alloc failed: %s", cudaGetErrorString(e)); tc_conv1_destroy(h); return AAE_ERR_OOM; }
   const uint64_t dims[2] = {128, (uint64_t)h->N};
   const uint64_t strides[1] = {256};
   const uint32_t box[2] = {64, (uint32_t)h->N};
+  const bool two = h->planes == 2;
   int st = make_tmap_f16(&h->tm_hi, h->w_hi, 2, dims, strides, box);
-  if (st == AAE_OK) st = make_tmap_f16(&h->tm_lo, h->w_lo, 2, dims, strides, box);
+  if (st == AAE_OK && two) st = make_tmap_f16(&h->tm_lo, h->w_lo, 2, dims, strides, box);
   if (st == AAE_OK) {
     e = cudaMalloc(&h->w8_hi, (size_t)h->N * 128 * sizeof(__half));
-    if (e == cudaSuccess) e = cudaMalloc(&h->w8_lo, (size_t)h->N * 128 * sizeof(__half));
+    if (e == cudaSuccess && two) e = cudaMalloc(&h->w8_lo, (size_t)h->N * 128 * sizeof(__half));
     if (e != cudaSuccess) { set_error("tc conv1 alloc failed: %s", cudaGetErrorString(e)); tc_conv1_destroy(h); return AAE_ERR_OOM; }
     st = make_tmap_f16(&h->tm8_hi, h->w8_hi, 2, dims, strides, box);
-    if (st == AAE_OK) st = make_tmap_f16(&h->tm8_lo, h->w8_lo, 2, dims, strides, box);
-    if (st == AAE_OK) st = cudaFuncSetAttribute(tc_conv1_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, U8_SMEM_TOTAL) == cudaSuccess ? AAE_OK : AAE_ERR_CUDA;
+    if (st == AAE_OK && two) st = make_tmap_f16(&h->tm8_lo, h->w8_lo, 2, dims, strides, box);
+    const void* u8_kernel = two ? (const void*)tc_conv1_u8_kernel<2> : (const void*)tc_conv1_u8_kernel<1>;
+    if (st == AAE_OK) st = cudaFuncSetAttribute(u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, U8_SMEM_TOTAL) == cudaSuccess ? AAE_OK : AAE_ERR_CUDA;
   }
   if (st != AAE_OK) { tc_conv1_destroy(h); return st; }
   *out = h;
@@ -542,11 +586,16 @@ void tc_conv1_destroy(TcConv1* h) {
 }
 
 int tc_conv1_pack(TcConv1* h, const float* w_dev, int K, float w_scale, unsigned* range_flag, unsigned range_bit, cudaStream_t s) {
-  pack_conv1_weights_kernel<<<(unsigned)ceil_div(h->N * 128, 256), 256, 0, s>>>(w_dev, K, h->N, w_scale, h->w_hi, h->w_lo, range_flag, range_bit);
+  const unsigned grid = (unsigned)ceil_div(h->N * 128, 256);
+  if (h->planes == 1) pack_conv1_weights_kernel<1><<<grid, 256, 0, s>>>(w_dev, K, h->N, w_scale, h->w_hi, nullptr, range_flag, range_bit);
+  else pack_conv1_weights_kernel<<<grid, 256, 0, s>>>(w_dev, K, h->N, w_scale, h->w_hi, h->w_lo, range_flag, range_bit);
   AAE_LAUNCH_OK();
   AAE_REQUIRE(K == 75, "tc conv1 (uint8 kernel): K = %d, expected 75", K);
-  pack_conv1_u8_weights_kernel<<<(unsigned)ceil_div(h->N * 128, 256), 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8_hi, h->w8_lo, range_flag,
-                                                                                  range_bit);
+  if (h->planes == 1)
+    pack_conv1_u8_weights_kernel<1><<<grid, 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8_hi, nullptr, range_flag, range_bit);
+  else
+    pack_conv1_u8_weights_kernel<<<(unsigned)ceil_div(h->N * 128, 256), 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8_hi, h->w8_lo, range_flag,
+                                                                                    range_bit);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -576,13 +625,17 @@ int tc_conv1_forward(TcConv1* h, const aae_net_cfg* cfg, const void* crops, int 
       const uint64_t strides[1] = {256};
       const uint32_t box32[2] = {32, 16};                   // one warp's 16 slots x 32 channels, 64-byte swizzle
       AAE_TRY(make_tmap_f16(&h->tm_out32_hi, out_hi, 2, dims, strides, box32, 64));
-      AAE_TRY(make_tmap_f16(&h->tm_out32_lo, out_lo, 2, dims, strides, box32, 64));
+      if (h->planes == 2) AAE_TRY(make_tmap_f16(&h->tm_out32_lo, out_lo, 2, dims, strides, box32, 64));
       h->bound_hi = out_hi; h->bound_lo = out_lo; h->slots = slots;
     }
     p.unscale = 1.f / (w_scale * 256.f);              // accumulators hold sum u8 * (w * w_scale * 256 / 255)
-    tc_conv1_u8_kernel<<<grid, U8_THREADS, U8_SMEM_TOTAL, s>>>(h->tm8_hi, h->tm8_lo, h->tm_out32_hi, h->tm_out32_lo, p);
+    if (h->planes == 1) tc_conv1_u8_kernel<1><<<grid, U8_THREADS, U8_SMEM_TOTAL, s>>>(h->tm8_hi, h->tm8_hi, h->tm_out32_hi, h->tm_out32_hi, p);
+    else tc_conv1_u8_kernel<<<grid, U8_THREADS, U8_SMEM_TOTAL, s>>>(h->tm8_hi, h->tm8_lo, h->tm_out32_hi, h->tm_out32_lo, p);
+  } else if (h->planes == 1) {
+    AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Conv1Smem::TOTAL));
+    tc_conv1_kernel<1><<<grid, C1_THREADS, Conv1Smem::TOTAL, s>>>(h->tm_hi, h->tm_hi, p);
   } else {
-    AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Conv1Smem::TOTAL));
+    AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Conv1Smem::TOTAL));
     tc_conv1_kernel<<<grid, C1_THREADS, Conv1Smem::TOTAL, s>>>(h->tm_hi, h->tm_lo, p);
   }
   AAE_LAUNCH_OK();

@@ -8,6 +8,8 @@
 // fp32-grade arithmetic on fp16 tensor cores: every fp32 operand x is stored as two fp16 terms, hi = rn(x) and
 // lo = rn(x - hi) (22 significant bits; operands pre-scaled by a power of two so lo stays a normal fp16), and each
 // K chunk issues three MMAs: hi*hi into the main fp32 accumulator, hi*lo + lo*hi into a second one.
+// The single-pass instantiation (PLANES = 1, AAE_PREC_TC_FP16, inference only) keeps the hi terms alone: it loads the hi
+// boxes only, issues hi*hi into one accumulator and writes the hi plane of the next layer's input.
 //
 // Data movement: activations live in HBM in a space-to-depth layout  Xs[b, h/2, w/2, (h%2, w%2, c)]  written by the
 // producing layer's epilogue, so that tap (kh, kw) of the stride-2 / asymmetric-SAME(1,2) convolution is a plain
@@ -57,12 +59,12 @@ int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* 
 }
 
 // ------------------------------------------------------------------------------------------------- kernel
-template <int N_TILE, int STAGES>
+template <int N_TILE, int STAGES, int PLANES = 2>
 struct TcSmem {
   static constexpr int A_BYTES = 128 * TC_KCH * 2;     // 128 rows x TC_KCH fp16
   static constexpr int W_BYTES = N_TILE * TC_KCH * 2;
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
-  static constexpr int ACC_LD = 2 * N_TILE + 4;        // fp32 accumulator image [128][ACC_LD] (main | cross), padded
+  static constexpr int STAGE_BYTES = PLANES * A_BYTES + PLANES * W_BYTES;
+  static constexpr int ACC_LD = PLANES * N_TILE + 4;   // fp32 accumulator image [128][ACC_LD] (main | cross), padded
   static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
   static constexpr int BODY = STAGES * STAGE_BYTES > ACC_BYTES ? STAGES * STAGE_BYTES : ACC_BYTES;
   static constexpr int TOTAL = BODY + 1024 /*align slack*/ + 256 /*barriers*/;
@@ -71,11 +73,12 @@ struct TcSmem {
 // Warp roles (384 threads): warp 0 TMA producer (warps 1-3 idle), warpgroups 1 and 2 (warps 4-11) issue the wgmma for pixel rows
 // [0,64) and [64,128) of the tile and then run the epilogue, two warps per 32-row quadrant.
 // Grid: x = N tile, y = M tile, z = K split (see tc_launch_layer).
-template <int N_TILE, int STAGES>
+// PLANES = 2: (hi, lo) operands, three products per K step; PLANES = 1: hi operands only (tm_a_lo / tm_w_lo unused), one product.
+template <int N_TILE, int STAGES, int PLANES = 2>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, const TcGemmParams p) {
-  using S = TcSmem<N_TILE, STAGES>;
+  using S = TcSmem<N_TILE, STAGES, PLANES>;
   constexpr int R = N_TILE / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -91,7 +94,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
   const int it_end = min(total_iters, it_begin + p.iters_per_split);
 
   if (threadIdx.x == 0) {
-    prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_w_lo);
+    if constexpr (PLANES == 1) {
+      prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_w_hi);
+    } else {
+      prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_w_lo);
+    }
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
@@ -112,12 +119,59 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
         mbar_arrive_expect_tx(&full_bar[s], S::STAGE_BYTES);
         const int c0 = p.tap_ch[tap] + cc * TC_KCH;
         const int x = ow0 + p.tap_dj[tap], y = oh0 + p.tap_di[tap];
-        tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
-        tma_load_4d(st + S::A_BYTES, &tm_a_lo, &full_bar[s], c0, x, y, b0);
         const int kcol = it * TC_KCH;
-        tma_load_2d(st + 2 * S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, n0);
-        tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tm_w_lo, &full_bar[s], kcol, n0);
+        if constexpr (PLANES == 1) {                   // stage = [A_hi | W_hi]
+          tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
+          tma_load_2d(st + S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, n0);
+        } else {
+          tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
+          tma_load_4d(st + S::A_BYTES, &tm_a_lo, &full_bar[s], c0, x, y, b0);
+          tma_load_2d(st + 2 * S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, n0);
+          tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tm_w_lo, &full_bar[s], kcol, n0);
+        }
       }
+    }
+  } else if (warp >= 4 && PLANES == 1) {
+    // ===================== wgmma consumers + epilogue, single pass =====================
+    const int wg = (warp - 4) >> 2;
+    float acc[R];
+#pragma unroll
+    for (int j = 0; j < R; ++j) acc[j] = 0.f;
+    for (int it = it_begin, i = 0; it < it_end; ++it, ++i) {
+      const int s = i % STAGES;
+      mbar_wait(&full_bar[s], (uint32_t)(i / STAGES) & 1u);
+      const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
+      const uint64_t a_hi = make_sw128_kmajor_desc(st + (uint32_t)(wg * 64 * TC_KCH * 2));
+      const uint64_t w_hi = make_sw128_kmajor_desc(st + S::A_BYTES);
+      wgmma_fence_regs(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_KCH / 16; ++k)
+        Wgmma<N_TILE>::template ss<0, 0>(acc, desc_advance_k(a_hi, k), desc_advance_k(w_hi, k), (i > 0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();                                // the previous stage's MMAs have read their operands: free it
+      wgmma_fence_regs(acc);
+      if (i > 0 && (warp & 3) == 0 && lane == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    named_bar_sync(1, 256);
+    float* img = reinterpret_cast<float*>(smem);
+    tc_park_acc(img, S::ACC_LD, wg, warp, lane, acc);
+    named_bar_sync(1, 256);
+    const int q = warp & 3, half = (warp - 4) >> 2;
+    const TcRow row = tc_decode_row(p, m0 + q * 32 + lane);
+    const bool has_work = it_end > it_begin;
+#pragma unroll 1
+    for (int c = half; c < N_TILE / 32; c += 2) {
+      const int n = n0 + c * 32;
+      if (!row.valid || n >= p.N) continue;
+      uint32_t v[32];
+      tc_acc_ld32(img, S::ACC_LD, q * 32 + lane, c * 32, v);
+      float f[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) f[j] = has_work ? __uint_as_float(v[j]) * p.unscale : 0.f;
+      tc_store_chunk<1>(p, row, n, f, (int)blockIdx.z);
     }
   } else if (warp >= 4) {
     // ===================== wgmma consumers =====================
@@ -179,7 +233,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
 // ------------------------------------------------------------------------------------------------- packing kernels
 namespace {
 
-// W fp32 [taps][Cin][Cout] (HWIO flattened) -> Wp_{hi,lo} fp16 [Cout][taps*Cin], value scaled by `scale`
+// W fp32 [taps][Cin][Cout] (HWIO flattened) -> Wp_{hi,lo} fp16 [Cout][taps*Cin], value scaled by `scale`; PLANES = 1 writes hi only
+template <int PLANES = 2>
 __global__ void pack_weights_kernel(const float* __restrict__ w, int taps, int cin, int cout, float scale, __half* __restrict__ hi,
                                     __half* __restrict__ lo, unsigned* __restrict__ range_flag, unsigned range_bit) {
   __shared__ float tile[32][33];
@@ -199,12 +254,14 @@ __global__ void pack_weights_kernel(const float* __restrict__ w, int taps, int c
       split_f16(v, h, l);
       const long long o = (long long)co * taps * cin + (long long)tap * cin + ci;
       hi[o] = h;
-      lo[o] = l;
+      if constexpr (PLANES == 2) lo[o] = l;
     }
   }
 }
 
-// (hi, lo) fp16 activations -> fp32 NHWC (undoing the space-to-depth layout and the scale); debug / test visibility only
+// (hi, lo) fp16 activations -> fp32 NHWC (undoing the space-to-depth layout and the scale); debug / test visibility only.
+// PLANES = 1: the hi plane alone (lo is not read).
+template <int PLANES = 2>
 __global__ void unpack_act_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, int B, int H, int W, int C, int s2d,
                                   float inv_scale, float* __restrict__ out) {
   const long long total = (long long)B * H * W * C;
@@ -216,7 +273,8 @@ __global__ void unpack_act_kernel(const __half* __restrict__ hi, const __half* _
     const int b = (int)(r / H);
     long long src = i;
     if (s2d) src = ((long long)(b * (H >> 1) + (h >> 1)) * (W >> 1) + (w >> 1)) * (4LL * C) + (((h & 1) << 1) | (w & 1)) * C + c;
-    out[i] = (__half2float(hi[src]) + __half2float(lo[src])) * inv_scale;
+    if constexpr (PLANES == 1) out[i] = __half2float(hi[src]) * inv_scale;
+    else out[i] = (__half2float(hi[src]) + __half2float(lo[src])) * inv_scale;
   }
 }
 
@@ -227,7 +285,9 @@ namespace {
 
 // Split-K forward of a conv layer at small batch: the GEMM leaves fp32 partial sums [splits][M][N] (OUT_F32); this kernel folds
 // them in a fixed order and applies the layer's real epilogue -- bias, ReLU, range guard, (hi, lo) split, store in the next
-// layer's layout (tc_store_chunk's OUT_S2D_SPLIT / OUT_PLAIN_SPLIT branch).  One thread per (row, 8 columns).
+// layer's layout (tc_store_chunk's OUT_S2D_SPLIT / OUT_PLAIN_SPLIT branch).  One thread per (row, 8 columns).  PLANES = 1
+// stores the hi plane only, rounded straight from fp32.
+template <int PLANES = 2>
 __global__ void __launch_bounds__(256) splitk_forward_finish_kernel(const float* __restrict__ partials, int splits, const TcGemmParams p) {
   const long long groups = (long long)p.M * (p.N >> 3);
   for (long long gi = (long long)blockIdx.x * blockDim.x + threadIdx.x; gi < groups; gi += (long long)gridDim.x * blockDim.x) {
@@ -248,11 +308,21 @@ __global__ void __launch_bounds__(256) splitk_forward_finish_kernel(const float*
     }
     if (p.range_flag != nullptr && !(amax * p.out_scale < TC_F16_OVERFLOW)) atomicOr(p.range_flag, p.range_bit);
     const TcRow r = tc_decode_row(p, m);
-    uint32_t hi[4], lo[4];
+    if constexpr (PLANES == 1) {
+      uint32_t hi[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) split_f16x2(f[2 * j], f[2 * j + 1], hi[j], lo[j]);
-    *reinterpret_cast<uint4*>(p.out_hi + r.row_off + n) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    *reinterpret_cast<uint4*>(p.out_lo + r.row_off + n) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+      for (int j = 0; j < 4; ++j) {
+        const __half2 h = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
+        hi[j] = *reinterpret_cast<const uint32_t*>(&h);
+      }
+      *reinterpret_cast<uint4*>(p.out_hi + r.row_off + n) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+    } else {
+      uint32_t hi[4], lo[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) split_f16x2(f[2 * j], f[2 * j + 1], hi[j], lo[j]);
+      *reinterpret_cast<uint4*>(p.out_hi + r.row_off + n) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+      *reinterpret_cast<uint4*>(p.out_lo + r.row_off + n) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+    }
   }
 }
 
@@ -272,10 +342,24 @@ int tc_dev_alloc(void** p, size_t bytes) {
 // tiles = (m_tiles, n_tiles, splits).  The kernel runs the N tiles on grid.x, so the N tiles of an M tile are adjacent in launch
 // order and read the activation tile (and its 5 x 5 tap re-reads) while it is in L2; M first would put all resident CTAs on one
 // weight column and stream every activation tile from HBM once per N tile.
-int tc_launch_layer(const TcLayer& T, dim3 tiles, cudaStream_t s) {
-  using S = TcSmem<TC_N_TILE, 3>;
-  auto kern = tc_gemm_kernel<TC_N_TILE, 3>;
+// Stage counts: the split kernel's 3 stages of 64 KB and the single-pass kernel's 6 stages of 32 KB are the same 192 KB ring,
+// so both keep the same bytes in flight and the same shared-memory footprint (and carveout); the single pass gets twice the
+// K-iterations of look-ahead.
+constexpr int TC_STAGES_SPLIT = 3, TC_STAGES_FP16 = 6;
+static_assert(TcSmem<TC_N_TILE, TC_STAGES_FP16, 1>::TOTAL == TcSmem<TC_N_TILE, TC_STAGES_SPLIT>::TOTAL, "same footprint");
+
+int tc_launch_layer(const TcLayer& T, dim3 tiles, cudaStream_t s, int planes) {
   AAE_REQUIRE(tiles.x <= 65535u, "tc_gemm: %u row tiles exceed the grid's y limit", tiles.x);
+  if (planes == 1) {
+    using S1 = TcSmem<TC_N_TILE, TC_STAGES_FP16, 1>;
+    auto kern1 = tc_gemm_kernel<TC_N_TILE, TC_STAGES_FP16, 1>;
+    AAE_CUDA_OK(cudaFuncSetAttribute(kern1, cudaFuncAttributeMaxDynamicSharedMemorySize, S1::TOTAL));
+    kern1<<<dim3(tiles.y, tiles.x, tiles.z), TC_THREADS, S1::TOTAL, s>>>(T.tm_a_hi, T.tm_a_hi, T.tm_w_hi, T.tm_w_hi, T.gp);
+    AAE_LAUNCH_OK();
+    return AAE_OK;
+  }
+  using S = TcSmem<TC_N_TILE, TC_STAGES_SPLIT>;
+  auto kern = tc_gemm_kernel<TC_N_TILE, TC_STAGES_SPLIT>;
   AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
   kern<<<dim3(tiles.y, tiles.x, tiles.z), TC_THREADS, S::TOTAL, s>>>(T.tm_a_hi, T.tm_a_lo, T.tm_w_hi, T.tm_w_lo, T.gp);
   AAE_LAUNCH_OK();
@@ -287,9 +371,15 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
   const int L = cfg->num_layers;
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   AAE_REQUIRE(L >= 2, "AAE_PREC_TC_SPLIT: at least two conv layers expected");
+  const bool fp16 = cfg->precision == AAE_PREC_TC_FP16;
+  if (fp16 && !tc_conv1_supported(cfg)) {   // the fp32 CUDA-core conv1 behind the split plan writes (hi, lo) pairs only
+    set_error("AAE_PREC_TC_FP16: the first layer needs the tensor-core conv1 (128 x 128 x 3 crops, 128 filters, k = 5, stride 2)");
+    return AAE_ERR_UNSUPPORTED;
+  }
   TcEncoder* h = new TcEncoder();
   h->device = device;
   h->cfg = *cfg;
+  h->planes = fp16 ? 1 : 2;
   int ih = (cfg->in_h + cfg->strides[0] - 1) / cfg->strides[0], iw = (cfg->in_w + cfg->strides[0] - 1) / cfg->strides[0], ic = cfg->filters[0];
   const int B = cfg->max_batch;
   int st = AAE_OK;
@@ -321,10 +411,10 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
     const int B_pad = (int)ceil_div(B, T.BB) * T.BB;
     const size_t act_alloc = (size_t)B_pad * T.in_h * T.in_w * T.in_c;
     if ((st = dev_alloc((void**)&T.in_hi, act_alloc * sizeof(__half))) != AAE_OK) break;
-    if ((st = dev_alloc((void**)&T.in_lo, act_alloc * sizeof(__half))) != AAE_OK) break;
+    if (!fp16 && (st = dev_alloc((void**)&T.in_lo, act_alloc * sizeof(__half))) != AAE_OK) break;
     const size_t w_elems = (size_t)T.out_c * T.taps * T.in_c;
     if ((st = dev_alloc((void**)&T.w_hi, w_elems * sizeof(__half))) != AAE_OK) break;
-    if ((st = dev_alloc((void**)&T.w_lo, w_elems * sizeof(__half))) != AAE_OK) break;
+    if (!fp16 && (st = dev_alloc((void**)&T.w_lo, w_elems * sizeof(__half))) != AAE_OK) break;
     // ---- tensor maps ----
     if (!dense) {
       const uint64_t C4 = 4ull * T.in_c, W2 = T.in_w / 2, H2 = T.in_h / 2;
@@ -332,13 +422,13 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
       const uint64_t strides[3] = {C4 * 2, W2 * C4 * 2, H2 * W2 * C4 * 2};
       const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
       if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box)) != AAE_OK) break;
-      if ((st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) break;
+      if (!fp16 && (st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) break;
     } else {
       const uint64_t dims[4] = {(uint64_t)T.in_c, 1, 1, (uint64_t)B_pad};
       const uint64_t strides[3] = {(uint64_t)T.in_c * 2, (uint64_t)T.in_c * 2, (uint64_t)T.in_c * 2};
       const uint32_t box[4] = {(uint32_t)TC_KCH, 1, 1, 128};
       if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box)) != AAE_OK) break;
-      if ((st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) break;
+      if (!fp16 && (st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) break;
     }
     {
       const uint64_t K = (uint64_t)T.taps * T.in_c;
@@ -346,7 +436,7 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
       const uint64_t strides[1] = {K * 2};
       const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)std::min(TC_N_TILE, T.out_c)};
       if ((st = make_tmap_f16(&T.tm_w_hi, T.w_hi, 2, dims, strides, box)) != AAE_OK) break;
-      if ((st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box)) != AAE_OK) break;
+      if (!fp16 && (st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box)) != AAE_OK) break;
     }
     // ---- static GEMM parameters ----
     TcGemmParams& g = T.gp;
@@ -415,7 +505,8 @@ int tc_encoder_pack_weights(TcEncoder* h, int layer, const float* w_dev, cudaStr
   AAE_REQUIRE(layer >= 1 && layer <= (int)h->layers.size(), "tc pack: layer %d out of range", layer);
   TcLayer& T = h->layers[layer - 1];
   dim3 grid((unsigned)ceil_div(T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), (unsigned)T.taps), block(32, 8);
-  pack_weights_kernel<<<grid, block, 0, s>>>(w_dev, T.taps, T.in_c, T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, 1u << (16 + layer));
+  if (h->planes == 1) pack_weights_kernel<1><<<grid, block, 0, s>>>(w_dev, T.taps, T.in_c, T.out_c, W_SCALE, T.w_hi, nullptr, h->range_flag, 1u << (16 + layer));
+  else pack_weights_kernel<<<grid, block, 0, s>>>(w_dev, T.taps, T.in_c, T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, 1u << (16 + layer));
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -480,12 +571,14 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
       S.gp.out_mode = OUT_F32;
       S.gp.out_f32 = h->fwd_partials;
       grid.z = (unsigned)splits;
-      AAE_TRY(tc_launch_layer(S, grid, s));
+      AAE_TRY(tc_launch_layer(S, grid, s, h->planes));
       const long long groups = (long long)T.gp.M * (T.gp.N >> 3);
-      splitk_forward_finish_kernel<<<(unsigned)std::min<long long>(132 * 8, ceil_div(groups, 256)), 256, 0, s>>>(h->fwd_partials, splits, T.gp);
+      const unsigned fin_grid = (unsigned)std::min<long long>(132 * 8, ceil_div(groups, 256));
+      if (h->planes == 1) splitk_forward_finish_kernel<1><<<fin_grid, 256, 0, s>>>(h->fwd_partials, splits, T.gp);
+      else splitk_forward_finish_kernel<<<fin_grid, 256, 0, s>>>(h->fwd_partials, splits, T.gp);
       AAE_LAUNCH_OK();
     } else {
-      AAE_TRY(tc_launch_layer(T, grid, s));
+      AAE_TRY(tc_launch_layer(T, grid, s, h->planes));
     }
     if (dense) AAE_TRY(launch_splitk_reduce(h->partials, h->dense_splits, (int64_t)B * cfg.latent, cfg.latent, dense_b, ACT_NONE, z_out, s));
     timer->mark(s);
@@ -513,7 +606,8 @@ int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int
     AAE_TRY(dev_alloc((void**)&h->dbg, n * sizeof(float)));
     h->dbg_floats = n;
   }
-  unpack_act_kernel<<<1024, 256, 0, s>>>(T.in_hi, T.in_lo, B, H, W, C, plain ? 0 : 1, 1.f / ACT_SCALE, h->dbg);
+  if (h->planes == 1) unpack_act_kernel<1><<<1024, 256, 0, s>>>(T.in_hi, nullptr, B, H, W, C, plain ? 0 : 1, 1.f / ACT_SCALE, h->dbg);
+  else unpack_act_kernel<<<1024, 256, 0, s>>>(T.in_hi, T.in_lo, B, H, W, C, plain ? 0 : 1, 1.f / ACT_SCALE, h->dbg);
   AAE_LAUNCH_OK();
   AAE_CUDA_OK(cudaStreamSynchronize(s));
   *ptr = h->dbg;

@@ -9,6 +9,8 @@
 // create time, streams through a TMA ring, each row read from HBM once; per tile  hi*hi + hi*lo + lo*hi  go into one fp32
 // accumulator (operands pre-scaled by 64, exact unscale).  Per-CTA winners merge through a 64-bit atomicMax on (score, ~index)
 // (k = 1) or per-CTA lists merged by the last CTA (k <= 8), deterministically; the last CTA re-arms the scratch.
+// The single-pass instantiation (PLANES = 1, AAE_PREC_TC_FP16) keeps the hi terms alone: 32 KB of queries, a 32 KB codebook
+// tile per stage and one product per k-step; the shared memory the lo planes held goes to a deeper ring (MtCfg).
 #include <stdlib.h>
 
 #include "tc.cuh"
@@ -29,6 +31,18 @@ constexpr float MT_SCALE = 64.f;
 constexpr int MT_Q_BYTES = 4 * MT_E_BYTES;      // the launch's 128 queries as (hi, lo) fp16, K = 128
 constexpr int MT_SMEM_TOTAL = MT_STAGES * MT_STAGE_BYTES + MT_Q_BYTES + 1024 + 256;
 constexpr int MT_MAX_GRID = 148;                // CTAs of one launch at most (sm_count is clamped to it)
+
+// Ring and query buffer per operand-plane count.  PLANES = 1: 32 KB stages, so the split kernel's 197,888 bytes of dynamic
+// shared memory hold 5 of them (160 KB of codebook in flight per SM instead of 128 KB): the same footprint and carveout as
+// the split kernel, which aae_launch_floor_probe measures.
+template <int PLANES>
+struct MtCfg {
+  static constexpr int STAGES = PLANES == 2 ? MT_STAGES : 5;
+  static constexpr int STAGE_BYTES = PLANES * 2 * MT_E_BYTES;
+  static constexpr int Q_BYTES = PLANES * 2 * MT_E_BYTES;
+  static constexpr int SMEM_TOTAL = STAGES * STAGE_BYTES + Q_BYTES + 1024 + 256;
+};
+static_assert(MtCfg<2>::SMEM_TOTAL == MT_SMEM_TOTAL && MtCfg<1>::SMEM_TOTAL == MT_SMEM_TOTAL, "same footprint at both precisions");
 constexpr int MT_BATCH = 128;                   // queries per launch
 
 __device__ __forceinline__ unsigned long long pack_best(float s, int idx) {
@@ -94,17 +108,20 @@ __device__ __forceinline__ void quad_merge(const TopList<K>& l, float unscale, u
 // [0,64) and [64,128) of the block into shared memory, then run wgmma (A = queries, B = a 128-row codebook tile) and scan their
 // accumulator fragments: thread (warp, lane) owns rows 16 (warp % 4) + lane / 4 (+8) of its warpgroup's 64 queries and 32 of
 // the 128 codebook rows of each tile.
-template <int K>
+// PLANES = 1: tm_e_lo is unused, queries and codebook are the hi terms alone.
+template <int K, int PLANES = 2>
 __global__ void __launch_bounds__(MT_THREADS, 1)
 tc_match_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_constant__ CUtensorMap tm_e_lo, const float* __restrict__ z,
                 int B, int n_rows, int n_tiles, int idx_mul, long long row_offset, int k_out, unsigned long long* __restrict__ best,
                 unsigned long long* __restrict__ lists, unsigned int* __restrict__ counter, float* __restrict__ scores_out,
                 int* __restrict__ idx_out) {
+  using Cfg = MtCfg<PLANES>;
+  constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* e_smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* q_smem = e_smem + MT_STAGES * MT_STAGE_BYTES;   // Q_hi k0, Q_hi k1, Q_lo k0, Q_lo k1: 128 queries x 128 B each
-  uint64_t* e_full = reinterpret_cast<uint64_t*>(q_smem + MT_Q_BYTES);
-  uint64_t* e_empty = e_full + MT_STAGES;
+  uint8_t* q_smem = e_smem + STAGES * STAGE_BYTES;         // Q_hi k0, Q_hi k1, Q_lo k0, Q_lo k1: 128 queries x 128 B each
+  uint64_t* e_full = reinterpret_cast<uint64_t*>(q_smem + Cfg::Q_BYTES);
+  uint64_t* e_empty = e_full + STAGES;
   __shared__ int s_is_last;
   __shared__ float s_part[2][128];
 
@@ -112,7 +129,7 @@ tc_match_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_consta
   const int my_tiles = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < MT_STAGES; ++s) { mbar_init(&e_full[s], 1); mbar_init(&e_empty[s], 2); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&e_full[s], 1); mbar_init(&e_empty[s], 2); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -120,15 +137,17 @@ tc_match_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_consta
   if (warp == 0) {
     if (lane == 0) {                                  // the codebook stream starts before the query prologue
       for (int i = 0; i < my_tiles; ++i) {
-        const int s = i % MT_STAGES;
-        mbar_wait(&e_empty[s], ((uint32_t)(i / MT_STAGES) & 1u) ^ 1u);
+        const int s = i % STAGES;
+        mbar_wait(&e_empty[s], ((uint32_t)(i / STAGES) & 1u) ^ 1u);
         const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * MT_ROWS;
-        uint8_t* st = e_smem + s * MT_STAGE_BYTES;
-        mbar_arrive_expect_tx(&e_full[s], MT_STAGE_BYTES);
+        uint8_t* st = e_smem + s * STAGE_BYTES;
+        mbar_arrive_expect_tx(&e_full[s], STAGE_BYTES);
         tma_load_2d(st, &tm_e_hi, &e_full[s], 0, row0);
         tma_load_2d(st + MT_E_BYTES, &tm_e_hi, &e_full[s], 64, row0);
-        tma_load_2d(st + 2 * MT_E_BYTES, &tm_e_lo, &e_full[s], 0, row0);
-        tma_load_2d(st + 3 * MT_E_BYTES, &tm_e_lo, &e_full[s], 64, row0);
+        if constexpr (PLANES == 2) {
+          tma_load_2d(st + 2 * MT_E_BYTES, &tm_e_lo, &e_full[s], 0, row0);
+          tma_load_2d(st + 3 * MT_E_BYTES, &tm_e_lo, &e_full[s], 64, row0);
+        }
       }
     }
   } else if (warp >= 4) {
@@ -155,15 +174,22 @@ tc_match_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_consta
       uint8_t* qh = q_smem + half * MT_E_BYTES + r * 128;
 #pragma unroll
       for (int g = 0; g < 8; ++g) {                    // 8 K elements = one 16-byte chunk of the row
-        uint32_t hi[4], lo[4];
         const float4 a = mine[2 * g], b = mine[2 * g + 1];
-        split_f16x2(a.x * inv, a.y * inv, hi[0], lo[0]);
-        split_f16x2(a.z * inv, a.w * inv, hi[1], lo[1]);
-        split_f16x2(b.x * inv, b.y * inv, hi[2], lo[2]);
-        split_f16x2(b.z * inv, b.w * inv, hi[3], lo[3]);
         const int off = (g ^ (r & 7)) << 4;
-        *reinterpret_cast<uint4*>(qh + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *reinterpret_cast<uint4*>(qh + 2 * MT_E_BYTES + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+        if constexpr (PLANES == 1) {
+          const __half2 h0 = __floats2half2_rn(a.x * inv, a.y * inv), h1 = __floats2half2_rn(a.z * inv, a.w * inv);
+          const __half2 h2 = __floats2half2_rn(b.x * inv, b.y * inv), h3 = __floats2half2_rn(b.z * inv, b.w * inv);
+          *reinterpret_cast<uint4*>(qh + off) = make_uint4(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1),
+                                                           *reinterpret_cast<const uint32_t*>(&h2), *reinterpret_cast<const uint32_t*>(&h3));
+        } else {
+          uint32_t hi[4], lo[4];
+          split_f16x2(a.x * inv, a.y * inv, hi[0], lo[0]);
+          split_f16x2(a.z * inv, a.w * inv, hi[1], lo[1]);
+          split_f16x2(b.x * inv, b.y * inv, hi[2], lo[2]);
+          split_f16x2(b.z * inv, b.w * inv, hi[3], lo[3]);
+          *reinterpret_cast<uint4*>(qh + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+          *reinterpret_cast<uint4*>(qh + 2 * MT_E_BYTES + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+        }
       }
       fence_proxy_async_smem();                        // generic-proxy writes -> visible to wgmma
       named_bar_sync(1, 256);
@@ -174,15 +200,23 @@ tc_match_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_consta
     la.init(); lb.init();
     float acc[MT_ROWS / 2];
     for (int i = 0; i < my_tiles; ++i) {
-      const int s = i % MT_STAGES;
+      const int s = i % STAGES;
       const int row0 = ((int)blockIdx.x + i * (int)gridDim.x) * MT_ROWS;
       const int nvalid = min(MT_ROWS, n_rows - row0);
-      mbar_wait(&e_full[s], (uint32_t)(i / MT_STAGES) & 1u);
-      const uint32_t est = smem_u32(e_smem + s * MT_STAGE_BYTES);
+      mbar_wait(&e_full[s], (uint32_t)(i / STAGES) & 1u);
+      const uint32_t est = smem_u32(e_smem + s * STAGE_BYTES);
       wgmma_fence_regs(acc);
       wgmma_fence();
 #pragma unroll
-      for (int kh = 0; kh < 2; ++kh) {
+      for (int kh = 0; kh < 2 && PLANES == 1; ++kh) {
+        const uint64_t q_hi = make_sw128_kmajor_desc(q_base + kh * MT_E_BYTES);
+        const uint64_t e_hi = make_sw128_kmajor_desc(est + kh * MT_E_BYTES);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          Wgmma<MT_ROWS>::template ss<0, 0>(acc, desc_advance_k(q_hi, k), desc_advance_k(e_hi, k), (kh > 0 || k > 0) ? 1u : 0u);
+      }
+#pragma unroll
+      for (int kh = 0; kh < 2 && PLANES == 2; ++kh) {
         const uint64_t q_hi = make_sw128_kmajor_desc(q_base + kh * MT_E_BYTES);
         const uint64_t q_lo = make_sw128_kmajor_desc(q_base + (2 + kh) * MT_E_BYTES);
         const uint64_t e_hi = make_sw128_kmajor_desc(est + kh * MT_E_BYTES);
@@ -298,7 +332,8 @@ __global__ void __launch_bounds__(MT_THREADS, 1) launch_floor_kernel(unsigned in
   if (sink != nullptr && threadIdx.x == 0 && smem_raw[0] == 0xFF && blockIdx.x == 0xFFFFFFFFu) *sink = 1u;   // never true: keeps smem_raw referenced
 }
 
-// fp32 [n_rows][128] -> (hi, lo) fp16 [n_pad][128], scaled by 64; rows >= n_rows are zero
+// fp32 [n_rows][128] -> (hi, lo) fp16 [n_pad][128], scaled by 64; rows >= n_rows are zero.  PLANES = 1 writes hi only.
+template <int PLANES = 2>
 __global__ void pack_codebook_kernel(const float* __restrict__ E, long long n_rows, long long n_pad, __half* __restrict__ hi,
                                      __half* __restrict__ lo) {
   const long long total = n_pad * 128;
@@ -307,7 +342,7 @@ __global__ void pack_codebook_kernel(const float* __restrict__ E, long long n_ro
     __half h, l;
     split_f16(x, h, l);
     hi[i] = h;
-    lo[i] = l;
+    if constexpr (PLANES == 2) lo[i] = l;
   }
 }
 
@@ -319,6 +354,7 @@ struct TcCodebook {
   int n_tiles, max_batch, sm_count, num_cyclo;
   long long n_up;                 // rows of the `upright` view (every num_cyclo-th row)
   int n_tiles_up;
+  int planes;                     // 2: (hi, lo) codebook (AAE_PREC_TC_SPLIT); 1: hi only (AAE_PREC_TC_FP16), e_lo not allocated
   __half *e_hi = nullptr, *e_lo = nullptr;
   CUtensorMap tm_hi, tm_lo, tm_hi_up, tm_lo_up;
   bool have_up = false;
@@ -345,12 +381,14 @@ int tc_launch_floor_probe(int device, int with_tmem, cudaStream_t s) {
   return AAE_OK;
 }
 
-int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int latent, int num_cyclo, int max_batch, TcCodebook** out) {
+int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int latent, int num_cyclo, int max_batch, int planes,
+                       TcCodebook** out) {
   *out = nullptr;
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   AAE_REQUIRE(latent == 128, "AAE_PREC_TC_SPLIT codebook match is built for latent = 128 (got %d)", latent);
   TcCodebook* h = new TcCodebook();
   h->device = device;
+  h->planes = planes;
   h->n_rows = n_rows;
   h->n_tiles = (int)ceil_div(n_rows, MT_ROWS);
   h->n_pad = (long long)h->n_tiles * MT_ROWS;
@@ -363,14 +401,15 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
   h->sm_count = std::min(prop.multiProcessorCount, MT_MAX_GRID);
   const int cap_b = std::min(MT_BATCH, std::max(1, max_batch));
   cudaError_t e = cudaMalloc(&h->e_hi, (size_t)h->n_pad * 128 * sizeof(__half));
-  if (e == cudaSuccess) e = cudaMalloc(&h->e_lo, (size_t)h->n_pad * 128 * sizeof(__half));
+  if (e == cudaSuccess && planes == 2) e = cudaMalloc(&h->e_lo, (size_t)h->n_pad * 128 * sizeof(__half));
   if (e == cudaSuccess) e = cudaMalloc(&h->best, 256 * sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaMalloc(&h->lists, (size_t)h->sm_count * cap_b * MT_KMAX * sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaMalloc(&h->counter, sizeof(unsigned int));
   if (e != cudaSuccess) { set_error("tc codebook alloc failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_OOM; }
   cudaMemset(h->best, 0, 256 * sizeof(unsigned long long));
   cudaMemset(h->counter, 0, sizeof(unsigned int));
-  pack_codebook_kernel<<<1024, 256>>>(E_dev, n_rows, h->n_pad, h->e_hi, h->e_lo);
+  if (planes == 1) pack_codebook_kernel<1><<<1024, 256>>>(E_dev, n_rows, h->n_pad, h->e_hi, nullptr);
+  else pack_codebook_kernel<<<1024, 256>>>(E_dev, n_rows, h->n_pad, h->e_hi, h->e_lo);
   g_launches.fetch_add(1);
   e = cudaDeviceSynchronize();
   if (e != cudaSuccess) { set_error("pack_codebook failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_CUDA; }
@@ -378,20 +417,25 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
   const uint64_t strides[1] = {256};
   const uint32_t box[2] = {64, MT_ROWS};
   int st = make_tmap_f16(&h->tm_hi, h->e_hi, 2, dims, strides, box);
-  if (st == AAE_OK) st = make_tmap_f16(&h->tm_lo, h->e_lo, 2, dims, strides, box);
+  if (st == AAE_OK && planes == 2) st = make_tmap_f16(&h->tm_lo, h->e_lo, 2, dims, strides, box);
   if (st == AAE_OK && h->num_cyclo > 1) {
     // `upright` view (codebook.py:66 cos[::num_cyclo]): the same memory with a row stride of num_cyclo rows; boxes past
     // the last such row are zero-filled by TMA and masked by the kernel
     const uint64_t dims_u[2] = {128, (uint64_t)h->n_up};
     const uint64_t strides_u[1] = {(uint64_t)256 * (uint64_t)h->num_cyclo};
     st = make_tmap_f16(&h->tm_hi_up, h->e_hi, 2, dims_u, strides_u, box);
-    if (st == AAE_OK) st = make_tmap_f16(&h->tm_lo_up, h->e_lo, 2, dims_u, strides_u, box);
+    if (st == AAE_OK && planes == 2) st = make_tmap_f16(&h->tm_lo_up, h->e_lo, 2, dims_u, strides_u, box);
     h->have_up = st == AAE_OK;
   }
   if (st != AAE_OK) { tc_codebook_destroy(h); return st; }
   auto attr = [&](const void* fn) { return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MT_SMEM_TOTAL); };
-  e = attr((const void*)tc_match_kernel<1>);
-  if (e == cudaSuccess) e = attr((const void*)tc_match_kernel<MT_KMAX>);
+  if (planes == 1) {
+    e = attr((const void*)tc_match_kernel<1, 1>);
+    if (e == cudaSuccess) e = attr((const void*)tc_match_kernel<MT_KMAX, 1>);
+  } else {
+    e = attr((const void*)tc_match_kernel<1>);
+    if (e == cudaSuccess) e = attr((const void*)tc_match_kernel<MT_KMAX>);
+  }
   if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(match kernels) failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_CUDA; }
   *out = h;
   return AAE_OK;
@@ -422,7 +466,10 @@ int tc_codebook_match(TcCodebook* h, const float* z_dev, int B, int64_t row_offs
     const float* z = z_dev + (size_t)a * 128;
     float* so = scores_out + (size_t)a * k;
     int32_t* io = idx_out + (size_t)a * k;
-    if (k == 1) tc_match_kernel<1><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, 1, h->best, h->lists, h->counter, so, io);
+    if (h->planes == 1) {
+      if (k == 1) tc_match_kernel<1, 1><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, th, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, 1, h->best, h->lists, h->counter, so, io);
+      else tc_match_kernel<MT_KMAX, 1><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, th, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best, h->lists, h->counter, so, io);
+    } else if (k == 1) tc_match_kernel<1><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, 1, h->best, h->lists, h->counter, so, io);
     else tc_match_kernel<MT_KMAX><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best, h->lists, h->counter, so, io);
     AAE_LAUNCH_OK();
   }

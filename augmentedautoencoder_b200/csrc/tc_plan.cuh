@@ -84,6 +84,7 @@ struct TcEncoder {
   size_t fwd_partial_floats = 0;
   int dense_splits = 1;
   TcConv1* conv1 = nullptr;      // tensor-core first layer (when the geometry allows), else the fp32 SIMT kernel
+  int planes = 2;                // fp16 planes per operand: 2 = (hi, lo) (AAE_PREC_TC_SPLIT), 1 = hi only (AAE_PREC_TC_FP16)
   float* dbg = nullptr;          // fp32 view of an activation (tests)
   size_t dbg_floats = 0;
 };
@@ -130,7 +131,9 @@ __device__ __forceinline__ TcRow tc_decode_row(const TcGemmParams& p, int m) {
   return r;
 }
 
-// f[0..31]: accumulator values (already hh + cross, times unscale) of columns n .. n+31 of this thread's row
+// f[0..31]: accumulator values (already hh + cross, times unscale) of columns n .. n+31 of this thread's row.  PLANES = 1
+// (AAE_PREC_TC_FP16) stores the hi plane only, rounded straight from fp32; out_lo is not touched.
+template <int PLANES = 2>
 __device__ __forceinline__ void tc_store_chunk(const TcGemmParams& p, const TcRow& r, int n, float (&f)[32], int split_z) {
   if (p.out_mode == OUT_F32) {
     float* dst = p.out_f32 + (long long)split_z * p.M * p.N + r.row_off + n;
@@ -156,20 +159,35 @@ __device__ __forceinline__ void tc_store_chunk(const TcGemmParams& p, const TcRo
     const int cq = p.N >> 2, cls = n / cq, co = n - cls * cq;     // a 32-column chunk never straddles a parity class (cq % 32 == 0)
     off = ((long long)(r.b * 2 * p.OH + 2 * r.i + (cls >> 1)) * (2 * p.OW) + 2 * r.j + (cls & 1)) * cq + co;
   }
-  uint32_t hi[16], lo[16];
-  float amax = 0.f;
+  if constexpr (PLANES == 1) {
+    uint32_t hi[16];
+    float amax = 0.f;
 #pragma unroll
-  for (int j = 0; j < 32; j += 2) {
-    amax = fmaxf(amax, fmaxf(fabsf(f[j]), fabsf(f[j + 1])));
-    tc::split_f16x2(f[j] * p.out_scale, f[j + 1] * p.out_scale, hi[j >> 1], lo[j >> 1]);
-  }
-  if (p.range_flag != nullptr && !(amax * p.out_scale < TC_F16_OVERFLOW)) atomicOr(p.range_flag, p.range_bit);
-  uint4* dh = reinterpret_cast<uint4*>(p.out_hi + off);
-  uint4* dl = reinterpret_cast<uint4*>(p.out_lo + off);
+    for (int j = 0; j < 32; j += 2) {
+      amax = fmaxf(amax, fmaxf(fabsf(f[j]), fabsf(f[j + 1])));
+      const __half2 h = __floats2half2_rn(f[j] * p.out_scale, f[j + 1] * p.out_scale);
+      hi[j >> 1] = *reinterpret_cast<const uint32_t*>(&h);
+    }
+    if (p.range_flag != nullptr && !(amax * p.out_scale < TC_F16_OVERFLOW)) atomicOr(p.range_flag, p.range_bit);
+    uint4* dh = reinterpret_cast<uint4*>(p.out_hi + off);
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    dh[j] = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-    dl[j] = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
+    for (int j = 0; j < 4; ++j) dh[j] = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
+  } else {
+    uint32_t hi[16], lo[16];
+    float amax = 0.f;
+#pragma unroll
+    for (int j = 0; j < 32; j += 2) {
+      amax = fmaxf(amax, fmaxf(fabsf(f[j]), fabsf(f[j + 1])));
+      tc::split_f16x2(f[j] * p.out_scale, f[j + 1] * p.out_scale, hi[j >> 1], lo[j >> 1]);
+    }
+    if (p.range_flag != nullptr && !(amax * p.out_scale < TC_F16_OVERFLOW)) atomicOr(p.range_flag, p.range_bit);
+    uint4* dh = reinterpret_cast<uint4*>(p.out_hi + off);
+    uint4* dl = reinterpret_cast<uint4*>(p.out_lo + off);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      dh[j] = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
+      dl[j] = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
+    }
   }
 }
 
@@ -187,6 +205,16 @@ __device__ __forceinline__ void tc_park_acc(float* img, int ld, int wg, int warp
     *reinterpret_cast<float2*>(img + (r0 + 8) * ld + 2 * R + 8 * j + c0) = make_float2(crs[4 * j + 2], crs[4 * j + 3]);
   }
 }
+// The same for a single accumulator (AAE_PREC_TC_FP16: no cross term): image [128][ld], ld >= 2 R
+template <int R>
+__device__ __forceinline__ void tc_park_acc(float* img, int ld, int wg, int warp, int lane, const float (&acc)[R]) {
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = (lane & 3) * 2;
+#pragma unroll
+  for (int j = 0; j < R / 4; ++j) {
+    *reinterpret_cast<float2*>(img + r0 * ld + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(img + (r0 + 8) * ld + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
+}
 __device__ __forceinline__ void tc_acc_ld32(const float* img, int ld, int row, int col, uint32_t (&v)[32]) {
   const float4* src = reinterpret_cast<const float4*>(img + row * ld + col);
 #pragma unroll
@@ -196,8 +224,8 @@ __device__ __forceinline__ void tc_acc_ld32(const float* img, int ld, int row, i
   }
 }
 
-// launches tc_gemm_kernel over grid = (M tiles, N tiles, K splits)
-int tc_launch_layer(const TcLayer& T, dim3 grid, cudaStream_t s);
+// launches tc_gemm_kernel over grid = (M tiles, N tiles, K splits); planes = 1 runs the single-pass (hi-only) instantiation
+int tc_launch_layer(const TcLayer& T, dim3 grid, cudaStream_t s, int planes = 2);
 int tc_dev_alloc(void** p, size_t bytes);
 // Tensor maps + packed-weight storage of a layer whose A operand is a PLAIN NHWC (hi, lo) tensor [B_pad, in_h, in_w, in_c]
 // (taps = unit-stride boxes): fills tm_a_*, allocates w_hi/w_lo [ceil(N / TC_N_TILE) * TC_N_TILE][taps * in_c] and their maps.

@@ -49,8 +49,18 @@ typedef enum {
  *   AAE_PREC_FP32_SIMT : IEEE fp32 FMA chains on the CUDA cores (exact-order reference path)
  *   AAE_PREC_TC_SPLIT  : wgmma tensor cores, every fp32 operand split into two fp16 terms
  *                        (hi + 2^-11 lo), three products hi*hi + hi*lo + lo*hi accumulated in
- *                        fp32 registers -- fp32-grade results at tensor-core rate. */
-typedef enum { AAE_PREC_FP32_SIMT = 0, AAE_PREC_TC_SPLIT = 1 } aae_precision;
+ *                        fp32 registers -- fp32-grade results at tensor-core rate.
+ *   AAE_PREC_TC_FP16   : inference only (encoder and codebook match; aae_decoder_create refuses it with
+ *                        AAE_ERR_UNSUPPORTED, aae_trainer_create refuses an encoder created with it).  Every
+ *                        operand is rounded once to fp16 (the hi term alone, unit roundoff 2^-11) and each K step
+ *                        issues the one product hi*hi into fp32 registers -- the precision class of TF32, which
+ *                        TensorFlow uses for fp32 convolutions and matmuls on Ampere and newer GPUs.  Same static
+ *                        scales and range guard as AAE_PREC_TC_SPLIT.  Error contract (DESIGN.md section 3): a layer
+ *                        output y deviates from the exact result by at most 2^-9 sum|a*w| + 2^-10 |y| plus an fp16-
+ *                        subnormal term; a codebook score by at most 2^-9 from the exact cosine of the handle's own
+ *                        latent, and the j-th returned index has a cosine at least the exact j-th best minus 2^-8.
+ * Any other value is rejected with AAE_ERR_INVALID_ARG. */
+typedef enum { AAE_PREC_FP32_SIMT = 0, AAE_PREC_TC_SPLIT = 1, AAE_PREC_TC_FP16 = 2 } aae_precision;
 
 #define AAE_MAX_LAYERS 8
 
@@ -107,7 +117,8 @@ AAE_API int aae_encoder_range_status(aae_encoder* h, void* stream);
  * pipeline is never synchronised for the check (Codebook.nearest_rotation_async). */
 AAE_API int aae_encoder_range_word(aae_encoder* h, const uint32_t** word_dev);
 /* Device pointer + element count of the activation of conv layer `layer` (NHWC fp32) from the last
- * forward; layer == num_layers gives the flattened encoder_out.  For tests and for the trainer. */
+ * forward; layer == num_layers gives the flattened encoder_out.  For tests and for the trainer.  On an AAE_PREC_TC_FP16
+ * handle this is the stored fp16 value (the only one there is), unscaled to fp32. */
 AAE_API int aae_encoder_activation(aae_encoder* h, int layer, const float** ptr_dev, int64_t* count);
 
 /* Device-side stage timing for benchmarks: `enable` switches cudaEvent bracketing of the stages of the NEXT forward calls
