@@ -9,7 +9,7 @@ HEADER_PATH = os.path.join(_HERE, "..", "include", "aae_b200.h")
 AAE_MAX_LAYERS = 8
 PREC_FP32_SIMT = 0
 PREC_TC_SPLIT = 1
-PREC_TC_FP16 = 2      # inference only (encoder + codebook match): one fp16 product per K step, see include/aae_b200.h
+PREC_TC_FP16 = 2      # encoder + codebook match handles, and the trainer's GEMMs (TrainOp(precision=...)): one fp16 product per K step
 
 
 class AaeError(RuntimeError):
@@ -59,6 +59,7 @@ _SIGS = {
     "aae_decoder_range_status": (_I, [_P, _P]),
     "aae_bootstrap_l2_loss": (_I, [_P, _P, _I, _I, _I, _P, _P, _P]),
     "aae_trainer_create": (_I, [_P, _P, _I, _F, _F, _F, _F, C.POINTER(_P)]),
+    "aae_trainer_create_prec": (_I, [_P, _P, _I, _F, _F, _F, _F, _I, C.POINTER(_P)]),
     "aae_trainer_destroy": (_I, [_P]),
     "aae_train_step": (_I, [_P, _P, _P, _I, _P, _P]),
     "aae_trainer_forward_backward": (_I, [_P, _P, _P, _I, _P, _P]),

@@ -100,12 +100,17 @@ def build_ae(encoder, decoder, args):
 
 class TrainOp(Tensor):
     """``session.run(train_op)``: encoder fwd, decoder fwd, bootstrapped L2, backward, TF-Adam, global_step += 1 -- one call
-    into aae_train_step (replaces slim.learning.create_train_op, ae_factory.py:86-88).  Evaluates to the loss."""
+    into aae_train_step (replaces slim.learning.create_train_op, ae_factory.py:86-88).  Evaluates to the loss.
 
-    def __init__(self, ae, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8):
+    ``precision`` picks the GEMM arithmetic of the step apart from the handles' (aae_trainer_create_prec).  None follows the
+    handles.  ``_lib.PREC_TC_FP16`` is the single-pass trainer: it needs PREC_TC_SPLIT encoder and decoder handles, which keep
+    that precision for inference, and raises for any other handles instead of switching their precision."""
+
+    def __init__(self, ae, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8, precision=None):
         super().__init__("train_op", (), np.float32, self._run)
         self._ae = ae
         self._hp = (float(learning_rate), float(beta1), float(beta2), float(epsilon))
+        self._precision = None if precision is None else int(precision)
         self._trainers = {}
 
     def trainer(self, device):
@@ -121,6 +126,12 @@ class TrainOp(Tensor):
             h = C.c_void_p()
             with torch.cuda.device(dev):
                 eh, dh = enc.handle(device), dec.handle(device)       # settles automatic precisions
+                if self._precision is not None:
+                    # an explicit GEMM precision: the handles must suit it as they are (an automatic fp32 fallback does not)
+                    _lib.check(_lib.lib().aae_trainer_create_prec(eh, dh, dec._bootstrap_ratio, *self._hp, self._precision, C.byref(h)),
+                               "trainer create (GEMM precision %d)" % self._precision)
+                    self._trainers[dev] = h
+                    return h
                 st = -3 if enc.precision != dec.precision else _lib.lib().aae_trainer_create(eh, dh, dec._bootstrap_ratio, *self._hp, C.byref(h))
                 if st == -3 and (enc._auto_precision or dec._auto_precision or enc.precision != dec.precision) and \
                         (enc.precision, dec.precision) != (_lib.PREC_FP32_SIMT, _lib.PREC_FP32_SIMT):
@@ -227,12 +238,13 @@ class TrainOp(Tensor):
         return out
 
 
-def build_train_op(ae, args):
+def build_train_op(ae, args, precision=None):
+    """precision: the GEMM arithmetic of the training step (see TrainOp); None follows the encoder and decoder handles."""
     LEARNING_RATE = args.getfloat('Training', 'LEARNING_RATE')
     OPTIMIZER_NAME = args.get('Training', 'OPTIMIZER')
     if OPTIMIZER_NAME != 'Adam':
         raise NotImplementedError("OPTIMIZER: %s (the fused step implements tf.train.AdamOptimizer)" % OPTIMIZER_NAME)
-    return TrainOp(ae, LEARNING_RATE)
+    return TrainOp(ae, LEARNING_RATE, precision=precision)
 
 
 def build_codebook(encoder, dataset, args):

@@ -256,6 +256,11 @@ struct aae_trainer {
   DevBuf dwm;           // gradient wrt merged sub-pixel weights
   TcTrainPlan* tc = nullptr;  // tensor-core backward plan (encoder and decoder created with AAE_PREC_TC_SPLIT)
   uint64_t packed_enc_version = 0, packed_dec_version = 0;   // master-weight versions the plan's dgrad operands were packed from
+  // single-pass trainer (aae_trainer_create_prec with AAE_PREC_TC_FP16): private hi-only forward plans built from the handles'
+  // geometry and packed from their fp32 masters (w_version rule); the handles' own split plans serve inference only
+  TcEncoder* fenc = nullptr;
+  TcDecoder* fdec = nullptr;
+  uint64_t fenc_version = 0, fdec_version = 0;
   PhaseTimer ptimer;
 };
 
@@ -403,16 +408,19 @@ extern "C" int aae_encoder_get_weights(aae_encoder* h, int layer, float* kernel_
   return AAE_OK;
 }
 
-// Re-derive the tensor-core plan's packed operands from the fp32 master weights after an optimizer step changed them in place
-// (inference in the training process -- Codebook.update_embedding, decoder.x -- must see the weights get_weights() returns).
-static int encoder_sync_tc(aae_encoder* h, cudaStream_t s) {
-  if (!h->tc || h->tc_version == h->w_version) return AAE_OK;
+// Re-derive a tensor-core plan's packed operands from the fp32 master weights when `version` (the w_version they were packed
+// from) is behind, e.g. after an optimizer step changed the masters in place.
+static int encoder_pack_plan(aae_encoder* h, TcEncoder* plan, uint64_t& version, cudaStream_t s) {
+  if (version == h->w_version) return AAE_OK;
   const int nl = (int)h->conv.size();
-  for (int i = 0; i < nl; ++i) AAE_TRY(tc_encoder_pack_weights(h->tc, i, h->conv[i].w.p, s));
-  AAE_TRY(tc_encoder_pack_weights(h->tc, nl, h->dense_w.p, s));
-  h->tc_version = h->w_version;
+  for (int i = 0; i < nl; ++i) AAE_TRY(tc_encoder_pack_weights(plan, i, h->conv[i].w.p, s));
+  AAE_TRY(tc_encoder_pack_weights(plan, nl, h->dense_w.p, s));
+  version = h->w_version;
   return AAE_OK;
 }
+
+// inference in the training process (Codebook.update_embedding, decoder.x) must see the weights get_weights() returns
+static int encoder_sync_tc(aae_encoder* h, cudaStream_t s) { return h->tc ? encoder_pack_plan(h, h->tc, h->tc_version, s) : AAE_OK; }
 
 static int encoder_forward_simt(aae_encoder* h, const void* crops, int src_u8, int B, float* z_out, cudaStream_t s) {
   SimtEncoder& S = *h->simt;
@@ -817,18 +825,10 @@ static int make_pg(std::vector<ParamGrad>& v, DevBuf& param) {
   return AAE_OK;
 }
 
-extern "C" int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate, float beta1,
-                                  float beta2, float epsilon, aae_trainer** out) {
-  AAE_REQUIRE(out != nullptr, "out is null");
-  *out = nullptr;
-  AAE_REQUIRE(enc && dec, "null handle");
-  AAE_REQUIRE(enc->device == dec->device, "encoder and decoder live on different devices");
-  if ((enc->cfg.precision != AAE_PREC_FP32_SIMT && enc->cfg.precision != AAE_PREC_TC_SPLIT) ||
-      (dec->cfg.precision != AAE_PREC_FP32_SIMT && dec->cfg.precision != AAE_PREC_TC_SPLIT)) {
-    set_error("training needs AAE_PREC_FP32_SIMT or AAE_PREC_TC_SPLIT handles (encoder precision %d, decoder precision %d; AAE_PREC_TC_FP16 is "
-              "inference-only)", enc->cfg.precision, dec->cfg.precision);
-    return AAE_ERR_UNSUPPORTED;
-  }
+// The trainer over handles whose precisions are known to be trainable (FP32_SIMT or TC_SPLIT).  single_pass: the forward, dgrad
+// and wgrad GEMMs run on private hi-only plans instead of the handles' split plans.
+static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate, float beta1, float beta2,
+                          float epsilon, bool single_pass, aae_trainer** out) {
   AAE_REQUIRE((enc->tc == nullptr) == (dec->tc == nullptr), "encoder and decoder must use the same aae_precision for training");
   AAE_REQUIRE(enc->cfg.max_batch == dec->cfg.max_batch && enc->cfg.in_h == dec->cfg.in_h, "encoder/decoder geometry mismatch");
   DeviceGuard g(enc->device);
@@ -872,10 +872,63 @@ extern "C" int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootst
   if (st == AAE_OK) st = h->z.alloc(B * enc->cfg.latent);
   if (st == AAE_OK) st = h->dz.alloc(B * enc->cfg.latent);
   if (st == AAE_OK && max_wm) st = h->dwm.alloc(max_wm);
-  if (st == AAE_OK && enc->tc) st = tc_train_create(enc->tc, dec->tc, enc->cfg.max_batch, &h->tc);
+  if (st == AAE_OK && single_pass) {
+    aae_net_cfg c = enc->cfg;
+    c.precision = AAE_PREC_TC_FP16;
+    st = tc_encoder_create(enc->device, &c, &h->fenc);
+    c = dec->cfg;
+    c.precision = AAE_PREC_TC_FP16;
+    if (st == AAE_OK) st = tc_decoder_create(dec->device, &c, &h->fdec);
+    // bias pointers are the masters' (conv1's and the dense layer's are passed to every forward)
+    for (int l = 1; st == AAE_OK && l < (int)enc->conv.size(); ++l) st = tc_encoder_set_bias(h->fenc, l, enc->conv[l].b.p);
+    if (st == AAE_OK) {   // range overflows of the training forward and weight packs report through the handles' guard words
+      tc_encoder_share_range_flag(h->fenc, tc_encoder_range_flag(enc->tc));
+      tc_decoder_share_range_flag(h->fdec, tc_decoder_range_flag(dec->tc));
+    }
+  }
+  if (st == AAE_OK && enc->tc) st = tc_train_create(h->fenc ? h->fenc : enc->tc, h->fdec ? h->fdec : dec->tc, enc->cfg.max_batch, &h->tc);
   if (st != AAE_OK) { aae_trainer_destroy(h); return st; }
   *out = h;
   return AAE_OK;
+}
+
+extern "C" int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate, float beta1,
+                                  float beta2, float epsilon, aae_trainer** out) {
+  AAE_REQUIRE(out != nullptr, "out is null");
+  *out = nullptr;
+  AAE_REQUIRE(enc && dec, "null handle");
+  AAE_REQUIRE(enc->device == dec->device, "encoder and decoder live on different devices");
+  if ((enc->cfg.precision != AAE_PREC_FP32_SIMT && enc->cfg.precision != AAE_PREC_TC_SPLIT) ||
+      (dec->cfg.precision != AAE_PREC_FP32_SIMT && dec->cfg.precision != AAE_PREC_TC_SPLIT)) {
+    set_error("training needs AAE_PREC_FP32_SIMT or AAE_PREC_TC_SPLIT handles (encoder precision %d, decoder precision %d; AAE_PREC_TC_FP16 is "
+              "inference-only)", enc->cfg.precision, dec->cfg.precision);
+    return AAE_ERR_UNSUPPORTED;
+  }
+  return trainer_create(enc, dec, bootstrap_ratio, learning_rate, beta1, beta2, epsilon, false, out);
+}
+
+static const char* precision_name(int p) {
+  return p == AAE_PREC_FP32_SIMT ? "AAE_PREC_FP32_SIMT" : p == AAE_PREC_TC_SPLIT ? "AAE_PREC_TC_SPLIT" : "AAE_PREC_TC_FP16";
+}
+
+extern "C" int aae_trainer_create_prec(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate, float beta1,
+                                       float beta2, float epsilon, int gemm_precision, aae_trainer** out) {
+  AAE_REQUIRE(out != nullptr, "out is null");
+  *out = nullptr;
+  AAE_REQUIRE(enc && dec, "null handle");
+  AAE_REQUIRE(enc->device == dec->device, "encoder and decoder live on different devices");
+  AAE_REQUIRE(gemm_precision == AAE_PREC_FP32_SIMT || gemm_precision == AAE_PREC_TC_SPLIT || gemm_precision == AAE_PREC_TC_FP16,
+              "gemm_precision=%d is not an aae_precision (0, 1 or 2)", gemm_precision);
+  const int ep = enc->cfg.precision, dp = dec->cfg.precision;
+  if (gemm_precision != AAE_PREC_TC_FP16 && gemm_precision == ep && gemm_precision == dp)
+    return aae_trainer_create(enc, dec, bootstrap_ratio, learning_rate, beta1, beta2, epsilon, out);
+  if (gemm_precision != AAE_PREC_TC_FP16 || ep != AAE_PREC_TC_SPLIT || dp != AAE_PREC_TC_SPLIT) {
+    set_error("trainer GEMM precision %s is unsupported with an %s encoder and an %s decoder: the GEMM precision must equal the handles' "
+              "(AAE_PREC_FP32_SIMT or AAE_PREC_TC_SPLIT), or be AAE_PREC_TC_FP16 with two AAE_PREC_TC_SPLIT handles",
+              precision_name(gemm_precision), precision_name(ep), precision_name(dp));
+    return AAE_ERR_UNSUPPORTED;
+  }
+  return trainer_create(enc, dec, bootstrap_ratio, learning_rate, beta1, beta2, epsilon, true, out);
 }
 
 extern "C" int aae_trainer_destroy(aae_trainer* h) {
@@ -886,6 +939,8 @@ extern "C" int aae_trainer_destroy(aae_trainer* h) {
   h->dx_out.release(); h->grad_a.release(); h->grad_b.release(); h->dxup.release(); h->flat.release(); h->wt.release(); h->partials.release();
   h->bias_scratch.release(); h->sample_sums.release(); h->z.release(); h->dz.release(); h->rec.release(); h->dwm.release();
   tc_train_destroy(h->tc);
+  tc_encoder_destroy(h->fenc);
+  tc_decoder_destroy(h->fdec);
   h->ptimer.release();
   delete h;
   return AAE_OK;
@@ -996,7 +1051,8 @@ static int encoder_dense_backward(aae_trainer* h, const float* flat, int B, floa
 
 // Training step on the tensor cores: forward through the split-fp16 plans (their (hi, lo) activations double as the ReLU
 // masks and the wgrad operands), conv backward as wgmma GEMMs (tc_train.cu) -- conv1's wgrad (K = 75) as a 1x1 wgrad GEMM over
-// the im2col of the input -- and the two dense layers and the elementwise pieces on the fp32 kernels.
+// the im2col of the input -- and the two dense layers and the elementwise pieces on the fp32 kernels.  The single-pass trainer
+// runs the same sequence on its private hi-only plans (h->fenc, h->fdec), whose hi activations play the same two roles.
 static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, int B, float* loss_out, cudaStream_t s) {
   aae_encoder* E = h->enc;
   aae_decoder* D = h->dec;
@@ -1009,16 +1065,20 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
   PhaseTimer& pt = h->ptimer;
   pt.reset();
   pt.mark(0, s);
+  const bool own = h->fenc != nullptr;           // single-pass trainer: forward on the private plans
+  TcEncoder* FE = own ? h->fenc : E->tc;
+  TcDecoder* FD = own ? h->fdec : D->tc;
+  uint64_t& fd_version = own ? h->fdec_version : D->tc_version;
   // ---- operands follow the fp32 master weights (Adam and set_weights change those) ----
-  AAE_TRY(encoder_sync_tc(E, s));
-  if (h->packed_dec_version != D->w_version || D->tc_version != D->w_version) {
+  AAE_TRY(own ? encoder_pack_plan(E, FE, h->fenc_version, s) : encoder_sync_tc(E, s));
+  if (h->packed_dec_version != D->w_version || fd_version != D->w_version) {
     // forward and dgrad operands of a decoder layer share one merge of its 5x5 taps
-    AAE_TRY(tc_decoder_pack_weights(D->tc, 0, D->dense_w.p, D->dense_b.p, s));
+    AAE_TRY(tc_decoder_pack_weights(FD, 0, D->dense_w.p, D->dense_b.p, s));
     for (int l = 1; l <= nd; ++l) {
-      AAE_TRY(tc_decoder_pack_weights(D->tc, l, D->conv[l - 1].w.p, D->conv[l - 1].b.p, s));
-      AAE_TRY(tc_train_pack_weights_merged(P, nd - l, tc_decoder_merged_weights(D->tc), s));
+      AAE_TRY(tc_decoder_pack_weights(FD, l, D->conv[l - 1].w.p, D->conv[l - 1].b.p, s));
+      AAE_TRY(tc_train_pack_weights_merged(P, nd - l, tc_decoder_merged_weights(FD), s));
     }
-    D->tc_version = h->packed_dec_version = D->w_version;
+    fd_version = h->packed_dec_version = D->w_version;
   }
   if (h->packed_enc_version != E->w_version) {
     for (int u = n_dec; u < n_units; ++u) AAE_TRY(tc_train_pack_weights(P, u, E->conv[nl - 1 - (u - n_dec)].w.p, s));
@@ -1027,9 +1087,9 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
   pt.mark(1, s);
   AAE_TRY(tc_train_begin_step(P, s));
   // ---- forward ----
-  E->last_batch = B;
-  AAE_TRY(tc_encoder_forward(E->tc, x, 0, B, E->conv[0].w.p, E->conv[0].b.p, E->dense_b.p, h->z.p, &E->timer, s));
-  AAE_TRY(tc_decoder_forward(D->tc, h->z.p, B, h->rec.p, s));
+  if (!own) E->last_batch = B;                   // aae_encoder_activation reads the handle's plan
+  AAE_TRY(tc_encoder_forward(FE, x, 0, B, E->conv[0].w.p, E->conv[0].b.p, E->dense_b.p, h->z.p, &E->timer, s));
+  AAE_TRY(tc_decoder_forward(FD, h->z.p, B, h->rec.p, s));
   const int k = h->bootstrap_ratio > 1 ? numel / h->bootstrap_ratio : numel;
   AAE_TRY(launch_bootstrap_l2(h->rec.p, y, B, numel, k, h->sample_sums.p, loss_out, h->dx_out.p, s));
   AAE_TRY(launch_sigmoid_grad(h->dx_out.p, h->rec.p, (int64_t)B * numel, s));

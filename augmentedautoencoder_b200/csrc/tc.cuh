@@ -1,5 +1,5 @@
-// Tensor-core (wgmma / TMA) execution plans behind AAE_PREC_TC_SPLIT and, for inference, AAE_PREC_TC_FP16 (cfg->precision
-// selects the plan's operand planes).  Internal to the library.
+// Tensor-core (wgmma / TMA) execution plans behind AAE_PREC_TC_SPLIT and AAE_PREC_TC_FP16 (encoder inference, and the
+// single-pass trainer's private plans); cfg->precision selects the plan's operand planes.  Internal to the library.
 #pragma once
 #include "common.cuh"
 
@@ -26,6 +26,8 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
 int tc_encoder_set_bias(TcEncoder* h, int layer, const float* bias_dev);
 // device word of the run-time range guard (tc_plan.cuh): bit l = activation of layer l overflowed fp16, bit 16 + l = a weight did
 unsigned* tc_encoder_range_flag(TcEncoder* h);
+// makes the plan record into `flag` (another plan's word, same bit layout, outliving this plan) instead of its own
+void tc_encoder_share_range_flag(TcEncoder* h, unsigned* flag);
 int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int64_t* count, cudaStream_t s);
 
 struct TcDecoder;
@@ -34,6 +36,7 @@ void tc_decoder_destroy(TcDecoder* h);
 int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const float* b_dev, cudaStream_t s);
 int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, cudaStream_t s);
 unsigned* tc_decoder_range_flag(TcDecoder* h);
+void tc_decoder_share_range_flag(TcDecoder* h, unsigned* flag);
 const float* tc_decoder_merged_weights(const TcDecoder* h);   // fp32 merged sub-pixel weights of the layer packed last
 
 // ---- training: backward GEMMs (tc_train.cu); units are the conv layers in backward order (decoder L..1, encoder L..2)

@@ -8,8 +8,9 @@
 // fp32-grade arithmetic on fp16 tensor cores: every fp32 operand x is stored as two fp16 terms, hi = rn(x) and
 // lo = rn(x - hi) (22 significant bits; operands pre-scaled by a power of two so lo stays a normal fp16), and each
 // K chunk issues three MMAs: hi*hi into the main fp32 accumulator, hi*lo + lo*hi into a second one.
-// The single-pass instantiation (PLANES = 1, AAE_PREC_TC_FP16, inference only) keeps the hi terms alone: it loads the hi
-// boxes only, issues hi*hi into one accumulator and writes the hi plane of the next layer's input.
+// The single-pass instantiation (PLANES = 1, AAE_PREC_TC_FP16: the fp16 encoder, and the forward and dgrad GEMMs of the
+// single-pass trainer) keeps the hi terms alone: it loads the hi boxes only, issues hi*hi into one accumulator and writes the
+// hi plane of the next layer's input.
 //
 // Data movement: activations live in HBM in a space-to-depth layout  Xs[b, h/2, w/2, (h%2, w%2, c)]  written by the
 // producing layer's epilogue, so that tap (kh, kw) of the stride-2 / asymmetric-SAME(1,2) convolution is a plain
@@ -162,6 +163,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
     const int q = warp & 3, half = (warp - 4) >> 2;
     const TcRow row = tc_decode_row(p, m0 + q * 32 + lane);
     const bool has_work = it_end > it_begin;
+    const float unscale = p.amax_bits ? p.unscale * tc_dyn_unscale(__ldg(p.amax_bits)) : p.unscale;
 #pragma unroll 1
     for (int c = half; c < N_TILE / 32; c += 2) {
       const int n = n0 + c * 32;
@@ -170,7 +172,7 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
       tc_acc_ld32(img, S::ACC_LD, q * 32 + lane, c * 32, v);
       float f[32];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = has_work ? __uint_as_float(v[j]) * p.unscale : 0.f;
+      for (int j = 0; j < 32; ++j) f[j] = has_work ? __uint_as_float(v[j]) * unscale : 0.f;
       tc_store_chunk<1>(p, row, n, f, (int)blockIdx.z);
     }
   } else if (warp >= 4) {
@@ -492,7 +494,7 @@ void tc_encoder_destroy(TcEncoder* h) {
   cudaFree(h->partials);
   cudaFree(h->fwd_partials);
   cudaFree(h->dbg);
-  cudaFree(h->range_flag);
+  if (h->owns_range_flag) cudaFree(h->range_flag);
   tc_conv1_destroy(h->conv1);
   delete h;
 }
@@ -513,6 +515,20 @@ int tc_encoder_pack_weights(TcEncoder* h, int layer, const float* w_dev, cudaStr
 
 unsigned* tc_encoder_range_flag(TcEncoder* h) { return h->range_flag; }
 unsigned* tc_decoder_range_flag(TcDecoder* h) { return h->range_flag; }
+
+void tc_encoder_share_range_flag(TcEncoder* h, unsigned* flag) {
+  if (h->owns_range_flag) cudaFree(h->range_flag);
+  h->range_flag = flag;
+  h->owns_range_flag = false;
+  for (size_t i = 0; i + 1 < h->layers.size(); ++i) h->layers[i].gp.range_flag = flag;   // the dense layer writes fp32: no guard
+}
+
+void tc_decoder_share_range_flag(TcDecoder* h, unsigned* flag) {
+  if (h->owns_range_flag) cudaFree(h->range_flag);
+  h->range_flag = flag;
+  h->owns_range_flag = false;
+  for (size_t i = 0; i + 1 < h->layers.size(); ++i) h->layers[i].gp.range_flag = flag;
+}
 
 int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const float* w0, const float* b0, const float* dense_b,
                        float* z_out, StageTimer* timer, cudaStream_t s) {
@@ -623,8 +639,11 @@ int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int
 // output parity; the epilogue scatters column (parity, co) of pixel (i, j) to pixel (2i+py, 2j+px) of the next layer's input
 // (depth-to-space).  The output layer (Cout <= 3) is tap-separable: a 1x1 GEMM into fp32 P with N = 9 taps x 4 parities x Cout
 // (padded to 128), then outlayer_gather_kernel sums the 3x3 neighbourhood, adds the bias, applies the sigmoid and writes fp32 NHWC.
+// A decoder plan with planes = 1 (hi-only operands, one product per K step) exists only inside the single-pass trainer: handles
+// refuse AAE_PREC_TC_FP16 for the decoder.
 namespace {
 
+template <int PLANES = 2>
 __global__ void split_scale_kernel(const float* __restrict__ x, long long n, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
                                    unsigned* __restrict__ range_flag, unsigned range_bit) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
@@ -632,11 +651,12 @@ __global__ void split_scale_kernel(const float* __restrict__ x, long long n, flo
     if (range_flag != nullptr && !(fabsf(x[i] * scale) < TC_F16_OVERFLOW)) atomicOr(range_flag, range_bit);
     split_f16(x[i] * scale, h, l);
     hi[i] = h;
-    lo[i] = l;
+    if constexpr (PLANES == 2) lo[i] = l;
   }
 }
 
 // merged weights Wm [9][cin][n4] -> operand of the tap-separable output layer: row (tap * n4 + m) = Wm[tap][:, m], rows >= 9*n4 zero
+template <int PLANES = 2>
 __global__ void pack_out_sep_kernel(const float* __restrict__ wm, int cin, int n4, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
                                     unsigned* __restrict__ range_flag, unsigned range_bit) {
   const int total = 128 * cin;
@@ -648,7 +668,7 @@ __global__ void pack_out_sep_kernel(const float* __restrict__ wm, int cin, int n
     __half a, d;
     split_f16(v, a, d);
     hi[i] = a;
-    lo[i] = d;
+    if constexpr (PLANES == 2) lo[i] = d;
   }
 }
 
@@ -687,31 +707,32 @@ __global__ void tile_bias_kernel(const float* __restrict__ b, int cout, float* _
 
 }  // namespace
 
-int tc_layer_setup_plain(TcLayer& T, int B, bool alloc_input) {
+int tc_layer_setup_plain(TcLayer& T, int B, bool alloc_input, int planes) {
   int st;
+  const bool two = planes == 2;
   const int B_pad = (int)ceil_div(B, T.BB) * T.BB;
   const size_t act = (size_t)B_pad * T.in_h * T.in_w * T.in_c;
   if (alloc_input) {
     if ((st = dev_alloc((void**)&T.in_hi, act * sizeof(__half))) != AAE_OK) return st;
-    if ((st = dev_alloc((void**)&T.in_lo, act * sizeof(__half))) != AAE_OK) return st;
+    if (two && (st = dev_alloc((void**)&T.in_lo, act * sizeof(__half))) != AAE_OK) return st;
   }
   const uint64_t K = (uint64_t)T.taps * T.in_c;
   const int rows = (int)ceil_div(T.gp.N, TC_N_TILE) * TC_N_TILE;
   if ((st = dev_alloc((void**)&T.w_hi, (size_t)rows * K * sizeof(__half))) != AAE_OK) return st;
-  if ((st = dev_alloc((void**)&T.w_lo, (size_t)rows * K * sizeof(__half))) != AAE_OK) return st;
+  if (two && (st = dev_alloc((void**)&T.w_lo, (size_t)rows * K * sizeof(__half))) != AAE_OK) return st;
   {
     const uint64_t dims[4] = {(uint64_t)T.in_c, (uint64_t)T.in_w, (uint64_t)T.in_h, (uint64_t)B_pad};
     const uint64_t strides[3] = {(uint64_t)T.in_c * 2, (uint64_t)T.in_w * T.in_c * 2, (uint64_t)T.in_h * T.in_w * T.in_c * 2};
     const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
     if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box)) != AAE_OK) return st;
-    if ((st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) return st;
+    if (two && (st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) return st;
   }
   {
     const uint64_t dims[2] = {K, (uint64_t)rows};
     const uint64_t strides[1] = {K * 2};
     const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)TC_N_TILE};
     if ((st = make_tmap_f16(&T.tm_w_hi, T.w_hi, 2, dims, strides, box)) != AAE_OK) return st;
-    if ((st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box)) != AAE_OK) return st;
+    if (two && (st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box)) != AAE_OK) return st;
   }
   return AAE_OK;
 }
@@ -724,6 +745,7 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
   TcDecoder* h = new TcDecoder();
   h->device = device;
   h->cfg = *cfg;
+  h->planes = cfg->precision == AAE_PREC_TC_FP16 ? 1 : 2;
   const int B = cfg->max_batch;
   int h0 = cfg->in_h;
   for (int i = 0; i < L; ++i) h0 /= 2;
@@ -770,7 +792,7 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
     }
     g.unscale = 1.f / (ACT_SCALE * W_SCALE);
     g.out_scale = ACT_SCALE;
-    if ((st = tc_layer_setup_plain(T, B, /*alloc_input=*/true)) != AAE_OK) { h->layers.push_back(T); break; }
+    if ((st = tc_layer_setup_plain(T, B, /*alloc_input=*/true, h->planes)) != AAE_OK) { h->layers.push_back(T); break; }
     h->layers.push_back(T);
     float* bz = nullptr;
     if (l > 0 && l < L) st = dev_alloc((void**)&bz, (size_t)g.N * sizeof(float));
@@ -798,7 +820,7 @@ void tc_decoder_destroy(TcDecoder* h) {
   for (auto b : h->bias_dev) cudaFree(b);
   cudaFree(h->wm_tmp);
   cudaFree(h->out_p);
-  cudaFree(h->range_flag);
+  if (h->owns_range_flag) cudaFree(h->range_flag);
   delete h;
 }
 
@@ -810,7 +832,8 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
   if (layer == 0) {
     if (w_dev) {
       dim3 grid((unsigned)ceil_div(T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), 1);
-      pack_weights_kernel<<<grid, block, 0, s>>>(w_dev, 1, T.in_c, T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, 1u << 16);
+      if (h->planes == 1) pack_weights_kernel<1><<<grid, block, 0, s>>>(w_dev, 1, T.in_c, T.out_c, W_SCALE, T.w_hi, nullptr, h->range_flag, 1u << 16);
+      else pack_weights_kernel<<<grid, block, 0, s>>>(w_dev, 1, T.in_c, T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, 1u << 16);
       AAE_LAUNCH_OK();
     }
     if (b_dev) T.gp.bias = b_dev;      // device pointer owned by the decoder handle
@@ -819,11 +842,14 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
   const bool out_layer = layer + 1 == (int)h->layers.size();
   if (w_dev) {
     AAE_TRY(launch_merge_subpixel_weights(w_dev, T.in_c, T.out_c, h->wm_tmp, s));
-    if (out_layer) {
-      pack_out_sep_kernel<<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, 1u << (16 + layer));
+    const unsigned bit = 1u << (16 + layer);
+    dim3 grid((unsigned)ceil_div(4 * T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), 9);
+    if (h->planes == 1) {
+      if (out_layer) pack_out_sep_kernel<1><<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, nullptr, h->range_flag, bit);
+      else pack_weights_kernel<1><<<grid, block, 0, s>>>(h->wm_tmp, 9, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, nullptr, h->range_flag, bit);
     } else {
-      dim3 grid((unsigned)ceil_div(4 * T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), 9);
-      pack_weights_kernel<<<grid, block, 0, s>>>(h->wm_tmp, 9, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, 1u << (16 + layer));
+      if (out_layer) pack_out_sep_kernel<<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, bit);
+      else pack_weights_kernel<<<grid, block, 0, s>>>(h->wm_tmp, 9, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, bit);
     }
     AAE_LAUNCH_OK();
   }
@@ -843,8 +869,9 @@ const float* tc_decoder_merged_weights(const TcDecoder* h) { return h->wm_tmp; }
 
 int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, cudaStream_t s) {
   TcLayer& D = h->layers[0];
-  split_scale_kernel<<<(unsigned)std::min<int64_t>(1024, ceil_div((int64_t)B * D.in_c, 256)), 256, 0, s>>>(z_dev, (long long)B * D.in_c, ACT_SCALE,
-                                                                                                          D.in_hi, D.in_lo, h->range_flag, 1u << 15);
+  const unsigned grid = (unsigned)std::min<int64_t>(1024, ceil_div((int64_t)B * D.in_c, 256));
+  if (h->planes == 1) split_scale_kernel<1><<<grid, 256, 0, s>>>(z_dev, (long long)B * D.in_c, ACT_SCALE, D.in_hi, nullptr, h->range_flag, 1u << 15);
+  else split_scale_kernel<<<grid, 256, 0, s>>>(z_dev, (long long)B * D.in_c, ACT_SCALE, D.in_hi, D.in_lo, h->range_flag, 1u << 15);
   AAE_LAUNCH_OK();
   for (size_t i = 0; i < h->layers.size(); ++i) {
     TcLayer& T = h->layers[i];
@@ -852,7 +879,7 @@ int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, cu
     const bool last = i + 1 == h->layers.size();
     if (last) T.gp.out_f32 = h->out_p;
     dim3 grid((unsigned)ceil_div(T.gp.M, 128), (unsigned)ceil_div(T.gp.N, TC_N_TILE), 1u);
-    AAE_TRY(tc_launch_layer(T, grid, s));
+    AAE_TRY(tc_launch_layer(T, grid, s, h->planes));
     if (last) {
       const long long total = (long long)T.gp.M * 4 * T.out_c;
       outlayer_gather_kernel<<<(unsigned)std::min<long long>(132 * 16, ceil_div(total, 256)), 256, 0, s>>>(h->out_p, h->out_bias, B, T.in_h, T.in_w,

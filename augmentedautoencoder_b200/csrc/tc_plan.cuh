@@ -77,6 +77,7 @@ struct TcEncoder {
   int device;
   aae_net_cfg cfg;
   unsigned* range_flag = nullptr;   // device word, see above
+  bool owns_range_flag = true;      // false once tc_encoder_share_range_flag pointed it at another plan's word
   std::vector<TcLayer> layers;   // conv layers 1..L-1 followed by the dense layer
   int flat;
   float* partials = nullptr;     // dense split-K partials [splits, max_batch, latent]
@@ -94,6 +95,7 @@ struct TcDecoder {
   int device;
   aae_net_cfg cfg;
   unsigned* range_flag = nullptr;
+  bool owns_range_flag = true;
   std::vector<TcLayer> layers;     // [0] dense_1, [1..L-1] sub-pixel convs, [L] sub-pixel output layer
   std::vector<float*> bias_dev;    // per sub-pixel conv: bias tiled 4x in GEMM-column order (nullptr for dense_1 and the output layer)
   float* wm_tmp = nullptr;         // fp32 merged-weight scratch
@@ -103,6 +105,7 @@ struct TcDecoder {
   float* out_p = nullptr;          // [B*h*w (padded to 128 rows)][128] fp32
   const float* out_bias = nullptr; // the caller's bias [Cout] (device)
   size_t wm_floats = 0;
+  int planes = 2;                  // fp16 planes per operand: 2 = (hi, lo); 1 = hi only (the single-pass trainer's private plan)
 };
 
 
@@ -229,7 +232,8 @@ int tc_launch_layer(const TcLayer& T, dim3 grid, cudaStream_t s, int planes = 2)
 int tc_dev_alloc(void** p, size_t bytes);
 // Tensor maps + packed-weight storage of a layer whose A operand is a PLAIN NHWC (hi, lo) tensor [B_pad, in_h, in_w, in_c]
 // (taps = unit-stride boxes): fills tm_a_*, allocates w_hi/w_lo [ceil(N / TC_N_TILE) * TC_N_TILE][taps * in_c] and their maps.
-// T.{in_h,in_w,in_c,taps,BW,BH,BB,gp.N} must be set; with alloc_input = false T.in_hi/in_lo are the caller's.
-int tc_layer_setup_plain(TcLayer& T, int B, bool alloc_input);
+// T.{in_h,in_w,in_c,taps,BW,BH,BB,gp.N} must be set; with alloc_input = false T.in_hi/in_lo are the caller's.  planes = 1
+// allocates and maps the hi planes only.
+int tc_layer_setup_plain(TcLayer& T, int B, bool alloc_input, int planes = 2);
 
 }  // namespace aae

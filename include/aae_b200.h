@@ -209,6 +209,22 @@ AAE_API int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, con
  * the gradients returned by aae_trainer_get_grads are fp32 in the reference layouts either way. */
 AAE_API int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate,
                                float beta1, float beta2, float epsilon, aae_trainer** out);
+/* The same trainer with the GEMM arithmetic chosen apart from the handles' precision.
+ *   gemm_precision equal to the precision of both handles: exactly aae_trainer_create.
+ *   AAE_PREC_TC_FP16 with two AAE_PREC_TC_SPLIT handles: the single-pass trainer.  Its forward, dgrad and wgrad
+ *     GEMMs round every operand once to fp16 and issue one hi*hi product per K step (the TF32 rounding class
+ *     of AAE_PREC_TC_FP16), on private hi-only plans packed from the handles' fp32 masters.  Gradients keep the
+ *     per-tensor, per-step power-of-two scale, the two dense layers' backward and Adam stay fp32, and the
+ *     handles keep AAE_PREC_TC_SPLIT: their weights are the trainer's masters and inference on them runs split.
+ *     Error contract (DESIGN.md section 3): each GEMM y = a*w adds at most (2^-9 + 2^-11) sum|a*w| (products,
+ *     then hi-only storage), i.e. (2^-9 + 2^-11) k of y in the L2 norm with k = ||(|a| |w|)|| / ||y||.  In the
+ *     linearised error model the terms of the GEMMs from the input to the loss and back to a gradient add, which
+ *     bounds the gradient's relative L2 error.
+ *   Any other combination (fp16 on AAE_PREC_FP32_SIMT or AAE_PREC_TC_FP16 handles, mixed handles, a split GEMM
+ *     precision on fp32 handles, ...) returns AAE_ERR_UNSUPPORTED, naming all three precisions in
+ *     aae_last_error_string(); a value outside {0, 1, 2} returns AAE_ERR_INVALID_ARG. */
+AAE_API int aae_trainer_create_prec(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate,
+                                    float beta1, float beta2, float epsilon, int gemm_precision, aae_trainer** out);
 AAE_API int aae_trainer_destroy(aae_trainer* h);
 /* x (augmented input) and y (reconstruction target) NHWC float32 [B,H,W,C]; loss_out_dev: 1 float. */
 AAE_API int aae_train_step(aae_trainer* h, const float* x_dev, const float* y_dev, int batch, float* loss_out_dev, void* stream);
