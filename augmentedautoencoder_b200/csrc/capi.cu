@@ -518,7 +518,7 @@ extern "C" int aae_codebook_create(int device, const float* embedding_any, int64
     if (e != cudaSuccess) { set_error("codebook upload failed: %s", cudaGetErrorString(e)); st = AAE_ERR_CUDA; }
   }
   if (st == AAE_OK && precision != AAE_PREC_FP32_SIMT)
-    st = tc_codebook_create(device, h->E.p, n_rows, latent, num_cyclo, max_batch, precision == AAE_PREC_TC_FP16 ? 1 : 2, &h->tc);
+    st = tc_codebook_create(device, h->E.p, n_rows, latent, num_cyclo, max_batch, tc_planes(precision), &h->tc);
   if (st != AAE_OK) { aae_codebook_destroy(h); return st; }
   *out = h;
   return AAE_OK;

@@ -9,6 +9,9 @@ struct TcEncoder;
 struct TcCodebook;
 struct TcConv1;
 
+// fp16 planes per operand of a tensor-core plan: 2 = (hi, lo) for AAE_PREC_TC_SPLIT, 1 = hi only for AAE_PREC_TC_FP16
+inline int tc_planes(int precision) { return precision == AAE_PREC_TC_FP16 ? 1 : 2; }
+
 bool tc_conv1_supported(const aae_net_cfg* cfg);
 int tc_conv1_create(int device, const aae_net_cfg* cfg, TcConv1** out);
 void tc_conv1_destroy(TcConv1* h);

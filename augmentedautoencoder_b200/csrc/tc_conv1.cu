@@ -16,6 +16,7 @@
 
 #include "tc.cuh"
 #include "tc_common.cuh"
+#include "tc_plan.cuh"
 
 namespace aae {
 
@@ -231,18 +232,11 @@ tc_conv1_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_consta
           const float a = fmaxf(acc[4 * j + 2 * h2] * p.unscale + bias_s[c], 0.f) * p.out_scale;
           const float bb = fmaxf(acc[4 * j + 2 * h2 + 1] * p.unscale + bias_s[c + 1], 0.f) * p.out_scale;
           amax = fmaxf(amax, fmaxf(a, bb));
-          if constexpr (PLANES == 1) {
-            const __half2 hh = __floats2half2_rn(a, bb);
-            *reinterpret_cast<uint32_t*>(my_hi[h2] + c * 2) = *reinterpret_cast<const uint32_t*>(&hh);
-          } else {
-            uint32_t hi, lo;
-            split_f16x2(a, bb, hi, lo);
-            *reinterpret_cast<uint32_t*>(my_hi[h2] + c * 2) = hi;
-            *reinterpret_cast<uint32_t*>(my_hi[h2] + 32 * C1_OUT_LD + c * 2) = lo;
-          }
+          const float v[2] = {a, bb};
+          tc_store_f16<PLANES>(v, 1.f, reinterpret_cast<__half*>(my_hi[h2]), reinterpret_cast<__half*>(my_hi[h2] + 32 * C1_OUT_LD), c);
         }
       }
-      if (p.range_flag != nullptr && !(amax < 65520.f)) atomicOr(p.range_flag, 1u);
+      if (p.range_flag != nullptr && !(amax < TC_F16_OVERFLOW)) atomicOr(p.range_flag, 1u);
       fence_proxy_async_smem();                      // generic-proxy writes -> visible to the bulk-copy engine
       named_bar_sync(2, 32 * C1_EPI_WARPS);
       if (warp == 4 && b < p.B) {                    // lane j ships group j (G KB) of the hi and of the lo slab
@@ -456,18 +450,11 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
           const float bb = fmaxf(fmaf(acc[4 * j + 2 * h2 + 1], us, bias_s[c + 1]), 0.f);
           amax = fmaxf(amax, fmaxf(a, bb));
           const int off = rr * 64 + (((j & 3) ^ ((rr >> 1) & 3)) << 4) + 4 * (lane & 3);
-          if constexpr (PLANES == 1) {
-            const __half2 hh = __floats2half2_rn(a, bb);
-            *reinterpret_cast<uint32_t*>(sb + off) = *reinterpret_cast<const uint32_t*>(&hh);
-          } else {
-            uint32_t hi, lo;
-            split_f16x2(a, bb, hi, lo);
-            *reinterpret_cast<uint32_t*>(sb + off) = hi;
-            *reinterpret_cast<uint32_t*>(sb + 1024 + off) = lo;
-          }
+          const float v[2] = {a, bb};
+          tc_store_f16<PLANES>(v, 1.f, reinterpret_cast<__half*>(sb + off), reinterpret_cast<__half*>(sb + 1024 + off), 0);
         }
       }
-      if (p.range_flag != nullptr && !(amax < 65520.f)) atomicOr(p.range_flag, 1u);
+      if (p.range_flag != nullptr && !(amax < TC_F16_OVERFLOW)) atomicOr(p.range_flag, 1u);
       fence_proxy_async_smem();                          // generic-proxy writes -> visible to the TMA engine
       __syncwarp();
       if (lane == 0) {
@@ -495,37 +482,26 @@ tc_conv1_u8_kernel(const __grid_constant__ CUtensorMap tm_w_hi, const __grid_con
   }
 }
 
-// W fp32 [75][N] (HWIO flattened) -> (hi, lo) fp16 [N][128] in the 5 x 16 slot order of the uint8 kernel: slot kh*16 + 1 + (kw*3 + c)
+// W fp32 [75][N] (HWIO flattened) -> fp16 [N][128] (format PLANES) in the 5 x 16 slot order of the uint8 kernel: slot kh*16 + 1 + (kw*3 + c)
 // holds scale * W[kh][kw][c][n] (scale = 2^16 / 255: the x/255 of codebook.py:58-59 lives here), every other slot is zero.
-// PLANES = 1 writes hi only.
-template <int PLANES = 2>
+template <int PLANES>
 __global__ void pack_conv1_u8_weights_kernel(const float* __restrict__ w, int N, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
                                              unsigned* __restrict__ range_flag, unsigned range_bit) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N * 128) return;
   const int n = i / 128, k = i - n * 128;
   const int kh = k >> 4, j = k & 15;
-  const float v = (kh < 5 && j >= 1) ? w[(long long)(kh * 15 + j - 1) * N + n] * scale : 0.f;
-  if (range_flag != nullptr && !(fabsf(v) < 65520.f)) atomicOr(range_flag, range_bit);
-  __half h, l;
-  split_f16(v, h, l);
-  hi[i] = h;
-  if constexpr (PLANES == 2) lo[i] = l;
+  tc_store_f16<PLANES>((kh < 5 && j >= 1) ? w[(long long)(kh * 15 + j - 1) * N + n] * scale : 0.f, hi, lo, i, range_flag, range_bit);
 }
 
-// W fp32 [75][N] (HWIO flattened) -> (hi, lo) fp16 [N][128] K-major, scaled, zero for k >= K; PLANES = 1 writes hi only
-template <int PLANES = 2>
+// W fp32 [75][N] (HWIO flattened) -> fp16 [N][128] K-major (format PLANES), scaled, zero for k >= K
+template <int PLANES>
 __global__ void pack_conv1_weights_kernel(const float* __restrict__ w, int K, int N, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
                                           unsigned* __restrict__ range_flag, unsigned range_bit) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N * 128) return;
   const int n = i / 128, k = i - n * 128;
-  const float v = k < K ? w[(long long)k * N + n] * scale : 0.f;
-  if (range_flag != nullptr && !(fabsf(v) < 65520.f)) atomicOr(range_flag, range_bit);
-  __half h, l;
-  split_f16(v, h, l);
-  hi[i] = h;
-  if constexpr (PLANES == 2) lo[i] = l;
+  tc_store_f16<PLANES>(k < K ? w[(long long)k * N + n] * scale : 0.f, hi, lo, i, range_flag, range_bit);
 }
 
 }  // namespace
@@ -533,12 +509,12 @@ __global__ void pack_conv1_weights_kernel(const float* __restrict__ w, int K, in
 struct TcConv1 {
   int N, sm_count;
   int planes;                     // 2: (hi, lo) operands and output (AAE_PREC_TC_SPLIT); 1: hi only (AAE_PREC_TC_FP16), no lo buffers
-  __half *w_hi = nullptr, *w_lo = nullptr;
-  CUtensorMap tm_hi, tm_lo;
-  // uint8 kernel: weights with 1/255 folded in, 5 x 16 slot order; output tensor maps over conv2's (hi, lo) input
-  __half *w8_hi = nullptr, *w8_lo = nullptr;
-  CUtensorMap tm8_hi, tm8_lo, tm_out32_hi, tm_out32_lo;   // output maps: one box = a warp's 32 slots x 32 channels
-  const __half *bound_hi = nullptr, *bound_lo = nullptr;
+  TcPlanes w;
+  TcMaps tm;
+  // uint8 kernel: weights with 1/255 folded in, 5 x 16 slot order; output tensor maps over conv2's input
+  TcPlanes w8;
+  TcMaps tm8, tm_out32;           // output maps: one box = a warp's 32 slots x 32 channels
+  TcPlanes bound;                 // the output the maps were encoded for (not owned)
   long long slots = 0;            // 256-byte output slots the tensor maps cover ((b, oh/2, ow/2, parity) positions)
 };
 
@@ -552,28 +528,21 @@ int tc_conv1_create(int device, const aae_net_cfg* cfg, TcConv1** out) {
   *out = nullptr;
   TcConv1* h = new TcConv1();
   h->N = cfg->filters[0];
-  h->planes = cfg->precision == AAE_PREC_TC_FP16 ? 1 : 2;
+  h->planes = tc_planes(cfg->precision);
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
   h->sm_count = prop.multiProcessorCount;
-  cudaError_t e = cudaMalloc(&h->w_hi, (size_t)h->N * 128 * sizeof(__half));
-  if (e == cudaSuccess && h->planes == 2) e = cudaMalloc(&h->w_lo, (size_t)h->N * 128 * sizeof(__half));
-  if (e != cudaSuccess) { set_error("tc conv1 alloc failed: %s", cudaGetErrorString(e)); tc_conv1_destroy(h); return AAE_ERR_OOM; }
   const uint64_t dims[2] = {128, (uint64_t)h->N};
   const uint64_t strides[1] = {256};
   const uint32_t box[2] = {64, (uint32_t)h->N};
-  const bool two = h->planes == 2;
-  int st = make_tmap_f16(&h->tm_hi, h->w_hi, 2, dims, strides, box);
-  if (st == AAE_OK && two) st = make_tmap_f16(&h->tm_lo, h->w_lo, 2, dims, strides, box);
-  if (st == AAE_OK) {
-    e = cudaMalloc(&h->w8_hi, (size_t)h->N * 128 * sizeof(__half));
-    if (e == cudaSuccess && two) e = cudaMalloc(&h->w8_lo, (size_t)h->N * 128 * sizeof(__half));
-    if (e != cudaSuccess) { set_error("tc conv1 alloc failed: %s", cudaGetErrorString(e)); tc_conv1_destroy(h); return AAE_ERR_OOM; }
-    st = make_tmap_f16(&h->tm8_hi, h->w8_hi, 2, dims, strides, box);
-    if (st == AAE_OK && two) st = make_tmap_f16(&h->tm8_lo, h->w8_lo, 2, dims, strides, box);
-    const void* u8_kernel = two ? (const void*)tc_conv1_u8_kernel<2> : (const void*)tc_conv1_u8_kernel<1>;
-    if (st == AAE_OK) st = cudaFuncSetAttribute(u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, U8_SMEM_TOTAL) == cudaSuccess ? AAE_OK : AAE_ERR_CUDA;
-  }
+  int st = h->w.alloc((size_t)h->N * 128, h->planes);
+  if (st == AAE_OK) st = h->w.encode(h->tm, 2, dims, strides, box);
+  if (st == AAE_OK) st = h->w8.alloc((size_t)h->N * 128, h->planes);
+  if (st == AAE_OK) st = h->w8.encode(h->tm8, 2, dims, strides, box);
+  if (st == AAE_OK)
+    st = with_planes(h->planes, [](auto P) {
+      return cudaFuncSetAttribute(tc_conv1_u8_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, U8_SMEM_TOTAL) == cudaSuccess ? AAE_OK : AAE_ERR_CUDA;
+    });
   if (st != AAE_OK) { tc_conv1_destroy(h); return st; }
   *out = h;
   return AAE_OK;
@@ -581,21 +550,19 @@ int tc_conv1_create(int device, const aae_net_cfg* cfg, TcConv1** out) {
 
 void tc_conv1_destroy(TcConv1* h) {
   if (!h) return;
-  cudaFree(h->w_hi); cudaFree(h->w_lo); cudaFree(h->w8_hi); cudaFree(h->w8_lo);
+  h->w.release();
+  h->w8.release();
   delete h;
 }
 
 int tc_conv1_pack(TcConv1* h, const float* w_dev, int K, float w_scale, unsigned* range_flag, unsigned range_bit, cudaStream_t s) {
   const unsigned grid = (unsigned)ceil_div(h->N * 128, 256);
-  if (h->planes == 1) pack_conv1_weights_kernel<1><<<grid, 256, 0, s>>>(w_dev, K, h->N, w_scale, h->w_hi, nullptr, range_flag, range_bit);
-  else pack_conv1_weights_kernel<<<grid, 256, 0, s>>>(w_dev, K, h->N, w_scale, h->w_hi, h->w_lo, range_flag, range_bit);
+  with_planes(h->planes, [&](auto P) { pack_conv1_weights_kernel<P><<<grid, 256, 0, s>>>(w_dev, K, h->N, w_scale, h->w.hi, h->w.lo, range_flag, range_bit); });
   AAE_LAUNCH_OK();
   AAE_REQUIRE(K == 75, "tc conv1 (uint8 kernel): K = %d, expected 75", K);
-  if (h->planes == 1)
-    pack_conv1_u8_weights_kernel<1><<<grid, 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8_hi, nullptr, range_flag, range_bit);
-  else
-    pack_conv1_u8_weights_kernel<<<(unsigned)ceil_div(h->N * 128, 256), 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8_hi, h->w8_lo, range_flag,
-                                                                                    range_bit);
+  with_planes(h->planes, [&](auto P) {
+    pack_conv1_u8_weights_kernel<P><<<grid, 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8.hi, h->w8.lo, range_flag, range_bit);
+  });
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -620,23 +587,24 @@ int tc_conv1_forward(TcConv1* h, const aae_net_cfg* cfg, const void* crops, int 
     // output tensor maps: [slot][128 channels] views of conv2's (hi, lo) input; the buffers hold max_batch crops, this call
     // may be shorter -- the maps cover exactly the slots this call writes
     const long long slots = (long long)p.num_tiles * 128;
-    if (h->bound_hi != out_hi || h->bound_lo != out_lo || h->slots != slots) {
+    const TcPlanes out{out_hi, out_lo};
+    if (h->bound.hi != out.hi || h->bound.lo != out.lo || h->slots != slots) {
       const uint64_t dims[2] = {128, (uint64_t)slots};
       const uint64_t strides[1] = {256};
       const uint32_t box32[2] = {32, 16};                   // one warp's 16 slots x 32 channels, 64-byte swizzle
-      AAE_TRY(make_tmap_f16(&h->tm_out32_hi, out_hi, 2, dims, strides, box32, 64));
-      if (h->planes == 2) AAE_TRY(make_tmap_f16(&h->tm_out32_lo, out_lo, 2, dims, strides, box32, 64));
-      h->bound_hi = out_hi; h->bound_lo = out_lo; h->slots = slots;
+      AAE_TRY(out.encode(h->tm_out32, 2, dims, strides, box32, 64));
+      h->bound = out; h->slots = slots;
     }
     p.unscale = 1.f / (w_scale * 256.f);              // accumulators hold sum u8 * (w * w_scale * 256 / 255)
-    if (h->planes == 1) tc_conv1_u8_kernel<1><<<grid, U8_THREADS, U8_SMEM_TOTAL, s>>>(h->tm8_hi, h->tm8_hi, h->tm_out32_hi, h->tm_out32_hi, p);
-    else tc_conv1_u8_kernel<<<grid, U8_THREADS, U8_SMEM_TOTAL, s>>>(h->tm8_hi, h->tm8_lo, h->tm_out32_hi, h->tm_out32_lo, p);
-  } else if (h->planes == 1) {
-    AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Conv1Smem::TOTAL));
-    tc_conv1_kernel<1><<<grid, C1_THREADS, Conv1Smem::TOTAL, s>>>(h->tm_hi, h->tm_hi, p);
+    with_planes(h->planes, [&](auto P) {
+      tc_conv1_u8_kernel<P><<<grid, U8_THREADS, U8_SMEM_TOTAL, s>>>(h->tm8.hi, h->tm8.lo, h->tm_out32.hi, h->tm_out32.lo, p);
+    });
   } else {
-    AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Conv1Smem::TOTAL));
-    tc_conv1_kernel<<<grid, C1_THREADS, Conv1Smem::TOTAL, s>>>(h->tm_hi, h->tm_lo, p);
+    AAE_TRY(with_planes(h->planes, [&](auto P) {
+      AAE_CUDA_OK(cudaFuncSetAttribute(tc_conv1_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, Conv1Smem::TOTAL));
+      tc_conv1_kernel<P><<<grid, C1_THREADS, Conv1Smem::TOTAL, s>>>(h->tm.hi, h->tm.lo, p);
+      return AAE_OK;
+    }));
   }
   AAE_LAUNCH_OK();
   return AAE_OK;

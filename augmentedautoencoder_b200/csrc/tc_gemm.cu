@@ -74,7 +74,7 @@ struct TcSmem {
 // Warp roles (384 threads): warp 0 TMA producer (warps 1-3 idle), warpgroups 1 and 2 (warps 4-11) issue the wgmma for pixel rows
 // [0,64) and [64,128) of the tile and then run the epilogue, two warps per 32-row quadrant.
 // Grid: x = N tile, y = M tile, z = K split (see tc_launch_layer).
-// PLANES = 2: (hi, lo) operands, three products per K step; PLANES = 1: hi operands only (tm_a_lo / tm_w_lo unused), one product.
+// PLANES = 2: (hi, lo) operands, three products per K step; PLANES = 1: hi operands only (the lo maps are not read), one product.
 template <int N_TILE, int STAGES, int PLANES = 2>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
@@ -95,18 +95,17 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
   const int it_end = min(total_iters, it_begin + p.iters_per_split);
 
   if (threadIdx.x == 0) {
-    if constexpr (PLANES == 1) {
-      prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_w_hi);
-    } else {
-      prefetch_tmap(&tm_a_hi); prefetch_tmap(&tm_a_lo); prefetch_tmap(&tm_w_hi); prefetch_tmap(&tm_w_lo);
-    }
+    prefetch_tmap(&tm_a_hi);
+    if constexpr (PLANES == 2) prefetch_tmap(&tm_a_lo);
+    prefetch_tmap(&tm_w_hi);
+    if constexpr (PLANES == 2) prefetch_tmap(&tm_w_lo);
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
   __syncthreads();
 
   if (warp == 0) {
-    // ===================== TMA producer =====================
+    // ===================== TMA producer: stage = [A_hi | A_lo | W_hi | W_lo], the lo boxes with PLANES = 2 only =====================
     if (lane == 0) {
       const int hw = p.OH * p.OW;
       const int b0 = m0 / hw, rem = m0 - b0 * hw;
@@ -121,59 +120,11 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
         const int c0 = p.tap_ch[tap] + cc * TC_KCH;
         const int x = ow0 + p.tap_dj[tap], y = oh0 + p.tap_di[tap];
         const int kcol = it * TC_KCH;
-        if constexpr (PLANES == 1) {                   // stage = [A_hi | W_hi]
-          tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
-          tma_load_2d(st + S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, n0);
-        } else {
-          tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
-          tma_load_4d(st + S::A_BYTES, &tm_a_lo, &full_bar[s], c0, x, y, b0);
-          tma_load_2d(st + 2 * S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, n0);
-          tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tm_w_lo, &full_bar[s], kcol, n0);
-        }
+        tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
+        if constexpr (PLANES == 2) tma_load_4d(st + S::A_BYTES, &tm_a_lo, &full_bar[s], c0, x, y, b0);
+        tma_load_2d(st + PLANES * S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, n0);
+        if constexpr (PLANES == 2) tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tm_w_lo, &full_bar[s], kcol, n0);
       }
-    }
-  } else if (warp >= 4 && PLANES == 1) {
-    // ===================== wgmma consumers + epilogue, single pass =====================
-    const int wg = (warp - 4) >> 2;
-    float acc[R];
-#pragma unroll
-    for (int j = 0; j < R; ++j) acc[j] = 0.f;
-    for (int it = it_begin, i = 0; it < it_end; ++it, ++i) {
-      const int s = i % STAGES;
-      mbar_wait(&full_bar[s], (uint32_t)(i / STAGES) & 1u);
-      const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
-      const uint64_t a_hi = make_sw128_kmajor_desc(st + (uint32_t)(wg * 64 * TC_KCH * 2));
-      const uint64_t w_hi = make_sw128_kmajor_desc(st + S::A_BYTES);
-      wgmma_fence_regs(acc);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < TC_KCH / 16; ++k)
-        Wgmma<N_TILE>::template ss<0, 0>(acc, desc_advance_k(a_hi, k), desc_advance_k(w_hi, k), (i > 0 || k > 0) ? 1u : 0u);
-      wgmma_commit();
-      wgmma_wait<1>();                                // the previous stage's MMAs have read their operands: free it
-      wgmma_fence_regs(acc);
-      if (i > 0 && (warp & 3) == 0 && lane == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
-    }
-    wgmma_wait<0>();
-    wgmma_fence_regs(acc);
-    named_bar_sync(1, 256);
-    float* img = reinterpret_cast<float*>(smem);
-    tc_park_acc(img, S::ACC_LD, wg, warp, lane, acc);
-    named_bar_sync(1, 256);
-    const int q = warp & 3, half = (warp - 4) >> 2;
-    const TcRow row = tc_decode_row(p, m0 + q * 32 + lane);
-    const bool has_work = it_end > it_begin;
-    const float unscale = p.amax_bits ? p.unscale * tc_dyn_unscale(__ldg(p.amax_bits)) : p.unscale;
-#pragma unroll 1
-    for (int c = half; c < N_TILE / 32; c += 2) {
-      const int n = n0 + c * 32;
-      if (!row.valid || n >= p.N) continue;
-      uint32_t v[32];
-      tc_acc_ld32(img, S::ACC_LD, q * 32 + lane, c * 32, v);
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = has_work ? __uint_as_float(v[j]) * unscale : 0.f;
-      tc_store_chunk<1>(p, row, n, f, (int)blockIdx.z);
     }
   } else if (warp >= 4) {
     // ===================== wgmma consumers =====================
@@ -188,9 +139,10 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
       const uint32_t a_off = (uint32_t)(wg * 64 * TC_KCH * 2);
       const uint64_t a_hi = make_sw128_kmajor_desc(st + a_off);
       const uint64_t a_lo = make_sw128_kmajor_desc(st + S::A_BYTES + a_off);
-      const uint64_t w_hi = make_sw128_kmajor_desc(st + 2 * S::A_BYTES);
+      const uint64_t w_hi = make_sw128_kmajor_desc(st + PLANES * S::A_BYTES);
       const uint64_t w_lo = make_sw128_kmajor_desc(st + 2 * S::A_BYTES + S::W_BYTES);
-      wgmma_fence_regs(acc); wgmma_fence_regs(crs);
+      wgmma_fence_regs(acc);
+      if constexpr (PLANES == 2) wgmma_fence_regs(crs);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < TC_KCH / 16; ++k) {
@@ -198,45 +150,33 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
         // accumulator of their own (small magnitude -> negligible truncation) and are folded in by the epilogue in RN fp32.
         const uint32_t first = (i > 0 || k > 0) ? 1u : 0u;
         Wgmma<N_TILE>::template ss<0, 0>(acc, desc_advance_k(a_hi, k), desc_advance_k(w_hi, k), first);
-        Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_lo, k), desc_advance_k(w_hi, k), first);
-        Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_hi, k), desc_advance_k(w_lo, k), 1u);
+        if constexpr (PLANES == 2) {
+          Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_lo, k), desc_advance_k(w_hi, k), first);
+          Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_hi, k), desc_advance_k(w_lo, k), 1u);
+        }
       }
       wgmma_commit();
       wgmma_wait<1>();                                // the previous stage's MMAs have read their operands: free it
-      wgmma_fence_regs(acc); wgmma_fence_regs(crs);
+      wgmma_fence_regs(acc);
+      if constexpr (PLANES == 2) wgmma_fence_regs(crs);
       if (i > 0 && (warp & 3) == 0 && lane == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
     }
     wgmma_wait<0>();
-    wgmma_fence_regs(acc); wgmma_fence_regs(crs);
+    wgmma_fence_regs(acc);
+    if constexpr (PLANES == 2) wgmma_fence_regs(crs);
     named_bar_sync(1, 256);                           // every MMA of both warpgroups is done: the ring becomes the accumulator image
     float* img = reinterpret_cast<float*>(smem);
-    tc_park_acc(img, S::ACC_LD, wg, warp, lane, acc, crs);
+    tc_park_acc<PLANES>(img, S::ACC_LD, wg, warp, lane, acc, crs);
     named_bar_sync(1, 256);
-    // ===================== epilogue =====================
-    const int q = warp & 3, half = (warp - 4) >> 2;   // two warps per 32-row quadrant, interleaved 32-column chunks
-    const TcRow row = tc_decode_row(p, m0 + q * 32 + lane);
-    const bool has_work = it_end > it_begin;
-    const float unscale = p.amax_bits ? p.unscale * tc_dyn_unscale(__ldg(p.amax_bits)) : p.unscale;
-#pragma unroll 1
-    for (int c = half; c < N_TILE / 32; c += 2) {
-      const int n = n0 + c * 32;
-      if (!row.valid || n >= p.N) continue;
-      uint32_t v[32], x[32];
-      tc_acc_ld32(img, S::ACC_LD, q * 32 + lane, c * 32, v);
-      tc_acc_ld32(img, S::ACC_LD, q * 32 + lane, N_TILE + c * 32, x);
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = has_work ? (__uint_as_float(v[j]) + __uint_as_float(x[j])) * unscale : 0.f;
-      tc_store_chunk(p, row, n, f, (int)blockIdx.z);
-    }
+    tc_epilogue<PLANES, N_TILE>(p, img, S::ACC_LD, m0, n0, it_end > it_begin, warp, lane);
   }
 }
 
 // ------------------------------------------------------------------------------------------------- packing kernels
 namespace {
 
-// W fp32 [taps][Cin][Cout] (HWIO flattened) -> Wp_{hi,lo} fp16 [Cout][taps*Cin], value scaled by `scale`; PLANES = 1 writes hi only
-template <int PLANES = 2>
+// W fp32 [taps][Cin][Cout] (HWIO flattened) -> Wp fp16 [Cout][taps*Cin] in the format PLANES, value scaled by `scale`
+template <int PLANES>
 __global__ void pack_weights_kernel(const float* __restrict__ w, int taps, int cin, int cout, float scale, __half* __restrict__ hi,
                                     __half* __restrict__ lo, unsigned* __restrict__ range_flag, unsigned range_bit) {
   __shared__ float tile[32][33];
@@ -249,21 +189,13 @@ __global__ void pack_weights_kernel(const float* __restrict__ w, int taps, int c
   __syncthreads();
   for (int i = threadIdx.y; i < 32; i += 8) {
     const int co = co0 + i, ci = ci0 + threadIdx.x;
-    if (co < cout && ci < cin) {
-      __half h, l;
-      const float v = tile[threadIdx.x][i] * scale;
-      if (range_flag != nullptr && !(fabsf(v) < TC_F16_OVERFLOW)) atomicOr(range_flag, range_bit);
-      split_f16(v, h, l);
-      const long long o = (long long)co * taps * cin + (long long)tap * cin + ci;
-      hi[o] = h;
-      if constexpr (PLANES == 2) lo[o] = l;
-    }
+    if (co < cout && ci < cin)
+      tc_store_f16<PLANES>(tile[threadIdx.x][i] * scale, hi, lo, (long long)co * taps * cin + (long long)tap * cin + ci, range_flag, range_bit);
   }
 }
 
-// (hi, lo) fp16 activations -> fp32 NHWC (undoing the space-to-depth layout and the scale); debug / test visibility only.
-// PLANES = 1: the hi plane alone (lo is not read).
-template <int PLANES = 2>
+// fp16 activations -> fp32 NHWC (undoing the space-to-depth layout and the scale); debug / test visibility only.
+template <int PLANES>
 __global__ void unpack_act_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, int B, int H, int W, int C, int s2d,
                                   float inv_scale, float* __restrict__ out) {
   const long long total = (long long)B * H * W * C;
@@ -275,8 +207,7 @@ __global__ void unpack_act_kernel(const __half* __restrict__ hi, const __half* _
     const int b = (int)(r / H);
     long long src = i;
     if (s2d) src = ((long long)(b * (H >> 1) + (h >> 1)) * (W >> 1) + (w >> 1)) * (4LL * C) + (((h & 1) << 1) | (w & 1)) * C + c;
-    if constexpr (PLANES == 1) out[i] = __half2float(hi[src]) * inv_scale;
-    else out[i] = (__half2float(hi[src]) + __half2float(lo[src])) * inv_scale;
+    out[i] = tc_load_f16<PLANES>(hi, lo, src) * inv_scale;
   }
 }
 
@@ -287,9 +218,8 @@ namespace {
 
 // Split-K forward of a conv layer at small batch: the GEMM leaves fp32 partial sums [splits][M][N] (OUT_F32); this kernel folds
 // them in a fixed order and applies the layer's real epilogue -- bias, ReLU, range guard, (hi, lo) split, store in the next
-// layer's layout (tc_store_chunk's OUT_S2D_SPLIT / OUT_PLAIN_SPLIT branch).  One thread per (row, 8 columns).  PLANES = 1
-// stores the hi plane only, rounded straight from fp32.
-template <int PLANES = 2>
+// layer's layout (tc_store_chunk's OUT_S2D_SPLIT / OUT_PLAIN_SPLIT branch).  One thread per (row, 8 columns).
+template <int PLANES>
 __global__ void __launch_bounds__(256) splitk_forward_finish_kernel(const float* __restrict__ partials, int splits, const TcGemmParams p) {
   const long long groups = (long long)p.M * (p.N >> 3);
   for (long long gi = (long long)blockIdx.x * blockDim.x + threadIdx.x; gi < groups; gi += (long long)gridDim.x * blockDim.x) {
@@ -309,22 +239,7 @@ __global__ void __launch_bounds__(256) splitk_forward_finish_kernel(const float*
       f[j] = v * p.out_scale;
     }
     if (p.range_flag != nullptr && !(amax * p.out_scale < TC_F16_OVERFLOW)) atomicOr(p.range_flag, p.range_bit);
-    const TcRow r = tc_decode_row(p, m);
-    if constexpr (PLANES == 1) {
-      uint32_t hi[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const __half2 h = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-        hi[j] = *reinterpret_cast<const uint32_t*>(&h);
-      }
-      *reinterpret_cast<uint4*>(p.out_hi + r.row_off + n) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    } else {
-      uint32_t hi[4], lo[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) split_f16x2(f[2 * j], f[2 * j + 1], hi[j], lo[j]);
-      *reinterpret_cast<uint4*>(p.out_hi + r.row_off + n) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-      *reinterpret_cast<uint4*>(p.out_lo + r.row_off + n) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-    }
+    tc_store_f16<PLANES>(f, 1.f, p.out_hi, p.out_lo, tc_decode_row(p, m).row_off + n);
   }
 }
 
@@ -341,6 +256,26 @@ int tc_dev_alloc(void** p, size_t bytes) {
   return AAE_OK;
 }
 
+int TcPlanes::alloc(size_t n, int planes) {
+  AAE_TRY(tc_dev_alloc((void**)&hi, n * sizeof(__half)));
+  return planes == 2 ? tc_dev_alloc((void**)&lo, n * sizeof(__half)) : AAE_OK;
+}
+
+void TcPlanes::release() {
+  cudaFree(hi);
+  cudaFree(lo);
+  hi = lo = nullptr;
+}
+
+int TcPlanes::encode(TcMaps& m, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes) const {
+  AAE_TRY(make_tmap_f16(&m.hi, hi, rank, dims, strides_bytes, box, swizzle_bytes));
+  if (lo == nullptr) {
+    m.lo = m.hi;
+    return AAE_OK;
+  }
+  return make_tmap_f16(&m.lo, lo, rank, dims, strides_bytes, box, swizzle_bytes);
+}
+
 // tiles = (m_tiles, n_tiles, splits).  The kernel runs the N tiles on grid.x, so the N tiles of an M tile are adjacent in launch
 // order and read the activation tile (and its 5 x 5 tap re-reads) while it is in L2; M first would put all resident CTAs on one
 // weight column and stream every activation tile from HBM once per N tile.
@@ -352,20 +287,15 @@ static_assert(TcSmem<TC_N_TILE, TC_STAGES_FP16, 1>::TOTAL == TcSmem<TC_N_TILE, T
 
 int tc_launch_layer(const TcLayer& T, dim3 tiles, cudaStream_t s, int planes) {
   AAE_REQUIRE(tiles.x <= 65535u, "tc_gemm: %u row tiles exceed the grid's y limit", tiles.x);
-  if (planes == 1) {
-    using S1 = TcSmem<TC_N_TILE, TC_STAGES_FP16, 1>;
-    auto kern1 = tc_gemm_kernel<TC_N_TILE, TC_STAGES_FP16, 1>;
-    AAE_CUDA_OK(cudaFuncSetAttribute(kern1, cudaFuncAttributeMaxDynamicSharedMemorySize, S1::TOTAL));
-    kern1<<<dim3(tiles.y, tiles.x, tiles.z), TC_THREADS, S1::TOTAL, s>>>(T.tm_a_hi, T.tm_a_hi, T.tm_w_hi, T.tm_w_hi, T.gp);
+  return with_planes(planes, [&](auto P) {
+    constexpr int STAGES = P == 1 ? TC_STAGES_FP16 : TC_STAGES_SPLIT;
+    using S = TcSmem<TC_N_TILE, STAGES, P>;
+    auto kern = tc_gemm_kernel<TC_N_TILE, STAGES, P>;
+    AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+    kern<<<dim3(tiles.y, tiles.x, tiles.z), TC_THREADS, S::TOTAL, s>>>(T.tm_a.hi, T.tm_a.lo, T.tm_w.hi, T.tm_w.lo, T.gp);
     AAE_LAUNCH_OK();
     return AAE_OK;
-  }
-  using S = TcSmem<TC_N_TILE, TC_STAGES_SPLIT>;
-  auto kern = tc_gemm_kernel<TC_N_TILE, TC_STAGES_SPLIT>;
-  AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-  kern<<<dim3(tiles.y, tiles.x, tiles.z), TC_THREADS, S::TOTAL, s>>>(T.tm_a_hi, T.tm_a_lo, T.tm_w_hi, T.tm_w_lo, T.gp);
-  AAE_LAUNCH_OK();
-  return AAE_OK;
+  });
 }
 
 int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
@@ -373,15 +303,15 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
   const int L = cfg->num_layers;
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   AAE_REQUIRE(L >= 2, "AAE_PREC_TC_SPLIT: at least two conv layers expected");
-  const bool fp16 = cfg->precision == AAE_PREC_TC_FP16;
-  if (fp16 && !tc_conv1_supported(cfg)) {   // the fp32 CUDA-core conv1 behind the split plan writes (hi, lo) pairs only
+  const int planes = tc_planes(cfg->precision);
+  if (planes == 1 && !tc_conv1_supported(cfg)) {   // the fp32 CUDA-core conv1 behind the split plan writes (hi, lo) pairs only
     set_error("AAE_PREC_TC_FP16: the first layer needs the tensor-core conv1 (128 x 128 x 3 crops, 128 filters, k = 5, stride 2)");
     return AAE_ERR_UNSUPPORTED;
   }
   TcEncoder* h = new TcEncoder();
   h->device = device;
   h->cfg = *cfg;
-  h->planes = fp16 ? 1 : 2;
+  h->planes = planes;
   int ih = (cfg->in_h + cfg->strides[0] - 1) / cfg->strides[0], iw = (cfg->in_w + cfg->strides[0] - 1) / cfg->strides[0], ic = cfg->filters[0];
   const int B = cfg->max_batch;
   int st = AAE_OK;
@@ -411,34 +341,27 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
     }
     // batch dimension padded to a whole number of TMA boxes, so a tile never addresses rows outside the tensor map
     const int B_pad = (int)ceil_div(B, T.BB) * T.BB;
-    const size_t act_alloc = (size_t)B_pad * T.in_h * T.in_w * T.in_c;
-    if ((st = dev_alloc((void**)&T.in_hi, act_alloc * sizeof(__half))) != AAE_OK) break;
-    if (!fp16 && (st = dev_alloc((void**)&T.in_lo, act_alloc * sizeof(__half))) != AAE_OK) break;
-    const size_t w_elems = (size_t)T.out_c * T.taps * T.in_c;
-    if ((st = dev_alloc((void**)&T.w_hi, w_elems * sizeof(__half))) != AAE_OK) break;
-    if (!fp16 && (st = dev_alloc((void**)&T.w_lo, w_elems * sizeof(__half))) != AAE_OK) break;
+    if ((st = T.in.alloc((size_t)B_pad * T.in_h * T.in_w * T.in_c, planes)) != AAE_OK) break;
+    if ((st = T.w.alloc((size_t)T.out_c * T.taps * T.in_c, planes)) != AAE_OK) break;
     // ---- tensor maps ----
     if (!dense) {
       const uint64_t C4 = 4ull * T.in_c, W2 = T.in_w / 2, H2 = T.in_h / 2;
       const uint64_t dims[4] = {C4, W2, H2, (uint64_t)B_pad};
       const uint64_t strides[3] = {C4 * 2, W2 * C4 * 2, H2 * W2 * C4 * 2};
       const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
-      if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box)) != AAE_OK) break;
-      if (!fp16 && (st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) break;
+      if ((st = T.in.encode(T.tm_a, 4, dims, strides, box)) != AAE_OK) break;
     } else {
       const uint64_t dims[4] = {(uint64_t)T.in_c, 1, 1, (uint64_t)B_pad};
       const uint64_t strides[3] = {(uint64_t)T.in_c * 2, (uint64_t)T.in_c * 2, (uint64_t)T.in_c * 2};
       const uint32_t box[4] = {(uint32_t)TC_KCH, 1, 1, 128};
-      if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box)) != AAE_OK) break;
-      if (!fp16 && (st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) break;
+      if ((st = T.in.encode(T.tm_a, 4, dims, strides, box)) != AAE_OK) break;
     }
     {
       const uint64_t K = (uint64_t)T.taps * T.in_c;
       const uint64_t dims[2] = {K, (uint64_t)T.out_c};
       const uint64_t strides[1] = {K * 2};
       const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)std::min(TC_N_TILE, T.out_c)};
-      if ((st = make_tmap_f16(&T.tm_w_hi, T.w_hi, 2, dims, strides, box)) != AAE_OK) break;
-      if (!fp16 && (st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box)) != AAE_OK) break;
+      if ((st = T.w.encode(T.tm_w, 2, dims, strides, box)) != AAE_OK) break;
     }
     // ---- static GEMM parameters ----
     TcGemmParams& g = T.gp;
@@ -463,8 +386,8 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
     // wire outputs: layer i writes the input buffers of layer i+1; the last conv writes plain NHWC (the flatten order)
     for (size_t i = 0; i + 1 < h->layers.size(); ++i) {
       TcGemmParams& g = h->layers[i].gp;
-      g.out_hi = h->layers[i + 1].in_hi;
-      g.out_lo = h->layers[i + 1].in_lo;
+      g.out_hi = h->layers[i + 1].in.hi;
+      g.out_lo = h->layers[i + 1].in.lo;
       g.out_mode = (i + 2 == h->layers.size()) ? OUT_PLAIN_SPLIT : OUT_S2D_SPLIT;
     }
     TcLayer& D = h->layers.back();
@@ -490,7 +413,7 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
 
 void tc_encoder_destroy(TcEncoder* h) {
   if (!h) return;
-  for (auto& T : h->layers) { cudaFree(T.in_hi); cudaFree(T.in_lo); cudaFree(T.w_hi); cudaFree(T.w_lo); }
+  for (auto& T : h->layers) { T.in.release(); T.w.release(); }
   cudaFree(h->partials);
   cudaFree(h->fwd_partials);
   cudaFree(h->dbg);
@@ -507,8 +430,9 @@ int tc_encoder_pack_weights(TcEncoder* h, int layer, const float* w_dev, cudaStr
   AAE_REQUIRE(layer >= 1 && layer <= (int)h->layers.size(), "tc pack: layer %d out of range", layer);
   TcLayer& T = h->layers[layer - 1];
   dim3 grid((unsigned)ceil_div(T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), (unsigned)T.taps), block(32, 8);
-  if (h->planes == 1) pack_weights_kernel<1><<<grid, block, 0, s>>>(w_dev, T.taps, T.in_c, T.out_c, W_SCALE, T.w_hi, nullptr, h->range_flag, 1u << (16 + layer));
-  else pack_weights_kernel<<<grid, block, 0, s>>>(w_dev, T.taps, T.in_c, T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, 1u << (16 + layer));
+  with_planes(h->planes, [&](auto P) {
+    pack_weights_kernel<P><<<grid, block, 0, s>>>(w_dev, T.taps, T.in_c, T.out_c, W_SCALE, T.w.hi, T.w.lo, h->range_flag, 1u << (16 + layer));
+  });
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -536,7 +460,7 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
   timer->reset();
   timer->mark(s);
   if (h->conv1) {
-    AAE_TRY(tc_conv1_forward(h->conv1, &cfg, crops, src_u8, B, b0, ACT_SCALE, W_SCALE, h->layers[0].in_hi, h->layers[0].in_lo, h->range_flag, s));
+    AAE_TRY(tc_conv1_forward(h->conv1, &cfg, crops, src_u8, B, b0, ACT_SCALE, W_SCALE, h->layers[0].in.hi, h->layers[0].in.lo, h->range_flag, s));
   } else {  // conv1 (Cin = 3, K = 75): fp32 SIMT implicit GEMM, epilogue writes conv2's space-to-depth (hi, lo) input directly
     IGemmParams p;
     memset(&p, 0, sizeof(p));
@@ -549,7 +473,7 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
     p.Bm = w0; p.N = cfg.filters[0]; p.bias = b0; p.act = ACT_RELU;
     p.M = B * p.PH * p.PW; p.K = p.KH * p.KW * p.SC;
     p.k_per_split = (int)ceil_div(p.K, 16) * 16;
-    p.split_hi = h->layers[0].in_hi; p.split_lo = h->layers[0].in_lo; p.split_scale = ACT_SCALE; p.split_s2d = 1;
+    p.split_hi = h->layers[0].in.hi; p.split_lo = h->layers[0].in.lo; p.split_scale = ACT_SCALE; p.split_s2d = 1;
     AAE_TRY(launch_igemm(p, GATHER_FWD, s));
   }
   timer->mark(s);
@@ -590,8 +514,7 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
       AAE_TRY(tc_launch_layer(S, grid, s, h->planes));
       const long long groups = (long long)T.gp.M * (T.gp.N >> 3);
       const unsigned fin_grid = (unsigned)std::min<long long>(132 * 8, ceil_div(groups, 256));
-      if (h->planes == 1) splitk_forward_finish_kernel<1><<<fin_grid, 256, 0, s>>>(h->fwd_partials, splits, T.gp);
-      else splitk_forward_finish_kernel<<<fin_grid, 256, 0, s>>>(h->fwd_partials, splits, T.gp);
+      with_planes(h->planes, [&](auto P) { splitk_forward_finish_kernel<P><<<fin_grid, 256, 0, s>>>(h->fwd_partials, splits, T.gp); });
       AAE_LAUNCH_OK();
     } else {
       AAE_TRY(tc_launch_layer(T, grid, s, h->planes));
@@ -622,8 +545,9 @@ int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int
     AAE_TRY(dev_alloc((void**)&h->dbg, n * sizeof(float)));
     h->dbg_floats = n;
   }
-  if (h->planes == 1) unpack_act_kernel<1><<<1024, 256, 0, s>>>(T.in_hi, nullptr, B, H, W, C, plain ? 0 : 1, 1.f / ACT_SCALE, h->dbg);
-  else unpack_act_kernel<<<1024, 256, 0, s>>>(T.in_hi, T.in_lo, B, H, W, C, plain ? 0 : 1, 1.f / ACT_SCALE, h->dbg);
+  with_planes(h->planes, [&](auto P) {
+    unpack_act_kernel<P><<<1024, 256, 0, s>>>(T.in.hi, T.in.lo, B, H, W, C, plain ? 0 : 1, 1.f / ACT_SCALE, h->dbg);
+  });
   AAE_LAUNCH_OK();
   AAE_CUDA_OK(cudaStreamSynchronize(s));
   *ptr = h->dbg;
@@ -643,32 +567,22 @@ int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int
 // refuse AAE_PREC_TC_FP16 for the decoder.
 namespace {
 
-template <int PLANES = 2>
+template <int PLANES>
 __global__ void split_scale_kernel(const float* __restrict__ x, long long n, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
                                    unsigned* __restrict__ range_flag, unsigned range_bit) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    __half h, l;
-    if (range_flag != nullptr && !(fabsf(x[i] * scale) < TC_F16_OVERFLOW)) atomicOr(range_flag, range_bit);
-    split_f16(x[i] * scale, h, l);
-    hi[i] = h;
-    if constexpr (PLANES == 2) lo[i] = l;
-  }
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    tc_store_f16<PLANES>(x[i] * scale, hi, lo, i, range_flag, range_bit);
 }
 
 // merged weights Wm [9][cin][n4] -> operand of the tap-separable output layer: row (tap * n4 + m) = Wm[tap][:, m], rows >= 9*n4 zero
-template <int PLANES = 2>
+template <int PLANES>
 __global__ void pack_out_sep_kernel(const float* __restrict__ wm, int cin, int n4, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
                                     unsigned* __restrict__ range_flag, unsigned range_bit) {
   const int total = 128 * cin;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int ci = i % cin, n = i / cin;
     const int tap = n / n4, m = n - tap * n4;
-    const float v = tap < 9 ? wm[((long long)tap * cin + ci) * n4 + m] * scale : 0.f;
-    if (range_flag != nullptr && !(fabsf(v) < TC_F16_OVERFLOW)) atomicOr(range_flag, range_bit);
-    __half a, d;
-    split_f16(v, a, d);
-    hi[i] = a;
-    if constexpr (PLANES == 2) lo[i] = d;
+    tc_store_f16<PLANES>(tap < 9 ? wm[((long long)tap * cin + ci) * n4 + m] * scale : 0.f, hi, lo, i, range_flag, range_bit);
   }
 }
 
@@ -707,34 +621,22 @@ __global__ void tile_bias_kernel(const float* __restrict__ b, int cout, float* _
 
 }  // namespace
 
-int tc_layer_setup_plain(TcLayer& T, int B, bool alloc_input, int planes) {
-  int st;
-  const bool two = planes == 2;
+int tc_layer_setup_plain(TcLayer& T, int B, int planes) {
   const int B_pad = (int)ceil_div(B, T.BB) * T.BB;
-  const size_t act = (size_t)B_pad * T.in_h * T.in_w * T.in_c;
-  if (alloc_input) {
-    if ((st = dev_alloc((void**)&T.in_hi, act * sizeof(__half))) != AAE_OK) return st;
-    if (two && (st = dev_alloc((void**)&T.in_lo, act * sizeof(__half))) != AAE_OK) return st;
-  }
   const uint64_t K = (uint64_t)T.taps * T.in_c;
   const int rows = (int)ceil_div(T.gp.N, TC_N_TILE) * TC_N_TILE;
-  if ((st = dev_alloc((void**)&T.w_hi, (size_t)rows * K * sizeof(__half))) != AAE_OK) return st;
-  if (two && (st = dev_alloc((void**)&T.w_lo, (size_t)rows * K * sizeof(__half))) != AAE_OK) return st;
+  AAE_TRY(T.in.alloc((size_t)B_pad * T.in_h * T.in_w * T.in_c, planes));
+  AAE_TRY(T.w.alloc((size_t)rows * K, planes));
   {
     const uint64_t dims[4] = {(uint64_t)T.in_c, (uint64_t)T.in_w, (uint64_t)T.in_h, (uint64_t)B_pad};
     const uint64_t strides[3] = {(uint64_t)T.in_c * 2, (uint64_t)T.in_w * T.in_c * 2, (uint64_t)T.in_h * T.in_w * T.in_c * 2};
     const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
-    if ((st = make_tmap_f16(&T.tm_a_hi, T.in_hi, 4, dims, strides, box)) != AAE_OK) return st;
-    if (two && (st = make_tmap_f16(&T.tm_a_lo, T.in_lo, 4, dims, strides, box)) != AAE_OK) return st;
+    AAE_TRY(T.in.encode(T.tm_a, 4, dims, strides, box));
   }
-  {
-    const uint64_t dims[2] = {K, (uint64_t)rows};
-    const uint64_t strides[1] = {K * 2};
-    const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)TC_N_TILE};
-    if ((st = make_tmap_f16(&T.tm_w_hi, T.w_hi, 2, dims, strides, box)) != AAE_OK) return st;
-    if (two && (st = make_tmap_f16(&T.tm_w_lo, T.w_lo, 2, dims, strides, box)) != AAE_OK) return st;
-  }
-  return AAE_OK;
+  const uint64_t dims[2] = {K, (uint64_t)rows};
+  const uint64_t strides[1] = {K * 2};
+  const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)TC_N_TILE};
+  return T.w.encode(T.tm_w, 2, dims, strides, box);
 }
 
 int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
@@ -745,7 +647,7 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
   TcDecoder* h = new TcDecoder();
   h->device = device;
   h->cfg = *cfg;
-  h->planes = cfg->precision == AAE_PREC_TC_FP16 ? 1 : 2;
+  h->planes = tc_planes(cfg->precision);
   const int B = cfg->max_batch;
   int h0 = cfg->in_h;
   for (int i = 0; i < L; ++i) h0 /= 2;
@@ -792,7 +694,7 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
     }
     g.unscale = 1.f / (ACT_SCALE * W_SCALE);
     g.out_scale = ACT_SCALE;
-    if ((st = tc_layer_setup_plain(T, B, /*alloc_input=*/true, h->planes)) != AAE_OK) { h->layers.push_back(T); break; }
+    if ((st = tc_layer_setup_plain(T, B, h->planes)) != AAE_OK) { h->layers.push_back(T); break; }
     h->layers.push_back(T);
     float* bz = nullptr;
     if (l > 0 && l < L) st = dev_alloc((void**)&bz, (size_t)g.N * sizeof(float));
@@ -803,8 +705,8 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
   if (st == AAE_OK) st = dev_alloc((void**)&h->range_flag, sizeof(unsigned));
   if (st == AAE_OK) {
     for (size_t i = 0; i + 1 < h->layers.size(); ++i) {
-      h->layers[i].gp.out_hi = h->layers[i + 1].in_hi;
-      h->layers[i].gp.out_lo = h->layers[i + 1].in_lo;
+      h->layers[i].gp.out_hi = h->layers[i + 1].in.hi;
+      h->layers[i].gp.out_lo = h->layers[i + 1].in.lo;
       h->layers[i].gp.range_flag = h->range_flag;       // bit i: the activation written by layer i (0 = dense_1)
       h->layers[i].gp.range_bit = 1u << i;
     }
@@ -816,7 +718,7 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
 
 void tc_decoder_destroy(TcDecoder* h) {
   if (!h) return;
-  for (auto& T : h->layers) { cudaFree(T.in_hi); cudaFree(T.in_lo); cudaFree(T.w_hi); cudaFree(T.w_lo); }
+  for (auto& T : h->layers) { T.in.release(); T.w.release(); }
   for (auto b : h->bias_dev) cudaFree(b);
   cudaFree(h->wm_tmp);
   cudaFree(h->out_p);
@@ -832,8 +734,9 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
   if (layer == 0) {
     if (w_dev) {
       dim3 grid((unsigned)ceil_div(T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), 1);
-      if (h->planes == 1) pack_weights_kernel<1><<<grid, block, 0, s>>>(w_dev, 1, T.in_c, T.out_c, W_SCALE, T.w_hi, nullptr, h->range_flag, 1u << 16);
-      else pack_weights_kernel<<<grid, block, 0, s>>>(w_dev, 1, T.in_c, T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, 1u << 16);
+      with_planes(h->planes, [&](auto P) {
+        pack_weights_kernel<P><<<grid, block, 0, s>>>(w_dev, 1, T.in_c, T.out_c, W_SCALE, T.w.hi, T.w.lo, h->range_flag, 1u << 16);
+      });
       AAE_LAUNCH_OK();
     }
     if (b_dev) T.gp.bias = b_dev;      // device pointer owned by the decoder handle
@@ -844,13 +747,10 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
     AAE_TRY(launch_merge_subpixel_weights(w_dev, T.in_c, T.out_c, h->wm_tmp, s));
     const unsigned bit = 1u << (16 + layer);
     dim3 grid((unsigned)ceil_div(4 * T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), 9);
-    if (h->planes == 1) {
-      if (out_layer) pack_out_sep_kernel<1><<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, nullptr, h->range_flag, bit);
-      else pack_weights_kernel<1><<<grid, block, 0, s>>>(h->wm_tmp, 9, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, nullptr, h->range_flag, bit);
-    } else {
-      if (out_layer) pack_out_sep_kernel<<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, bit);
-      else pack_weights_kernel<<<grid, block, 0, s>>>(h->wm_tmp, 9, T.in_c, 4 * T.out_c, W_SCALE, T.w_hi, T.w_lo, h->range_flag, bit);
-    }
+    with_planes(h->planes, [&](auto P) {
+      if (out_layer) pack_out_sep_kernel<P><<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, W_SCALE, T.w.hi, T.w.lo, h->range_flag, bit);
+      else pack_weights_kernel<P><<<grid, block, 0, s>>>(h->wm_tmp, 9, T.in_c, 4 * T.out_c, W_SCALE, T.w.hi, T.w.lo, h->range_flag, bit);
+    });
     AAE_LAUNCH_OK();
   }
   if (out_layer) {
@@ -870,8 +770,9 @@ const float* tc_decoder_merged_weights(const TcDecoder* h) { return h->wm_tmp; }
 int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, cudaStream_t s) {
   TcLayer& D = h->layers[0];
   const unsigned grid = (unsigned)std::min<int64_t>(1024, ceil_div((int64_t)B * D.in_c, 256));
-  if (h->planes == 1) split_scale_kernel<1><<<grid, 256, 0, s>>>(z_dev, (long long)B * D.in_c, ACT_SCALE, D.in_hi, nullptr, h->range_flag, 1u << 15);
-  else split_scale_kernel<<<grid, 256, 0, s>>>(z_dev, (long long)B * D.in_c, ACT_SCALE, D.in_hi, D.in_lo, h->range_flag, 1u << 15);
+  with_planes(h->planes, [&](auto P) {
+    split_scale_kernel<P><<<grid, 256, 0, s>>>(z_dev, (long long)B * D.in_c, ACT_SCALE, D.in.hi, D.in.lo, h->range_flag, 1u << 15);
+  });
   AAE_LAUNCH_OK();
   for (size_t i = 0; i < h->layers.size(); ++i) {
     TcLayer& T = h->layers[i];

@@ -15,6 +15,7 @@
 
 #include "tc.cuh"
 #include "tc_common.cuh"
+#include "tc_plan.cuh"
 
 namespace aae {
 
@@ -176,20 +177,8 @@ tc_match_kernel(const __grid_constant__ CUtensorMap tm_e_hi, const __grid_consta
       for (int g = 0; g < 8; ++g) {                    // 8 K elements = one 16-byte chunk of the row
         const float4 a = mine[2 * g], b = mine[2 * g + 1];
         const int off = (g ^ (r & 7)) << 4;
-        if constexpr (PLANES == 1) {
-          const __half2 h0 = __floats2half2_rn(a.x * inv, a.y * inv), h1 = __floats2half2_rn(a.z * inv, a.w * inv);
-          const __half2 h2 = __floats2half2_rn(b.x * inv, b.y * inv), h3 = __floats2half2_rn(b.z * inv, b.w * inv);
-          *reinterpret_cast<uint4*>(qh + off) = make_uint4(*reinterpret_cast<const uint32_t*>(&h0), *reinterpret_cast<const uint32_t*>(&h1),
-                                                           *reinterpret_cast<const uint32_t*>(&h2), *reinterpret_cast<const uint32_t*>(&h3));
-        } else {
-          uint32_t hi[4], lo[4];
-          split_f16x2(a.x * inv, a.y * inv, hi[0], lo[0]);
-          split_f16x2(a.z * inv, a.w * inv, hi[1], lo[1]);
-          split_f16x2(b.x * inv, b.y * inv, hi[2], lo[2]);
-          split_f16x2(b.z * inv, b.w * inv, hi[3], lo[3]);
-          *reinterpret_cast<uint4*>(qh + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-          *reinterpret_cast<uint4*>(qh + 2 * MT_E_BYTES + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-        }
+        const float v[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+        tc_store_f16<PLANES>(v, inv, reinterpret_cast<__half*>(qh + off), reinterpret_cast<__half*>(qh + 2 * MT_E_BYTES + off), 0);
       }
       fence_proxy_async_smem();                        // generic-proxy writes -> visible to wgmma
       named_bar_sync(1, 256);
@@ -332,17 +321,13 @@ __global__ void __launch_bounds__(MT_THREADS, 1) launch_floor_kernel(unsigned in
   if (sink != nullptr && threadIdx.x == 0 && smem_raw[0] == 0xFF && blockIdx.x == 0xFFFFFFFFu) *sink = 1u;   // never true: keeps smem_raw referenced
 }
 
-// fp32 [n_rows][128] -> (hi, lo) fp16 [n_pad][128], scaled by 64; rows >= n_rows are zero.  PLANES = 1 writes hi only.
-template <int PLANES = 2>
+// fp32 [n_rows][128] -> fp16 [n_pad][128] (format PLANES), scaled by 64; rows >= n_rows are zero.
+template <int PLANES>
 __global__ void pack_codebook_kernel(const float* __restrict__ E, long long n_rows, long long n_pad, __half* __restrict__ hi,
                                      __half* __restrict__ lo) {
   const long long total = n_pad * 128;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const float x = (i / 128 < n_rows) ? E[i] * MT_SCALE : 0.f;
-    __half h, l;
-    split_f16(x, h, l);
-    hi[i] = h;
-    if constexpr (PLANES == 2) lo[i] = l;
+    tc_store_f16<PLANES>((i / 128 < n_rows) ? E[i] * MT_SCALE : 0.f, hi, lo, i);
   }
 }
 
@@ -354,9 +339,9 @@ struct TcCodebook {
   int n_tiles, max_batch, sm_count, num_cyclo;
   long long n_up;                 // rows of the `upright` view (every num_cyclo-th row)
   int n_tiles_up;
-  int planes;                     // 2: (hi, lo) codebook (AAE_PREC_TC_SPLIT); 1: hi only (AAE_PREC_TC_FP16), e_lo not allocated
-  __half *e_hi = nullptr, *e_lo = nullptr;
-  CUtensorMap tm_hi, tm_lo, tm_hi_up, tm_lo_up;
+  int planes;                     // 2: (hi, lo) codebook (AAE_PREC_TC_SPLIT); 1: hi only (AAE_PREC_TC_FP16), no lo plane
+  TcPlanes e;
+  TcMaps tm, tm_up;
   bool have_up = false;
   unsigned long long* best = nullptr;
   unsigned long long* lists = nullptr;   // [grid][max_batch][8] packed keys of the per-CTA top-k lists (k > 1)
@@ -400,42 +385,35 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
   cudaGetDeviceProperties(&prop, device);
   h->sm_count = std::min(prop.multiProcessorCount, MT_MAX_GRID);
   const int cap_b = std::min(MT_BATCH, std::max(1, max_batch));
-  cudaError_t e = cudaMalloc(&h->e_hi, (size_t)h->n_pad * 128 * sizeof(__half));
-  if (e == cudaSuccess && planes == 2) e = cudaMalloc(&h->e_lo, (size_t)h->n_pad * 128 * sizeof(__half));
-  if (e == cudaSuccess) e = cudaMalloc(&h->best, 256 * sizeof(unsigned long long));
+  if (int st = h->e.alloc((size_t)h->n_pad * 128, planes)) { tc_codebook_destroy(h); return st; }
+  cudaError_t e = cudaMalloc(&h->best, 256 * sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaMalloc(&h->lists, (size_t)h->sm_count * cap_b * MT_KMAX * sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaMalloc(&h->counter, sizeof(unsigned int));
   if (e != cudaSuccess) { set_error("tc codebook alloc failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_OOM; }
   cudaMemset(h->best, 0, 256 * sizeof(unsigned long long));
   cudaMemset(h->counter, 0, sizeof(unsigned int));
-  if (planes == 1) pack_codebook_kernel<1><<<1024, 256>>>(E_dev, n_rows, h->n_pad, h->e_hi, nullptr);
-  else pack_codebook_kernel<<<1024, 256>>>(E_dev, n_rows, h->n_pad, h->e_hi, h->e_lo);
+  with_planes(planes, [&](auto P) { pack_codebook_kernel<P><<<1024, 256>>>(E_dev, n_rows, h->n_pad, h->e.hi, h->e.lo); });
   g_launches.fetch_add(1);
   e = cudaDeviceSynchronize();
   if (e != cudaSuccess) { set_error("pack_codebook failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_CUDA; }
   const uint64_t dims[2] = {128, (uint64_t)h->n_pad};
   const uint64_t strides[1] = {256};
   const uint32_t box[2] = {64, MT_ROWS};
-  int st = make_tmap_f16(&h->tm_hi, h->e_hi, 2, dims, strides, box);
-  if (st == AAE_OK && planes == 2) st = make_tmap_f16(&h->tm_lo, h->e_lo, 2, dims, strides, box);
+  int st = h->e.encode(h->tm, 2, dims, strides, box);
   if (st == AAE_OK && h->num_cyclo > 1) {
     // `upright` view (codebook.py:66 cos[::num_cyclo]): the same memory with a row stride of num_cyclo rows; boxes past
     // the last such row are zero-filled by TMA and masked by the kernel
     const uint64_t dims_u[2] = {128, (uint64_t)h->n_up};
     const uint64_t strides_u[1] = {(uint64_t)256 * (uint64_t)h->num_cyclo};
-    st = make_tmap_f16(&h->tm_hi_up, h->e_hi, 2, dims_u, strides_u, box);
-    if (st == AAE_OK && planes == 2) st = make_tmap_f16(&h->tm_lo_up, h->e_lo, 2, dims_u, strides_u, box);
+    st = h->e.encode(h->tm_up, 2, dims_u, strides_u, box);
     h->have_up = st == AAE_OK;
   }
   if (st != AAE_OK) { tc_codebook_destroy(h); return st; }
   auto attr = [&](const void* fn) { return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MT_SMEM_TOTAL); };
-  if (planes == 1) {
-    e = attr((const void*)tc_match_kernel<1, 1>);
-    if (e == cudaSuccess) e = attr((const void*)tc_match_kernel<MT_KMAX, 1>);
-  } else {
-    e = attr((const void*)tc_match_kernel<1>);
-    if (e == cudaSuccess) e = attr((const void*)tc_match_kernel<MT_KMAX>);
-  }
+  e = with_planes(planes, [&](auto P) {
+    const cudaError_t e1 = attr((const void*)tc_match_kernel<1, P>);
+    return e1 == cudaSuccess ? attr((const void*)tc_match_kernel<MT_KMAX, P>) : e1;
+  });
   if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(match kernels) failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_CUDA; }
   *out = h;
   return AAE_OK;
@@ -443,7 +421,8 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
 
 void tc_codebook_destroy(TcCodebook* h) {
   if (!h) return;
-  cudaFree(h->e_hi); cudaFree(h->e_lo); cudaFree(h->best); cudaFree(h->lists); cudaFree(h->counter);
+  h->e.release();
+  cudaFree(h->best); cudaFree(h->lists); cudaFree(h->counter);
   delete h;
 }
 
@@ -458,19 +437,17 @@ int tc_codebook_match(TcCodebook* h, const float* z_dev, int B, int64_t row_offs
   const int n_tiles = up ? h->n_tiles_up : h->n_tiles;
   const int n_rows = (int)(up ? h->n_up : h->n_rows);
   const int idx_mul = up ? h->num_cyclo : 1;
-  const CUtensorMap& th = up ? h->tm_hi_up : h->tm_hi;
-  const CUtensorMap& tl = up ? h->tm_lo_up : h->tm_lo;
+  const TcMaps& tm = up ? h->tm_up : h->tm;
   const int grid = std::min(h->sm_count, n_tiles);
   for (int a = 0; a < B; a += MT_BATCH) {
     const int nb = std::min(MT_BATCH, B - a);
     const float* z = z_dev + (size_t)a * 128;
     float* so = scores_out + (size_t)a * k;
     int32_t* io = idx_out + (size_t)a * k;
-    if (h->planes == 1) {
-      if (k == 1) tc_match_kernel<1, 1><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, th, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, 1, h->best, h->lists, h->counter, so, io);
-      else tc_match_kernel<MT_KMAX, 1><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, th, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best, h->lists, h->counter, so, io);
-    } else if (k == 1) tc_match_kernel<1><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, 1, h->best, h->lists, h->counter, so, io);
-    else tc_match_kernel<MT_KMAX><<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(th, tl, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best, h->lists, h->counter, so, io);
+    with_planes(h->planes, [&](auto P) {
+      auto kern = k == 1 ? tc_match_kernel<1, P> : tc_match_kernel<MT_KMAX, P>;
+      kern<<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(tm.hi, tm.lo, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best, h->lists, h->counter, so, io);
+    });
     AAE_LAUNCH_OK();
   }
   return AAE_OK;

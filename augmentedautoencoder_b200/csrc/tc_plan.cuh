@@ -3,6 +3,7 @@
 #pragma once
 #include <stdlib.h>
 
+#include <type_traits>
 #include <vector>
 
 #include "tc.cuh"
@@ -62,12 +63,36 @@ constexpr int TC_THREADS = 384;       // warp 0 TMA, 1-3 idle, warpgroups 1-2 (w
 constexpr int TC_N_TILE = 128;        // output channels per GEMM tile
 constexpr int TC_KCH = 64;            // K chunk per pipeline stage: 64 fp16 = one 128-byte swizzle row
 
+// Tensor maps of both planes of an operand.  Without a lo plane, lo is a copy of hi: the kernels never read it, and every launch
+// passes the pair as it is.
+struct TcMaps {
+  CUtensorMap hi, lo;
+};
+
+// An fp16 operand tensor in the plan's format: hi always, lo only for (hi, lo) split operands (planes = 2).
+struct TcPlanes {
+  __half* hi = nullptr;
+  __half* lo = nullptr;
+  // n zero-filled elements per plane
+  int alloc(size_t n, int planes);
+  void release();
+  // the same map for each plane that exists (make_tmap_f16 arguments)
+  int encode(TcMaps& m, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes = 128) const;
+};
+
+// Runs f(std::integral_constant<int, P>{}) with P = planes (1 or 2): the one place a plan's run-time plane count becomes a kernel's
+// PLANES template argument.
+template <class F>
+auto with_planes(int planes, F&& f) {
+  return planes == 1 ? f(std::integral_constant<int, 1>{}) : f(std::integral_constant<int, 2>{});
+}
+
 struct TcLayer {
   int in_h, in_w, in_c, out_h, out_w, out_c;   // conv geometry (input is the space-to-depth tensor [B, in_h/2, in_w/2, 4*in_c])
   int taps, BW, BH, BB;
-  __half *in_hi = nullptr, *in_lo = nullptr;    // activations entering this layer
-  __half *w_hi = nullptr, *w_lo = nullptr;      // packed weights [out_c][taps*in_c]
-  CUtensorMap tm_a_hi, tm_a_lo, tm_w_hi, tm_w_lo;
+  TcPlanes in;                                  // activations entering this layer
+  TcPlanes w;                                   // packed weights [out_c][taps*in_c]
+  TcMaps tm_a, tm_w;
   TcGemmParams gp;
 };
 
@@ -134,9 +159,65 @@ __device__ __forceinline__ TcRow tc_decode_row(const TcGemmParams& p, int m) {
   return r;
 }
 
-// f[0..31]: accumulator values (already hh + cross, times unscale) of columns n .. n+31 of this thread's row.  PLANES = 1
-// (AAE_PREC_TC_FP16) stores the hi plane only, rounded straight from fp32; out_lo is not touched.
-template <int PLANES = 2>
+// ------------------------------------------------------------------------------------------------- operand formats
+// Every fp16 operand is written in one of two formats.  PLANES = 2 (AAE_PREC_TC_SPLIT): hi and lo planes, pairs through the
+// Veltkamp split_f16x2, single values through split_f16.  PLANES = 1 (AAE_PREC_TC_FP16): the hi plane alone, rn(x) straight
+// from fp32 -- not split_f16x2's hi term, which can round twice for fp16 subnormals; lo is never touched.
+
+// v[0..N) * scale (N = 2, 4 or a multiple of 8) -> hi[off ..) and lo[off ..), one 4-, 8- or 16-byte store per plane and 8 values.
+// With range_flag, a value whose magnitude reaches TC_F16_OVERFLOW sets range_bit in *range_flag before the stores.
+template <int PLANES, int N>
+__device__ __forceinline__ void tc_store_f16(const float (&v)[N], float scale, __half* hi, __half* lo, long long off,
+                                             unsigned* range_flag = nullptr, unsigned range_bit = 0) {
+  uint32_t h[N / 2], l[N / 2];
+  float amax = 0.f;
+#pragma unroll
+  for (int j = 0; j < N; j += 2) {
+    amax = fmaxf(amax, fmaxf(fabsf(v[j]), fabsf(v[j + 1])));
+    if constexpr (PLANES == 1) {
+      const __half2 p = __floats2half2_rn(v[j] * scale, v[j + 1] * scale);
+      h[j >> 1] = *reinterpret_cast<const uint32_t*>(&p);
+    } else {
+      tc::split_f16x2(v[j] * scale, v[j + 1] * scale, h[j >> 1], l[j >> 1]);
+    }
+  }
+  if (range_flag != nullptr && !(amax * scale < TC_F16_OVERFLOW)) atomicOr(range_flag, range_bit);
+  if constexpr (N == 2) {
+    *reinterpret_cast<uint32_t*>(hi + off) = h[0];
+    if constexpr (PLANES == 2) *reinterpret_cast<uint32_t*>(lo + off) = l[0];
+  } else if constexpr (N == 4) {
+    *reinterpret_cast<uint2*>(hi + off) = make_uint2(h[0], h[1]);
+    if constexpr (PLANES == 2) *reinterpret_cast<uint2*>(lo + off) = make_uint2(l[0], l[1]);
+  } else {
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      reinterpret_cast<uint4*>(hi + off)[j] = make_uint4(h[4 * j], h[4 * j + 1], h[4 * j + 2], h[4 * j + 3]);
+      if constexpr (PLANES == 2) reinterpret_cast<uint4*>(lo + off)[j] = make_uint4(l[4 * j], l[4 * j + 1], l[4 * j + 2], l[4 * j + 3]);
+    }
+  }
+}
+
+// One value -> hi[i] (and lo[i]), with the same optional range guard.
+template <int PLANES>
+__device__ __forceinline__ void tc_store_f16(float v, __half* hi, __half* lo, long long i, unsigned* range_flag = nullptr,
+                                             unsigned range_bit = 0) {
+  if (range_flag != nullptr && !(fabsf(v) < TC_F16_OVERFLOW)) atomicOr(range_flag, range_bit);
+  __half h, l;
+  tc::split_f16(v, h, l);
+  hi[i] = h;
+  if constexpr (PLANES == 2) lo[i] = l;
+}
+
+// hi[i] (+ lo[i]) as fp32
+template <int PLANES>
+__device__ __forceinline__ float tc_load_f16(const __half* hi, const __half* lo, long long i) {
+  if constexpr (PLANES == 1) return __half2float(hi[i]);
+  else return __half2float(hi[i]) + __half2float(lo[i]);
+}
+
+// f[0..31]: accumulator values (already hh + cross, times unscale) of columns n .. n+31 of this thread's row, stored in the
+// format PLANES.
+template <int PLANES>
 __device__ __forceinline__ void tc_store_chunk(const TcGemmParams& p, const TcRow& r, int n, float (&f)[32], int split_z) {
   if (p.out_mode == OUT_F32) {
     float* dst = p.out_f32 + (long long)split_z * p.M * p.N + r.row_off + n;
@@ -162,60 +243,24 @@ __device__ __forceinline__ void tc_store_chunk(const TcGemmParams& p, const TcRo
     const int cq = p.N >> 2, cls = n / cq, co = n - cls * cq;     // a 32-column chunk never straddles a parity class (cq % 32 == 0)
     off = ((long long)(r.b * 2 * p.OH + 2 * r.i + (cls >> 1)) * (2 * p.OW) + 2 * r.j + (cls & 1)) * cq + co;
   }
-  if constexpr (PLANES == 1) {
-    uint32_t hi[16];
-    float amax = 0.f;
-#pragma unroll
-    for (int j = 0; j < 32; j += 2) {
-      amax = fmaxf(amax, fmaxf(fabsf(f[j]), fabsf(f[j + 1])));
-      const __half2 h = __floats2half2_rn(f[j] * p.out_scale, f[j + 1] * p.out_scale);
-      hi[j >> 1] = *reinterpret_cast<const uint32_t*>(&h);
-    }
-    if (p.range_flag != nullptr && !(amax * p.out_scale < TC_F16_OVERFLOW)) atomicOr(p.range_flag, p.range_bit);
-    uint4* dh = reinterpret_cast<uint4*>(p.out_hi + off);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) dh[j] = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-  } else {
-    uint32_t hi[16], lo[16];
-    float amax = 0.f;
-#pragma unroll
-    for (int j = 0; j < 32; j += 2) {
-      amax = fmaxf(amax, fmaxf(fabsf(f[j]), fabsf(f[j + 1])));
-      tc::split_f16x2(f[j] * p.out_scale, f[j + 1] * p.out_scale, hi[j >> 1], lo[j >> 1]);
-    }
-    if (p.range_flag != nullptr && !(amax * p.out_scale < TC_F16_OVERFLOW)) atomicOr(p.range_flag, p.range_bit);
-    uint4* dh = reinterpret_cast<uint4*>(p.out_hi + off);
-    uint4* dl = reinterpret_cast<uint4*>(p.out_lo + off);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      dh[j] = make_uint4(hi[4 * j], hi[4 * j + 1], hi[4 * j + 2], hi[4 * j + 3]);
-      dl[j] = make_uint4(lo[4 * j], lo[4 * j + 1], lo[4 * j + 2], lo[4 * j + 3]);
-    }
-  }
+  tc_store_f16<PLANES>(f, p.out_scale, p.out_hi, p.out_lo, off, p.range_flag, p.range_bit);
 }
 
 
-// The two consumer warpgroups' accumulators (rows 64 wg .. 64 wg + 63, main and cross term) -> the fp32 image [128][ld]
-// that the row-per-thread epilogue reads (it takes the place of the stage ring once every MMA has completed).
-template <int R>
+// The two consumer warpgroups' accumulators (rows 64 wg .. 64 wg + 63; the main term, and with PLANES = 2 the cross term in
+// columns [2 R, 4 R)) -> the fp32 image [128][ld] that the row-per-thread epilogue reads (it takes the place of the stage ring
+// once every MMA has completed).
+template <int PLANES, int R>
 __device__ __forceinline__ void tc_park_acc(float* img, int ld, int wg, int warp, int lane, const float (&acc)[R], const float (&crs)[R]) {
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = (lane & 3) * 2;
 #pragma unroll
   for (int j = 0; j < R / 4; ++j) {
     *reinterpret_cast<float2*>(img + r0 * ld + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
     *reinterpret_cast<float2*>(img + (r0 + 8) * ld + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-    *reinterpret_cast<float2*>(img + r0 * ld + 2 * R + 8 * j + c0) = make_float2(crs[4 * j], crs[4 * j + 1]);
-    *reinterpret_cast<float2*>(img + (r0 + 8) * ld + 2 * R + 8 * j + c0) = make_float2(crs[4 * j + 2], crs[4 * j + 3]);
-  }
-}
-// The same for a single accumulator (AAE_PREC_TC_FP16: no cross term): image [128][ld], ld >= 2 R
-template <int R>
-__device__ __forceinline__ void tc_park_acc(float* img, int ld, int wg, int warp, int lane, const float (&acc)[R]) {
-  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = (lane & 3) * 2;
-#pragma unroll
-  for (int j = 0; j < R / 4; ++j) {
-    *reinterpret_cast<float2*>(img + r0 * ld + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-    *reinterpret_cast<float2*>(img + (r0 + 8) * ld + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    if constexpr (PLANES == 2) {
+      *reinterpret_cast<float2*>(img + r0 * ld + 2 * R + 8 * j + c0) = make_float2(crs[4 * j], crs[4 * j + 1]);
+      *reinterpret_cast<float2*>(img + (r0 + 8) * ld + 2 * R + 8 * j + c0) = make_float2(crs[4 * j + 2], crs[4 * j + 3]);
+    }
   }
 }
 __device__ __forceinline__ void tc_acc_ld32(const float* img, int ld, int row, int col, uint32_t (&v)[32]) {
@@ -227,13 +272,37 @@ __device__ __forceinline__ void tc_acc_ld32(const float* img, int ld, int row, i
   }
 }
 
+// Epilogue of tc_gemm_kernel and tc_wgrad_kernel over the parked image of the tile at (m0, n0): main (+ cross) term times the
+// unscale (and the dynamic gradient unscale when p.amax_bits is set), zero when the CTA's K range was empty, then tc_store_chunk.
+// Warps 4-11: two warps per 32-row quadrant, interleaved 32-column chunks.
+template <int PLANES, int N_TILE>
+__device__ __forceinline__ void tc_epilogue(const TcGemmParams& p, const float* img, int ld, int m0, int n0, bool has_work, int warp, int lane) {
+  const int q = warp & 3, half = (warp - 4) >> 2;
+  const TcRow row = tc_decode_row(p, m0 + q * 32 + lane);
+  const float unscale = p.amax_bits ? p.unscale * tc_dyn_unscale(__ldg(p.amax_bits)) : p.unscale;
+#pragma unroll 1
+  for (int c = half; c < N_TILE / 32; c += 2) {
+    const int n = n0 + c * 32;
+    if (!row.valid || n >= p.N) continue;
+    uint32_t v[32], x[32];
+    tc_acc_ld32(img, ld, q * 32 + lane, c * 32, v);
+    if constexpr (PLANES == 2) tc_acc_ld32(img, ld, q * 32 + lane, N_TILE + c * 32, x);
+    float f[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      if constexpr (PLANES == 1) f[j] = has_work ? __uint_as_float(v[j]) * unscale : 0.f;
+      else f[j] = has_work ? (__uint_as_float(v[j]) + __uint_as_float(x[j])) * unscale : 0.f;
+    }
+    tc_store_chunk<PLANES>(p, row, n, f, (int)blockIdx.z);
+  }
+}
+
 // launches tc_gemm_kernel over grid = (M tiles, N tiles, K splits); planes = 1 runs the single-pass (hi-only) instantiation
-int tc_launch_layer(const TcLayer& T, dim3 grid, cudaStream_t s, int planes = 2);
+int tc_launch_layer(const TcLayer& T, dim3 grid, cudaStream_t s, int planes);
 int tc_dev_alloc(void** p, size_t bytes);
-// Tensor maps + packed-weight storage of a layer whose A operand is a PLAIN NHWC (hi, lo) tensor [B_pad, in_h, in_w, in_c]
-// (taps = unit-stride boxes): fills tm_a_*, allocates w_hi/w_lo [ceil(N / TC_N_TILE) * TC_N_TILE][taps * in_c] and their maps.
-// T.{in_h,in_w,in_c,taps,BW,BH,BB,gp.N} must be set; with alloc_input = false T.in_hi/in_lo are the caller's.  planes = 1
-// allocates and maps the hi planes only.
-int tc_layer_setup_plain(TcLayer& T, int B, bool alloc_input, int planes = 2);
+// Tensor maps + packed-weight storage of a layer whose A operand is a PLAIN NHWC tensor [B_pad, in_h, in_w, in_c] in `planes`
+// planes (taps = unit-stride boxes): allocates T.in, fills tm_a, allocates T.w [ceil(N / TC_N_TILE) * TC_N_TILE][taps * in_c]
+// and fills tm_w.  T.{in_h,in_w,in_c,taps,BW,BH,BB,gp.N} must be set.
+int tc_layer_setup_plain(TcLayer& T, int B, int planes);
 
 }  // namespace aae

@@ -60,8 +60,8 @@ struct WgSmem {
 
 // Both operands are MN-major (channels contiguous, K = pixels): warpgroup wg takes the X box of channels [64 wg, 64 wg + 64) as
 // its 64 rows of A, and the whole G tile (N_TILE / 64 boxes, LBO apart) as B.
-// PLANES = 2: stage = [X_hi | X_lo | G_hi | G_lo], three products per K step; PLANES = 1: stage = [X_hi | G_hi] (tm_x_lo and
-// tm_g_lo unused), one product into one accumulator.
+// PLANES = 2: stage = [X_hi | X_lo | G_hi | G_lo], three products per K step; PLANES = 1: stage = [X_hi | G_hi] (the lo maps
+// are not read), one product into one accumulator.
 template <int N_TILE, int STAGES, int PLANES = 2>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_wgrad_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_constant__ CUtensorMap tm_x_lo,
@@ -82,11 +82,10 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_consta
   const int q_end = min(p.total_chunks, q_begin + p.chunks_per_split);
 
   if (threadIdx.x == 0) {
-    if constexpr (PLANES == 1) {
-      prefetch_tmap(&tm_x_hi); prefetch_tmap(&tm_g_hi);
-    } else {
-      prefetch_tmap(&tm_x_hi); prefetch_tmap(&tm_x_lo); prefetch_tmap(&tm_g_hi); prefetch_tmap(&tm_g_lo);
-    }
+    prefetch_tmap(&tm_x_hi);
+    if constexpr (PLANES == 2) prefetch_tmap(&tm_x_lo);
+    prefetch_tmap(&tm_g_hi);
+    if constexpr (PLANES == 2) prefetch_tmap(&tm_g_lo);
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
     fence_barrier_init();
   }
@@ -104,68 +103,17 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_consta
         const int y0 = (r / cols) * p.BHk, x0 = (r - (r / cols) * cols) * p.BWk;
         uint8_t* st = smem + s * S::STAGE_BYTES;
         mbar_arrive_expect_tx(&full_bar[s], S::STAGE_BYTES);
-        if constexpr (PLANES == 1) {
 #pragma unroll
-          for (int g = 0; g < 2; ++g) tma_load_4d(st + g * BOX_BYTES, &tm_x_hi, &full_bar[s], cx + 64 * g, x0 + dj, y0 + di, b);
+        for (int g = 0; g < 2; ++g) {
+          tma_load_4d(st + g * BOX_BYTES, &tm_x_hi, &full_bar[s], cx + 64 * g, x0 + dj, y0 + di, b);
+          if constexpr (PLANES == 2) tma_load_4d(st + S::X_BYTES + g * BOX_BYTES, &tm_x_lo, &full_bar[s], cx + 64 * g, x0 + dj, y0 + di, b);
+        }
 #pragma unroll
-          for (int g = 0; g < N_TILE / 64; ++g) tma_load_4d(st + S::X_BYTES + g * BOX_BYTES, &tm_g_hi, &full_bar[s], n0 + 64 * g, x0, y0, b);
-        } else {
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            tma_load_4d(st + g * BOX_BYTES, &tm_x_hi, &full_bar[s], cx + 64 * g, x0 + dj, y0 + di, b);
-            tma_load_4d(st + S::X_BYTES + g * BOX_BYTES, &tm_x_lo, &full_bar[s], cx + 64 * g, x0 + dj, y0 + di, b);
-          }
-#pragma unroll
-          for (int g = 0; g < N_TILE / 64; ++g) {
-            tma_load_4d(st + 2 * S::X_BYTES + g * BOX_BYTES, &tm_g_hi, &full_bar[s], n0 + 64 * g, x0, y0, b);
-            tma_load_4d(st + 2 * S::X_BYTES + S::G_BYTES + g * BOX_BYTES, &tm_g_lo, &full_bar[s], n0 + 64 * g, x0, y0, b);
-          }
+        for (int g = 0; g < N_TILE / 64; ++g) {
+          tma_load_4d(st + PLANES * S::X_BYTES + g * BOX_BYTES, &tm_g_hi, &full_bar[s], n0 + 64 * g, x0, y0, b);
+          if constexpr (PLANES == 2) tma_load_4d(st + 2 * S::X_BYTES + S::G_BYTES + g * BOX_BYTES, &tm_g_lo, &full_bar[s], n0 + 64 * g, x0, y0, b);
         }
       }
-    }
-  } else if (warp >= 4 && PLANES == 1) {
-    const int wg = (warp - 4) >> 2;
-    float acc[R];
-#pragma unroll
-    for (int j = 0; j < R; ++j) acc[j] = 0.f;
-    for (int q = q_begin, i = 0; q < q_end; ++q, ++i) {
-      const int s = i % STAGES;
-      mbar_wait(&full_bar[s], ((uint32_t)(i / STAGES)) & 1u);
-      const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
-      wgmma_fence_regs(acc);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < S::KP / 16; ++k) {
-        const uint32_t ko = (uint32_t)k * 16u * 128u;
-        const uint64_t x_hi = make_sw128_mnmajor_desc(st + wg * BOX_BYTES + ko, BOX_BYTES, 1024);
-        const uint64_t g_hi = make_sw128_mnmajor_desc(st + S::X_BYTES + ko, BOX_BYTES, 1024);
-        Wgmma<N_TILE>::template ss<1, 1>(acc, x_hi, g_hi, (i > 0 || k > 0) ? 1u : 0u);
-      }
-      wgmma_commit();
-      wgmma_wait<1>();
-      wgmma_fence_regs(acc);
-      if (i > 0 && (warp & 3) == 0 && lane == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
-    }
-    wgmma_wait<0>();
-    wgmma_fence_regs(acc);
-    named_bar_sync(1, 256);
-    float* img = reinterpret_cast<float*>(smem);
-    tc_park_acc(img, S::ACC_LD, wg, warp, lane, acc);
-    named_bar_sync(1, 256);
-    const int q4 = warp & 3, half = (warp - 4) >> 2;
-    const TcRow row = tc_decode_row(p.ep, m0 + q4 * 32 + lane);
-    const bool has_work = q_end > q_begin;
-    const float unscale = p.ep.amax_bits ? p.ep.unscale * tc_dyn_unscale(__ldg(p.ep.amax_bits)) : p.ep.unscale;
-#pragma unroll 1
-    for (int c = half; c < N_TILE / 32; c += 2) {
-      const int n = n0 + c * 32;
-      if (!row.valid || n >= p.ep.N) continue;
-      uint32_t v[32];
-      tc_acc_ld32(img, S::ACC_LD, q4 * 32 + lane, c * 32, v);
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = has_work ? __uint_as_float(v[j]) * unscale : 0.f;
-      tc_store_chunk<1>(p.ep, row, n, f, (int)blockIdx.z);
     }
   } else if (warp >= 4) {
     const int wg = (warp - 4) >> 2;
@@ -176,47 +124,37 @@ tc_wgrad_kernel(const __grid_constant__ CUtensorMap tm_x_hi, const __grid_consta
       const int s = i % STAGES;
       mbar_wait(&full_bar[s], ((uint32_t)(i / STAGES)) & 1u);
       const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
-      wgmma_fence_regs(acc); wgmma_fence_regs(crs);
+      wgmma_fence_regs(acc);
+      if constexpr (PLANES == 2) wgmma_fence_regs(crs);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < S::KP / 16; ++k) {
         const uint32_t ko = (uint32_t)k * 16u * 128u;   // 16 pixel rows of 128 B
         const uint64_t x_hi = make_sw128_mnmajor_desc(st + wg * BOX_BYTES + ko, BOX_BYTES, 1024);
         const uint64_t x_lo = make_sw128_mnmajor_desc(st + S::X_BYTES + wg * BOX_BYTES + ko, BOX_BYTES, 1024);
-        const uint64_t g_hi = make_sw128_mnmajor_desc(st + 2 * S::X_BYTES + ko, BOX_BYTES, 1024);
+        const uint64_t g_hi = make_sw128_mnmajor_desc(st + PLANES * S::X_BYTES + ko, BOX_BYTES, 1024);
         const uint64_t g_lo = make_sw128_mnmajor_desc(st + 2 * S::X_BYTES + S::G_BYTES + ko, BOX_BYTES, 1024);
         const uint32_t first = (i > 0 || k > 0) ? 1u : 0u;
         Wgmma<N_TILE>::template ss<1, 1>(acc, x_hi, g_hi, first);
-        Wgmma<N_TILE>::template ss<1, 1>(crs, x_lo, g_hi, first);
-        Wgmma<N_TILE>::template ss<1, 1>(crs, x_hi, g_lo, 1u);
+        if constexpr (PLANES == 2) {
+          Wgmma<N_TILE>::template ss<1, 1>(crs, x_lo, g_hi, first);
+          Wgmma<N_TILE>::template ss<1, 1>(crs, x_hi, g_lo, 1u);
+        }
       }
       wgmma_commit();
       wgmma_wait<1>();
-      wgmma_fence_regs(acc); wgmma_fence_regs(crs);
+      wgmma_fence_regs(acc);
+      if constexpr (PLANES == 2) wgmma_fence_regs(crs);
       if (i > 0 && (warp & 3) == 0 && lane == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
     }
     wgmma_wait<0>();
-    wgmma_fence_regs(acc); wgmma_fence_regs(crs);
+    wgmma_fence_regs(acc);
+    if constexpr (PLANES == 2) wgmma_fence_regs(crs);
     named_bar_sync(1, 256);
     float* img = reinterpret_cast<float*>(smem);
-    tc_park_acc(img, S::ACC_LD, wg, warp, lane, acc, crs);
+    tc_park_acc<PLANES>(img, S::ACC_LD, wg, warp, lane, acc, crs);
     named_bar_sync(1, 256);
-    const int q4 = warp & 3, half = (warp - 4) >> 2;
-    const TcRow row = tc_decode_row(p.ep, m0 + q4 * 32 + lane);
-    const bool has_work = q_end > q_begin;
-    const float unscale = p.ep.amax_bits ? p.ep.unscale * tc_dyn_unscale(__ldg(p.ep.amax_bits)) : p.ep.unscale;
-#pragma unroll 1
-    for (int c = half; c < N_TILE / 32; c += 2) {
-      const int n = n0 + c * 32;
-      if (!row.valid || n >= p.ep.N) continue;
-      uint32_t v[32], x[32];
-      tc_acc_ld32(img, S::ACC_LD, q4 * 32 + lane, c * 32, v);
-      tc_acc_ld32(img, S::ACC_LD, q4 * 32 + lane, N_TILE + c * 32, x);
-      float f[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) f[j] = has_work ? (__uint_as_float(v[j]) + __uint_as_float(x[j])) * unscale : 0.f;
-      tc_store_chunk(p.ep, row, n, f, (int)blockIdx.z);
-    }
+    tc_epilogue<PLANES, N_TILE>(p.ep, img, S::ACC_LD, m0, n0, q_end > q_begin, warp, lane);
   }
 }
 
@@ -245,12 +183,6 @@ __device__ __forceinline__ long long remap_offset(long long i, int mode, int h, 
   const int y = (int)(r % h);
   const long long b = r / h;
   return ((b * 2 * h + 2 * y + (cls >> 1)) * (2LL * w) + 2 * x + (cls & 1)) * C + c;
-}
-
-// two fp32 -> the packed pair of their fp16 roundings (the hi term of the single-pass operands)
-__device__ __forceinline__ uint32_t rn_f16x2(float a, float b) {
-  const __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&h);
 }
 
 __device__ __forceinline__ void load8(const float* p, float (&v)[8]) {
@@ -292,11 +224,11 @@ __global__ void amax_kernel(const float* __restrict__ x, const __half* __restric
   }
 }
 
-// raw (fp32 dgrad result, source layout) -> ReLU mask of the forward activation (same layout as raw) -> (hi, lo) fp16 (PLANES = 1:
-// hi only) of value * tc_dyn_scale(amax) in the remapped layout; optionally the masked fp32 back in place (fp32 consumers)
+// raw (fp32 dgrad result, source layout) -> ReLU mask of the forward activation (same layout as raw) -> fp16 operand (format
+// PLANES) of value * tc_dyn_scale(amax) in the remapped layout; optionally the masked fp32 back in place (fp32 consumers)
 // and the per-column sums of the masked values (bias gradient): a thread always meets the same 8-column group because
 // 256 % groups_per_row == 0, so it sums in registers and the block folds the threads of a group in fixed order.
-template <int PLANES = 2>
+template <int PLANES>
 __global__ void __launch_bounds__(256) finish_kernel(float* __restrict__ raw, const __half* __restrict__ mask, long long groups, int mode, int h, int w,
                                                      int C, const unsigned* __restrict__ amax, __half* __restrict__ hi, __half* __restrict__ lo,
                                                      int write_masked, float* __restrict__ colsum, int groups_per_row) {
@@ -316,20 +248,7 @@ __global__ void __launch_bounds__(256) finish_kernel(float* __restrict__ raw, co
 #pragma unroll
     for (int j = 0; j < 8; ++j) cs[j] += v[j];
     const long long j = remap_offset(i, mode, h, w, C);
-    if (hi) {
-      if constexpr (PLANES == 1) {
-        uint32_t hh[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) hh[t] = rn_f16x2(v[2 * t] * scale, v[2 * t + 1] * scale);
-        *reinterpret_cast<uint4*>(hi + j) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-      } else {
-        uint32_t hh[4], ll[4];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) split_f16x2(v[2 * t] * scale, v[2 * t + 1] * scale, hh[t], ll[t]);
-        *reinterpret_cast<uint4*>(hi + j) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-        *reinterpret_cast<uint4*>(lo + j) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
-      }
-    }
+    if (hi) tc_store_f16<PLANES>(v, scale, hi, lo, j);
   }
   if (colsum) {
 #pragma unroll
@@ -382,8 +301,8 @@ __global__ void amax_scalar_kernel(const float* __restrict__ x, long long n, uns
 
 // tap-separable output layer: G[pixel (b,y,x)][tap * n4 + m] = gs[(b, y - (ty-1), x - (tx-1))][m], gs = space-to-depth of the
 // pre-sigmoid gradient g [B, 2h, 2w, c] (m = cls * c + co); columns >= 9 * n4 stay zero.  With this im2col both the dgrad
-// (K = 128) and the wgrad (N = 128) of the layer read the big activation tensor exactly once.  PLANES = 1 writes hi only.
-template <int PLANES = 2>
+// (K = 128) and the wgrad (N = 128) of the layer read the big activation tensor exactly once.
+template <int PLANES>
 __global__ void pack_loss_grad_sep_kernel(const float* __restrict__ g, int B, int h, int w, int c, const unsigned* __restrict__ amax,
                                           __half* __restrict__ hi, __half* __restrict__ lo) {
   const float scale = tc_dyn_scale(__ldg(amax));
@@ -398,7 +317,7 @@ __global__ void pack_loss_grad_sep_kernel(const float* __restrict__ g, int B, in
     const int ys = y - (tap / 3 - 1), xs = x - (tap % 3 - 1);
     const bool in = ys >= 0 && ys < h && xs >= 0 && xs < w;
     const long long o = ((b * h + y) * w + x) * 128 + tap * n4;
-    // n4 = 4c values -> c groups of 4 halves (8 bytes) each for hi and lo
+    // n4 = 4c values -> c groups of 4 halves (8 bytes) per plane
     for (int q = 0; q < c; ++q) {
       float v[4];
 #pragma unroll
@@ -406,32 +325,20 @@ __global__ void pack_loss_grad_sep_kernel(const float* __restrict__ g, int B, in
         const int m = q * 4 + e, cls = m / c, co = m - cls * c;
         v[e] = in ? g[((b * 2 * h + 2 * ys + (cls >> 1)) * (2LL * w) + 2 * xs + (cls & 1)) * c + co] * scale : 0.f;
       }
-      if constexpr (PLANES == 1) {
-        *reinterpret_cast<uint2*>(hi + o + q * 4) = make_uint2(rn_f16x2(v[0], v[1]), rn_f16x2(v[2], v[3]));
-      } else {
-        uint32_t h0, l0, h1, l1;
-        split_f16x2(v[0], v[1], h0, l0);
-        split_f16x2(v[2], v[3], h1, l1);
-        *reinterpret_cast<uint2*>(hi + o + q * 4) = make_uint2(h0, h1);
-        *reinterpret_cast<uint2*>(lo + o + q * 4) = make_uint2(l0, l1);
-      }
+      tc_store_f16<PLANES>(v, 1.f, hi, lo, o + q * 4);
     }
   }
 }
 
-// tap-separable output layer: dgrad operand [cin][128], column (tap * n4 + m) = Wm[tap][ci][m]; PLANES = 1 writes hi only
-template <int PLANES = 2>
+// tap-separable output layer: dgrad operand [cin][128], column (tap * n4 + m) = Wm[tap][ci][m]
+template <int PLANES>
 __global__ void pack_dec_dgrad_sep_kernel(const float* __restrict__ wm, int cin, int n4, float scale, __half* __restrict__ hi,
                                           __half* __restrict__ lo) {
   const int total = cin * 128;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int k = i & 127, ci = i >> 7;
     const int tap = k / n4, m = k - tap * n4;
-    const float v = tap < 9 ? wm[((long long)tap * cin + ci) * n4 + m] * scale : 0.f;
-    __half a, d;
-    split_f16(v, a, d);
-    hi[i] = a;
-    if constexpr (PLANES == 2) lo[i] = d;
+    tc_store_f16<PLANES>(tap < 9 ? wm[((long long)tap * cin + ci) * n4 + m] * scale : 0.f, hi, lo, i);
   }
 }
 
@@ -444,26 +351,9 @@ __global__ void rearrange_sep_wgrad_kernel(const float* __restrict__ in, int cin
   }
 }
 
-// 8 consecutive fp32 -> (hi, lo) fp16, one 16-byte store each; PLANES = 1: hi only
-template <int PLANES = 2>
-__device__ __forceinline__ void split_store8(const float (&v)[8], float scale, __half* hi, __half* lo) {
-  if constexpr (PLANES == 1) {
-    uint32_t hh[4];
-#pragma unroll
-    for (int t = 0; t < 4; ++t) hh[t] = rn_f16x2(v[2 * t] * scale, v[2 * t + 1] * scale);
-    *reinterpret_cast<uint4*>(hi) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-  } else {
-    uint32_t hh[4], ll[4];
-#pragma unroll
-    for (int t = 0; t < 4; ++t) split_f16x2(v[2 * t] * scale, v[2 * t + 1] * scale, hh[t], ll[t]);
-    *reinterpret_cast<uint4*>(hi) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-    *reinterpret_cast<uint4*>(lo) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
-  }
-}
-
 // decoder sub-pixel unit: merged weights Wm [9][cin][n4] -> dgrad operand [cin][9 * n4] with the taps flipped.
 // One thread per 8 consecutive columns (n4 % 8 == 0).
-template <int PLANES = 2>
+template <int PLANES>
 __global__ void pack_dec_dgrad_kernel(const float* __restrict__ wm, int cin, int n4, float scale, __half* __restrict__ hi,
                                       __half* __restrict__ lo) {
   const int g8 = n4 / 8;
@@ -475,13 +365,13 @@ __global__ void pack_dec_dgrad_kernel(const float* __restrict__ wm, int cin, int
     const int ci = (int)(r / 9);
     float v[8];
     load8(wm + ((long long)(8 - t) * cin + ci) * n4 + n, v);
-    split_store8<PLANES>(v, scale, hi + i * 8, lo + i * 8);
+    tc_store_f16<PLANES>(v, scale, hi, lo, i * 8);
   }
 }
 
 // encoder unit: W HWIO [5][5][cin][cout] -> dgrad operand [(py,px,ci)][9 * cout]; tap (ty,tx) of the 3x3 window over dY
 // carries kernel element (3 - 2ty + py, 3 - 2tx + px) when that lies inside the 5x5 kernel.  8 output channels per thread.
-template <int PLANES = 2>
+template <int PLANES>
 __global__ void pack_enc_dgrad_kernel(const float* __restrict__ w, int cin, int cout, float scale, __half* __restrict__ hi,
                                       __half* __restrict__ lo) {
   const int c8 = cout / 8;
@@ -500,17 +390,15 @@ __global__ void pack_enc_dgrad_kernel(const float* __restrict__ w, int cin, int 
 #pragma unroll
       for (int j = 0; j < 8; ++j) v[j] = 0.f;
     }
-    split_store8<PLANES>(v, scale, hi + i * 8, lo + i * 8);
+    tc_store_f16<PLANES>(v, scale, hi, lo, i * 8);
   }
 }
 
-template <int PLANES = 2>
+template <int PLANES>
 __global__ void unpack_plain_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, long long n, float inv_scale,
                                     float* __restrict__ out) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    if constexpr (PLANES == 1) out[i] = __half2float(hi[i]) * inv_scale;
-    else out[i] = (__half2float(hi[i]) + __half2float(lo[i])) * inv_scale;
-  }
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    out[i] = tc_load_f16<PLANES>(hi, lo, i) * inv_scale;
 }
 
 inline unsigned ew_grid(long long n, int threads = 256) {
@@ -519,10 +407,9 @@ inline unsigned ew_grid(long long n, int threads = 256) {
 }
 
 // First encoder layer (Cin = 3, K = 75): its weight gradient is a 1x1 wgrad GEMM over the im2col matrix of the input image.
-// x fp32 [B, H, W, 3] -> A (hi, lo) fp16 [B*OH*OW][128]: column k = (kh*5 + kw)*3 + c < 75 holds scale * x[b, 2oh - pad_t + kh, 2ow - pad_l + kw, c]
-// (zero outside the image), columns 75..127 are zero.  One thread per (pixel, 8-column group): 16-byte stores.  PLANES = 1
-// writes hi only.
-template <int PLANES = 2>
+// x fp32 [B, H, W, 3] -> A fp16 [B*OH*OW][128] (format PLANES): column k = (kh*5 + kw)*3 + c < 75 holds scale * x[b, 2oh - pad_t + kh, 2ow - pad_l + kw, c]
+// (zero outside the image), columns 75..127 are zero.  One thread per (pixel, 8-column group): 16-byte stores.
+template <int PLANES>
 __global__ void conv1_im2col_kernel(const float* __restrict__ x, long long pixels, int H, int W, int OH, int OW, int pad_t, int pad_l, float scale,
                                     __half* __restrict__ hi, __half* __restrict__ lo) {
   const long long total = pixels * 16;
@@ -542,15 +429,7 @@ __global__ void conv1_im2col_kernel(const float* __restrict__ x, long long pixel
         if (ih >= 0 && ih < H && iw >= 0 && iw < W) v[j] = __ldg(x + ((b * H + ih) * W + iw) * 3 + c) * scale;
       }
     }
-    if constexpr (PLANES == 1) {
-      *reinterpret_cast<uint4*>(hi + pix * 128 + g * 8) = make_uint4(rn_f16x2(v[0], v[1]), rn_f16x2(v[2], v[3]), rn_f16x2(v[4], v[5]), rn_f16x2(v[6], v[7]));
-    } else {
-      uint32_t hh[4], ll[4];
-#pragma unroll
-      for (int t = 0; t < 4; ++t) split_f16x2(v[2 * t], v[2 * t + 1], hh[t], ll[t]);
-      *reinterpret_cast<uint4*>(hi + pix * 128 + g * 8) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-      *reinterpret_cast<uint4*>(lo + pix * 128 + g * 8) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
-    }
+    tc_store_f16<PLANES>(v, 1.f, hi, lo, pix * 128 + g * 8);
   }
 }
 
@@ -561,13 +440,13 @@ constexpr int WG_STAGES_SPLIT = 6, WG_STAGES_FP16 = 12;
 static_assert(WgSmem<128, WG_STAGES_FP16, 1>::TOTAL == WgSmem<128, WG_STAGES_SPLIT>::TOTAL, "same footprint");
 static_assert(WgSmem<64, WG_STAGES_FP16, 1>::TOTAL == WgSmem<64, WG_STAGES_SPLIT>::TOTAL, "same footprint");
 
-template <int N_TILE, int STAGES, int PLANES = 2>
-int launch_wgrad(const CUtensorMap& xh, const CUtensorMap& xl, const CUtensorMap& gh, const CUtensorMap& gl, const TcWgradParams& p, dim3 grid,
-                 cudaStream_t s) {
+template <int N_TILE, int PLANES>
+int launch_wgrad(const TcMaps& x, const TcMaps& g, const TcWgradParams& p, dim3 grid, cudaStream_t s) {
+  constexpr int STAGES = PLANES == 1 ? WG_STAGES_FP16 : WG_STAGES_SPLIT;
   using S = WgSmem<N_TILE, STAGES, PLANES>;
   auto kern = tc_wgrad_kernel<N_TILE, STAGES, PLANES>;
   AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-  kern<<<grid, TC_THREADS, S::TOTAL, s>>>(xh, xl, gh, gl, p);
+  kern<<<grid, TC_THREADS, S::TOTAL, s>>>(x.hi, x.lo, g.hi, g.lo, p);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -582,11 +461,11 @@ struct TcUnit {
   int taps_w;               // taps of the wgrad (25 / 9; 1 for the tap-separable output layer)
   int dg_taps;              // taps of the dgrad conv over G (9; 1 for the tap-separable output layer)
   bool sep;                 // decoder output layer in tap-separable form: G is the im2col [pixel][(tap, cls, co)] of the loss gradient
-  TcLayer dg;               // dgrad GEMM: A = G (dg.in_hi / in_lo are the G buffers), B = re-packed weights
+  TcLayer dg;               // dgrad GEMM: A = G (dg.in is the G buffer), B = re-packed weights
   int nd;                   // dgrad output columns (decoder: cin, encoder: 4*cin)
-  const __half *x_hi, *x_lo;  // the layer's forward input (owned by the encoder / decoder plan)
+  TcPlanes x;               // the layer's forward input (owned by the encoder / decoder plan, or the plan's c1_x)
   const __half* mask_hi;    // forward activation whose ReLU masks this unit's dgrad result (same layout as the result)
-  CUtensorMap tm_x_hi, tm_x_lo, tm_g_hi, tm_g_lo;   // wgrad operand maps (64-channel x 32-pixel boxes)
+  TcMaps tm_x, tm_g;        // wgrad operand maps (64-channel x 32-pixel boxes)
   TcWgradParams wp;
   int wg_n_tile;
 };
@@ -607,24 +486,22 @@ struct TcTrainPlan {
   size_t wm_floats = 0;
   // conv1 (Cin = 3): wgrad-only unit appended after the encoder units (index c1): X = im2col of the input image
   int c1 = -1;
-  __half *c1_x_hi = nullptr, *c1_x_lo = nullptr;
+  TcPlanes c1_x;
 };
 
-static int make_wgrad_maps(TcUnit& U, int x_c_total, int x_bpad, int g_bpad, int planes) {
+static int make_wgrad_maps(TcUnit& U, int x_c_total, int x_bpad, int g_bpad) {
   const int bw = std::min(U.gw, 32), bh = 32 / bw;
   {
     const uint64_t dims[4] = {(uint64_t)x_c_total, (uint64_t)U.gw, (uint64_t)U.gh, (uint64_t)x_bpad};
     const uint64_t str[3] = {(uint64_t)x_c_total * 2, (uint64_t)U.gw * x_c_total * 2, (uint64_t)U.gh * U.gw * x_c_total * 2};
     const uint32_t box[4] = {64, (uint32_t)bw, (uint32_t)bh, 1};
-    AAE_TRY(make_tmap_f16(&U.tm_x_hi, U.x_hi, 4, dims, str, box, 128));
-    if (planes == 2) AAE_TRY(make_tmap_f16(&U.tm_x_lo, U.x_lo, 4, dims, str, box, 128));
+    AAE_TRY(U.x.encode(U.tm_x, 4, dims, str, box));
   }
   {
     const uint64_t dims[4] = {(uint64_t)U.gN, (uint64_t)U.gw, (uint64_t)U.gh, (uint64_t)g_bpad};
     const uint64_t str[3] = {(uint64_t)U.gN * 2, (uint64_t)U.gw * U.gN * 2, (uint64_t)U.gh * U.gw * U.gN * 2};
     const uint32_t box[4] = {64, (uint32_t)bw, (uint32_t)bh, 1};
-    AAE_TRY(make_tmap_f16(&U.tm_g_hi, U.dg.in_hi, 4, dims, str, box, 128));
-    if (planes == 2) AAE_TRY(make_tmap_f16(&U.tm_g_lo, U.dg.in_lo, 4, dims, str, box, 128));
+    AAE_TRY(U.dg.in.encode(U.tm_g, 4, dims, str, box));
   }
   TcWgradParams& w = U.wp;
   memset(&w, 0, sizeof(w));
@@ -674,10 +551,10 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     }
     g.unscale = 1.f / W_SCALE;
     g.out_mode = OUT_F32;
-    AAE_TRY(tc_layer_setup_plain(T, B, /*alloc_input=*/true, h->planes));
-    U.x_hi = F.in_hi; U.x_lo = F.in_lo;
+    AAE_TRY(tc_layer_setup_plain(T, B, h->planes));
+    U.x = F.in;
     const int x_bpad = (int)ceil_div(B, F.BB) * F.BB, g_bpad = (int)ceil_div(B, T.BB) * T.BB;
-    AAE_TRY(make_wgrad_maps(U, x_c_total, x_bpad, g_bpad, h->planes));
+    AAE_TRY(make_wgrad_maps(U, x_c_total, x_bpad, g_bpad));
     for (int t = 0; t < U.taps_w; ++t) { U.wp.tap_di[t] = F.gp.tap_di[t]; U.wp.tap_dj[t] = F.gp.tap_dj[t]; U.wp.tap_ch[t] = F.gp.tap_ch[t]; }
     raw_max = std::max(raw_max, (size_t)B * U.gh * U.gw * U.nd);
     wm_max = std::max(wm_max, (size_t)U.taps_w * U.cin * U.gN);
@@ -691,7 +568,7 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     U.sep = l == Ld;
     U.gN = U.sep ? 128 : 4 * F.out_c;
     U.taps_w = U.sep ? 1 : 9; U.dg_taps = U.sep ? 1 : 9; U.nd = F.in_c;
-    U.mask_hi = F.in_hi;                                   // dgrad result = gradient wrt this layer's input activation
+    U.mask_hi = F.in.hi;                                   // dgrad result = gradient wrt this layer's input activation
     h->units.push_back(U);
     st = add_unit(h->units.back(), F, F.in_c);
   }
@@ -702,20 +579,18 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     U.enc = true; U.cin = F.in_c; U.cout = F.out_c;
     U.gh = F.out_h; U.gw = F.out_w; U.gN = F.out_c;
     U.taps_w = 25; U.dg_taps = 9; U.sep = false; U.nd = 4 * F.in_c;
-    U.mask_hi = F.in_hi;                                   // space-to-depth activation, same layout as the dgrad result
+    U.mask_hi = F.in.hi;                                   // space-to-depth activation, same layout as the dgrad result
     h->units.push_back(U);
     st = add_unit(h->units.back(), F, 4 * F.in_c);
   }
   if (st == AAE_OK) {
     // dW1[75, 128] = sum over pixels of im2col(x)[pixel, :75]^T G1[pixel, :]: the same 1x1 wgrad GEMM as the tap-separable output layer
     const TcLayer& F2 = enc->layers[0];                    // conv2: in_h x in_w x in_c are the dims of conv1's output (stored space-to-depth)
-    const size_t n = (size_t)B * F2.in_h * F2.in_w * 128;
-    st = tc_dev_alloc((void**)&h->c1_x_hi, n * sizeof(__half));
-    if (st == AAE_OK && h->planes == 2) st = tc_dev_alloc((void**)&h->c1_x_lo, n * sizeof(__half));
+    st = h->c1_x.alloc((size_t)B * F2.in_h * F2.in_w * 128, h->planes);
     if (st == AAE_OK) {
-      TcLayer Fx;                                          // stands for "the layer whose input is X": only in_hi/in_lo, BB and the tap tables are read
+      TcLayer Fx;                                          // stands for "the layer whose input is X": only in, BB and the tap tables are read
       memset(&Fx.gp, 0, sizeof(Fx.gp));
-      Fx.in_hi = h->c1_x_hi; Fx.in_lo = h->c1_x_lo; Fx.BB = 1;
+      Fx.in = h->c1_x; Fx.BB = 1;
       TcUnit U;
       U.enc = true; U.cin = 128; U.cout = F2.in_c;
       U.gh = F2.in_h; U.gw = F2.in_w; U.gN = F2.in_c;
@@ -739,9 +614,9 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
 
 void tc_train_destroy(TcTrainPlan* h) {
   if (!h) return;
-  for (auto& U : h->units) { cudaFree(U.dg.in_hi); cudaFree(U.dg.in_lo); cudaFree(U.dg.w_hi); cudaFree(U.dg.w_lo); }
+  for (auto& U : h->units) { U.dg.in.release(); U.dg.w.release(); }
   cudaFree(h->amax); cudaFree(h->raw); cudaFree(h->partials); cudaFree(h->wm);
-  cudaFree(h->c1_x_hi); cudaFree(h->c1_x_lo);
+  h->c1_x.release();
   delete h;
 }
 
@@ -761,8 +636,7 @@ int tc_train_pack_weights(TcTrainPlan* h, int u, const float* w_dev, cudaStream_
   TcUnit& U = h->units[u];
   if (U.enc) {
     const unsigned grid = ew_grid(4LL * U.cin * 9 * U.cout / 8);
-    if (h->planes == 1) pack_enc_dgrad_kernel<1><<<grid, 256, 0, s>>>(w_dev, U.cin, U.cout, W_SCALE, U.dg.w_hi, nullptr);
-    else pack_enc_dgrad_kernel<<<grid, 256, 0, s>>>(w_dev, U.cin, U.cout, W_SCALE, U.dg.w_hi, U.dg.w_lo);
+    with_planes(h->planes, [&](auto P) { pack_enc_dgrad_kernel<P><<<grid, 256, 0, s>>>(w_dev, U.cin, U.cout, W_SCALE, U.dg.w.hi, U.dg.w.lo); });
     AAE_LAUNCH_OK();
     return AAE_OK;
   }
@@ -775,13 +649,10 @@ int tc_train_pack_weights_merged(TcTrainPlan* h, int u, const float* wm_dev, cud
   AAE_REQUIRE(u >= 0 && u < h->n_dec, "tc trainer: unit %d is not a decoder unit", u);
   TcUnit& U = h->units[u];
   const unsigned sep_grid = ew_grid((long long)U.cin * 128), grid = ew_grid((long long)U.cin * 9 * U.gN);
-  if (h->planes == 1) {
-    if (U.sep) pack_dec_dgrad_sep_kernel<1><<<sep_grid, 256, 0, s>>>(wm_dev, U.cin, 4 * U.cout, W_SCALE, U.dg.w_hi, nullptr);
-    else pack_dec_dgrad_kernel<1><<<grid, 256, 0, s>>>(wm_dev, U.cin, U.gN, W_SCALE, U.dg.w_hi, nullptr);
-  } else {
-    if (U.sep) pack_dec_dgrad_sep_kernel<<<sep_grid, 256, 0, s>>>(wm_dev, U.cin, 4 * U.cout, W_SCALE, U.dg.w_hi, U.dg.w_lo);
-    else pack_dec_dgrad_kernel<<<grid, 256, 0, s>>>(wm_dev, U.cin, U.gN, W_SCALE, U.dg.w_hi, U.dg.w_lo);
-  }
+  with_planes(h->planes, [&](auto P) {
+    if (U.sep) pack_dec_dgrad_sep_kernel<P><<<sep_grid, 256, 0, s>>>(wm_dev, U.cin, 4 * U.cout, W_SCALE, U.dg.w.hi, U.dg.w.lo);
+    else pack_dec_dgrad_kernel<P><<<grid, 256, 0, s>>>(wm_dev, U.cin, U.gN, W_SCALE, U.dg.w.hi, U.dg.w.lo);
+  });
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -794,8 +665,9 @@ int tc_train_set_loss_grad(TcTrainPlan* h, const float* g_dev, int B, cudaStream
   amax_scalar_kernel<<<ew_grid(n), 256, 0, s>>>(g_dev, n, h->amax + 0);
   AAE_LAUNCH_OK();
   const unsigned grid = ew_grid((long long)B * U.gh * U.gw * 9);
-  if (h->planes == 1) pack_loss_grad_sep_kernel<1><<<grid, 256, 0, s>>>(g_dev, B, U.gh, U.gw, c, h->amax + 0, U.dg.in_hi, nullptr);
-  else pack_loss_grad_sep_kernel<<<grid, 256, 0, s>>>(g_dev, B, U.gh, U.gw, c, h->amax + 0, U.dg.in_hi, U.dg.in_lo);
+  with_planes(h->planes, [&](auto P) {
+    pack_loss_grad_sep_kernel<P><<<grid, 256, 0, s>>>(g_dev, B, U.gh, U.gw, c, h->amax + 0, U.dg.in.hi, U.dg.in.lo);
+  });
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -806,12 +678,10 @@ int tc_train_set_unit_grad(TcTrainPlan* h, int u, const float* g_dev, int B, cud
   const long long groups = (long long)B * U.gh * U.gw * U.gN / 8;
   amax_kernel<<<ew_grid(groups), 256, 0, s>>>(g_dev, nullptr, groups, h->amax + u);
   AAE_LAUNCH_OK();
-  if (h->planes == 1)
-    finish_kernel<1><<<ew_grid(groups), 256, 0, s>>>(const_cast<float*>(g_dev), nullptr, groups, REMAP_SAME, U.gh, U.gw, U.gN, h->amax + u,
-                                                     U.dg.in_hi, nullptr, 0, nullptr, 1);
-  else
-    finish_kernel<<<ew_grid(groups), 256, 0, s>>>(const_cast<float*>(g_dev), nullptr, groups, REMAP_SAME, U.gh, U.gw, U.gN, h->amax + u, U.dg.in_hi,
-                                                  U.dg.in_lo, 0, nullptr, 1);
+  with_planes(h->planes, [&](auto P) {
+    finish_kernel<P><<<ew_grid(groups), 256, 0, s>>>(const_cast<float*>(g_dev), nullptr, groups, REMAP_SAME, U.gh, U.gw, U.gN, h->amax + u,
+                                                     U.dg.in.hi, U.dg.in.lo, 0, nullptr, 1);
+  });
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -832,13 +702,9 @@ int tc_train_unit_wgrad(TcTrainPlan* h, int u, int B, float* dw_out, cudaStream_
   w.ep.amax_bits = h->amax + u;
   w.ep.out_f32 = h->partials;
   dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)splits);
-  if (h->planes == 1) {   // the lo maps are never encoded: the hi maps fill the unused parameter slots
-    if (U.wg_n_tile == 128) AAE_TRY((launch_wgrad<128, WG_STAGES_FP16, 1>(U.tm_x_hi, U.tm_x_hi, U.tm_g_hi, U.tm_g_hi, w, grid, s)));
-    else AAE_TRY((launch_wgrad<64, WG_STAGES_FP16, 1>(U.tm_x_hi, U.tm_x_hi, U.tm_g_hi, U.tm_g_hi, w, grid, s)));
-  } else {
-    if (U.wg_n_tile == 128) AAE_TRY((launch_wgrad<128, WG_STAGES_SPLIT>(U.tm_x_hi, U.tm_x_lo, U.tm_g_hi, U.tm_g_lo, w, grid, s)));
-    else AAE_TRY((launch_wgrad<64, WG_STAGES_SPLIT>(U.tm_x_hi, U.tm_x_lo, U.tm_g_hi, U.tm_g_lo, w, grid, s)));
-  }
+  AAE_TRY(with_planes(h->planes, [&](auto P) {
+    return U.wg_n_tile == 128 ? launch_wgrad<128, P>(U.tm_x, U.tm_g, w, grid, s) : launch_wgrad<64, P>(U.tm_x, U.tm_g, w, grid, s);
+  }));
   if (!U.sep) return launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, dw_out, s);
   AAE_REQUIRE((size_t)mn <= h->wm_floats, "tc trainer: merged-gradient scratch too small");
   AAE_TRY(launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, h->wm, s));
@@ -853,10 +719,10 @@ int tc_train_conv1_wgrad(TcTrainPlan* h, const float* x_dev, int B, float* dw_ou
   const aae_net_cfg& cfg = h->enc->cfg;
   const long long pixels = (long long)B * U.gh * U.gw;
   const int pad_t = std::max((U.gh - 1) * 2 + 5 - cfg.in_h, 0) / 2, pad_l = std::max((U.gw - 1) * 2 + 5 - cfg.in_w, 0) / 2;
-  if (h->planes == 1)
-    conv1_im2col_kernel<1><<<ew_grid(pixels * 16), 256, 0, s>>>(x_dev, pixels, cfg.in_h, cfg.in_w, U.gh, U.gw, pad_t, pad_l, ACT_SCALE, h->c1_x_hi, nullptr);
-  else
-    conv1_im2col_kernel<<<ew_grid(pixels * 16), 256, 0, s>>>(x_dev, pixels, cfg.in_h, cfg.in_w, U.gh, U.gw, pad_t, pad_l, ACT_SCALE, h->c1_x_hi, h->c1_x_lo);
+  with_planes(h->planes, [&](auto P) {
+    conv1_im2col_kernel<P><<<ew_grid(pixels * 16), 256, 0, s>>>(x_dev, pixels, cfg.in_h, cfg.in_w, U.gh, U.gw, pad_t, pad_l, ACT_SCALE, h->c1_x.hi,
+                                                                h->c1_x.lo);
+  });
   AAE_LAUNCH_OK();
   AAE_REQUIRE((size_t)128 * U.gN <= h->wm_floats, "tc trainer: scratch too small for the conv1 wgrad");
   AAE_TRY(tc_train_unit_wgrad(h, h->c1, B, h->wm, s));         // [128 im2col columns][cout]; rows 75.. are zero
@@ -897,7 +763,7 @@ int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, fl
   if (next >= 0) {
     TcUnit& Nx = h->units[next];
     AAE_REQUIRE((long long)Nx.gh * Nx.gw * Nx.gN == (long long)U.gh * U.gw * U.nd, "tc trainer: unit %d does not feed unit %d", u, next);
-    hi = Nx.dg.in_hi; lo = Nx.dg.in_lo; slot = h->amax + next;
+    hi = Nx.dg.in.hi; lo = Nx.dg.in.lo; slot = h->amax + next;
     amax_kernel<<<ew_grid(groups), 256, 0, s>>>(h->raw, U.mask_hi, groups, slot);
     AAE_LAUNCH_OK();
   }
@@ -913,12 +779,9 @@ int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, fl
     AAE_REQUIRE((size_t)grid * U.nd <= h->partial_floats, "tc trainer: column-sum scratch too small");
     colsum = h->partials;
   }
-  if (h->planes == 1)
-    finish_kernel<1><<<grid, 256, 0, s>>>(h->raw, U.mask_hi, groups, mode, U.gh, U.gw, C, slot, hi, nullptr, keep_masked ? 1 : 0, colsum,
-                                          std::max(gpr, 1));
-  else
-    finish_kernel<<<grid, 256, 0, s>>>(h->raw, U.mask_hi, groups, mode, U.gh, U.gw, C, slot, hi, lo, keep_masked ? 1 : 0, colsum,
-                                       std::max(gpr, 1));
+  with_planes(h->planes, [&](auto P) {
+    finish_kernel<P><<<grid, 256, 0, s>>>(h->raw, U.mask_hi, groups, mode, U.gh, U.gw, C, slot, hi, lo, keep_masked ? 1 : 0, colsum, std::max(gpr, 1));
+  });
   AAE_LAUNCH_OK();
   if (db_out) {
     colsum_final_kernel<<<(unsigned)ceil_div(C, 32), dim3(32, 32), 0, s>>>(colsum, (int)grid, U.nd / C, C, db_out);
@@ -931,8 +794,7 @@ int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, fl
 int tc_train_unpack_flat(TcTrainPlan* h, int B, float* out, cudaStream_t s) {
   const TcLayer& D = h->enc->layers.back();
   const long long n = (long long)B * D.in_c;
-  if (h->planes == 1) unpack_plain_kernel<1><<<ew_grid(n), 256, 0, s>>>(D.in_hi, nullptr, n, 1.f / ACT_SCALE, out);
-  else unpack_plain_kernel<<<ew_grid(n), 256, 0, s>>>(D.in_hi, D.in_lo, n, 1.f / ACT_SCALE, out);
+  with_planes(h->planes, [&](auto P) { unpack_plain_kernel<P><<<ew_grid(n), 256, 0, s>>>(D.in.hi, D.in.lo, n, 1.f / ACT_SCALE, out); });
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
