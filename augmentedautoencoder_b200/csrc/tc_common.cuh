@@ -133,6 +133,13 @@ __device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Per-thread register budget of the executing warpgroup (every thread of the warpgroup executes it): dec hands registers back to
+// the CTA's pool, inc waits until the pool has them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // 16-byte asynchronous global -> shared copy (LDGSTS); completion via cp_async_wait_all
 __device__ __forceinline__ void cp_async_16(void* smem_dst, const void* gmem_src, bool pred) {
   const int bytes = pred ? 16 : 0;   // src-size 0 -> zero fill

@@ -18,8 +18,11 @@
 // buffer, no stride-2 gathers.  Weights are pre-packed [Cout][25*Cin] K-major.  Both operands land in shared memory in
 // the 128-byte-swizzle canonical layout wgmma consumes directly.
 //
-// Warp roles (384 threads): warp 0 TMA producer, warpgroups 1-2 wgmma consumers and then epilogue (registers -> shared-memory
-// accumulator image -> bias/ReLU -> hi/lo split -> global, in the next layer's space-to-depth layout).
+// Warp roles (384 threads): warp 0 TMA producer, warpgroups 1-2 wgmma consumers and then epilogue (wgmma fragments in registers
+// -> bias/ReLU -> hi/lo split -> global, in the next layer's space-to-depth layout).  Persistent: one CTA per SM walks a
+// strided list of tiles, and the producer keeps filling the ring across tile boundaries while the consumers run an epilogue.
+#include <limits.h>
+
 #include <algorithm>
 #include <vector>
 
@@ -65,20 +68,42 @@ struct TcSmem {
   static constexpr int A_BYTES = 128 * TC_KCH * 2;     // 128 rows x TC_KCH fp16
   static constexpr int W_BYTES = N_TILE * TC_KCH * 2;
   static constexpr int STAGE_BYTES = PLANES * A_BYTES + PLANES * W_BYTES;
-  static constexpr int ACC_LD = PLANES * N_TILE + 4;   // fp32 accumulator image [128][ACC_LD] (main | cross), padded
-  static constexpr int ACC_BYTES = 128 * ACC_LD * 4;
-  static constexpr int BODY = STAGES * STAGE_BYTES > ACC_BYTES ? STAGES * STAGE_BYTES : ACC_BYTES;
+  static constexpr int BODY = STAGES * STAGE_BYTES;
   static constexpr int TOTAL = BODY + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
+// One output tile of the launch: linear id t -> (x = N tile, y = M tile, z = K split), N fastest, and its K-iteration range.
+struct TcTile {
+  int m0, n0, z, it_begin, it_end;
+};
+template <int N_TILE>
+__device__ __forceinline__ TcTile tc_tile(const TcGemmParams& p, const TcTiles& g, int t) {
+  TcTile r;
+  const int yz = t / g.n;
+  const int y = yz % g.m;
+  r.z = yz / g.m;
+  r.m0 = y * 128;
+  r.n0 = (t - yz * g.n) * N_TILE;
+  r.it_begin = r.z * p.iters_per_split;
+  r.it_end = min(p.taps * p.chunks_per_tap, r.it_begin + p.iters_per_split);
+  return r;
+}
+
 // Warp roles (384 threads): warp 0 TMA producer (warps 1-3 idle), warpgroups 1 and 2 (warps 4-11) issue the wgmma for pixel rows
-// [0,64) and [64,128) of the tile and then run the epilogue, two warps per 32-row quadrant.
-// Grid: x = N tile, y = M tile, z = K split (see tc_launch_layer).
+// [0,64) and [64,128) of the tile and run the epilogue on their own fragments.
+// Persistent grid (see tc_launch_layer): CTA b takes tiles b, b + gridDim.x, ...  Producer and consumers walk the same tiles and
+// K ranges, so one running K-iteration count i over all of the CTA's tiles gives both sides stage i % STAGES and phase
+// (i / STAGES) & 1; the producer runs up to STAGES iterations ahead, into the next tile while the consumers finish this one.
+// Epilogue overlap: at the end of a tile the consumers only fold the accumulators into the unscaled values v and start the next
+// tile; the rest of the epilogue (bias, ReLU, split, stores) runs in two column halves while the MMAs of the next tile's first
+// and second stage execute, so the tensor cores do not wait for it.  v needs a third register array beside acc and crs, so the
+// producer warpgroup gives up registers (setmaxnreg) and the consumers hold it without spilling.
 // PLANES = 2: (hi, lo) operands, three products per K step; PLANES = 1: hi operands only (the lo maps are not read), one product.
 template <int N_TILE, int STAGES, int PLANES = 2>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
-               const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, const TcGemmParams p) {
+               const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, const TcGemmParams p,
+               const TcTiles tiles) {
   using S = TcSmem<N_TILE, STAGES, PLANES>;
   constexpr int R = N_TILE / 2;
   extern __shared__ uint8_t smem_raw[];
@@ -88,11 +113,6 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int m0 = blockIdx.y * 128;
-  const int n0 = blockIdx.x * N_TILE;
-  const int total_iters = p.taps * p.chunks_per_tap;
-  const int it_begin = blockIdx.z * p.iters_per_split;
-  const int it_end = min(total_iters, it_begin + p.iters_per_split);
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tm_a_hi);
@@ -104,71 +124,91 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
   }
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp < 4) {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
     // ===================== TMA producer: stage = [A_hi | A_lo | W_hi | W_lo], the lo boxes with PLANES = 2 only =====================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       const int hw = p.OH * p.OW;
-      const int b0 = m0 / hw, rem = m0 - b0 * hw;
-      const int oh0 = rem / p.OW, ow0 = rem - oh0 * p.OW;
-      for (int it = it_begin, i = 0; it < it_end; ++it, ++i) {
-        const int s = i % STAGES;
-        const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
-        mbar_wait(&empty_bar[s], ph ^ 1u);
-        const int tap = it / p.chunks_per_tap, cc = it - tap * p.chunks_per_tap;
-        uint8_t* st = smem + s * S::STAGE_BYTES;
-        mbar_arrive_expect_tx(&full_bar[s], S::STAGE_BYTES);
-        const int c0 = p.tap_ch[tap] + cc * TC_KCH;
-        const int x = ow0 + p.tap_dj[tap], y = oh0 + p.tap_di[tap];
-        const int kcol = it * TC_KCH;
-        tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
-        if constexpr (PLANES == 2) tma_load_4d(st + S::A_BYTES, &tm_a_lo, &full_bar[s], c0, x, y, b0);
-        tma_load_2d(st + PLANES * S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, n0);
-        if constexpr (PLANES == 2) tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tm_w_lo, &full_bar[s], kcol, n0);
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== wgmma consumers =====================
-    const int wg = (warp - 4) >> 2;
-    float acc[R], crs[R];
-#pragma unroll
-    for (int j = 0; j < R; ++j) { acc[j] = 0.f; crs[j] = 0.f; }
-    for (int it = it_begin, i = 0; it < it_end; ++it, ++i) {
-      const int s = i % STAGES;
-      mbar_wait(&full_bar[s], (uint32_t)(i / STAGES) & 1u);
-      const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
-      const uint32_t a_off = (uint32_t)(wg * 64 * TC_KCH * 2);
-      const uint64_t a_hi = make_sw128_kmajor_desc(st + a_off);
-      const uint64_t a_lo = make_sw128_kmajor_desc(st + S::A_BYTES + a_off);
-      const uint64_t w_hi = make_sw128_kmajor_desc(st + PLANES * S::A_BYTES);
-      const uint64_t w_lo = make_sw128_kmajor_desc(st + 2 * S::A_BYTES + S::W_BYTES);
-      wgmma_fence_regs(acc);
-      if constexpr (PLANES == 2) wgmma_fence_regs(crs);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < TC_KCH / 16; ++k) {
-        // The tensor core truncates when it adds into a large fp32 accumulator, so the 2^-11-sized cross terms get an
-        // accumulator of their own (small magnitude -> negligible truncation) and are folded in by the epilogue in RN fp32.
-        const uint32_t first = (i > 0 || k > 0) ? 1u : 0u;
-        Wgmma<N_TILE>::template ss<0, 0>(acc, desc_advance_k(a_hi, k), desc_advance_k(w_hi, k), first);
-        if constexpr (PLANES == 2) {
-          Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_lo, k), desc_advance_k(w_hi, k), first);
-          Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_hi, k), desc_advance_k(w_lo, k), 1u);
+      int i = 0;
+      for (int t = blockIdx.x; t < tiles.count; t += gridDim.x) {
+        const TcTile T = tc_tile<N_TILE>(p, tiles, t);
+        const int b0 = T.m0 / hw, rem = T.m0 - b0 * hw;
+        const int oh0 = rem / p.OW, ow0 = rem - oh0 * p.OW;
+        for (int it = T.it_begin; it < T.it_end; ++it, ++i) {
+          const int s = i % STAGES;
+          const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
+          mbar_wait(&empty_bar[s], ph ^ 1u);
+          const int tap = it / p.chunks_per_tap, cc = it - tap * p.chunks_per_tap;
+          uint8_t* st = smem + s * S::STAGE_BYTES;
+          mbar_arrive_expect_tx(&full_bar[s], S::STAGE_BYTES);
+          const int c0 = p.tap_ch[tap] + cc * TC_KCH;
+          const int x = ow0 + p.tap_dj[tap], y = oh0 + p.tap_di[tap];
+          const int kcol = it * TC_KCH;
+          tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
+          if constexpr (PLANES == 2) tma_load_4d(st + S::A_BYTES, &tm_a_lo, &full_bar[s], c0, x, y, b0);
+          tma_load_2d(st + PLANES * S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, T.n0);
+          if constexpr (PLANES == 2) tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tm_w_lo, &full_bar[s], kcol, T.n0);
         }
       }
-      wgmma_commit();
-      wgmma_wait<1>();                                // the previous stage's MMAs have read their operands: free it
+    }
+  } else {
+    // ===================== wgmma consumers =====================
+    setmaxnreg_inc<TC_CONSUMER_REGS>();
+    const int wg = (warp - 4) >> 2;
+    const bool releases = (warp & 3) == 0 && lane == 0;   // one arrive per warpgroup on a stage's empty barrier (count 2)
+    constexpr int H = R / 8;                              // column groups per epilogue half (R / 4 groups of 8 columns)
+    float acc[R], crs[R], v[R];
+#pragma unroll
+    for (int j = 0; j < R; ++j) { acc[j] = 0.f; crs[j] = 0.f; v[j] = 0.f; }
+    // the previous tile, whose values v still wait for epilogue halves [half, 2)
+    int pm0 = 0, pn0 = 0, pz = 0, half = 2;
+    auto epilogue_half = [&](int h) {
+      if (h == 0) tc_epilogue_frag<PLANES, 0, H>(p, v, pm0, pn0, pz, warp, lane);
+      else tc_epilogue_frag<PLANES, H, 2 * H>(p, v, pm0, pn0, pz, warp, lane);
+    };
+    int i = 0;
+    for (int t = blockIdx.x; t < tiles.count; t += gridDim.x) {
+      const TcTile T = tc_tile<N_TILE>(p, tiles, t);
+      for (int it = T.it_begin; it < T.it_end; ++it, ++i) {
+        const int s = i % STAGES;
+        mbar_wait(&full_bar[s], (uint32_t)(i / STAGES) & 1u);
+        const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
+        const uint32_t a_off = (uint32_t)(wg * 64 * TC_KCH * 2);
+        const uint64_t a_hi = make_sw128_kmajor_desc(st + a_off);
+        const uint64_t a_lo = make_sw128_kmajor_desc(st + S::A_BYTES + a_off);
+        const uint64_t w_hi = make_sw128_kmajor_desc(st + PLANES * S::A_BYTES);
+        const uint64_t w_lo = make_sw128_kmajor_desc(st + 2 * S::A_BYTES + S::W_BYTES);
+        wgmma_fence_regs(acc);
+        if constexpr (PLANES == 2) wgmma_fence_regs(crs);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < TC_KCH / 16; ++k) {
+          // The tensor core truncates when it adds into a large fp32 accumulator, so the 2^-11-sized cross terms get an
+          // accumulator of their own (small magnitude -> negligible truncation) and are folded in by the epilogue in RN fp32.
+          const uint32_t first = (it > T.it_begin || k > 0) ? 1u : 0u;
+          Wgmma<N_TILE>::template ss<0, 0>(acc, desc_advance_k(a_hi, k), desc_advance_k(w_hi, k), first);
+          if constexpr (PLANES == 2) {
+            Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_lo, k), desc_advance_k(w_hi, k), first);
+            Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_hi, k), desc_advance_k(w_lo, k), 1u);
+          }
+        }
+        wgmma_commit();
+        if (half < 2) epilogue_half(half++);          // the previous tile's stores, while this stage's MMAs run
+        wgmma_wait<1>();                                // the previous stage's MMAs have read their operands: free it
+        wgmma_fence_regs(acc);
+        if constexpr (PLANES == 2) wgmma_fence_regs(crs);
+        if (it > T.it_begin && releases) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+      }
+      wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if constexpr (PLANES == 2) wgmma_fence_regs(crs);
-      if (i > 0 && (warp & 3) == 0 && lane == 0) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+      // the tile's last stage is free as well: without this arrive the producer would wait for it forever on a later tile
+      if (T.it_end > T.it_begin && releases) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+      while (half < 2) epilogue_half(half++);         // a tile of fewer than two K stages did not cover the previous epilogue
+      tc_epilogue_values<PLANES>(p, acc, crs, T.it_end > T.it_begin, v);
+      pm0 = T.m0 + wg * 64; pn0 = T.n0; pz = T.z; half = 0;
     }
-    wgmma_wait<0>();
-    wgmma_fence_regs(acc);
-    if constexpr (PLANES == 2) wgmma_fence_regs(crs);
-    named_bar_sync(1, 256);                           // every MMA of both warpgroups is done: the ring becomes the accumulator image
-    float* img = reinterpret_cast<float*>(smem);
-    tc_park_acc<PLANES>(img, S::ACC_LD, wg, warp, lane, acc, crs);
-    named_bar_sync(1, 256);
-    tc_epilogue<PLANES, N_TILE>(p, img, S::ACC_LD, m0, n0, it_end > it_begin, warp, lane);
+    while (half < 2) epilogue_half(half++);
   }
 }
 
@@ -276,9 +316,9 @@ int TcPlanes::encode(TcMaps& m, int rank, const uint64_t* dims, const uint64_t* 
   return make_tmap_f16(&m.lo, lo, rank, dims, strides_bytes, box, swizzle_bytes);
 }
 
-// tiles = (m_tiles, n_tiles, splits).  The kernel runs the N tiles on grid.x, so the N tiles of an M tile are adjacent in launch
-// order and read the activation tile (and its 5 x 5 tap re-reads) while it is in L2; M first would put all resident CTAs on one
-// weight column and stream every activation tile from HBM once per N tile.
+// tiles = (m_tiles, n_tiles, splits).  min(SM count, tiles) persistent CTAs walk the linear tile id with stride gridDim.x, N tile
+// fastest, so the N tiles of an M tile run side by side and read the activation tile (and its 5 x 5 tap re-reads) while it is
+// in L2; M first would put all resident CTAs on one weight column and stream every activation tile from HBM once per N tile.
 // Stage counts: the split kernel's 3 stages of 64 KB and the single-pass kernel's 6 stages of 32 KB are the same 192 KB ring,
 // so both keep the same bytes in flight and the same shared-memory footprint (and carveout); the single pass gets twice the
 // K-iterations of look-ahead.
@@ -286,13 +326,19 @@ constexpr int TC_STAGES_SPLIT = 3, TC_STAGES_FP16 = 6;
 static_assert(TcSmem<TC_N_TILE, TC_STAGES_FP16, 1>::TOTAL == TcSmem<TC_N_TILE, TC_STAGES_SPLIT>::TOTAL, "same footprint");
 
 int tc_launch_layer(const TcLayer& T, dim3 tiles, cudaStream_t s, int planes) {
-  AAE_REQUIRE(tiles.x <= 65535u, "tc_gemm: %u row tiles exceed the grid's y limit", tiles.x);
+  const long long count = (long long)tiles.x * tiles.y * tiles.z;
+  AAE_REQUIRE(count <= INT_MAX, "tc_gemm: %lld tiles exceed the kernel's int tile index", count);
+  int device = 0, sms = 0;
+  AAE_CUDA_OK(cudaGetDevice(&device));
+  AAE_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  const TcTiles g{(int)tiles.y, (int)tiles.x, (int)count};
+  const unsigned ctas = (unsigned)std::min<long long>(count, sms);
   return with_planes(planes, [&](auto P) {
     constexpr int STAGES = P == 1 ? TC_STAGES_FP16 : TC_STAGES_SPLIT;
     using S = TcSmem<TC_N_TILE, STAGES, P>;
     auto kern = tc_gemm_kernel<TC_N_TILE, STAGES, P>;
     AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    kern<<<dim3(tiles.y, tiles.x, tiles.z), TC_THREADS, S::TOTAL, s>>>(T.tm_a.hi, T.tm_a.lo, T.tm_w.hi, T.tm_w.lo, T.gp);
+    kern<<<ctas, TC_THREADS, S::TOTAL, s>>>(T.tm_a.hi, T.tm_a.lo, T.tm_w.hi, T.tm_w.lo, T.gp, g);
     AAE_LAUNCH_OK();
     return AAE_OK;
   });

@@ -61,6 +61,9 @@ constexpr float W_SCALE = 256.f;      // weights are stored as 256 * w
 constexpr int TC_STAGES = 2;
 constexpr int TC_THREADS = 384;       // warp 0 TMA, 1-3 idle, warpgroups 1-2 (warps 4-11) wgmma + epilogue
 constexpr int TC_N_TILE = 128;        // output channels per GEMM tile
+// setmaxnreg budgets of tc_gemm_kernel: 128 producer threads x 24 + 256 consumer threads x 240 = 64512 registers,
+// the 384 x 168 the launch reserves
+constexpr int TC_PRODUCER_REGS = 24, TC_CONSUMER_REGS = 240;
 constexpr int TC_KCH = 64;            // K chunk per pipeline stage: 64 fp16 = one 128-byte swizzle row
 
 // Tensor maps of both planes of an operand.  Without a lo plane, lo is a copy of hi: the kernels never read it, and every launch
@@ -272,7 +275,7 @@ __device__ __forceinline__ void tc_acc_ld32(const float* img, int ld, int row, i
   }
 }
 
-// Epilogue of tc_gemm_kernel and tc_wgrad_kernel over the parked image of the tile at (m0, n0): main (+ cross) term times the
+// Epilogue of tc_wgrad_kernel over the parked image of the tile at (m0, n0): main (+ cross) term times the
 // unscale (and the dynamic gradient unscale when p.amax_bits is set), zero when the CTA's K range was empty, then tc_store_chunk.
 // Warps 4-11: two warps per 32-row quadrant, interleaved 32-column chunks.
 template <int PLANES, int N_TILE>
@@ -297,8 +300,71 @@ __device__ __forceinline__ void tc_epilogue(const TcGemmParams& p, const float* 
   }
 }
 
-// launches tc_gemm_kernel over grid = (M tiles, N tiles, K splits); planes = 1 runs the single-pass (hi-only) instantiation
-int tc_launch_layer(const TcLayer& T, dim3 grid, cudaStream_t s, int planes);
+// Epilogue of tc_gemm_kernel on one consumer warpgroup's own wgmma fragments (Wgmma's layout: rows m0 + 16 (warp % 4) + lane / 4
+// and + 8, column pairs n0 + 8 j + 2 (lane % 4)), with the arithmetic of tc_epilogue + tc_store_chunk element for element and
+// in the same order, in two steps.  tc_epilogue_values: (main + cross) times the unscale (zero for an empty K range) into v,
+// which frees the accumulators for the next tile.  tc_epilogue_frag over column groups j in [J0, J1): either the fp32 partials,
+// or + bias, the ReLU floor, out_scale and the fp16 split.  The _rn intrinsics keep the compiler from contracting any of it into
+// an FMA.  Each thread stores 2-column pairs and checks the range guard once per call.  Shared memory is not touched.
+template <int PLANES, int R>
+__device__ __forceinline__ void tc_epilogue_values(const TcGemmParams& p, const float (&acc)[R], const float (&crs)[R], bool has_work,
+                                                   float (&v)[R]) {
+  const float unscale = p.amax_bits ? p.unscale * tc_dyn_unscale(__ldg(p.amax_bits)) : p.unscale;
+#pragma unroll
+  for (int e = 0; e < R; ++e) {
+    if constexpr (PLANES == 1) v[e] = has_work ? __fmul_rn(acc[e], unscale) : 0.f;
+    else v[e] = has_work ? __fmul_rn(__fadd_rn(acc[e], crs[e]), unscale) : 0.f;
+  }
+}
+
+template <int PLANES, int J0, int J1, int R>
+__device__ __forceinline__ void tc_epilogue_frag(const TcGemmParams& p, const float (&v)[R], int m0, int n0, int split_z, int warp, int lane) {
+  const int r0 = m0 + (warp & 3) * 16 + (lane >> 2), c0 = n0 + 2 * (lane & 3);
+  const TcRow rows[2] = {tc_decode_row(p, r0), tc_decode_row(p, r0 + 8)};
+  if (p.out_mode == OUT_F32) {
+    float* dst = p.out_f32 + (long long)split_z * p.M * p.N;
+#pragma unroll
+    for (int j = J0; j < J1; ++j) {
+      const int n = c0 + 8 * j;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (rows[h].valid && n < p.N) *reinterpret_cast<float2*>(dst + rows[h].row_off + n) = make_float2(v[4 * j + 2 * h], v[4 * j + 2 * h + 1]);
+    }
+    return;
+  }
+  const float floor_v = p.relu == 1 ? 0.f : -INFINITY;       // fmaxf(a, -inf) = a
+  const int cq = p.N >> 2;
+  float amax = 0.f;
+#pragma unroll
+  for (int j = J0; j < J1; ++j) {
+    const int n = c0 + 8 * j;
+    if (n >= p.N) continue;
+    const float b0 = p.bias != nullptr ? __ldg(p.bias + n) : 0.f, b1 = p.bias != nullptr ? __ldg(p.bias + n + 1) : 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const TcRow& r = rows[h];
+      if (!r.valid) continue;
+      float f[2] = {fmaxf(__fadd_rn(v[4 * j + 2 * h], b0), floor_v), fmaxf(__fadd_rn(v[4 * j + 2 * h + 1], b1), floor_v)};
+      amax = fmaxf(amax, fmaxf(fabsf(f[0]), fabsf(f[1])));
+      long long off = r.row_off + n;
+      if (p.out_mode == OUT_D2S_SPLIT) {             // a column pair never straddles a parity class (cq is even)
+        const int cls = n / cq, co = n - cls * cq;
+        off = ((long long)(r.b * 2 * p.OH + 2 * r.i + (cls >> 1)) * (2 * p.OW) + 2 * r.j + (cls & 1)) * cq + co;
+      }
+      tc_store_f16<PLANES>(f, p.out_scale, p.out_hi, p.out_lo, off);
+    }
+  }
+  if (p.range_flag != nullptr && !(amax * p.out_scale < TC_F16_OVERFLOW)) atomicOr(p.range_flag, p.range_bit);
+}
+
+// Tile counts of a tc_gemm_kernel launch: n N tiles, m M tiles, count = n * m * K splits
+struct TcTiles {
+  int n, m, count;
+};
+
+// launches tc_gemm_kernel over tiles = (M tiles, N tiles, K splits) with min(SM count, tiles) persistent CTAs; planes = 1 runs
+// the single-pass (hi-only) instantiation
+int tc_launch_layer(const TcLayer& T, dim3 tiles, cudaStream_t s, int planes);
 int tc_dev_alloc(void** p, size_t bytes);
 // Tensor maps + packed-weight storage of a layer whose A operand is a PLAIN NHWC tensor [B_pad, in_h, in_w, in_c] in `planes`
 // planes (taps = unit-stride boxes): allocates T.in, fills tm_a, allocates T.w [ceil(N / TC_N_TILE) * TC_N_TILE][taps * in_c]
