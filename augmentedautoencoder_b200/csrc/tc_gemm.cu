@@ -63,18 +63,19 @@ int make_tmap_f16(CUtensorMap* out, const void* base, int rank, const uint64_t* 
 }
 
 // ------------------------------------------------------------------------------------------------- kernel
-template <int N_TILE, int STAGES, int PLANES = 2>
+// Shared memory: the A ring (p.a_slots slots of [A_hi | A_lo], p.a_rows rows x TC_KCH fp16 per plane) in the first
+// TC_A_RING_BYTES, then W_STAGES stages of [W_hi | W_lo], then the barriers.
+template <int N_TILE, int W_STAGES, int PLANES = 2>
 struct TcSmem {
-  static constexpr int A_BYTES = 128 * TC_KCH * 2;     // 128 rows x TC_KCH fp16
   static constexpr int W_BYTES = N_TILE * TC_KCH * 2;
-  static constexpr int STAGE_BYTES = PLANES * A_BYTES + PLANES * W_BYTES;
-  static constexpr int BODY = STAGES * STAGE_BYTES;
+  static constexpr int W_STAGE_BYTES = PLANES * W_BYTES;
+  static constexpr int BODY = TC_A_RING_BYTES + W_STAGES * W_STAGE_BYTES;
   static constexpr int TOTAL = BODY + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-// One output tile of the launch: linear id t -> (x = N tile, y = M tile, z = K split), N fastest, and its K-iteration range.
+// One output tile of the launch: linear id t -> (x = N tile, y = M tile, z = K split), N fastest, and its (group, chunk) unit range.
 struct TcTile {
-  int m0, n0, z, it_begin, it_end;
+  int m0, n0, z, u_begin, u_end;
 };
 template <int N_TILE>
 __device__ __forceinline__ TcTile tc_tile(const TcGemmParams& p, const TcTiles& g, int t) {
@@ -84,32 +85,40 @@ __device__ __forceinline__ TcTile tc_tile(const TcGemmParams& p, const TcTiles& 
   r.z = yz / g.m;
   r.m0 = y * 128;
   r.n0 = (t - yz * g.n) * N_TILE;
-  r.it_begin = r.z * p.iters_per_split;
-  r.it_end = min(p.taps * p.chunks_per_tap, r.it_begin + p.iters_per_split);
+  r.u_begin = r.z * p.units_per_split;
+  r.u_end = min(p.groups * p.chunks_per_tap, r.u_begin + p.units_per_split);
   return r;
 }
 
 // Warp roles (384 threads): warp 0 TMA producer (warps 1-3 idle), warpgroups 1 and 2 (warps 4-11) issue the wgmma for pixel rows
 // [0,64) and [64,128) of the tile and run the epilogue on their own fragments.
+// K loop: per (tap group, 64-channel chunk) unit one A box lands in the A ring, and per tap of the group one W box in the W
+// ring; each tap's MMAs read the shared A box from its own row offset (tc_plan_groups), so a 5 x 5 stride-2 conv loads 10 halo
+// boxes per chunk instead of 25 tap boxes.  A W stage is freed once its MMAs have retired, an A slot once its group's last
+// tap's have.
 // Persistent grid (see tc_launch_layer): CTA b takes tiles b, b + gridDim.x, ...  Producer and consumers walk the same tiles and
-// K ranges, so one running K-iteration count i over all of the CTA's tiles gives both sides stage i % STAGES and phase
-// (i / STAGES) & 1; the producer runs up to STAGES iterations ahead, into the next tile while the consumers finish this one.
+// K ranges, so running slot/phase counters over all of the CTA's tiles agree on both sides; the producer runs up to the ring
+// depths ahead, into the next tile while the consumers finish this one.
 // Epilogue overlap: at the end of a tile the consumers only fold the accumulators into the unscaled values v and start the next
 // tile; the rest of the epilogue (bias, ReLU, split, stores) runs in two column halves while the MMAs of the next tile's first
-// and second stage execute, so the tensor cores do not wait for it.  v needs a third register array beside acc and crs, so the
+// and second W stage execute, so the tensor cores do not wait for it.  v needs a third register array beside acc and crs, so the
 // producer warpgroup gives up registers (setmaxnreg) and the consumers hold it without spilling.
 // PLANES = 2: (hi, lo) operands, three products per K step; PLANES = 1: hi operands only (the lo maps are not read), one product.
-template <int N_TILE, int STAGES, int PLANES = 2>
+template <int N_TILE, int W_STAGES, int PLANES = 2>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constant__ CUtensorMap tm_a_lo,
                const __grid_constant__ CUtensorMap tm_w_hi, const __grid_constant__ CUtensorMap tm_w_lo, const TcGemmParams p,
                const TcTiles tiles) {
-  using S = TcSmem<N_TILE, STAGES, PLANES>;
+  using S = TcSmem<N_TILE, W_STAGES, PLANES>;
   constexpr int R = N_TILE / 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::BODY);
-  uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + S::BODY);
+  uint64_t* a_empty = a_full + TC_A_SLOTS_MAX;
+  uint64_t* w_full = a_empty + TC_A_SLOTS_MAX;
+  uint64_t* w_empty = w_full + W_STAGES;
+  uint8_t* w_ring = smem + TC_A_RING_BYTES;
+  const int a_plane = p.a_rows * TC_KCH * 2, a_slot = PLANES * a_plane;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -119,35 +128,42 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
     if constexpr (PLANES == 2) prefetch_tmap(&tm_a_lo);
     prefetch_tmap(&tm_w_hi);
     if constexpr (PLANES == 2) prefetch_tmap(&tm_w_lo);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
+    for (int s = 0; s < p.a_slots; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 2); }
+    for (int s = 0; s < W_STAGES; ++s) { mbar_init(&w_full[s], 1); mbar_init(&w_empty[s], 2); }
     fence_barrier_init();
   }
   __syncthreads();
 
   if (warp < 4) {
     setmaxnreg_dec<TC_PRODUCER_REGS>();
-    // ===================== TMA producer: stage = [A_hi | A_lo | W_hi | W_lo], the lo boxes with PLANES = 2 only =====================
+    // ===================== TMA producer: A slot = [A_hi | A_lo], W stage = [W_hi | W_lo], the lo boxes with PLANES = 2 only =====================
     if (warp == 0 && lane == 0) {
       const int hw = p.OH * p.OW;
-      int i = 0;
+      int ia = 0, iw = 0;
       for (int t = blockIdx.x; t < tiles.count; t += gridDim.x) {
         const TcTile T = tc_tile<N_TILE>(p, tiles, t);
         const int b0 = T.m0 / hw, rem = T.m0 - b0 * hw;
         const int oh0 = rem / p.OW, ow0 = rem - oh0 * p.OW;
-        for (int it = T.it_begin; it < T.it_end; ++it, ++i) {
-          const int s = i % STAGES;
-          const uint32_t ph = (uint32_t)(i / STAGES) & 1u;
-          mbar_wait(&empty_bar[s], ph ^ 1u);
-          const int tap = it / p.chunks_per_tap, cc = it - tap * p.chunks_per_tap;
-          uint8_t* st = smem + s * S::STAGE_BYTES;
-          mbar_arrive_expect_tx(&full_bar[s], S::STAGE_BYTES);
-          const int c0 = p.tap_ch[tap] + cc * TC_KCH;
-          const int x = ow0 + p.tap_dj[tap], y = oh0 + p.tap_di[tap];
-          const int kcol = it * TC_KCH;
-          tma_load_4d(st, &tm_a_hi, &full_bar[s], c0, x, y, b0);
-          if constexpr (PLANES == 2) tma_load_4d(st + S::A_BYTES, &tm_a_lo, &full_bar[s], c0, x, y, b0);
-          tma_load_2d(st + PLANES * S::A_BYTES, &tm_w_hi, &full_bar[s], kcol, T.n0);
-          if constexpr (PLANES == 2) tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tm_w_lo, &full_bar[s], kcol, T.n0);
+        for (int u = T.u_begin; u < T.u_end; ++u, ++ia) {
+          const int g = u / p.chunks_per_tap, cc = u - g * p.chunks_per_tap;
+          const int sa = ia & (p.a_slots - 1);
+          mbar_wait(&a_empty[sa], (ia & p.a_slots) ? 0u : 1u);
+          uint8_t* a = smem + sa * a_slot;
+          mbar_arrive_expect_tx(&a_full[sa], a_slot);
+          const int c0 = p.grp_ch[g] + cc * TC_KCH;
+          const int x = ow0 + p.grp_dx[g], y = oh0 + p.grp_dy[g];
+          tma_load_4d(a, &tm_a_hi, &a_full[sa], c0, x, y, b0);
+          if constexpr (PLANES == 2) tma_load_4d(a + a_plane, &tm_a_lo, &a_full[sa], c0, x, y, b0);
+          const int first = p.grp_first[g], ntaps = p.grp_ntaps[g];
+          for (int k = 0; k < ntaps; ++k, ++iw) {
+            const int sw = iw % W_STAGES;
+            mbar_wait(&w_empty[sw], ((uint32_t)(iw / W_STAGES) & 1u) ^ 1u);
+            uint8_t* w = w_ring + sw * S::W_STAGE_BYTES;
+            mbar_arrive_expect_tx(&w_full[sw], S::W_STAGE_BYTES);
+            const int kcol = (p.grp_tap[first + k] * p.chunks_per_tap + cc) * TC_KCH;
+            tma_load_2d(w, &tm_w_hi, &w_full[sw], kcol, T.n0);
+            if constexpr (PLANES == 2) tma_load_2d(w + S::W_BYTES, &tm_w_lo, &w_full[sw], kcol, T.n0);
+          }
         }
       }
     }
@@ -155,58 +171,79 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tm_a_hi, const __grid_constan
     // ===================== wgmma consumers =====================
     setmaxnreg_inc<TC_CONSUMER_REGS>();
     const int wg = (warp - 4) >> 2;
-    const bool releases = (warp & 3) == 0 && lane == 0;   // one arrive per warpgroup on a stage's empty barrier (count 2)
+    const bool releases = (warp & 3) == 0 && lane == 0;   // one arrive per warpgroup on a slot's or stage's empty barrier (count 2)
     constexpr int H = R / 8;                              // column groups per epilogue half (R / 4 groups of 8 columns)
     float acc[R], crs[R], v[R];
 #pragma unroll
     for (int j = 0; j < R; ++j) { acc[j] = 0.f; crs[j] = 0.f; v[j] = 0.f; }
-    // the previous tile, whose values v still wait for epilogue halves [half, 2)
-    int pm0 = 0, pn0 = 0, pz = 0, half = 2;
+    // the previous tile (id pt), whose values v still wait for epilogue halves [half, 2)
+    int pt = 0, half = 2;
     auto epilogue_half = [&](int h) {
-      if (h == 0) tc_epilogue_frag<PLANES, 0, H>(p, v, pm0, pn0, pz, warp, lane);
-      else tc_epilogue_frag<PLANES, H, 2 * H>(p, v, pm0, pn0, pz, warp, lane);
+      const TcTile P = tc_tile<N_TILE>(p, tiles, pt);
+      if (h == 0) tc_epilogue_frag<PLANES, 0, H>(p, v, P.m0 + wg * 64, P.n0, P.z, warp, lane);
+      else tc_epilogue_frag<PLANES, H, 2 * H>(p, v, P.m0 + wg * 64, P.n0, P.z, warp, lane);
     };
-    int i = 0;
+    // running counts: A slot ia & (a_slots - 1), phase bit (ia & a_slots) (a_slots is a power of two); W stage iw % W_STAGES,
+    // phase (iw / W_STAGES) & 1
+    int ia = 0, iw = 0;
     for (int t = blockIdx.x; t < tiles.count; t += gridDim.x) {
       const TcTile T = tc_tile<N_TILE>(p, tiles, t);
-      for (int it = T.it_begin; it < T.it_end; ++it, ++i) {
-        const int s = i % STAGES;
-        mbar_wait(&full_bar[s], (uint32_t)(i / STAGES) & 1u);
-        const uint32_t st = smem_u32(smem + s * S::STAGE_BYTES);
-        const uint32_t a_off = (uint32_t)(wg * 64 * TC_KCH * 2);
-        const uint64_t a_hi = make_sw128_kmajor_desc(st + a_off);
-        const uint64_t a_lo = make_sw128_kmajor_desc(st + S::A_BYTES + a_off);
-        const uint64_t w_hi = make_sw128_kmajor_desc(st + PLANES * S::A_BYTES);
-        const uint64_t w_lo = make_sw128_kmajor_desc(st + 2 * S::A_BYTES + S::W_BYTES);
-        wgmma_fence_regs(acc);
-        if constexpr (PLANES == 2) wgmma_fence_regs(crs);
-        wgmma_fence();
+      for (int u = T.u_begin; u < T.u_end; ++u, ++ia) {
+        const int g = u / p.chunks_per_tap;
+        const int sa = ia & (p.a_slots - 1);
+        mbar_wait(&a_full[sa], (ia & p.a_slots) ? 1u : 0u);
+        const int first = p.grp_first[g], ntaps = p.grp_ntaps[g];
+        for (int k = 0; k < ntaps; ++k, ++iw) {
+          const int sw = iw % W_STAGES;
+          mbar_wait(&w_full[sw], (uint32_t)(iw / W_STAGES) & 1u);
+          // a tap's slice starts a whole number of 8-row swizzle atoms into the box (tc_plan_groups), so the descriptor of the
+          // 128-byte-swizzle layout only moves its start address
+          const uint32_t a_tap = smem_u32(smem + sa * a_slot) + (uint32_t)((wg * p.a_wg_rows + p.grp_row[first + k]) * TC_KCH * 2);
+          const uint32_t st = smem_u32(w_ring + sw * S::W_STAGE_BYTES);
+          const uint64_t a_hi = make_sw128_kmajor_desc(a_tap);
+          const uint64_t a_lo = make_sw128_kmajor_desc(a_tap + (uint32_t)a_plane);
+          const uint64_t w_hi = make_sw128_kmajor_desc(st);
+          const uint64_t w_lo = make_sw128_kmajor_desc(st + S::W_BYTES);
+          const bool accumulate = u > T.u_begin || k > 0;
+          wgmma_fence_regs(acc);
+          if constexpr (PLANES == 2) wgmma_fence_regs(crs);
+          wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < TC_KCH / 16; ++k) {
-          // The tensor core truncates when it adds into a large fp32 accumulator, so the 2^-11-sized cross terms get an
-          // accumulator of their own (small magnitude -> negligible truncation) and are folded in by the epilogue in RN fp32.
-          const uint32_t first = (it > T.it_begin || k > 0) ? 1u : 0u;
-          Wgmma<N_TILE>::template ss<0, 0>(acc, desc_advance_k(a_hi, k), desc_advance_k(w_hi, k), first);
-          if constexpr (PLANES == 2) {
-            Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_lo, k), desc_advance_k(w_hi, k), first);
-            Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_hi, k), desc_advance_k(w_lo, k), 1u);
+          for (int kk = 0; kk < TC_KCH / 16; ++kk) {
+            // The tensor core truncates when it adds into a large fp32 accumulator, so the 2^-11-sized cross terms get an
+            // accumulator of their own (small magnitude -> negligible truncation) and are folded in by the epilogue in RN fp32.
+            const uint32_t scale_d = (accumulate || kk > 0) ? 1u : 0u;
+            Wgmma<N_TILE>::template ss<0, 0>(acc, desc_advance_k(a_hi, kk), desc_advance_k(w_hi, kk), scale_d);
+            if constexpr (PLANES == 2) {
+              Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_lo, kk), desc_advance_k(w_hi, kk), scale_d);
+              Wgmma<N_TILE>::template ss<0, 0>(crs, desc_advance_k(a_hi, kk), desc_advance_k(w_lo, kk), 1u);
+            }
+          }
+          wgmma_commit();
+          if (half < 2) epilogue_half(half++);          // the previous tile's stores, while this stage's MMAs run
+          wgmma_wait<1>();                                // the previous W stage's MMAs have read their operands: free it
+          wgmma_fence_regs(acc);
+          if constexpr (PLANES == 2) wgmma_fence_regs(crs);
+          if (accumulate && releases) {
+            mbar_arrive(&w_empty[(iw - 1) % W_STAGES]);
+            // that stage was the previous group's last tap: its A slot is free too
+            if (k == 0) mbar_arrive(&a_empty[(ia - 1) & (p.a_slots - 1)]);
           }
         }
-        wgmma_commit();
-        if (half < 2) epilogue_half(half++);          // the previous tile's stores, while this stage's MMAs run
-        wgmma_wait<1>();                                // the previous stage's MMAs have read their operands: free it
-        wgmma_fence_regs(acc);
-        if constexpr (PLANES == 2) wgmma_fence_regs(crs);
-        if (it > T.it_begin && releases) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if constexpr (PLANES == 2) wgmma_fence_regs(crs);
-      // the tile's last stage is free as well: without this arrive the producer would wait for it forever on a later tile
-      if (T.it_end > T.it_begin && releases) mbar_arrive(&empty_bar[(i - 1) % STAGES]);
+      // the tile's last W stage and A slot are free as well: without these arrives the producer would wait for them forever on
+      // a later tile
+      const bool has_work = T.u_end > T.u_begin;
+      if (has_work && releases) {
+        mbar_arrive(&w_empty[(iw - 1) % W_STAGES]);
+        mbar_arrive(&a_empty[(ia - 1) & (p.a_slots - 1)]);
+      }
       while (half < 2) epilogue_half(half++);         // a tile of fewer than two K stages did not cover the previous epilogue
-      tc_epilogue_values<PLANES>(p, acc, crs, T.it_end > T.it_begin, v);
-      pm0 = T.m0 + wg * 64; pn0 = T.n0; pz = T.z; half = 0;
+      tc_epilogue_values<PLANES>(p, acc, crs, has_work, v);
+      pt = t; half = 0;
     }
     while (half < 2) epilogue_half(half++);
   }
@@ -319,26 +356,80 @@ int TcPlanes::encode(TcMaps& m, int rank, const uint64_t* dims, const uint64_t* 
 // tiles = (m_tiles, n_tiles, splits).  min(SM count, tiles) persistent CTAs walk the linear tile id with stride gridDim.x, N tile
 // fastest, so the N tiles of an M tile run side by side and read the activation tile (and its 5 x 5 tap re-reads) while it is
 // in L2; M first would put all resident CTAs on one weight column and stream every activation tile from HBM once per N tile.
-// Stage counts: the split kernel's 3 stages of 64 KB and the single-pass kernel's 6 stages of 32 KB are the same 192 KB ring,
-// so both keep the same bytes in flight and the same shared-memory footprint (and carveout); the single pass gets twice the
-// K-iterations of look-ahead.
-constexpr int TC_STAGES_SPLIT = 3, TC_STAGES_FP16 = 6;
-static_assert(TcSmem<TC_N_TILE, TC_STAGES_FP16, 1>::TOTAL == TcSmem<TC_N_TILE, TC_STAGES_SPLIT>::TOTAL, "same footprint");
+// W ring depths: the split kernel's 3 stages of 32 KB and the single-pass kernel's 6 stages of 16 KB are the same 96 KB, and
+// both share the 128 KB A ring (2 encoder halo slots of up to 48 KB split, 4 single-pass), so both have the same
+// shared-memory footprint (and carveout) and the single pass gets twice the look-ahead.
+constexpr int TC_W_STAGES_SPLIT = 3, TC_W_STAGES_FP16 = 6;
+static_assert(TcSmem<TC_N_TILE, TC_W_STAGES_FP16, 1>::TOTAL == TcSmem<TC_N_TILE, TC_W_STAGES_SPLIT>::TOTAL, "same footprint");
+static_assert(TcSmem<TC_N_TILE, TC_W_STAGES_SPLIT>::TOTAL <= 227 * 1024, "tc_gemm_kernel: shared memory over the sm_90 limit");
+
+int tc_plan_groups(TcLayer& T, int planes, const uint64_t* dims, const uint64_t* strides_bytes) {
+  TcGemmParams& g = T.gp;
+  AAE_REQUIRE(g.taps >= 1 && g.taps <= 32, "tc plan: %d taps (at most 32)", g.taps);
+  AAE_REQUIRE(T.BW * T.BH * T.BB == 128, "tc plan: box %d x %d x %d is not one 128-row tile", T.BW, T.BH, T.BB);
+  const int halo_rows = (T.BH + 2) * T.BW * T.BB;
+  bool halo = g.taps > 1 && T.BW % 8 == 0 && (T.BB == 1 || (T.BB == 2 && T.BH * T.BW == 64)) &&
+              2 * planes * halo_rows * TC_KCH * 2 <= TC_A_RING_BYTES && T.BH + 2 <= 256;
+  for (int t = 0; t < g.taps; ++t) halo = halo && g.tap_di[t] >= -1 && g.tap_di[t] <= 1;
+  g.groups = 0;
+  for (int t = 0; t < g.taps; ++t) {
+    int grp = -1;
+    for (int q = 0; halo && q < g.groups; ++q)
+      if (g.grp_ch[q] == g.tap_ch[t] && g.grp_dx[q] == g.tap_dj[t]) grp = q;
+    if (grp < 0) {
+      grp = g.groups++;
+      g.grp_ch[grp] = g.tap_ch[t];
+      g.grp_dx[grp] = g.tap_dj[t];
+      g.grp_dy[grp] = (int8_t)(halo ? -1 : g.tap_di[t]);
+      g.grp_ntaps[grp] = 0;
+    }
+    g.grp_ntaps[grp]++;
+  }
+  // taps in group order, K order within a group
+  int n = 0;
+  for (int q = 0; q < g.groups; ++q) {
+    g.grp_first[q] = (int8_t)n;
+    for (int t = 0; t < g.taps; ++t) {
+      if (halo ? (g.grp_ch[q] != g.tap_ch[t] || g.grp_dx[q] != g.tap_dj[t]) : t != q) continue;
+      g.grp_tap[n] = (int8_t)t;
+      g.grp_row[n] = (int16_t)(halo ? (g.tap_di[t] + 1) * T.BW : 0);
+      ++n;
+    }
+  }
+  AAE_REQUIRE(n == g.taps, "tc plan: tap groups cover %d of %d taps", n, g.taps);
+  g.a_rows = halo ? halo_rows : 128;
+  g.a_wg_rows = halo && T.BB == 2 ? (T.BH + 2) * T.BW : 64;
+  const int slot_bytes = planes * g.a_rows * TC_KCH * 2;
+  // a power of two, so that the kernel's running count gives slot and phase with a mask
+  g.a_slots = 1;
+  while (2 * g.a_slots <= TC_A_SLOTS_MAX && 2 * g.a_slots * slot_bytes <= TC_A_RING_BYTES) g.a_slots *= 2;
+  AAE_REQUIRE(g.a_slots >= 2, "tc plan: an A slot of %d bytes leaves fewer than two in the ring", slot_bytes);
+  // every slice a wgmma descriptor starts at must be 1024-byte (8-row swizzle atom) aligned
+  AAE_REQUIRE(g.a_rows % 8 == 0 && g.a_wg_rows % 8 == 0, "tc plan: A box rows %d / warpgroup offset %d off the 8-row atom", g.a_rows, g.a_wg_rows);
+  for (int i = 0; i < n; ++i) AAE_REQUIRE(g.grp_row[i] % 8 == 0 && g.grp_row[i] + g.a_wg_rows + 64 <= g.a_rows, "tc plan: tap row %d outside the A box", g.grp_row[i]);
+  g.units_per_split = g.groups * g.chunks_per_tap;
+  if (!halo) return AAE_OK;
+  const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)(T.BH + 2), (uint32_t)T.BB};
+  return T.in.encode(T.tm_halo, 4, dims, strides_bytes, box);
+}
 
 int tc_launch_layer(const TcLayer& T, dim3 tiles, cudaStream_t s, int planes) {
   const long long count = (long long)tiles.x * tiles.y * tiles.z;
   AAE_REQUIRE(count <= INT_MAX, "tc_gemm: %lld tiles exceed the kernel's int tile index", count);
+  AAE_REQUIRE(T.gp.a_slots >= 2 && T.gp.a_slots <= TC_A_SLOTS_MAX && (T.gp.a_slots & (T.gp.a_slots - 1)) == 0 &&
+              T.gp.a_slots * planes * T.gp.a_rows * TC_KCH * 2 <= TC_A_RING_BYTES, "tc_gemm: layer without a tap-group plan");
   int device = 0, sms = 0;
   AAE_CUDA_OK(cudaGetDevice(&device));
   AAE_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
   const TcTiles g{(int)tiles.y, (int)tiles.x, (int)count};
   const unsigned ctas = (unsigned)std::min<long long>(count, sms);
+  const TcMaps& a = T.gp.a_rows == 128 ? T.tm_a : T.tm_halo;
   return with_planes(planes, [&](auto P) {
-    constexpr int STAGES = P == 1 ? TC_STAGES_FP16 : TC_STAGES_SPLIT;
-    using S = TcSmem<TC_N_TILE, STAGES, P>;
-    auto kern = tc_gemm_kernel<TC_N_TILE, STAGES, P>;
+    constexpr int W_STAGES = P == 1 ? TC_W_STAGES_FP16 : TC_W_STAGES_SPLIT;
+    using S = TcSmem<TC_N_TILE, W_STAGES, P>;
+    auto kern = tc_gemm_kernel<TC_N_TILE, W_STAGES, P>;
     AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    kern<<<ctas, TC_THREADS, S::TOTAL, s>>>(T.tm_a.hi, T.tm_a.lo, T.tm_w.hi, T.tm_w.lo, T.gp, g);
+    kern<<<ctas, TC_THREADS, S::TOTAL, s>>>(a.hi, a.lo, T.tm_w.hi, T.tm_w.lo, T.gp, g);
     AAE_LAUNCH_OK();
     return AAE_OK;
   });
@@ -390,17 +481,20 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
     if ((st = T.in.alloc((size_t)B_pad * T.in_h * T.in_w * T.in_c, planes)) != AAE_OK) break;
     if ((st = T.w.alloc((size_t)T.out_c * T.taps * T.in_c, planes)) != AAE_OK) break;
     // ---- tensor maps ----
+    uint64_t a_dims[4], a_strides[3];
     if (!dense) {
       const uint64_t C4 = 4ull * T.in_c, W2 = T.in_w / 2, H2 = T.in_h / 2;
       const uint64_t dims[4] = {C4, W2, H2, (uint64_t)B_pad};
       const uint64_t strides[3] = {C4 * 2, W2 * C4 * 2, H2 * W2 * C4 * 2};
-      const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
-      if ((st = T.in.encode(T.tm_a, 4, dims, strides, box)) != AAE_OK) break;
+      memcpy(a_dims, dims, sizeof(dims)); memcpy(a_strides, strides, sizeof(strides));
     } else {
       const uint64_t dims[4] = {(uint64_t)T.in_c, 1, 1, (uint64_t)B_pad};
       const uint64_t strides[3] = {(uint64_t)T.in_c * 2, (uint64_t)T.in_c * 2, (uint64_t)T.in_c * 2};
-      const uint32_t box[4] = {(uint32_t)TC_KCH, 1, 1, 128};
-      if ((st = T.in.encode(T.tm_a, 4, dims, strides, box)) != AAE_OK) break;
+      memcpy(a_dims, dims, sizeof(dims)); memcpy(a_strides, strides, sizeof(strides));
+    }
+    {
+      const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};   // dense: [64, 1, 1, 128]
+      if ((st = T.in.encode(T.tm_a, 4, a_dims, a_strides, box)) != AAE_OK) break;
     }
     {
       const uint64_t K = (uint64_t)T.taps * T.in_c;
@@ -413,7 +507,6 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
     TcGemmParams& g = T.gp;
     g.N = T.out_c; g.OH = T.out_h; g.OW = T.out_w; g.BW = T.BW; g.BH = T.BH;
     g.taps = T.taps; g.chunks_per_tap = T.in_c / TC_KCH;
-    g.iters_per_split = g.taps * g.chunks_per_tap;
     for (int t = 0; t < T.taps; ++t) {
       if (dense) { g.tap_di[t] = 0; g.tap_dj[t] = 0; g.tap_ch[t] = 0; continue; }
       const int kh = t / 5, kw = t % 5;
@@ -422,6 +515,8 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
       g.tap_dj[t] = (int8_t)((kw + 1) / 2 - 1);
       g.tap_ch[t] = ((((kh + 1) & 1) << 1) | ((kw + 1) & 1)) * T.in_c;
     }
+    // 5 x 5 stride 2: taps of one kw and one row parity (kh in {0, 2, 4} or {1, 3}) share a halo box -> 10 groups
+    if ((st = tc_plan_groups(T, planes, a_dims, a_strides)) != AAE_OK) break;
     g.unscale = 1.f / (ACT_SCALE * W_SCALE);
     g.out_scale = ACT_SCALE;
     g.relu = dense ? 0 : 1;
@@ -437,10 +532,10 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
       g.out_mode = (i + 2 == h->layers.size()) ? OUT_PLAIN_SPLIT : OUT_S2D_SPLIT;
     }
     TcLayer& D = h->layers.back();
-    const int total = D.gp.taps * D.gp.chunks_per_tap;
+    const int total = D.gp.groups * D.gp.chunks_per_tap;     // one tap: units are chunks
     h->dense_splits = std::min(total, 66);
-    D.gp.iters_per_split = (total + h->dense_splits - 1) / h->dense_splits;
-    h->dense_splits = (total + D.gp.iters_per_split - 1) / D.gp.iters_per_split;
+    D.gp.units_per_split = (total + h->dense_splits - 1) / h->dense_splits;
+    h->dense_splits = (total + D.gp.units_per_split - 1) / D.gp.units_per_split;
     D.gp.out_mode = OUT_F32;
     st = dev_alloc((void**)&h->partials, (size_t)h->dense_splits * (B + 128) * cfg->latent * sizeof(float));
     D.gp.out_f32 = h->partials;
@@ -551,9 +646,9 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
     }
     if (splits > 1) {
       TcLayer S = T;                                   // same operands and maps, partial sums out
-      const int total_iters = T.gp.taps * T.gp.chunks_per_tap;
-      S.gp.iters_per_split = (int)ceil_div(total_iters, splits);
-      splits = (int)ceil_div(total_iters, S.gp.iters_per_split);
+      const int total_units = T.gp.groups * T.gp.chunks_per_tap;   // K is cut on (tap group, chunk) boundaries
+      S.gp.units_per_split = (int)ceil_div(total_units, splits);
+      splits = (int)ceil_div(total_units, S.gp.units_per_split);
       S.gp.out_mode = OUT_F32;
       S.gp.out_f32 = h->fwd_partials;
       grid.z = (unsigned)splits;
@@ -678,6 +773,7 @@ int tc_layer_setup_plain(TcLayer& T, int B, int planes) {
     const uint64_t strides[3] = {(uint64_t)T.in_c * 2, (uint64_t)T.in_w * T.in_c * 2, (uint64_t)T.in_h * T.in_w * T.in_c * 2};
     const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
     AAE_TRY(T.in.encode(T.tm_a, 4, dims, strides, box));
+    AAE_TRY(tc_plan_groups(T, planes, dims, strides));   // 3 x 3 taps: one group per column offset dj
   }
   const uint64_t dims[2] = {K, (uint64_t)rows};
   const uint64_t strides[1] = {K * 2};
@@ -732,7 +828,6 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
       }
     }
     g.BW = T.BW; g.BH = T.BH; g.taps = T.taps; g.chunks_per_tap = T.in_c / TC_KCH;
-    g.iters_per_split = g.taps * g.chunks_per_tap;
     for (int t = 0; t < T.taps; ++t) {
       g.tap_di[t] = (int8_t)(T.taps == 1 ? 0 : t / 3 - 1);
       g.tap_dj[t] = (int8_t)(T.taps == 1 ? 0 : t % 3 - 1);

@@ -25,9 +25,20 @@ struct TcGemmParams {
   int BW, BH;            // pixel box of one 128-row tile: BW*BH*BB = 128
   int taps;              // 25 (conv) or 1 (dense)
   int chunks_per_tap;    // Cin / 64
-  int iters_per_split;   // K iterations (tap, chunk) handled per blockIdx.z
+  int units_per_split;   // K units (tap group, chunk) handled per blockIdx.z
   int8_t tap_di[32], tap_dj[32];
   int tap_ch[32];        // channel offset of the tap's parity plane in the space-to-depth tensor
+  // Tap groups (tc_plan_groups): the K loop runs group -> 64-channel chunk -> tap of the group.  Per chunk, group g loads ONE
+  // A box (channels grp_ch[g] + 64 chunk, columns ow0 + grp_dx[g], rows from oh0 + grp_dy[g]) and each of its taps
+  // grp_tap[grp_first[g] ..+ grp_ntaps[g]) (K order) reads that box from row grp_row[.] on, beside its own W stage.
+  int groups;
+  int a_rows;            // rows per plane of an A box: 128, or (BH + 2) BW BB for a halo box
+  int a_wg_rows;         // first row of consumer warpgroup 1's 64-row slice in an A box
+  int a_slots;           // depth of the A ring (a power of two)
+  int grp_ch[32];
+  int8_t grp_dy[32], grp_dx[32], grp_first[32], grp_ntaps[32];
+  int8_t grp_tap[32];
+  int16_t grp_row[32];
   float unscale;         // 1 / (scale_A * scale_W)
   const unsigned* amax_bits;  // optional: the A operand was scaled by tc_dyn_scale(*amax_bits) (training gradients); folded into unscale
   float out_scale;       // scale applied before the hi/lo split of the output (next layer's scale_A)
@@ -65,6 +76,8 @@ constexpr int TC_N_TILE = 128;        // output channels per GEMM tile
 // the 384 x 168 the launch reserves
 constexpr int TC_PRODUCER_REGS = 24, TC_CONSUMER_REGS = 240;
 constexpr int TC_KCH = 64;            // K chunk per pipeline stage: 64 fp16 = one 128-byte swizzle row
+// tc_gemm_kernel's A ring: a_slots = the largest power of two <= min(TC_A_SLOTS_MAX, TC_A_RING_BYTES / slot bytes), at least two
+constexpr int TC_A_RING_BYTES = 128 * 1024, TC_A_SLOTS_MAX = 8;
 
 // Tensor maps of both planes of an operand.  Without a lo plane, lo is a copy of hi: the kernels never read it, and every launch
 // passes the pair as it is.
@@ -96,6 +109,7 @@ struct TcLayer {
   TcPlanes in;                                  // activations entering this layer
   TcPlanes w;                                   // packed weights [out_c][taps*in_c]
   TcMaps tm_a, tm_w;
+  TcMaps tm_halo;                               // A boxes of BH + 2 rows, when gp groups its taps (gp.a_rows != 128)
   TcGemmParams gp;
 };
 
@@ -370,5 +384,11 @@ int tc_dev_alloc(void** p, size_t bytes);
 // planes (taps = unit-stride boxes): allocates T.in, fills tm_a, allocates T.w [ceil(N / TC_N_TILE) * TC_N_TILE][taps * in_c]
 // and fills tm_w.  T.{in_h,in_w,in_c,taps,BW,BH,BB,gp.N} must be set.
 int tc_layer_setup_plain(TcLayer& T, int B, int planes);
+// Tap groups of a layer whose tap tables (gp.taps, tap_di/dj/ch, chunks_per_tap) and T.{BW,BH,BB} are set; dims/strides describe
+// T.in as tm_a does.  Taps with the same (tap_ch, tap_dj) and di in {-1, 0, 1} share a halo box [64, BW, BH + 2, BB] at row
+// oh0 - 1 (encoded into T.tm_halo) when every warpgroup slice starts on a whole 8-row swizzle atom (BW % 8 == 0), each warpgroup
+// reads one contiguous box (BB == 1, or BB == 2 with BH BW == 64) and two halo slots fit the A ring; otherwise every tap is a
+// group of its own with today's BH-row box.  Sets units_per_split to the whole K range (no split).
+int tc_plan_groups(TcLayer& T, int planes, const uint64_t* dims, const uint64_t* strides_bytes);
 
 }  // namespace aae

@@ -543,7 +543,7 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     }
     TcGemmParams& g = T.gp;
     g.N = U.nd; g.OH = U.gh; g.OW = U.gw; g.BW = T.BW; g.BH = T.BH;
-    g.taps = T.taps; g.chunks_per_tap = U.gN / TC_KCH; g.iters_per_split = g.taps * g.chunks_per_tap;
+    g.taps = T.taps; g.chunks_per_tap = U.gN / TC_KCH;
     for (int t = 0; t < T.taps; ++t) {
       g.tap_di[t] = (int8_t)(T.taps == 1 ? 0 : t / 3 - 1);
       g.tap_dj[t] = (int8_t)(T.taps == 1 ? 0 : t % 3 - 1);
@@ -737,14 +737,15 @@ int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s) {
   T.gp.M = B * U.gh * U.gw;
   T.gp.amax_bits = h->amax + u;
   const int m_tiles = (int)ceil_div(T.gp.M, 128), n_tiles = U.nd / TC_N_TILE;
-  const int total_iters = T.gp.taps * T.gp.chunks_per_tap;
-  // few output tiles and a long K (the 8x8 layers): split K so that the grid covers the SMs, fold the partials afterwards
+  const int total_iters = T.gp.taps * T.gp.chunks_per_tap, total_units = T.gp.groups * T.gp.chunks_per_tap;
+  // few output tiles and a long K (the 8x8 layers): split K so that the grid covers the SMs, fold the partials afterwards;
+  // the splits cut K on (tap group, chunk) boundaries
   int splits = std::max(1, 132 / std::max(1, m_tiles * n_tiles));
   splits = std::min(splits, std::max(1, total_iters / 64));
   const long long mn = (long long)T.gp.M * U.nd;
   if ((size_t)splits * (size_t)mn > h->partial_floats) splits = 1;
-  T.gp.iters_per_split = (int)ceil_div(total_iters, splits);
-  splits = (int)ceil_div(total_iters, T.gp.iters_per_split);
+  T.gp.units_per_split = (int)ceil_div(total_units, splits);
+  splits = (int)ceil_div(total_units, T.gp.units_per_split);
   T.gp.out_f32 = splits > 1 ? h->partials : h->raw;
   dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)splits);
   AAE_TRY(tc_launch_layer(T, grid, s, h->planes));
