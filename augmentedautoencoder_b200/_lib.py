@@ -26,6 +26,7 @@ _P = C.c_void_p
 _I = C.c_int
 _L = C.c_int64
 _F = C.c_float
+_D = C.c_double
 _SIGS = {
     "aae_version": (_I, []),
     "aae_last_error_string": (C.c_char_p, []),
@@ -71,6 +72,7 @@ _SIGS = {
     "aae_trainer_set_global_step": (_I, [_P, _L]),
     "aae_extract_square_patches": (_I, [_P, _I, _I, _P, _I, _F, _I, _P, _P]),
     "aae_augment_batch": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P]),
+    "aae_augment_occlusion": (_I, [_P, _I, _I, _I, _P, _I, _P, _I, _I, _D, _I, _D, _P, _P, _I, _I, _P, _P, _P]),
 }
 
 _lib = None

@@ -11,6 +11,9 @@ Supported chain: any subset of the template's ops IN THE TEMPLATE'S ORDER (Affin
 Multiply, Multiply, ContrastNormalization; another order raises): Sometimes(p, Affine(scale=(a, b))), Sometimes(p, CoarseDropout(p=, size_percent=)),
 Sometimes(p, GaussianBlur(sigma)), Sometimes(p, Add((a, b), per_channel=)), Sometimes(p, Invert(p, per_channel=True)),
 Sometimes(p, Multiply((a, b), per_channel=)), Sometimes(p, ContrastNormalization((a, b), per_channel=)).  Anything else raises.
+
+``Occlusion`` adds the two occlusion switches of the cfg's ``[Augmentation]`` section (REALISTIC_OCCLUSION, SQUARE_OCCLUSION,
+dataset.py:421-454), which edit the masks before the paste; ``aae_augment_occlusion`` applies them.
 """
 import ctypes as C
 
@@ -316,3 +319,150 @@ class Augmenter(object):
                                                 _lib.ptr(out_u) if out_u is not None else None, _lib.ptr(out_f),
                                                 C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "augment batch")
         return (out_f, out_u) if want_u8 else out_f
+
+
+# ----------------------------------------------------------------------------------------------------------- occlusion
+OCCLUSION_BANK_SIDE = 224                  # arbitrary_syn_masks_1000.bin: raw bits of 224 x 224 masks (dataset.py:405-418)
+OCCLUSION_MIN_TRANS, OCCLUSION_MAX_TRANS = 0.2, 0.7      # augment_occlusion_mask's defaults (dataset.py:421)
+SQUARE_P_ON, SQUARE_P_DROP, SQUARE_SIZE_PERCENT = 0.7, 0.4, 0.01    # Sometimes(0.7, CoarseDropout(p=0.4, size_percent=0.01))
+# Cells per side of the square-occlusion dropout grid: max(int(side * 0.01), min_size) = min_size at 128.  min_size is a default
+# of imgaug 0.4.0's CoarseDropout (the version the reference pins), whose source is not available here: 3 is that default as
+# remembered (imgaug 0.2.x used 4).  UNVERIFIED.
+SQUARE_OCCLUSION_MIN_SIZE = 3
+# Candidates per image and step.  Taking the first accepted one in draw order is the reference's unbounded rejection loop
+# conditioned on success within K.  An image whose draws pass with probability p falls back with probability (1 - p)^K:
+# 1.2e-3 at p = 0.1, 6e-7 at p = 0.2.  The kernel stops at the first round of 8 candidates with an accept, so a larger K costs
+# device time only on images that keep failing; on the host it costs 14 draws and 12 bytes of upload per candidate.
+OCCLUSION_CANDIDATES = 64
+
+
+def occlusion_limit(value):
+    """``max_occl`` of an occlusion switch read as the reference reads it (dataset.py:468-471): the cfg string evaluated,
+    as a float; ``False`` / ``0`` (or a missing key) = off."""
+    if value is None:
+        return 0.0
+    return float(eval(str(value), {"__builtins__": {}}))
+
+
+def square_grid(h, w):
+    """Cells (rows, cols) of the square-occlusion dropout grid (imgaug's FromLowerResolution(size_percent, min_size))."""
+    return max(int(h * SQUARE_SIZE_PERCENT), SQUARE_OCCLUSION_MIN_SIZE), max(int(w * SQUARE_SIZE_PERCENT), SQUARE_OCCLUSION_MIN_SIZE)
+
+
+def load_occlusion_bank(path, shape):
+    """The occluder bank of ``Dataset.random_syn_masks`` (dataset.py:405-418) bit-packed: uint32 [n, rows, cols / 32] with bit
+    j of word w = column 32 w + j, as ``aae_augment_occlusion`` reads it.  The reference unpacks the file with bitarray (default
+    big-endian bit order, the order of np.unpackbits), reshapes to 224 x 224 masks and resizes each one with
+    cv2.resize(mask, (shape[0], shape[1]), INTER_NEAREST) -- dsize is (width, height), so the result has shape[1] rows."""
+    bits = np.unpackbits(np.fromfile(path, dtype=np.uint8))
+    side = OCCLUSION_BANK_SIDE
+    if bits.size == 0 or bits.size % (side * side):
+        raise ValueError("%s holds %d bits, not a whole number of %d x %d masks" % (path, bits.size, side, side))
+    rows, cols = int(shape[1]), int(shape[0])
+    if cols % 32:
+        raise NotImplementedError("occlusion masks %d pixels wide: the device step packs rows into 32-bit words" % cols)
+    masks = bits.reshape(-1, side, side)
+    masks = masks[:, nearest_cells(rows, side)][:, :, nearest_cells(cols, side)]
+    return np.ascontiguousarray(np.packbits(masks, axis=-1, bitorder="little")).view("<u4").astype(np.uint32)
+
+
+class Occlusion(object):
+    """REALISTIC_OCCLUSION and SQUARE_OCCLUSION of Dataset.batch (dataset.py:468-471) on the device.  ``realistic`` / ``square``
+    are the switches' ``max_occl`` (0 = off).  Draws come from a RandomState of their own, so the other streams of a batch are
+    the same whether the switches are on or off."""
+
+    def __init__(self, shape, realistic=0.0, square=0.0, seed=None, candidates=OCCLUSION_CANDIDATES):
+        self.h, self.w = int(shape[0]), int(shape[1])
+        if self.h != self.w:
+            raise NotImplementedError("occlusion augmentation needs square crops (the reference mixes the two axes)")
+        if self.w % 32:
+            raise NotImplementedError("occlusion augmentation needs a crop width that is a multiple of 32")
+        self.realistic, self.square = float(realistic), float(square)
+        self.K = int(candidates)
+        self.low = square_grid(self.h, self.w)
+        if self.low[0] * self.low[1] > 32:
+            raise NotImplementedError("square occlusion grids of more than 32 cells are not supported")
+        self.rng = np.random.RandomState(None if seed is None else [int(seed), 1])     # not the Augmenter's RandomState(seed)
+        self._dev = {}
+
+    # -- host: random draws ------------------------------------------------------------------------------------------
+    def sample(self, B, n_bank=0):
+        """Candidates of one batch: occluder index [B] and shifts tx, ty [B, K] (realistic), Sometimes flags [B, K] and keep
+        cells [B, K, rows, cols] (square), in the reference's distributions (dataset.py:424-430, 392-402)."""
+        r, K, P = self.rng, self.K, {}
+        if self.realistic:
+            P["occluder"] = r.choice(n_bank, B)
+            sx, ux, sy, uy = r.choice((-1, 1), (B, K)), r.rand(B, K), r.choice((-1, 1), (B, K)), r.rand(B, K)
+            span = OCCLUSION_MAX_TRANS - OCCLUSION_MIN_TRANS
+            P["tx"] = np.trunc(sx * (ux * span + OCCLUSION_MIN_TRANS) * self.h).astype(np.int32)     # int(): toward zero
+            P["ty"] = np.trunc(sy * (uy * span + OCCLUSION_MIN_TRANS) * self.w).astype(np.int32)
+        if self.square:
+            P["square_on"] = r.rand(B, K) < SQUARE_P_ON
+            P["square_keep"] = r.rand(B, K, *self.low) >= SQUARE_P_DROP
+        return P
+
+    def pack(self, P):
+        """-> int32 [B, 1 + 3K]: occluder, tx[K], ty[K], keep bits[K] (include/aae_b200.h: aae_augment_occlusion)."""
+        K = self.K
+        cells = self.low[0] * self.low[1]
+        B = len(P["occluder"]) if "occluder" in P else len(P["square_on"])
+        cand = np.zeros((B, 1 + 3 * K), np.int32)
+        full = np.uint32((1 << cells) - 1)
+        keep = np.full((B, K), full, np.uint32)
+        if self.realistic:
+            cand[:, 0] = P["occluder"]
+            cand[:, 1:K + 1] = P["tx"]
+            cand[:, K + 1:2 * K + 1] = P["ty"]
+        if self.square:
+            weights = np.uint64(1) << np.arange(cells, dtype=np.uint64)
+            bits = (P["square_keep"].reshape(B, K, cells).astype(np.uint64) * weights).sum(-1, dtype=np.uint64).astype(np.uint32)
+            keep = np.where(P["square_on"], bits, full)
+        cand[:, 2 * K + 1:] = keep.view(np.int32)
+        return cand
+
+    # -- device ------------------------------------------------------------------------------------------------------
+    def _state(self, dev):
+        key = str(dev)
+        if key not in self._dev:
+            self._dev[key] = {
+                "rows": torch.from_numpy(nearest_cells(self.h, self.low[0])).to(dev),
+                "cols": torch.from_numpy(nearest_cells(self.w, self.low[1])).to(dev),
+                "fallbacks": torch.zeros(2, dtype=torch.int32, device=dev),
+                "bank_src": None, "bank": None,
+            }
+        return self._dev[key]
+
+    def apply_device(self, mask, bank=None, params=None):
+        """mask: bool / uint8 CUDA tensor [B,H,W] (True = background); bank: ``load_occlusion_bank`` array (realistic step).
+        Returns the occluded uint8 mask [B,H,W] (1 = background).  Asynchronous; ``fallbacks()`` reads the counters."""
+        dev = mask.device
+        B = int(mask.shape[0])
+        if tuple(mask.shape) != (B, self.h, self.w):
+            raise ValueError("occlusion: mask of shape %s, expected [B, %d, %d]" % (tuple(mask.shape), self.h, self.w))
+        st = self._state(dev)
+        if self.realistic:
+            if bank is None or bank.ndim != 3 or bank.shape[1:] != (self.h, self.w // 32):
+                raise ValueError("realistic occlusion needs an occluder bank of [n, %d, %d] words" % (self.h, self.w // 32))
+            if st["bank_src"] is not bank:                  # one upload per device and bank
+                st["bank"], st["bank_src"] = torch.from_numpy(np.ascontiguousarray(bank, np.uint32).view(np.int32)).to(dev), bank
+        P = params if params is not None else self.sample(B, len(bank) if bank is not None else 0)
+        cand = torch.from_numpy(self.pack(P)).to(dev, non_blocking=True)
+        mask8 = mask.to(torch.uint8).contiguous()
+        out = torch.empty_like(mask8)
+        bank_d = st["bank"] if self.realistic else None
+        _lib.check(_lib.lib().aae_augment_occlusion(
+            _lib.ptr(mask8), B, self.h, self.w, _lib.ptr(bank_d), len(bank_d) if bank_d is not None else 0, _lib.ptr(cand), self.K,
+            int(self.realistic != 0), self.realistic, int(self.square != 0), 1.0 - self.square,      # dataset.py:451: 1-max_occl
+            _lib.ptr(st["rows"]), _lib.ptr(st["cols"]), self.low[0], self.low[1], _lib.ptr(out), _lib.ptr(st["fallbacks"]),
+            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "augment occlusion")
+        return out
+
+    def fallbacks(self):
+        """Images that exhausted their K candidates since the last call, per step: {"realistic": n, "square": n}.  Clears the
+        counters; synchronises the devices that ran the step."""
+        n = np.zeros(2, np.int64)
+        for key, st in self._dev.items():
+            torch.cuda.synchronize(torch.device(key))
+            n += st["fallbacks"].cpu().numpy()
+            st["fallbacks"].zero_()
+        return {"realistic": int(n[0]), "square": int(n[1])}

@@ -3,6 +3,7 @@
 and the square-patch crop helper (dataset.py:354-373).  Rendering / augmentation (OpenGL, imgaug) are out of scope
 (SURVEY.md section 2 rows 7, 11): ``render_embedding_image_batch`` delegates to a user-supplied renderer."""
 import math
+import os
 
 import numpy as np
 
@@ -176,15 +177,46 @@ class Dataset(object):
             raise NotImplementedError("no [Augmentation] CODE in the dataset arguments")
         return Augmenter(code, self.shape, seed=self._kw.get("seed"))
 
+    @lazy_property
+    def _occlusion(self):
+        """The [Augmentation] switches REALISTIC_OCCLUSION / SQUARE_OCCLUSION (dataset.py:468-471); None when both are off."""
+        from .augment import Occlusion, occlusion_limit
+        realistic = occlusion_limit(self._kw.get("realistic_occlusion"))
+        square = occlusion_limit(self._kw.get("square_occlusion"))
+        if not realistic and not square:
+            return None
+        return Occlusion(self.shape, realistic, square, seed=self._kw.get("seed"))
+
+    def load_occlusion_masks(self, path=None):
+        """The occluder bank of REALISTIC_OCCLUSION (``random_syn_masks``, dataset.py:405-418), kept bit-packed (2 KB per
+        128 x 128 mask).  Default path: $AE_WORKSPACE_PATH/random_tless_masks/arbitrary_syn_masks_1000.bin, as the reference."""
+        from .augment import load_occlusion_bank
+        if path is None:
+            ws = os.environ.get("AE_WORKSPACE_PATH")
+            if not ws:
+                raise RuntimeError("REALISTIC_OCCLUSION needs the occluder bank: set AE_WORKSPACE_PATH or call load_occlusion_masks(path)")
+            path = os.path.join(ws, "random_tless_masks", "arbitrary_syn_masks_1000.bin")
+        self.occlusion_masks = load_occlusion_bank(path, self.shape)
+        return len(self.occlusion_masks)
+
+    def occlusion_fallbacks(self):
+        """Images that kept their mask because all their occlusion candidates failed, since the last call: {"realistic": n,
+        "square": n}.  The reference re-draws without bound instead (and never returns for an image without object pixels or
+        whose realistic occlusion already took more than SQUARE_OCCLUSION of it).  Clears the counts; synchronises."""
+        occl = self._occlusion
+        return occl.fallbacks() if occl is not None else {"realistic": 0, "square": 0}
+
     def batch_device(self, batch_size, device=None):
         """Dataset.batch (dataset.py:456-495) with the image work on the GPU: draws the rendering / background indices like the
-        reference, uploads the uint8 images once and returns (x, y) float32 CUDA tensors in [0, 1]."""
+        reference, uploads the uint8 images once and returns (x, y) float32 CUDA tensors in [0, 1].  With REALISTIC_OCCLUSION or
+        SQUARE_OCCLUSION set, the masks are occluded on the device before the paste (see ``occlusion_fallbacks``)."""
         import torch
         for name in ("train_x", "mask_x", "train_y", "bg_imgs"):
             if not hasattr(self, name):
                 raise RuntimeError("Dataset.%s is not loaded (load_training_images / set the arrays)" % name)
-        if eval(str(self._kw.get("realistic_occlusion", "False"))) or eval(str(self._kw.get("square_occlusion", "False"))):
-            raise NotImplementedError("REALISTIC_OCCLUSION / SQUARE_OCCLUSION are off in the template cfg and not supported")
+        occl = self._occlusion
+        if occl is not None and occl.realistic and getattr(self, "occlusion_masks", None) is None:
+            self.load_occlusion_masks()
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else device
         idx = np.random.choice(len(self.train_x), batch_size, replace=False)
         idx_bg = np.random.choice(len(self.bg_imgs), batch_size, replace=False)
@@ -192,6 +224,8 @@ class Dataset(object):
         m = torch.from_numpy(np.ascontiguousarray(self.mask_x[idx]).astype(np.uint8)).to(dev, non_blocking=True)
         bg = torch.from_numpy(self.bg_imgs[idx_bg]).to(dev, non_blocking=True)
         y = torch.from_numpy(self.train_y[idx]).to(dev, non_blocking=True)
+        if occl is not None:
+            m = occl.apply_device(m, getattr(self, "occlusion_masks", None))
         xf = self._aug.augment_device(x, m, bg)
         return xf, y.to(torch.float32) / 255.0
 

@@ -623,6 +623,31 @@ extern "C" int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, 
                         blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, (cudaStream_t)stream);
 }
 
+extern "C" int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, int w, const uint32_t* bank_dev, int n_bank,
+                                     const int32_t* cand_dev, int n_cand, int realistic, double max_occl, int square, double min_kept,
+                                     const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_h, int low_w,
+                                     uint8_t* mask_out_dev, int32_t* fallbacks_dev, void* stream) {
+  AAE_REQUIRE(mask_dev && cand_dev && mask_out_dev && fallbacks_dev, "null argument");
+  AAE_REQUIRE(batch >= 1 && h >= 1 && w >= 1 && n_cand >= 1, "bad geometry / candidate count");
+  AAE_REQUIRE(!realistic || (bank_dev && n_bank >= 1), "realistic occlusion needs an occluder bank");
+  AAE_REQUIRE(!square || (row_cell_dev && col_cell_dev && low_h >= 1 && low_w >= 1), "square occlusion needs the dropout cell maps");
+  if (w % 32 != 0) {
+    set_error("occlusion: mask width %d is not a multiple of 32 (rows are packed into 32-bit words)", w);
+    return AAE_ERR_UNSUPPORTED;
+  }
+  if (square && low_h * low_w > 32) {
+    set_error("occlusion: %d x %d dropout cells do not fit the 32 keep bits of a candidate", low_h, low_w);
+    return AAE_ERR_UNSUPPORTED;
+  }
+  const size_t smem = occlusion_smem_bytes(h, w, square ? low_w : 0);
+  if (smem > 48 * 1024) {
+    set_error("occlusion: a %d x %d mask needs %zu bytes of shared memory (48 KB supported)", h, w, smem);
+    return AAE_ERR_UNSUPPORTED;
+  }
+  return launch_occlusion(mask_dev, batch, h, w, bank_dev, n_bank, cand_dev, n_cand, realistic, max_occl, square, min_kept,
+                          row_cell_dev, col_cell_dev, low_w, mask_out_dev, fallbacks_dev, (cudaStream_t)stream);
+}
+
 // ============================================================================ decoder
 static int simt_decoder_create(aae_decoder* h) {
   SimtDecoder* S = h->simt = new (std::nothrow) SimtDecoder();

@@ -167,6 +167,11 @@ int launch_wgrad_small_n(const IGemmParams& p, int chunks, float* partial, cudaS
 int launch_augment(const uint8_t* x, const uint8_t* mask, const uint8_t* bg, int B, int H, int W, int C, const int32_t* geom, const uint8_t* lut,
                    const unsigned short* tab, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, const int32_t* blur_q8, const float* to_float,
                    uint8_t* tmp, uint8_t* out_u8, float* out_f32, cudaStream_t s);
+// occlusion-mask augmentations (occlusion.cu)
+size_t occlusion_smem_bytes(int H, int W, int low_w);
+int launch_occlusion(const uint8_t* mask, int B, int H, int W, const uint32_t* bank, int n_bank, const int32_t* cand, int K, int realistic,
+                     double max_occl, int square, double min_kept, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, uint8_t* out,
+                     int32_t* fallbacks, cudaStream_t s);
 
 // ---- codebook ------------------------------------------------------------------------------
 int launch_l2_normalize(const float* z, int B, int J, float* out, cudaStream_t stream);

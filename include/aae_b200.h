@@ -198,6 +198,26 @@ AAE_API int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, con
                               const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
                               const float* u8_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, void* stream);
 
+/* The occlusion switches of the training cfg, applied to the masks before aae_augment_batch (auto_pose/ae/dataset.py:421-454,
+ * called at dataset.py:468-471).  mask_dev / mask_out_dev: uint8 [B][H][W], nonzero = BACKGROUND (the reference's mask_x);
+ * mask_out_dev receives 0 / 1.  cand_dev: int32 [B][1 + 3K] per image, every draw made by the caller:
+ *   [0]           occluder index into bank_dev (outside [0, n_bank): an occluder without pixels)
+ *   [1, K + 1)    column shifts tx,  [K + 1, 2K + 1) row shifts ty  (REALISTIC_OCCLUSION candidates, in draw order)
+ *   [2K + 1, 3K + 1)  keep bits of the low_h x low_w dropout cells, row-major (SQUARE_OCCLUSION candidates; all cells set
+ *                 when the Sometimes draw did not fire)
+ * bank_dev: uint32 [n_bank][H][W/32] occluders, bit j of word w of a row = column 32 w + j.  row_cell_dev [H] / col_cell_dev
+ * [W]: cv2.resize INTER_NEAREST index maps of the dropout cells.  realistic: the occluder shifted by (tx, ty) with zero fill
+ * removes the object pixels it covers; the first candidate with 0 < removed / object < max_occl (double) is taken.  square:
+ * the first candidate with NOT (kept / object < min_kept) (double, min_kept = 1 - SQUARE_OCCLUSION, object = the count of the
+ * incoming mask) is taken.  An image whose K candidates of a step all fail keeps its mask from before that step and adds 1 to
+ * fallbacks_dev[0] (realistic) or [1] (square); the reference re-draws without bound instead.  Either step may be off
+ * (realistic = 0 / square = 0; its pointers may then be NULL).  W % 32 != 0, low_h * low_w > 32 or more than 48 KB of
+ * shared memory per image return AAE_ERR_UNSUPPORTED. */
+AAE_API int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, int w, const uint32_t* bank_dev, int n_bank,
+                                  const int32_t* cand_dev, int n_cand, int realistic, double max_occl, int square, double min_kept,
+                                  const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_h, int low_w,
+                                  uint8_t* mask_out_dev, int32_t* fallbacks_dev, void* stream);
+
 /* ---------------------------------------------------------------- Training step ------------
  * Replaces sess.run(train_op): encoder fwd, decoder fwd, bootstrapped L2, backward, TF-Adam
  * (auto_pose/ae/ae_train.py:128, auto_pose/ae/ae_factory.py:79-95).
