@@ -42,6 +42,8 @@ _SIGS = {
     "aae_encoder_range_word": (_I, [_P, C.POINTER(_P)]),
     "aae_encoder_activation": (_I, [_P, _I, C.POINTER(_P), C.POINTER(_L)]),
     "aae_encoder_profile": (_I, [_P, _I, _P, _I]),
+    "aae_encoder_enable_sigma_head": (_I, [_P]),
+    "aae_encoder_sigma_forward": (_I, [_P, _I, _P, _P]),
     "aae_codebook_profile": (_I, [_P, _I, _P, _I]),
     "aae_codebook_create": (_I, [_I, _P, _L, _I, _I, _L, _I, _I, C.POINTER(_P)]),
     "aae_codebook_destroy": (_I, [_P]),
@@ -70,6 +72,8 @@ _SIGS = {
     "aae_trainer_get_state": (_I, [_P, _I, _I, _P, _P, _P, _P, _P]),
     "aae_trainer_set_state": (_I, [_P, _I, _I, _P, _P, _P, _P, _P]),
     "aae_trainer_set_global_step": (_I, [_P, _L]),
+    "aae_trainer_set_latent_terms": (_I, [_P, _F, _F]),
+    "aae_trainer_set_latent_noise": (_I, [_P, _F]),
     "aae_extract_square_patches": (_I, [_P, _I, _I, _P, _I, _F, _I, _P, _P]),
     "aae_augment_batch": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P]),
     "aae_augment_occlusion": (_I, [_P, _I, _I, _I, _P, _I, _P, _I, _I, _D, _I, _D, _P, _P, _I, _I, _P, _P, _P]),

@@ -8,8 +8,6 @@ from .utils import lazy_property
 class AE(object):
 
     def __init__(self, encoder, decoder, norm_regularize, variational):
-        if variational:
-            raise NotImplementedError("VARIATIONAL > 0 is not supported (0 in the template cfg)")
         self._encoder = encoder
         self._decoder = decoder
         self._norm_regularize = norm_regularize
@@ -43,5 +41,7 @@ class AE(object):
             loss = ctx.get(self._decoder.reconstr_loss)
             if self._norm_regularize > 0:
                 loss = loss + ctx.get(self._encoder.reg_loss) * float(self._norm_regularize)
+            if self._variational:
+                loss = loss + ctx.get(self._encoder.kl_div_loss) * float(self._variational)
             return loss
         return Tensor("total_loss", (), np.float32, fn)

@@ -85,9 +85,8 @@ def build_decoder(reconstruction_target, encoder, args, is_training=False):
     VARIATIONAL = args.getfloat('Network', 'VARIATIONAL') if is_training else False
     AUXILIARY_MASK = args.getboolean('Network', 'AUXILIARY_MASK')
     BATCH_NORM = args.getboolean('Network', 'BATCH_NORMALIZATION')
-    if VARIATIONAL:
-        raise NotImplementedError("VARIATIONAL > 0 is not supported")
-    return Decoder(reconstruction_target, encoder.z, list(reversed(NUM_FILTER)), KERNEL_SIZE_DECODER, list(reversed(STRIDES)),
+    return Decoder(reconstruction_target, encoder.sampled_z if VARIATIONAL else encoder.z, list(reversed(NUM_FILTER)), KERNEL_SIZE_DECODER,
+                   list(reversed(STRIDES)),
                    LOSS, BOOTSTRAP_RATIO, AUXILIARY_MASK, BATCH_NORM, is_training=is_training, max_batch=encoder.max_batch,
                    n_encoder_convs=len(NUM_FILTER))
 
@@ -106,23 +105,28 @@ class TrainOp(Tensor):
     handles.  ``_lib.PREC_TC_FP16`` is the single-pass trainer: it needs PREC_TC_SPLIT encoder and decoder handles, which keep
     that precision for inference, and raises for any other handles instead of switching their precision."""
 
-    def __init__(self, ae, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8, precision=None):
+    def __init__(self, ae, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8, precision=None, noise_seed=0):
+        """noise_seed seeds the stream of VARIATIONAL's eps, one N(0,1) draw per step (Encoder.run_eps)."""
         super().__init__("train_op", (), np.float32, self._run)
         self._ae = ae
         self._hp = (float(learning_rate), float(beta1), float(beta2), float(epsilon))
         self._precision = None if precision is None else int(precision)
         self._trainers = {}
+        self._eps_rng = np.random.RandomState(noise_seed)
 
     def trainer(self, device):
         dev = device.index
         if dev not in self._trainers:
-            enc, dec = self._ae._encoder, self._ae._decoder
-            if self._ae._norm_regularize > 0:
-                raise NotImplementedError("NORM_REGULARIZE > 0 is not part of the fused training step")
+            ae = self._ae
+            enc, dec = ae._encoder, ae._decoder
             if _lib.PREC_TC_FP16 in (enc.precision, dec.precision):
                 # never switch a precision the caller chose: the fp16 mode has no backward pass
                 raise _lib.AaeError("training needs precision PREC_TC_SPLIT or PREC_FP32_SIMT; PREC_TC_FP16 is inference-only "
                                     "(create the encoder with another precision for training)")
+            if ae._variational and dec._latent_code is not enc.sampled_z:
+                # the fused step feeds the decoder the sampled z exactly when VARIATIONAL is set, as build_decoder wires it
+                raise NotImplementedError("VARIATIONAL != 0 trains a decoder built on encoder.sampled_z (build_decoder(..., "
+                                          "is_training=True)); this decoder reads %s" % dec._latent_code.name)
             h = C.c_void_p()
             with torch.cuda.device(dev):
                 eh, dh = enc.handle(device), dec.handle(device)       # settles automatic precisions
@@ -130,16 +134,23 @@ class TrainOp(Tensor):
                     # an explicit GEMM precision: the handles must suit it as they are (an automatic fp32 fallback does not)
                     _lib.check(_lib.lib().aae_trainer_create_prec(eh, dh, dec._bootstrap_ratio, *self._hp, self._precision, C.byref(h)),
                                "trainer create (GEMM precision %d)" % self._precision)
-                    self._trainers[dev] = h
-                    return h
-                st = -3 if enc.precision != dec.precision else _lib.lib().aae_trainer_create(eh, dh, dec._bootstrap_ratio, *self._hp, C.byref(h))
-                if st == -3 and (enc._auto_precision or dec._auto_precision or enc.precision != dec.precision) and \
-                        (enc.precision, dec.precision) != (_lib.PREC_FP32_SIMT, _lib.PREC_FP32_SIMT):
-                    # a geometry the tensor-core trainer is not built for: the fp32 CUDA-core trainer handles every geometry
-                    enc.set_precision(_lib.PREC_FP32_SIMT)
-                    dec.set_precision(_lib.PREC_FP32_SIMT)
-                    st = _lib.lib().aae_trainer_create(enc.handle(device), dec.handle(device), dec._bootstrap_ratio, *self._hp, C.byref(h))
-                _lib.check(st, "trainer create")
+                else:
+                    st = -3 if enc.precision != dec.precision else _lib.lib().aae_trainer_create(eh, dh, dec._bootstrap_ratio, *self._hp, C.byref(h))
+                    if st == -3 and (enc._auto_precision or dec._auto_precision or enc.precision != dec.precision) and \
+                            (enc.precision, dec.precision) != (_lib.PREC_FP32_SIMT, _lib.PREC_FP32_SIMT):
+                        # a geometry the tensor-core trainer is not built for: the fp32 CUDA-core trainer handles every geometry
+                        enc.set_precision(_lib.PREC_FP32_SIMT)
+                        dec.set_precision(_lib.PREC_FP32_SIMT)
+                        st = _lib.lib().aae_trainer_create(enc.handle(device), dec.handle(device), dec._bootstrap_ratio, *self._hp, C.byref(h))
+                    _lib.check(st, "trainer create")
+                if ae._variational or ae._norm_regularize > 0:
+                    # AE.loss adds reg_loss only for NORM_REGULARIZE > 0 and the KL term for VARIATIONAL != 0 (ae.py:43-53)
+                    st = _lib.lib().aae_trainer_set_latent_terms(h, float(ae._variational), float(max(ae._norm_regularize, 0.0)))
+                    if st != 0:
+                        msg = _lib.lib().aae_last_error_string().decode("utf-8", "replace")
+                        _lib.lib().aae_trainer_destroy(h)
+                        raise _lib.AaeError("latent terms (VARIATIONAL %g, NORM_REGULARIZE %g) failed (status %d): %s"
+                                            % (ae._variational, ae._norm_regularize, st, msg))
             self._trainers[dev] = h
         return self._trainers[dev]
 
@@ -153,9 +164,14 @@ class TrainOp(Tensor):
             y = y.to(torch.float32) / 255.0
         return x.contiguous(), y.contiguous()
 
-    def step_device(self, x, y, update=True):
+    def step_device(self, x, y, update=True, eps=None):
+        """One step on device tensors; returns the total loss.  With VARIATIONAL, ``eps`` is the step's noise scalar (None: the
+        next draw of this TrainOp's seeded stream)."""
         dev = x.device
         h = self.trainer(dev)
+        if self._ae._variational:
+            eps = self._eps_rng.standard_normal() if eps is None else eps
+            _lib.check(_lib.lib().aae_trainer_set_latent_noise(h, float(np.float32(eps))), "latent noise")
         loss = torch.empty((1,), dtype=torch.float32, device=dev)
         fn = _lib.lib().aae_train_step if update else _lib.lib().aae_trainer_forward_backward
         _lib.check(fn(h, _lib.ptr(x), _lib.ptr(y), x.shape[0], _lib.ptr(loss), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
@@ -169,7 +185,8 @@ class TrainOp(Tensor):
         for m in (self._ae._encoder, self._ae._decoder):
             if m not in ctx.touched:
                 ctx.touched.append(m)
-        return self.step_device(x, y, update=True)
+        eps = self._ae._encoder.run_eps(ctx, draw=self._eps_rng.standard_normal) if self._ae._variational else None
+        return self.step_device(x, y, update=True, eps=eps)
 
     # -- optimizer state under TensorFlow's names: "<var>/Adam", "<var>/Adam_1", "<scope>/beta1_power", "<scope>/beta2_power" ------
     def _scope_prefix(self):

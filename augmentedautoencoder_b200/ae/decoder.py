@@ -43,8 +43,11 @@ class Decoder(_DeviceModule):
         nl = len(self._num_filters)
         dims = [int(h / np.prod(self._strides[i:])) for i in range(nl)]
         k0 = n_encoder_convs if n_encoder_convs is not None else nl
-        var_shapes = [(scoped("dense_1/kernel"), (latent, dims[0] * dims[0] * self._num_filters[0]),
-                       scoped("dense_1/bias"), (dims[0] * dims[0] * self._num_filters[0],))]
+        # TF numbers dense layers per scope: after the encoder's sigma head (built when the decoder reads the sampled z) this is
+        # the third one
+        dense = "dense_2" if getattr(latent_code, "sigma_head", False) else "dense_1"
+        var_shapes = [(scoped(dense + "/kernel"), (latent, dims[0] * dims[0] * self._num_filters[0]),
+                       scoped(dense + "/bias"), (dims[0] * dims[0] * self._num_filters[0],))]
         cin = self._num_filters[0]
         for j, f in enumerate(self._num_filters[1:] + [c]):
             base = scoped("conv2d_%d" % (k0 + j))

@@ -113,12 +113,16 @@ class _DeviceModule:
                 st = self._create(dev, C.byref(cfg), C.byref(h))
             _lib.check(st, type(self).__name__ + " create")
             try:
+                self._prepare(h)
                 self._upload(dev, h)
             except Exception:          # e.g. a weight outside the tensor-core range: no half-initialised handle may stay behind
                 self._destroy(h)
                 raise
             self._handles[dev] = h
         return self._handles[dev]
+
+    def _prepare(self, h):
+        """Called on a new handle before the variables are uploaded to it."""
 
     def check_range(self, device=None):
         """Raises AaeError if a forward / training step launched so far on this module left the range of the split-fp16
@@ -194,6 +198,9 @@ class Encoder(_DeviceModule):
         var_shapes.append((scoped("dense/kernel"), (self._flat, self._latent_space_size), scoped("dense/bias"), (self._latent_space_size,)))
         self._init_module((h, w, c, self._num_filters, self._strides, self._kernel_size, self._latent_space_size,
                            self.max_batch, self.precision), var_shapes, seed)
+        self._scope_prefix = scoped("dense/kernel")[:-len("dense/kernel")]
+        self._has_sigma_head = False
+        self._eps_rng = np.random.RandomState(seed)
         self.encoder_out
         self.z
 
@@ -264,6 +271,82 @@ class Encoder(_DeviceModule):
             hh, ww = -(-hh // s), -(-ww // s)
         B = n.value // (hh * ww * f)
         return tensor_from_ptr(p.value, (B, hh, ww, f), device).clone()
+
+    # -- variational AE: sigma head, sampled z, KL term (auto_pose/ae/encoder.py:70-95) -------------------------------
+    def _register_sigma_head(self):
+        """Creates the head's variables, zero-initialised (kernel_initializer=zeros, default zero bias).  TF numbers dense layers
+        per scope: the head is the second one, "<scope>/dense_1" (the decoder's dense layer then becomes "dense_2")."""
+        if self._has_sigma_head:
+            return
+        J = self._latent_space_size
+        kn, bn = self._scope_prefix + "dense_1/kernel", self._scope_prefix + "dense_1/bias"
+        self._var_shapes.append((kn, (self._flat, J), bn, (J,)))
+        self._host[kn] = np.zeros((self._flat, J), np.float32)
+        self._host[bn] = np.zeros((J,), np.float32)
+        self._has_sigma_head = True
+        layer = len(self._num_filters) + 1
+        for dev, h in self._handles.items():
+            with torch.cuda.device(dev):
+                self._prepare(h)
+                _lib.check(self._set(h, layer, _lib.ptr(self._host[kn]), _lib.ptr(self._host[bn]), None), "set_weights(%s)" % kn)
+
+    def _prepare(self, h):
+        if self._has_sigma_head:
+            _lib.check(_lib.lib().aae_encoder_enable_sigma_head(h), "enable sigma head")
+
+    def _sigma_of_last_forward(self, device, B):
+        out = torch.empty((B, self._latent_space_size), dtype=torch.float32, device=device)
+        _lib.check(_lib.lib().aae_encoder_sigma_forward(self.handle(device), B, _lib.ptr(out),
+                                                        C.c_void_p(torch.cuda.current_stream(device).cuda_stream)), "sigma forward")
+        return out
+
+    def run_eps(self, ctx, draw=None):
+        """eps of sampled_z in this Session.run: one scalar N(0,1) per run (tf.shape of the Python int latent_space_size is an
+        empty shape, so tf.random_normal draws a single value), shared by every fetch of the run.  ``draw`` (a callable)
+        supplies it when this run has none yet; else the encoder's own seeded stream does."""
+        key = ("latent_eps", id(self))                 # the Encoder outlives every RunContext, so its id is stable
+        if key not in ctx.memo:
+            ctx.memo[key] = np.float32(draw() if draw is not None else self._eps_rng.standard_normal())
+        return ctx.memo[key]
+
+    @lazy_property
+    def q_sigma(self):
+        """1e-8 + softplus(encoder_out . W + b) on the device (aae_encoder_sigma_forward)."""
+        self._register_sigma_head()
+
+        def fn(ctx):
+            dev = ctx.session.device
+            x = self._eval_input(ctx)
+            if x.shape[0] <= self.max_batch:
+                ctx.get(self.z)
+                return self._sigma_of_last_forward(dev, x.shape[0])
+            parts = []
+            for a in range(0, x.shape[0], self.max_batch):
+                chunk = x[a:a + self.max_batch]
+                self.encode_device(chunk)
+                parts.append(self._sigma_of_last_forward(dev, chunk.shape[0]))
+            return torch.cat(parts)
+        return Tensor("add", (None, self._latent_space_size), np.float32, fn)
+
+    @lazy_property
+    def sampled_z(self):
+        """z + q_sigma * eps, eps one scalar per Session.run (run_eps)."""
+        q_sigma = self.q_sigma
+        t = Tensor("add_1", (None, self._latent_space_size), np.float32,
+                   lambda ctx: ctx.get(self.z) + ctx.get(q_sigma) * float(self.run_eps(ctx)))
+        t.sigma_head = True                            # a decoder built on it is the scope's third dense layer
+        return t
+
+    @lazy_property
+    def kl_div_loss(self):
+        """mean over [B, latent] of KL(N(z, q_sigma) || N(0, 1)) in TF's form z^2/2 + (s^2 - 1 - log s^2)/2; torch on the device
+        tensors, like reg_loss."""
+        q_sigma = self.q_sigma
+
+        def fn(ctx):
+            z, s2 = ctx.get(self.z), ctx.get(q_sigma) ** 2
+            return (0.5 * z * z + 0.5 * (s2 - 1.0 - torch.log(s2))).mean()
+        return Tensor("kl_div_loss", (), np.float32, fn)
 
     @lazy_property
     def reg_loss(self):

@@ -197,6 +197,9 @@ struct aae_encoder {
   std::vector<ConvLayer> conv;
   int flat;                 // features entering the dense layer
   DevBuf dense_w, dense_b;  // [flat, latent], [latent]
+  // sigma head of the variational AE (aae_encoder_enable_sigma_head; empty until then): [flat, latent], [latent], and the
+  // pre-activation [max_batch, latent] and split-K scratch of aae_encoder_sigma_forward (the scratch on tensor-core handles only)
+  DevBuf sig_w, sig_b, sig_pre, sig_partials;
   SimtEncoder* simt = nullptr;  // fp32 CUDA-core workspace (AAE_PREC_FP32_SIMT)
   TcEncoder* tc = nullptr;  // tensor-core execution plan (AAE_PREC_TC_SPLIT or AAE_PREC_TC_FP16)
   int last_batch = 0;
@@ -254,6 +257,11 @@ struct aae_trainer {
   DevBuf bias_scratch;  // 256 * max(out_c)
   DevBuf sample_sums, z, dz, rec;
   DevBuf dwm;           // gradient wrt merged sub-pixel weights
+  // latent terms (aae_trainer_set_latent_terms): weights, the eps of the next step, and -- when the encoder had a sigma head at
+  // creation (enc_k / enc_b then hold it at num_layers + 1) -- head pre-activation, sampled z, its gradient, [dz | dpre]
+  float w_v = 0.f, w_n = 0.f, noise = 0.f;
+  bool head = false;
+  DevBuf pre, sz, dpre, dcat, lat_sums;
   TcTrainPlan* tc = nullptr;  // tensor-core backward plan (encoder and decoder created with AAE_PREC_TC_SPLIT)
   uint64_t packed_enc_version = 0, packed_dec_version = 0;   // master-weight versions the plan's dgrad operands were packed from
   // single-pass trainer (aae_trainer_create_prec with AAE_PREC_TC_FP16): private hi-only forward plans built from the handles'
@@ -357,6 +365,7 @@ extern "C" int aae_encoder_destroy(aae_encoder* h) {
   DeviceGuard g(h->device);
   for (auto& L : h->conv) { L.w.release(); L.b.release(); }
   h->dense_w.release(); h->dense_b.release();
+  h->sig_w.release(); h->sig_b.release(); h->sig_pre.release(); h->sig_partials.release();
   delete h->simt;
   if (h->tc) tc_encoder_destroy(h->tc);
   h->timer.release();
@@ -364,15 +373,30 @@ extern "C" int aae_encoder_destroy(aae_encoder* h) {
   return AAE_OK;
 }
 
+// layer < num_layers: conv; num_layers: dense; num_layers + 1: the sigma head (once enabled)
+static int encoder_layer_bufs(aae_encoder* h, int layer, DevBuf** w, DevBuf** b) {
+  const int nl = (int)h->conv.size();
+  AAE_REQUIRE(layer >= 0 && (layer <= nl || (layer == nl + 1 && h->sig_w.p)), "layer %d out of range%s", layer,
+              layer == nl + 1 ? " (no sigma head: aae_encoder_enable_sigma_head)" : "");
+  *w = layer < nl ? &h->conv[layer].w : layer == nl ? &h->dense_w : &h->sig_w;
+  *b = layer < nl ? &h->conv[layer].b : layer == nl ? &h->dense_b : &h->sig_b;
+  return AAE_OK;
+}
+
 extern "C" int aae_encoder_set_weights(aae_encoder* h, int layer, const float* kernel_any, const float* bias_any, void* stream) {
   AAE_REQUIRE(h != nullptr, "encoder handle is null");
-  AAE_REQUIRE(layer >= 0 && layer <= (int)h->conv.size(), "layer %d out of range", layer);
+  DevBuf *wp, *bp;
+  AAE_TRY(encoder_layer_bufs(h, layer, &wp, &bp));
   DeviceGuard g(h->device);
   cudaStream_t s = (cudaStream_t)stream;
-  DevBuf& w = layer < (int)h->conv.size() ? h->conv[layer].w : h->dense_w;
-  DevBuf& b = layer < (int)h->conv.size() ? h->conv[layer].b : h->dense_b;
+  DevBuf& w = *wp;
+  DevBuf& b = *bp;
   if (kernel_any) AAE_TRY(copy_any(w.p, kernel_any, w.n * sizeof(float), s));
   if (bias_any) AAE_TRY(copy_any(b.p, bias_any, b.n * sizeof(float), s));
+  if (layer > (int)h->conv.size()) {   // the head runs on the fp32 masters only: no packed copy to follow
+    AAE_CUDA_OK(cudaStreamSynchronize(s));
+    return AAE_OK;
+  }
   const bool tc_current = h->tc_version == h->w_version;
   h->w_version += 1;
   if (h->tc && kernel_any) AAE_TRY(tc_encoder_pack_weights(h->tc, layer, w.p, s));
@@ -397,11 +421,12 @@ extern "C" int aae_encoder_range_status(aae_encoder* h, void* stream) {
 
 extern "C" int aae_encoder_get_weights(aae_encoder* h, int layer, float* kernel_any, float* bias_any, void* stream) {
   AAE_REQUIRE(h != nullptr, "encoder handle is null");
-  AAE_REQUIRE(layer >= 0 && layer <= (int)h->conv.size(), "layer %d out of range", layer);
+  DevBuf *wp, *bp;
+  AAE_TRY(encoder_layer_bufs(h, layer, &wp, &bp));
   DeviceGuard g(h->device);
   cudaStream_t s = (cudaStream_t)stream;
-  DevBuf& w = layer < (int)h->conv.size() ? h->conv[layer].w : h->dense_w;
-  DevBuf& b = layer < (int)h->conv.size() ? h->conv[layer].b : h->dense_b;
+  DevBuf& w = *wp;
+  DevBuf& b = *bp;
   if (kernel_any) AAE_TRY(copy_any(kernel_any, w.p, w.n * sizeof(float), s));
   if (bias_any) AAE_TRY(copy_any(bias_any, b.p, b.n * sizeof(float), s));
   AAE_CUDA_OK(cudaStreamSynchronize(s));
@@ -480,6 +505,53 @@ extern "C" int aae_encoder_profile(aae_encoder* h, int enable, float* stage_ms_o
   if (stage_ms_out && capacity > 0) n = h->timer.read(stage_ms_out, capacity);
   h->timer.enabled = enable != 0;
   return n;
+}
+
+// ---- sigma head of the variational AE (auto_pose/ae/encoder.py:70-79) ----
+extern "C" int aae_encoder_enable_sigma_head(aae_encoder* h) {
+  AAE_REQUIRE(h != nullptr, "encoder handle is null");
+  if (h->sig_w.p) return AAE_OK;
+  DeviceGuard g(h->device);
+  const size_t J = h->cfg.latent, B = h->cfg.max_batch;
+  int st = h->sig_w.alloc((size_t)h->flat * J);
+  if (st == AAE_OK) st = h->sig_b.alloc(J);
+  if (st == AAE_OK) st = h->sig_pre.alloc(B * J);
+  if (st == AAE_OK && h->tc) st = h->sig_partials.alloc(64 * B * J);   // fp32 handles split K in their own scratch
+  if (st == AAE_OK) {
+    cudaError_t e = cudaMemset(h->sig_w.p, 0, h->sig_w.n * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemset(h->sig_b.p, 0, h->sig_b.n * sizeof(float));
+    if (e != cudaSuccess) { set_error("sigma head: %s", cudaGetErrorString(e)); st = AAE_ERR_CUDA; }
+  }
+  if (st != AAE_OK) { h->sig_w.release(); h->sig_b.release(); h->sig_pre.release(); h->sig_partials.release(); }
+  return st;
+}
+
+// pre = flat . W_sigma + b_sigma on the fp32 GEMM (the trainer's step and aae_encoder_sigma_forward)
+static int sigma_head_pre(aae_encoder* h, const float* flat, int B, DevBuf& partials, float* pre, cudaStream_t s) {
+  IGemmParams p = dense_params(flat, B, h->flat, h->sig_w.p, h->cfg.latent);
+  return run_igemm(p, GATHER_FWD, partials, pre, h->sig_b.p, ACT_NONE, nullptr, s);
+}
+
+extern "C" int aae_encoder_sigma_forward(aae_encoder* h, int batch, float* q_sigma_out_dev, void* stream) {
+  AAE_REQUIRE(h != nullptr && q_sigma_out_dev != nullptr, "null argument");
+  if (!h->sig_w.p) {
+    set_error("sigma_forward: the encoder has no sigma head (aae_encoder_enable_sigma_head)");
+    return AAE_ERR_UNSUPPORTED;
+  }
+  AAE_REQUIRE(batch >= 1 && batch <= h->last_batch, "batch %d outside [1, %d] (the batch of the last forward)", batch, h->last_batch);
+  DeviceGuard g(h->device);
+  cudaStream_t s = (cudaStream_t)stream;
+  const float* flat = nullptr;
+  if (h->tc) {
+    int64_t n = 0;
+    AAE_TRY(tc_encoder_activation(h->tc, (int)h->conv.size() - 1, batch, &flat, &n, s));
+  } else {
+    flat = h->simt->out.back().p;
+  }
+  AAE_TRY(sigma_head_pre(h, flat, batch, h->tc ? h->sig_partials : h->simt->partials, h->sig_pre.p, s));
+  LatentArgs a;
+  a.pre = h->sig_pre.p; a.B = batch; a.J = h->cfg.latent; a.sigma = q_sigma_out_dev;
+  return launch_latent(a, 0, s);
 }
 
 // ============================================================================ codebook
@@ -865,6 +937,9 @@ static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_rati
   for (auto& L : enc->conv) { if (st == AAE_OK) st = make_pg(h->enc_k, L.w); if (st == AAE_OK) st = make_pg(h->enc_b, L.b); }
   if (st == AAE_OK) st = make_pg(h->enc_k, enc->dense_w);
   if (st == AAE_OK) st = make_pg(h->enc_b, enc->dense_b);
+  h->head = enc->sig_w.p != nullptr;
+  if (st == AAE_OK && h->head) st = make_pg(h->enc_k, enc->sig_w);
+  if (st == AAE_OK && h->head) st = make_pg(h->enc_b, enc->sig_b);
   if (st == AAE_OK) st = make_pg(h->dec_k, dec->dense_w);
   if (st == AAE_OK) st = make_pg(h->dec_b, dec->dense_b);
   for (auto& L : dec->conv) { if (st == AAE_OK) st = make_pg(h->dec_k, L.w); if (st == AAE_OK) st = make_pg(h->dec_b, L.b); }
@@ -890,7 +965,14 @@ static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_rati
   if (st == AAE_OK) st = h->grad_b.alloc(simt ? max_act : 0);
   if (st == AAE_OK) st = h->dxup.alloc(simt ? max_up : 0);
   if (st == AAE_OK) st = h->flat.alloc(simt ? 0 : B * enc->flat);
-  if (st == AAE_OK) st = h->wt.alloc(simt ? max_w : max_dense_w);
+  // with the sigma head, the data gradient of `flat` is one GEMM over [W_z^T ; W_sigma^T] (K = 2 latent)
+  const size_t head_wt = h->head ? 2 * enc->dense_w.n : 0;
+  if (st == AAE_OK) st = h->wt.alloc(std::max(simt ? max_w : max_dense_w, head_wt));
+  const size_t BJ = B * enc->cfg.latent;
+  if (st == AAE_OK) st = h->pre.alloc(h->head ? BJ : 0);
+  if (st == AAE_OK) st = h->sz.alloc(h->head ? BJ : 0);
+  if (st == AAE_OK) st = h->dpre.alloc(h->head ? BJ : 0);
+  if (st == AAE_OK) st = h->dcat.alloc(h->head ? 2 * BJ : 0);
   if (st == AAE_OK) st = h->partials.alloc((size_t)48 << 20);
   if (st == AAE_OK) st = h->bias_scratch.alloc(256 * max_c);
   if (st == AAE_OK) st = h->sample_sums.alloc(B);
@@ -963,6 +1045,7 @@ extern "C" int aae_trainer_destroy(aae_trainer* h) {
     for (auto& pg : *v) { pg.g.release(); pg.m.release(); pg.v.release(); }
   h->dx_out.release(); h->grad_a.release(); h->grad_b.release(); h->dxup.release(); h->flat.release(); h->wt.release(); h->partials.release();
   h->bias_scratch.release(); h->sample_sums.release(); h->z.release(); h->dz.release(); h->rec.release(); h->dwm.release();
+  h->pre.release(); h->sz.release(); h->dpre.release(); h->dcat.release(); h->lat_sums.release();
   tc_train_destroy(h->tc);
   tc_encoder_destroy(h->fenc);
   tc_decoder_destroy(h->fdec);
@@ -1001,6 +1084,29 @@ extern "C" int aae_trainer_set_state(aae_trainer* h, int which, int layer, const
 extern "C" int aae_trainer_set_global_step(aae_trainer* h, int64_t step) {
   AAE_REQUIRE(h != nullptr && step >= 0, "bad arguments");
   h->step = step;      // the bias correction of the next update uses t = step + 1, as after `step` updates
+  return AAE_OK;
+}
+
+extern "C" int aae_trainer_set_latent_terms(aae_trainer* h, float variational, float norm_regularize) {
+  AAE_REQUIRE(h != nullptr, "trainer handle is null");
+  AAE_REQUIRE(variational >= 0.f && norm_regularize >= 0.f, "latent term weights must be >= 0 (VARIATIONAL %g, NORM_REGULARIZE %g)",
+              (double)variational, (double)norm_regularize);
+  if (variational > 0.f && !h->head) {
+    set_error("VARIATIONAL > 0 needs the sigma head: call aae_encoder_enable_sigma_head before creating the trainer");
+    return AAE_ERR_UNSUPPORTED;
+  }
+  if ((variational > 0.f || norm_regularize > 0.f) && !h->lat_sums.p) {
+    DeviceGuard g(h->enc->device);
+    AAE_TRY(h->lat_sums.alloc(2));
+  }
+  h->w_v = variational;
+  h->w_n = norm_regularize;
+  return AAE_OK;
+}
+
+extern "C" int aae_trainer_set_latent_noise(aae_trainer* h, float eps) {
+  AAE_REQUIRE(h != nullptr, "trainer handle is null");
+  h->noise = eps;
   return AAE_OK;
 }
 
@@ -1047,12 +1153,28 @@ static int conv_dgrad(aae_trainer* h, const ConvLayer& L, int B, const float* dy
   return run_igemm(p, GATHER_DGRAD, h->partials, dx, nullptr, ACT_NONE, relu_mask, s);
 }
 
-// dense_1 of the decoder: dy = pre-activation gradient [B, h0*w0*f0] -> bias / kernel gradients and dz
-static int decoder_dense_backward(aae_trainer* h, const float* dy, int B, cudaStream_t s) {
+// The latent terms (latent.cu) run when either weight is > 0; VARIATIONAL > 0 also runs the sigma head and feeds the decoder
+// the sampled z (auto_pose/ae/ae_factory.py:58).
+static bool latent_terms_on(const aae_trainer* h) { return h->w_v > 0.f || h->w_n > 0.f; }
+static const float* decoder_input(const aae_trainer* h) { return h->w_v > 0.f ? h->sz.p : h->z.p; }
+
+static LatentArgs latent_args(aae_trainer* h, int B, float* loss_out) {
+  const bool head = h->w_v > 0.f;
+  LatentArgs a;
+  a.z = h->z.p; a.pre = head ? h->pre.p : nullptr; a.B = B; a.J = h->enc->cfg.latent;
+  a.eps = h->noise; a.w_v = h->w_v; a.w_n = h->w_n;
+  a.sz = head ? h->sz.p : nullptr; a.sums = h->lat_sums.p;
+  a.dz = h->dz.p; a.dpre = head ? h->dpre.p : nullptr; a.dcat = head ? h->dcat.p : nullptr; a.loss = loss_out;
+  return a;
+}
+
+// dense_1 of the decoder: dy = pre-activation gradient [B, h0*w0*f0] -> bias / kernel gradients and the gradient wrt its input
+// zin (z, or the sampled z) in h->dz
+static int decoder_dense_backward(aae_trainer* h, const float* zin, const float* dy, int B, cudaStream_t s) {
   aae_decoder* D = h->dec;
   const int dense_out = D->h0 * D->w0 * D->f0, J = D->cfg.latent;
   AAE_TRY(launch_bias_grad(dy, B, dense_out, h->dec_b[0].g.p, h->bias_scratch.p, s));
-  IGemmParams p = dense_params(h->z.p, B, J, dy, dense_out);  // WGRAD: src = z, "pixels" = B
+  IGemmParams p = dense_params(zin, B, J, dy, dense_out);  // WGRAD: src = z, "pixels" = B
   p.K = B; p.M = J;
   AAE_TRY(run_igemm(p, GATHER_WGRAD, h->partials, h->dec_k[0].g.p, nullptr, ACT_NONE, nullptr, s));
   AAE_TRY(launch_transpose_last2(D->dense_w.p, h->wt.p, 1, J, dense_out, s));  // [dense_out, J]
@@ -1060,17 +1182,26 @@ static int decoder_dense_backward(aae_trainer* h, const float* dy, int B, cudaSt
   return run_igemm(q, GATHER_FWD, h->partials, h->dz.p, nullptr, ACT_NONE, nullptr, s);
 }
 
-// dense layer of the encoder: dz -> bias / kernel gradients and the gradient wrt the flattened activation `flat` (fp32,
-// [B, flat]) masked by its ReLU, written to da_out
+// dense layer of the encoder (and the sigma head, when the step runs it): dz (dpre) -> bias / kernel gradients and the gradient
+// wrt the flattened activation `flat` (fp32, [B, flat]) masked by its ReLU, written to da_out.  With the head, that gradient is
+// one GEMM [dz | dpre] . [W_z^T ; W_sigma^T] (K = 2 latent): `flat` is read once and no add pass follows.
 static int encoder_dense_backward(aae_trainer* h, const float* flat, int B, float* da_out, cudaStream_t s) {
   aae_encoder* E = h->enc;
   const int J = E->cfg.latent, nl = (int)E->conv.size();
+  const bool head = h->w_v > 0.f;
   AAE_TRY(launch_bias_grad(h->dz.p, B, J, h->enc_b[nl].g.p, h->bias_scratch.p, s));
   IGemmParams p = dense_params(flat, B, E->flat, h->dz.p, J);  // WGRAD: dW[flat, J]
   p.K = B; p.M = E->flat;
   AAE_TRY(run_igemm(p, GATHER_WGRAD, h->partials, h->enc_k[nl].g.p, nullptr, ACT_NONE, nullptr, s));
+  if (head) {
+    AAE_TRY(launch_bias_grad(h->dpre.p, B, J, h->enc_b[nl + 1].g.p, h->bias_scratch.p, s));
+    IGemmParams ps = dense_params(flat, B, E->flat, h->dpre.p, J);
+    ps.K = B; ps.M = E->flat;
+    AAE_TRY(run_igemm(ps, GATHER_WGRAD, h->partials, h->enc_k[nl + 1].g.p, nullptr, ACT_NONE, nullptr, s));
+    AAE_TRY(launch_transpose_last2(E->sig_w.p, h->wt.p + (size_t)J * E->flat, 1, E->flat, J, s));  // rows J..2J-1
+  }
   AAE_TRY(launch_transpose_last2(E->dense_w.p, h->wt.p, 1, E->flat, J, s));  // [J, flat]
-  IGemmParams q = dense_params(h->dz.p, B, J, h->wt.p, E->flat);
+  IGemmParams q = dense_params(head ? h->dcat.p : h->dz.p, B, head ? 2 * J : J, h->wt.p, E->flat);
   return run_igemm(q, GATHER_FWD, h->partials, da_out, nullptr, ACT_NONE, flat, s);  // masked by the ReLU of the last conv
 }
 
@@ -1114,7 +1245,20 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
   // ---- forward ----
   if (!own) E->last_batch = B;                   // aae_encoder_activation reads the handle's plan
   AAE_TRY(tc_encoder_forward(FE, x, 0, B, E->conv[0].w.p, E->conv[0].b.p, E->dense_b.p, h->z.p, &E->timer, s));
-  AAE_TRY(tc_decoder_forward(FD, h->z.p, B, h->rec.p, s));
+  float* flat = h->flat.p;                       // fp32 view of the last conv activation for the fp32 dense layers
+  const bool head = h->w_v > 0.f;
+  if (head) {                                    // the sigma head reads it in the forward pass already
+    pt.mark(4, s);
+    AAE_TRY(tc_train_unpack_flat(P, B, flat, s));
+    pt.mark(1, s);
+    AAE_TRY(sigma_head_pre(E, flat, B, h->partials, h->pre.p, s));
+  }
+  if (latent_terms_on(h)) {
+    pt.mark(4, s);
+    AAE_TRY(launch_latent(latent_args(h, B, loss_out), 0, s));
+    pt.mark(1, s);
+  }
+  AAE_TRY(tc_decoder_forward(FD, decoder_input(h), B, h->rec.p, s));
   const int k = h->bootstrap_ratio > 1 ? numel / h->bootstrap_ratio : numel;
   AAE_TRY(launch_bootstrap_l2(h->rec.p, y, B, numel, k, h->sample_sums.p, loss_out, h->dx_out.p, s));
   AAE_TRY(launch_sigmoid_grad(h->dx_out.p, h->rec.p, (int64_t)B * numel, s));
@@ -1139,11 +1283,11 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
     AAE_TRY(tc_train_finish(P, u, u + 1 < n_dec ? u + 1 : -1, B, /*keep_masked=*/l == 1, l > 1 ? h->dec_b[l - 1].g.p : nullptr, s));
   }
   pt.mark(5, s);
-  AAE_TRY(decoder_dense_backward(h, raw, B, s));
+  AAE_TRY(decoder_dense_backward(h, decoder_input(h), raw, B, s));
   // ---- encoder backward ----
-  float* flat = h->flat.p;                       // fp32 view of the last conv activation for the fp32 dense backward
   pt.mark(4, s);
-  AAE_TRY(tc_train_unpack_flat(P, B, flat, s));
+  if (latent_terms_on(h)) AAE_TRY(launch_latent(latent_args(h, B, loss_out), 1, s));
+  if (!head) AAE_TRY(tc_train_unpack_flat(P, B, flat, s));
   float* da = h->grad_a.p;
   pt.mark(5, s);
   AAE_TRY(encoder_dense_backward(h, flat, B, da, s));
@@ -1181,7 +1325,9 @@ static int trainer_fwd_bwd(aae_trainer* h, const float* x, const float* y, int B
   const SimtEncoder& SE = *E->simt; const SimtDecoder& SD = *D->simt;
   E->last_batch = B;
   AAE_TRY(encoder_forward_simt(E, x, 0, B, h->z.p, s));
-  AAE_TRY(decoder_forward_impl(D, h->z.p, B, h->rec.p, s));
+  if (h->w_v > 0.f) AAE_TRY(sigma_head_pre(E, SE.out.back().p, B, h->partials, h->pre.p, s));
+  if (latent_terms_on(h)) AAE_TRY(launch_latent(latent_args(h, B, loss_out), 0, s));
+  AAE_TRY(decoder_forward_impl(D, decoder_input(h), B, h->rec.p, s));
   const int k = h->bootstrap_ratio > 1 ? numel / h->bootstrap_ratio : numel;
   AAE_TRY(launch_bootstrap_l2(h->rec.p, y, B, numel, k, h->sample_sums.p, loss_out, h->dx_out.p, s));
   // ---- decoder backward ----
@@ -1224,7 +1370,8 @@ static int trainer_fwd_bwd(aae_trainer* h, const float* x, const float* y, int B
     dy = ping;
     std::swap(ping, pong);
   }
-  AAE_TRY(decoder_dense_backward(h, dy, B, s));
+  AAE_TRY(decoder_dense_backward(h, decoder_input(h), dy, B, s));
+  if (latent_terms_on(h)) AAE_TRY(launch_latent(latent_args(h, B, loss_out), 1, s));
   // ---- encoder backward ----
   {
     const int nl = (int)E->conv.size();
@@ -1272,6 +1419,8 @@ extern "C" int aae_train_step(aae_trainer* h, const float* x_dev, const float* y
   ab.count = 0;
   for (auto* v : {&h->enc_k, &h->enc_b, &h->dec_k, &h->dec_b})
     for (auto& pg : *v) {
+      // a step without VARIATIONAL leaves the sigma head out of the loss: no gradient, no update (TF skips None gradients)
+      if (h->head && !(h->w_v > 0.f) && (pg.p == h->enc->sig_w.p || pg.p == h->enc->sig_b.p)) continue;
       if (ab.count == AdamBatch::kMax) { AAE_TRY(launch_adam_multi(ab, lr_t, h->b1, h->b2, h->eps, s)); ab.count = 0; }
       const int t = ab.count++;
       ab.p[t] = pg.p; ab.g[t] = pg.g.p; ab.m[t] = pg.m.p; ab.v[t] = pg.v.p; ab.n[t] = (long long)pg.n;

@@ -173,6 +173,25 @@ int launch_occlusion(const uint8_t* mask, int B, int H, int W, const uint32_t* b
                      double max_occl, int square, double min_kept, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, uint8_t* out,
                      int32_t* fallbacks, cudaStream_t s);
 
+// ---- latent terms of the loss (latent.cu): sigma head activation, sampled z, KL and norm terms, their backward ----------
+// Every tensor is [B, J] row-major (dcat [B, 2J]); a null pointer leaves that part out.  Forward: sigma / sz from pre and z,
+// sums[0] = KL mean, sums[1] = norm-term mean.  Backward: dz holds d(sampled z) on entry and dz on exit; dpre and dcat = [dz | dpre]
+// are written; loss += sums[1] w_n (w_n > 0), then += sums[0] w_v (w_v != 0).
+struct LatentArgs {
+  const float* z = nullptr;
+  const float* pre = nullptr;   // sigma head pre-activation; null: no head
+  int B = 0, J = 0;
+  float eps = 0.f, w_v = 0.f, w_n = 0.f;
+  float* sigma = nullptr;
+  float* sz = nullptr;
+  float* sums = nullptr;        // [2]
+  float* dz = nullptr;
+  float* dpre = nullptr;
+  float* dcat = nullptr;
+  float* loss = nullptr;
+};
+int launch_latent(const LatentArgs& a, int backward, cudaStream_t stream);
+
 // ---- codebook ------------------------------------------------------------------------------
 int launch_l2_normalize(const float* z, int B, int J, float* out, cudaStream_t stream);
 

@@ -126,6 +126,16 @@ AAE_API int aae_encoder_activation(aae_encoder* h, int layer, const float** ptr_
  * order, then the dense layer) and their count is returned (>= 0; negative = error). */
 AAE_API int aae_encoder_profile(aae_encoder* h, int enable, float* stage_ms_out, int capacity);
 
+/* Sigma head of the variational AE, q_sigma = 1e-8 + softplus(encoder_out . W + b) (auto_pose/ae/encoder.py:70-79; built
+ * only when the training cfg sets VARIATIONAL, auto_pose/ae/ae_factory.py:50-58).  Allocates W [flat, latent] and b [latent],
+ * zero-initialised like the reference's kernel_initializer=zeros (a fresh head gives sigma = ln 2); calling it again is a
+ * no-op.  Afterwards layer num_layers + 1 of aae_encoder_set_weights / get_weights addresses the head (TF name
+ * "<scope>/dense_1").  Call it before aae_trainer_create*: a trainer created over the handle earlier runs without the head. */
+AAE_API int aae_encoder_enable_sigma_head(aae_encoder* h);
+/* q_sigma [batch, latent] of the first `batch` crops of the last forward (Encoder.q_sigma, auto_pose/ae/encoder.py:70-79):
+ * the fp32 head GEMM and the forward half of the training step's latent kernel.  No head: AAE_ERR_UNSUPPORTED. */
+AAE_API int aae_encoder_sigma_forward(aae_encoder* h, int batch, float* q_sigma_out_dev, void* stream);
+
 /* ---------------------------------------------------------------- Codebook -----------------
  * Replaces the Codebook graph: tf.nn.l2_normalize(z,1), matmul(zq, embedding_normalized^T),
  * argmax (auto_pose/ae/codebook.py:27,50-51) and the host-side np.argmax / strided argmax /
@@ -263,6 +273,19 @@ AAE_API int aae_trainer_get_state(aae_trainer* h, int which, int layer, float* k
 AAE_API int aae_trainer_set_state(aae_trainer* h, int which, int layer, const float* kernel_m_any, const float* kernel_v_any,
                                   const float* bias_m_any, const float* bias_v_any, void* stream);
 AAE_API int aae_trainer_set_global_step(aae_trainer* h, int64_t step);
+/* The latent terms of AE.loss (auto_pose/ae/ae.py:43-53): loss = reconstr_loss, + reg_loss * norm_regularize if that is > 0,
+ * + kl_div_loss * variational if that is non-zero, fp32 adds in this order (auto_pose/ae/encoder.py:82-100):
+ *   reg_loss    = mean_b | ||z_b|| - 1 |                        (on z; a row with ||z|| = 0 is outside the contract)
+ *   kl_div_loss = mean_{b,j} KL(N(z, q_sigma) || N(0, 1))
+ * variational > 0 also feeds the decoder sampled_z = z + q_sigma * eps (auto_pose/ae/ae_factory.py:58), with eps ONE scalar
+ * per step shared by every sample and latent dimension (tf.random_normal(tf.shape(<python int>)) is a 0-d draw; DESIGN.md
+ * section 3), set by aae_trainer_set_latent_noise; the sigma head is then trained too (get_grads / get_state / set_state with
+ * which = 0, layer = num_layers + 1).  Both 0 (the default): the step is exactly the one without latent terms.
+ * variational > 0 on a trainer whose encoder had no sigma head when it was created: AAE_ERR_UNSUPPORTED; a negative weight:
+ * AAE_ERR_INVALID_ARG.  Host-side settings only: nothing is synchronised. */
+AAE_API int aae_trainer_set_latent_terms(aae_trainer* h, float variational, float norm_regularize);
+/* eps of the next forward / backward (a draw of N(0,1); the caller owns the random stream). */
+AAE_API int aae_trainer_set_latent_noise(aae_trainer* h, float eps);
 /* Per-phase device time of the last training step (cudaEvents on the launching stream; tensor-core trainer only):
  * phase_ms_out[0..6] = operand packs, forward + loss, wgrad GEMMs, dgrad GEMMs, glue (masks / bias sums / re-splits),
  * fp32 backward of the dense layers and of conv1, Adam.  Same enable/read contract as aae_encoder_profile; returns the

@@ -1,0 +1,81 @@
+"""CPU oracle of the latent terms of the AE loss (VARIATIONAL and NORM_REGULARIZE).  TEST INFRASTRUCTURE ONLY, like
+aae_oracle.py, whose TF op restatements it builds on: torch on the CPU, float64 = "truth", float32 = "TF stand-in".
+Restates auto_pose/ae/encoder.py:70-100, ae.py:43-53 and ae_factory.py:50-77 (paths relative to /root/reference)."""
+from __future__ import annotations
+
+from typing import Dict, Optional, Tuple
+
+import numpy as np
+import torch
+import torch.nn.functional as F
+
+from oracle.aae_oracle import BOOTSTRAP_RATIO, STRIDES, _t, bootstrapped_l2, conv2d_same, decoder_layers
+
+
+def q_sigma(flat: torch.Tensor, kernel: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
+    """1e-8 + tf.layers.dense(encoder_out, latent, activation=tf.nn.softplus) (encoder.py:70-79)."""
+    return 1e-8 + F.softplus(flat @ kernel + bias)
+
+
+def sampled_z(z: torch.Tensor, sigma: torch.Tensor, eps: float) -> torch.Tensor:
+    """z + q_sigma * eps with eps = tf.random_normal(tf.shape(<python int>)): ONE scalar for the whole batch
+    (encoder.py:81-84)."""
+    return z + sigma * eps
+
+
+def kl_div_loss(z: torch.Tensor, sigma: torch.Tensor) -> torch.Tensor:
+    """reduce_mean(kl_divergence(Normal(z, sigma), Normal(0, 1))) in TF's form (z^2 + sigma^2 - 1 - log sigma^2) / 2
+    (encoder.py:87-94)."""
+    s2 = sigma * sigma
+    return (0.5 * z * z + 0.5 * (s2 - 1.0 - torch.log(s2))).mean()
+
+
+def norm_reg_loss(z: torch.Tensor) -> torch.Tensor:
+    """reduce_mean(|norm(z, axis=1) - 1|) (encoder.py:97-100)."""
+    return (torch.linalg.vector_norm(z, dim=1) - 1.0).abs().mean()
+
+
+def vae_forward_loss(x: np.ndarray, target: np.ndarray, enc: Dict[str, np.ndarray], dec: Dict[str, np.ndarray],
+                     head: Optional[Tuple[np.ndarray, np.ndarray]] = None, variational: float = 0.0,
+                     norm_regularize: float = 0.0, eps: float = 0.0, dtype: torch.dtype = torch.float32,
+                     bootstrap_ratio: int = BOOTSTRAP_RATIO, with_grads: bool = False):
+    """AE.loss with the latent terms (ae.py:43-53): reconstr_loss, + reg_loss * norm_regularize if that is > 0, + kl_div_loss *
+    variational if that is non-zero; the decoder reads sampled_z when variational is set (ae_factory.py:58).
+    ``enc`` / ``dec`` as for aae_oracle.ae_forward_loss (decoder dense under "dense_1"); ``head`` = (kernel [flat, latent],
+    bias [latent]) of the sigma head, required when variational.
+    Returns (loss, terms, grads or None).  terms: z, q_sigma, sampled_z (numpy), kl, reg (floats).  Gradients are keyed by the
+    variational graph's TF names when variational (head "dense_1", decoder dense "dense_2"), else by the plain names."""
+    if variational and head is None:
+        raise ValueError("variational needs the sigma head")
+    tp = {k: _t(v, dtype).requires_grad_(with_grads) for k, v in {**enc, **dec}.items()}
+    hk = hb = None
+    if head is not None:
+        hk, hb = (_t(a, dtype).requires_grad_(with_grads) for a in head)
+    strides = STRIDES[:sum(1 for k in enc if k.startswith("conv2d") and k.endswith("kernel"))]
+    with torch.set_grad_enabled(with_grads):
+        h = _t(x, dtype)
+        for i, s in enumerate(strides):
+            name = "conv2d" if i == 0 else f"conv2d_{i}"
+            h = conv2d_same(h, tp[f"{name}/kernel"], tp[f"{name}/bias"], s, "relu")
+        flat = h.reshape(h.shape[0], -1)
+        z = flat @ tp["dense/kernel"] + tp["dense/bias"]
+        sigma = q_sigma(flat, hk, hb) if head is not None else None
+        zin = sampled_z(z, sigma, eps) if variational else z
+        rec = decoder_layers(zin, tp, out_hw=x.shape[1], strides=strides, n_encoder_convs=len(strides))[-1]
+        loss = bootstrapped_l2(rec, _t(target, dtype), bootstrap_ratio)
+        reg = norm_reg_loss(z)
+        kl = kl_div_loss(z, sigma) if sigma is not None else None
+        if norm_regularize > 0:
+            loss = loss + reg * norm_regularize
+        if variational:
+            loss = loss + kl * variational
+        grads = None
+        if with_grads:
+            loss.backward()
+            grads = {k: v.grad.numpy() for k, v in tp.items()}
+            if variational:
+                grads["dense_2/kernel"], grads["dense_2/bias"] = grads.pop("dense_1/kernel"), grads.pop("dense_1/bias")
+                grads["dense_1/kernel"], grads["dense_1/bias"] = hk.grad.numpy(), hb.grad.numpy()
+    terms = {"z": z.detach().numpy(), "q_sigma": None if sigma is None else sigma.detach().numpy(),
+             "sampled_z": zin.detach().numpy(), "kl": None if kl is None else float(kl.detach()), "reg": float(reg.detach())}
+    return float(loss.item()), terms, grads
