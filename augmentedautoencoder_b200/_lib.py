@@ -10,6 +10,14 @@ AAE_MAX_LAYERS = 8
 PREC_FP32_SIMT = 0
 PREC_TC_SPLIT = 1
 PREC_TC_FP16 = 2      # encoder + codebook match handles, and the trainer's GEMMs (TrainOp(precision=...)): one fp16 product per K step
+# aae_optimizer_kind: the update rule of the training step (ae_factory.OPTIMIZERS maps cfg names to these)
+OPT_ADAM = 0
+OPT_GRADIENT_DESCENT = 1
+OPT_ADAGRAD = 2
+OPT_PROXIMAL_ADAGRAD = 3
+OPT_ADADELTA = 4
+OPT_RMSPROP = 5
+OPT_FTRL = 6
 
 
 class AaeError(RuntimeError):
@@ -20,6 +28,10 @@ class NetCfg(C.Structure):
     _fields_ = [("in_h", C.c_int32), ("in_w", C.c_int32), ("in_c", C.c_int32), ("num_layers", C.c_int32),
                 ("filters", C.c_int32 * AAE_MAX_LAYERS), ("strides", C.c_int32 * AAE_MAX_LAYERS),
                 ("kernel_size", C.c_int32), ("latent", C.c_int32), ("max_batch", C.c_int32), ("precision", C.c_int32)]
+
+
+class Optimizer(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("learning_rate", C.c_float), ("hp", C.c_float * 4)]
 
 
 _P = C.c_void_p
@@ -63,6 +75,7 @@ _SIGS = {
     "aae_bootstrap_l2_loss": (_I, [_P, _P, _I, _I, _I, _P, _P, _P]),
     "aae_trainer_create": (_I, [_P, _P, _I, _F, _F, _F, _F, C.POINTER(_P)]),
     "aae_trainer_create_prec": (_I, [_P, _P, _I, _F, _F, _F, _F, _I, C.POINTER(_P)]),
+    "aae_trainer_create_opt": (_I, [_P, _P, _I, C.POINTER(Optimizer), _I, C.POINTER(_P)]),
     "aae_trainer_destroy": (_I, [_P]),
     "aae_train_step": (_I, [_P, _P, _P, _I, _P, _P]),
     "aae_trainer_forward_backward": (_I, [_P, _P, _P, _I, _P, _P]),

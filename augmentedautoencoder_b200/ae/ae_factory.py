@@ -97,19 +97,52 @@ def build_ae(encoder, decoder, args):
     return AE(encoder, decoder, NORM_REGULARIZE, VARIATIONAL)
 
 
+# cfg OPTIMIZER -> (aae_optimizer_kind, aae_optimizer.hp at TF's defaults, slot names in TF's creation order).  The reference builds
+# tf.train.<OPTIMIZER>Optimizer(LEARNING_RATE) (ae_factory.py:79-95), so every other constructor argument keeps TF's default.
+# Formulas, initial slot values and what is unverified: DESIGN.md section 3.
+OPTIMIZERS = {
+    "Adam": (_lib.OPT_ADAM, (0.9, 0.999, 1e-8), ("Adam", "Adam_1")),
+    "GradientDescent": (_lib.OPT_GRADIENT_DESCENT, (), ()),
+    "ProximalGradientDescent": (_lib.OPT_GRADIENT_DESCENT, (), ()),      # l1 = l2 = 0: gradient descent bit for bit
+    "Adagrad": (_lib.OPT_ADAGRAD, (0.1,), ("Adagrad",)),                   # initial_accumulator_value
+    "ProximalAdagrad": (_lib.OPT_PROXIMAL_ADAGRAD, (0.1,), ("ProximalAdagrad",)),
+    "Adadelta": (_lib.OPT_ADADELTA, (0.95, 1e-8), ("Adadelta", "Adadelta_1")),       # rho, epsilon
+    "RMSProp": (_lib.OPT_RMSPROP, (0.9, 0.0, 1e-10), ("RMSProp", "RMSProp_1")),      # decay, momentum, epsilon
+    "Ftrl": (_lib.OPT_FTRL, (0.1,), ("Ftrl", "Ftrl_1")),                            # initial_accumulator_value
+}
+# tf.train optimizers whose constructor needs an argument besides the learning rate: the reference's call fails for them
+_NEEDS_ARGUMENT = {"Momentum": "momentum", "AdagradDA": "global_step"}
+
+
+def optimizer_spec(name):
+    """(kind, hp, slot names) of a cfg OPTIMIZER; ValueError for a name no reference cfg can train with."""
+    if name in _NEEDS_ARGUMENT:
+        raise ValueError("OPTIMIZER: %s: tf.train.%sOptimizer needs `%s`, which a cfg cannot pass, so the reference cannot build it from a "
+                         "cfg either" % (name, name, _NEEDS_ARGUMENT[name]))
+    if name not in OPTIMIZERS:
+        raise ValueError("OPTIMIZER: %s is not one of the tf.train optimizers a cfg can build: %s" % (name, ", ".join(OPTIMIZERS)))
+    return OPTIMIZERS[name]
+
+
 class TrainOp(Tensor):
-    """``session.run(train_op)``: encoder fwd, decoder fwd, bootstrapped L2, backward, TF-Adam, global_step += 1 -- one call
-    into aae_train_step (replaces slim.learning.create_train_op, ae_factory.py:86-88).  Evaluates to the loss.
+    """``session.run(train_op)``: encoder fwd, decoder fwd, bootstrapped L2, backward, the optimizer update, global_step += 1 -- one
+    call into aae_train_step (replaces slim.learning.create_train_op, ae_factory.py:86-88).  Evaluates to the loss.
+
+    ``optimizer`` is a cfg OPTIMIZER name (OPTIMIZERS).  beta1, beta2 and epsilon are Adam's; every other rule runs at TF's
+    defaults, the only values a cfg reaches.
 
     ``precision`` picks the GEMM arithmetic of the step apart from the handles' (aae_trainer_create_prec).  None follows the
     handles.  ``_lib.PREC_TC_FP16`` is the single-pass trainer: it needs PREC_TC_SPLIT encoder and decoder handles, which keep
     that precision for inference, and raises for any other handles instead of switching their precision."""
 
-    def __init__(self, ae, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8, precision=None, noise_seed=0):
+    def __init__(self, ae, learning_rate, beta1=0.9, beta2=0.999, epsilon=1e-8, precision=None, noise_seed=0, optimizer="Adam"):
         """noise_seed seeds the stream of VARIATIONAL's eps, one N(0,1) draw per step (Encoder.run_eps)."""
         super().__init__("train_op", (), np.float32, self._run)
         self._ae = ae
         self._hp = (float(learning_rate), float(beta1), float(beta2), float(epsilon))
+        kind, hp, self._slots = optimizer_spec(optimizer)
+        hp = self._hp[1:] if kind == _lib.OPT_ADAM else hp
+        self._opt = _lib.Optimizer(kind, self._hp[0], (C.c_float * 4)(*hp))
         self._precision = None if precision is None else int(precision)
         self._trainers = {}
         self._eps_rng = np.random.RandomState(noise_seed)
@@ -130,18 +163,20 @@ class TrainOp(Tensor):
             h = C.c_void_p()
             with torch.cuda.device(dev):
                 eh, dh = enc.handle(device), dec.handle(device)       # settles automatic precisions
+                def create(eh, dh, gemm):
+                    return _lib.lib().aae_trainer_create_opt(eh, dh, dec._bootstrap_ratio, C.byref(self._opt), gemm, C.byref(h))
                 if self._precision is not None:
                     # an explicit GEMM precision: the handles must suit it as they are (an automatic fp32 fallback does not)
-                    _lib.check(_lib.lib().aae_trainer_create_prec(eh, dh, dec._bootstrap_ratio, *self._hp, self._precision, C.byref(h)),
-                               "trainer create (GEMM precision %d)" % self._precision)
+                    _lib.check(create(eh, dh, self._precision), "trainer create (GEMM precision %d)" % self._precision)
                 else:
-                    st = -3 if enc.precision != dec.precision else _lib.lib().aae_trainer_create(eh, dh, dec._bootstrap_ratio, *self._hp, C.byref(h))
+                    # GEMMs at the handles' own precision (aae_trainer_create)
+                    st = -3 if enc.precision != dec.precision else create(eh, dh, enc.precision)
                     if st == -3 and (enc._auto_precision or dec._auto_precision or enc.precision != dec.precision) and \
                             (enc.precision, dec.precision) != (_lib.PREC_FP32_SIMT, _lib.PREC_FP32_SIMT):
                         # a geometry the tensor-core trainer is not built for: the fp32 CUDA-core trainer handles every geometry
                         enc.set_precision(_lib.PREC_FP32_SIMT)
                         dec.set_precision(_lib.PREC_FP32_SIMT)
-                        st = _lib.lib().aae_trainer_create(enc.handle(device), dec.handle(device), dec._bootstrap_ratio, *self._hp, C.byref(h))
+                        st = create(enc.handle(device), dec.handle(device), _lib.PREC_FP32_SIMT)
                     _lib.check(st, "trainer create")
                 if ae._variational or ae._norm_regularize > 0:
                     # AE.loss adds reg_loss only for NORM_REGULARIZE > 0 and the KL term for VARIATIONAL != 0 (ae.py:43-53)
@@ -188,14 +223,19 @@ class TrainOp(Tensor):
         eps = self._ae._encoder.run_eps(ctx, draw=self._eps_rng.standard_normal) if self._ae._variational else None
         return self.step_device(x, y, update=True, eps=eps)
 
-    # -- optimizer state under TensorFlow's names: "<var>/Adam", "<var>/Adam_1", "<scope>/beta1_power", "<scope>/beta2_power" ------
+    # -- optimizer state under TensorFlow's names: "<var>/<slot>" (OPTIMIZERS), and Adam's "<scope>/beta1_power", "<scope>/beta2_power"
     def _scope_prefix(self):
         name = self._ae._encoder._var_shapes[0][0]                    # e.g. "obj_05/conv2d/kernel"
         return name.rsplit("/", 2)[0] + "/" if name.count("/") >= 2 else ""
 
+    def _slot_arrays(self, ks, bs):
+        """(kernel slot 0, kernel slot 1, bias slot 0, bias slot 1): arrays for the rule's slots, None for the others"""
+        n = len(self._slots)
+        return [np.empty(shape, np.float32) if k < n else None for shape in (ks, bs) for k in (0, 1)]
+
     def optimizer_variables(self, device=None):
-        """{TF name: array} of the Adam slots and beta powers (what tf.train.Saver stores beside the weights, ae_train.py:82).
-        Empty until a trainer exists (no step has run): a fresh optimizer has nothing to save."""
+        """{TF name: array} of the optimizer's slots, and Adam's beta powers (what tf.train.Saver stores beside the weights,
+        ae_train.py:82).  Empty until a trainer exists (no step has run): a fresh optimizer has nothing to save."""
         if not self._trainers:
             return {}
         dev = next(iter(self._trainers)) if device is None else (device.index if isinstance(device, torch.device) else int(device))
@@ -204,10 +244,14 @@ class TrainOp(Tensor):
         with torch.cuda.device(dev):
             for which, mod in ((0, self._ae._encoder), (1, self._ae._decoder)):
                 for i, (kn, ks, bn, bs) in enumerate(mod._var_shapes):
-                    km, kv, bm, bv = np.empty(ks, np.float32), np.empty(ks, np.float32), np.empty(bs, np.float32), np.empty(bs, np.float32)
+                    km, kv, bm, bv = self._slot_arrays(ks, bs)
                     _lib.check(_lib.lib().aae_trainer_get_state(h, which, i, _lib.ptr(km), _lib.ptr(kv), _lib.ptr(bm), _lib.ptr(bv), None), "get_state")
-                    out[kn + "/Adam"], out[kn + "/Adam_1"], out[bn + "/Adam"], out[bn + "/Adam_1"] = km, kv, bm, bv
+                    for name, arrs in ((kn, (km, kv)), (bn, (bm, bv))):
+                        for suffix, a in zip(self._slots, arrs):
+                            out[name + "/" + suffix] = a
             step = int(_lib.lib().aae_trainer_global_step(h))
+        if self._opt.kind != _lib.OPT_ADAM:
+            return out
         lr, b1, b2, eps = self._hp
         # TF keeps beta^(t+1) after t updates (initialised to beta, multiplied once per apply)
         out[self._scope_prefix() + "beta1_power"] = np.asarray(b1 ** (step + 1), dtype=np.float32)
@@ -215,16 +259,18 @@ class TrainOp(Tensor):
         return out
 
     def load_optimizer_variables(self, weights, device, global_step=None):
-        """Restore the Adam slots (and the update count) from a checkpoint dict; returns the names it used.  Variables without
-        slots in the dict keep their current (zero) moments -- a weights-only checkpoint restarts the optimizer, as in TF."""
+        """Restore the optimizer's slots (and the update count) from a checkpoint dict; returns the names it used.  Variables
+        without slots in the dict keep their current ones -- for a new trainer the rule's initial values, so a weights-only
+        checkpoint restarts the optimizer, as in TF.  The step comes from ``global_step``, or for Adam from beta1_power."""
         h = self.trainer(device)
         used = []
         with torch.cuda.device(device):
             for which, mod in ((0, self._ae._encoder), (1, self._ae._decoder)):
                 for i, (kn, ks, bn, bs) in enumerate(mod._var_shapes):
                     arrs = []
-                    for name, shape in ((kn + "/Adam", ks), (kn + "/Adam_1", ks), (bn + "/Adam", bs), (bn + "/Adam_1", bs)):
-                        a = weights.get(name)
+                    names = [base + "/" + self._slots[k] if k < len(self._slots) else None for base in (kn, bn) for k in (0, 1)]
+                    for name, shape in zip(names, (ks, ks, bs, bs)):
+                        a = weights.get(name) if name else None
                         if a is not None:
                             a = np.ascontiguousarray(np.asarray(a, dtype=np.float32))
                             if a.shape != tuple(shape):
@@ -234,7 +280,7 @@ class TrainOp(Tensor):
                     if any(a is not None for a in arrs):
                         _lib.check(_lib.lib().aae_trainer_set_state(h, which, i, *[_lib.ptr(a) for a in arrs], None), "set_state")
             step = global_step
-            b1p = weights.get(self._scope_prefix() + "beta1_power")
+            b1p = weights.get(self._scope_prefix() + "beta1_power") if self._opt.kind == _lib.OPT_ADAM else None
             if step is None and b1p is not None and 0.0 < float(b1p) < 1.0:
                 step = int(round(np.log(float(b1p)) / np.log(self._hp[1]))) - 1
             if step is not None:
@@ -259,9 +305,8 @@ def build_train_op(ae, args, precision=None):
     """precision: the GEMM arithmetic of the training step (see TrainOp); None follows the encoder and decoder handles."""
     LEARNING_RATE = args.getfloat('Training', 'LEARNING_RATE')
     OPTIMIZER_NAME = args.get('Training', 'OPTIMIZER')
-    if OPTIMIZER_NAME != 'Adam':
-        raise NotImplementedError("OPTIMIZER: %s (the fused step implements tf.train.AdamOptimizer)" % OPTIMIZER_NAME)
-    return TrainOp(ae, LEARNING_RATE, precision=precision)
+    optimizer_spec(OPTIMIZER_NAME)
+    return TrainOp(ae, LEARNING_RATE, precision=precision, optimizer=OPTIMIZER_NAME)
 
 
 def build_codebook(encoder, dataset, args):

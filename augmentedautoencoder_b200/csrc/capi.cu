@@ -132,7 +132,7 @@ IGemmParams dense_params(const float* src, int B, int in_features, const float* 
 
 // Per-phase device timing of the training step: every mark opens a phase; the time until the next mark is charged to it.
 struct PhaseTimer {
-  static constexpr int kPhases = 7;   // 0 operand packs, 1 forward + loss, 2 wgrad GEMMs, 3 dgrad GEMMs, 4 glue, 5 fp32 dense / conv1 backward, 6 Adam
+  static constexpr int kPhases = 7;   // 0 operand packs, 1 forward + loss, 2 wgrad GEMMs, 3 dgrad GEMMs, 4 glue, 5 fp32 dense / conv1 backward, 6 optimizer update
   bool enabled = false;
   std::vector<cudaEvent_t> ev;
   std::vector<int> phase;
@@ -203,7 +203,7 @@ struct aae_encoder {
   SimtEncoder* simt = nullptr;  // fp32 CUDA-core workspace (AAE_PREC_FP32_SIMT)
   TcEncoder* tc = nullptr;  // tensor-core execution plan (AAE_PREC_TC_SPLIT or AAE_PREC_TC_FP16)
   int last_batch = 0;
-  // the fp32 tensors above are the master copy.  w_version counts its changes (set_weights, Adam); every copy derived from it
+  // the fp32 tensors above are the master copy.  w_version counts its changes (set_weights, optimizer steps); every copy derived from it
   // (the tensor-core plan's packed (hi, lo) fp16 operands, the fp32 decoder's merged sub-pixel weights, the trainer's dgrad
   // operands) records the w_version it was built from and is rebuilt just before its next use when the two differ.
   uint64_t w_version = 1;
@@ -237,16 +237,16 @@ struct aae_codebook {
 
 struct ParamGrad {
   float* p; size_t n;   // parameter (owned by encoder/decoder)
-  DevBuf g, m, v;
+  DevBuf g, s0, s1;     // gradient; the optimizer's slots in TF's creation order (only those the rule has are allocated)
 };
 
 struct aae_trainer {
   aae_encoder* enc;
   aae_decoder* dec;
   int bootstrap_ratio;
-  float lr, b1, b2, eps;
+  aae_optimizer opt;
   int64_t step = 0;
-  // gradients / Adam state: enc conv kernels+biases, enc dense, dec dense, dec convs (same order as *_set_weights)
+  // gradients / optimizer slots: enc conv kernels+biases, enc dense, dec dense, dec convs (same order as *_set_weights)
   std::vector<ParamGrad> enc_k, enc_b, dec_k, dec_b;
   DevBuf dx_out;        // dLoss/d(decoder output) then pre-sigmoid grad  [B, H, W, C]
   DevBuf grad_a;        // fp32 trainer: ping-pong pre-activation gradients with grad_b; tensor-core trainer: gradient wrt `flat`
@@ -401,7 +401,7 @@ extern "C" int aae_encoder_set_weights(aae_encoder* h, int layer, const float* k
   h->w_version += 1;
   if (h->tc && kernel_any) AAE_TRY(tc_encoder_pack_weights(h->tc, layer, w.p, s));
   if (h->tc) AAE_TRY(tc_encoder_set_bias(h->tc, layer, b.p));
-  if (tc_current) h->tc_version = h->w_version;   // this layer is packed again; a plan behind by an Adam step stays behind
+  if (tc_current) h->tc_version = h->w_version;   // this layer is packed again; a plan behind by an optimizer step stays behind
   AAE_CUDA_OK(cudaStreamSynchronize(s));  // host source buffers may be freed by the caller on return
   if (h->tc) AAE_TRY(range_peek(tc_encoder_range_flag(h->tc), "encoder set_weights", 0, s, h->cfg.precision));
   return AAE_OK;
@@ -911,38 +911,58 @@ extern "C" int aae_bootstrap_l2_loss(const float* x_dev, const float* target_dev
 }
 
 // ============================================================================ trainer
-static int make_pg(std::vector<ParamGrad>& v, DevBuf& param) {
+// initial value of slot k, as the tf.train optimizer creates it: the accumulators start at initial_accumulator_value, RMSProp's
+// rms at 1, every other slot at 0
+static float opt_slot_init(const aae_optimizer& o, int k) {
+  if (k == 0 && (o.kind == AAE_OPT_ADAGRAD || o.kind == AAE_OPT_PROXIMAL_ADAGRAD || o.kind == AAE_OPT_FTRL)) return o.hp[0];
+  if (k == 0 && o.kind == AAE_OPT_RMSPROP) return 1.f;
+  return 0.f;
+}
+
+static int fill_slot(DevBuf& b, float value) {
+  if (value == 0.f) AAE_CUDA_OK(cudaMemset(b.p, 0, b.n * 4));
+  else {
+    std::vector<float> init(b.n, value);
+    AAE_CUDA_OK(cudaMemcpy(b.p, init.data(), b.n * 4, cudaMemcpyHostToDevice));
+  }
+  return AAE_OK;
+}
+
+static int make_pg(std::vector<ParamGrad>& v, DevBuf& param, const aae_optimizer& opt) {
   v.emplace_back();
   ParamGrad& g = v.back();
   g.p = param.p; g.n = param.n;
+  const int slots = opt_slot_count(opt.kind);
   AAE_TRY(g.g.alloc(param.n));
-  AAE_TRY(g.m.alloc(param.n));
-  AAE_TRY(g.v.alloc(param.n));
-  cudaMemset(g.g.p, 0, param.n * 4); cudaMemset(g.m.p, 0, param.n * 4); cudaMemset(g.v.p, 0, param.n * 4);
+  AAE_TRY(g.s0.alloc(slots >= 1 ? param.n : 0));
+  AAE_TRY(g.s1.alloc(slots >= 2 ? param.n : 0));
+  cudaMemset(g.g.p, 0, param.n * 4);
+  if (slots >= 1) AAE_TRY(fill_slot(g.s0, opt_slot_init(opt, 0)));
+  if (slots >= 2) AAE_TRY(fill_slot(g.s1, opt_slot_init(opt, 1)));
   return AAE_OK;
 }
 
 // The trainer over handles whose precisions are known to be trainable (FP32_SIMT or TC_SPLIT).  single_pass: the forward, dgrad
 // and wgrad GEMMs run on private hi-only plans instead of the handles' split plans.
-static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate, float beta1, float beta2,
-                          float epsilon, bool single_pass, aae_trainer** out) {
+static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, const aae_optimizer& opt, bool single_pass,
+                          aae_trainer** out) {
   AAE_REQUIRE((enc->tc == nullptr) == (dec->tc == nullptr), "encoder and decoder must use the same aae_precision for training");
   AAE_REQUIRE(enc->cfg.max_batch == dec->cfg.max_batch && enc->cfg.in_h == dec->cfg.in_h, "encoder/decoder geometry mismatch");
   DeviceGuard g(enc->device);
   aae_trainer* h = new (std::nothrow) aae_trainer();
   AAE_REQUIRE(h != nullptr, "host allocation failed");
   h->enc = enc; h->dec = dec; h->bootstrap_ratio = bootstrap_ratio;
-  h->lr = learning_rate; h->b1 = beta1; h->b2 = beta2; h->eps = epsilon;
+  h->opt = opt;
   int st = AAE_OK;
-  for (auto& L : enc->conv) { if (st == AAE_OK) st = make_pg(h->enc_k, L.w); if (st == AAE_OK) st = make_pg(h->enc_b, L.b); }
-  if (st == AAE_OK) st = make_pg(h->enc_k, enc->dense_w);
-  if (st == AAE_OK) st = make_pg(h->enc_b, enc->dense_b);
+  for (auto& L : enc->conv) { if (st == AAE_OK) st = make_pg(h->enc_k, L.w, opt); if (st == AAE_OK) st = make_pg(h->enc_b, L.b, opt); }
+  if (st == AAE_OK) st = make_pg(h->enc_k, enc->dense_w, opt);
+  if (st == AAE_OK) st = make_pg(h->enc_b, enc->dense_b, opt);
   h->head = enc->sig_w.p != nullptr;
-  if (st == AAE_OK && h->head) st = make_pg(h->enc_k, enc->sig_w);
-  if (st == AAE_OK && h->head) st = make_pg(h->enc_b, enc->sig_b);
-  if (st == AAE_OK) st = make_pg(h->dec_k, dec->dense_w);
-  if (st == AAE_OK) st = make_pg(h->dec_b, dec->dense_b);
-  for (auto& L : dec->conv) { if (st == AAE_OK) st = make_pg(h->dec_k, L.w); if (st == AAE_OK) st = make_pg(h->dec_b, L.b); }
+  if (st == AAE_OK && h->head) st = make_pg(h->enc_k, enc->sig_w, opt);
+  if (st == AAE_OK && h->head) st = make_pg(h->enc_b, enc->sig_b, opt);
+  if (st == AAE_OK) st = make_pg(h->dec_k, dec->dense_w, opt);
+  if (st == AAE_OK) st = make_pg(h->dec_b, dec->dense_b, opt);
+  for (auto& L : dec->conv) { if (st == AAE_OK) st = make_pg(h->dec_k, L.w, opt); if (st == AAE_OK) st = make_pg(h->dec_b, L.b, opt); }
   const size_t B = enc->cfg.max_batch, max_dense_w = std::max(enc->dense_w.n, dec->dense_w.n);
   size_t max_act = 0, max_up = 0, max_w = max_dense_w, max_c = 0;
   for (auto& L : enc->conv) { max_act = std::max(max_act, L.out_count(B)); max_w = std::max(max_w, L.w_count()); max_c = std::max<size_t>(max_c, L.out_c); }
@@ -999,8 +1019,8 @@ static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_rati
   return AAE_OK;
 }
 
-extern "C" int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate, float beta1,
-                                  float beta2, float epsilon, aae_trainer** out) {
+// The trainer whose GEMMs follow the handles' precision (aae_trainer_create's contract).
+static int trainer_create_follow(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, const aae_optimizer& opt, aae_trainer** out) {
   AAE_REQUIRE(out != nullptr, "out is null");
   *out = nullptr;
   AAE_REQUIRE(enc && dec, "null handle");
@@ -1011,38 +1031,61 @@ extern "C" int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootst
               "inference-only)", enc->cfg.precision, dec->cfg.precision);
     return AAE_ERR_UNSUPPORTED;
   }
-  return trainer_create(enc, dec, bootstrap_ratio, learning_rate, beta1, beta2, epsilon, false, out);
+  return trainer_create(enc, dec, bootstrap_ratio, opt, false, out);
+}
+
+static aae_optimizer adam_optimizer(float learning_rate, float beta1, float beta2, float epsilon) {
+  aae_optimizer o;
+  o.kind = AAE_OPT_ADAM;
+  o.learning_rate = learning_rate;
+  o.hp[0] = beta1; o.hp[1] = beta2; o.hp[2] = epsilon; o.hp[3] = 0.f;
+  return o;
+}
+
+extern "C" int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate, float beta1,
+                                  float beta2, float epsilon, aae_trainer** out) {
+  return trainer_create_follow(enc, dec, bootstrap_ratio, adam_optimizer(learning_rate, beta1, beta2, epsilon), out);
 }
 
 static const char* precision_name(int p) {
   return p == AAE_PREC_FP32_SIMT ? "AAE_PREC_FP32_SIMT" : p == AAE_PREC_TC_SPLIT ? "AAE_PREC_TC_SPLIT" : "AAE_PREC_TC_FP16";
 }
 
-extern "C" int aae_trainer_create_prec(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate, float beta1,
-                                       float beta2, float epsilon, int gemm_precision, aae_trainer** out) {
+extern "C" int aae_trainer_create_opt(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, const aae_optimizer* opt,
+                                      int gemm_precision, aae_trainer** out) {
   AAE_REQUIRE(out != nullptr, "out is null");
   *out = nullptr;
-  AAE_REQUIRE(enc && dec, "null handle");
+  AAE_REQUIRE(enc && dec && opt, "null handle or optimizer");
+  AAE_REQUIRE(opt->kind >= AAE_OPT_ADAM && opt->kind <= AAE_OPT_FTRL, "optimizer kind %d is not an aae_optimizer_kind (0..6)", opt->kind);
+  // tf.train's AdagradOptimizer, ProximalAdagradOptimizer and FtrlOptimizer raise ValueError for this
+  AAE_REQUIRE(!(opt->kind == AAE_OPT_ADAGRAD || opt->kind == AAE_OPT_PROXIMAL_ADAGRAD || opt->kind == AAE_OPT_FTRL) || opt->hp[0] > 0.f,
+              "initial accumulator value must be > 0 (got %g)", (double)opt->hp[0]);
   AAE_REQUIRE(enc->device == dec->device, "encoder and decoder live on different devices");
   AAE_REQUIRE(gemm_precision == AAE_PREC_FP32_SIMT || gemm_precision == AAE_PREC_TC_SPLIT || gemm_precision == AAE_PREC_TC_FP16,
               "gemm_precision=%d is not an aae_precision (0, 1 or 2)", gemm_precision);
   const int ep = enc->cfg.precision, dp = dec->cfg.precision;
   if (gemm_precision != AAE_PREC_TC_FP16 && gemm_precision == ep && gemm_precision == dp)
-    return aae_trainer_create(enc, dec, bootstrap_ratio, learning_rate, beta1, beta2, epsilon, out);
+    return trainer_create_follow(enc, dec, bootstrap_ratio, *opt, out);
   if (gemm_precision != AAE_PREC_TC_FP16 || ep != AAE_PREC_TC_SPLIT || dp != AAE_PREC_TC_SPLIT) {
     set_error("trainer GEMM precision %s is unsupported with an %s encoder and an %s decoder: the GEMM precision must equal the handles' "
               "(AAE_PREC_FP32_SIMT or AAE_PREC_TC_SPLIT), or be AAE_PREC_TC_FP16 with two AAE_PREC_TC_SPLIT handles",
               precision_name(gemm_precision), precision_name(ep), precision_name(dp));
     return AAE_ERR_UNSUPPORTED;
   }
-  return trainer_create(enc, dec, bootstrap_ratio, learning_rate, beta1, beta2, epsilon, true, out);
+  return trainer_create(enc, dec, bootstrap_ratio, *opt, true, out);
+}
+
+extern "C" int aae_trainer_create_prec(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate, float beta1,
+                                       float beta2, float epsilon, int gemm_precision, aae_trainer** out) {
+  const aae_optimizer o = adam_optimizer(learning_rate, beta1, beta2, epsilon);
+  return aae_trainer_create_opt(enc, dec, bootstrap_ratio, &o, gemm_precision, out);
 }
 
 extern "C" int aae_trainer_destroy(aae_trainer* h) {
   if (!h) return AAE_OK;
   DeviceGuard g(h->enc->device);
   for (auto* v : {&h->enc_k, &h->enc_b, &h->dec_k, &h->dec_b})
-    for (auto& pg : *v) { pg.g.release(); pg.m.release(); pg.v.release(); }
+    for (auto& pg : *v) { pg.g.release(); pg.s0.release(); pg.s1.release(); }
   h->dx_out.release(); h->grad_a.release(); h->grad_b.release(); h->dxup.release(); h->flat.release(); h->wt.release(); h->partials.release();
   h->bias_scratch.release(); h->sample_sums.release(); h->z.release(); h->dz.release(); h->rec.release(); h->dwm.release();
   h->pre.release(); h->sz.release(); h->dpre.release(); h->dcat.release(); h->lat_sums.release();
@@ -1056,16 +1099,20 @@ extern "C" int aae_trainer_destroy(aae_trainer* h) {
 
 extern "C" int64_t aae_trainer_global_step(const aae_trainer* h) { return h ? h->step : -1; }
 
-// Adam slots of one variable pair (kernel, bias): m = TF's "<var>/Adam", v = "<var>/Adam_1".  get: dir = 0, set: dir = 1.
+// Optimizer slots of one variable pair (kernel, bias): slot 0 (km, bm) and slot 1 (kv, bv) of the trainer's rule, e.g. Adam's
+// m = TF's "<var>/Adam", v = "<var>/Adam_1".  get: dir = 0, set: dir = 1.
 static int trainer_state_io(aae_trainer* h, int which, int layer, float* km, float* kv, float* bm, float* bv, int dir, void* stream) {
   AAE_REQUIRE(h != nullptr && (which == 0 || which == 1), "bad arguments");
   std::vector<ParamGrad>& ks = which == 0 ? h->enc_k : h->dec_k;
   std::vector<ParamGrad>& bs = which == 0 ? h->enc_b : h->dec_b;
   AAE_REQUIRE(layer >= 0 && layer < (int)ks.size(), "layer %d out of range", layer);
+  const int slots = opt_slot_count(h->opt.kind);
+  struct { float* host; float* dev; size_t n; int slot; } io[4] = {{km, ks[layer].s0.p, ks[layer].n, 0}, {kv, ks[layer].s1.p, ks[layer].n, 1},
+                                                                   {bm, bs[layer].s0.p, bs[layer].n, 0}, {bv, bs[layer].s1.p, bs[layer].n, 1}};
+  for (auto& t : io)
+    AAE_REQUIRE(!t.host || t.slot < slots, "optimizer kind %d has %d slot(s); slot %d was passed", h->opt.kind, slots, t.slot);
   DeviceGuard g(h->enc->device);
   cudaStream_t s = (cudaStream_t)stream;
-  struct { float* host; float* dev; size_t n; } io[4] = {{km, ks[layer].m.p, ks[layer].n}, {kv, ks[layer].v.p, ks[layer].n},
-                                                          {bm, bs[layer].m.p, bs[layer].n}, {bv, bs[layer].v.p, bs[layer].n}};
   for (auto& t : io)
     if (t.host) AAE_TRY(dir ? copy_any(t.dev, t.host, t.n * sizeof(float), s) : copy_any(t.host, t.dev, t.n * sizeof(float), s));
   AAE_CUDA_OK(cudaStreamSynchronize(s));
@@ -1225,7 +1272,7 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
   TcEncoder* FE = own ? h->fenc : E->tc;
   TcDecoder* FD = own ? h->fdec : D->tc;
   uint64_t& fd_version = own ? h->fdec_version : D->tc_version;
-  // ---- operands follow the fp32 master weights (Adam and set_weights change those) ----
+  // ---- operands follow the fp32 master weights (optimizer steps and set_weights change those) ----
   AAE_TRY(own ? encoder_pack_plan(E, FE, h->fenc_version, s) : encoder_sync_tc(E, s));
   if (h->packed_dec_version != D->w_version || fd_version != D->w_version) {
     // forward and dgrad operands of a decoder layer share one merge of its 5x5 taps
@@ -1311,7 +1358,7 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
   }
   pt.mark(2, s);
   AAE_TRY(tc_train_conv1_wgrad(P, x, B, h->enc_k[0].g.p, s));
-  pt.mark(6, s);   // closes the last phase; aae_train_step charges Adam to phase 6 and closes it with one more mark
+  pt.mark(6, s);   // closes the last phase; aae_train_step charges the optimizer update to phase 6 and closes it with one more mark
   return AAE_OK;
 }
 
@@ -1413,19 +1460,23 @@ extern "C" int aae_train_step(aae_trainer* h, const float* x_dev, const float* y
   cudaStream_t s = (cudaStream_t)stream;
   AAE_TRY(trainer_fwd_bwd(h, x_dev, y_dev, batch, loss_out_dev, s));
   h->step += 1;
-  const double t = (double)h->step;
-  const float lr_t = (float)((double)h->lr * sqrt(1.0 - pow((double)h->b2, t)) / (1.0 - pow((double)h->b1, t)));
-  AdamBatch ab;
-  ab.count = 0;
+  const aae_optimizer& o = h->opt;
+  float lr = o.learning_rate;
+  if (o.kind == AAE_OPT_ADAM) {
+    const double t = (double)h->step;
+    lr = (float)((double)o.learning_rate * sqrt(1.0 - pow((double)o.hp[1], t)) / (1.0 - pow((double)o.hp[0], t)));
+  }
+  OptBatch ob;
+  ob.count = 0;
   for (auto* v : {&h->enc_k, &h->enc_b, &h->dec_k, &h->dec_b})
     for (auto& pg : *v) {
       // a step without VARIATIONAL leaves the sigma head out of the loss: no gradient, no update (TF skips None gradients)
       if (h->head && !(h->w_v > 0.f) && (pg.p == h->enc->sig_w.p || pg.p == h->enc->sig_b.p)) continue;
-      if (ab.count == AdamBatch::kMax) { AAE_TRY(launch_adam_multi(ab, lr_t, h->b1, h->b2, h->eps, s)); ab.count = 0; }
-      const int t = ab.count++;
-      ab.p[t] = pg.p; ab.g[t] = pg.g.p; ab.m[t] = pg.m.p; ab.v[t] = pg.v.p; ab.n[t] = (long long)pg.n;
+      if (ob.count == OptBatch::kMax) { AAE_TRY(launch_opt_multi(ob, o.kind, lr, o.hp, s)); ob.count = 0; }
+      const int t = ob.count++;
+      ob.p[t] = pg.p; ob.g[t] = pg.g.p; ob.s0[t] = pg.s0.p; ob.s1[t] = pg.s1.p; ob.n[t] = (long long)pg.n;
     }
-  if (ab.count) AAE_TRY(launch_adam_multi(ab, lr_t, h->b1, h->b2, h->eps, s));
+  if (ob.count) AAE_TRY(launch_opt_multi(ob, o.kind, lr, o.hp, s));
   h->ptimer.mark(6, s);
   // the masters changed in place: every derived copy (merged sub-pixel weights, inference plans, trainer dgrad operands) is now
   // one step behind

@@ -133,20 +133,24 @@ int launch_sumpool2_mask(const float* in, const float* mask, float* out, int B, 
 int launch_bias_grad(const float* dy, int64_t rows, int N, float* db, float* scratch256N, cudaStream_t stream);  // db[n] = sum_rows dy[row,n]
 int launch_mul_mask(float* dy, const float* y, int64_t n, cudaStream_t stream);              // dy *= (y > 0)
 int launch_sigmoid_grad(float* dx, const float* x, int64_t n, cudaStream_t stream);          // dx *= x (1 - x)
-int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, float lr_t, float b1, float b2, float eps,
-                cudaStream_t stream);
-// the same update for up to kMax tensors in one launch (fill p/g/m/v/n and count; chunk_begin is computed by the launcher)
-struct AdamBatch {
+// number of slots per variable of an aae_optimizer_kind: 0 gradient descent, 1 (Proximal)Adagrad, 2 the others
+constexpr int opt_slot_count(int kind) {
+  return kind == AAE_OPT_GRADIENT_DESCENT ? 0 : (kind == AAE_OPT_ADAGRAD || kind == AAE_OPT_PROXIMAL_ADAGRAD) ? 1 : 2;
+}
+// One optimizer update (aae_optimizer_kind) for up to kMax tensors in one launch.  Fill p/g/n, the rule's slots s0 (and s1)
+// and count; slots the rule does not have are not read.  chunk_begin is computed by the launcher.
+struct OptBatch {
   static constexpr int kMax = 32;
   float* p[kMax];
   const float* g[kMax];
-  float* m[kMax];
-  float* v[kMax];
+  float* s0[kMax];
+  float* s1[kMax];
   long long n[kMax];
   int chunk_begin[kMax + 1];
   int count;
 };
-int launch_adam_multi(AdamBatch& b, float lr_t, float b1, float b2, float eps, cudaStream_t stream);
+// lr: Adam's lr_t (bias correction applied on the host), else the learning rate.  hp as aae_optimizer.hp.
+int launch_opt_multi(OptBatch& b, int kind, float lr, const float hp[4], cudaStream_t stream);
 // Sub-pixel form of "nearest-neighbour x2 upsample, then conv 5x5 stride 1 SAME" (auto_pose/ae/decoder.py:54-62): the four
 // output parities (py, px) are four 3x3 convolutions of the LOW-resolution input whose taps are sums of the original
 // taps that land on the same source pixel -- 9/25 of the multiply-adds.  W [5,5,ci,co] -> Wm [3,3,ci,(py,px,co)].

@@ -1,7 +1,7 @@
 // Small HBM-bound kernels around the contractions: layout transposes for the backward pass, ReLU /
 // sigmoid derivative masks, 2x2 sum-pooling (backward of the decoder's nearest-neighbour x2 resize,
-// auto_pose/ae/decoder.py:54,66), bias gradients, the TF-Adam update
-// (auto_pose/ae/ae_factory.py:86-88) and the tiny-Cout output convolution of the decoder
+// auto_pose/ae/decoder.py:54,66), bias gradients, the tf.train optimizer updates
+// (auto_pose/ae/ae_factory.py:79-95) and the tiny-Cout output convolution of the decoder
 // (auto_pose/ae/decoder.py:77-83).
 #include <algorithm>
 
@@ -115,56 +115,85 @@ __global__ void sigmoid_grad_kernel(float* __restrict__ dx, const float* __restr
   }
 }
 
-// tf.train.AdamOptimizer (ApplyAdam): m = b1 m + (1-b1) g; v = b2 v + (1-b2) g^2; p -= lr_t m / (sqrt(v) + eps),
-// lr_t = lr sqrt(1-b2^t)/(1-b1^t) computed on the host.  7 fp32 streams per parameter.
-__global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                            long long n, float lr_t, float b1, float b2, float eps) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float gi = g[i];
-    const float mi = b1 * m[i] + (1.f - b1) * gi;
-    const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-    m[i] = mi;
-    v[i] = vi;
-    p[i] = p[i] - lr_t * mi / (sqrtf(vi) + eps);
+// rsqrt correctly rounded (rsqrtf is not)
+__device__ __forceinline__ float rsqrt_rn(float x) { return __fdiv_rn(1.f, __fsqrt_rn(x)); }
+
+// One parameter of one tf.train optimizer, in the order of TF's training_ops functors (DESIGN.md section 3).  s0 / s1: the rule's
+// slots in TF's creation order.  Every rule is written with _rn intrinsics so that the compiler contracts nothing on its own and
+// a float32 restatement in the same order replays it bit for bit.  Adam keeps the two FMAs its update has always had.
+// l1 = l2 = 0, RMSProp's centered = False and Ftrl's learning_rate_power = -0.5 are the only values a cfg can reach.
+template <int K>
+__device__ __forceinline__ void opt_update(float& p, float g, float& s0, float& s1, float lr, float h0, float h1, float h2) {
+  if constexpr (K == AAE_OPT_ADAM) {          // m = b1 m + (1-b1) g; v = b2 v + (1-b2) g^2; p -= lr_t m / (sqrt(v) + eps)
+    s0 = __fmaf_rn(g, __fsub_rn(1.f, h0), __fmul_rn(h0, s0));
+    s1 = __fmaf_rn(g, __fmul_rn(__fsub_rn(1.f, h1), g), __fmul_rn(h1, s1));
+    p = __fsub_rn(p, __fdiv_rn(__fmul_rn(lr, s0), __fadd_rn(__fsqrt_rn(s1), h2)));
+  } else if constexpr (K == AAE_OPT_GRADIENT_DESCENT) {   // var -= grad * lr
+    p = __fsub_rn(p, __fmul_rn(g, lr));
+  } else if constexpr (K == AAE_OPT_ADAGRAD) {            // accum += grad^2; var -= (grad * lr) * rsqrt(accum)
+    s0 = __fadd_rn(s0, __fmul_rn(g, g));
+    p = __fsub_rn(p, __fmul_rn(__fmul_rn(g, lr), rsqrt_rn(s0)));
+  } else if constexpr (K == AAE_OPT_PROXIMAL_ADAGRAD) {   // accum += grad^2; lr_t = lr rsqrt(accum); var = (var - grad lr_t) / 1
+    s0 = __fadd_rn(s0, __fmul_rn(g, g));
+    p = __fsub_rn(p, __fmul_rn(g, __fmul_rn(lr, rsqrt_rn(s0))));
+  } else if constexpr (K == AAE_OPT_ADADELTA) {           // h0 = rho, h1 = epsilon
+    const float c = __fsub_rn(1.f, h0);
+    s0 = __fadd_rn(__fmul_rn(s0, h0), __fmul_rn(__fmul_rn(g, g), c));
+    const float upd = __fmul_rn(__fmul_rn(__fsqrt_rn(__fadd_rn(s1, h1)), rsqrt_rn(__fadd_rn(s0, h1))), g);
+    p = __fsub_rn(p, __fmul_rn(upd, lr));
+    s1 = __fadd_rn(__fmul_rn(s1, h0), __fmul_rn(__fmul_rn(upd, upd), c));
+  } else if constexpr (K == AAE_OPT_RMSPROP) {            // h0 = decay, h1 = momentum, h2 = epsilon
+    s0 = __fadd_rn(s0, __fmul_rn(__fsub_rn(__fmul_rn(g, g), s0), __fsub_rn(1.f, h0)));
+    s1 = __fadd_rn(__fmul_rn(s1, h1), __fdiv_rn(__fmul_rn(g, lr), __fsqrt_rn(__fadd_rn(s0, h2))));
+    p = __fsub_rn(p, s1);
+  } else {                                                // Ftrl: s0 = accum, s1 = linear
+    const float na = __fadd_rn(s0, __fmul_rn(g, g));
+    const float sq = __fsqrt_rn(na);
+    s1 = __fadd_rn(s1, __fsub_rn(g, __fmul_rn(__fdiv_rn(__fsub_rn(sq, __fsqrt_rn(s0)), lr), p)));
+    p = fabsf(s1) > 0.f ? __fdiv_rn(-s1, __fdiv_rn(sq, lr)) : 0.f;   // (l1 sign(linear) - linear) / (sqrt(new)/lr + 2 l2)
+    s0 = na;
   }
 }
 
-// The same update over a list of tensors in ONE launch (29.7 M parameters in 20 tensors, half of them tiny biases):
-// block = one 4096-element chunk of one tensor.
-__global__ void __launch_bounds__(256) adam_multi_kernel(const AdamBatch b, float lr_t, float b1, float b2, float eps) {
+// The update over a list of tensors in ONE launch (29.7 M parameters in 20 tensors, half of them tiny biases):
+// block = one 4096-element chunk of one tensor.  Streams per parameter: 3 + 2 x (slots).
+template <int K>
+__global__ void __launch_bounds__(256) opt_multi_kernel(const OptBatch b, float lr, float h0, float h1, float h2) {
+  constexpr int kSlots = opt_slot_count(K);
   int t = 0;
   while (t + 1 < b.count && (int)blockIdx.x >= b.chunk_begin[t + 1]) ++t;
   const long long off = (long long)((int)blockIdx.x - b.chunk_begin[t]) * 4096;
   const long long n = b.n[t];
   float* __restrict__ p = b.p[t] + off;
   const float* __restrict__ g = b.g[t] + off;
-  float* __restrict__ m = b.m[t] + off;
-  float* __restrict__ v = b.v[t] + off;
+  float* __restrict__ s0 = kSlots >= 1 ? b.s0[t] + off : nullptr;
+  float* __restrict__ s1 = kSlots >= 2 ? b.s1[t] + off : nullptr;
   const int len = (int)min((long long)4096, n - off);
   if (len == 4096) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int i = (j * 256 + threadIdx.x) * 4;
       const float4 gi = *reinterpret_cast<const float4*>(g + i);
-      float4 mi = *reinterpret_cast<const float4*>(m + i), vi = *reinterpret_cast<const float4*>(v + i), pi = *reinterpret_cast<const float4*>(p + i);
-      mi.x = b1 * mi.x + (1.f - b1) * gi.x; mi.y = b1 * mi.y + (1.f - b1) * gi.y; mi.z = b1 * mi.z + (1.f - b1) * gi.z; mi.w = b1 * mi.w + (1.f - b1) * gi.w;
-      vi.x = b2 * vi.x + (1.f - b2) * gi.x * gi.x; vi.y = b2 * vi.y + (1.f - b2) * gi.y * gi.y;
-      vi.z = b2 * vi.z + (1.f - b2) * gi.z * gi.z; vi.w = b2 * vi.w + (1.f - b2) * gi.w * gi.w;
-      pi.x = pi.x - lr_t * mi.x / (sqrtf(vi.x) + eps); pi.y = pi.y - lr_t * mi.y / (sqrtf(vi.y) + eps);
-      pi.z = pi.z - lr_t * mi.z / (sqrtf(vi.z) + eps); pi.w = pi.w - lr_t * mi.w / (sqrtf(vi.w) + eps);
-      *reinterpret_cast<float4*>(m + i) = mi;
-      *reinterpret_cast<float4*>(v + i) = vi;
+      float4 ai = make_float4(0.f, 0.f, 0.f, 0.f), bi = ai;
+      if constexpr (kSlots >= 1) ai = *reinterpret_cast<const float4*>(s0 + i);
+      if constexpr (kSlots >= 2) bi = *reinterpret_cast<const float4*>(s1 + i);
+      float4 pi = *reinterpret_cast<const float4*>(p + i);
+      opt_update<K>(pi.x, gi.x, ai.x, bi.x, lr, h0, h1, h2);
+      opt_update<K>(pi.y, gi.y, ai.y, bi.y, lr, h0, h1, h2);
+      opt_update<K>(pi.z, gi.z, ai.z, bi.z, lr, h0, h1, h2);
+      opt_update<K>(pi.w, gi.w, ai.w, bi.w, lr, h0, h1, h2);
+      if constexpr (kSlots >= 1) *reinterpret_cast<float4*>(s0 + i) = ai;
+      if constexpr (kSlots >= 2) *reinterpret_cast<float4*>(s1 + i) = bi;
       *reinterpret_cast<float4*>(p + i) = pi;
     }
     return;
   }
   for (int i = threadIdx.x; i < len; i += 256) {
-    const float gi = g[i];
-    const float mi = b1 * m[i] + (1.f - b1) * gi;
-    const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-    m[i] = mi;
-    v[i] = vi;
-    p[i] = p[i] - lr_t * mi / (sqrtf(vi) + eps);
+    float a = kSlots >= 1 ? s0[i] : 0.f, c = kSlots >= 2 ? s1[i] : 0.f, pi = p[i];
+    opt_update<K>(pi, g[i], a, c, lr, h0, h1, h2);
+    if constexpr (kSlots >= 1) s0[i] = a;
+    if constexpr (kSlots >= 2) s1[i] = c;
+    p[i] = pi;
   }
 }
 
@@ -461,19 +490,22 @@ int launch_sigmoid_grad(float* dx, const float* x, int64_t n, cudaStream_t strea
   return AAE_OK;
 }
 
-int launch_adam(float* p, const float* g, float* m, float* v, int64_t n, float lr_t, float b1, float b2, float eps,
-                cudaStream_t stream) {
-  adam_kernel<<<grid_for(n, 256), 256, 0, stream>>>(p, g, m, v, n, lr_t, b1, b2, eps);
-  AAE_LAUNCH_OK();
-  return AAE_OK;
-}
-
-int launch_adam_multi(AdamBatch& b, float lr_t, float b1, float b2, float eps, cudaStream_t stream) {
-  AAE_REQUIRE(b.count >= 1 && b.count <= AdamBatch::kMax, "adam_multi: %d tensors (max %d)", b.count, AdamBatch::kMax);
+int launch_opt_multi(OptBatch& b, int kind, float lr, const float hp[4], cudaStream_t stream) {
+  AAE_REQUIRE(b.count >= 1 && b.count <= OptBatch::kMax, "opt_multi: %d tensors (max %d)", b.count, OptBatch::kMax);
   int chunks = 0;
   for (int t = 0; t < b.count; ++t) { b.chunk_begin[t] = chunks; chunks += (int)ceil_div(b.n[t], 4096); }
   b.chunk_begin[b.count] = chunks;
-  adam_multi_kernel<<<(unsigned)chunks, 256, 0, stream>>>(b, lr_t, b1, b2, eps);
+  const unsigned grid = (unsigned)chunks;
+  switch (kind) {
+    case AAE_OPT_ADAM: opt_multi_kernel<AAE_OPT_ADAM><<<grid, 256, 0, stream>>>(b, lr, hp[0], hp[1], hp[2]); break;
+    case AAE_OPT_GRADIENT_DESCENT: opt_multi_kernel<AAE_OPT_GRADIENT_DESCENT><<<grid, 256, 0, stream>>>(b, lr, hp[0], hp[1], hp[2]); break;
+    case AAE_OPT_ADAGRAD: opt_multi_kernel<AAE_OPT_ADAGRAD><<<grid, 256, 0, stream>>>(b, lr, hp[0], hp[1], hp[2]); break;
+    case AAE_OPT_PROXIMAL_ADAGRAD: opt_multi_kernel<AAE_OPT_PROXIMAL_ADAGRAD><<<grid, 256, 0, stream>>>(b, lr, hp[0], hp[1], hp[2]); break;
+    case AAE_OPT_ADADELTA: opt_multi_kernel<AAE_OPT_ADADELTA><<<grid, 256, 0, stream>>>(b, lr, hp[0], hp[1], hp[2]); break;
+    case AAE_OPT_RMSPROP: opt_multi_kernel<AAE_OPT_RMSPROP><<<grid, 256, 0, stream>>>(b, lr, hp[0], hp[1], hp[2]); break;
+    case AAE_OPT_FTRL: opt_multi_kernel<AAE_OPT_FTRL><<<grid, 256, 0, stream>>>(b, lr, hp[0], hp[1], hp[2]); break;
+    default: AAE_REQUIRE(false, "opt_multi: aae_optimizer_kind %d", kind);
+  }
   AAE_LAUNCH_OK();
   return AAE_OK;
 }

@@ -229,13 +229,13 @@ AAE_API int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, int
                                   uint8_t* mask_out_dev, int32_t* fallbacks_dev, void* stream);
 
 /* ---------------------------------------------------------------- Training step ------------
- * Replaces sess.run(train_op): encoder fwd, decoder fwd, bootstrapped L2, backward, TF-Adam
+ * Replaces sess.run(train_op): encoder fwd, decoder fwd, bootstrapped L2, backward, optimizer update
  * (auto_pose/ae/ae_train.py:128, auto_pose/ae/ae_factory.py:79-95).
  * The arithmetic follows the handles: encoder and decoder must have been created with the same
  * aae_precision.  AAE_PREC_FP32_SIMT runs every contraction as fp32 FMA chains; AAE_PREC_TC_SPLIT
  * runs the forward pass, the data gradients and the weight gradients of all convs with Cin >= 128
  * as wgmma GEMMs (split-fp16 x3, gradients re-scaled per tensor and per step by a power of two),
- * the two dense layers and conv1's weight gradient as fp32 kernels; parameters, Adam state and
+ * the two dense layers and conv1's weight gradient as fp32 kernels; parameters, optimizer slots and
  * the gradients returned by aae_trainer_get_grads are fp32 in the reference layouts either way. */
 AAE_API int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate,
                                float beta1, float beta2, float epsilon, aae_trainer** out);
@@ -244,7 +244,7 @@ AAE_API int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap
  *   AAE_PREC_TC_FP16 with two AAE_PREC_TC_SPLIT handles: the single-pass trainer.  Its forward, dgrad and wgrad
  *     GEMMs round every operand once to fp16 and issue one hi*hi product per K step (the TF32 rounding class
  *     of AAE_PREC_TC_FP16), on private hi-only plans packed from the handles' fp32 masters.  Gradients keep the
- *     per-tensor, per-step power-of-two scale, the two dense layers' backward and Adam stay fp32, and the
+ *     per-tensor, per-step power-of-two scale, the two dense layers' backward and the update stay fp32, and the
  *     handles keep AAE_PREC_TC_SPLIT: their weights are the trainer's masters and inference on them runs split.
  *     Error contract (DESIGN.md section 3): each GEMM y = a*w adds at most (2^-9 + 2^-11) sum|a*w| (products,
  *     then hi-only storage), i.e. (2^-9 + 2^-11) k of y in the L2 norm with k = ||(|a| |w|)|| / ||y||.  In the
@@ -255,6 +255,37 @@ AAE_API int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap
  *     aae_last_error_string(); a value outside {0, 1, 2} returns AAE_ERR_INVALID_ARG. */
 AAE_API int aae_trainer_create_prec(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate,
                                     float beta1, float beta2, float epsilon, int gemm_precision, aae_trainer** out);
+/* The update rule of the training step: the tf.train optimizers a cfg's OPTIMIZER can build (auto_pose/ae/ae_factory.py:79-95;
+ * formulas, slot names and initial values in DESIGN.md section 3).  ProximalGradientDescent with l1 = l2 = 0 is
+ * AAE_OPT_GRADIENT_DESCENT bit for bit. */
+typedef enum {
+  AAE_OPT_ADAM = 0,
+  AAE_OPT_GRADIENT_DESCENT = 1,
+  AAE_OPT_ADAGRAD = 2,
+  AAE_OPT_PROXIMAL_ADAGRAD = 3,
+  AAE_OPT_ADADELTA = 4,
+  AAE_OPT_RMSPROP = 5,
+  AAE_OPT_FTRL = 6
+} aae_optimizer_kind;
+
+/* hp per kind (unused entries are ignored):
+ *   AAE_OPT_ADAM                                        beta1, beta2, epsilon
+ *   AAE_OPT_GRADIENT_DESCENT                            -
+ *   AAE_OPT_ADAGRAD, AAE_OPT_PROXIMAL_ADAGRAD, AAE_OPT_FTRL   initial accumulator value (> 0)
+ *   AAE_OPT_ADADELTA                                    rho, epsilon
+ *   AAE_OPT_RMSPROP                                     decay, momentum, epsilon
+ * l1 = l2 = 0, centered = False and Ftrl's learning_rate_power = -0.5 are fixed (the only values a cfg reaches). */
+typedef struct {
+  int32_t kind;                        /* aae_optimizer_kind */
+  float learning_rate;
+  float hp[4];
+} aae_optimizer;
+
+/* aae_trainer_create_prec with any update rule; aae_trainer_create(_prec) are this call with AAE_OPT_ADAM.  The trainer
+ * allocates only the rule's slots (none for gradient descent) and sets them to the rule's initial values.  A kind outside
+ * aae_optimizer_kind or an initial accumulator <= 0: AAE_ERR_INVALID_ARG.  Precision contract as aae_trainer_create_prec. */
+AAE_API int aae_trainer_create_opt(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, const aae_optimizer* opt,
+                                   int gemm_precision, aae_trainer** out);
 AAE_API int aae_trainer_destroy(aae_trainer* h);
 /* x (augmented input) and y (reconstruction target) NHWC float32 [B,H,W,C]; loss_out_dev: 1 float. */
 AAE_API int aae_train_step(aae_trainer* h, const float* x_dev, const float* y_dev, int batch, float* loss_out_dev, void* stream);
@@ -264,10 +295,11 @@ AAE_API int aae_trainer_forward_backward(aae_trainer* h, const float* x_dev, con
 AAE_API int aae_trainer_get_grads(aae_trainer* h, int which, int layer, float* kernel_grad_any, float* bias_grad_any, void* stream);
 AAE_API int64_t aae_trainer_global_step(const aae_trainer* h);
 /* Optimizer state, so that a training run can be resumed from a checkpoint the way tf.train.Saver does (the reference's
- * Saver stores every variable's Adam slots and the beta powers: auto_pose/ae/ae_train.py:82,111-115).  which / layer as in
- * aae_trainer_get_grads; *_m = first moment (TF slot name "<var>/Adam"), *_v = second moment ("<var>/Adam_1"), same shapes
- * as the variable; NULL pointers are skipped.  aae_trainer_set_global_step(h, n) makes the next update the (n+1)-th
- * (bias correction with beta^(n+1), TF's beta1_power / beta2_power after n steps). */
+ * Saver stores every variable's slots and Adam's beta powers: auto_pose/ae/ae_train.py:82,111-115).  which / layer as in
+ * aae_trainer_get_grads; *_m = slot 0 of the trainer's rule, *_v = slot 1, same shapes as the variable (Adam: first moment
+ * "<var>/Adam" and second moment "<var>/Adam_1"; other rules: DESIGN.md section 3).  NULL pointers are skipped; a non-NULL
+ * pointer for a slot the rule does not have returns AAE_ERR_INVALID_ARG.  aae_trainer_set_global_step(h, n) makes the next
+ * update the (n+1)-th (Adam: bias correction with beta^(n+1), TF's beta1_power / beta2_power after n steps). */
 AAE_API int aae_trainer_get_state(aae_trainer* h, int which, int layer, float* kernel_m_any, float* kernel_v_any, float* bias_m_any,
                                   float* bias_v_any, void* stream);
 AAE_API int aae_trainer_set_state(aae_trainer* h, int which, int layer, const float* kernel_m_any, const float* kernel_v_any,
@@ -288,7 +320,7 @@ AAE_API int aae_trainer_set_latent_terms(aae_trainer* h, float variational, floa
 AAE_API int aae_trainer_set_latent_noise(aae_trainer* h, float eps);
 /* Per-phase device time of the last training step (cudaEvents on the launching stream; tensor-core trainer only):
  * phase_ms_out[0..6] = operand packs, forward + loss, wgrad GEMMs, dgrad GEMMs, glue (masks / bias sums / re-splits),
- * fp32 backward of the dense layers and of conv1, Adam.  Same enable/read contract as aae_encoder_profile; returns the
+ * fp32 backward of the dense layers and of conv1, optimizer update.  Same enable/read contract as aae_encoder_profile; returns the
  * number of values written (0 when nothing was recorded).  Measurement aid for bench.py --workload train. */
 AAE_API int aae_trainer_profile(aae_trainer* h, int enable, float* phase_ms_out, int capacity);
 
