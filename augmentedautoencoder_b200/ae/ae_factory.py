@@ -189,6 +189,15 @@ class TrainOp(Tensor):
             self._trainers[dev] = h
         return self._trainers[dev]
 
+    def close(self):
+        """Frees this op's device trainers: their gradient, scratch and optimizer-slot buffers.  Call it while the encoder and decoder
+        are still open (a trainer is destroyed through their handles).  A later step creates a new trainer with fresh optimizer
+        state."""
+        for dev, h in self._trainers.items():
+            with torch.cuda.device(dev):
+                _lib.lib().aae_trainer_destroy(h)
+        self._trainers = {}
+
     def _io(self, ctx):
         ae = self._ae
         x = S.to_device_input(ctx.get(ae._encoder.x), ctx.session.device)

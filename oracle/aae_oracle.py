@@ -186,13 +186,20 @@ def resize_nearest_2x(x_nhwc: torch.Tensor, out_hw: Tuple[int, int]) -> torch.Te
     (auto_pose/ae/decoder.py:54,66)."""
     ih, iw = x_nhwc.shape[1], x_nhwc.shape[2]
     oh, ow = out_hw
-    ri = torch.clamp((torch.arange(oh, dtype=torch.float64) * (ih / oh)).floor().long(), max=ih - 1)
-    ci = torch.clamp((torch.arange(ow, dtype=torch.float64) * (iw / ow)).floor().long(), max=iw - 1)
+    dev = x_nhwc.device
+    ri = torch.clamp((torch.arange(oh, dtype=torch.float64, device=dev) * (ih / oh)).floor().long(), max=ih - 1)
+    ci = torch.clamp((torch.arange(ow, dtype=torch.float64, device=dev) * (iw / ow)).floor().long(), max=iw - 1)
     return x_nhwc[:, ri][:, :, ci]
 
 
-def _t(a: np.ndarray, dtype: torch.dtype) -> torch.Tensor:
-    return torch.from_numpy(np.ascontiguousarray(a)).to(dtype)
+def _t(a: np.ndarray, dtype: torch.dtype, device: str = "cpu") -> torch.Tensor:
+    return torch.from_numpy(np.ascontiguousarray(a)).to(device, dtype)
+
+
+def _check_device(dtype: torch.dtype, device: str) -> None:
+    """Only float64 runs on the GPU: torch's float32 convolutions and matmuls there may use TF32, which is no fp32 reference."""
+    if torch.device(device).type != "cpu" and dtype != torch.float64:
+        raise ValueError("the oracle runs %s on the CPU only; on %s it evaluates float64" % (dtype, device))
 
 
 def encoder_layers(x: np.ndarray, params: Dict[str, np.ndarray], strides=STRIDES,
@@ -295,44 +302,50 @@ def bootstrapped_l2(x: torch.Tensor, target: torch.Tensor, bootstrap_ratio: int 
 
 def ae_forward_loss(x: np.ndarray, target: np.ndarray, enc: Dict[str, np.ndarray], dec: Dict[str, np.ndarray],
                     dtype: torch.dtype = torch.float32, bootstrap_ratio: int = BOOTSTRAP_RATIO,
-                    with_grads: bool = False):
+                    with_grads: bool = False, device: str = "cpu"):
     """encode -> decode -> bootstrapped L2 (auto_pose/ae/ae.py:42-53 with NORM_REGULARIZE=0, VARIATIONAL=0).
-    Returns (loss, reconstruction, grads-dict or None)."""
-    tp = {k: _t(v, dtype).requires_grad_(with_grads) for k, v in {**enc, **dec}.items()}
+    Returns (loss, reconstruction, grads-dict or None) as numpy.  device="cuda" evaluates the same graph on the GPU (float64
+    only), which makes the reference affordable at training batch sizes."""
+    _check_device(dtype, device)
+    tp = {k: _t(v, dtype, device).requires_grad_(with_grads) for k, v in {**enc, **dec}.items()}
     strides = STRIDES[:sum(1 for k in enc if k.startswith("conv2d") and k.endswith("kernel"))]
     hw = x.shape[1]
     with torch.set_grad_enabled(with_grads):
-        h = _t(x, dtype)
+        h = _t(x, dtype, device)
         for i, s in enumerate(strides):
             name = "conv2d" if i == 0 else f"conv2d_{i}"
             h = conv2d_same(h, tp[f"{name}/kernel"], tp[f"{name}/bias"], s, "relu")
         z = h.reshape(h.shape[0], -1) @ tp["dense/kernel"] + tp["dense/bias"]
         rec = decoder_layers(z, tp, out_hw=hw, strides=strides, n_encoder_convs=len(strides))[-1]
-        loss = bootstrapped_l2(rec, _t(target, dtype), bootstrap_ratio)
+        loss = bootstrapped_l2(rec, _t(target, dtype, device), bootstrap_ratio)
         grads = None
         if with_grads:
             loss.backward()
-            grads = {k: v.grad.numpy() for k, v in tp.items()}
-    return float(loss.item()), rec.detach().numpy(), grads
+            grads = {k: v.grad.cpu().numpy() for k, v in tp.items()}
+    return float(loss.item()), rec.detach().cpu().numpy(), grads
 
 
-def relu_margin(x: np.ndarray, enc: Dict[str, np.ndarray], dec: Dict[str, np.ndarray]) -> float:
+def relu_margin(x: np.ndarray, enc: Dict[str, np.ndarray], dec: Dict[str, np.ndarray], device: str = "cpu",
+                latent: Optional[np.ndarray] = None) -> float:
     """Smallest |pre-activation| over every ReLU unit of encoder + decoder, in float64.  A unit closer to zero than fp32
     rounding can land on either side of the ReLU in any fp32 implementation (TF included), which changes its gradient
-    path discretely; gradient parity tests pick inputs whose margin is comfortably above that."""
+    path discretely; gradient parity tests pick inputs whose margin is comfortably above that.  ``latent``: the decoder's
+    input when it is not the encoder's z (the sampled z of the variational AE)."""
     dt = torch.float64
-    tp = {k: _t(v, dt) for k, v in {**enc, **dec}.items()}
+    tp = {k: _t(v, dt, device) for k, v in {**enc, **dec}.items()}
     n_enc = sum(1 for k in enc if k.startswith("conv2d") and k.endswith("kernel"))
     strides = STRIDES[:n_enc]
     m = float("inf")
     with torch.no_grad():
-        h = _t(x, dt)
+        h = _t(x, dt, device)
         for i, s_ in enumerate(strides):
             name = "conv2d" if i == 0 else f"conv2d_{i}"
             pre = conv2d_same(h, tp[f"{name}/kernel"], tp[f"{name}/bias"], s_, None)
             m = min(m, float(pre.abs().min()))
             h = torch.relu(pre)
         z = h.reshape(h.shape[0], -1) @ tp["dense/kernel"] + tp["dense/bias"]
+        if latent is not None:
+            z = _t(latent, dt, device)
         pre = z @ tp["dense_1/kernel"] + tp["dense_1/bias"]
         m = min(m, float(pre.abs().min()))
         st = list(reversed(strides))

@@ -9,7 +9,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-from oracle.aae_oracle import BOOTSTRAP_RATIO, STRIDES, _t, bootstrapped_l2, conv2d_same, decoder_layers
+from oracle.aae_oracle import BOOTSTRAP_RATIO, STRIDES, _check_device, _t, bootstrapped_l2, conv2d_same, decoder_layers
 
 
 def q_sigma(flat: torch.Tensor, kernel: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
@@ -38,22 +38,24 @@ def norm_reg_loss(z: torch.Tensor) -> torch.Tensor:
 def vae_forward_loss(x: np.ndarray, target: np.ndarray, enc: Dict[str, np.ndarray], dec: Dict[str, np.ndarray],
                      head: Optional[Tuple[np.ndarray, np.ndarray]] = None, variational: float = 0.0,
                      norm_regularize: float = 0.0, eps: float = 0.0, dtype: torch.dtype = torch.float32,
-                     bootstrap_ratio: int = BOOTSTRAP_RATIO, with_grads: bool = False):
+                     bootstrap_ratio: int = BOOTSTRAP_RATIO, with_grads: bool = False, device: str = "cpu"):
     """AE.loss with the latent terms (ae.py:43-53): reconstr_loss, + reg_loss * norm_regularize if that is > 0, + kl_div_loss *
     variational if that is non-zero; the decoder reads sampled_z when variational is set (ae_factory.py:58).
     ``enc`` / ``dec`` as for aae_oracle.ae_forward_loss (decoder dense under "dense_1"); ``head`` = (kernel [flat, latent],
     bias [latent]) of the sigma head, required when variational.
     Returns (loss, terms, grads or None).  terms: z, q_sigma, sampled_z (numpy), kl, reg (floats).  Gradients are keyed by the
-    variational graph's TF names when variational (head "dense_1", decoder dense "dense_2"), else by the plain names."""
+    variational graph's TF names when variational (head "dense_1", decoder dense "dense_2"), else by the plain names.
+    device="cuda" evaluates the graph on the GPU (float64 only), as aae_oracle.ae_forward_loss."""
     if variational and head is None:
         raise ValueError("variational needs the sigma head")
-    tp = {k: _t(v, dtype).requires_grad_(with_grads) for k, v in {**enc, **dec}.items()}
+    _check_device(dtype, device)
+    tp = {k: _t(v, dtype, device).requires_grad_(with_grads) for k, v in {**enc, **dec}.items()}
     hk = hb = None
     if head is not None:
-        hk, hb = (_t(a, dtype).requires_grad_(with_grads) for a in head)
+        hk, hb = (_t(a, dtype, device).requires_grad_(with_grads) for a in head)
     strides = STRIDES[:sum(1 for k in enc if k.startswith("conv2d") and k.endswith("kernel"))]
     with torch.set_grad_enabled(with_grads):
-        h = _t(x, dtype)
+        h = _t(x, dtype, device)
         for i, s in enumerate(strides):
             name = "conv2d" if i == 0 else f"conv2d_{i}"
             h = conv2d_same(h, tp[f"{name}/kernel"], tp[f"{name}/bias"], s, "relu")
@@ -62,7 +64,7 @@ def vae_forward_loss(x: np.ndarray, target: np.ndarray, enc: Dict[str, np.ndarra
         sigma = q_sigma(flat, hk, hb) if head is not None else None
         zin = sampled_z(z, sigma, eps) if variational else z
         rec = decoder_layers(zin, tp, out_hw=x.shape[1], strides=strides, n_encoder_convs=len(strides))[-1]
-        loss = bootstrapped_l2(rec, _t(target, dtype), bootstrap_ratio)
+        loss = bootstrapped_l2(rec, _t(target, dtype, device), bootstrap_ratio)
         reg = norm_reg_loss(z)
         kl = kl_div_loss(z, sigma) if sigma is not None else None
         if norm_regularize > 0:
@@ -72,10 +74,10 @@ def vae_forward_loss(x: np.ndarray, target: np.ndarray, enc: Dict[str, np.ndarra
         grads = None
         if with_grads:
             loss.backward()
-            grads = {k: v.grad.numpy() for k, v in tp.items()}
+            grads = {k: v.grad.cpu().numpy() for k, v in tp.items()}
             if variational:
                 grads["dense_2/kernel"], grads["dense_2/bias"] = grads.pop("dense_1/kernel"), grads.pop("dense_1/bias")
-                grads["dense_1/kernel"], grads["dense_1/bias"] = hk.grad.numpy(), hb.grad.numpy()
-    terms = {"z": z.detach().numpy(), "q_sigma": None if sigma is None else sigma.detach().numpy(),
-             "sampled_z": zin.detach().numpy(), "kl": None if kl is None else float(kl.detach()), "reg": float(reg.detach())}
+                grads["dense_1/kernel"], grads["dense_1/bias"] = hk.grad.cpu().numpy(), hb.grad.cpu().numpy()
+    terms = {"z": z.detach().cpu().numpy(), "q_sigma": None if sigma is None else sigma.detach().cpu().numpy(),
+             "sampled_z": zin.detach().cpu().numpy(), "kl": None if kl is None else float(kl.detach()), "reg": float(reg.detach())}
     return float(loss.item()), terms, grads
