@@ -72,6 +72,9 @@ _SIGS = {
     "aae_decoder_get_weights": (_I, [_P, _I, _P, _P, _P]),
     "aae_decoder_forward": (_I, [_P, _P, _I, _P, _P]),
     "aae_decoder_range_status": (_I, [_P, _P]),
+    "aae_decoder_enable_mask_head": (_I, [_P]),
+    "aae_decoder_forward_mask": (_I, [_P, _P, _I, _P, _P, _P]),
+    "aae_mask_loss": (_I, [_P, _P, _I, _I, _I, _P, _P, _P]),
     "aae_bootstrap_l2_loss": (_I, [_P, _P, _I, _I, _I, _P, _P, _P]),
     "aae_trainer_create": (_I, [_P, _P, _I, _F, _F, _F, _F, C.POINTER(_P)]),
     "aae_trainer_create_prec": (_I, [_P, _P, _I, _F, _F, _F, _F, _I, C.POINTER(_P)]),

@@ -220,6 +220,10 @@ struct aae_decoder {
   SimtDecoder* simt = nullptr;  // fp32 CUDA-core workspace (AAE_PREC_FP32_SIMT)
   TcDecoder* tc = nullptr;      // tensor-core execution plan (AAE_PREC_TC_SPLIT, forward only)
   uint64_t w_version = 1, tc_version = 1;   // see aae_encoder
+  // mask head of AUXILIARY_MASK (aae_decoder_enable_mask_head; empty until then): kernel [k,k,Cin,1] and bias [1] of a conv over
+  // the output layer's input.  The kernels run it joined with the output conv along Cout (DESIGN.md section 3).
+  DevBuf mask_w, mask_b;
+  int trainers = 0;             // live trainers over this handle: the head cannot be added under them
 };
 
 struct aae_codebook {
@@ -262,6 +266,10 @@ struct aae_trainer {
   float w_v = 0.f, w_n = 0.f, noise = 0.f;
   bool head = false;
   DevBuf pre, sz, dpre, dcat, lat_sums;
+  // mask head (the decoder had it at creation; dec_k / dec_b then hold it at num_layers + 1): its output and gradient [B, H, W],
+  // the loss's per-sample sums, and on the fp32 trainer the output conv and head joined along Cout for the data gradient
+  bool mask = false;
+  DevBuf rec_mask, dmask, mask_sums, wcat, dycat;
   TcTrainPlan* tc = nullptr;  // tensor-core backward plan (encoder and decoder created with AAE_PREC_TC_SPLIT)
   uint64_t packed_enc_version = 0, packed_dec_version = 0;   // master-weight versions the plan's dgrad operands were packed from
   // single-pass trainer (aae_trainer_create_prec with AAE_PREC_TC_FP16): private hi-only forward plans built from the handles'
@@ -785,7 +793,7 @@ extern "C" int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decode
     cudaMemset(R.w.p, 0, R.w.n * 4); cudaMemset(R.b.p, 0, R.b.n * 4);
     ih = R.out_h; ic = R.out_c;
   }
-  if (status == AAE_OK) status = cfg->precision == AAE_PREC_TC_SPLIT ? tc_decoder_create(device, cfg, &h->tc) : simt_decoder_create(h);
+  if (status == AAE_OK) status = cfg->precision == AAE_PREC_TC_SPLIT ? tc_decoder_create(device, cfg, false, &h->tc) : simt_decoder_create(h);
   if (status != AAE_OK) { aae_decoder_destroy(h); return status; }
   *out = h;
   return AAE_OK;
@@ -796,24 +804,39 @@ extern "C" int aae_decoder_destroy(aae_decoder* h) {
   DeviceGuard g(h->device);
   h->dense_w.release(); h->dense_b.release();
   for (auto& L : h->conv) { L.w.release(); L.b.release(); }
+  h->mask_w.release(); h->mask_b.release();
   delete h->simt;
   if (h->tc) tc_decoder_destroy(h->tc);
   delete h;
   return AAE_OK;
 }
 
+// layer 0: dense_1; 1..num_layers: the convs; num_layers + 1: the mask head (once enabled)
+static int decoder_layer_bufs(aae_decoder* h, int layer, DevBuf** w, DevBuf** b) {
+  const int nl = (int)h->conv.size();
+  AAE_REQUIRE(layer >= 0 && (layer <= nl || (layer == nl + 1 && h->mask_w.p)), "layer %d out of range%s", layer,
+              layer == nl + 1 ? " (no mask head: aae_decoder_enable_mask_head)" : "");
+  *w = layer == 0 ? &h->dense_w : layer <= nl ? &h->conv[layer - 1].w : &h->mask_w;
+  *b = layer == 0 ? &h->dense_b : layer <= nl ? &h->conv[layer - 1].b : &h->mask_b;
+  return AAE_OK;
+}
+
 extern "C" int aae_decoder_set_weights(aae_decoder* h, int layer, const float* kernel_any, const float* bias_any, void* stream) {
   AAE_REQUIRE(h != nullptr, "decoder handle is null");
-  AAE_REQUIRE(layer >= 0 && layer <= (int)h->conv.size(), "layer %d out of range", layer);
+  DevBuf *wp, *bp;
+  AAE_TRY(decoder_layer_bufs(h, layer, &wp, &bp));
   DeviceGuard g(h->device);
   cudaStream_t s = (cudaStream_t)stream;
-  DevBuf& w = layer == 0 ? h->dense_w : h->conv[layer - 1].w;
-  DevBuf& b = layer == 0 ? h->dense_b : h->conv[layer - 1].b;
+  DevBuf& w = *wp;
+  DevBuf& b = *bp;
   if (kernel_any) AAE_TRY(copy_any(w.p, kernel_any, w.n * sizeof(float), s));
   if (bias_any) AAE_TRY(copy_any(b.p, bias_any, b.n * sizeof(float), s));
   const bool tc_current = h->tc_version == h->w_version;
   h->w_version += 1;   // the fp32 path's merged sub-pixel weights are rebuilt by the next forward
-  if (h->tc) AAE_TRY(tc_decoder_pack_weights(h->tc, layer, kernel_any ? w.p : nullptr, bias_any ? b.p : nullptr, s));
+  const int nl = (int)h->conv.size();
+  // the head's kernel is packed as part of the output layer (its bias is read from the master)
+  if (h->tc && layer == nl + 1) AAE_TRY(tc_decoder_pack_weights(h->tc, nl, kernel_any ? h->conv.back().w.p : nullptr, nullptr, s));
+  else if (h->tc) AAE_TRY(tc_decoder_pack_weights(h->tc, layer, kernel_any ? w.p : nullptr, bias_any ? b.p : nullptr, s));
   if (tc_current) h->tc_version = h->w_version;   // see aae_encoder_set_weights
   AAE_CUDA_OK(cudaStreamSynchronize(s));
   if (h->tc) AAE_TRY(range_peek(tc_decoder_range_flag(h->tc), "decoder set_weights", 0, s));
@@ -828,11 +851,12 @@ extern "C" int aae_decoder_range_status(aae_decoder* h, void* stream) {
 
 extern "C" int aae_decoder_get_weights(aae_decoder* h, int layer, float* kernel_any, float* bias_any, void* stream) {
   AAE_REQUIRE(h != nullptr, "decoder handle is null");
-  AAE_REQUIRE(layer >= 0 && layer <= (int)h->conv.size(), "layer %d out of range", layer);
+  DevBuf *wp, *bp;
+  AAE_TRY(decoder_layer_bufs(h, layer, &wp, &bp));
   DeviceGuard g(h->device);
   cudaStream_t s = (cudaStream_t)stream;
-  DevBuf& w = layer == 0 ? h->dense_w : h->conv[layer - 1].w;
-  DevBuf& b = layer == 0 ? h->dense_b : h->conv[layer - 1].b;
+  DevBuf& w = *wp;
+  DevBuf& b = *bp;
   if (kernel_any) AAE_TRY(copy_any(kernel_any, w.p, w.n * sizeof(float), s));
   if (bias_any) AAE_TRY(copy_any(bias_any, b.p, b.n * sizeof(float), s));
   AAE_CUDA_OK(cudaStreamSynchronize(s));
@@ -847,7 +871,9 @@ static int decoder_sync_tc(aae_decoder* h, cudaStream_t s) {   // see encoder_sy
   return AAE_OK;
 }
 
-static int decoder_forward_impl(aae_decoder* h, const float* z, int B, float* x_out, cudaStream_t s) {
+// mask_out (optional, [B, H, W]): the mask head's output, a Cout = 1 conv over the output layer's input on the same kernel
+// as x's own tiny-Cout conv, so x is the same with and without the head
+static int decoder_forward_impl(aae_decoder* h, const float* z, int B, float* x_out, float* mask_out, cudaStream_t s) {
   SimtDecoder& S = *h->simt;
   const int dense_out = h->h0 * h->w0 * h->f0;
   IGemmParams p = dense_params(z, B, h->cfg.latent, h->dense_w.p, dense_out);
@@ -856,6 +882,11 @@ static int decoder_forward_impl(aae_decoder* h, const float* z, int B, float* x_
   const bool remerge = S.wm_version != h->w_version;
   for (size_t i = 0; i < h->conv.size(); ++i) {
     ConvLayer& L = h->conv[i];
+    if (mask_out && i + 1 == h->conv.size()) {
+      IGemmParams q = conv_params(L, src, 0, B);
+      q.Bm = h->mask_w.p; q.N = 1; q.C = mask_out; q.bias = h->mask_b.p; q.act = ACT_SIGMOID;
+      AAE_TRY(launch_conv_small_n(q, s));
+    }
     float* dst = (i + 1 == h->conv.size() && x_out) ? x_out : S.out[i].p;
     if (L.subpixel()) {
       // upsample x2 + conv5x5 == four 3x3 convs of the low-res input with merged taps: one GEMM, N = 4*Cout, 9/25 of the MACs
@@ -892,9 +923,67 @@ extern "C" int aae_decoder_forward(aae_decoder* h, const float* z_dev, int batch
   DeviceGuard g(h->device);
   if (h->tc) {
     AAE_TRY(decoder_sync_tc(h, (cudaStream_t)stream));
-    return tc_decoder_forward(h->tc, z_dev, batch, x_out_dev, (cudaStream_t)stream);
+    return tc_decoder_forward(h->tc, z_dev, batch, x_out_dev, nullptr, (cudaStream_t)stream);
   }
-  return decoder_forward_impl(h, z_dev, batch, x_out_dev, (cudaStream_t)stream);
+  return decoder_forward_impl(h, z_dev, batch, x_out_dev, nullptr, (cudaStream_t)stream);
+}
+
+// ---- mask head of AUXILIARY_MASK (auto_pose/ae/decoder.py:68-75) ----
+extern "C" int aae_decoder_enable_mask_head(aae_decoder* h) {
+  AAE_REQUIRE(h != nullptr, "decoder handle is null");
+  if (h->mask_w.p) return AAE_OK;
+  if (h->trainers > 0) {
+    set_error("enable_mask_head: %d trainer(s) exist over this decoder; enable the head before aae_trainer_create*", h->trainers);
+    return AAE_ERR_UNSUPPORTED;
+  }
+  DeviceGuard g(h->device);
+  const ConvLayer& L = h->conv.back();
+  int st = h->mask_w.alloc((size_t)L.ksize * L.ksize * L.in_c);
+  if (st == AAE_OK) st = h->mask_b.alloc(1);
+  if (st == AAE_OK) {
+    cudaError_t e = cudaMemset(h->mask_w.p, 0, h->mask_w.n * sizeof(float));
+    if (e == cudaSuccess) e = cudaMemset(h->mask_b.p, 0, sizeof(float));
+    if (e != cudaSuccess) { set_error("mask head: %s", cudaGetErrorString(e)); st = AAE_ERR_CUDA; }
+  }
+  if (st == AAE_OK && h->tc) {           // the output layer's plan gains the head's channel (N = 256)
+    TcDecoder* t = nullptr;
+    st = tc_decoder_create(h->device, &h->cfg, true, &t);
+    if (st == AAE_OK) {
+      tc_decoder_destroy(h->tc);
+      h->tc = t;
+      tc_decoder_set_mask_head(t, h->mask_w.p, h->mask_b.p);
+      h->tc_version = 0;                 // the new plan is packed from the masters before its first use
+    }
+  }
+  if (st != AAE_OK) { h->mask_w.release(); h->mask_b.release(); }
+  return st;
+}
+
+extern "C" int aae_decoder_forward_mask(aae_decoder* h, const float* z_dev, int batch, float* x_out_dev, float* mask_out_dev, void* stream) {
+  AAE_REQUIRE(h != nullptr && z_dev != nullptr && x_out_dev != nullptr && mask_out_dev != nullptr, "null argument");
+  AAE_REQUIRE(batch >= 1 && batch <= h->cfg.max_batch, "batch %d outside [1, max_batch=%d]", batch, h->cfg.max_batch);
+  if (!h->mask_w.p) {
+    set_error("forward_mask: the decoder has no mask head (aae_decoder_enable_mask_head)");
+    return AAE_ERR_UNSUPPORTED;
+  }
+  DeviceGuard g(h->device);
+  if (h->tc) {
+    AAE_TRY(decoder_sync_tc(h, (cudaStream_t)stream));
+    return tc_decoder_forward(h->tc, z_dev, batch, x_out_dev, mask_out_dev, (cudaStream_t)stream);
+  }
+  return decoder_forward_impl(h, z_dev, batch, x_out_dev, mask_out_dev, (cudaStream_t)stream);
+}
+
+extern "C" int aae_mask_loss(const float* mask_dev, const float* target_dev, int batch, int pixels_per_sample, int channels,
+                             float* loss_inout_dev, float* grad_out_dev, void* stream) {
+  AAE_REQUIRE(mask_dev && target_dev && loss_inout_dev, "null argument");
+  AAE_REQUIRE(batch >= 1 && pixels_per_sample >= 1 && channels >= 1, "bad sizes");
+  cudaStream_t s = (cudaStream_t)stream;
+  float* sums = nullptr;
+  AAE_CUDA_OK(cudaMallocAsync(&sums, (size_t)batch * sizeof(float), s));
+  int st = launch_mask_loss(mask_dev, target_dev, batch, pixels_per_sample, channels, sums, loss_inout_dev, grad_out_dev, s);
+  cudaFreeAsync(sums, s);
+  return st;
 }
 
 extern "C" int aae_bootstrap_l2_loss(const float* x_dev, const float* target_dev, int batch, int numel_per_sample,
@@ -953,6 +1042,7 @@ static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_rati
   AAE_REQUIRE(h != nullptr, "host allocation failed");
   h->enc = enc; h->dec = dec; h->bootstrap_ratio = bootstrap_ratio;
   h->opt = opt;
+  dec->trainers += 1;                            // aae_trainer_destroy takes it back, on the failure paths below too
   int st = AAE_OK;
   for (auto& L : enc->conv) { if (st == AAE_OK) st = make_pg(h->enc_k, L.w, opt); if (st == AAE_OK) st = make_pg(h->enc_b, L.b, opt); }
   if (st == AAE_OK) st = make_pg(h->enc_k, enc->dense_w, opt);
@@ -963,6 +1053,13 @@ static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_rati
   if (st == AAE_OK) st = make_pg(h->dec_k, dec->dense_w, opt);
   if (st == AAE_OK) st = make_pg(h->dec_b, dec->dense_b, opt);
   for (auto& L : dec->conv) { if (st == AAE_OK) st = make_pg(h->dec_k, L.w, opt); if (st == AAE_OK) st = make_pg(h->dec_b, L.b, opt); }
+  h->mask = dec->mask_w.p != nullptr;
+  if (st == AAE_OK && h->mask) st = make_pg(h->dec_k, dec->mask_w, opt);
+  if (st == AAE_OK && h->mask) st = make_pg(h->dec_b, dec->mask_b, opt);
+  if (st == AAE_OK && h->mask && enc->tc == nullptr && dec->conv.back().subpixel()) {
+    set_error("mask head: the fp32 trainer joins the head with an output conv of at most 3 channels (this one has %d)", dec->conv.back().out_c);
+    st = AAE_ERR_UNSUPPORTED;
+  }
   const size_t B = enc->cfg.max_batch, max_dense_w = std::max(enc->dense_w.n, dec->dense_w.n);
   size_t max_act = 0, max_up = 0, max_w = max_dense_w, max_c = 0;
   for (auto& L : enc->conv) { max_act = std::max(max_act, L.out_count(B)); max_w = std::max(max_w, L.w_count()); max_c = std::max<size_t>(max_c, L.out_c); }
@@ -999,13 +1096,24 @@ static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_rati
   if (st == AAE_OK) st = h->z.alloc(B * enc->cfg.latent);
   if (st == AAE_OK) st = h->dz.alloc(B * enc->cfg.latent);
   if (st == AAE_OK && max_wm) st = h->dwm.alloc(max_wm);
+  if (st == AAE_OK && h->mask) {
+    const ConvLayer& L = dec->conv.back();
+    const size_t pixels = B * L.out_h * L.out_w, joined = (size_t)(L.out_c + 1);
+    st = h->rec_mask.alloc(pixels);
+    if (st == AAE_OK) st = h->dmask.alloc(pixels);
+    if (st == AAE_OK) st = h->mask_sums.alloc(B);
+    // fp32 trainer: [k,k,Cin,C+1] kernel and [pixels, C+1] gradient of the joined layer; the tensor-core trainer joins them in its plan
+    if (st == AAE_OK) st = h->wcat.alloc(simt ? L.w_count() / L.out_c * joined : 0);
+    if (st == AAE_OK) st = h->dycat.alloc(simt ? pixels * joined : 0);
+  }
   if (st == AAE_OK && single_pass) {
     aae_net_cfg c = enc->cfg;
     c.precision = AAE_PREC_TC_FP16;
     st = tc_encoder_create(enc->device, &c, &h->fenc);
     c = dec->cfg;
     c.precision = AAE_PREC_TC_FP16;
-    if (st == AAE_OK) st = tc_decoder_create(dec->device, &c, &h->fdec);
+    if (st == AAE_OK) st = tc_decoder_create(dec->device, &c, h->mask, &h->fdec);
+    if (st == AAE_OK && h->mask) tc_decoder_set_mask_head(h->fdec, dec->mask_w.p, dec->mask_b.p);
     // bias pointers are the masters' (conv1's and the dense layer's are passed to every forward)
     for (int l = 1; st == AAE_OK && l < (int)enc->conv.size(); ++l) st = tc_encoder_set_bias(h->fenc, l, enc->conv[l].b.p);
     if (st == AAE_OK) {   // range overflows of the training forward and weight packs report through the handles' guard words
@@ -1089,6 +1197,8 @@ extern "C" int aae_trainer_destroy(aae_trainer* h) {
   h->dx_out.release(); h->grad_a.release(); h->grad_b.release(); h->dxup.release(); h->flat.release(); h->wt.release(); h->partials.release();
   h->bias_scratch.release(); h->sample_sums.release(); h->z.release(); h->dz.release(); h->rec.release(); h->dwm.release();
   h->pre.release(); h->sz.release(); h->dpre.release(); h->dcat.release(); h->lat_sums.release();
+  h->rec_mask.release(); h->dmask.release(); h->mask_sums.release(); h->wcat.release(); h->dycat.release();
+  h->dec->trainers -= 1;
   tc_train_destroy(h->tc);
   tc_encoder_destroy(h->fenc);
   tc_decoder_destroy(h->fdec);
@@ -1305,14 +1415,17 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
     AAE_TRY(launch_latent(latent_args(h, B, loss_out), 0, s));
     pt.mark(1, s);
   }
-  AAE_TRY(tc_decoder_forward(FD, decoder_input(h), B, h->rec.p, s));
+  AAE_TRY(tc_decoder_forward(FD, decoder_input(h), B, h->rec.p, h->mask ? h->rec_mask.p : nullptr, s));
   const int k = h->bootstrap_ratio > 1 ? numel / h->bootstrap_ratio : numel;
   AAE_TRY(launch_bootstrap_l2(h->rec.p, y, B, numel, k, h->sample_sums.p, loss_out, h->dx_out.p, s));
+  if (h->mask) AAE_TRY(launch_mask_loss(h->rec_mask.p, y, B, H * W, C, h->mask_sums.p, loss_out, h->dmask.p, s));
   AAE_TRY(launch_sigmoid_grad(h->dx_out.p, h->rec.p, (int64_t)B * numel, s));
+  if (h->mask) AAE_TRY(launch_sigmoid_grad(h->dmask.p, h->rec_mask.p, (int64_t)B * H * W, s));
   // ---- decoder backward ----
   pt.mark(4, s);
   AAE_TRY(launch_bias_grad(h->dx_out.p, (int64_t)B * H * W, C, h->dec_b[nd].g.p, h->bias_scratch.p, s));
-  AAE_TRY(tc_train_set_loss_grad(P, h->dx_out.p, B, s));
+  if (h->mask) AAE_TRY(launch_bias_grad(h->dmask.p, (int64_t)B * H * W, 1, h->dec_b[nd + 1].g.p, h->bias_scratch.p, s));
+  AAE_TRY(tc_train_set_loss_grad(P, h->dx_out.p, h->mask ? h->dmask.p : nullptr, B, s));
   float* raw = tc_train_raw(P);
   for (int u = 0; u < n_dec; ++u) {
     const int l = nd - u;                        // decoder conv layer l (1-based; dec_k[l], D->conv[l-1])
@@ -1321,7 +1434,14 @@ static int trainer_fwd_bwd_tc(aae_trainer* h, const float* x, const float* y, in
     pt.mark(2, s);
     AAE_TRY(tc_train_unit_wgrad(P, u, B, h->dwm.p, s));
     pt.mark(4, s);
-    AAE_TRY(launch_unmerge_subpixel_grads(h->dwm.p, cin, cout, h->dec_k[l].g.p, s));
+    if (u == 0 && h->mask) {                     // the joined output layer [k,k,Cin,C+1] -> output conv (C channels) and mask head
+      AAE_REQUIRE(h->wt.n >= (size_t)25 * cin * cout, "tensor-core trainer: scratch too small for the joined output layer");
+      AAE_TRY(launch_unmerge_subpixel_grads(h->dwm.p, cin, cout, h->wt.p, s));
+      AAE_TRY(launch_copy_channels(h->wt.p, cout, 0, h->dec_k[l].g.p, C, 0, C, 25LL * cin, s));
+      AAE_TRY(launch_copy_channels(h->wt.p, cout, C, h->dec_k[nd + 1].g.p, 1, 0, 1, 25LL * cin, s));
+    } else {
+      AAE_TRY(launch_unmerge_subpixel_grads(h->dwm.p, cin, cout, h->dec_k[l].g.p, s));
+    }
     pt.mark(3, s);
     AAE_TRY(tc_train_unit_dgrad(P, u, B, s));
     pt.mark(4, s);
@@ -1374,11 +1494,13 @@ static int trainer_fwd_bwd(aae_trainer* h, const float* x, const float* y, int B
   AAE_TRY(encoder_forward_simt(E, x, 0, B, h->z.p, s));
   if (h->w_v > 0.f) AAE_TRY(sigma_head_pre(E, SE.out.back().p, B, h->partials, h->pre.p, s));
   if (latent_terms_on(h)) AAE_TRY(launch_latent(latent_args(h, B, loss_out), 0, s));
-  AAE_TRY(decoder_forward_impl(D, decoder_input(h), B, h->rec.p, s));
+  AAE_TRY(decoder_forward_impl(D, decoder_input(h), B, h->rec.p, h->mask ? h->rec_mask.p : nullptr, s));
   const int k = h->bootstrap_ratio > 1 ? numel / h->bootstrap_ratio : numel;
   AAE_TRY(launch_bootstrap_l2(h->rec.p, y, B, numel, k, h->sample_sums.p, loss_out, h->dx_out.p, s));
+  if (h->mask) AAE_TRY(launch_mask_loss(h->rec_mask.p, y, B, H * W, C, h->mask_sums.p, loss_out, h->dmask.p, s));
   // ---- decoder backward ----
   AAE_TRY(launch_sigmoid_grad(h->dx_out.p, h->rec.p, (int64_t)B * numel, s));  // grad wrt pre-sigmoid
+  if (h->mask) AAE_TRY(launch_sigmoid_grad(h->dmask.p, h->rec_mask.p, (int64_t)B * H * W, s));
   const float* dy = h->dx_out.p;
   float* ping = h->grad_a.p;
   float* pong = h->grad_b.p;
@@ -1411,7 +1533,25 @@ static int trainer_fwd_bwd(aae_trainer* h, const float* x, const float* y, int B
       continue;
     }
     AAE_TRY(conv_wgrad(h, L, in_act, B, dy, h->dec_k[i + 1].g.p, s));
-    AAE_TRY(conv_dgrad(h, L, B, dy, h->dxup.p, nullptr, s));
+    if (h->mask && i + 1 == (int)D->conv.size()) {
+      // mask head: bias and kernel gradients as a Cout = 1 conv; the data gradient is that of the output conv and the head
+      // joined along Cout (kernel [k,k,Cin,C+1], gradient [pixels, C+1]), one GEMM with K = taps (C+1)
+      const int nd = (int)D->conv.size();
+      ConvLayer M = L;                           // non-owning view with the head's kernel
+      M.out_c = 1; M.w = D->mask_w;
+      AAE_TRY(launch_bias_grad(h->dmask.p, rows, 1, h->dec_b[nd + 1].g.p, h->bias_scratch.p, s));
+      AAE_TRY(conv_wgrad(h, M, in_act, B, h->dmask.p, h->dec_k[nd + 1].g.p, s));
+      const int64_t taps_cin = (int64_t)L.ksize * L.ksize * L.in_c;
+      AAE_TRY(launch_copy_channels(L.w.p, L.out_c, 0, h->wcat.p, L.out_c + 1, 0, L.out_c, taps_cin, s));
+      AAE_TRY(launch_copy_channels(D->mask_w.p, 1, 0, h->wcat.p, L.out_c + 1, L.out_c, 1, taps_cin, s));
+      AAE_TRY(launch_copy_channels(dy, L.out_c, 0, h->dycat.p, L.out_c + 1, 0, L.out_c, rows, s));
+      AAE_TRY(launch_copy_channels(h->dmask.p, 1, 0, h->dycat.p, L.out_c + 1, L.out_c, 1, rows, s));
+      ConvLayer J = L;
+      J.out_c = L.out_c + 1; J.w = h->wcat;
+      AAE_TRY(conv_dgrad(h, J, B, h->dycat.p, h->dxup.p, nullptr, s));
+    } else {
+      AAE_TRY(conv_dgrad(h, L, B, dy, h->dxup.p, nullptr, s));
+    }
     // backward of the x2 nearest-neighbour resize + ReLU of the producing layer
     AAE_TRY(launch_sumpool2_mask(h->dxup.p, in_act, ping, B, L.in_h, L.in_w, L.in_c, s));
     dy = ping;

@@ -157,6 +157,10 @@ int launch_opt_multi(OptBatch& b, int kind, float lr, const float hp[4], cudaStr
 int launch_merge_subpixel_weights(const float* w, int cin, int cout, float* wm, cudaStream_t stream);
 // gradient wrt the original taps: dW[kh,kw] = sum over the parities of the merged tap it was folded into
 int launch_unmerge_subpixel_grads(const float* dwm, int cin, int cout, float* dw, cudaStream_t stream);
+// out[r, out_off + j] = in[r, in_off + j] for r < rows, j < n (row widths in_ld / out_ld): joins the decoder's output conv and
+// mask head along Cout, and splits them again
+int launch_copy_channels(const float* in, int in_ld, int in_off, float* out, int out_ld, int out_off, int n, int64_t rows,
+                         cudaStream_t stream);
 // plain NHWC [B, 2h, 2w, C] -> space-to-depth [B, h, w, (py, px, c)]
 int launch_space_to_depth(const float* in, float* out, int B, int h, int w, int C, cudaStream_t stream);
 // dedicated wgrad of the first encoder layer (5x5 / stride 2 / Cin 3 / Cout 128): x fp32 NHWC, dy fp32 [B,OH,OW,128] -> dw [75,128]

@@ -121,7 +121,49 @@ __global__ void loss_finalize_kernel(const float* __restrict__ sample_sums, int 
   }
 }
 
+// Mask loss of AUXILIARY_MASK (auto_pose/ae/decoder.py:134-140): m = float(sum_c target[.., c] > 0.0001) per pixel (fp32 sum in
+// channel order), loss term = mean over B*P pixels of (xmask - m)^2, gradient 2 (xmask - m) / (B P).  One CTA per sample with
+// contiguous per-thread pixel ranges, so the sum order is fixed.
+__global__ void __launch_bounds__(LT) mask_loss_kernel(const float* __restrict__ xm, const float* __restrict__ y, int P, int C,
+                                                       float inv_bp, float* __restrict__ sample_sums, float* __restrict__ grad) {
+  __shared__ float fscratch[32];
+  const int t = threadIdx.x;
+  const long long off = (long long)blockIdx.x * P;
+  const int per = (P + LT - 1) / LT;
+  const int i0 = t * per, i1 = min(P, i0 + per);
+  float s = 0.f;
+  for (int i = i0; i < i1; ++i) {
+    const float* yp = y + (off + i) * C;
+    float cs = 0.f;
+    for (int c = 0; c < C; ++c) cs += yp[c];
+    const float d = xm[off + i] - (cs > 0.0001f ? 1.f : 0.f);
+    s += d * d;
+    if (grad) grad[off + i] = 2.f * d * inv_bp;
+  }
+  const float tot = block_sum(s, fscratch);
+  if (t == 0) sample_sums[blockIdx.x] = tot;
+}
+
+__global__ void loss_add_kernel(const float* __restrict__ sample_sums, int B, float inv, float* __restrict__ loss_inout) {
+  if (threadIdx.x == 0 && blockIdx.x == 0) {
+    float s = 0.f;
+    for (int b = 0; b < B; ++b) s += sample_sums[b];  // fixed order
+    *loss_inout += s * inv;
+  }
+}
+
 }  // namespace
+
+int launch_mask_loss(const float* xmask, const float* y, int B, int pixels, int C, float* sample_sums, float* loss_inout,
+                     float* grad_out, cudaStream_t stream) {
+  AAE_REQUIRE(B >= 1 && pixels >= 1 && C >= 1, "mask_loss: bad sizes");
+  const float inv_bp = 1.0f / ((float)B * (float)pixels);
+  mask_loss_kernel<<<B, LT, 0, stream>>>(xmask, y, pixels, C, inv_bp, sample_sums, grad_out);
+  AAE_LAUNCH_OK();
+  loss_add_kernel<<<1, 32, 0, stream>>>(sample_sums, B, inv_bp, loss_inout);
+  AAE_LAUNCH_OK();
+  return AAE_OK;
+}
 
 int launch_bootstrap_l2(const float* x, const float* y, int B, int numel, int k, float* sample_sums, float* loss_out,
                         float* grad_out, cudaStream_t stream) {

@@ -17,5 +17,9 @@ int launch_topk_merge(const float* s_in, const int* i_in, long long shard_stride
 // bootstrapped L2 loss (decoder.py:90-101)
 int launch_bootstrap_l2(const float* x, const float* y, int B, int numel, int k, float* sample_sums, float* loss_out,
                         float* grad_out, cudaStream_t stream);
+// mask loss of AUXILIARY_MASK (decoder.py:134-140): loss_inout += mean((xmask - m)^2), m from the target's channel sum;
+// grad_out (optional, [B, pixels]) receives dLoss/dxmask
+int launch_mask_loss(const float* xmask, const float* y, int B, int pixels, int C, float* sample_sums, float* loss_inout,
+                     float* grad_out, cudaStream_t stream);
 
 }  // namespace aae

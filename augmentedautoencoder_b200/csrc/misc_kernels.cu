@@ -405,6 +405,15 @@ __global__ void unmerge_subpixel_grads_kernel(const float* __restrict__ dwm, int
   }
 }
 
+__global__ void copy_channels_kernel(const float* __restrict__ in, int in_ld, int in_off, float* __restrict__ out, int out_ld, int out_off,
+                                     int n, long long rows) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < rows * n; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / n;
+    const int j = (int)(i - r * n);
+    out[r * out_ld + out_off + j] = in[r * in_ld + in_off + j];
+  }
+}
+
 __global__ void space_to_depth_kernel(const float4* __restrict__ in, float4* __restrict__ out, int B, int h, int w, int C4) {
   const long long total = (long long)B * h * w * 4 * C4;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -537,6 +546,13 @@ int launch_merge_subpixel_weights(const float* w, int cin, int cout, float* wm, 
 
 int launch_unmerge_subpixel_grads(const float* dwm, int cin, int cout, float* dw, cudaStream_t stream) {
   unmerge_subpixel_grads_kernel<<<grid_for(25LL * cin * cout, 256), 256, 0, stream>>>(dwm, cin, cout, dw);
+  AAE_LAUNCH_OK();
+  return AAE_OK;
+}
+
+int launch_copy_channels(const float* in, int in_ld, int in_off, float* out, int out_ld, int out_off, int n, int64_t rows,
+                         cudaStream_t stream) {
+  copy_channels_kernel<<<grid_for((long long)rows * n, 256), 256, 0, stream>>>(in, in_ld, in_off, out, out_ld, out_off, n, rows);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }

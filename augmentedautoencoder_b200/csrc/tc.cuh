@@ -34,10 +34,13 @@ void tc_encoder_share_range_flag(TcEncoder* h, unsigned* flag);
 int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int64_t* count, cudaStream_t s);
 
 struct TcDecoder;
-int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out);
+// mask_head: the output layer also computes the AUXILIARY_MASK head (Cout = C + 1); its masters are named by tc_decoder_set_mask_head
+int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcDecoder** out);
 void tc_decoder_destroy(TcDecoder* h);
+void tc_decoder_set_mask_head(TcDecoder* h, const float* w_dev, const float* b_dev);
+// the output layer's pack (layer num_layers) reads the mask head's kernel too, so a changed head kernel is packed through it
 int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const float* b_dev, cudaStream_t s);
-int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, cudaStream_t s);
+int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, float* mask_out, cudaStream_t s);   // mask_out may be null
 unsigned* tc_decoder_range_flag(TcDecoder* h);
 void tc_decoder_share_range_flag(TcDecoder* h, unsigned* flag);
 const float* tc_decoder_merged_weights(const TcDecoder* h);   // fp32 merged sub-pixel weights of the layer packed last
@@ -55,7 +58,8 @@ float* tc_train_raw(TcTrainPlan* h);
 int tc_train_begin_step(TcTrainPlan* h, cudaStream_t s);
 int tc_train_pack_weights(TcTrainPlan* h, int u, const float* w_dev, cudaStream_t s);
 int tc_train_pack_weights_merged(TcTrainPlan* h, int u, const float* wm_dev, cudaStream_t s);
-int tc_train_set_loss_grad(TcTrainPlan* h, const float* g_dev, int B, cudaStream_t s);
+// g_dev: pre-sigmoid gradient of x [B, H, W, C]; gm_dev: that of the mask [B, H, W] (the decoder has the mask head) or null
+int tc_train_set_loss_grad(TcTrainPlan* h, const float* g_dev, const float* gm_dev, int B, cudaStream_t s);
 int tc_train_set_unit_grad(TcTrainPlan* h, int u, const float* g_dev, int B, cudaStream_t s);
 int tc_train_unit_wgrad(TcTrainPlan* h, int u, int B, float* dw_out, cudaStream_t s);
 int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s);

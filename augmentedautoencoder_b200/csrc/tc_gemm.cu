@@ -717,9 +717,9 @@ __global__ void split_scale_kernel(const float* __restrict__ x, long long n, flo
 
 // merged weights Wm [9][cin][n4] -> operand of the tap-separable output layer: row (tap * n4 + m) = Wm[tap][:, m], rows >= 9*n4 zero
 template <int PLANES>
-__global__ void pack_out_sep_kernel(const float* __restrict__ wm, int cin, int n4, float scale, __half* __restrict__ hi, __half* __restrict__ lo,
-                                    unsigned* __restrict__ range_flag, unsigned range_bit) {
-  const int total = 128 * cin;
+__global__ void pack_out_sep_kernel(const float* __restrict__ wm, int cin, int n4, int rows, float scale, __half* __restrict__ hi,
+                                    __half* __restrict__ lo, unsigned* __restrict__ range_flag, unsigned range_bit) {
+  const int total = rows * cin;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int ci = i % cin, n = i / cin;
     const int tap = n / n4, m = n - tap * n4;
@@ -727,10 +727,11 @@ __global__ void pack_out_sep_kernel(const float* __restrict__ wm, int cin, int n
   }
 }
 
-// x[b, 2i+py, 2j+px, co] = sigmoid(bias[co] + sum_{tap=(ty,tx)} P[(b, i+ty-1, j+tx-1)][tap*4c + (py*2+px)*c + co]); one thread per output value
-__global__ void outlayer_gather_kernel(const float* __restrict__ P, const float* __restrict__ bias, int B, int h, int w, int c,
-                                       float* __restrict__ x) {
-  const int n4 = 4 * c;
+// x[b, 2i+py, 2j+px, co] = sigmoid(bias[co] + sum_{tap=(ty,tx)} P[(b, i+ty-1, j+tx-1)][tap*4ct + (py*2+px)*ct + co]) with ct = c + cm;
+// channel co = c (cm = 1: the mask head) goes to mask[b, 2i+py, 2j+px] with its own bias.  One thread per output value.
+__global__ void outlayer_gather_kernel(const float* __restrict__ P, int ldp, const float* __restrict__ bias, const float* __restrict__ mask_bias,
+                                       int B, int h, int w, int c, int cm, float* __restrict__ x, float* __restrict__ mask) {
+  const int ct = c + cm, n4 = 4 * ct;
   const long long total = (long long)B * h * w * n4;
   for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (long long)gridDim.x * blockDim.x) {
     const int m = (int)(t % n4);
@@ -738,8 +739,9 @@ __global__ void outlayer_gather_kernel(const float* __restrict__ P, const float*
     const int j = (int)(r % w); r /= w;
     const int i = (int)(r % h);
     const long long b = r / h;
-    const int cls = m / c, co = m - cls * c;
-    float s = bias ? __ldg(bias + co) : 0.f;
+    const int cls = m / ct, co = m - cls * ct;
+    const float* bp = co < c ? bias : mask_bias;
+    float s = bp ? __ldg(bp + (co < c ? co : 0)) : 0.f;
 #pragma unroll
     for (int ty = 0; ty < 3; ++ty) {
       const int ii = i + ty - 1;
@@ -748,10 +750,12 @@ __global__ void outlayer_gather_kernel(const float* __restrict__ P, const float*
       for (int tx = 0; tx < 3; ++tx) {
         const int jj = j + tx - 1;
         if (jj < 0 || jj >= w) continue;
-        s += P[((b * h + ii) * w + jj) * 128 + (ty * 3 + tx) * n4 + m];
+        s += P[((b * h + ii) * w + jj) * ldp + (ty * 3 + tx) * n4 + m];
       }
     }
-    x[((b * 2 * h + 2 * i + (cls >> 1)) * (2LL * w) + 2 * j + (cls & 1)) * c + co] = 1.f / (1.f + expf(-s));
+    const long long px = (b * 2 * h + 2 * i + (cls >> 1)) * (2LL * w) + 2 * j + (cls & 1);
+    if (co < c) x[px * c + co] = 1.f / (1.f + expf(-s));
+    else if (mask) mask[px] = 1.f / (1.f + expf(-s));
   }
 }
 
@@ -781,7 +785,7 @@ int tc_layer_setup_plain(TcLayer& T, int B, int planes) {
   return T.w.encode(T.tm_w, 2, dims, strides, box);
 }
 
-int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
+int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcDecoder** out) {
   *out = nullptr;
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   const int L = cfg->num_layers;
@@ -808,7 +812,7 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
     } else {                                        // sub-pixel conv on the (h x w x C) low-resolution activation
       const int hh = h0 << (l - 1);
       T.in_h = T.in_w = hh; T.in_c = nf[l - 1];
-      const int cout = l < L ? nf[l] : cfg->in_c;
+      const int cout = l < L ? nf[l] : cfg->in_c + (mask_head ? 1 : 0);
       T.out_h = T.out_w = 2 * hh; T.out_c = cout;
       T.taps = 9;
       if (hh > 128 || (hh & (hh - 1)) || T.in_c % 64 != 0 || (l < L && cout % 64 != 0)) {
@@ -818,12 +822,15 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, TcDecoder** out) {
       g.OH = g.OW = hh;
       if (l < L) { g.N = 4 * cout; g.relu = 1; g.out_mode = OUT_D2S_SPLIT; }
       else {                                        // 1x1 GEMM into P, neighbourhood sum in outlayer_gather_kernel
-        if (36 * cout > 128) {
-          set_error("tc decoder: %d output channels, the tensor-core output layer takes at most 3 (AAE_PREC_FP32_SIMT takes any count)", cout);
+        if (cfg->in_c > 3) {
+          set_error("tc decoder: %d output channels, the tensor-core output layer takes at most 3 (AAE_PREC_FP32_SIMT takes any count)", cfg->in_c);
           st = AAE_ERR_UNSUPPORTED; break;
         }
-        T.taps = 1; g.N = 128; g.relu = 0; g.out_mode = OUT_F32;
-        st = dev_alloc((void**)&h->out_p, (size_t)ceil_div((int64_t)B * hh * hh, 128) * 128 * 128 * sizeof(float));
+        // 9 taps x 4 parities x Cout columns: 128 for x alone, 256 with the mask head (one pass over the activation either way)
+        T.taps = 1; g.N = (int)ceil_div(36 * cout, 128) * 128; g.relu = 0; g.out_mode = OUT_F32;
+        h->out_x = cfg->in_c;
+        st = dev_alloc((void**)&h->out_p, (size_t)ceil_div((int64_t)B * hh * hh, 128) * 128 * g.N * sizeof(float));
+        if (st == AAE_OK && mask_head) st = dev_alloc((void**)&h->cat_tmp, (size_t)25 * T.in_c * cout * sizeof(float));
         if (st != AAE_OK) break;
       }
     }
@@ -863,6 +870,7 @@ void tc_decoder_destroy(TcDecoder* h) {
   for (auto b : h->bias_dev) cudaFree(b);
   cudaFree(h->wm_tmp);
   cudaFree(h->out_p);
+  cudaFree(h->cat_tmp);
   if (h->owns_range_flag) cudaFree(h->range_flag);
   delete h;
 }
@@ -885,11 +893,17 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
   }
   const bool out_layer = layer + 1 == (int)h->layers.size();
   if (w_dev) {
+    if (out_layer && h->cat_tmp) {      // join the output conv [5,5,Cin,C] and the mask head [5,5,Cin,1] along Cout
+      AAE_REQUIRE(h->mask_w != nullptr, "tc decoder: the mask head's weights are not set");
+      AAE_TRY(launch_copy_channels(w_dev, h->out_x, 0, h->cat_tmp, T.out_c, 0, h->out_x, 25LL * T.in_c, s));
+      AAE_TRY(launch_copy_channels(h->mask_w, 1, 0, h->cat_tmp, T.out_c, h->out_x, 1, 25LL * T.in_c, s));
+      w_dev = h->cat_tmp;
+    }
     AAE_TRY(launch_merge_subpixel_weights(w_dev, T.in_c, T.out_c, h->wm_tmp, s));
     const unsigned bit = 1u << (16 + layer);
     dim3 grid((unsigned)ceil_div(4 * T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), 9);
     with_planes(h->planes, [&](auto P) {
-      if (out_layer) pack_out_sep_kernel<P><<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, W_SCALE, T.w.hi, T.w.lo, h->range_flag, bit);
+      if (out_layer) pack_out_sep_kernel<P><<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, T.gp.N, W_SCALE, T.w.hi, T.w.lo, h->range_flag, bit);
       else pack_weights_kernel<P><<<grid, block, 0, s>>>(h->wm_tmp, 9, T.in_c, 4 * T.out_c, W_SCALE, T.w.hi, T.w.lo, h->range_flag, bit);
     });
     AAE_LAUNCH_OK();
@@ -908,7 +922,13 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
 
 const float* tc_decoder_merged_weights(const TcDecoder* h) { return h->wm_tmp; }
 
-int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, cudaStream_t s) {
+void tc_decoder_set_mask_head(TcDecoder* h, const float* w_dev, const float* b_dev) {
+  h->mask_w = w_dev;
+  h->mask_b = b_dev;
+}
+
+// mask_out: [B, H, W] mask of the head (null: not written)
+int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, float* mask_out, cudaStream_t s) {
   TcLayer& D = h->layers[0];
   const unsigned grid = (unsigned)std::min<int64_t>(1024, ceil_div((int64_t)B * D.in_c, 256));
   with_planes(h->planes, [&](auto P) {
@@ -924,8 +944,8 @@ int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, cu
     AAE_TRY(tc_launch_layer(T, grid, s, h->planes));
     if (last) {
       const long long total = (long long)T.gp.M * 4 * T.out_c;
-      outlayer_gather_kernel<<<(unsigned)std::min<long long>(132 * 16, ceil_div(total, 256)), 256, 0, s>>>(h->out_p, h->out_bias, B, T.in_h, T.in_w,
-                                                                                                         T.out_c, x_out);
+      outlayer_gather_kernel<<<(unsigned)std::min<long long>(132 * 16, ceil_div(total, 256)), 256, 0, s>>>(
+          h->out_p, T.gp.N, h->out_bias, h->mask_b, B, T.in_h, T.in_w, h->out_x, T.out_c - h->out_x, x_out, mask_out);
       AAE_LAUNCH_OK();
     }
   }

@@ -144,8 +144,14 @@ struct TcDecoder {
   // Output layer (Cout <= 3, so that 36 * Cout <= 128) in "tap-separable" form.  P[pixel, (tap, cls, co)] = X[pixel, :] . Wm[tap, :, (cls, co)]
   // is ONE 1x1 GEMM (K = Cin, N = 128) that reads the activation once instead of once per tap; the 3x3 neighbourhood sum,
   // bias, sigmoid and depth-to-space scatter happen in a small gather kernel over P.
-  float* out_p = nullptr;          // [B*h*w (padded to 128 rows)][128] fp32
-  const float* out_bias = nullptr; // the caller's bias [Cout] (device)
+  // With the mask head (AUXILIARY_MASK) the head and the output conv read the same input and both end in a sigmoid: they are
+  // one output layer of Cout = C + 1 channels (N = 256), channel C being the mask.
+  float* out_p = nullptr;          // [B*h*w (padded to 128 rows)][N] fp32
+  const float* out_bias = nullptr; // the caller's bias [C] (device)
+  int out_x = 0;                   // C: output-layer channels of x (the layer's out_c is C + 1 with the mask head)
+  const float* mask_w = nullptr;   // mask head kernel [5,5,Cin,1] and bias [1] (device masters; null without the head)
+  const float* mask_b = nullptr;
+  float* cat_tmp = nullptr;        // [5,5,Cin,C+1]: the output conv's kernel joined with the head's along Cout
   size_t wm_floats = 0;
   int planes = 2;                  // fp16 planes per operand: 2 = (hi, lo); 1 = hi only (the single-pass trainer's private plan)
 };

@@ -300,13 +300,14 @@ __global__ void amax_scalar_kernel(const float* __restrict__ x, long long n, uns
 }
 
 // tap-separable output layer: G[pixel (b,y,x)][tap * n4 + m] = gs[(b, y - (ty-1), x - (tx-1))][m], gs = space-to-depth of the
-// pre-sigmoid gradient g [B, 2h, 2w, c] (m = cls * c + co); columns >= 9 * n4 stay zero.  With this im2col both the dgrad
-// (K = 128) and the wgrad (N = 128) of the layer read the big activation tensor exactly once.
+// pre-sigmoid gradient [B, 2h, 2w, ct] (m = cls * ct + co); columns >= 9 * n4 stay zero.  With this im2col both the dgrad
+// (K = ldg) and the wgrad (N = ldg) of the layer read the big activation tensor exactly once.  Channels co < c come from g
+// [B, 2h, 2w, c]; with the mask head (cm = 1) channel c comes from gm [B, 2h, 2w].
 template <int PLANES>
-__global__ void pack_loss_grad_sep_kernel(const float* __restrict__ g, int B, int h, int w, int c, const unsigned* __restrict__ amax,
-                                          __half* __restrict__ hi, __half* __restrict__ lo) {
+__global__ void pack_loss_grad_sep_kernel(const float* __restrict__ g, const float* __restrict__ gm, int B, int h, int w, int c, int cm,
+                                          int ldg, const unsigned* __restrict__ amax, __half* __restrict__ hi, __half* __restrict__ lo) {
   const float scale = tc_dyn_scale(__ldg(amax));
-  const int n4 = 4 * c;
+  const int ct = c + cm, n4 = 4 * ct;
   const long long total = (long long)B * h * w * 9;       // one thread per (pixel, tap): n4 consecutive columns
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int tap = (int)(i % 9);
@@ -316,38 +317,39 @@ __global__ void pack_loss_grad_sep_kernel(const float* __restrict__ g, int B, in
     const long long b = r / h;
     const int ys = y - (tap / 3 - 1), xs = x - (tap % 3 - 1);
     const bool in = ys >= 0 && ys < h && xs >= 0 && xs < w;
-    const long long o = ((b * h + y) * w + x) * 128 + tap * n4;
-    // n4 = 4c values -> c groups of 4 halves (8 bytes) per plane
-    for (int q = 0; q < c; ++q) {
+    const long long o = ((b * h + y) * w + x) * ldg + tap * n4;
+    // n4 = 4ct values -> ct groups of 4 halves (8 bytes) per plane
+    for (int q = 0; q < ct; ++q) {
       float v[4];
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const int m = q * 4 + e, cls = m / c, co = m - cls * c;
-        v[e] = in ? g[((b * 2 * h + 2 * ys + (cls >> 1)) * (2LL * w) + 2 * xs + (cls & 1)) * c + co] * scale : 0.f;
+        const int m = q * 4 + e, cls = m / ct, co = m - cls * ct;
+        const long long px = (b * 2 * h + 2 * ys + (cls >> 1)) * (2LL * w) + 2 * xs + (cls & 1);
+        v[e] = in ? (co < c ? g[px * c + co] : gm[px]) * scale : 0.f;
       }
       tc_store_f16<PLANES>(v, 1.f, hi, lo, o + q * 4);
     }
   }
 }
 
-// tap-separable output layer: dgrad operand [cin][128], column (tap * n4 + m) = Wm[tap][ci][m]
+// tap-separable output layer: dgrad operand [cin][ldg], column (tap * n4 + m) = Wm[tap][ci][m]
 template <int PLANES>
-__global__ void pack_dec_dgrad_sep_kernel(const float* __restrict__ wm, int cin, int n4, float scale, __half* __restrict__ hi,
+__global__ void pack_dec_dgrad_sep_kernel(const float* __restrict__ wm, int cin, int n4, int ldg, float scale, __half* __restrict__ hi,
                                           __half* __restrict__ lo) {
-  const int total = cin * 128;
+  const int total = cin * ldg;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-    const int k = i & 127, ci = i >> 7;
+    const int k = i % ldg, ci = i / ldg;
     const int tap = k / n4, m = k - tap * n4;
     tc_store_f16<PLANES>(tap < 9 ? wm[((long long)tap * cin + ci) * n4 + m] * scale : 0.f, hi, lo, i);
   }
 }
 
-// wgrad result of the tap-separable layer [cin][128] (column = tap * n4 + m) -> merged-gradient layout [9][cin][n4]
-__global__ void rearrange_sep_wgrad_kernel(const float* __restrict__ in, int cin, int n4, float* __restrict__ out) {
+// wgrad result of the tap-separable layer [cin][ldg] (column = tap * n4 + m) -> merged-gradient layout [9][cin][n4]
+__global__ void rearrange_sep_wgrad_kernel(const float* __restrict__ in, int cin, int n4, int ldg, float* __restrict__ out) {
   const int total = 9 * cin * n4;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int m = i % n4, ci = (i / n4) % cin, tap = i / (n4 * cin);
-    out[i] = in[ci * 128 + tap * n4 + m];
+    out[i] = in[ci * ldg + tap * n4 + m];
   }
 }
 
@@ -456,7 +458,8 @@ int launch_wgrad(const TcMaps& x, const TcMaps& g, const TcWgradParams& p, dim3 
 // ------------------------------------------------------------------------------------------------- plan
 struct TcUnit {
   bool enc;                 // encoder 5x5/s2 layer (X in space-to-depth form) or decoder sub-pixel layer
-  int cin, cout;            // the layer's real channel counts
+  int cin, cout;            // the layer's real channel counts (the output layer's cout includes the mask head)
+  int cx;                   // output layer: channels of x (cout - 1 with the mask head)
   int gh, gw, gN;           // G = pre-activation gradient of the layer's GEMM output: plain [B, gh, gw, gN]
   int taps_w;               // taps of the wgrad (25 / 9; 1 for the tap-separable output layer)
   int dg_taps;              // taps of the dgrad conv over G (9; 1 for the tap-separable output layer)
@@ -563,10 +566,10 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
   for (int l = Ld; l >= 1 && st == AAE_OK; --l) {          // decoder units
     const TcLayer& F = dec->layers[l];
     TcUnit U;
-    U.enc = false; U.cin = F.in_c; U.cout = F.out_c;
+    U.enc = false; U.cin = F.in_c; U.cout = F.out_c; U.cx = l == Ld ? dec->out_x : F.out_c;
     U.gh = F.in_h; U.gw = F.in_w;
     U.sep = l == Ld;
-    U.gN = U.sep ? 128 : 4 * F.out_c;
+    U.gN = U.sep ? F.gp.N : 4 * F.out_c;           // the tap-separable layer's G has the forward GEMM's 128 or 256 columns
     U.taps_w = U.sep ? 1 : 9; U.dg_taps = U.sep ? 1 : 9; U.nd = F.in_c;
     U.mask_hi = F.in.hi;                                   // dgrad result = gradient wrt this layer's input activation
     h->units.push_back(U);
@@ -576,7 +579,7 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
   for (int i = Le - 1; i >= 0 && st == AAE_OK; --i) {      // encoder units (enc->layers[i] = conv i+2)
     const TcLayer& F = enc->layers[i];
     TcUnit U;
-    U.enc = true; U.cin = F.in_c; U.cout = F.out_c;
+    U.enc = true; U.cin = F.in_c; U.cout = F.out_c; U.cx = F.out_c;
     U.gh = F.out_h; U.gw = F.out_w; U.gN = F.out_c;
     U.taps_w = 25; U.dg_taps = 9; U.sep = false; U.nd = 4 * F.in_c;
     U.mask_hi = F.in.hi;                                   // space-to-depth activation, same layout as the dgrad result
@@ -592,7 +595,7 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
       memset(&Fx.gp, 0, sizeof(Fx.gp));
       Fx.in = h->c1_x; Fx.BB = 1;
       TcUnit U;
-      U.enc = true; U.cin = 128; U.cout = F2.in_c;
+      U.enc = true; U.cin = 128; U.cout = F2.in_c; U.cx = F2.in_c;
       U.gh = F2.in_h; U.gw = F2.in_w; U.gN = F2.in_c;
       U.taps_w = 1; U.dg_taps = 1; U.sep = false; U.nd = 128;   // (no dgrad is ever run for this unit: the input image needs no gradient)
       U.mask_hi = nullptr;
@@ -648,9 +651,9 @@ int tc_train_pack_weights(TcTrainPlan* h, int u, const float* w_dev, cudaStream_
 int tc_train_pack_weights_merged(TcTrainPlan* h, int u, const float* wm_dev, cudaStream_t s) {
   AAE_REQUIRE(u >= 0 && u < h->n_dec, "tc trainer: unit %d is not a decoder unit", u);
   TcUnit& U = h->units[u];
-  const unsigned sep_grid = ew_grid((long long)U.cin * 128), grid = ew_grid((long long)U.cin * 9 * U.gN);
+  const unsigned sep_grid = ew_grid((long long)U.cin * U.gN), grid = ew_grid((long long)U.cin * 9 * U.gN);
   with_planes(h->planes, [&](auto P) {
-    if (U.sep) pack_dec_dgrad_sep_kernel<P><<<sep_grid, 256, 0, s>>>(wm_dev, U.cin, 4 * U.cout, W_SCALE, U.dg.w.hi, U.dg.w.lo);
+    if (U.sep) pack_dec_dgrad_sep_kernel<P><<<sep_grid, 256, 0, s>>>(wm_dev, U.cin, 4 * U.cout, U.gN, W_SCALE, U.dg.w.hi, U.dg.w.lo);
     else pack_dec_dgrad_kernel<P><<<grid, 256, 0, s>>>(wm_dev, U.cin, U.gN, W_SCALE, U.dg.w.hi, U.dg.w.lo);
   });
   AAE_LAUNCH_OK();
@@ -658,15 +661,21 @@ int tc_train_pack_weights_merged(TcTrainPlan* h, int u, const float* wm_dev, cud
 }
 
 // pre-sigmoid gradient of the reconstruction [B, H, W, C] -> G of unit 0 (the decoder output layer)
-int tc_train_set_loss_grad(TcTrainPlan* h, const float* g_dev, int B, cudaStream_t s) {
+int tc_train_set_loss_grad(TcTrainPlan* h, const float* g_dev, const float* gm_dev, int B, cudaStream_t s) {
   TcUnit& U = h->units[0];
-  const int c = U.cout;
+  const int c = U.cx, cm = U.cout - U.cx;
+  AAE_REQUIRE((gm_dev != nullptr) == (cm == 1), "tc trainer: the mask gradient is required exactly with the mask head");
   const long long n = (long long)B * U.gh * U.gw * 4 * c;
   amax_scalar_kernel<<<ew_grid(n), 256, 0, s>>>(g_dev, n, h->amax + 0);
   AAE_LAUNCH_OK();
+  if (gm_dev) {      // one scale for the whole G of the joined layer
+    const long long nm = (long long)B * U.gh * U.gw * 4;
+    amax_scalar_kernel<<<ew_grid(nm), 256, 0, s>>>(gm_dev, nm, h->amax + 0);
+    AAE_LAUNCH_OK();
+  }
   const unsigned grid = ew_grid((long long)B * U.gh * U.gw * 9);
   with_planes(h->planes, [&](auto P) {
-    pack_loss_grad_sep_kernel<P><<<grid, 256, 0, s>>>(g_dev, B, U.gh, U.gw, c, h->amax + 0, U.dg.in.hi, U.dg.in.lo);
+    pack_loss_grad_sep_kernel<P><<<grid, 256, 0, s>>>(g_dev, gm_dev, B, U.gh, U.gw, c, cm, U.gN, h->amax + 0, U.dg.in.hi, U.dg.in.lo);
   });
   AAE_LAUNCH_OK();
   return AAE_OK;
@@ -708,7 +717,7 @@ int tc_train_unit_wgrad(TcTrainPlan* h, int u, int B, float* dw_out, cudaStream_
   if (!U.sep) return launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, dw_out, s);
   AAE_REQUIRE((size_t)mn <= h->wm_floats, "tc trainer: merged-gradient scratch too small");
   AAE_TRY(launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, h->wm, s));
-  rearrange_sep_wgrad_kernel<<<ew_grid(9LL * U.cin * 4 * U.cout), 256, 0, s>>>(h->wm, U.cin, 4 * U.cout, dw_out);
+  rearrange_sep_wgrad_kernel<<<ew_grid(9LL * U.cin * 4 * U.cout), 256, 0, s>>>(h->wm, U.cin, 4 * U.cout, U.gN, dw_out);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }

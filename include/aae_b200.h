@@ -180,13 +180,29 @@ AAE_API int aae_codebook_profile(aae_codebook* h, int enable, float* stage_ms_ou
  * NN-resize x2, conv5x5 -> C + sigmoid (auto_pose/ae/decoder.py:36-84). */
 AAE_API int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decoder** out);
 AAE_API int aae_decoder_destroy(aae_decoder* h);
-/* layer 0 = dense_1 [latent, h0*w0*f0]; layers 1..num_layers = the convs in forward order. */
+/* layer 0 = dense_1 [latent, h0*w0*f0]; layers 1..num_layers = the convs in forward order; num_layers + 1 = the mask head
+ * (aae_decoder_enable_mask_head). */
 AAE_API int aae_decoder_set_weights(aae_decoder* h, int layer, const float* kernel_any, const float* bias_any, void* stream);
 AAE_API int aae_decoder_get_weights(aae_decoder* h, int layer, float* kernel_any, float* bias_any, void* stream);
 AAE_API int aae_decoder_forward(aae_decoder* h, const float* z_dev, int batch, float* x_out_dev, void* stream);
 /* Same contract as aae_encoder_range_status for the decoder (dense_1 counts as layer 0; the latent fed to the decoder is
  * covered too). */
 AAE_API int aae_decoder_range_status(aae_decoder* h, void* stream);
+/* Mask head of AUXILIARY_MASK: xmask = sigmoid(conv(x_in, W, padding SAME) + b) with x_in the output conv's input
+ * (auto_pose/ae/decoder.py:68-75).  Allocates W [k, k, Cin, 1] and b [1], zero until set; calling it again is a no-op.
+ * Afterwards layer num_layers + 1 of aae_decoder_set_weights / get_weights addresses the head (TF names: the head is
+ * "conv2d_<k>" and the output conv "conv2d_<k+1>", k = encoder convs + decoder hidden convs), the range guard covers its
+ * kernel, and a trainer created over the handle trains it (reconstruction loss + mask loss; get_grads / get_state / set_state
+ * with which = 1, layer = num_layers + 1).  The kernels run the head and the output conv as ONE conv with C + 1 output
+ * channels, so x is unchanged by it.  A live trainer over the handle: AAE_ERR_UNSUPPORTED (enable the head first). */
+AAE_API int aae_decoder_enable_mask_head(aae_decoder* h);
+/* x [batch, H, W, C] and the mask [batch, H, W] in one forward.  No head: AAE_ERR_UNSUPPORTED. */
+AAE_API int aae_decoder_forward_mask(aae_decoder* h, const float* z_dev, int batch, float* x_out_dev, float* mask_out_dev, void* stream);
+/* Mask loss of AUXILIARY_MASK (auto_pose/ae/decoder.py:134-140): *loss_inout_dev += mean over [batch, pixels] of (xmask - m)^2,
+ * m = 1 where the fp32 sum of the target's channels (in channel order) is > 0.0001, else 0.  target_dev [batch, pixels,
+ * channels] fp32.  grad_out_dev (optional, [batch, pixels]) receives 2 (xmask - m) / (batch pixels).  Fixed reduction order. */
+AAE_API int aae_mask_loss(const float* mask_dev, const float* target_dev, int batch, int pixels_per_sample, int channels,
+                          float* loss_inout_dev, float* grad_out_dev, void* stream);
 /* Bootstrapped L2 (LOSS: L2, BOOTSTRAP_RATIO r): per-sample top-k of the flattened squared error,
  * k = numel/r, mean over the [B,k] survivors (auto_pose/ae/decoder.py:90-101).
  * grad_out_dev (optional, [B,numel]) receives dLoss/dx. */
