@@ -439,7 +439,10 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
   *out = nullptr;
   const int L = cfg->num_layers;
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
-  AAE_REQUIRE(L >= 2, "AAE_PREC_TC_SPLIT: at least two conv layers expected");
+  if (L < 2) {
+    set_error("AAE_PREC_TC_SPLIT: at least two conv layers expected (this network has %d)", L);
+    return AAE_ERR_UNSUPPORTED;
+  }
   const int planes = tc_planes(cfg->precision);
   if (planes == 1 && !tc_conv1_supported(cfg)) {   // the fp32 CUDA-core conv1 behind the split plan writes (hi, lo) pairs only
     set_error("AAE_PREC_TC_FP16: the first layer needs the tensor-core conv1 (128 x 128 x 3 crops, 128 filters, k = 5, stride 2)");
@@ -478,8 +481,11 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
     }
     // batch dimension padded to a whole number of TMA boxes, so a tile never addresses rows outside the tensor map
     const int B_pad = (int)ceil_div(B, T.BB) * T.BB;
+    // weight rows padded to whole N tiles (zero-filled; pack_weights_kernel writes rows < out_c only): the producer arms every W
+    // stage for TC_N_TILE rows, so a box of fewer rows (out_c < 128) would never complete the stage's barrier
+    const int w_rows = (int)ceil_div(T.out_c, TC_N_TILE) * TC_N_TILE;
     if ((st = T.in.alloc((size_t)B_pad * T.in_h * T.in_w * T.in_c, planes)) != AAE_OK) break;
-    if ((st = T.w.alloc((size_t)T.out_c * T.taps * T.in_c, planes)) != AAE_OK) break;
+    if ((st = T.w.alloc((size_t)w_rows * T.taps * T.in_c, planes)) != AAE_OK) break;
     // ---- tensor maps ----
     uint64_t a_dims[4], a_strides[3];
     if (!dense) {
@@ -498,9 +504,9 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
     }
     {
       const uint64_t K = (uint64_t)T.taps * T.in_c;
-      const uint64_t dims[2] = {K, (uint64_t)T.out_c};
+      const uint64_t dims[2] = {K, (uint64_t)w_rows};
       const uint64_t strides[1] = {K * 2};
-      const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)std::min(TC_N_TILE, T.out_c)};
+      const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)TC_N_TILE};
       if ((st = T.w.encode(T.tm_w, 2, dims, strides, box)) != AAE_OK) break;
     }
     // ---- static GEMM parameters ----
@@ -789,7 +795,10 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcDeco
   *out = nullptr;
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   const int L = cfg->num_layers;
-  AAE_REQUIRE(cfg->kernel_size == 5 && cfg->in_h == cfg->in_w, "AAE_PREC_TC_SPLIT decoder: kernel 5, square crops");
+  if (cfg->kernel_size != 5 || cfg->in_h != cfg->in_w) {
+    set_error("AAE_PREC_TC_SPLIT decoder: kernel 5 and square crops required (kernel %d, %d x %d crops)", cfg->kernel_size, cfg->in_h, cfg->in_w);
+    return AAE_ERR_UNSUPPORTED;
+  }
   TcDecoder* h = new TcDecoder();
   h->device = device;
   h->cfg = *cfg;

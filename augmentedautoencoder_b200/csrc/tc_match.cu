@@ -370,7 +370,10 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
                        TcCodebook** out) {
   *out = nullptr;
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
-  AAE_REQUIRE(latent == 128, "AAE_PREC_TC_SPLIT codebook match is built for latent = 128 (got %d)", latent);
+  if (latent != 128) {
+    set_error("AAE_PREC_TC_SPLIT codebook match is built for latent = 128 (got %d)", latent);
+    return AAE_ERR_UNSUPPORTED;
+  }
   TcCodebook* h = new TcCodebook();
   h->device = device;
   h->planes = planes;

@@ -523,7 +523,12 @@ static int make_wgrad_maps(TcUnit& U, int x_c_total, int x_bpad, int g_bpad) {
 
 int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan** out) {
   *out = nullptr;
-  AAE_REQUIRE(enc && dec && enc->conv1, "tensor-core trainer: needs the tensor-core encoder (incl. conv1) and decoder plans");
+  AAE_REQUIRE(enc && dec, "tensor-core trainer: needs the tensor-core encoder and decoder plans");
+  if (!enc->conv1) {
+    set_error("tensor-core trainer: conv1 runs on the fp32 kernel for this geometry (the trainer needs the tensor-core conv1: "
+              "128 x 128 x 3 crops, 128 filters, k = 5, stride 2)");
+    return AAE_ERR_UNSUPPORTED;
+  }
   AAE_REQUIRE(enc->planes == dec->planes, "tensor-core trainer: the encoder and decoder plans use different operand planes");
   TcTrainPlan* h = new TcTrainPlan();
   h->device = enc->device; h->max_batch = max_batch; h->enc = enc; h->dec = dec; h->planes = enc->planes;

@@ -66,19 +66,20 @@ def glorot_uniform(rng: np.random.RandomState, shape: Sequence[int]) -> np.ndarr
 
 
 def make_encoder_params(seed: int = 42, num_filters=NUM_FILTER, ksize=KSIZE, latent=LATENT,
-                        in_ch=C, in_hw=H, strides=STRIDES, bias_scale: float = 0.0) -> Dict[str, np.ndarray]:
+                        in_ch=C, in_hw=H, strides=STRIDES, bias_scale: float = 0.0,
+                        in_w: Optional[int] = None) -> Dict[str, np.ndarray]:
     """Variable names / layouts of auto_pose/ae/encoder.py:43-66 (conv kernels HWIO, dense [in,out]).
     TF zero-initialises biases; ``bias_scale`` > 0 draws small random biases so that parity tests
-    actually exercise the bias path."""
+    actually exercise the bias path.  ``in_w``: crop width when it differs from the height ``in_hw``."""
     rng = np.random.RandomState(seed)
     p: Dict[str, np.ndarray] = {}
-    cin, hw = in_ch, in_hw
+    cin, hh, ww = in_ch, in_hw, in_hw if in_w is None else in_w
     for i, (f, s) in enumerate(zip(num_filters, strides)):
         name = "conv2d" if i == 0 else f"conv2d_{i}"
         p[f"{name}/kernel"] = glorot_uniform(rng, (ksize, ksize, cin, f))
         p[f"{name}/bias"] = (bias_scale * rng.standard_normal(f)).astype(np.float32)
-        cin, hw = f, hw // s
-    p["dense/kernel"] = glorot_uniform(rng, (hw * hw * cin, latent))
+        cin, hh, ww = f, hh // s, ww // s
+    p["dense/kernel"] = glorot_uniform(rng, (hh * ww * cin, latent))
     p["dense/bias"] = (bias_scale * rng.standard_normal(latent)).astype(np.float32)
     return p
 
@@ -108,18 +109,19 @@ def make_decoder_params(seed: int = 43, num_filters=NUM_FILTER, ksize=KSIZE, lat
     return p
 
 
-def make_crops_u8(seed: int, batch: int, hw: int = H, ch: int = C, structured: bool = True) -> np.ndarray:
+def make_crops_u8(seed: int, batch: int, hw: int = H, ch: int = C, structured: bool = True, w: Optional[int] = None) -> np.ndarray:
     """Synthetic BGR crops, NHWC uint8 (auto_pose/ae/ae_factory.py:133 placeholder shape).  structured=True draws a
     different coarse random pattern per crop (8x8 blocks + pixel noise) so that the latents -- and therefore the
     matched codebook rows -- differ from crop to crop; structured=False is i.i.d. U{0..255} (every crop then encodes
-    to almost the same latent)."""
+    to almost the same latent).  ``w``: crop width when it differs from the height ``hw``."""
     rng = np.random.RandomState(seed)
+    w = hw if w is None else w
     if not structured:
-        return rng.randint(0, 256, size=(batch, hw, hw, ch), dtype=np.uint8)
-    cells = max(hw // 16, 1)
-    coarse = rng.randint(0, 256, size=(batch, cells, cells, ch)).astype(np.int32)
-    img = np.repeat(np.repeat(coarse, hw // cells, axis=1), hw // cells, axis=2)
-    img = img + rng.randint(-40, 41, size=(batch, hw, hw, ch))
+        return rng.randint(0, 256, size=(batch, hw, w, ch), dtype=np.uint8)
+    cells, cells_w = max(hw // 16, 1), max(w // 16, 1)
+    coarse = rng.randint(0, 256, size=(batch, cells, cells_w, ch)).astype(np.int32)
+    img = np.repeat(np.repeat(coarse, hw // cells, axis=1), w // cells_w, axis=2)
+    img = img + rng.randint(-40, 41, size=(batch, hw, w, ch))
     return np.clip(img, 0, 255).astype(np.uint8)
 
 
@@ -302,13 +304,15 @@ def bootstrapped_l2(x: torch.Tensor, target: torch.Tensor, bootstrap_ratio: int 
 
 def ae_forward_loss(x: np.ndarray, target: np.ndarray, enc: Dict[str, np.ndarray], dec: Dict[str, np.ndarray],
                     dtype: torch.dtype = torch.float32, bootstrap_ratio: int = BOOTSTRAP_RATIO,
-                    with_grads: bool = False, device: str = "cpu"):
+                    with_grads: bool = False, device: str = "cpu", strides=None):
     """encode -> decode -> bootstrapped L2 (auto_pose/ae/ae.py:42-53 with NORM_REGULARIZE=0, VARIATIONAL=0).
     Returns (loss, reconstruction, grads-dict or None) as numpy.  device="cuda" evaluates the same graph on the GPU (float64
-    only), which makes the reference affordable at training batch sizes."""
+    only), which makes the reference affordable at training batch sizes.  ``strides``: the encoder's, one per conv (default: the
+    template's for as many convs as ``enc`` has)."""
     _check_device(dtype, device)
     tp = {k: _t(v, dtype, device).requires_grad_(with_grads) for k, v in {**enc, **dec}.items()}
-    strides = STRIDES[:sum(1 for k in enc if k.startswith("conv2d") and k.endswith("kernel"))]
+    if strides is None:
+        strides = STRIDES[:_n_convs(enc)]
     hw = x.shape[1]
     with torch.set_grad_enabled(with_grads):
         h = _t(x, dtype, device)
@@ -325,16 +329,21 @@ def ae_forward_loss(x: np.ndarray, target: np.ndarray, enc: Dict[str, np.ndarray
     return float(loss.item()), rec.detach().cpu().numpy(), grads
 
 
+def _n_convs(enc: Dict[str, np.ndarray]) -> int:
+    return sum(1 for k in enc if k.startswith("conv2d") and k.endswith("kernel"))
+
+
 def relu_margin(x: np.ndarray, enc: Dict[str, np.ndarray], dec: Dict[str, np.ndarray], device: str = "cpu",
-                latent: Optional[np.ndarray] = None) -> float:
+                latent: Optional[np.ndarray] = None, strides=None) -> float:
     """Smallest |pre-activation| over every ReLU unit of encoder + decoder, in float64.  A unit closer to zero than fp32
     rounding can land on either side of the ReLU in any fp32 implementation (TF included), which changes its gradient
     path discretely; gradient parity tests pick inputs whose margin is comfortably above that.  ``latent``: the decoder's
-    input when it is not the encoder's z (the sampled z of the variational AE)."""
+    input when it is not the encoder's z (the sampled z of the variational AE).  ``strides``: as in ae_forward_loss."""
     dt = torch.float64
     tp = {k: _t(v, dt, device) for k, v in {**enc, **dec}.items()}
-    n_enc = sum(1 for k in enc if k.startswith("conv2d") and k.endswith("kernel"))
-    strides = STRIDES[:n_enc]
+    n_enc = _n_convs(enc)
+    if strides is None:
+        strides = STRIDES[:n_enc]
     m = float("inf")
     with torch.no_grad():
         h = _t(x, dt, device)
