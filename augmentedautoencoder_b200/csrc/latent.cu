@@ -74,9 +74,10 @@ __global__ void __launch_bounds__(kThreads) latent_kernel(LatentArgs a, int back
   }
   if (backward) {
     if (threadIdx.x == 0 && a.loss) {
+      // two graph ops per term (reg_loss * w, then loss + ...): the _rn intrinsics keep nvcc from contracting them into an FMA
       float l = *a.loss;
-      if (a.w_n > 0.f) l += a.sums[1] * a.w_n;
-      if (a.w_v != 0.f) l += a.sums[0] * a.w_v;
+      if (a.w_n > 0.f) l = __fadd_rn(l, __fmul_rn(a.sums[1], a.w_n));
+      if (a.w_v != 0.f) l = __fadd_rn(l, __fmul_rn(a.sums[0], a.w_v));
       *a.loss = l;
     }
     return;

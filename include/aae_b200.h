@@ -322,7 +322,8 @@ AAE_API int aae_trainer_set_state(aae_trainer* h, int which, int layer, const fl
                                   const float* bias_m_any, const float* bias_v_any, void* stream);
 AAE_API int aae_trainer_set_global_step(aae_trainer* h, int64_t step);
 /* The latent terms of AE.loss (auto_pose/ae/ae.py:43-53): loss = reconstr_loss, + reg_loss * norm_regularize if that is > 0,
- * + kl_div_loss * variational if that is non-zero, fp32 adds in this order (auto_pose/ae/encoder.py:82-100):
+ * + kl_div_loss * variational if that is non-zero, in this order, each term as TF's two fp32 ops (a rounded product, then a
+ * rounded add; no fused multiply-add) (auto_pose/ae/encoder.py:82-100):
  *   reg_loss    = mean_b | ||z_b|| - 1 |                        (on z; a row with ||z|| = 0 is outside the contract)
  *   kl_div_loss = mean_{b,j} KL(N(z, q_sigma) || N(0, 1))
  * variational > 0 also feeds the decoder sampled_z = z + q_sigma * eps (auto_pose/ae/ae_factory.py:58), with eps ONE scalar

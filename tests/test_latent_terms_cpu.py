@@ -67,6 +67,102 @@ def test_latent_term_gradients_match_central_differences():
     LO.norm_reg_loss(zz).backward()
     n = torch.linalg.vector_norm(z, dim=1, keepdim=True)
     assert torch.allclose(zz.grad, torch.sign(n - 1) * z / (n * B), rtol=1e-12)
+    # the whole graph with both heads and both terms (vae_forward_loss with mask_head): every one of its 16 gradients (24 at the
+    # template's depth), keyed by the TF names of that graph, against central differences of the float64 loss at sampled entries
+    x, y, ep, dp, head, mhead = _small_graph()
+    kw = dict(head=head, mask_head=mhead, variational=0.7, norm_regularize=0.4, eps=0.8, dtype=torch.float64, bootstrap_ratio=1)
+    _, _, g = LO.vae_forward_loss(x, y, ep, dp, with_grads=True, **kw)
+    assert len(g) == 16 and sorted(g) == sorted(_small_graph_names())
+    var = {**ep, **dp}
+    var = {("dense_2" + k[7:] if k.startswith("dense_1/") else "conv2d_4" + k[8:] if k.startswith("conv2d_3/") else k): v.astype(np.float64)
+           for k, v in var.items()}
+    var.update({"dense_1/kernel": head[0].astype(np.float64), "dense_1/bias": head[1].astype(np.float64),
+                "conv2d_3/kernel": mhead[0].astype(np.float64), "conv2d_3/bias": mhead[1].astype(np.float64)})
+    assert sorted(var) == sorted(g)
+
+    def loss_of(v):
+        e = {k: v[k] for k in ep}
+        d = {("dense_1" + k[7:] if k.startswith("dense_2/") else "conv2d_3" + k[8:] if k.startswith("conv2d_4/") else k): v[k]
+             for k in v if k not in ep and k not in ("dense_1/kernel", "dense_1/bias", "conv2d_3/kernel", "conv2d_3/bias")}
+        return LO.vae_forward_loss(x, y, e, d, **{**kw, "head": (v["dense_1/kernel"], v["dense_1/bias"]),
+                                                  "mask_head": (v["conv2d_3/kernel"], v["conv2d_3/bias"])})[0]
+    rng = np.random.RandomState(0)
+    h = 1e-6
+    for name in sorted(var):
+        for i in rng.choice(var[name].size, min(4, var[name].size), replace=False):
+            old = var[name].flat[i]
+            var[name].flat[i] = old + h
+            fp = loss_of(var)
+            var[name].flat[i] = old - h
+            fm = loss_of(var)
+            var[name].flat[i] = old
+            want = (fp - fm) / (2 * h)
+            assert abs(g[name].flat[i] - want) <= 1e-6 * max(abs(want), 1e-3), (name, i, g[name].flat[i], want)
+
+
+def _small_graph():
+    """16x16 input, encoder filters (4, 8), latent 8, with a sigma head and a mask head: every variable of the graph with both heads
+    at a size where central differences of the whole loss are cheap."""
+    from oracle import aae_oracle as O
+    from oracle import mask_oracle as MO
+    geo = dict(num_filters=(4, 8), strides=(2, 2), latent=8, bias_scale=0.1)
+    ep = O.make_encoder_params(5, in_hw=16, **geo)
+    dp = O.make_decoder_params(6, out_hw=16, n_encoder_convs=2, **geo)
+    rng = np.random.RandomState(7)
+    head = ((0.3 * rng.standard_normal((128, 8))).astype(np.float32), (0.1 * rng.standard_normal(8)).astype(np.float32))
+    mhead = MO.make_mask_head(8, 4, bias_scale=0.1)
+    x = rng.rand(2, 16, 16, 3).astype(np.float32)
+    y = rng.rand(2, 16, 16, 3).astype(np.float32)
+    y[rng.rand(2, 16, 16) < 0.3] = 0.0                   # background pixels: the mask target takes both values
+    return x, y, ep, dp, head, mhead
+
+
+def _small_graph_names():
+    """TF's names for _small_graph's graph with both heads: the sigma head is dense_1 and the decoder dense dense_2; the mask head
+    is conv2d_3 (created before the output conv) and the output conv conv2d_4"""
+    layers = ["conv2d", "conv2d_1", "dense", "dense_1", "dense_2", "conv2d_2", "conv2d_3", "conv2d_4"]
+    return [l + "/" + p for l in layers for p in ("kernel", "bias")]
+
+
+@pytest.mark.parametrize("terms", [(0.0, 0.0), (0.3, 0.0), (0.0, 0.4), (0.3, 0.4)])
+def test_vae_oracle_without_the_mask_head_is_unchanged(terms):
+    """vae_forward_loss without mask_head: the loss and gradients of the graph without the mask head, bit for bit -- with the terms
+    off, aae_oracle.ae_forward_loss; with them on, that reconstruction loss plus the weighted terms composed in the reference's
+    order, on the sampled z."""
+    from oracle import aae_oracle as O
+    x, y, ep, dp, head, _ = _small_graph()
+    variational, norm = terms
+    loss, t, g = LO.vae_forward_loss(x, y, ep, dp, head=head, variational=variational, norm_regularize=norm, eps=0.8,
+                                     dtype=torch.float64, with_grads=True)
+    assert len(g) == (14 if variational else 12) and not any(k.startswith("conv2d_4/") for k in g)
+    if not variational and not norm:
+        want, _, gw = O.ae_forward_loss(x, y, ep, dp, dtype=torch.float64, with_grads=True)
+        assert loss == want and all(np.array_equal(g[k], gw[k]) for k in gw)
+        return
+    tp = {k: torch.from_numpy(v).double() for k, v in dp.items()}
+    zin = torch.from_numpy(t["sampled_z"])
+    rec = O.decoder_layers(zin, tp, out_hw=16, strides=(2, 2), n_encoder_convs=2)[-1]
+    want = O.bootstrapped_l2(rec, torch.from_numpy(y).double(), 4)
+    if norm:
+        want = want + t["reg"] * norm
+    if variational:
+        want = want + t["kl"] * variational
+    assert loss == float(want)
+
+
+def test_vae_oracle_with_the_mask_head_and_the_terms_off_is_the_mask_oracle():
+    """vae_forward_loss with mask_head and VARIATIONAL = NORM_REGULARIZE = 0 equals mask_oracle.mask_forward_loss: the same loss and
+    the same 14 gradients under the same names, bit for bit"""
+    from oracle import mask_oracle as MO
+    x, y, ep, dp, head, mhead = _small_graph()
+    loss, _, g = LO.vae_forward_loss(x, y, ep, dp, mask_head=mhead, dtype=torch.float64, with_grads=True)
+    want, _, _, gw = MO.mask_forward_loss(x, y, ep, dp, mhead, dtype=torch.float64, with_grads=True)
+    assert loss == want and sorted(g) == sorted(gw) and len(g) == 14
+    assert all(np.array_equal(g[k], gw[k]) for k in gw)
+    assert "conv2d_3/kernel" in g and g["conv2d_3/kernel"].shape == (5, 5, 4, 1) and g["conv2d_4/kernel"].shape == (5, 5, 4, 3)
+    # the sigma head given but VARIATIONAL 0: still the mask oracle (the head is not part of that loss)
+    loss2, _, g2 = LO.vae_forward_loss(x, y, ep, dp, head=head, mask_head=mhead, dtype=torch.float64, with_grads=True)
+    assert loss2 == want and all(np.array_equal(g2[k], gw[k]) for k in gw) and len(g2) == 14
 
 
 def _cfg(variational, norm_regularize=0.0):

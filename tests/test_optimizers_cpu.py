@@ -144,3 +144,31 @@ def test_proximal_adagrad_rounds_differently_from_adagrad():
     tol = np.spacing(np.maximum(np.abs(a), np.abs(b))).astype(np.float64) + 2.0 ** -22 * np.abs(step_a)
     assert np.all(np.abs(a.astype(np.float64) - b) <= tol)
     assert not np.array_equal(a, b) and np.abs(step_a - step_b).max() > 0
+
+
+def _round_f32(x):
+    """the float32 nearest to the rational x, ties to the even significand"""
+    from fractions import Fraction
+    r = np.float32(float(x))
+    cands = [np.nextafter(r, np.float32(-np.inf)), r, np.nextafter(r, np.float32(np.inf))]
+    return min(cands, key=lambda c: (abs(Fraction(float(c)) - x), int(np.array(c).view(np.uint32)) & 1))
+
+
+def test_fma32_rounds_once():
+    """OO.fma32 (the kernel's Adam FMAs in the replay) against the exact product-sum rounded once, on random operands of mixed
+    magnitude and on a constructed case where the float64 sum lands on a float32 midpoint: there the sum rounded twice is one ulp
+    off and fma32 is not."""
+    from fractions import Fraction
+    rng = np.random.RandomState(0)
+    n = 4000
+    a = (rng.standard_normal(n) * 2.0 ** rng.randint(-30, 10, n)).astype(np.float32)
+    b = (rng.standard_normal(n) * 2.0 ** rng.randint(-30, 10, n)).astype(np.float32)
+    c = (rng.standard_normal(n) * 2.0 ** rng.randint(-40, 10, n)).astype(np.float32)
+    got = OO.fma32(a, b, c)
+    want = np.array([_round_f32(Fraction(float(x)) * Fraction(float(y)) + Fraction(float(z))) for x, y, z in zip(a, b, c)], np.float32)
+    assert np.array_equal(got, want)
+    u = 2.0 ** -23
+    a, b, c = np.float32(1 + u), np.float32((1 - u) * 2.0 ** -24), np.float32(1 + u)     # a b + c = 1 + u + u/2 - 2^-70
+    exact = Fraction(float(a)) * Fraction(float(b)) + Fraction(float(c))
+    assert OO.fma32(a, b, c) == np.float32(1 + u) == _round_f32(exact)
+    assert np.float32(np.float64(a) * np.float64(b) + np.float64(c)) == np.float32(1 + 2 * u)    # rounded twice
