@@ -251,10 +251,11 @@ class TrainOp(Tensor):
         h = self._trainers[dev]
         out = {}
         with torch.cuda.device(dev):
+            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)     # behind the steps the caller launched on it
             for which, mod in ((0, self._ae._encoder), (1, self._ae._decoder)):
                 for i, (kn, ks, bn, bs) in enumerate(mod._var_shapes):
                     km, kv, bm, bv = self._slot_arrays(ks, bs)
-                    _lib.check(_lib.lib().aae_trainer_get_state(h, which, i, _lib.ptr(km), _lib.ptr(kv), _lib.ptr(bm), _lib.ptr(bv), None), "get_state")
+                    _lib.check(_lib.lib().aae_trainer_get_state(h, which, i, _lib.ptr(km), _lib.ptr(kv), _lib.ptr(bm), _lib.ptr(bv), stream), "get_state")
                     for name, arrs in ((kn, (km, kv)), (bn, (bm, bv))):
                         for suffix, a in zip(self._slots, arrs):
                             out[name + "/" + suffix] = a
@@ -274,6 +275,7 @@ class TrainOp(Tensor):
         h = self.trainer(device)
         used = []
         with torch.cuda.device(device):
+            stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
             for which, mod in ((0, self._ae._encoder), (1, self._ae._decoder)):
                 for i, (kn, ks, bn, bs) in enumerate(mod._var_shapes):
                     arrs = []
@@ -287,7 +289,7 @@ class TrainOp(Tensor):
                             used.append(name)
                         arrs.append(a)
                     if any(a is not None for a in arrs):
-                        _lib.check(_lib.lib().aae_trainer_set_state(h, which, i, *[_lib.ptr(a) for a in arrs], None), "set_state")
+                        _lib.check(_lib.lib().aae_trainer_set_state(h, which, i, *[_lib.ptr(a) for a in arrs], stream), "set_state")
             step = global_step
             b1p = weights.get(self._scope_prefix() + "beta1_power") if self._opt.kind == _lib.OPT_ADAM else None
             if step is None and b1p is not None and 0.0 < float(b1p) < 1.0:
@@ -301,11 +303,12 @@ class TrainOp(Tensor):
         """{variable name: gradient} from the last forward/backward (for parity tests)."""
         h = self.trainer(device)
         out = {}
+        stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream)      # behind the step the caller launched on it
         for which, mod in ((0, self._ae._encoder), (1, self._ae._decoder)):
             for i, (kn, ks, bn, bs) in enumerate(mod._var_shapes):
                 k, b = np.empty(ks, np.float32), np.empty(bs, np.float32)
                 with torch.cuda.device(device):
-                    _lib.check(_lib.lib().aae_trainer_get_grads(h, which, i, _lib.ptr(k), _lib.ptr(b), None), "get_grads")
+                    _lib.check(_lib.lib().aae_trainer_get_grads(h, which, i, _lib.ptr(k), _lib.ptr(b), stream), "get_grads")
                 out[kn], out[bn] = k, b
         return out
 

@@ -84,10 +84,11 @@ class _DeviceModule:
             dev = device if device is not None else next(iter(self._handles))
             h = self._handles[dev]
             with torch.cuda.device(dev):
+                stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)     # behind the steps the caller launched on it
                 for i, (kn, ks, bn, bs) in enumerate(self._var_shapes):
                     k = np.empty(ks, np.float32)
                     b = np.empty(bs, np.float32)
-                    _lib.check(self._get(h, i, _lib.ptr(k), _lib.ptr(b), None), "get_weights")
+                    _lib.check(self._get(h, i, _lib.ptr(k), _lib.ptr(b), stream), "get_weights")
                     self._host[kn], self._host[bn] = k, b
         if short_names:
             return {"/".join(k.split("/")[-2:]): v for k, v in self._host.items()}
@@ -95,8 +96,9 @@ class _DeviceModule:
 
     def _upload(self, dev, h):
         with torch.cuda.device(dev):
+            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)         # ahead of the forwards the caller launches on it
             for i, (kn, ks, bn, bs) in enumerate(self._var_shapes):
-                _lib.check(self._set(h, i, _lib.ptr(self._host[kn]), _lib.ptr(self._host[bn]), None), "set_weights(%s)" % kn)
+                _lib.check(self._set(h, i, _lib.ptr(self._host[kn]), _lib.ptr(self._host[bn]), stream), "set_weights(%s)" % kn)
 
     def handle(self, device):
         dev = device.index if isinstance(device, torch.device) else int(device)
@@ -288,7 +290,8 @@ class Encoder(_DeviceModule):
         for dev, h in self._handles.items():
             with torch.cuda.device(dev):
                 self._prepare(h)
-                _lib.check(self._set(h, layer, _lib.ptr(self._host[kn]), _lib.ptr(self._host[bn]), None), "set_weights(%s)" % kn)
+                _lib.check(self._set(h, layer, _lib.ptr(self._host[kn]), _lib.ptr(self._host[bn]),
+                                     C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "set_weights(%s)" % kn)
 
     def _prepare(self, h):
         if self._has_sigma_head:

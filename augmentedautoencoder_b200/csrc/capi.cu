@@ -363,6 +363,7 @@ extern "C" int aae_encoder_create(int device, const aae_net_cfg* cfg, aae_encode
     }
   }
   if (st == AAE_OK) st = cfg->precision != AAE_PREC_FP32_SIMT ? tc_encoder_create(device, cfg, &h->tc) : simt_encoder_create(h);
+  if (st == AAE_OK) st = creation_fence("aae_encoder_create");
   if (st != AAE_OK) { aae_encoder_destroy(h); return st; }
   *out = h;
   return AAE_OK;
@@ -500,7 +501,12 @@ extern "C" int aae_encoder_activation(aae_encoder* h, int layer, const float** p
   AAE_REQUIRE(layer >= 0 && layer <= (int)h->conv.size(), "layer %d out of range", layer);
   const int l = std::min(layer, (int)h->conv.size() - 1);
   DeviceGuard g(h->device);
-  if (h->tc) return tc_encoder_activation(h->tc, l, h->last_batch, ptr_dev, count, nullptr);
+  if (h->tc) {
+    // no stream argument: the forward may have run on any stream, and the unpack below runs on the legacy stream, which a
+    // non-blocking stream is not ordered against.  A device-wide wait is the only ordering that covers every caller.
+    AAE_CUDA_OK(cudaDeviceSynchronize());
+    return tc_encoder_activation(h->tc, l, h->last_batch, ptr_dev, count, nullptr);
+  }
   *ptr_dev = h->simt->out[l].p;
   *count = (int64_t)h->conv[l].out_count(h->last_batch);
   return AAE_OK;
@@ -530,6 +536,7 @@ extern "C" int aae_encoder_enable_sigma_head(aae_encoder* h) {
     if (e == cudaSuccess) e = cudaMemset(h->sig_b.p, 0, h->sig_b.n * sizeof(float));
     if (e != cudaSuccess) { set_error("sigma head: %s", cudaGetErrorString(e)); st = AAE_ERR_CUDA; }
   }
+  if (st == AAE_OK) st = creation_fence("aae_encoder_enable_sigma_head");
   if (st != AAE_OK) { h->sig_w.release(); h->sig_b.release(); h->sig_pre.release(); h->sig_partials.release(); }
   return st;
 }
@@ -599,6 +606,7 @@ extern "C" int aae_codebook_create(int device, const float* embedding_any, int64
   }
   if (st == AAE_OK && precision != AAE_PREC_FP32_SIMT)
     st = tc_codebook_create(device, h->E.p, n_rows, latent, num_cyclo, max_batch, tc_planes(precision), &h->tc);
+  if (st == AAE_OK) st = creation_fence("aae_codebook_create");
   if (st != AAE_OK) { aae_codebook_destroy(h); return st; }
   *out = h;
   return AAE_OK;
@@ -794,6 +802,7 @@ extern "C" int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decode
     ih = R.out_h; ic = R.out_c;
   }
   if (status == AAE_OK) status = cfg->precision == AAE_PREC_TC_SPLIT ? tc_decoder_create(device, cfg, false, &h->tc) : simt_decoder_create(h);
+  if (status == AAE_OK) status = creation_fence("aae_decoder_create");
   if (status != AAE_OK) { aae_decoder_destroy(h); return status; }
   *out = h;
   return AAE_OK;
@@ -955,6 +964,7 @@ extern "C" int aae_decoder_enable_mask_head(aae_decoder* h) {
       h->tc_version = 0;                 // the new plan is packed from the masters before its first use
     }
   }
+  if (st == AAE_OK) st = creation_fence("aae_decoder_enable_mask_head");
   if (st != AAE_OK) { h->mask_w.release(); h->mask_b.release(); }
   return st;
 }
@@ -1122,6 +1132,7 @@ static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_rati
     }
   }
   if (st == AAE_OK && enc->tc) st = tc_train_create(h->fenc ? h->fenc : enc->tc, h->fdec ? h->fdec : dec->tc, enc->cfg.max_batch, &h->tc);
+  if (st == AAE_OK) st = creation_fence("aae_trainer_create");
   if (st != AAE_OK) { aae_trainer_destroy(h); return st; }
   *out = h;
   return AAE_OK;

@@ -59,6 +59,17 @@ struct DeviceGuard {
 
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
+// Creators (aae_*_create*, aae_*_enable_*_head) fill what they allocate with cudaMemset / cudaMemcpy / set-up kernels on the
+// legacy default stream.  Those fills are asynchronous to the host, and a caller's non-blocking stream does not wait for the
+// legacy stream, so each creator ends here: everything it issued is complete on the device when it returns, and the new
+// object can be used on any stream at once.  Creation costs milliseconds of cudaMalloc already.
+inline int creation_fence(const char* what) {
+  const cudaError_t e = cudaDeviceSynchronize();
+  if (e == cudaSuccess) return AAE_OK;
+  set_error("%s: device initialisation failed: %s", what, cudaGetErrorString(e));
+  return AAE_ERR_CUDA;
+}
+
 // Optional per-stage device timing (cudaEvents on the launching stream), read back by bench.py for the roofline lines.
 struct StageTimer {
   bool enabled = false;

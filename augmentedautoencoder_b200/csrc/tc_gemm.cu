@@ -322,6 +322,18 @@ __global__ void __launch_bounds__(256) splitk_forward_finish_kernel(const float*
 
 int dev_alloc(void** p, size_t bytes) { return tc_dev_alloc(p, bytes); }
 
+// Scratch that grows inside a stream call (first use at a larger size): zero-filled on the caller's stream.  tc_dev_alloc fills
+// on the legacy stream, which is ordered for creators only (creation_fence).  Growing frees the old buffer, and cudaFree
+// waits for the device, so the call that grows is not asynchronous; every later call at that size is.
+int scratch_grow(void** p, size_t bytes, cudaStream_t s) {
+  cudaFree(*p);
+  *p = nullptr;
+  cudaError_t e = cudaMalloc(p, bytes);
+  if (e != cudaSuccess) { *p = nullptr; set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return AAE_ERR_OOM; }
+  AAE_CUDA_OK(cudaMemsetAsync(*p, 0, bytes, s));
+  return AAE_OK;
+}
+
 bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
 }  // namespace
@@ -640,9 +652,8 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
         if (per_split * (size_t)splits > h->fwd_partial_floats) {
           const size_t want = std::min<size_t>(per_split * (size_t)splits, (size_t)32 << 20);     // at most 128 MB of partials
           if (want > h->fwd_partial_floats) {
-            cudaFree(h->fwd_partials);
-            h->fwd_partials = nullptr; h->fwd_partial_floats = 0;
-            AAE_TRY(dev_alloc((void**)&h->fwd_partials, want * sizeof(float)));
+            h->fwd_partial_floats = 0;
+            AAE_TRY(scratch_grow((void**)&h->fwd_partials, want * sizeof(float), s));
             h->fwd_partial_floats = want;
           }
           splits = (int)std::min<size_t>((size_t)splits, h->fwd_partial_floats / per_split);
@@ -687,9 +698,8 @@ int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int
   else { H = T.in_h; W = T.in_w; C = T.in_c; }
   const size_t n = (size_t)B * H * W * C;
   if (h->dbg_floats < n) {
-    cudaFree(h->dbg);
-    h->dbg = nullptr;
-    AAE_TRY(dev_alloc((void**)&h->dbg, n * sizeof(float)));
+    h->dbg_floats = 0;
+    AAE_TRY(scratch_grow((void**)&h->dbg, n * sizeof(float), s));
     h->dbg_floats = n;
   }
   with_planes(h->planes, [&](auto P) {

@@ -16,7 +16,20 @@
  *     and never aborts.  aae_last_error_string() describes the last failure on the
  *     calling thread.
  *   - handles are re-entrant per (handle, stream): no global mutable state; a handle owns
- *     its weights, packed operand copies and a private workspace sized by max_batch.
+ *     its weights, packed operand copies and a private workspace sized by max_batch.  That one
+ *     workspace serves one stream at a time: any stream, and the caller orders the hand-over from
+ *     one stream to the next (an event).  Different handles run concurrently on different streams.
+ *   - streams: every launch, fill and copy of a call goes to its `stream` and to no other, so a
+ *     non-blocking stream (which does not wait for the legacy default stream) is as good as any.
+ *     Forwards, match, losses, input-pipeline calls and the training entry points do not wait for
+ *     the device; calls that hand data to the host (*_set_weights, *_get_weights, *_range_status,
+ *     aae_trainer_get_grads, aae_trainer_{get,set}_state, the *_profile reads) wait for their own
+ *     stream only.  Two exceptions wait for the whole device: aae_encoder_activation (it takes no
+ *     stream), and a forward that has to grow a tensor-core scratch buffer (the first one at a
+ *     larger batch).
+ *   - creation is complete on return: aae_*_create* and aae_*_enable_*_head fill what they
+ *     allocate on the legacy default stream and end with one cudaDeviceSynchronize, so the new
+ *     object can be used on any stream at once.
  *   - tensor layouts follow the reference: activations NHWC float32, conv kernels HWIO,
  *     dense kernels [in,out], crops BGR uint8 or float32 in [0,1]
  *     (auto_pose/ae/ae_factory.py:133, auto_pose/ae/encoder.py:43-66).
@@ -118,7 +131,9 @@ AAE_API int aae_encoder_range_status(aae_encoder* h, void* stream);
 AAE_API int aae_encoder_range_word(aae_encoder* h, const uint32_t** word_dev);
 /* Device pointer + element count of the activation of conv layer `layer` (NHWC fp32) from the last
  * forward; layer == num_layers gives the flattened encoder_out.  For tests and for the trainer.  On an AAE_PREC_TC_FP16
- * handle this is the stored fp16 value (the only one there is), unscaled to fp32. */
+ * handle this is the stored fp16 value (the only one there is), unscaled to fp32.  The call takes no stream: on a tensor-core
+ * handle it waits for the whole device (the forward may have run on any stream), unpacks into a buffer of its own and waits
+ * again; on an AAE_PREC_FP32_SIMT handle it returns the workspace pointer, to be read behind the forward's stream. */
 AAE_API int aae_encoder_activation(aae_encoder* h, int layer, const float** ptr_dev, int64_t* count);
 
 /* Device-side stage timing for benchmarks: `enable` switches cudaEvent bracketing of the stages of the NEXT forward calls
