@@ -128,7 +128,7 @@ class _DeviceModule:
 
     def check_range(self, device=None):
         """Raises AaeError if a forward / training step launched so far on this module left the range of the split-fp16
-        tensor-core arithmetic (|activation| >= 4094; include/aae_b200.h: aae_*_range_status).  Synchronises the current
+        tensor-core arithmetic (|activation| >= 4095, or weights an optimizer step carried out of range; include/aae_b200.h: aae_*_range_status).  Synchronises the current
         stream, so the asynchronous device entry points (encode_device / decode_device) do not call it; every path that
         hands results to the host does."""
         for dev, h in self._handles.items():

@@ -163,25 +163,51 @@ int copy_any(void* dst, const void* src, size_t bytes, cudaStream_t s) {
   return AAE_OK;
 }
 
+constexpr unsigned RANGE_WEIGHT_BITS = 0xffff0000u;
+
+// " 0 2 5" for the set bits of `mask` (bit l -> l)
+void list_layers(unsigned mask, char* out, size_t cap) {
+  out[0] = '\0';
+  for (int l = 0; l < 16; ++l)
+    if (mask & (1u << l)) snprintf(out + strlen(out), cap - strlen(out), " %d", l);
+}
+
 // Run-time range guard of the tensor-core path's static fp16 scaling (DESIGN.md section 3): kernels set bits in a device word
 // instead of producing inf silently.  `peek` reads the word (the caller has synchronised the stream the work ran on), names
-// the offending layers in the error string, clears it and returns AAE_ERR_UNSUPPORTED; 0 bits -> AAE_OK.
-int range_peek(unsigned* flag_dev, const char* what, int act_layer_base, cudaStream_t s, int precision = AAE_PREC_TC_SPLIT) {
+// the offending layers in the error string, clears what it reports and returns AAE_ERR_UNSUPPORTED; nothing to report -> AAE_OK.
+// `report` selects the bits it consumes: set_weights takes the weight bits only and leaves a pending activation overflow to
+// *_range_status.  A weight bit is also added to *refused (bit l = packed layer l), the handle's record of refused weights: its
+// forwards and training steps fail (refused_check) until a clean set_weights of that layer clears the bit.
+int range_peek(unsigned* flag_dev, const char* what, cudaStream_t s, int precision, unsigned* refused, unsigned report = ~0u) {
   if (!flag_dev) return AAE_OK;
-  unsigned bits = 0;
-  AAE_CUDA_OK(cudaMemcpyAsync(&bits, flag_dev, sizeof(bits), cudaMemcpyDeviceToHost, s));
+  unsigned word = 0;
+  AAE_CUDA_OK(cudaMemcpyAsync(&word, flag_dev, sizeof(word), cudaMemcpyDeviceToHost, s));
   AAE_CUDA_OK(cudaStreamSynchronize(s));
+  const unsigned bits = word & report;
   if (bits == 0) return AAE_OK;
-  AAE_CUDA_OK(cudaMemsetAsync(flag_dev, 0, sizeof(bits), s));
-  char acts[128] = "", wts[128] = "";
-  for (int l = 0; l < 15; ++l) {
-    if (bits & (1u << l)) snprintf(acts + strlen(acts), sizeof(acts) - strlen(acts), " %d", l + act_layer_base);
-    if (bits & (1u << (16 + l))) snprintf(wts + strlen(wts), sizeof(wts) - strlen(wts), " %d", l);
-  }
+  const unsigned rest = word & ~bits;
+  AAE_CUDA_OK(cudaMemcpyAsync(flag_dev, &rest, sizeof(rest), cudaMemcpyHostToDevice, s));
+  AAE_CUDA_OK(cudaStreamSynchronize(s));
+  *refused |= bits >> 16;
+  char acts[128], wts[128];
+  list_layers(bits & 0x7fffu, acts, sizeof(acts));
+  list_layers(bits >> 16, wts, sizeof(wts));
   set_error("%s: values outside the range of the %s tensor-core arithmetic (%s)%s%s%s%s%s -- use AAE_PREC_FP32_SIMT for "
             "this model", what, precision == AAE_PREC_TC_FP16 ? "fp16" : "split-fp16", precision == AAE_PREC_TC_FP16 ? "AAE_PREC_TC_FP16" : "AAE_PREC_TC_SPLIT",
-            acts[0] ? "; |activation| >= 4094 written by layer(s)" : "", acts, wts[0] ? "; |weight| >= 255.9 in layer(s)" : "", wts,
-            (bits & (1u << 15)) ? "; |latent| >= 4094 at the decoder input" : "");
+            acts[0] ? "; |activation| >= 4095 written by layer(s)" : "", acts,
+            wts[0] ? "; |weight| >= 255.9375 as packed (tensor-core conv1: >= 254.94, decoder convs: the merged sub-pixel weight, a "
+                     "sum of up to four 5x5 taps) in layer(s)" : "", wts,
+            (bits & (1u << 15)) ? "; |latent| >= 4095 at the decoder input" : "");
+  return AAE_ERR_UNSUPPORTED;
+}
+
+// A handle whose weights the range guard refused computes nothing: its packed operands hold infinities.
+int refused_check(unsigned refused, const char* what) {
+  if (refused == 0) return AAE_OK;
+  char wts[128];
+  list_layers(refused, wts, sizeof(wts));
+  set_error("%s: the range guard refused the weights of layer(s)%s -- set them again with values inside the tensor-core range, "
+            "or use AAE_PREC_FP32_SIMT for this model", what, wts);
   return AAE_ERR_UNSUPPORTED;
 }
 
@@ -208,6 +234,7 @@ struct aae_encoder {
   // operands) records the w_version it was built from and is rebuilt just before its next use when the two differ.
   uint64_t w_version = 1;
   uint64_t tc_version = 1;  // the plan's operands start as zeros, like the masters
+  unsigned refused = 0;     // bit l: the range guard refused layer l's weights (range_peek); forwards fail until it is set cleanly
   StageTimer timer;
 };
 
@@ -220,6 +247,7 @@ struct aae_decoder {
   SimtDecoder* simt = nullptr;  // fp32 CUDA-core workspace (AAE_PREC_FP32_SIMT)
   TcDecoder* tc = nullptr;      // tensor-core execution plan (AAE_PREC_TC_SPLIT, forward only)
   uint64_t w_version = 1, tc_version = 1;   // see aae_encoder
+  unsigned refused = 0;                     // see aae_encoder; the mask head is packed with the output conv: bit num_layers
   // mask head of AUXILIARY_MASK (aae_decoder_enable_mask_head; empty until then): kernel [k,k,Cin,1] and bias [1] of a conv over
   // the output layer's input.  The kernels run it joined with the output conv along Cout (DESIGN.md section 3).
   DevBuf mask_w, mask_b;
@@ -412,7 +440,8 @@ extern "C" int aae_encoder_set_weights(aae_encoder* h, int layer, const float* k
   if (h->tc) AAE_TRY(tc_encoder_set_bias(h->tc, layer, b.p));
   if (tc_current) h->tc_version = h->w_version;   // this layer is packed again; a plan behind by an optimizer step stays behind
   AAE_CUDA_OK(cudaStreamSynchronize(s));  // host source buffers may be freed by the caller on return
-  if (h->tc) AAE_TRY(range_peek(tc_encoder_range_flag(h->tc), "encoder set_weights", 0, s, h->cfg.precision));
+  if (h->tc && kernel_any) h->refused &= ~(1u << layer);   // re-packed: the guard below decides again
+  if (h->tc) AAE_TRY(range_peek(tc_encoder_range_flag(h->tc), "encoder set_weights", s, h->cfg.precision, &h->refused, RANGE_WEIGHT_BITS));
   return AAE_OK;
 }
 
@@ -425,7 +454,7 @@ extern "C" int aae_encoder_range_word(aae_encoder* h, const uint32_t** word_dev)
 extern "C" int aae_encoder_range_status(aae_encoder* h, void* stream) {
   AAE_REQUIRE(h != nullptr, "encoder handle is null");
   DeviceGuard g(h->device);
-  return h->tc ? range_peek(tc_encoder_range_flag(h->tc), "encoder", 0, (cudaStream_t)stream, h->cfg.precision) : AAE_OK;
+  return h->tc ? range_peek(tc_encoder_range_flag(h->tc), "encoder", (cudaStream_t)stream, h->cfg.precision, &h->refused) : AAE_OK;
 }
 
 extern "C" int aae_encoder_get_weights(aae_encoder* h, int layer, float* kernel_any, float* bias_any, void* stream) {
@@ -480,6 +509,7 @@ static int encoder_forward(aae_encoder* h, const void* crops, int src_u8, int B,
   AAE_REQUIRE(h != nullptr, "encoder handle is null");
   AAE_REQUIRE(crops != nullptr && z_out != nullptr, "null tensor pointer");
   AAE_REQUIRE(B >= 1 && B <= h->cfg.max_batch, "batch %d outside [1, max_batch=%d]", B, h->cfg.max_batch);
+  AAE_TRY(refused_check(h->refused, "encoder forward"));
   DeviceGuard g(h->device);
   h->last_batch = B;
   if (h->tc) {
@@ -848,14 +878,15 @@ extern "C" int aae_decoder_set_weights(aae_decoder* h, int layer, const float* k
   else if (h->tc) AAE_TRY(tc_decoder_pack_weights(h->tc, layer, kernel_any ? w.p : nullptr, bias_any ? b.p : nullptr, s));
   if (tc_current) h->tc_version = h->w_version;   // see aae_encoder_set_weights
   AAE_CUDA_OK(cudaStreamSynchronize(s));
-  if (h->tc) AAE_TRY(range_peek(tc_decoder_range_flag(h->tc), "decoder set_weights", 0, s));
+  if (h->tc && kernel_any) h->refused &= ~(1u << std::min(layer, nl));   // see aae_encoder_set_weights (the head: the output layer)
+  if (h->tc) AAE_TRY(range_peek(tc_decoder_range_flag(h->tc), "decoder set_weights", s, AAE_PREC_TC_SPLIT, &h->refused, RANGE_WEIGHT_BITS));
   return AAE_OK;
 }
 
 extern "C" int aae_decoder_range_status(aae_decoder* h, void* stream) {
   AAE_REQUIRE(h != nullptr, "decoder handle is null");
   DeviceGuard g(h->device);
-  return h->tc ? range_peek(tc_decoder_range_flag(h->tc), "decoder", 0, (cudaStream_t)stream) : AAE_OK;
+  return h->tc ? range_peek(tc_decoder_range_flag(h->tc), "decoder", (cudaStream_t)stream, AAE_PREC_TC_SPLIT, &h->refused) : AAE_OK;
 }
 
 extern "C" int aae_decoder_get_weights(aae_decoder* h, int layer, float* kernel_any, float* bias_any, void* stream) {
@@ -929,6 +960,7 @@ static int decoder_forward_impl(aae_decoder* h, const float* z, int B, float* x_
 extern "C" int aae_decoder_forward(aae_decoder* h, const float* z_dev, int batch, float* x_out_dev, void* stream) {
   AAE_REQUIRE(h != nullptr && z_dev != nullptr && x_out_dev != nullptr, "null argument");
   AAE_REQUIRE(batch >= 1 && batch <= h->cfg.max_batch, "batch %d outside [1, max_batch=%d]", batch, h->cfg.max_batch);
+  AAE_TRY(refused_check(h->refused, "decoder forward"));
   DeviceGuard g(h->device);
   if (h->tc) {
     AAE_TRY(decoder_sync_tc(h, (cudaStream_t)stream));
@@ -976,6 +1008,7 @@ extern "C" int aae_decoder_forward_mask(aae_decoder* h, const float* z_dev, int 
     set_error("forward_mask: the decoder has no mask head (aae_decoder_enable_mask_head)");
     return AAE_ERR_UNSUPPORTED;
   }
+  AAE_TRY(refused_check(h->refused, "decoder forward"));
   DeviceGuard g(h->device);
   if (h->tc) {
     AAE_TRY(decoder_sync_tc(h, (cudaStream_t)stream));
@@ -1595,7 +1628,8 @@ static int trainer_fwd_bwd(aae_trainer* h, const float* x, const float* y, int B
 static int trainer_check(aae_trainer* h, const float* x, const float* y, int B, float* loss) {
   AAE_REQUIRE(h && x && y && loss, "null argument");
   AAE_REQUIRE(B >= 1 && B <= h->enc->cfg.max_batch, "batch %d outside [1, max_batch=%d]", B, h->enc->cfg.max_batch);
-  return AAE_OK;
+  AAE_TRY(refused_check(h->enc->refused, "training step (encoder)"));
+  return refused_check(h->dec->refused, "training step (decoder)");
 }
 
 extern "C" int aae_trainer_forward_backward(aae_trainer* h, const float* x_dev, const float* y_dev, int batch, float* loss_out_dev,

@@ -102,6 +102,8 @@ enum GatherMode : int {
 
 enum Activation : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SIGMOID = 2 };
 
+constexpr float TC_F16_OVERFLOW = 65520.f;   // smallest magnitude that rounds to infinity in fp16 (round to nearest even)
+
 struct IGemmParams {
   // gathered tensor (NHWC): stored dims
   const void* src;      // float* (or uint8_t* when src_u8)
@@ -128,6 +130,10 @@ struct IGemmParams {
   __half* split_lo;
   float split_scale;
   int split_s2d;
+  // run-time range guard of that output (tc_plan.cuh): a value whose magnitude times split_scale is not below
+  // TC_F16_OVERFLOW (inf and NaN included) sets range_bit in *range_flag
+  unsigned* range_flag;
+  unsigned range_bit;
   // depth-to-space output (FWD): C column n = (cls, co), cls = (py, px); row m = (b, i, j) on the PH x PW grid is written
   // to pixel (2i+py, 2j+px) of a plain NHWC tensor [B, 2PH, 2PW, N/4]  (sub-pixel form of upsample-x2 + conv5x5)
   int d2s_out;

@@ -288,12 +288,15 @@ __global__ void __launch_bounds__(NT) igemm_f32_kernel(const IGemmParams p) {
               (((pc.ph & 1) << 1) | (pc.pw & 1)) * p.N + n;
         }
         __half h[4], l[4];
+        bool out_of_range = false;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
           const float x = v[j] * p.split_scale;
+          out_of_range |= !(fabsf(x) < TC_F16_OVERFLOW);
           h[j] = __float2half_rn(x);
           l[j] = __float2half_rn(x - __half2float(h[j]));
         }
+        if (out_of_range && p.range_flag != nullptr) atomicOr(p.range_flag, p.range_bit);
         uint2 hv, lv;
         hv.x = (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16);
         hv.y = (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16);

@@ -633,6 +633,7 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
     p.M = B * p.PH * p.PW; p.K = p.KH * p.KW * p.SC;
     p.k_per_split = (int)ceil_div(p.K, 16) * 16;
     p.split_hi = h->layers[0].in.hi; p.split_lo = h->layers[0].in.lo; p.split_scale = ACT_SCALE; p.split_s2d = 1;
+    p.range_flag = h->range_flag; p.range_bit = 1u;   // bit 0: conv1's activation, as on the tensor-core conv1
     AAE_TRY(launch_igemm(p, GATHER_FWD, s));
   }
   timer->mark(s);

@@ -49,12 +49,11 @@ struct TcGemmParams {
   __half* out_lo;
   float* out_f32;        // OUT_F32: [splits, M, N]
   // run-time range guard of the static fp16 scaling: an output whose magnitude times out_scale would round to fp16 infinity
-  // (|activation| >= 4094 at scale 16) sets `range_bit` in *range_flag instead of producing inf/garbage silently
+  // (|activation| >= 4095 at scale 16; TC_F16_OVERFLOW, common.cuh) sets `range_bit` in *range_flag instead of producing
+  // inf/garbage silently
   unsigned* range_flag;
   unsigned range_bit;
 };
-
-constexpr float TC_F16_OVERFLOW = 65520.f;   // smallest magnitude that rounds to infinity in fp16 (round to nearest even)
 
 
 

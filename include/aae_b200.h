@@ -116,14 +116,26 @@ AAE_API int aae_encoder_get_weights(aae_encoder* h, int layer, float* kernel_any
 AAE_API int aae_encoder_forward_u8(aae_encoder* h, const uint8_t* crops_dev, int batch, float* z_out_dev, void* stream);
 /* crops NHWC float32 in [0,1] (the placeholder of auto_pose/ae/ae_factory.py:133). */
 AAE_API int aae_encoder_forward_f32(aae_encoder* h, const float* crops_dev, int batch, float* z_out_dev, void* stream);
-/* Run-time range guard of AAE_PREC_TC_SPLIT.  The tensor-core path stores activations as 16*x and weights as 256*w in fp16
- * (hi, lo) pairs, i.e. it needs |activation| < 4094 and |weight| < 255.9 -- true for every trained AAE we know of, but not a
- * law.  A value outside that range is never turned into inf/garbage silently: the kernels record it, aae_*_set_weights
- * fails with AAE_ERR_UNSUPPORTED when a weight is out of range, and this call (which synchronises `stream`) reports -- and
- * clears -- an activation overflow of any forward / training step launched on the handle so far, naming the layers in
- * aae_last_error_string().  The forward entry points stay asynchronous; callers that read results on the host
- * (Session.run, Codebook.nearest_rotation) call this after their own synchronisation.  AAE_PREC_FP32_SIMT handles have no
- * such limit and always return AAE_OK.  (The reference's fp32 TF graph has no counterpart: auto_pose/ae/encoder.py:37-68.) */
+/* Run-time range guard of the tensor-core precisions.  The tensor-core path stores activations as 16*x and weights as 256*w in
+ * fp16 (hi, lo) pairs, and fp16 rounds magnitudes from 65520 up to infinity.  So it needs, exactly:
+ *   - |activation| < 4095 for every conv activation (the fp32 conv1 of geometries without the tensor-core conv1 included) and
+ *     for the latent fed to the decoder;
+ *   - |weight| < 255.9375 for encoder conv2..L, the dense layer and the decoder's dense_1;
+ *   - |weight| < 254.94140625 (65520 * 255 / 65536) for a conv1 on the tensor cores: its uint8 operand is packed at
+ *     256 * 256/255 whichever feed the caller uses; a conv1 on the fp32 kernel has no weight limit;
+ *   - |merged weight| < 255.9375 for the decoder's convs and output conv: they run in sub-pixel form, where each weight is the
+ *     sum of up to four taps of the 5x5 kernel, so taps below 64 can already be refused.
+ * That holds for every trained AAE we know of, but it is not a law.  A value outside that range is never turned into
+ * inf/garbage silently: the kernels record it (inf and NaN count as outside), and
+ *   - aae_*_set_weights fails with AAE_ERR_UNSUPPORTED when a weight of the layer is out of range.  The handle keeps the refusal:
+ *     its forwards and training steps fail with AAE_ERR_UNSUPPORTED, naming the layer, until a set_weights of that layer with
+ *     a kernel in range.  set_weights reports weights only; an activation overflow of an earlier forward stays for this call;
+ *   - this call (which synchronises `stream`) reports -- and clears -- an activation overflow of any forward / training step
+ *     launched on the handle so far, and a weight that an optimizer step carried out of range (kept as a refusal like the
+ *     above), naming the layers in aae_last_error_string(): activations by conv layer (0-based), weights by set_weights layer.
+ * The forward entry points stay asynchronous; callers that read results on the host (Session.run, Codebook.nearest_rotation)
+ * call this after their own synchronisation.  AAE_PREC_FP32_SIMT handles have no such limit and always return AAE_OK.  (The
+ * reference's fp32 TF graph has no counterpart: auto_pose/ae/encoder.py:37-68.) */
 AAE_API int aae_encoder_range_status(aae_encoder* h, void* stream);
 /* Device address of the guard's 32-bit word (NULL for AAE_PREC_FP32_SIMT handles): streaming callers copy it to pinned host
  * memory behind their own results on their own stream and call aae_encoder_range_status only when it is non-zero, so the
@@ -200,14 +212,16 @@ AAE_API int aae_decoder_destroy(aae_decoder* h);
 AAE_API int aae_decoder_set_weights(aae_decoder* h, int layer, const float* kernel_any, const float* bias_any, void* stream);
 AAE_API int aae_decoder_get_weights(aae_decoder* h, int layer, float* kernel_any, float* bias_any, void* stream);
 AAE_API int aae_decoder_forward(aae_decoder* h, const float* z_dev, int batch, float* x_out_dev, void* stream);
-/* Same contract as aae_encoder_range_status for the decoder (dense_1 counts as layer 0; the latent fed to the decoder is
- * covered too). */
+/* Same contract as aae_encoder_range_status for the decoder: activations and weights both by set_weights layer (dense_1 is
+ * layer 0, the hidden convs 1..num_layers-1); the latent fed to the decoder is reported on its own.  The output conv writes
+ * fp32 and has no activation limit.  The mask head's kernel is packed inside the output conv (aae_decoder_enable_mask_head): a
+ * refusal of either names layer num_layers, and a clean set_weights of either (num_layers or num_layers + 1) lifts it. */
 AAE_API int aae_decoder_range_status(aae_decoder* h, void* stream);
 /* Mask head of AUXILIARY_MASK: xmask = sigmoid(conv(x_in, W, padding SAME) + b) with x_in the output conv's input
  * (auto_pose/ae/decoder.py:68-75).  Allocates W [k, k, Cin, 1] and b [1], zero until set; calling it again is a no-op.
  * Afterwards layer num_layers + 1 of aae_decoder_set_weights / get_weights addresses the head (TF names: the head is
  * "conv2d_<k>" and the output conv "conv2d_<k+1>", k = encoder convs + decoder hidden convs), the range guard covers its
- * kernel, and a trainer created over the handle trains it (reconstruction loss + mask loss; get_grads / get_state / set_state
+ * kernel (a refusal names layer num_layers, aae_decoder_range_status), and a trainer created over the handle trains it (reconstruction loss + mask loss; get_grads / get_state / set_state
  * with which = 1, layer = num_layers + 1).  The kernels run the head and the output conv as ONE conv with C + 1 output
  * channels, so x is unchanged by it.  A live trainer over the handle: AAE_ERR_UNSUPPORTED (enable the head first). */
 AAE_API int aae_decoder_enable_mask_head(aae_decoder* h);
