@@ -28,12 +28,25 @@ def build_dataset(dataset_path, args):
 
 class Queue(object):
     """Stand-in for auto_pose/ae/queue.py:14-74 (TF FIFOQueue fed by Python threads): ``x`` / ``y`` evaluate to the next
-    (augmented input, reconstruction target) batch from ``dataset.batch(batch_size)`` or a user-supplied callable."""
+    (augmented input, reconstruction target) batch from ``dataset.batch(batch_size)`` or a user-supplied callable.
+
+    Until ``start(session)`` every run makes its batch synchronously.  ``start`` with the default source runs a producer thread
+    (batch_producer.BatchProducer) that makes batches ahead on its own CUDA stream into QUEUE_SIZE device slots, from the
+    training set kept on the device (``Dataset.upload``; ``start`` uploads it if it is not there yet).  The batches are the
+    ones repeated synchronous calls would make, in the same order and with the same bits.  NUM_THREADS is accepted and does not
+    change them: one thread makes every batch.  While the producer runs it is the only user of numpy's global random stream.
+    ``stop`` joins the thread (batches made ahead are dropped); start / stop can be repeated.  With a ``source`` callable,
+    start / stop do nothing.  A ``Session.run_device`` fetch of ``x`` / ``y`` of a started queue is the slot itself: valid
+    until the next run that pulls a batch."""
 
     def __init__(self, dataset, num_threads, queue_size, batch_size, source=None):
         self._dataset = dataset
         self._batch_size = batch_size
+        self._num_threads = num_threads
+        self._queue_size = queue_size
+        self._custom_source = source is not None
         self._source = source or (lambda n: dataset.batch(n))
+        self._producer = None
         shape = (None,) + tuple(dataset.shape)
         self.x = Tensor("queue_x", shape, np.float32, lambda ctx: self._pull(ctx)[0])
         self.y = Tensor("queue_y", shape, np.float32, lambda ctx: self._pull(ctx)[1])
@@ -43,15 +56,23 @@ class Queue(object):
         one.  The batch lives in the run's own memo (not keyed by ``id(ctx)``: a freed context's address is reused)."""
         key = ("queue_batch", id(self))            # the Queue outlives every RunContext, so its id is stable
         if key not in ctx.memo:
-            x, y = self._source(self._batch_size)
-            ctx.memo[key] = (S.to_device_input(x, ctx.session.device), S.to_device_input(y, ctx.session.device))
+            if self._producer is not None:
+                ctx.memo[key] = self._producer.pull()
+            else:
+                x, y = self._source(self._batch_size)
+                ctx.memo[key] = (S.to_device_input(x, ctx.session.device), S.to_device_input(y, ctx.session.device))
         return ctx.memo[key]
 
     def start(self, session):
-        pass
+        if self._custom_source or self._producer is not None:
+            return
+        from .batch_producer import BatchProducer
+        self._producer = BatchProducer(self._dataset, self._batch_size, self._queue_size, session.device)
 
     def stop(self, session):
-        pass
+        if self._producer is not None:
+            self._producer.close()
+            self._producer = None
 
 
 def build_queue(dataset, args, source=None):

@@ -292,7 +292,10 @@ class Augmenter(object):
                 "cols": torch.from_numpy(nearest_cells(self.w, self.low[1])).to(dev),
                 "to_float": torch.from_numpy((np.arange(256) / 255.).astype(np.float32)).to(dev),     # batch_x / 255. then the float32 feed
                 "taps": gaussian_taps_q8(self.sigma).astype(np.int32) if self.sigma > 1e-3 else None,
+                # the target's float32 y / 255. as torch computes it (Dataset.batch_device), for the indexed call's y output
+                "y_to_float": torch.arange(256, dtype=torch.int32, device=dev).to(torch.uint8).to(torch.float32) / 255.0,
             }
+            torch.cuda.current_stream(dev).synchronize()    # usable from any stream (the batch producer's) from here on
         return self._dev[key]
 
     def augment_device(self, x, mask, bg, params=None, want_u8=False):
@@ -319,6 +322,24 @@ class Augmenter(object):
                                                 _lib.ptr(out_u) if out_u is not None else None, _lib.ptr(out_f),
                                                 C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "augment batch")
         return (out_f, out_u) if want_u8 else out_f
+
+    def augment_indexed(self, stacks, idx_d, idx_bg_d, geom_d, lut_d, out_f, y_out, stream, mask_batch=None, tmp=None):
+        """``augment_device`` on device-resident stacks (``aae_augment_batch_indexed``): image b is row idx_d[b] of stacks["x"] /
+        ["mask"] / ["y"] and row idx_bg_d[b] of stacks["bg"]; mask_batch (uint8 [B,H,W], e.g. an occlusion output) replaces the
+        mask rows.  Writes the float32 input into out_f and the target y / 255. into y_out; geom_d / lut_d are ``pack``'s tables on
+        the device; tmp (uint8 [B,H,W,C]) is the scratch of the geometry pass, allocated here when None.  Asynchronous on ``stream``."""
+        dev = out_f.device
+        B = int(out_f.shape[0])
+        k = self._constants(dev)
+        if tmp is None:
+            tmp = torch.empty((B, self.h, self.w, self.c), dtype=torch.uint8, device=dev)
+        taps = k["taps"]
+        _lib.check(_lib.lib().aae_augment_batch_indexed(
+            _lib.ptr(stacks["x"]), _lib.ptr(stacks["mask"]), _lib.ptr(stacks["bg"]), _lib.ptr(stacks["y"]), len(stacks["x"]),
+            len(stacks["bg"]), _lib.ptr(idx_d), _lib.ptr(idx_bg_d), _lib.ptr(mask_batch), B, self.h, self.w, self.c, _lib.ptr(geom_d),
+            _lib.ptr(lut_d), _lib.ptr(k["tab"]), _lib.ptr(k["rows"]), _lib.ptr(k["cols"]), self.low[1],
+            _lib.ptr(taps) if taps is not None else None, _lib.ptr(k["to_float"]), _lib.ptr(k["y_to_float"]), _lib.ptr(tmp), None,
+            _lib.ptr(out_f), _lib.ptr(y_out), C.c_void_p(stream.cuda_stream)), "augment batch (indexed)")
 
 
 # ----------------------------------------------------------------------------------------------------------- occlusion
@@ -430,7 +451,15 @@ class Occlusion(object):
                 "fallbacks": torch.zeros(2, dtype=torch.int32, device=dev),
                 "bank_src": None, "bank": None,
             }
+            torch.cuda.current_stream(dev).synchronize()    # usable from any stream (the batch producer's) from here on
         return self._dev[key]
+
+    def _bank(self, st, dev, bank):
+        if bank is None or bank.ndim != 3 or bank.shape[1:] != (self.h, self.w // 32):
+            raise ValueError("realistic occlusion needs an occluder bank of [n, %d, %d] words" % (self.h, self.w // 32))
+        if st["bank_src"] is not bank:                  # one upload per device and bank
+            st["bank"], st["bank_src"] = torch.from_numpy(np.ascontiguousarray(bank, np.uint32).view(np.int32)).to(dev), bank
+        return st["bank"]
 
     def apply_device(self, mask, bank=None, params=None):
         """mask: bool / uint8 CUDA tensor [B,H,W] (True = background); bank: ``load_occlusion_bank`` array (realistic step).
@@ -441,10 +470,7 @@ class Occlusion(object):
             raise ValueError("occlusion: mask of shape %s, expected [B, %d, %d]" % (tuple(mask.shape), self.h, self.w))
         st = self._state(dev)
         if self.realistic:
-            if bank is None or bank.ndim != 3 or bank.shape[1:] != (self.h, self.w // 32):
-                raise ValueError("realistic occlusion needs an occluder bank of [n, %d, %d] words" % (self.h, self.w // 32))
-            if st["bank_src"] is not bank:                  # one upload per device and bank
-                st["bank"], st["bank_src"] = torch.from_numpy(np.ascontiguousarray(bank, np.uint32).view(np.int32)).to(dev), bank
+            self._bank(st, dev, bank)
         P = params if params is not None else self.sample(B, len(bank) if bank is not None else 0)
         cand = torch.from_numpy(self.pack(P)).to(dev, non_blocking=True)
         mask8 = mask.to(torch.uint8).contiguous()
@@ -456,6 +482,20 @@ class Occlusion(object):
             _lib.ptr(st["rows"]), _lib.ptr(st["cols"]), self.low[0], self.low[1], _lib.ptr(out), _lib.ptr(st["fallbacks"]),
             C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "augment occlusion")
         return out
+
+    def apply_indexed(self, mask_stack, idx_d, cand_d, bank, out, stream):
+        """``apply_device`` on the masks mask_stack[idx_d[b]] of a device-resident stack (``aae_augment_occlusion_indexed``):
+        cand_d is ``pack``'s candidate table on the device, out the uint8 [B,H,W] result.  Asynchronous on ``stream``; counts
+        into the same fallback counters."""
+        dev = out.device
+        B = int(out.shape[0])
+        st = self._state(dev)
+        bank_d = self._bank(st, dev, bank) if self.realistic else None
+        _lib.check(_lib.lib().aae_augment_occlusion_indexed(
+            _lib.ptr(mask_stack), len(mask_stack), _lib.ptr(idx_d), B, self.h, self.w, _lib.ptr(bank_d),
+            len(bank_d) if bank_d is not None else 0, _lib.ptr(cand_d), self.K, int(self.realistic != 0), self.realistic,
+            int(self.square != 0), 1.0 - self.square, _lib.ptr(st["rows"]), _lib.ptr(st["cols"]), self.low[0], self.low[1],
+            _lib.ptr(out), _lib.ptr(st["fallbacks"]), C.c_void_p(stream.cuda_stream)), "augment occlusion (indexed)")
 
     def fallbacks(self):
         """Images that exhausted their K candidates since the last call, per step: {"realistic": n, "square": n}.  Clears the

@@ -2,6 +2,8 @@
 (``viewsphere_for_embedding``, dataset.py:39-58, built on pysixd_stuff/view_sampler.py:19-188), ``embedding_size``
 and the square-patch crop helper (dataset.py:354-373).  Rendering / augmentation (OpenGL, imgaug) are out of scope
 (SURVEY.md section 2 rows 7, 11): ``render_embedding_image_batch`` delegates to a user-supplied renderer."""
+import glob
+import hashlib
 import math
 import os
 
@@ -159,15 +161,116 @@ class Dataset(object):
         return cv2.resize(crop, resize, interpolation=interpolation)
 
     # ------------------------------------------------------------------------------------------------ training batches
-    def load_training_images(self, path, bg_path=None):
+    def load_training_images(self, path, bg_path=None, device=None):
         """The cache the reference writes after rendering (``np.savez(current_file_name, train_x=, mask_x=, train_y=)``,
-        dataset.py:101-113) and, optionally, the background image stack (``.npy``, dataset.py:229-255)."""
+        dataset.py:101-113) and, optionally, the background image stack (``.npy``, dataset.py:229-255).  With ``device`` the
+        stacks are also uploaded once and kept there (``upload``) for ``batch_resident`` and the started ``Queue``; the host
+        arrays stay as they are either way."""
         data = np.load(path)
         self.train_x, self.mask_x, self.train_y = data["train_x"].astype(np.uint8), data["mask_x"], data["train_y"].astype(np.uint8)
         self.noof_training_imgs = len(self.train_x)
         if bg_path is not None:
             self.bg_imgs = np.load(bg_path).astype(np.uint8)
             self.noof_bg_imgs = len(self.bg_imgs)
+        if device is not None:
+            self.upload(device)
+
+    def training_images_path(self, dataset_path, args):
+        """Where the reference caches the rendered training set of a cfg: md5 of ``str(args.items('Dataset') +
+        args.items('Paths'))`` (dataset.py:91-92), so a cache the reference rendered is found under the same name."""
+        digest = hashlib.md5((str(args.items('Dataset') + args.items('Paths'))).encode('utf-8')).hexdigest()
+        return os.path.join(dataset_path, digest + '.npz')
+
+    def get_training_images(self, dataset_path, args, device=None):
+        """dataset.py:90-103 without rendering: loads the cache of ``training_images_path``; a missing cache raises and names it."""
+        path = self.training_images_path(dataset_path, args)
+        if not os.path.exists(path):
+            raise FileNotFoundError("no training-image cache for this cfg: %s (rendering the training set is not part of this "
+                                    "package; render it with the reference's ae_train -gen and copy the .npz there)" % path)
+        self.load_training_images(path)
+        self.noof_obj_pixels = np.count_nonzero(np.asarray(self.mask_x) == 0, axis=(1, 2))
+        if device is not None:
+            self.upload(device, which=("x", "mask", "y"))
+        return path
+
+    def bg_images_path(self, dataset_path):
+        """Where the reference caches the background stack (dataset.py:146-147): md5 of ``str(shape) + str(noof_bg_imgs) +
+        BACKGROUND_IMAGES_GLOB``, noof_bg_imgs = min(NOOF_BG_IMGS, files the glob matches) (dataset.py:24-25)."""
+        pattern = str(self._kw['background_images_glob'])
+        n = min(int(self._kw['noof_bg_imgs']), len(glob.glob(pattern)))
+        digest = hashlib.md5((str(self.shape) + str(n) + pattern).encode('utf-8')).hexdigest()
+        return os.path.join(dataset_path, digest + '.npy')
+
+    def load_bg_images(self, dataset_path, device=None):
+        """The background stack of dataset.py:145-170: the cache of ``bg_images_path``, or, when it is missing, built from
+        BACKGROUND_IMAGES_GLOB with the reference's rule and saved there: the first noof_bg_imgs files in a shuffled order, each
+        cropped to H x W at a random anchor (grey for C = 1).  An image smaller than the crop leaves its row zero (the
+        reference leaves it uninitialised).  With ``device`` the stack is also kept on the device (``upload``)."""
+        path = self.bg_images_path(dataset_path)
+        if os.path.exists(path):
+            self.bg_imgs = np.load(path).astype(np.uint8)
+        else:
+            import random
+            import cv2
+            h, w, c = self.shape
+            files = glob.glob(str(self._kw['background_images_glob']))
+            n = min(int(self._kw['noof_bg_imgs']), len(files))
+            if n == 0:
+                raise FileNotFoundError("no background images match BACKGROUND_IMAGES_GLOB %s (and no cache at %s)"
+                                        % (self._kw['background_images_glob'], path))
+            files = files[:n]
+            random.shuffle(files)
+            bg = np.zeros((n, h, w, c), np.uint8)
+            for j, fname in enumerate(files):
+                bgr = cv2.imread(fname)
+                if bgr is None:
+                    raise IOError("cannot read background image %s" % fname)
+                H, W = bgr.shape[:2]
+                y0 = int(np.random.rand() * (H - h))
+                x0 = int(np.random.rand() * (W - w))
+                bgr = bgr[y0:y0 + h, x0:x0 + w, :]
+                if bgr.shape[0] != h or bgr.shape[1] != w:
+                    continue
+                if c == 1:
+                    bgr = cv2.cvtColor(np.uint8(bgr), cv2.COLOR_BGR2GRAY)[:, :, np.newaxis]
+                bg[j] = bgr
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+            np.save(path, bg)
+            self.bg_imgs = bg
+        self.noof_bg_imgs = len(self.bg_imgs)
+        if device is not None:
+            self.upload(device, which=("bg",))
+        return path
+
+    # -- the training set resident on the device --------------------------------------------------------------------
+    def upload(self, device, which=("x", "mask", "y", "bg")):
+        """Keeps train_x, mask_x (as uint8), train_y and bg_imgs on ``device``, uploaded once: N H W (2C + 1) + N_bg H W C bytes.
+        ``batch_resident`` and the started ``Queue`` read batches from there through index arrays instead of gathering them."""
+        import torch
+        dev = torch.device(device) if not isinstance(device, torch.device) else device
+        if dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        sources = {"x": "train_x", "mask": "mask_x", "y": "train_y", "bg": "bg_imgs"}
+        res = self.__dict__.setdefault("_resident", {})
+        for key in which:
+            arr = getattr(self, sources[key], None)
+            if arr is None:
+                raise RuntimeError("Dataset.%s is not loaded (load_training_images / load_bg_images)" % sources[key])
+            host = np.ascontiguousarray(np.asarray(arr).astype(np.uint8, copy=False))
+            res[key] = (arr, torch.from_numpy(host).to(dev))
+        return dev
+
+    def resident(self, device):
+        """{"x", "mask", "y", "bg"} -> the device stacks of ``upload`` on ``device``; RuntimeError naming what is missing or stale
+        (a host array replaced after the upload)."""
+        res = self.__dict__.get("_resident", {})
+        sources = {"x": "train_x", "mask": "mask_x", "y": "train_y", "bg": "bg_imgs"}
+        out = {}
+        for key, name in sources.items():
+            if key not in res or res[key][0] is not getattr(self, name, None) or res[key][1].device != device:
+                raise RuntimeError("Dataset.%s is not resident on %s: call upload(device) (or load_*(..., device=))" % (name, device))
+            out[key] = res[key][1]
+        return out
 
     @lazy_property
     def _aug(self):
@@ -228,6 +331,82 @@ class Dataset(object):
             m = occl.apply_device(m, getattr(self, "occlusion_masks", None))
         xf = self._aug.augment_device(x, m, bg)
         return xf, y.to(torch.float32) / 255.0
+
+    def _draws(self, batch_size):
+        """The random draws of one batch in ``batch_device``'s order and from its generators: rendering and background indices
+        (numpy's global stream), occlusion candidates (the Occlusion's own stream), augmentation parameters (the Augmenter's);
+        then the packed tables: (idx, idx_bg, cand or None, geom, lut)."""
+        occl = self._occlusion
+        if occl is not None and occl.realistic and getattr(self, "occlusion_masks", None) is None:
+            self.load_occlusion_masks()
+        idx = np.random.choice(len(self.train_x), batch_size, replace=False)
+        idx_bg = np.random.choice(len(self.bg_imgs), batch_size, replace=False)
+        cand = None
+        if occl is not None:
+            bank = getattr(self, "occlusion_masks", None)
+            cand = occl.pack(occl.sample(batch_size, len(bank) if bank is not None else 0))
+        aug = self._aug                 # built here on first use, as in batch_device: CODE may draw from numpy's stream
+        geom, lut = aug.pack(aug.sample(batch_size))
+        return idx, idx_bg, cand, geom, lut
+
+    def _resident_scratch(self, batch_size, device):
+        """Device buffers of one batch of ``_enqueue_resident``: the uploaded draws, the augment scratch and the occluded masks.
+        The batch producer keeps one set per slot, so its loop allocates no device memory."""
+        import torch
+        B = int(batch_size)
+        (h, w, c), occl = self.shape, self._occlusion
+        n_cand = B * (1 + 3 * occl.K) if occl is not None else 0
+        return {"draws": torch.empty(2 * B + B * (4 + 2 * w + 2 * h) + n_cand, dtype=torch.int32, device=device),
+                "lut": torch.empty(B * c * 256, dtype=torch.uint8, device=device),
+                "tmp": torch.empty((B, h, w, c), dtype=torch.uint8, device=device),
+                "mask": torch.empty((B, h, w), dtype=torch.uint8, device=device) if occl is not None else None}
+
+    def _enqueue_resident(self, stacks, draws, x_out, y_out, stream, scratch=None):
+        """One batch from the resident stacks into x_out / y_out (float32 [B,H,W,C]) on ``stream``: the draws go up from pinned
+        staging (torch's caching host allocator keeps a block until its copy has run), then the indexed occlusion and augment
+        kernels.  ``scratch`` (``_resident_scratch``, ordered by the caller) replaces the device buffers allocated here.  Nothing
+        waits for the device."""
+        import torch
+        idx, idx_bg, cand, geom, lut = draws
+        B = len(idx)
+        dev = x_out.device
+        n_cand = cand.size if cand is not None else 0
+        if scratch is None:
+            with torch.cuda.stream(stream):
+                scratch = self._resident_scratch(B, dev)
+        with torch.cuda.stream(stream):
+            host = torch.empty(2 * B + geom.size + n_cand, dtype=torch.int32, pin_memory=True)
+            h = host.numpy()
+            h[:B], h[B:2 * B], h[2 * B:2 * B + geom.size] = idx, idx_bg, geom.ravel()
+            if cand is not None:
+                h[2 * B + geom.size:] = cand.ravel()
+            host_lut = torch.empty(lut.size, dtype=torch.uint8, pin_memory=True)
+            host_lut.numpy()[:] = lut.ravel()
+            d = scratch["draws"][:host.numel()]
+            d.copy_(host, non_blocking=True)
+            lut_d = scratch["lut"]
+            lut_d.copy_(host_lut, non_blocking=True)
+            idx_d, idx_bg_d, geom_d = d[:B], d[B:2 * B], d[2 * B:2 * B + geom.size]
+            mask = None
+            if cand is not None:
+                mask = scratch["mask"]
+                self._occlusion.apply_indexed(stacks["mask"], idx_d, d[2 * B + geom.size:], getattr(self, "occlusion_masks", None),
+                                              mask, stream)
+            self._aug.augment_indexed(stacks, idx_d, idx_bg_d, geom_d, lut_d, x_out, y_out, stream, mask_batch=mask,
+                                      tmp=scratch["tmp"])
+
+    def batch_resident(self, batch_size, device=None):
+        """``batch_device`` on the stacks kept on the device by ``upload``: the same draws in the same order, so the same
+        (x, y), bit for bit, and the same occlusion fallback counts; only the draws (indices and packed tables, ~0.2 MB at
+        batch 64) are uploaded, and the target y / 255. comes out of the same launch.  Asynchronous on the current stream."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        stacks = self.resident(dev)
+        draws = self._draws(batch_size)
+        x = torch.empty((batch_size,) + self.shape, dtype=torch.float32, device=dev)
+        y = torch.empty_like(x)
+        self._enqueue_resident(stacks, draws, x, y, torch.cuda.current_stream(dev))
+        return x, y
 
     def batch(self, batch_size):
         """numpy (batch_x, batch_y) like the reference's ``Dataset.batch``."""

@@ -58,3 +58,23 @@ def get_eval_config_file_path(workspace_path, eval_cfg="eval.cfg"):
 
 def get_eval_dir(log_dir, evaluation_name, data):
     return os.path.join(log_dir, "eval", evaluation_name, data)
+
+
+def tiles(batch, rows, cols, spacing_x=0, spacing_y=0, scale=1.0):
+    """One image of the first rows * cols images of ``batch`` ([N, H, W, C] or [N, H, W]) laid out row by row, each resized to
+    (H * scale, W * scale) with cv2.resize, ``spacing_x`` / ``spacing_y`` pixels apart; cells without an image and the spacing
+    are 1.  Always [rows * h + (rows - 1) * spacing_y, cols * w + (cols - 1) * spacing_x, C] float64 (auto_pose/ae/utils.py:93)."""
+    import cv2
+    batch = np.asarray(batch)
+    if batch.ndim not in (3, 4):
+        raise ValueError("Invalid batch shape: {}".format(batch.shape))
+    n, h, w = batch.shape[:3]
+    c = batch.shape[3] if batch.ndim == 4 else 1
+    h, w = int(h * scale), int(w * scale)
+    out = np.ones((rows * h + (rows - 1) * spacing_y, cols * w + (cols - 1) * spacing_x, c))
+    for i in range(min(n, rows * cols)):
+        r, q = divmod(i, cols)
+        y0, x0 = r * (h + spacing_y), q * (w + spacing_x)
+        img = cv2.resize(batch[i], (w, h))
+        out[y0:y0 + h, x0:x0 + w, :] = img if img.ndim == 3 else img[:, :, None]
+    return out

@@ -741,10 +741,10 @@ extern "C" int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, 
                         blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, (cudaStream_t)stream);
 }
 
-extern "C" int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, int w, const uint32_t* bank_dev, int n_bank,
-                                     const int32_t* cand_dev, int n_cand, int realistic, double max_occl, int square, double min_kept,
-                                     const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_h, int low_w,
-                                     uint8_t* mask_out_dev, int32_t* fallbacks_dev, void* stream) {
+static int occlusion_checked(const uint8_t* mask_dev, int batch, int h, int w, const uint32_t* bank_dev, int n_bank, const int32_t* cand_dev,
+                             int n_cand, int realistic, double max_occl, int square, double min_kept, const uint8_t* row_cell_dev,
+                             const uint8_t* col_cell_dev, int low_h, int low_w, uint8_t* mask_out_dev, int32_t* fallbacks_dev, cudaStream_t s,
+                             const int32_t* idx_dev, long long n_images) {
   AAE_REQUIRE(mask_dev && cand_dev && mask_out_dev && fallbacks_dev, "null argument");
   AAE_REQUIRE(batch >= 1 && h >= 1 && w >= 1 && n_cand >= 1, "bad geometry / candidate count");
   AAE_REQUIRE(!realistic || (bank_dev && n_bank >= 1), "realistic occlusion needs an occluder bank");
@@ -763,7 +763,59 @@ extern "C" int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, 
     return AAE_ERR_UNSUPPORTED;
   }
   return launch_occlusion(mask_dev, batch, h, w, bank_dev, n_bank, cand_dev, n_cand, realistic, max_occl, square, min_kept,
-                          row_cell_dev, col_cell_dev, low_w, mask_out_dev, fallbacks_dev, (cudaStream_t)stream);
+                          row_cell_dev, col_cell_dev, low_w, mask_out_dev, fallbacks_dev, s, idx_dev, n_images);
+}
+
+extern "C" int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, int w, const uint32_t* bank_dev, int n_bank,
+                                     const int32_t* cand_dev, int n_cand, int realistic, double max_occl, int square, double min_kept,
+                                     const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_h, int low_w,
+                                     uint8_t* mask_out_dev, int32_t* fallbacks_dev, void* stream) {
+  return occlusion_checked(mask_dev, batch, h, w, bank_dev, n_bank, cand_dev, n_cand, realistic, max_occl, square, min_kept,
+                           row_cell_dev, col_cell_dev, low_h, low_w, mask_out_dev, fallbacks_dev, (cudaStream_t)stream, nullptr, 0);
+}
+
+extern "C" int aae_augment_batch_indexed(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
+                                         const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
+                                         const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
+                                         const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
+                                         const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
+                                         const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
+                                         float* out_f32_dev, float* y_out_dev, void* stream) {
+  AAE_REQUIRE(x_stack_dev && bg_stack_dev && idx_dev && idx_bg_dev && (mask_stack_dev || mask_batch_dev), "null argument");
+  AAE_REQUIRE(!y_out_dev || (y_stack_dev && y_to_float_dev), "y_out_dev needs y_stack_dev and y_to_float_dev");
+  AAE_REQUIRE(n_images >= 1 && n_bg >= 1, "empty image stack (%lld images, %lld backgrounds)", (long long)n_images, (long long)n_bg);
+  AAE_REQUIRE(geom_dev && lut_dev && bilinear_tab_dev && row_cell_dev && col_cell_dev && tmp_dev, "null argument");
+  AAE_REQUIRE(out_u8_dev || out_f32_dev, "no output requested");
+  AAE_REQUIRE(!out_f32_dev || u8_to_float_dev, "out_f32_dev needs u8_to_float_dev");
+  AAE_REQUIRE(batch >= 1 && h >= 1 && w >= 1 && low_w >= 1, "bad geometry");
+  if (blur_kernel_q8) {
+    int sum = 0;
+    for (int i = 0; i < 5; ++i) sum += blur_kernel_q8[i];
+    AAE_REQUIRE(sum == 256, "blur kernel must sum to 256 (8 fractional bits), got %d", sum);
+  }
+  AugIndex ix;
+  ix.idx = idx_dev;
+  ix.idx_bg = idx_bg_dev;
+  ix.n_images = n_images;
+  ix.n_bg = n_bg;
+  ix.mask_gathered = mask_batch_dev != nullptr;
+  ix.y = y_stack_dev;
+  ix.y_to_float = y_to_float_dev;
+  ix.y_out = y_out_dev;
+  return launch_augment(x_stack_dev, mask_batch_dev ? mask_batch_dev : mask_stack_dev, bg_stack_dev, batch, h, w, c, geom_dev, lut_dev,
+                        bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w, blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev,
+                        (cudaStream_t)stream, ix);
+}
+
+extern "C" int aae_augment_occlusion_indexed(const uint8_t* mask_stack_dev, int64_t n_images, const int32_t* idx_dev, int batch, int h, int w,
+                                             const uint32_t* bank_dev, int n_bank, const int32_t* cand_dev, int n_cand, int realistic,
+                                             double max_occl, int square, double min_kept, const uint8_t* row_cell_dev,
+                                             const uint8_t* col_cell_dev, int low_h, int low_w, uint8_t* mask_out_dev, int32_t* fallbacks_dev,
+                                             void* stream) {
+  AAE_REQUIRE(mask_stack_dev && idx_dev, "null argument");
+  AAE_REQUIRE(n_images >= 1, "empty mask stack");
+  return occlusion_checked(mask_stack_dev, batch, h, w, bank_dev, n_bank, cand_dev, n_cand, realistic, max_occl, square, min_kept,
+                           row_cell_dev, col_cell_dev, low_h, low_w, mask_out_dev, fallbacks_dev, (cudaStream_t)stream, idx_dev, n_images);
 }
 
 // ============================================================================ decoder

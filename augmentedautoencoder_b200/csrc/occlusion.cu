@@ -55,7 +55,8 @@ __global__ void __launch_bounds__(OCCL_THREADS) occlusion_kernel(const uint8_t* 
                                                                  const uint32_t* __restrict__ bank, int n_bank, const int32_t* __restrict__ cand,
                                                                  int K, int realistic, double max_occl, int square, double min_kept,
                                                                  const uint8_t* __restrict__ row_cell, const uint8_t* __restrict__ col_cell,
-                                                                 int low_w, uint8_t* __restrict__ mask_out, int32_t* __restrict__ fallbacks) {
+                                                                 int low_w, uint8_t* __restrict__ mask_out, int32_t* __restrict__ fallbacks,
+                                                                 const int32_t* __restrict__ idx, long long n_images) {
   extern __shared__ uint32_t smem[];
   const int Wd = W >> 5, NW = H * Wd;
   uint32_t* obj = smem;                  // [H][Wd] object plane (~mask)
@@ -67,18 +68,20 @@ __global__ void __launch_bounds__(OCCL_THREADS) occlusion_kernel(const uint8_t* 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const long long b = blockIdx.x;
   const int32_t* rec = cand + b * (1 + 3 * (long long)K);
-  const uint8_t* m = mask_in + b * H * W;
+  // indexed form: row idx[b] of the mask stack; a row outside it is all background
+  const long long row = idx == nullptr ? b : ((idx[b] >= 0 && idx[b] < n_images) ? (long long)idx[b] : -1);
+  const uint8_t* m = row >= 0 ? mask_in + row * H * W : nullptr;
 
   int cnt = 0;
   for (int i = warp; i < NW; i += OCCL_WARPS) {
-    const uint32_t bits = __ballot_sync(0xffffffffu, m[i * 32 + lane] == 0);
+    const uint32_t bits = __ballot_sync(0xffffffffu, m != nullptr && m[i * 32 + lane] == 0);
     if (lane == 0) { obj[i] = bits; cnt += __popc(bits); }
   }
   if (lane == 0) s_count[warp] = cnt;
   if (realistic) {
-    const int idx = rec[0];
-    const bool ok = idx >= 0 && idx < n_bank;        // an index outside the bank is an occluder without pixels
-    for (int i = tid; i < NW; i += OCCL_THREADS) occ[i] = ok ? bank[(long long)idx * NW + i] : 0u;
+    const int occluder = rec[0];
+    const bool ok = occluder >= 0 && occluder < n_bank;        // an index outside the bank is an occluder without pixels
+    for (int i = tid; i < NW; i += OCCL_THREADS) occ[i] = ok ? bank[(long long)occluder * NW + i] : 0u;
   }
   if (square) {
     for (int i = tid; i < low_w * Wd; i += OCCL_THREADS) {
@@ -176,9 +179,9 @@ size_t occlusion_smem_bytes(int H, int W, int low_w) { return (size_t)(2 * H + l
 
 int launch_occlusion(const uint8_t* mask, int B, int H, int W, const uint32_t* bank, int n_bank, const int32_t* cand, int K, int realistic,
                      double max_occl, int square, double min_kept, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, uint8_t* out,
-                     int32_t* fallbacks, cudaStream_t s) {
+                     int32_t* fallbacks, cudaStream_t s, const int32_t* idx, long long n_images) {
   occlusion_kernel<<<B, OCCL_THREADS, occlusion_smem_bytes(H, W, square ? low_w : 0), s>>>(
-      mask, H, W, bank, n_bank, cand, K, realistic, max_occl, square, min_kept, row_cell, col_cell, low_w, out, fallbacks);
+      mask, H, W, bank, n_bank, cand, K, realistic, max_occl, square, min_kept, row_cell, col_cell, low_w, out, fallbacks, idx, n_images);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }

@@ -273,6 +273,31 @@ AAE_API int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, int
                                   const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_h, int low_w,
                                   uint8_t* mask_out_dev, int32_t* fallbacks_dev, void* stream);
 
+/* Indexed forms of the two calls above, for a training set resident on the device (Dataset.load_training_images(device=...)):
+ * nothing of the batch is gathered.  x_stack_dev / y_stack_dev: uint8 [n_images][H][W][C], mask_stack_dev: uint8 [n_images][H][W]
+ * (nonzero = background), bg_stack_dev: uint8 [n_bg][H][W][C].  Image b of the batch is row idx_dev[b] of the x, mask and y stacks
+ * and row idx_bg_dev[b] of the background stack (int32 [batch] each, on the device).  Indices outside their stack: an image b
+ * whose idx_dev[b] OR idx_bg_dev[b] is outside is pasted and warped as all zeros (its value tables still apply), and its target
+ * is y_to_float_dev[0]; aae_augment_occlusion_indexed reads a mask row outside the stack as a mask without object pixels.
+ *   aae_augment_occlusion_indexed: aae_augment_occlusion on the masks mask_stack_dev[idx_dev[b]]; mask_out_dev [batch][H][W].
+ *   aae_augment_batch_indexed: aae_augment_batch on x_stack_dev[idx_dev[b]], background bg_stack_dev[idx_bg_dev[b]] and mask
+ *     mask_stack_dev[idx_dev[b]] -- or, when mask_batch_dev is not NULL, row b of mask_batch_dev [batch][H][W] (an occlusion output;
+ *     mask_stack_dev may then be NULL).  y_out_dev (optional, float32 [batch][H][W][C]) receives the reconstruction target
+ *     y_to_float_dev[y_stack_dev[idx_dev[b]]], 256 floats chosen by the caller (Dataset passes the float32 values of y / 255. its gathered path computes).
+ * Same stream rules as every input-pipeline call: every launch on `stream`, no allocation, no synchronisation. */
+AAE_API int aae_augment_batch_indexed(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
+                                      const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
+                                      const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
+                                      const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
+                                      const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
+                                      const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
+                                      float* out_f32_dev, float* y_out_dev, void* stream);
+AAE_API int aae_augment_occlusion_indexed(const uint8_t* mask_stack_dev, int64_t n_images, const int32_t* idx_dev, int batch, int h, int w,
+                                          const uint32_t* bank_dev, int n_bank, const int32_t* cand_dev, int n_cand, int realistic,
+                                          double max_occl, int square, double min_kept, const uint8_t* row_cell_dev,
+                                          const uint8_t* col_cell_dev, int low_h, int low_w, uint8_t* mask_out_dev, int32_t* fallbacks_dev,
+                                          void* stream);
+
 /* ---------------------------------------------------------------- Training step ------------
  * Replaces sess.run(train_op): encoder fwd, decoder fwd, bootstrapped L2, backward, optimizer update
  * (auto_pose/ae/ae_train.py:128, auto_pose/ae/ae_factory.py:79-95).
