@@ -14,13 +14,14 @@ pytestmark = pytest.mark.gpu
 H = W = 128
 
 
-def _objects(rng, B):
-    """True = background: random ellipses and rectangles of very different sizes."""
-    yy, xx = np.mgrid[:H, :W]
-    masks = np.ones((B, H, W), bool)
+def _objects(rng, B, h=H, w=W):
+    """True = background: random ellipses and rectangles of very different sizes.  Centres and radii are drawn on the 128 x 128
+    grid and scaled to h x w, so the default draws the same masks from the same stream."""
+    yy, xx = np.mgrid[:h, :w]
+    masks = np.ones((B, h, w), bool)
     for b in range(B):
-        cy, cx = rng.randint(10, 118, 2)
-        ry, rx = rng.randint(6, 60, 2)
+        cy, cx = 10 + rng.randint(0, 108, 2) * np.array([h - 20, w - 20]) // 108
+        ry, rx = 6 + rng.randint(0, 54, 2) * np.array([h, w]) // 128
         if b % 4 == 3:
             masks[b] = ~((np.abs(yy - cy) <= ry) & (np.abs(xx - cx) <= rx))
         else:
@@ -28,7 +29,7 @@ def _objects(rng, B):
     return masks
 
 
-def _bank(tmp_path, rng, n=12):
+def _bank(tmp_path, rng, n=12, h=H, w=W):
     side = A.OCCLUSION_BANK_SIDE
     yy, xx = np.mgrid[:side, :side]
     bits = np.zeros((n, side, side), bool)
@@ -39,8 +40,8 @@ def _bank(tmp_path, rng, n=12):
             bits[i] |= ((yy - cy) / float(ry)) ** 2 + ((xx - cx) / float(rx)) ** 2 <= 1.0
     path = tmp_path / "arbitrary_syn_masks.bin"
     np.packbits(bits.reshape(-1)).tofile(path)
-    words = A.load_occlusion_bank(str(path), (H, W))
-    f32 = np.unpackbits(words.view(np.uint8), axis=-1, bitorder="little").reshape(n, H, W).astype(np.float32)
+    words = A.load_occlusion_bank(str(path), (h, w))
+    f32 = np.unpackbits(words.view(np.uint8), axis=-1, bitorder="little").reshape(n, h, w).astype(np.float32)
     return str(path), words, f32
 
 
