@@ -95,6 +95,9 @@ _SIGS = {
     "aae_augment_occlusion": (_I, [_P, _I, _I, _I, _P, _I, _P, _I, _I, _D, _I, _D, _P, _P, _I, _I, _P, _P, _P]),
     "aae_augment_batch_indexed": (_I, [_P, _P, _P, _P, _L, _L, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P,
                                        _P, _P, _P]),
+    "aae_augment_batch_crop": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _P, _P]),
+    "aae_augment_batch_indexed_crop": (_I, [_P, _P, _P, _P, _L, _L, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P,
+                                            _P, _P, _P, _P, _P, _L, _I, _I, _P, _P]),
     "aae_augment_occlusion_indexed": (_I, [_P, _L, _P, _I, _I, _I, _P, _I, _P, _I, _I, _D, _I, _D, _P, _P, _I, _I, _P, _P, _P]),
 }
 

@@ -7,10 +7,14 @@ random draws are made here with numpy (same distributions as imgaug's stochastic
 value ops as composed 256-entry tables (include/aae_b200.h).  At the tensor-core trainer's ~10 000 images/s the reference's
 10 Python threads of imgaug would be the bottleneck by more than an order of magnitude.
 
-Supported chain: any subset of the template's ops IN THE TEMPLATE'S ORDER (Affine, CoarseDropout, GaussianBlur, Add, Invert,
-Multiply, Multiply, ContrastNormalization; another order raises): Sometimes(p, Affine(scale=(a, b))), Sometimes(p, CoarseDropout(p=, size_percent=)),
+Supported chain: any subset of the template's ops IN THE TEMPLATE'S ORDER (CropAndPad, Affine, CoarseDropout, GaussianBlur, Add,
+Invert, Multiply, Multiply, ContrastNormalization; another order raises): Sometimes(p, CropAndPad(percent= or px=, pad_cval=,
+sample_independently=)), Sometimes(p, Affine(scale=(a, b))), Sometimes(p, CoarseDropout(p=, size_percent=)),
 Sometimes(p, GaussianBlur(sigma)), Sometimes(p, Add((a, b), per_channel=)), Sometimes(p, Invert(p, per_channel=True)),
 Sometimes(p, Multiply((a, b), per_channel=)), Sometimes(p, ContrastNormalization((a, b), per_channel=)).  Anything else raises.
+CropAndPad (the template's commented-out ``Sometimes(0.5, CropAndPad(percent=(-0.05, 0.1)))``) takes a scalar or a (low, high)
+range for ``percent`` / ``px`` and ``pad_cval``, ``pad_mode="constant"`` and ``keep_size=True`` only; its image is resized
+back to (H, W) with cv2.resize's INTER_CUBIC / INTER_AREA arithmetic (``crop_pad_rule`` and the helpers below it).
 
 ``Occlusion`` adds the two occlusion switches of the cfg's ``[Augmentation]`` section (REALISTIC_OCCLUSION, SQUARE_OCCLUSION,
 dataset.py:421-454), which edit the masks before the paste; ``aae_augment_occlusion`` applies them.
@@ -22,7 +26,7 @@ import torch
 
 from .. import _lib
 
-FLAG_AFFINE, FLAG_DROP, FLAG_BLUR = 1, 2, 4
+FLAG_AFFINE, FLAG_DROP, FLAG_BLUR, FLAG_CROP = 1, 2, 4, 8
 
 
 # ----------------------------------------------------------------------------------------------------------- cfg parsing
@@ -53,7 +57,8 @@ def parse_code(code):
     out = []
     for item in ops:
         p, op = item if isinstance(item, tuple) else (1.0, item)
-        if op.kind not in ("Affine", "CoarseDropout", "GaussianBlur", "Add", "Invert", "Multiply", "ContrastNormalization", "LinearContrast"):
+        if op.kind not in ("CropAndPad", "Affine", "CoarseDropout", "GaussianBlur", "Add", "Invert", "Multiply", "ContrastNormalization",
+                           "LinearContrast"):
             raise NotImplementedError("augmenter %s is not supported on the device pipeline" % op.kind)
         out.append((p, op))
     return out
@@ -131,6 +136,83 @@ def nearest_cells(dst, src):
     return np.minimum(np.floor(np.arange(dst, dtype=np.float64) * ifx).astype(np.int64), src - 1).astype(np.uint8)
 
 
+# CropAndPad (imgaug 0.4.0, the version the reference pins; its source is not available here).  Each rule below is imgaug as
+# remembered: UNVERIFIED (DESIGN.md section 2).
+CROP_PAD_SIDES = ("top", "right", "bottom", "left")     # draw order of the four sides with sample_independently=True
+
+
+def crop_pad_pixels(size, value, percent):
+    """Pixels of one side from its drawn value: in percent mode np.round(float32(size) * pct) (half to even) as int32; px
+    values are used as drawn.  Negative = crop, positive = pad."""
+    if not percent:
+        return np.asarray(value).astype(np.int32)
+    return np.round(np.float32(size) * np.asarray(value, np.float64)).astype(np.int32)
+
+
+def crop_pad_limit_crops(size, start, end):
+    """_prevent_zero_sizes_after_crops_: crops of one axis (start, end >= 0) reduced so that at least one pixel remains; the
+    excess is taken back floor-half from the start and ceil-half from the end."""
+    start, end = np.array(start, np.int32), np.array(end, np.int32)
+    excess = np.maximum(start + end - (size - 1), 0)
+    start, end = start - excess // 2, end - (excess - excess // 2)
+    return np.maximum(start, 0) + np.minimum(end, 0), np.maximum(end, 0) + np.minimum(start, 0)
+
+
+def crop_pad_rule(src_h, src_w, dst_h, dst_w):
+    """imresize_single_image's default interpolation for keep_size: "cubic" when the target is larger than the source along
+    either axis, else "area" (cv2.resize copies an image whose size did not change; area at ratio 1 is that copy)."""
+    return "cubic" if dst_h > src_h or dst_w > src_w else "area"
+
+
+def cubic_taps(dst, src):
+    """cv2.resize(INTER_CUBIC) along one axis, uint8: source indices [dst, 4] (clamped to the image) and fixed-point weights
+    [dst, 4] with 11 fractional bits (interpolateCubic, A = -0.75, float32 arithmetic, saturate_cast<short>)."""
+    f = np.float32
+    scale = 1.0 / (float(dst) / float(src))
+    fx = ((np.arange(dst, dtype=np.float64) + 0.5) * scale - 0.5).astype(np.float32)
+    sx = np.floor(fx).astype(np.int64)
+    x = (fx - sx.astype(np.float32)).astype(np.float32)
+    A = f(-0.75)
+    x1, om = x + f(1), f(1) - x
+    c0 = ((A * x1 - f(5) * A) * x1 + f(8) * A) * x1 - f(4) * A
+    c1 = ((A + f(2)) * x - (A + f(3))) * x * x + f(1)
+    c2 = ((A + f(2)) * om - (A + f(3))) * om * om + f(1)
+    c3 = f(1) - c0 - c1 - c2
+    w = np.rint(np.stack([c0, c1, c2, c3], 1).astype(np.float32) * f(2048)).astype(np.int32)
+    idx = np.clip(sx[:, None] + np.arange(-1, 3)[None, :], 0, src - 1).astype(np.int32)
+    return idx, w
+
+
+def area_taps(dst, src, taps=4):
+    """cv2.resize(INTER_AREA) along one axis for src >= dst (computeResizeAreaTab): per destination index the source indices
+    and float32 weights in OpenCV's accumulation order, padded to ``taps`` with weight 0 on the last index (adding +0 leaves
+    a float sum unchanged).  More taps than ``taps`` raise NotImplementedError."""
+    scale = 1.0 / (float(dst) / float(src))
+    idx, w = np.zeros((dst, taps), np.int32), np.zeros((dst, taps), np.float32)
+    for dx in range(dst):
+        f1 = dx * scale
+        f2 = f1 + scale
+        cell = min(scale, src - f1)
+        s1, s2 = int(np.ceil(f1)), int(np.floor(f2))
+        s2 = min(s2, src - 1)
+        s1 = min(s1, s2)
+        row = []
+        if s1 - f1 > 1e-3:
+            row.append((s1 - 1, np.float32((s1 - f1) / cell)))
+        row += [(s, np.float32(1.0 / cell)) for s in range(s1, s2)]
+        if f2 - s2 > 1e-3:
+            row.append((s2, np.float32(min(min(f2 - s2, 1.0), cell) / cell)))
+        if len(row) > taps:
+            raise NotImplementedError("CropAndPad: INTER_AREA from %d to %d pixels needs %d taps (%d supported)" % (src, dst, len(row), taps))
+        row += [(row[-1][0], np.float32(0))] * (taps - len(row))
+        idx[dx], w[dx] = [r[0] for r in row], [r[1] for r in row]
+    return idx, w
+
+
+CROP_PAD_ROWS = 8              # output rows of one crop-pad CTA (csrc/augment.cu)
+CROP_PAD_SMEM_LIMIT = 48 * 1024
+
+
 _IDENT = np.arange(256, dtype=np.uint8)
 
 
@@ -151,7 +233,7 @@ class Augmenter(object):
     def __init__(self, code, shape=(128, 128, 3), seed=None):
         self.h, self.w, self.c = int(shape[0]), int(shape[1]), int(shape[2])
         self.ops = parse_code(code) if isinstance(code, str) else list(code)
-        canon = ["Affine", "CoarseDropout", "GaussianBlur", "Add", "Invert", "Multiply", "Multiply", "ContrastNormalization"]
+        canon = ["CropAndPad", "Affine", "CoarseDropout", "GaussianBlur", "Add", "Invert", "Multiply", "Multiply", "ContrastNormalization"]
         pos = 0
         for _, op in self.ops:                                  # the kernels apply the ops in the template's order
             kind = "ContrastNormalization" if op.kind == "LinearContrast" else op.kind
@@ -173,7 +255,71 @@ class Augmenter(object):
                 self.low = (max(int(self.h * sp), 4), max(int(self.w * sp), 4))     # FromLowerResolution(min_size=4)
                 if self.low[0] * self.low[1] > 64:
                     raise NotImplementedError("CoarseDropout masks with more than 64 cells are not supported")
+        self.crop = None
+        for _, op in self.ops:
+            if op.kind == "CropAndPad":
+                self.crop = self._crop_pad_setup(op)
         self._dev = {}
+
+    def _crop_pad_setup(self, op):
+        """Checks CropAndPad's arguments and builds the resampling tables of every reachable source size: one int32 array of
+        [dst][4 indices, 4 weights] blocks (weights int for cubic, float32 bits for area), with the offset of each block."""
+        kw = dict(op.kw)
+        if op.args:
+            raise NotImplementedError("CropAndPad: positional arguments are not supported (use px= or percent=)")
+        unknown = set(kw) - {"px", "percent", "pad_mode", "pad_cval", "keep_size", "sample_independently", "name", "deterministic",
+                             "random_state"}
+        if unknown:
+            raise NotImplementedError("CropAndPad: argument %s is not supported" % sorted(unknown)[0])
+        if (kw.get("px") is None) == (kw.get("percent") is None):
+            raise NotImplementedError("CropAndPad: exactly one of px= and percent= is supported")
+        percent = kw.get("percent") is not None
+        value = kw["percent"] if percent else kw["px"]
+        if isinstance(value, (tuple, list)) and (len(value) != 2 or any(isinstance(v, (tuple, list)) for v in value)):
+            raise NotImplementedError("CropAndPad: %s as per-side tuples or lists is not supported (a scalar or one (low, high) range)"
+                                      % ("percent" if percent else "px"))
+        if kw.get("pad_mode", "constant") != "constant":
+            raise NotImplementedError("CropAndPad: pad_mode=%r is not supported (only \"constant\")" % (kw["pad_mode"],))
+        if not kw.get("keep_size", True):
+            raise NotImplementedError("CropAndPad: keep_size=False is not supported (batch images must keep one shape)")
+        cval = kw.get("pad_cval", 0)
+        if isinstance(cval, (tuple, list)) and len(cval) != 2:
+            raise NotImplementedError("CropAndPad: pad_cval as a list is not supported (a scalar or one (low, high) range)")
+        lo, hi = _range(value)
+        if not 0 <= _range(cval)[0] <= _range(cval)[1] <= 255:
+            raise NotImplementedError("CropAndPad: pad_cval=%r is not a uint8 value or range" % (cval,))
+        if not percent and (lo != int(lo) or hi != int(hi)):
+            raise NotImplementedError("CropAndPad: px= needs integer pixel counts")
+        cz = _range(cval)
+        c = dict(percent=percent, lo=lo, hi=hi, cval=(int(cz[0]), int(cz[1])), independent=bool(kw.get("sample_independently", True)))
+        # reachable source sizes per axis: every side between its smallest and its largest pixel count
+        sizes = {}
+        for axis, n in (("y", self.h), ("x", self.w)):
+            a, b = (int(crop_pad_pixels(n, v, percent)) for v in (lo, hi))
+            sizes[axis] = range(max(1, n + 2 * a), n + 2 * b + 1)
+        blocks, off, rows = [], {}, 1
+        pos = 0
+        for axis, dst in (("y", self.h), ("x", self.w)):
+            for n in sizes[axis]:
+                if n > dst and n % dst == 0:
+                    raise NotImplementedError("CropAndPad: %d -> %d pixels is an integer ratio, which cv2.resize's INTER_AREA takes "
+                                              "through its separate fast path (not supported)" % (n, dst))
+                kinds = [("cubic", cubic_taps(dst, n))] + ([("area", area_taps(dst, n))] if n >= dst else [])
+                for kind, (idx, w) in kinds:
+                    blk = np.concatenate([idx, w.view(np.int32) if w.dtype == np.float32 else w], 1).astype(np.int32)
+                    off[(axis, kind, n)] = pos
+                    blocks.append(blk.ravel())
+                    pos += blk.size
+                    if axis == "y":
+                        first, last = idx[::CROP_PAD_ROWS, 0], idx[np.minimum(np.arange(CROP_PAD_ROWS - 1, dst + CROP_PAD_ROWS - 1,
+                                                                                         CROP_PAD_ROWS), dst - 1), 3]
+                        rows = max(rows, int((last - first).max()) + 1)
+        c.update(sizes=sizes, table=np.concatenate(blocks), offsets=off, max_rows=rows, max_w=sizes["x"][-1])
+        smem = rows * c["max_w"] * self.c
+        if smem > CROP_PAD_SMEM_LIMIT:
+            raise NotImplementedError("CropAndPad: source rows of %d x %d x %d bytes per CTA exceed the %d bytes of shared memory "
+                                      "the crop-pad kernel uses" % (rows, c["max_w"], self.c, CROP_PAD_SMEM_LIMIT))
+        return c
 
     # -- host: random draws (imgaug's distributions; numpy's stream) -------------------------------------------------
     def sample(self, B):
@@ -196,7 +342,21 @@ class Augmenter(object):
 
         for p, op in self.ops:
             on = r.rand(B) < p
-            if op.kind == "Affine":
+            if op.kind == "CropAndPad":
+                c = self.crop
+                if c["percent"]:
+                    draw = lambda sz: r.uniform(c["lo"], c["hi"], sz)      # noqa: E731
+                else:
+                    draw = lambda sz: r.randint(int(c["lo"]), int(c["hi"]) + 1, sz)      # noqa: E731
+                v = draw((B, 4)) if c["independent"] else np.repeat(draw(B)[:, None], 4, 1)
+                px = np.stack([crop_pad_pixels(self.h if k % 2 == 0 else self.w, v[:, k], c["percent"]) for k in range(4)], 1)
+                for a, b, n in ((0, 2, self.h), (3, 1, self.w)):
+                    cs, ce = crop_pad_limit_crops(n, np.maximum(-px[:, a], 0), np.maximum(-px[:, b], 0))
+                    px[:, a], px[:, b] = np.where(px[:, a] < 0, -cs, px[:, a]), np.where(px[:, b] < 0, -ce, px[:, b])
+                P["crop_on"], P["crop_px"] = on, px.astype(np.int32)
+                lo, hi = c["cval"]
+                P["crop_cval"] = np.full(B, lo, np.int32) if lo == hi else r.randint(lo, hi + 1, B).astype(np.int32)
+            elif op.kind == "Affine":
                 lo, hi = _range(op.kw.get("scale", 1.0))
                 s = r.uniform(lo, hi, B)
                 cx, cy = self.w / 2.0 - 0.5, self.h / 2.0 - 0.5
@@ -239,6 +399,8 @@ class Augmenter(object):
         blur = bool(self.sigma > 1e-3)
         geom[:, 0] = (P["affine_on"].astype(np.int32) * FLAG_AFFINE) | (P["drop_on"].astype(np.int32) * FLAG_DROP) | \
                      ((P["blur_on"] & blur).astype(np.int32) * FLAG_BLUR)
+        if "crop_on" in P:
+            geom[:, 0] |= P["crop_on"].astype(np.int32) * FLAG_CROP
         weights = (np.uint64(1) << np.arange(self.low[0] * self.low[1], dtype=np.uint64))
         keep = (P["drop_keep"].reshape(B, -1).astype(np.uint64) * weights[None, :]).sum(1, dtype=np.uint64)
         geom[:, 1] = (keep & np.uint64(0xFFFFFFFF)).astype(np.uint32).view(np.int32)
@@ -282,6 +444,23 @@ class Augmenter(object):
         # kernel reads raw [B][C][256] memory
         return np.ascontiguousarray(geom), np.ascontiguousarray(t, dtype=np.uint8)
 
+    def pack_crop(self, P):
+        """-> the CropAndPad table int32 [B, 8] (include/aae_b200.h: aae_augment_batch_crop): mode (0 off, 1 cubic, 2 area),
+        source height and width after crop and pad, signed top and left pixels, pad value, offsets of the row and column
+        resampling blocks in the Augmenter's table.  None for a chain without CropAndPad."""
+        if self.crop is None:
+            return None
+        B, H, W = len(P["crop_on"]), self.h, self.w
+        t = np.zeros((B, 8), np.int32)
+        off = self.crop["offsets"]
+        px = P["crop_px"]
+        for b in np.nonzero(P["crop_on"])[0]:
+            top, right, bottom, left = (int(v) for v in px[b])
+            sh, sw = H + top + bottom, W + left + right
+            kind = crop_pad_rule(sh, sw, H, W)
+            t[b] = (1 if kind == "cubic" else 2, sh, sw, top, left, P["crop_cval"][b], off[("y", kind, sh)], off[("x", kind, sw)])
+        return t
+
     # -- device ------------------------------------------------------------------------------------------------------
     def _constants(self, dev):
         key = str(dev)
@@ -294,6 +473,8 @@ class Augmenter(object):
                 "taps": gaussian_taps_q8(self.sigma).astype(np.int32) if self.sigma > 1e-3 else None,
                 # the target's float32 y / 255. as torch computes it (Dataset.batch_device), for the indexed call's y output
                 "y_to_float": torch.arange(256, dtype=torch.int32, device=dev).to(torch.uint8).to(torch.float32) / 255.0,
+                # CropAndPad's resampling blocks of every reachable source size, built once per Augmenter
+                "resample": torch.from_numpy(self.crop["table"]).to(dev) if self.crop is not None else None,
             }
             torch.cuda.current_stream(dev).synchronize()    # usable from any stream (the batch producer's) from here on
         return self._dev[key]
@@ -316,30 +497,49 @@ class Augmenter(object):
         out_f = torch.empty(x.shape, dtype=torch.float32, device=dev)
         out_u = torch.empty_like(x) if want_u8 else None
         taps = k["taps"]
-        _lib.check(_lib.lib().aae_augment_batch(_lib.ptr(x.contiguous()), _lib.ptr(mask8), _lib.ptr(bg.contiguous()), B, self.h, self.w, self.c,
-                                                _lib.ptr(geom_d), _lib.ptr(lut_d), _lib.ptr(k["tab"]), _lib.ptr(k["rows"]), _lib.ptr(k["cols"]),
-                                                self.low[1], _lib.ptr(taps) if taps is not None else None, _lib.ptr(k["to_float"]), _lib.ptr(tmp),
-                                                _lib.ptr(out_u) if out_u is not None else None, _lib.ptr(out_f),
-                                                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "augment batch")
+        args = [_lib.ptr(x.contiguous()), _lib.ptr(mask8), _lib.ptr(bg.contiguous()), B, self.h, self.w, self.c, _lib.ptr(geom_d), _lib.ptr(lut_d),
+                _lib.ptr(k["tab"]), _lib.ptr(k["rows"]), _lib.ptr(k["cols"]), self.low[1], _lib.ptr(taps) if taps is not None else None,
+                _lib.ptr(k["to_float"]), _lib.ptr(tmp), _lib.ptr(out_u) if out_u is not None else None, _lib.ptr(out_f)]
+        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        if self.crop is None:
+            _lib.check(_lib.lib().aae_augment_batch(*args, stream), "augment batch")
+        else:
+            crop_d = torch.from_numpy(self.pack_crop(P)).to(dev, non_blocking=True)
+            _lib.check(_lib.lib().aae_augment_batch_crop(*args, *self._crop_args(k, crop_d, torch.empty_like(x)), stream), "augment batch (crop-pad)")
         return (out_f, out_u) if want_u8 else out_f
 
-    def augment_indexed(self, stacks, idx_d, idx_bg_d, geom_d, lut_d, out_f, y_out, stream, mask_batch=None, tmp=None):
+    def _crop_args(self, k, crop_d, crop_tmp):
+        return [_lib.ptr(crop_d), _lib.ptr(k["resample"]), int(k["resample"].numel()), self.crop["max_rows"], self.crop["max_w"],
+                _lib.ptr(crop_tmp)]
+
+    def augment_indexed(self, stacks, idx_d, idx_bg_d, geom_d, lut_d, out_f, y_out, stream, mask_batch=None, tmp=None, crop_d=None,
+                        crop_tmp=None):
         """``augment_device`` on device-resident stacks (``aae_augment_batch_indexed``): image b is row idx_d[b] of stacks["x"] /
         ["mask"] / ["y"] and row idx_bg_d[b] of stacks["bg"]; mask_batch (uint8 [B,H,W], e.g. an occlusion output) replaces the
         mask rows.  Writes the float32 input into out_f and the target y / 255. into y_out; geom_d / lut_d are ``pack``'s tables on
-        the device; tmp (uint8 [B,H,W,C]) is the scratch of the geometry pass, allocated here when None.  Asynchronous on ``stream``."""
+        the device; tmp (uint8 [B,H,W,C]) is the scratch of the geometry pass, allocated here when None.  With CropAndPad in the
+        chain crop_d is ``pack_crop``'s table on the device and crop_tmp (uint8 [B,H,W,C], allocated here when None) the
+        crop-pad output (``aae_augment_batch_indexed_crop``).  Asynchronous on ``stream``."""
         dev = out_f.device
         B = int(out_f.shape[0])
         k = self._constants(dev)
         if tmp is None:
             tmp = torch.empty((B, self.h, self.w, self.c), dtype=torch.uint8, device=dev)
         taps = k["taps"]
-        _lib.check(_lib.lib().aae_augment_batch_indexed(
-            _lib.ptr(stacks["x"]), _lib.ptr(stacks["mask"]), _lib.ptr(stacks["bg"]), _lib.ptr(stacks["y"]), len(stacks["x"]),
-            len(stacks["bg"]), _lib.ptr(idx_d), _lib.ptr(idx_bg_d), _lib.ptr(mask_batch), B, self.h, self.w, self.c, _lib.ptr(geom_d),
-            _lib.ptr(lut_d), _lib.ptr(k["tab"]), _lib.ptr(k["rows"]), _lib.ptr(k["cols"]), self.low[1],
-            _lib.ptr(taps) if taps is not None else None, _lib.ptr(k["to_float"]), _lib.ptr(k["y_to_float"]), _lib.ptr(tmp), None,
-            _lib.ptr(out_f), _lib.ptr(y_out), C.c_void_p(stream.cuda_stream)), "augment batch (indexed)")
+        args = [_lib.ptr(stacks["x"]), _lib.ptr(stacks["mask"]), _lib.ptr(stacks["bg"]), _lib.ptr(stacks["y"]), len(stacks["x"]),
+                len(stacks["bg"]), _lib.ptr(idx_d), _lib.ptr(idx_bg_d), _lib.ptr(mask_batch), B, self.h, self.w, self.c, _lib.ptr(geom_d),
+                _lib.ptr(lut_d), _lib.ptr(k["tab"]), _lib.ptr(k["rows"]), _lib.ptr(k["cols"]), self.low[1],
+                _lib.ptr(taps) if taps is not None else None, _lib.ptr(k["to_float"]), _lib.ptr(k["y_to_float"]), _lib.ptr(tmp), None,
+                _lib.ptr(out_f), _lib.ptr(y_out)]
+        if self.crop is None:
+            _lib.check(_lib.lib().aae_augment_batch_indexed(*args, C.c_void_p(stream.cuda_stream)), "augment batch (indexed)")
+            return
+        if crop_d is None:
+            raise ValueError("a chain with CropAndPad needs pack_crop's table (crop_d)")
+        if crop_tmp is None:
+            crop_tmp = torch.empty((B, self.h, self.w, self.c), dtype=torch.uint8, device=dev)
+        _lib.check(_lib.lib().aae_augment_batch_indexed_crop(*args, *self._crop_args(k, crop_d, crop_tmp), C.c_void_p(stream.cuda_stream)),
+                   "augment batch (indexed, crop-pad)")
 
 
 # ----------------------------------------------------------------------------------------------------------- occlusion

@@ -335,7 +335,7 @@ class Dataset(object):
     def _draws(self, batch_size):
         """The random draws of one batch in ``batch_device``'s order and from its generators: rendering and background indices
         (numpy's global stream), occlusion candidates (the Occlusion's own stream), augmentation parameters (the Augmenter's);
-        then the packed tables: (idx, idx_bg, cand or None, geom, lut)."""
+        then the packed tables: (idx, idx_bg, cand or None, geom, lut, crop or None -- the CropAndPad table)."""
         occl = self._occlusion
         if occl is not None and occl.realistic and getattr(self, "occlusion_masks", None) is None:
             self.load_occlusion_masks()
@@ -346,8 +346,23 @@ class Dataset(object):
             bank = getattr(self, "occlusion_masks", None)
             cand = occl.pack(occl.sample(batch_size, len(bank) if bank is not None else 0))
         aug = self._aug                 # built here on first use, as in batch_device: CODE may draw from numpy's stream
-        geom, lut = aug.pack(aug.sample(batch_size))
-        return idx, idx_bg, cand, geom, lut
+        P = aug.sample(batch_size)
+        geom, lut = aug.pack(P)
+        return idx, idx_bg, cand, geom, lut, aug.pack_crop(P)
+
+    def _chain_has_crop_pad(self):
+        """Whether [Augmentation] CODE has CropAndPad, without building the Augmenter: the first batch's draws build it (CODE
+        may draw from numpy's global stream there), so the stream is left as it was."""
+        if "_cache__aug" in self.__dict__:
+            return self._aug.crop is not None
+        if self._kw.get("code") is None:
+            return False
+        from .augment import parse_code
+        state = np.random.get_state()
+        try:
+            return any(op.kind == "CropAndPad" for _, op in parse_code(self._kw["code"]))
+        finally:
+            np.random.set_state(state)
 
     def _resident_scratch(self, batch_size, device):
         """Device buffers of one batch of ``_enqueue_resident``: the uploaded draws, the augment scratch and the occluded masks.
@@ -356,10 +371,12 @@ class Dataset(object):
         B = int(batch_size)
         (h, w, c), occl = self.shape, self._occlusion
         n_cand = B * (1 + 3 * occl.K) if occl is not None else 0
-        return {"draws": torch.empty(2 * B + B * (4 + 2 * w + 2 * h) + n_cand, dtype=torch.int32, device=device),
+        crop = self._chain_has_crop_pad()
+        return {"draws": torch.empty(2 * B + B * (4 + 2 * w + 2 * h) + n_cand + (8 * B if crop else 0), dtype=torch.int32, device=device),
                 "lut": torch.empty(B * c * 256, dtype=torch.uint8, device=device),
                 "tmp": torch.empty((B, h, w, c), dtype=torch.uint8, device=device),
-                "mask": torch.empty((B, h, w), dtype=torch.uint8, device=device) if occl is not None else None}
+                "mask": torch.empty((B, h, w), dtype=torch.uint8, device=device) if occl is not None else None,
+                "crop": torch.empty((B, h, w, c), dtype=torch.uint8, device=device) if crop else None}
 
     def _enqueue_resident(self, stacks, draws, x_out, y_out, stream, scratch=None):
         """One batch from the resident stacks into x_out / y_out (float32 [B,H,W,C]) on ``stream``: the draws go up from pinned
@@ -367,19 +384,22 @@ class Dataset(object):
         kernels.  ``scratch`` (``_resident_scratch``, ordered by the caller) replaces the device buffers allocated here.  Nothing
         waits for the device."""
         import torch
-        idx, idx_bg, cand, geom, lut = draws
+        idx, idx_bg, cand, geom, lut, crop = draws
         B = len(idx)
         dev = x_out.device
         n_cand = cand.size if cand is not None else 0
+        n_crop = crop.size if crop is not None else 0
         if scratch is None:
             with torch.cuda.stream(stream):
                 scratch = self._resident_scratch(B, dev)
         with torch.cuda.stream(stream):
-            host = torch.empty(2 * B + geom.size + n_cand, dtype=torch.int32, pin_memory=True)
+            host = torch.empty(2 * B + geom.size + n_cand + n_crop, dtype=torch.int32, pin_memory=True)
             h = host.numpy()
             h[:B], h[B:2 * B], h[2 * B:2 * B + geom.size] = idx, idx_bg, geom.ravel()
             if cand is not None:
-                h[2 * B + geom.size:] = cand.ravel()
+                h[2 * B + geom.size:2 * B + geom.size + n_cand] = cand.ravel()
+            if crop is not None:
+                h[2 * B + geom.size + n_cand:] = crop.ravel()
             host_lut = torch.empty(lut.size, dtype=torch.uint8, pin_memory=True)
             host_lut.numpy()[:] = lut.ravel()
             d = scratch["draws"][:host.numel()]
@@ -390,10 +410,11 @@ class Dataset(object):
             mask = None
             if cand is not None:
                 mask = scratch["mask"]
-                self._occlusion.apply_indexed(stacks["mask"], idx_d, d[2 * B + geom.size:], getattr(self, "occlusion_masks", None),
-                                              mask, stream)
+                self._occlusion.apply_indexed(stacks["mask"], idx_d, d[2 * B + geom.size:2 * B + geom.size + n_cand],
+                                              getattr(self, "occlusion_masks", None), mask, stream)
+            crop_d = d[2 * B + geom.size + n_cand:] if crop is not None else None
             self._aug.augment_indexed(stacks, idx_d, idx_bg_d, geom_d, lut_d, x_out, y_out, stream, mask_batch=mask,
-                                      tmp=scratch["tmp"])
+                                      tmp=scratch["tmp"], crop_d=crop_d, crop_tmp=scratch["crop"])
 
     def batch_resident(self, batch_size, device=None):
         """``batch_device`` on the stacks kept on the device by ``upload``: the same draws in the same order, so the same

@@ -16,12 +16,18 @@
 // All random draws (which ops fire, scales, masks, offsets, factors) are made on the host and arrive as per-image parameters,
 // so the kernels are deterministic and are checked bit for bit against a CPU restatement pinned to OpenCV (tests/).
 // Two passes: geometry (paste + warp + dropout) into a uint8 scratch image, then blur + tables.  HBM-bound: ~5 B/value.
+//
+// CropAndPad, when the chain has it (aae_augment_batch_crop / aae_augment_batch_indexed_crop), is a third pass in front: the
+// pasted image cropped and padded by per-image pixel counts, then resized back to H x W with cv2.resize's uint8 arithmetic --
+// INTER_CUBIC (11-bit fixed-point taps on clamped indices, integer horizontal sums, then the vertical sum in float32 as
+// OpenCV's vector path computes it: S0 b0 + (S1 b1 + (S2 b2 + S3 b3)), rounded to nearest even) or INTER_AREA (float32
+// weights, horizontal then vertical sums in OpenCV's order).  Flagged images (geom[0] & 8) are then read from its output.
 #include "common.cuh"
 
 namespace aae {
 namespace {
 
-constexpr int AUG_FLAG_AFFINE = 1, AUG_FLAG_DROP = 2, AUG_FLAG_BLUR = 4;
+constexpr int AUG_FLAG_AFFINE = 1, AUG_FLAG_DROP = 2, AUG_FLAG_BLUR = 4, AUG_FLAG_CROP = 8;
 
 struct AugGeomView {
   const int32_t* base;   // [4 + 2W + 2H] ints of this image: flags, keep_lo, keep_hi, 0, adelta[W], bdelta[W], X0[H], Y0[H]
@@ -48,6 +54,19 @@ __device__ __forceinline__ void fetch_pasted(const uint8_t* __restrict__ x, cons
   for (int c = 0; c < 4; ++c) v[c] = c < C ? src[pix * C + c] : 0;
 }
 
+// source pixel of the geometry pass: the crop-pad output of this image (ci, border 0) or the pasted image
+__device__ __forceinline__ void fetch_src(const uint8_t* __restrict__ ci, const uint8_t* __restrict__ x, const uint8_t* __restrict__ mask,
+                                          const uint8_t* __restrict__ bg, int H, int W, int C, int yy, int xx, int (&v)[4]) {
+  if (ci == nullptr) {
+    fetch_pasted(x, mask, bg, H, W, C, yy, xx, v);
+    return;
+  }
+  const bool in = yy >= 0 && yy < H && xx >= 0 && xx < W;
+  const long long pix = in ? (long long)yy * W + xx : 0;
+#pragma unroll
+  for (int c = 0; c < 4; ++c) v[c] = in && c < C ? ci[pix * C + c] : 0;
+}
+
 // stack row of batch image b: idx[b] when 0 <= idx[b] < n, -1 outside the stack; b itself without an index
 __device__ __forceinline__ long long stack_row(const int32_t* idx, long long n, long long b) {
   if (idx == nullptr) return b;
@@ -57,7 +76,8 @@ __device__ __forceinline__ long long stack_row(const int32_t* idx, long long n, 
 
 __global__ void aug_geometry_kernel(const uint8_t* __restrict__ x, const uint8_t* __restrict__ mask, const uint8_t* __restrict__ bg, int B, int H,
                                     int W, int C, const int32_t* __restrict__ geom, const unsigned short* __restrict__ tab, const uint8_t* __restrict__ row_cell,
-                                    const uint8_t* __restrict__ col_cell, int low_w, uint8_t* __restrict__ out, AugIndex ix) {
+                                    const uint8_t* __restrict__ col_cell, int low_w, const uint8_t* __restrict__ crop_img, uint8_t* __restrict__ out,
+                                    AugIndex ix) {
   const long long total = (long long)B * H * W;
   const long long plane = (long long)H * W;
   const int gstride = 4 + 2 * W + 2 * H;
@@ -72,29 +92,30 @@ __global__ void aug_geometry_kernel(const uint8_t* __restrict__ x, const uint8_t
     const uint8_t* xi = ok ? x + rx * plane * C : nullptr;
     const uint8_t* mi = ok ? mask + (ix.mask_gathered ? b : rx) * plane : nullptr;
     const uint8_t* bi = ok ? bg + rb * plane * C : nullptr;
+    const uint8_t* ci = (crop_img != nullptr && (flags & AUG_FLAG_CROP)) ? crop_img + b * plane * C : nullptr;
     int v[4];
     if (flags & AUG_FLAG_AFFINE) {
       const int X = (g.X0(yo) + g.adelta(xo)) >> 5, Y = (g.Y0(yo) + g.bdelta(xo)) >> 5;
       const int sx = X >> 5, sy = Y >> 5;
       const unsigned short* w4 = tab + (((Y & 31) << 5) | (X & 31)) * 4;
       int a[4], acc[4] = {0, 0, 0, 0};
-      fetch_pasted(xi, mi, bi, H, W, C, sy, sx, a);
+      fetch_src(ci, xi, mi, bi, H, W, C, sy, sx, a);
 #pragma unroll
       for (int c = 0; c < 4; ++c) acc[c] += a[c] * (int)w4[0];
-      fetch_pasted(xi, mi, bi, H, W, C, sy, sx + 1, a);
+      fetch_src(ci, xi, mi, bi, H, W, C, sy, sx + 1, a);
 #pragma unroll
       for (int c = 0; c < 4; ++c) acc[c] += a[c] * (int)w4[1];
-      fetch_pasted(xi, mi, bi, H, W, C, sy + 1, sx, a);
+      fetch_src(ci, xi, mi, bi, H, W, C, sy + 1, sx, a);
 #pragma unroll
       for (int c = 0; c < 4; ++c) acc[c] += a[c] * (int)w4[2];
-      fetch_pasted(xi, mi, bi, H, W, C, sy + 1, sx + 1, a);
+      fetch_src(ci, xi, mi, bi, H, W, C, sy + 1, sx + 1, a);
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
         acc[c] += a[c] * (int)w4[3];
         v[c] = min(255, max(0, (acc[c] + (1 << 14)) >> 15));
       }
     } else {
-      fetch_pasted(xi, mi, bi, H, W, C, yo, xo, v);
+      fetch_src(ci, xi, mi, bi, H, W, C, yo, xo, v);
     }
     if (flags & AUG_FLAG_DROP) {
       const int cell = (int)row_cell[yo] * low_w + (int)col_cell[xo];
@@ -104,6 +125,86 @@ __global__ void aug_geometry_kernel(const uint8_t* __restrict__ x, const uint8_t
       }
     }
     for (int c = 0; c < C; ++c) out[i * C + c] = (uint8_t)v[c];
+  }
+}
+
+// CropAndPad: CTA (b, chunk) writes output rows [8 chunk, 8 chunk + 8) of image b when its mode (crop[b][0]) is 1 (cubic) or
+// 2 (area).  The source rows those rows read -- rows of the pasted image shifted by (top, left), pad_cval outside it -- are
+// staged in shared memory as uint8 [rows][sw][C]; each output value then sums 4 x 4 taps of the row / column blocks of rs.
+constexpr int CROP_ROWS = 8;
+
+__global__ void __launch_bounds__(256) aug_crop_pad_kernel(const uint8_t* __restrict__ x, const uint8_t* __restrict__ mask,
+                                                           const uint8_t* __restrict__ bg, int H, int W, int C, const int32_t* __restrict__ crop,
+                                                           const int32_t* __restrict__ rs, long long rs_len, int max_rows, int max_w,
+                                                           uint8_t* __restrict__ out, AugIndex ix) {
+  extern __shared__ uint8_t src_rows[];
+  const long long b = blockIdx.x;
+  const int y0 = blockIdx.y * CROP_ROWS, y1 = min(H, y0 + CROP_ROWS);
+  const int32_t* ct = crop + b * 8;
+  const int mode = ct[0];
+  if (mode == 0) return;
+  const int sh = ct[1], sw = ct[2], top = ct[3], left = ct[4], cval = ct[5];
+  const long long yoff = ct[6], xoff = ct[7];
+  uint8_t* dst = out + (b * H + y0) * W * C;
+  const bool tab_ok = (mode == 1 || mode == 2) && sh >= 1 && sw >= 1 && sw <= max_w && yoff >= 0 && xoff >= 0 &&
+                      yoff + 8ll * H <= rs_len && xoff + 8ll * W <= rs_len;
+  const int32_t* ty = rs + (tab_ok ? yoff : 0);
+  const int32_t* tx = rs + (tab_ok ? xoff : 0);
+  const int r_lo = tab_ok ? ty[y0 * 8] : 0, r_hi = tab_ok ? ty[(y1 - 1) * 8 + 3] : -1;
+  const int nrows = r_hi - r_lo + 1;
+  if (!tab_ok || r_lo < 0 || r_hi >= sh || nrows > max_rows) {      // a table this launch was not sized for: zeros
+    for (int i = threadIdx.x; i < (y1 - y0) * W * C; i += blockDim.x) dst[i] = 0;
+    return;
+  }
+  const long long plane = (long long)H * W;
+  const long long rx = stack_row(ix.idx, ix.n_images, b), rb = stack_row(ix.idx_bg, ix.n_bg, b);
+  const bool ok = rx >= 0 && rb >= 0;
+  const uint8_t* xi = ok ? x + rx * plane * C : nullptr;
+  const uint8_t* mi = ok ? mask + (ix.mask_gathered ? b : rx) * plane : nullptr;
+  const uint8_t* bi = ok ? bg + rb * plane * C : nullptr;
+  for (int i = threadIdx.x; i < nrows * sw; i += blockDim.x) {
+    const int py = r_lo + i / sw - top, px = i % sw - left;
+    int v[4] = {cval, cval, cval, cval};
+    if (py >= 0 && py < H && px >= 0 && px < W) fetch_pasted(xi, mi, bi, H, W, C, py, px, v);
+    for (int c = 0; c < C; ++c) src_rows[i * C + c] = (uint8_t)v[c];
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < (y1 - y0) * W; i += blockDim.x) {
+    const int32_t* wy = ty + (y0 + i / W) * 8;
+    const int32_t* wx = tx + (i % W) * 8;
+    int ry[4], cx[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      ry[k] = min(max(wy[k] - r_lo, 0), nrows - 1) * sw;
+      cx[k] = min(max(wx[k], 0), sw - 1);
+    }
+    for (int c = 0; c < C; ++c) {
+      float f;
+      if (mode == 1) {
+        float h[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          int s = 0;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) s += (int)src_rows[(ry[k] + cx[j]) * C + c] * wx[4 + j];
+          h[k] = (float)s;                       // exact: |s| < 2^24
+        }
+        const float sc = 1.f / (2048.f * 2048.f);
+        const float b0 = __fmul_rn((float)wy[4], sc), b1 = __fmul_rn((float)wy[5], sc), b2 = __fmul_rn((float)wy[6], sc),
+                    b3 = __fmul_rn((float)wy[7], sc);
+        f = __fadd_rn(__fmul_rn(h[0], b0), __fadd_rn(__fmul_rn(h[1], b1), __fadd_rn(__fmul_rn(h[2], b2), __fmul_rn(h[3], b3))));
+      } else {
+        f = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          float buf = 0.f;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) buf = __fadd_rn(buf, __fmul_rn((float)src_rows[(ry[k] + cx[j]) * C + c], __int_as_float(wx[4 + j])));
+          f = __fadd_rn(f, __fmul_rn(__int_as_float(wy[4 + k]), buf));
+        }
+      }
+      dst[i * C + c] = (uint8_t)min(255, max(0, __float2int_rn(f)));
+    }
   }
 }
 
@@ -160,11 +261,20 @@ inline unsigned aug_grid(long long n) {
 
 }  // namespace
 
+size_t crop_pad_smem_bytes(int max_rows, int max_w, int C) { return (size_t)max_rows * max_w * C; }
+
 int launch_augment(const uint8_t* x, const uint8_t* mask, const uint8_t* bg, int B, int H, int W, int C, const int32_t* geom, const uint8_t* lut,
                    const unsigned short* tab, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, const int32_t* blur_q8, const float* to_float,
-                   uint8_t* tmp, uint8_t* out_u8, float* out_f32, cudaStream_t s, const AugIndex& ix) {
+                   uint8_t* tmp, uint8_t* out_u8, float* out_f32, cudaStream_t s, const AugIndex& ix, const AugCrop* crop) {
   AAE_REQUIRE(C >= 1 && C <= 4, "augment: %d channels unsupported (1..4)", C);
-  aug_geometry_kernel<<<aug_grid((long long)B * H * W), 256, 0, s>>>(x, mask, bg, B, H, W, C, geom, tab, row_cell, col_cell, low_w, tmp, ix);
+  if (crop != nullptr) {
+    const dim3 grid((unsigned)B, (unsigned)ceil_div(H, CROP_ROWS));
+    aug_crop_pad_kernel<<<grid, 256, crop_pad_smem_bytes(crop->max_rows, crop->max_w, C), s>>>(
+        x, mask, bg, H, W, C, crop->table, crop->resample, crop->resample_len, crop->max_rows, crop->max_w, crop->out, ix);
+    AAE_LAUNCH_OK();
+  }
+  aug_geometry_kernel<<<aug_grid((long long)B * H * W), 256, 0, s>>>(x, mask, bg, B, H, W, C, geom, tab, row_cell, col_cell, low_w,
+                                                                     crop ? crop->out : nullptr, tmp, ix);
   AAE_LAUNCH_OK();
   BlurTaps taps;
   for (int i = 0; i < 5; ++i) taps.k[i] = blur_q8 ? blur_q8[i] : (i == 2 ? 256 : 0);

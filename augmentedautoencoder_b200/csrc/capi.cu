@@ -724,10 +724,10 @@ extern "C" int aae_topk_merge_packed(const void* packed_dev, int n_shards, int b
 }
 
 // ============================================================================ training input pipeline
-extern "C" int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
-                                 const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev, const uint8_t* row_cell_dev,
-                                 const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8, const float* u8_to_float_dev,
-                                 uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, void* stream) {
+static int augment_gathered(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
+                            const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev, const uint8_t* row_cell_dev,
+                            const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8, const float* u8_to_float_dev,
+                            uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, cudaStream_t s, const AugCrop* crop) {
   AAE_REQUIRE(x_dev && mask_dev && bg_dev && geom_dev && lut_dev && bilinear_tab_dev && row_cell_dev && col_cell_dev && tmp_dev, "null argument");
   AAE_REQUIRE(out_u8_dev || out_f32_dev, "no output requested");
   AAE_REQUIRE(!out_f32_dev || u8_to_float_dev, "out_f32_dev needs u8_to_float_dev");
@@ -738,7 +738,48 @@ extern "C" int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, 
     AAE_REQUIRE(sum == 256, "blur kernel must sum to 256 (8 fractional bits), got %d", sum);
   }
   return launch_augment(x_dev, mask_dev, bg_dev, batch, h, w, c, geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w,
-                        blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, (cudaStream_t)stream);
+                        blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, s, AugIndex(), crop);
+}
+
+extern "C" int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
+                                 const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev, const uint8_t* row_cell_dev,
+                                 const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8, const float* u8_to_float_dev,
+                                 uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, void* stream) {
+  return augment_gathered(x_dev, mask_dev, bg_dev, batch, h, w, c, geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w,
+                          blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, (cudaStream_t)stream, nullptr);
+}
+
+// the CropAndPad arguments of the *_crop entry points: pointers present, and the staged rows within the 48 KB of shared memory
+static int crop_pad_checked(AugCrop& cp, const int32_t* crop_dev, const int32_t* resample_dev, int64_t resample_len, int max_src_rows,
+                            int max_src_w, uint8_t* crop_tmp_dev, int c) {
+  AAE_REQUIRE(crop_dev && resample_dev && crop_tmp_dev, "null argument");
+  AAE_REQUIRE(resample_len >= 1 && max_src_rows >= 1 && max_src_w >= 1, "bad crop-pad bounds (%lld table ints, %d rows, %d columns)",
+              (long long)resample_len, max_src_rows, max_src_w);
+  AAE_REQUIRE(c >= 1 && c <= 4, "augment: %d channels unsupported (1..4)", c);
+  const size_t smem = crop_pad_smem_bytes(max_src_rows, max_src_w, c);
+  if (smem > 48 * 1024) {
+    set_error("crop-pad: %d source rows of %d x %d bytes need %zu bytes of shared memory (48 KB supported)", max_src_rows, max_src_w, c, smem);
+    return AAE_ERR_UNSUPPORTED;
+  }
+  cp.table = crop_dev;
+  cp.resample = resample_dev;
+  cp.resample_len = resample_len;
+  cp.max_rows = max_src_rows;
+  cp.max_w = max_src_w;
+  cp.out = crop_tmp_dev;
+  return AAE_OK;
+}
+
+extern "C" int aae_augment_batch_crop(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
+                                      const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev, const uint8_t* row_cell_dev,
+                                      const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8, const float* u8_to_float_dev,
+                                      uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, const int32_t* crop_dev,
+                                      const int32_t* resample_dev, int64_t resample_len, int max_src_rows, int max_src_w, uint8_t* crop_tmp_dev,
+                                      void* stream) {
+  AugCrop cp;
+  AAE_TRY(crop_pad_checked(cp, crop_dev, resample_dev, resample_len, max_src_rows, max_src_w, crop_tmp_dev, c));
+  return augment_gathered(x_dev, mask_dev, bg_dev, batch, h, w, c, geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w,
+                          blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, (cudaStream_t)stream, &cp);
 }
 
 static int occlusion_checked(const uint8_t* mask_dev, int batch, int h, int w, const uint32_t* bank_dev, int n_bank, const int32_t* cand_dev,
@@ -774,13 +815,13 @@ extern "C" int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, 
                            row_cell_dev, col_cell_dev, low_h, low_w, mask_out_dev, fallbacks_dev, (cudaStream_t)stream, nullptr, 0);
 }
 
-extern "C" int aae_augment_batch_indexed(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
+static int augment_indexed(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
                                          const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
                                          const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
                                          const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
                                          const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
                                          const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
-                                         float* out_f32_dev, float* y_out_dev, void* stream) {
+                                         float* out_f32_dev, float* y_out_dev, cudaStream_t s, const AugCrop* crop) {
   AAE_REQUIRE(x_stack_dev && bg_stack_dev && idx_dev && idx_bg_dev && (mask_stack_dev || mask_batch_dev), "null argument");
   AAE_REQUIRE(!y_out_dev || (y_stack_dev && y_to_float_dev), "y_out_dev needs y_stack_dev and y_to_float_dev");
   AAE_REQUIRE(n_images >= 1 && n_bg >= 1, "empty image stack (%lld images, %lld backgrounds)", (long long)n_images, (long long)n_bg);
@@ -804,7 +845,35 @@ extern "C" int aae_augment_batch_indexed(const uint8_t* x_stack_dev, const uint8
   ix.y_out = y_out_dev;
   return launch_augment(x_stack_dev, mask_batch_dev ? mask_batch_dev : mask_stack_dev, bg_stack_dev, batch, h, w, c, geom_dev, lut_dev,
                         bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w, blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev,
-                        (cudaStream_t)stream, ix);
+                        s, ix, crop);
+}
+
+extern "C" int aae_augment_batch_indexed(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
+                                         const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
+                                         const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
+                                         const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
+                                         const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
+                                         const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
+                                         float* out_f32_dev, float* y_out_dev, void* stream) {
+  return augment_indexed(x_stack_dev, mask_stack_dev, bg_stack_dev, y_stack_dev, n_images, n_bg, idx_dev, idx_bg_dev, mask_batch_dev, batch, h, w, c,
+                         geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w, blur_kernel_q8, u8_to_float_dev,
+                         y_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, y_out_dev, (cudaStream_t)stream, nullptr);
+}
+
+extern "C" int aae_augment_batch_indexed_crop(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
+                                         const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
+                                         const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
+                                         const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
+                                         const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
+                                         const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
+                                         float* out_f32_dev, float* y_out_dev, const int32_t* crop_dev,
+                                              const int32_t* resample_dev, int64_t resample_len, int max_src_rows, int max_src_w,
+                                              uint8_t* crop_tmp_dev, void* stream) {
+  AugCrop cp;
+  AAE_TRY(crop_pad_checked(cp, crop_dev, resample_dev, resample_len, max_src_rows, max_src_w, crop_tmp_dev, c));
+  return augment_indexed(x_stack_dev, mask_stack_dev, bg_stack_dev, y_stack_dev, n_images, n_bg, idx_dev, idx_bg_dev, mask_batch_dev, batch, h, w, c,
+                         geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w, blur_kernel_q8, u8_to_float_dev,
+                         y_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, y_out_dev, (cudaStream_t)stream, &cp);
 }
 
 extern "C" int aae_augment_occlusion_indexed(const uint8_t* mask_stack_dev, int64_t n_images, const int32_t* idx_dev, int batch, int h, int w,

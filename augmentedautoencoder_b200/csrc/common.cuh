@@ -202,9 +202,19 @@ struct AugIndex {
   const float* y_to_float = nullptr;
   float* y_out = nullptr;
 };
+// CropAndPad pass in front of the geometry pass (aae_augment_batch_crop): per-image table [B][8], resampling blocks, the bound on
+// staged source rows / row width the launch's shared memory is sized for, and its uint8 [B][H][W][C] output
+struct AugCrop {
+  const int32_t* table = nullptr;
+  const int32_t* resample = nullptr;
+  long long resample_len = 0;
+  int max_rows = 0, max_w = 0;
+  uint8_t* out = nullptr;
+};
+size_t crop_pad_smem_bytes(int max_rows, int max_w, int C);
 int launch_augment(const uint8_t* x, const uint8_t* mask, const uint8_t* bg, int B, int H, int W, int C, const int32_t* geom, const uint8_t* lut,
                    const unsigned short* tab, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, const int32_t* blur_q8, const float* to_float,
-                   uint8_t* tmp, uint8_t* out_u8, float* out_f32, cudaStream_t s, const AugIndex& ix = AugIndex());
+                   uint8_t* tmp, uint8_t* out_u8, float* out_f32, cudaStream_t s, const AugIndex& ix = AugIndex(), const AugCrop* crop = nullptr);
 // occlusion-mask augmentations (occlusion.cu); idx (optional, n_images rows): image b's mask is row idx[b] of the mask stack
 size_t occlusion_smem_bytes(int H, int W, int low_w);
 int launch_occlusion(const uint8_t* mask, int B, int H, int W, const uint32_t* bank, int n_bank, const int32_t* cand, int K, int realistic,

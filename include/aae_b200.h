@@ -253,6 +253,27 @@ AAE_API int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, con
                               const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
                               const float* u8_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, void* stream);
 
+/* aae_augment_batch with CropAndPad in front (the training template's optional Sometimes(0.5, CropAndPad(percent=(-0.05, 0.1))),
+ * imgaug's crop-pad-resize at keep_size=True): image b, when crop_dev[b][0] != 0, is the pasted image cropped / padded and resized
+ * back to H x W before the geometry pass, which then reads it for the images whose geom flags have bit 8 set (set it exactly for
+ * those images).  crop_dev int32 [B][8] per image:
+ *   [0] 0 off, 1 INTER_CUBIC, 2 INTER_AREA (cv2.resize's uint8 arithmetic);  [1] sh, [2] sw: size after crop and pad;
+ *   [3] top, [4] left: signed pixels (negative = crop, positive = pad; source pixel (qy, qx) is pasted (qy - top, qx - left),
+ *       pad_cval outside the image);  [5] pad_cval (0..255, all channels);  [6], [7]: offsets into resample_dev of the row
+ *       block (H entries) and the column block (W entries).
+ * resample_dev int32 [resample_len]: blocks of [dst][8] = 4 source indices (non-decreasing; in range of sh / sw) then 4 weights:
+ *   cubic: fixed-point ints with 11 fractional bits; area: float32 bit patterns in OpenCV's summation order (unused taps weight 0).
+ * max_src_rows / max_src_w bound the source rows one 8-row output band reads and sw; max_src_rows * max_src_w * c above 48 KB:
+ * AAE_ERR_UNSUPPORTED.  An entry that breaks these bounds or its table's range writes zeros.  crop_tmp_dev: uint8 [B][H][W][C]
+ * scratch of the pass.  Same stream rules as every input-pipeline call: every launch on `stream`, no allocation, no
+ * synchronisation. */
+AAE_API int aae_augment_batch_crop(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
+                                   const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
+                                   const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
+                                   const float* u8_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev,
+                                   const int32_t* crop_dev, const int32_t* resample_dev, int64_t resample_len, int max_src_rows,
+                                   int max_src_w, uint8_t* crop_tmp_dev, void* stream);
+
 /* The occlusion switches of the training cfg, applied to the masks before aae_augment_batch (auto_pose/ae/dataset.py:421-454,
  * called at dataset.py:468-471).  mask_dev / mask_out_dev: uint8 [B][H][W], nonzero = BACKGROUND (the reference's mask_x);
  * mask_out_dev receives 0 / 1.  cand_dev: int32 [B][1 + 3K] per image, every draw made by the caller:
@@ -292,6 +313,16 @@ AAE_API int aae_augment_batch_indexed(const uint8_t* x_stack_dev, const uint8_t*
                                       const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
                                       const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
                                       float* out_f32_dev, float* y_out_dev, void* stream);
+/* aae_augment_batch_indexed with the CropAndPad pass of aae_augment_batch_crop (same crop arguments).  An image outside its
+ * stack is pasted as zeros, and its crop and pad (pad_cval) still apply. */
+AAE_API int aae_augment_batch_indexed_crop(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
+                                           const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
+                                           const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
+                                           const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
+                                           const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
+                                           const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
+                                           float* out_f32_dev, float* y_out_dev, const int32_t* crop_dev, const int32_t* resample_dev,
+                                           int64_t resample_len, int max_src_rows, int max_src_w, uint8_t* crop_tmp_dev, void* stream);
 AAE_API int aae_augment_occlusion_indexed(const uint8_t* mask_stack_dev, int64_t n_images, const int32_t* idx_dev, int batch, int h, int w,
                                           const uint32_t* bank_dev, int n_bank, const int32_t* cand_dev, int n_cand, int realistic,
                                           double max_occl, int square, double min_kept, const uint8_t* row_cell_dev,

@@ -107,7 +107,7 @@ def batch_device_parts(ds, dev, n=30):
     draws, gather, upload, whole = [], [], [], []
     for _ in range(n):
         t0 = time.perf_counter()
-        idx, idx_bg, _, _, _ = ds._draws(B)
+        idx, idx_bg = ds._draws(B)[:2]
         t1 = time.perf_counter()
         parts = [ds.train_x[idx], np.ascontiguousarray(ds.mask_x[idx]).astype(np.uint8), ds.bg_imgs[idx_bg], ds.train_y[idx]]
         t2 = time.perf_counter()
