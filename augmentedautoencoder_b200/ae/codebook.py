@@ -75,7 +75,10 @@ class Codebook(object):
         return self._handles[dev][0]
 
     def match_device(self, z_dev, k=1, upright=False):
-        """z_dev: CUDA tensor [B, J] (un-normalised latent).  Returns (scores [B,k] float32, idx [B,k] int32) on the device."""
+        """z_dev: CUDA tensor [B, J] (un-normalised latent).  Returns (scores [B,k] float32, idx [B,k] int32) on the device:
+        scores descending, ties to the lowest index, positions past the eligible rows (-inf, -1).  ``upright`` restricts the
+        search to every num_cyclo-th row for every k -- this device API's own choice; ``nearest_rotation`` follows the
+        reference and applies it for top_n == 1 only."""
         dev = z_dev.device
         h = self.handle(dev)
         B = z_dev.shape[0]
@@ -89,7 +92,8 @@ class Codebook(object):
         return scores, idx
 
     def nearest_idx_device(self, x_dev, k=1, upright=False):
-        """crops (CUDA uint8/float32 NHWC) -> (scores, idx) without leaving the device: encoder + fused match."""
+        """crops (CUDA uint8/float32 NHWC) -> (scores, idx) without leaving the device: encoder + fused match (``upright`` for
+        every k, as in ``match_device``)."""
         return self.match_device(self._encoder.encode_device(x_dev), k, upright)
 
     def _match(self, ctx, k, upright):
@@ -114,14 +118,15 @@ class Codebook(object):
     # ------------------------------------------------------------------ reference surface
     def nearest_rotation(self, session, x, top_n=1, upright=False, return_idcs=False):
         """R_model2cam of the best codebook row(s) (auto_pose/ae/codebook.py:55-75).  uint8 crops are divided by 255 inside
-        the first kernel (a true fp32 divide -- identical to the reference's float64 x/255. rounded at the feed)."""
+        the first kernel (a true fp32 divide -- identical to the reference's float64 x/255. rounded at the feed).  As in the
+        reference, ``upright`` applies to top_n == 1 only: top_n > 1 ranks every row."""
         if not isinstance(x, torch.Tensor):
             x = np.asarray(x)
         if x.ndim == 3:
             x = x[None]
         xd = to_device_input(x, session.device)
         with torch.cuda.device(session.device):
-            _, idx = self.nearest_idx_device(xd, k=top_n, upright=upright)
+            _, idx = self.nearest_idx_device(xd, k=top_n, upright=upright and top_n == 1)
         idx = idx.cpu().numpy().astype(np.int64)
         self._encoder.check_range(session.device)      # synchronised by the copy above: out-of-range activations raise instead of passing as indices
         if top_n == 1:

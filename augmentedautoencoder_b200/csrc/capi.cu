@@ -635,7 +635,7 @@ extern "C" int aae_codebook_create(int device, const float* embedding_any, int64
     if (e != cudaSuccess) { set_error("codebook upload failed: %s", cudaGetErrorString(e)); st = AAE_ERR_CUDA; }
   }
   if (st == AAE_OK && precision != AAE_PREC_FP32_SIMT)
-    st = tc_codebook_create(device, h->E.p, n_rows, latent, num_cyclo, max_batch, tc_planes(precision), &h->tc);
+    st = tc_codebook_create(device, h->E.p, n_rows, row_offset, latent, num_cyclo, max_batch, tc_planes(precision), &h->tc);
   if (st == AAE_OK) st = creation_fence("aae_codebook_create");
   if (st != AAE_OK) { aae_codebook_destroy(h); return st; }
   *out = h;
@@ -682,8 +682,8 @@ extern "C" int aae_codebook_match(aae_codebook* h, const float* z_dev, int batch
   AAE_REQUIRE(k >= 1 && k <= h->n_rows, "k=%d outside [1, n_rows]", k);
   DeviceGuard g(h->device);
   cudaStream_t s = (cudaStream_t)stream;
-  // tensor-core kernel: k <= 8, with or without `upright` (codebook.py:64-71) -- one fused launch, nothing else
-  if (h->tc && k <= tc_codebook_max_k() && (!upright || h->row_offset % h->num_cyclo == 0)) {
+  // tensor-core kernel: k <= 8, with or without `upright` (codebook.py:64-71), for a shard at any offset -- one fused launch
+  if (h->tc && k <= tc_codebook_max_k() && (!upright || tc_codebook_has_upright(h->tc))) {
     h->timer.reset();
     h->timer.mark(s);
     AAE_TRY(tc_codebook_match(h->tc, z_dev, batch, h->row_offset, k, upright, scores_out_dev, idx_out_dev, s));

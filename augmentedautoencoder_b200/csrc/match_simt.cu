@@ -114,10 +114,14 @@ __global__ void match_final_kernel(const float* __restrict__ partial_s, const in
     const int i = __shfl_xor_sync(0xffffffffu, bi, o);
     if (better(s, i, bs, bi)) { bs = s; bi = i; }
   }
-  if (lane == 0) { scores_out[q] = bs; idx_out[q] = bi; }
+  if (lane == 0) {                       // no eligible row (an `upright` shard without upright rows): the empty slot (-inf, -1)
+    scores_out[q] = bi == INT_MAX ? -INFINITY : bs;
+    idx_out[q] = bi == INT_MAX ? -1 : bi;
+  }
 }
 
-// k passes of a constrained block-wide argmax over one cosine row: output sorted by (score desc, index asc).
+// k passes of a constrained block-wide argmax over one cosine row: output sorted by (score desc, index asc); slots past the
+// eligible rows are (-inf, -1), as the fused kernel writes them.
 __global__ void __launch_bounds__(1024) topk_from_cos_kernel(const float* __restrict__ cos, long long n_rows, long long row_offset,
                                                              int num_cyclo, int upright, int k, float* __restrict__ scores_out,
                                                              int* __restrict__ idx_out) {
@@ -151,7 +155,7 @@ __global__ void __launch_bounds__(1024) topk_from_cos_kernel(const float* __rest
     if (threadIdx.x == 0) {
       for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
         if (better(ws[w], wi[w], ws[0], wi[0])) { ws[0] = ws[w]; wi[0] = wi[w]; }
-      scores_out[(long long)blockIdx.x * k + j] = ws[0];
+      scores_out[(long long)blockIdx.x * k + j] = wi[0] == INT_MAX ? -INFINITY : ws[0];
       idx_out[(long long)blockIdx.x * k + j] = wi[0] == INT_MAX ? -1 : wi[0];
       prev_s = ws[0];
       prev_i = wi[0];
@@ -179,7 +183,7 @@ __global__ void topk_merge_kernel(const float* __restrict__ s_in, const int* __r
       if (better(s_in[o], idx, bs, bi)) { bs = s_in[o]; bi = idx; bsh = s; }
     }
     if (bsh >= 0) head[bsh]++;
-    s_out[(long long)q * k + j] = bs;
+    s_out[(long long)q * k + j] = bsh >= 0 ? bs : -INFINITY;
     i_out[(long long)q * k + j] = bsh >= 0 ? bi : -1;
   }
 }

@@ -66,11 +66,14 @@ int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s);
 int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, float* db_out, cudaStream_t s);
 int tc_train_unpack_flat(TcTrainPlan* h, int B, float* out, cudaStream_t s);
 
-// planes: 2 = (hi, lo) codebook and three products per k-step (AAE_PREC_TC_SPLIT), 1 = hi only, one product (AAE_PREC_TC_FP16)
-int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int latent, int num_cyclo, int max_batch, int planes,
-                       TcCodebook** out);
+// planes: 2 = (hi, lo) codebook and three products per k-step (AAE_PREC_TC_SPLIT), 1 = hi only, one product (AAE_PREC_TC_FP16).
+// row_offset: global index of row 0 (a shard); it places the `upright` rows, whose global index is a multiple of num_cyclo.
+int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int64_t row_offset, int latent, int num_cyclo, int max_batch,
+                       int planes, TcCodebook** out);
 void tc_codebook_destroy(TcCodebook* h);
 int tc_codebook_max_k();
+// false when an `upright` search of this (shard of a) codebook has no row to visit
+bool tc_codebook_has_upright(const TcCodebook* h);
 int tc_launch_floor_probe(int device, int with_tmem, cudaStream_t s);
 // fused normalise + scores + top-k (k <= tc_codebook_max_k()), optionally over every num_cyclo-th row only (upright)
 int tc_codebook_match(TcCodebook* h, const float* z_dev, int B, int64_t row_offset, int k, int upright, float* scores_out, int32_t* idx_out,

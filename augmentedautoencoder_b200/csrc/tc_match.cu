@@ -337,7 +337,8 @@ struct TcCodebook {
   int device;
   long long n_rows, n_pad;
   int n_tiles, max_batch, sm_count, num_cyclo;
-  long long n_up;                 // rows of the `upright` view (every num_cyclo-th row)
+  long long up_first;             // local index of the first upright row: (-row_offset) mod num_cyclo
+  long long n_up;                 // rows of the `upright` view (every num_cyclo-th row from up_first; 0 when the shard has none)
   int n_tiles_up;
   int planes;                     // 2: (hi, lo) codebook (AAE_PREC_TC_SPLIT); 1: hi only (AAE_PREC_TC_FP16), no lo plane
   TcPlanes e;
@@ -366,8 +367,8 @@ int tc_launch_floor_probe(int device, int with_tmem, cudaStream_t s) {
   return AAE_OK;
 }
 
-int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int latent, int num_cyclo, int max_batch, int planes,
-                       TcCodebook** out) {
+int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int64_t row_offset, int latent, int num_cyclo, int max_batch,
+                       int planes, TcCodebook** out) {
   *out = nullptr;
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   if (latent != 128) {
@@ -382,7 +383,8 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
   h->n_pad = (long long)h->n_tiles * MT_ROWS;
   h->max_batch = max_batch;
   h->num_cyclo = std::max(1, num_cyclo);
-  h->n_up = ceil_div(n_rows, (int64_t)h->num_cyclo);
+  h->up_first = (h->num_cyclo - row_offset % h->num_cyclo) % h->num_cyclo;
+  h->n_up = n_rows > h->up_first ? ceil_div(n_rows - h->up_first, (int64_t)h->num_cyclo) : 0;
   h->n_tiles_up = (int)ceil_div(h->n_up, (int64_t)MT_ROWS);
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, device);
@@ -403,12 +405,15 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int laten
   const uint64_t strides[1] = {256};
   const uint32_t box[2] = {64, MT_ROWS};
   int st = h->e.encode(h->tm, 2, dims, strides, box);
-  if (st == AAE_OK && h->num_cyclo > 1) {
-    // `upright` view (codebook.py:66 cos[::num_cyclo]): the same memory with a row stride of num_cyclo rows; boxes past
-    // the last such row are zero-filled by TMA and masked by the kernel
+  if (st == AAE_OK && h->num_cyclo > 1 && h->n_up > 0) {
+    // `upright` view (codebook.py:66 cos[::num_cyclo]): the same memory from the shard's first upright row on, with a row
+    // stride of num_cyclo rows; boxes past the last such row are zero-filled by TMA and masked by the kernel
+    TcPlanes view = h->e;                               // (a view: no ownership, never released)
+    view.hi += h->up_first * 128;
+    if (view.lo) view.lo += h->up_first * 128;
     const uint64_t dims_u[2] = {128, (uint64_t)h->n_up};
     const uint64_t strides_u[1] = {(uint64_t)256 * (uint64_t)h->num_cyclo};
-    st = h->e.encode(h->tm_up, 2, dims_u, strides_u, box);
+    st = view.encode(h->tm_up, 2, dims_u, strides_u, box);
     h->have_up = st == AAE_OK;
   }
   if (st != AAE_OK) { tc_codebook_destroy(h); return st; }
@@ -429,17 +434,20 @@ void tc_codebook_destroy(TcCodebook* h) {
   delete h;
 }
 
-// k in [1, 8]; upright != 0 searches rows (row_offset + r * num_cyclo) only -- needs row_offset % num_cyclo == 0 (shard_bounds aligns shards so)
+bool tc_codebook_has_upright(const TcCodebook* h) { return h->num_cyclo == 1 || h->have_up; }
+
+// k in [1, 8]; upright != 0 searches the rows whose global index (row_offset + local row) is a multiple of num_cyclo only:
+// local rows up_first + r * num_cyclo, which the create-time view holds whatever the shard's offset
 int tc_codebook_match(TcCodebook* h, const float* z_dev, int B, int64_t row_offset, int k, int upright, float* scores_out, int32_t* idx_out,
                       cudaStream_t s) {
   AAE_REQUIRE(k >= 1 && k <= MT_KMAX, "tc match: k=%d outside [1, %d]", k, MT_KMAX);
-  AAE_REQUIRE(!upright || (h->have_up || h->num_cyclo == 1), "tc match: no upright view");
-  AAE_REQUIRE(!upright || row_offset % h->num_cyclo == 0, "tc match: upright needs a shard offset that is a multiple of num_cyclo");
+  AAE_REQUIRE(!upright || tc_codebook_has_upright(h), "tc match: no upright row in this codebook");
   AAE_REQUIRE(B <= h->max_batch || k == 1, "tc match: batch %d > max_batch %d", B, h->max_batch);
   const bool up = upright && h->num_cyclo > 1;
   const int n_tiles = up ? h->n_tiles_up : h->n_tiles;
   const int n_rows = (int)(up ? h->n_up : h->n_rows);
   const int idx_mul = up ? h->num_cyclo : 1;
+  if (up) row_offset += h->up_first;
   const TcMaps& tm = up ? h->tm_up : h->tm;
   const int grid = std::min(h->sm_count, n_tiles);
   for (int a = 0; a < B; a += MT_BATCH) {

@@ -20,6 +20,8 @@ import torch.distributed as dist
 
 from . import _lib
 
+TC_MAX_K = 8   # aae_codebook_match runs k <= 8 on a tensor-core handle's fused kernel, larger k on the fp32 kernels
+
 
 # --------------------------------------------------------------------------------------------------------- partitioning
 def shard_bounds(n_rows, world_size, rank, align=1):
@@ -78,6 +80,7 @@ class ShardedCodebook:
         self.device = device
         self._local = np.ascontiguousarray(emb)
         self._handle = None
+        self._handle32 = None
         self._setup()
 
     # -- device hooks (overridden by the CPU/gloo tests with host stand-ins) -----------------------------------------
@@ -99,7 +102,10 @@ class ShardedCodebook:
 
     def _local_match(self, z, k, upright, s_out, i_out):
         """z [B, J] on self.device -> this shard's top-k written into s_out [B, k] float32 / i_out [B, k] int32 (global row
-        indices); list positions past the shard's size, and every position of an empty shard, hold (-inf, -1)."""
+        indices); list positions past the shard's eligible rows, and every position of an empty shard, hold (-inf, -1).
+        On a tensor-core shard with fewer rows than k, for k > 8, the first call creates a second, fp32 handle over the
+        shard's rows (``_fp32_handle``): that call waits for the whole device once, and the shard then holds a second copy
+        of its rows plus that handle's workspace."""
         B = z.shape[0]
         kk = min(k, self.hi - self.lo) if self._handle is not None else 0
         if kk < k:
@@ -107,16 +113,33 @@ class ShardedCodebook:
             i_out.fill_(-1)
             if kk == 0:
                 return
+        handle = self._handle
+        if kk < k and k > TC_MAX_K and self.precision != _lib.PREC_FP32_SIMT:
+            # a tensor-core handle scores k > 8 on the fp32 kernels and k <= 8 on the fused one: a shard shorter than k asks
+            # for kk <= 8 rows but must score them as the unsharded handle scores k, or the merge is not bit-identical
+            handle = self._fp32_handle()
         direct = kk == k and s_out.is_contiguous() and i_out.is_contiguous()
         s_loc = s_out if direct else torch.empty((B, kk), dtype=torch.float32, device=z.device)
         i_loc = i_out if direct else torch.empty((B, kk), dtype=torch.int32, device=z.device)
         stream = C.c_void_p(torch.cuda.current_stream(z.device).cuda_stream)
         for a in range(0, B, self.max_batch):
             e = min(B, a + self.max_batch)
-            _lib.check(_lib.lib().aae_codebook_match(self._handle, _lib.ptr(z[a:e]), e - a, kk, int(bool(upright)), _lib.ptr(s_loc[a:e]),
+            _lib.check(_lib.lib().aae_codebook_match(handle, _lib.ptr(z[a:e]), e - a, kk, int(bool(upright)), _lib.ptr(s_loc[a:e]),
                                                      _lib.ptr(i_loc[a:e]), stream), "sharded match")
         if not direct:
             s_out[:, :kk], i_out[:, :kk] = s_loc, i_loc
+
+    def _fp32_handle(self):
+        """AAE_PREC_FP32_SIMT handle over this shard's rows, created on first use.  aae_codebook_create ends in
+        cudaDeviceSynchronize, so the first use waits for the whole device."""
+        if self._handle32 is None:
+            h = C.c_void_p()
+            with torch.cuda.device(self.device):
+                _lib.check(_lib.lib().aae_codebook_create(self.device.index, _lib.ptr(self._local), self._local.shape[0], self.latent,
+                                                          self.num_cyclo, self.lo, self.max_batch, _lib.PREC_FP32_SIMT, C.byref(h)),
+                           "sharded codebook create")
+            self._handle32 = h
+        return self._handle32
 
     def _merge(self, packed):
         """[W, 2, B, k] gathered exchange buffers (plane 0 = float32 score bits, plane 1 = int32 global indices) -> [B, k]:
@@ -132,7 +155,9 @@ class ShardedCodebook:
     def match(self, z, k=1, upright=False):
         """Every rank passes the same queries z [B, J]; every rank gets the global (scores [B,k], idx [B,k]).
         ONE collective: the shard's scores and indices are produced side by side in one [2, B, k] buffer (8 bytes per entry)
-        and all-gathered together -- the exchange is pure latency, so one NCCL call instead of two halves its cost."""
+        and all-gathered together -- the exchange is pure latency, so one NCCL call instead of two halves its cost.
+        A tensor-core shard with fewer rows than k > 8 creates an fp32 handle on its first such call, which waits for the
+        whole device once (``_local_match``)."""
         z = z.contiguous()
         B = z.shape[0]
         pk = torch.empty((2, B, k), dtype=torch.int32, device=z.device)
@@ -160,9 +185,10 @@ class ShardedCodebook:
         return self.match(all_z[:batch_total], k, upright)
 
     def close(self):
-        if self._handle is not None:
-            _lib.lib().aae_codebook_destroy(self._handle)
-            self._handle = None
+        for name in ("_handle", "_handle32"):
+            if getattr(self, name, None) is not None:
+                _lib.lib().aae_codebook_destroy(getattr(self, name))
+                setattr(self, name, None)
 
     def __del__(self):
         try:

@@ -24,9 +24,12 @@
  *     Forwards, match, losses, input-pipeline calls and the training entry points do not wait for
  *     the device; calls that hand data to the host (*_set_weights, *_get_weights, *_range_status,
  *     aae_trainer_get_grads, aae_trainer_{get,set}_state, the *_profile reads) wait for their own
- *     stream only.  Two exceptions wait for the whole device: aae_encoder_activation (it takes no
- *     stream), and a forward that has to grow a tensor-core scratch buffer (the first one at a
- *     larger batch).
+ *     stream only.  Three exceptions wait for the whole device: aae_encoder_activation (it takes no
+ *     stream), a forward that has to grow a tensor-core scratch buffer (the first one at a
+ *     larger batch), and the first aae_codebook_match on a handle that takes the cosine-matrix
+ *     route (k > 1 on an AAE_PREC_FP32_SIMT handle, k > 8 on a tensor-core one, or k > 1 with
+ *     `upright` on a shard without upright rows): it allocates the handle's [max_batch, n_rows]
+ *     cosine buffer.
  *   - creation is complete on return: aae_*_create* and aae_*_enable_*_head fill what they
  *     allocate on the legacy default stream and end with one cudaDeviceSynchronize, so the new
  *     object can be used on any stream at once.
@@ -177,21 +180,28 @@ AAE_API int aae_codebook_destroy(aae_codebook* h);
 AAE_API int aae_l2_normalize(const float* z_dev, int batch, int latent, float* zq_out_dev, void* stream);
 /* Fused normalise + score + top-k: for every query the k best rows, scores descending, ties broken
  * towards the LOWEST index (np.argmax semantics, codebook.py:64-68).  upright != 0 restricts the
- * search to rows with (global index % num_cyclo) == 0 (codebook.py:66).  The [B,N] cosine matrix is
- * never materialised.  scores_out_dev [B,k] float32, idx_out_dev [B,k] int32 (global row index). */
+ * search to rows with (global index % num_cyclo) == 0 (codebook.py:66), for any row_offset, and for
+ * every k: the device API applies it to top-k lists too (Codebook.nearest_rotation, like the
+ * reference, passes it for k = 1 only).  k in [1, n_rows]: list positions past the eligible rows
+ * (k above the upright rows) are the empty slot (score -inf, index -1), on every precision.
+ * k <= 8 on a tensor-core handle is one fused launch and never materialises the [B,N] cosine matrix;
+ * other k (and k > 1 on AAE_PREC_FP32_SIMT) score the full matrix into the handle's buffer, then
+ * select.  scores_out_dev [B,k] float32, idx_out_dev [B,k] int32 (global row index). */
 AAE_API int aae_codebook_match(aae_codebook* h, const float* z_dev, int batch, int k, int upright,
                                float* scores_out_dev, int32_t* idx_out_dev, void* stream);
 /* Full cosine matrix [B, n_rows] = `session.run(codebook.cos_similarity)` (codebook.py:50,63). */
 AAE_API int aae_codebook_cosine(aae_codebook* h, const float* z_dev, int batch, float* cos_out_dev, void* stream);
 /* Merge per-shard top-k lists (all-gathered over NCCL by the host): in [n_shards,B,k] -> out [B,k];
  * equal scores resolve to the lowest global index, so the result is bit-identical to the
- * unsharded match. */
+ * unsharded match of the same precision.  An input entry with index -1 is an empty slot and is
+ * skipped; output positions no shard fills are (-inf, -1). */
 AAE_API int aae_topk_merge(const float* scores_dev, const int32_t* idx_dev, int n_shards, int batch, int k,
                            float* scores_out_dev, int32_t* idx_out_dev, void* stream);
 /* Same merge for the single-collective exchange: every rank's match writes its scores and indices into ONE buffer
  * [2][B][k] (plane 0 float32 scores, plane 1 int32 global indices -- 8 bytes per (query, k)), one NCCL all-gather
  * concatenates them to packed_dev = [n_shards][2][B][k].  Halves the collective count of the row-sharded path, whose
- * whole cost is collective latency (SURVEY.md 8e row 3; no reference counterpart: codebook.py:63-71 is single-device). */
+ * whole cost is collective latency (SURVEY.md 8e row 3; no reference counterpart: codebook.py:63-71 is single-device).
+ * Empty slots as in aae_topk_merge: skipped on input, (-inf, -1) on output. */
 AAE_API int aae_topk_merge_packed(const void* packed_dev, int n_shards, int batch, int k,
                                   float* scores_out_dev, int32_t* idx_out_dev, void* stream);
 AAE_API int64_t aae_codebook_rows(const aae_codebook* h);
