@@ -34,6 +34,49 @@ class Optimizer(C.Structure):
     _fields_ = [("kind", C.c_int32), ("learning_rate", C.c_float), ("hp", C.c_float * 4)]
 
 
+class _Args(C.Structure):
+    """Argument struct of an input-pipeline call: struct_size is filled in, and a field given a tensor or array takes its
+    address (None: NULL)."""
+
+    def __init__(self, **fields):
+        super().__init__(struct_size=C.sizeof(type(self)))
+        self.set(**fields)
+
+    def set(self, **fields):
+        for name, v in fields.items():
+            setattr(self, name, v if v is None or isinstance(v, (int, float)) else ptr(v).value)
+        return self
+
+    def copy(self):
+        return type(self).from_buffer_copy(self)
+
+
+class AugmentArgs(_Args):
+    """aae_augment_args"""
+    _fields_ = [("struct_size", C.c_int32),
+                ("batch", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("c", C.c_int32), ("low_w", C.c_int32),
+                ("x", C.c_void_p), ("mask", C.c_void_p), ("bg", C.c_void_p), ("y", C.c_void_p), ("idx", C.c_void_p),
+                ("idx_bg", C.c_void_p), ("n_images", C.c_int64), ("n_bg", C.c_int64), ("mask_batch", C.c_void_p),
+                ("geom", C.c_void_p), ("lut", C.c_void_p), ("crop", C.c_void_p),
+                ("bilinear_tab", C.c_void_p), ("row_cell", C.c_void_p), ("col_cell", C.c_void_p), ("blur_kernel_q8", C.c_void_p),
+                ("u8_to_float", C.c_void_p), ("y_to_float", C.c_void_p), ("resample", C.c_void_p), ("resample_len", C.c_int64),
+                ("max_src_rows", C.c_int32), ("max_src_w", C.c_int32),
+                ("tmp", C.c_void_p), ("crop_tmp", C.c_void_p),
+                ("out_u8", C.c_void_p), ("out_f32", C.c_void_p), ("y_out", C.c_void_p)]
+
+
+class OcclusionArgs(_Args):
+    """aae_occlusion_args"""
+    _fields_ = [("struct_size", C.c_int32),
+                ("batch", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
+                ("realistic", C.c_int32), ("square", C.c_int32), ("max_occl", C.c_double), ("min_kept", C.c_double),
+                ("mask", C.c_void_p), ("idx", C.c_void_p), ("n_images", C.c_int64),
+                ("cand", C.c_void_p), ("n_cand", C.c_int32),
+                ("n_bank", C.c_int32), ("bank", C.c_void_p), ("row_cell", C.c_void_p), ("col_cell", C.c_void_p),
+                ("low_h", C.c_int32), ("low_w", C.c_int32),
+                ("mask_out", C.c_void_p), ("fallbacks", C.c_void_p)]
+
+
 _P = C.c_void_p
 _I = C.c_int
 _L = C.c_int64
@@ -91,14 +134,8 @@ _SIGS = {
     "aae_trainer_set_latent_terms": (_I, [_P, _F, _F]),
     "aae_trainer_set_latent_noise": (_I, [_P, _F]),
     "aae_extract_square_patches": (_I, [_P, _I, _I, _P, _I, _F, _I, _P, _P]),
-    "aae_augment_batch": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P]),
-    "aae_augment_occlusion": (_I, [_P, _I, _I, _I, _P, _I, _P, _I, _I, _D, _I, _D, _P, _P, _I, _I, _P, _P, _P]),
-    "aae_augment_batch_indexed": (_I, [_P, _P, _P, _P, _L, _L, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P,
-                                       _P, _P, _P]),
-    "aae_augment_batch_crop": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _L, _I, _I, _P, _P]),
-    "aae_augment_batch_indexed_crop": (_I, [_P, _P, _P, _P, _L, _L, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _I, _P, _P, _P, _P,
-                                            _P, _P, _P, _P, _P, _L, _I, _I, _P, _P]),
-    "aae_augment_occlusion_indexed": (_I, [_P, _L, _P, _I, _I, _I, _P, _I, _P, _I, _I, _D, _I, _D, _P, _P, _I, _I, _P, _P, _P]),
+    "aae_augment": (_I, [C.POINTER(AugmentArgs), _P]),
+    "aae_occlusion": (_I, [C.POINTER(OcclusionArgs), _P]),
 }
 
 _lib = None

@@ -3,7 +3,7 @@ paste by mask + the imgaug chain the training cfg names under ``[Augmentation] C
 
 The cfg string is evaluated against recording stand-ins for the imgaug classes (imgaug itself is not needed), the per-image
 random draws are made here with numpy (same distributions as imgaug's stochastic parameters, not its random stream), and
-``aae_augment_batch`` applies them: cv2.warpAffine / cv2.GaussianBlur / cv2.resize(NEAREST) arithmetic bit for bit, the
+``aae_augment`` applies them: cv2.warpAffine / cv2.GaussianBlur / cv2.resize(NEAREST) arithmetic bit for bit, the
 value ops as composed 256-entry tables (include/aae_b200.h).  At the tensor-core trainer's ~10 000 images/s the reference's
 10 Python threads of imgaug would be the bottleneck by more than an order of magnitude.
 
@@ -17,7 +17,7 @@ range for ``percent`` / ``px`` and ``pad_cval``, ``pad_mode="constant"`` and ``k
 back to (H, W) with cv2.resize's INTER_CUBIC / INTER_AREA arithmetic (``crop_pad_rule`` and the helpers below it).
 
 ``Occlusion`` adds the two occlusion switches of the cfg's ``[Augmentation]`` section (REALISTIC_OCCLUSION, SQUARE_OCCLUSION,
-dataset.py:421-454), which edit the masks before the paste; ``aae_augment_occlusion`` applies them.
+dataset.py:421-454), which edit the masks before the paste; ``aae_occlusion`` applies them.
 """
 import ctypes as C
 
@@ -392,7 +392,7 @@ class Augmenter(object):
 
     # -- host: pack the draws into the two device buffers ------------------------------------------------------------
     def pack(self, P):
-        """-> geom int32 [B, 4 + 2W + 2H], lut uint8 [B, C, 256] (include/aae_b200.h: aae_augment_batch); vectorised over the batch."""
+        """-> geom int32 [B, 4 + 2W + 2H], lut uint8 [B, C, 256] (include/aae_b200.h: aae_augment_args); vectorised over the batch."""
         B = len(P["affine_on"])
         H, W, C_ = self.h, self.w, self.c
         geom = np.zeros((B, 4 + 2 * W + 2 * H), np.int32)
@@ -445,7 +445,7 @@ class Augmenter(object):
         return np.ascontiguousarray(geom), np.ascontiguousarray(t, dtype=np.uint8)
 
     def pack_crop(self, P):
-        """-> the CropAndPad table int32 [B, 8] (include/aae_b200.h: aae_augment_batch_crop): mode (0 off, 1 cubic, 2 area),
+        """-> the CropAndPad table int32 [B, 8] (include/aae_b200.h: aae_augment): mode (0 off, 1 cubic, 2 area),
         source height and width after crop and pad, signed top and left pixels, pad value, offsets of the row and column
         resampling blocks in the Augmenter's table.  None for a chain without CropAndPad."""
         if self.crop is None:
@@ -465,7 +465,7 @@ class Augmenter(object):
     def _constants(self, dev):
         key = str(dev)
         if key not in self._dev:
-            self._dev[key] = {
+            k = self._dev[key] = {
                 "tab": torch.from_numpy(bilinear_table().view(np.int16)).to(dev),     # raw 16-bit patterns (torch has no uint16 arithmetic)
                 "rows": torch.from_numpy(nearest_cells(self.h, self.low[0])).to(dev),
                 "cols": torch.from_numpy(nearest_cells(self.w, self.low[1])).to(dev),
@@ -476,8 +476,20 @@ class Augmenter(object):
                 # CropAndPad's resampling blocks of every reachable source size, built once per Augmenter
                 "resample": torch.from_numpy(self.crop["table"]).to(dev) if self.crop is not None else None,
             }
+            # the fields of aae_augment_args that stay the same from batch to batch; the tensors above keep them alive
+            k["args"] = _lib.AugmentArgs(h=self.h, w=self.w, c=self.c, low_w=self.low[1], bilinear_tab=k["tab"], row_cell=k["rows"],
+                                         col_cell=k["cols"], blur_kernel_q8=k["taps"], u8_to_float=k["to_float"],
+                                         y_to_float=k["y_to_float"])
+            if self.crop is not None:
+                k["args"].set(resample=k["resample"], resample_len=int(k["resample"].numel()), max_src_rows=self.crop["max_rows"],
+                              max_src_w=self.crop["max_w"])
             torch.cuda.current_stream(dev).synchronize()    # usable from any stream (the batch producer's) from here on
         return self._dev[key]
+
+    def _launch(self, dev, stream, what, **batch):
+        """aae_augment on ``stream`` with the device's constant fields and this batch's (``batch``: field -> tensor or value)."""
+        a = self._constants(dev)["args"].copy().set(**batch)
+        _lib.check(_lib.lib().aae_augment(C.byref(a), C.c_void_p(stream.cuda_stream)), what)
 
     def augment_device(self, x, mask, bg, params=None, want_u8=False):
         """x, bg: uint8 CUDA tensors [B,H,W,C]; mask: bool/uint8 CUDA tensor [B,H,W] (True = background).  Returns the float32
@@ -489,57 +501,39 @@ class Augmenter(object):
         geom, lut = np.ascontiguousarray(geom, dtype=np.int32), np.ascontiguousarray(lut, dtype=np.uint8)
         if geom.shape != (B, 4 + 2 * self.w + 2 * self.h) or lut.shape != (B, self.c, 256):
             raise ValueError("augmentation tables have shapes %s / %s for a batch of %d" % (geom.shape, lut.shape, B))
-        k = self._constants(dev)
         geom_d, lut_d = torch.from_numpy(geom).to(dev, non_blocking=True), torch.from_numpy(lut).to(dev, non_blocking=True)
         assert geom_d.is_contiguous() and lut_d.is_contiguous()
-        mask8 = mask.to(torch.uint8).contiguous()
-        tmp = torch.empty_like(x)
+        x, bg, mask8 = x.contiguous(), bg.contiguous(), mask.to(torch.uint8).contiguous()
         out_f = torch.empty(x.shape, dtype=torch.float32, device=dev)
         out_u = torch.empty_like(x) if want_u8 else None
-        taps = k["taps"]
-        args = [_lib.ptr(x.contiguous()), _lib.ptr(mask8), _lib.ptr(bg.contiguous()), B, self.h, self.w, self.c, _lib.ptr(geom_d), _lib.ptr(lut_d),
-                _lib.ptr(k["tab"]), _lib.ptr(k["rows"]), _lib.ptr(k["cols"]), self.low[1], _lib.ptr(taps) if taps is not None else None,
-                _lib.ptr(k["to_float"]), _lib.ptr(tmp), _lib.ptr(out_u) if out_u is not None else None, _lib.ptr(out_f)]
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        if self.crop is None:
-            _lib.check(_lib.lib().aae_augment_batch(*args, stream), "augment batch")
-        else:
-            crop_d = torch.from_numpy(self.pack_crop(P)).to(dev, non_blocking=True)
-            _lib.check(_lib.lib().aae_augment_batch_crop(*args, *self._crop_args(k, crop_d, torch.empty_like(x)), stream), "augment batch (crop-pad)")
+        crop = {}
+        if self.crop is not None:
+            crop = dict(crop=torch.from_numpy(self.pack_crop(P)).to(dev, non_blocking=True), crop_tmp=torch.empty_like(x))
+        self._launch(dev, torch.cuda.current_stream(dev), "augment batch", batch=B, x=x, mask=mask8, bg=bg, geom=geom_d, lut=lut_d,
+                     tmp=torch.empty_like(x), out_u8=out_u, out_f32=out_f, **crop)
         return (out_f, out_u) if want_u8 else out_f
-
-    def _crop_args(self, k, crop_d, crop_tmp):
-        return [_lib.ptr(crop_d), _lib.ptr(k["resample"]), int(k["resample"].numel()), self.crop["max_rows"], self.crop["max_w"],
-                _lib.ptr(crop_tmp)]
 
     def augment_indexed(self, stacks, idx_d, idx_bg_d, geom_d, lut_d, out_f, y_out, stream, mask_batch=None, tmp=None, crop_d=None,
                         crop_tmp=None):
-        """``augment_device`` on device-resident stacks (``aae_augment_batch_indexed``): image b is row idx_d[b] of stacks["x"] /
-        ["mask"] / ["y"] and row idx_bg_d[b] of stacks["bg"]; mask_batch (uint8 [B,H,W], e.g. an occlusion output) replaces the
+        """``augment_device`` on device-resident stacks (``aae_augment`` with idx / idx_bg): image b is row idx_d[b] of stacks["x"]
+        / ["mask"] / ["y"] and row idx_bg_d[b] of stacks["bg"]; mask_batch (uint8 [B,H,W], e.g. an occlusion output) replaces the
         mask rows.  Writes the float32 input into out_f and the target y / 255. into y_out; geom_d / lut_d are ``pack``'s tables on
         the device; tmp (uint8 [B,H,W,C]) is the scratch of the geometry pass, allocated here when None.  With CropAndPad in the
         chain crop_d is ``pack_crop``'s table on the device and crop_tmp (uint8 [B,H,W,C], allocated here when None) the
-        crop-pad output (``aae_augment_batch_indexed_crop``).  Asynchronous on ``stream``."""
+        crop-pad output.  Asynchronous on ``stream``."""
         dev = out_f.device
         B = int(out_f.shape[0])
-        k = self._constants(dev)
+        shape = (B, self.h, self.w, self.c)
         if tmp is None:
-            tmp = torch.empty((B, self.h, self.w, self.c), dtype=torch.uint8, device=dev)
-        taps = k["taps"]
-        args = [_lib.ptr(stacks["x"]), _lib.ptr(stacks["mask"]), _lib.ptr(stacks["bg"]), _lib.ptr(stacks["y"]), len(stacks["x"]),
-                len(stacks["bg"]), _lib.ptr(idx_d), _lib.ptr(idx_bg_d), _lib.ptr(mask_batch), B, self.h, self.w, self.c, _lib.ptr(geom_d),
-                _lib.ptr(lut_d), _lib.ptr(k["tab"]), _lib.ptr(k["rows"]), _lib.ptr(k["cols"]), self.low[1],
-                _lib.ptr(taps) if taps is not None else None, _lib.ptr(k["to_float"]), _lib.ptr(k["y_to_float"]), _lib.ptr(tmp), None,
-                _lib.ptr(out_f), _lib.ptr(y_out)]
-        if self.crop is None:
-            _lib.check(_lib.lib().aae_augment_batch_indexed(*args, C.c_void_p(stream.cuda_stream)), "augment batch (indexed)")
-            return
-        if crop_d is None:
-            raise ValueError("a chain with CropAndPad needs pack_crop's table (crop_d)")
-        if crop_tmp is None:
-            crop_tmp = torch.empty((B, self.h, self.w, self.c), dtype=torch.uint8, device=dev)
-        _lib.check(_lib.lib().aae_augment_batch_indexed_crop(*args, *self._crop_args(k, crop_d, crop_tmp), C.c_void_p(stream.cuda_stream)),
-                   "augment batch (indexed, crop-pad)")
+            tmp = torch.empty(shape, dtype=torch.uint8, device=dev)
+        crop = {}
+        if self.crop is not None:
+            if crop_d is None:
+                raise ValueError("a chain with CropAndPad needs pack_crop's table (crop_d)")
+            crop = dict(crop=crop_d, crop_tmp=crop_tmp if crop_tmp is not None else torch.empty(shape, dtype=torch.uint8, device=dev))
+        self._launch(dev, stream, "augment batch (indexed)", batch=B, x=stacks["x"], mask=stacks["mask"], bg=stacks["bg"],
+                     y=stacks["y"], idx=idx_d, idx_bg=idx_bg_d, n_images=len(stacks["x"]), n_bg=len(stacks["bg"]),
+                     mask_batch=mask_batch, geom=geom_d, lut=lut_d, tmp=tmp, out_f32=out_f, y_out=y_out, **crop)
 
 
 # ----------------------------------------------------------------------------------------------------------- occlusion
@@ -572,7 +566,7 @@ def square_grid(h, w):
 
 def load_occlusion_bank(path, shape):
     """The occluder bank of ``Dataset.random_syn_masks`` (dataset.py:405-418) bit-packed: uint32 [n, rows, cols / 32] with bit
-    j of word w = column 32 w + j, as ``aae_augment_occlusion`` reads it.  The reference unpacks the file with bitarray (default
+    j of word w = column 32 w + j, as ``aae_occlusion`` reads it.  The reference unpacks the file with bitarray (default
     big-endian bit order, the order of np.unpackbits), reshapes to 224 x 224 masks and resizes each one with
     cv2.resize(mask, (shape[0], shape[1]), INTER_NEAREST) -- dsize is (width, height), so the result has shape[1] rows."""
     bits = np.unpackbits(np.fromfile(path, dtype=np.uint8))
@@ -623,7 +617,7 @@ class Occlusion(object):
         return P
 
     def pack(self, P):
-        """-> int32 [B, 1 + 3K]: occluder, tx[K], ty[K], keep bits[K] (include/aae_b200.h: aae_augment_occlusion)."""
+        """-> int32 [B, 1 + 3K]: occluder, tx[K], ty[K], keep bits[K] (include/aae_b200.h: aae_occlusion)."""
         K = self.K
         cells = self.low[0] * self.low[1]
         B = len(P["occluder"]) if "occluder" in P else len(P["square_on"])
@@ -645,12 +639,17 @@ class Occlusion(object):
     def _state(self, dev):
         key = str(dev)
         if key not in self._dev:
-            self._dev[key] = {
+            st = self._dev[key] = {
                 "rows": torch.from_numpy(nearest_cells(self.h, self.low[0])).to(dev),
                 "cols": torch.from_numpy(nearest_cells(self.w, self.low[1])).to(dev),
                 "fallbacks": torch.zeros(2, dtype=torch.int32, device=dev),
                 "bank_src": None, "bank": None,
             }
+            # the fields of aae_occlusion_args that stay the same from batch to batch
+            st["args"] = _lib.OcclusionArgs(h=self.h, w=self.w, realistic=int(self.realistic != 0), max_occl=self.realistic,
+                                            square=int(self.square != 0), min_kept=1.0 - self.square,      # dataset.py:451: 1-max_occl
+                                            n_cand=self.K, row_cell=st["rows"], col_cell=st["cols"], low_h=self.low[0],
+                                            low_w=self.low[1], fallbacks=st["fallbacks"])
             torch.cuda.current_stream(dev).synchronize()    # usable from any stream (the batch producer's) from here on
         return self._dev[key]
 
@@ -660,6 +659,12 @@ class Occlusion(object):
         if st["bank_src"] is not bank:                  # one upload per device and bank
             st["bank"], st["bank_src"] = torch.from_numpy(np.ascontiguousarray(bank, np.uint32).view(np.int32)).to(dev), bank
         return st["bank"]
+
+    def _launch(self, st, stream, what, **batch):
+        """aae_occlusion on ``stream`` with the device's constant fields, its bank, and this batch's (field -> tensor or value)."""
+        bank_d = st["bank"] if self.realistic else None
+        a = st["args"].copy().set(bank=bank_d, n_bank=len(bank_d) if bank_d is not None else 0, **batch)
+        _lib.check(_lib.lib().aae_occlusion(C.byref(a), C.c_void_p(stream.cuda_stream)), what)
 
     def apply_device(self, mask, bank=None, params=None):
         """mask: bool / uint8 CUDA tensor [B,H,W] (True = background); bank: ``load_occlusion_bank`` array (realistic step).
@@ -675,27 +680,18 @@ class Occlusion(object):
         cand = torch.from_numpy(self.pack(P)).to(dev, non_blocking=True)
         mask8 = mask.to(torch.uint8).contiguous()
         out = torch.empty_like(mask8)
-        bank_d = st["bank"] if self.realistic else None
-        _lib.check(_lib.lib().aae_augment_occlusion(
-            _lib.ptr(mask8), B, self.h, self.w, _lib.ptr(bank_d), len(bank_d) if bank_d is not None else 0, _lib.ptr(cand), self.K,
-            int(self.realistic != 0), self.realistic, int(self.square != 0), 1.0 - self.square,      # dataset.py:451: 1-max_occl
-            _lib.ptr(st["rows"]), _lib.ptr(st["cols"]), self.low[0], self.low[1], _lib.ptr(out), _lib.ptr(st["fallbacks"]),
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "augment occlusion")
+        self._launch(st, torch.cuda.current_stream(dev), "augment occlusion", batch=B, mask=mask8, cand=cand, mask_out=out)
         return out
 
     def apply_indexed(self, mask_stack, idx_d, cand_d, bank, out, stream):
-        """``apply_device`` on the masks mask_stack[idx_d[b]] of a device-resident stack (``aae_augment_occlusion_indexed``):
-        cand_d is ``pack``'s candidate table on the device, out the uint8 [B,H,W] result.  Asynchronous on ``stream``; counts
-        into the same fallback counters."""
-        dev = out.device
-        B = int(out.shape[0])
-        st = self._state(dev)
-        bank_d = self._bank(st, dev, bank) if self.realistic else None
-        _lib.check(_lib.lib().aae_augment_occlusion_indexed(
-            _lib.ptr(mask_stack), len(mask_stack), _lib.ptr(idx_d), B, self.h, self.w, _lib.ptr(bank_d),
-            len(bank_d) if bank_d is not None else 0, _lib.ptr(cand_d), self.K, int(self.realistic != 0), self.realistic,
-            int(self.square != 0), 1.0 - self.square, _lib.ptr(st["rows"]), _lib.ptr(st["cols"]), self.low[0], self.low[1],
-            _lib.ptr(out), _lib.ptr(st["fallbacks"]), C.c_void_p(stream.cuda_stream)), "augment occlusion (indexed)")
+        """``apply_device`` on the masks mask_stack[idx_d[b]] of a device-resident stack (``aae_occlusion`` with idx): cand_d is
+        ``pack``'s candidate table on the device, out the uint8 [B,H,W] result.  Asynchronous on ``stream``; counts into the same
+        fallback counters."""
+        st = self._state(out.device)
+        if self.realistic:
+            self._bank(st, out.device, bank)
+        self._launch(st, stream, "augment occlusion (indexed)", batch=int(out.shape[0]), mask=mask_stack, idx=idx_d,
+                     n_images=len(mask_stack), cand=cand_d, mask_out=out)
 
     def fallbacks(self):
         """Images that exhausted their K candidates since the last call, per step: {"realistic": n, "square": n}.  Clears the

@@ -10,14 +10,14 @@
 //   Add, Invert, Multiply x2, ContrastNormalization   per-image, per-channel uint8 -> uint8 tables, composed on the host into one
 //   x / 255.             table of 256 floats
 //
-// The indexed form (aae_augment_batch_indexed) reads image b from rows idx[b] / idx_bg[b] of device-resident stacks and also
-// writes the target y[idx[b]] / 255., so a batch is never gathered.
+// With idx / idx_bg set (aae_augment_args) image b is read from rows idx[b] / idx_bg[b] of device-resident stacks, and the
+// target y[idx[b]] / 255. can be written too, so a batch is never gathered.
 //
 // All random draws (which ops fire, scales, masks, offsets, factors) are made on the host and arrive as per-image parameters,
 // so the kernels are deterministic and are checked bit for bit against a CPU restatement pinned to OpenCV (tests/).
 // Two passes: geometry (paste + warp + dropout) into a uint8 scratch image, then blur + tables.  HBM-bound: ~5 B/value.
 //
-// CropAndPad, when the chain has it (aae_augment_batch_crop / aae_augment_batch_indexed_crop), is a third pass in front: the
+// CropAndPad, when the chain has it (aae_augment_args.crop set), is a third pass in front: the
 // pasted image cropped and padded by per-image pixel counts, then resized back to H x W with cv2.resize's uint8 arithmetic --
 // INTER_CUBIC (11-bit fixed-point taps on clamped indices, integer horizontal sums, then the vertical sum in float32 as
 // OpenCV's vector path computes it: S0 b0 + (S1 b1 + (S2 b2 + S3 b3)), rounded to nearest even) or INTER_AREA (float32
@@ -28,6 +28,18 @@ namespace aae {
 namespace {
 
 constexpr int AUG_FLAG_AFFINE = 1, AUG_FLAG_DROP = 2, AUG_FLAG_BLUR = 4, AUG_FLAG_CROP = 8;
+
+// Where the kernels read image b: row idx[b] of the x / mask / y stacks and row idx_bg[b] of the background stack, an image whose
+// idx[b] or idx_bg[b] is outside its stack pasted from zeros with target y_to_float[0]; with idx == nullptr, row b of every input.
+struct AugIndex {
+  const int32_t* idx = nullptr;
+  const int32_t* idx_bg = nullptr;
+  long long n_images = 0, n_bg = 0;
+  bool mask_gathered = false;       // the mask is already [B][H][W] (an occlusion output), not a stack read through idx
+  const uint8_t* y = nullptr;       // target stack; y_out[b] = y_to_float[y[idx[b]]]
+  const float* y_to_float = nullptr;
+  float* y_out = nullptr;
+};
 
 struct AugGeomView {
   const int32_t* base;   // [4 + 2W + 2H] ints of this image: flags, keep_lo, keep_hi, 0, adelta[W], bdelta[W], X0[H], Y0[H]
@@ -263,22 +275,31 @@ inline unsigned aug_grid(long long n) {
 
 size_t crop_pad_smem_bytes(int max_rows, int max_w, int C) { return (size_t)max_rows * max_w * C; }
 
-int launch_augment(const uint8_t* x, const uint8_t* mask, const uint8_t* bg, int B, int H, int W, int C, const int32_t* geom, const uint8_t* lut,
-                   const unsigned short* tab, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, const int32_t* blur_q8, const float* to_float,
-                   uint8_t* tmp, uint8_t* out_u8, float* out_f32, cudaStream_t s, const AugIndex& ix, const AugCrop* crop) {
-  AAE_REQUIRE(C >= 1 && C <= 4, "augment: %d channels unsupported (1..4)", C);
-  if (crop != nullptr) {
+int launch_augment(const aae_augment_args& a, cudaStream_t s) {
+  const int B = a.batch, H = a.h, W = a.w, C = a.c;
+  AugIndex ix;
+  ix.idx = a.idx;
+  ix.idx_bg = a.idx_bg;
+  ix.n_images = a.n_images;
+  ix.n_bg = a.n_bg;
+  ix.mask_gathered = a.mask_batch != nullptr;
+  ix.y = a.y;
+  ix.y_to_float = a.y_to_float;
+  ix.y_out = a.y_out;
+  const uint8_t* mask = a.mask_batch ? a.mask_batch : a.mask;
+  if (a.crop != nullptr) {
     const dim3 grid((unsigned)B, (unsigned)ceil_div(H, CROP_ROWS));
-    aug_crop_pad_kernel<<<grid, 256, crop_pad_smem_bytes(crop->max_rows, crop->max_w, C), s>>>(
-        x, mask, bg, H, W, C, crop->table, crop->resample, crop->resample_len, crop->max_rows, crop->max_w, crop->out, ix);
+    aug_crop_pad_kernel<<<grid, 256, crop_pad_smem_bytes(a.max_src_rows, a.max_src_w, C), s>>>(
+        a.x, mask, a.bg, H, W, C, a.crop, a.resample, a.resample_len, a.max_src_rows, a.max_src_w, a.crop_tmp, ix);
     AAE_LAUNCH_OK();
   }
-  aug_geometry_kernel<<<aug_grid((long long)B * H * W), 256, 0, s>>>(x, mask, bg, B, H, W, C, geom, tab, row_cell, col_cell, low_w,
-                                                                     crop ? crop->out : nullptr, tmp, ix);
+  aug_geometry_kernel<<<aug_grid((long long)B * H * W), 256, 0, s>>>(a.x, mask, a.bg, B, H, W, C, a.geom, a.bilinear_tab, a.row_cell,
+                                                                     a.col_cell, a.low_w, a.crop ? a.crop_tmp : nullptr, a.tmp, ix);
   AAE_LAUNCH_OK();
   BlurTaps taps;
-  for (int i = 0; i < 5; ++i) taps.k[i] = blur_q8 ? blur_q8[i] : (i == 2 ? 256 : 0);
-  aug_blur_lut_kernel<<<aug_grid((long long)B * H * W * C), 256, 0, s>>>(tmp, B, H, W, C, geom, taps, lut, to_float, out_u8, out_f32, ix);
+  for (int i = 0; i < 5; ++i) taps.k[i] = a.blur_kernel_q8 ? a.blur_kernel_q8[i] : (i == 2 ? 256 : 0);
+  aug_blur_lut_kernel<<<aug_grid((long long)B * H * W * C), 256, 0, s>>>(a.tmp, B, H, W, C, a.geom, taps, a.lut, a.u8_to_float, a.out_u8,
+                                                                         a.out_f32, ix);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }

@@ -309,7 +309,7 @@ struct aae_trainer {
 };
 
 // ============================================================================ misc
-extern "C" int aae_version(void) { return 100; }
+extern "C" int aae_version(void) { return 101; }
 extern "C" int64_t aae_launch_count(void) { return (int64_t)g_launches.load(); }
 extern "C" const char* aae_last_error_string(void) { return g_err; }
 
@@ -724,167 +724,62 @@ extern "C" int aae_topk_merge_packed(const void* packed_dev, int n_shards, int b
 }
 
 // ============================================================================ training input pipeline
-static int augment_gathered(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
-                            const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev, const uint8_t* row_cell_dev,
-                            const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8, const float* u8_to_float_dev,
-                            uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, cudaStream_t s, const AugCrop* crop) {
-  AAE_REQUIRE(x_dev && mask_dev && bg_dev && geom_dev && lut_dev && bilinear_tab_dev && row_cell_dev && col_cell_dev && tmp_dev, "null argument");
-  AAE_REQUIRE(out_u8_dev || out_f32_dev, "no output requested");
-  AAE_REQUIRE(!out_f32_dev || u8_to_float_dev, "out_f32_dev needs u8_to_float_dev");
-  AAE_REQUIRE(batch >= 1 && h >= 1 && w >= 1 && low_w >= 1, "bad geometry");
-  if (blur_kernel_q8) {
+extern "C" int aae_augment(const aae_augment_args* a, void* stream) {
+  AAE_REQUIRE(a, "null argument");
+  AAE_REQUIRE(a->struct_size == (int32_t)sizeof(aae_augment_args), "aae_augment_args: struct_size %d, expected %d", a->struct_size,
+              (int)sizeof(aae_augment_args));
+  AAE_REQUIRE((a->idx == nullptr) == (a->idx_bg == nullptr), "idx and idx_bg must both be set or both be NULL");
+  AAE_REQUIRE(!a->idx || (a->n_images >= 1 && a->n_bg >= 1), "empty image stack (%lld images, %lld backgrounds)",
+              (long long)a->n_images, (long long)a->n_bg);
+  AAE_REQUIRE(a->x && a->bg && (a->mask || a->mask_batch), "null argument");
+  AAE_REQUIRE(a->geom && a->lut && a->bilinear_tab && a->row_cell && a->col_cell && a->tmp, "null argument");
+  AAE_REQUIRE(!a->y_out || (a->y && a->y_to_float), "y_out needs y and y_to_float");
+  AAE_REQUIRE(a->out_u8 || a->out_f32, "no output requested");
+  AAE_REQUIRE(!a->out_f32 || a->u8_to_float, "out_f32 needs u8_to_float");
+  AAE_REQUIRE(a->batch >= 1 && a->h >= 1 && a->w >= 1 && a->low_w >= 1, "bad geometry");
+  AAE_REQUIRE(a->c >= 1 && a->c <= 4, "augment: %d channels unsupported (1..4)", a->c);
+  if (a->blur_kernel_q8) {
     int sum = 0;
-    for (int i = 0; i < 5; ++i) sum += blur_kernel_q8[i];
+    for (int i = 0; i < 5; ++i) sum += a->blur_kernel_q8[i];
     AAE_REQUIRE(sum == 256, "blur kernel must sum to 256 (8 fractional bits), got %d", sum);
   }
-  return launch_augment(x_dev, mask_dev, bg_dev, batch, h, w, c, geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w,
-                        blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, s, AugIndex(), crop);
+  if (a->crop) {
+    AAE_REQUIRE(a->resample && a->crop_tmp, "null argument");
+    AAE_REQUIRE(a->resample_len >= 1 && a->max_src_rows >= 1 && a->max_src_w >= 1,
+                "bad crop-pad bounds (%lld table ints, %d rows, %d columns)", (long long)a->resample_len, a->max_src_rows, a->max_src_w);
+    const size_t smem = crop_pad_smem_bytes(a->max_src_rows, a->max_src_w, a->c);
+    if (smem > 48 * 1024) {
+      set_error("crop-pad: %d source rows of %d x %d bytes need %zu bytes of shared memory (48 KB supported)", a->max_src_rows,
+                a->max_src_w, a->c, smem);
+      return AAE_ERR_UNSUPPORTED;
+    }
+  }
+  return launch_augment(*a, (cudaStream_t)stream);
 }
 
-extern "C" int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
-                                 const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev, const uint8_t* row_cell_dev,
-                                 const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8, const float* u8_to_float_dev,
-                                 uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, void* stream) {
-  return augment_gathered(x_dev, mask_dev, bg_dev, batch, h, w, c, geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w,
-                          blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, (cudaStream_t)stream, nullptr);
-}
-
-// the CropAndPad arguments of the *_crop entry points: pointers present, and the staged rows within the 48 KB of shared memory
-static int crop_pad_checked(AugCrop& cp, const int32_t* crop_dev, const int32_t* resample_dev, int64_t resample_len, int max_src_rows,
-                            int max_src_w, uint8_t* crop_tmp_dev, int c) {
-  AAE_REQUIRE(crop_dev && resample_dev && crop_tmp_dev, "null argument");
-  AAE_REQUIRE(resample_len >= 1 && max_src_rows >= 1 && max_src_w >= 1, "bad crop-pad bounds (%lld table ints, %d rows, %d columns)",
-              (long long)resample_len, max_src_rows, max_src_w);
-  AAE_REQUIRE(c >= 1 && c <= 4, "augment: %d channels unsupported (1..4)", c);
-  const size_t smem = crop_pad_smem_bytes(max_src_rows, max_src_w, c);
+extern "C" int aae_occlusion(const aae_occlusion_args* a, void* stream) {
+  AAE_REQUIRE(a, "null argument");
+  AAE_REQUIRE(a->struct_size == (int32_t)sizeof(aae_occlusion_args), "aae_occlusion_args: struct_size %d, expected %d", a->struct_size,
+              (int)sizeof(aae_occlusion_args));
+  AAE_REQUIRE(a->mask && a->cand && a->mask_out && a->fallbacks, "null argument");
+  AAE_REQUIRE(!a->idx || a->n_images >= 1, "empty mask stack");
+  AAE_REQUIRE(a->batch >= 1 && a->h >= 1 && a->w >= 1 && a->n_cand >= 1, "bad geometry / candidate count");
+  AAE_REQUIRE(!a->realistic || (a->bank && a->n_bank >= 1), "realistic occlusion needs an occluder bank");
+  AAE_REQUIRE(!a->square || (a->row_cell && a->col_cell && a->low_h >= 1 && a->low_w >= 1), "square occlusion needs the dropout cell maps");
+  if (a->w % 32 != 0) {
+    set_error("occlusion: mask width %d is not a multiple of 32 (rows are packed into 32-bit words)", a->w);
+    return AAE_ERR_UNSUPPORTED;
+  }
+  if (a->square && a->low_h * a->low_w > 32) {
+    set_error("occlusion: %d x %d dropout cells do not fit the 32 keep bits of a candidate", a->low_h, a->low_w);
+    return AAE_ERR_UNSUPPORTED;
+  }
+  const size_t smem = occlusion_smem_bytes(a->h, a->w, a->square ? a->low_w : 0);
   if (smem > 48 * 1024) {
-    set_error("crop-pad: %d source rows of %d x %d bytes need %zu bytes of shared memory (48 KB supported)", max_src_rows, max_src_w, c, smem);
+    set_error("occlusion: a %d x %d mask needs %zu bytes of shared memory (48 KB supported)", a->h, a->w, smem);
     return AAE_ERR_UNSUPPORTED;
   }
-  cp.table = crop_dev;
-  cp.resample = resample_dev;
-  cp.resample_len = resample_len;
-  cp.max_rows = max_src_rows;
-  cp.max_w = max_src_w;
-  cp.out = crop_tmp_dev;
-  return AAE_OK;
-}
-
-extern "C" int aae_augment_batch_crop(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
-                                      const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev, const uint8_t* row_cell_dev,
-                                      const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8, const float* u8_to_float_dev,
-                                      uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, const int32_t* crop_dev,
-                                      const int32_t* resample_dev, int64_t resample_len, int max_src_rows, int max_src_w, uint8_t* crop_tmp_dev,
-                                      void* stream) {
-  AugCrop cp;
-  AAE_TRY(crop_pad_checked(cp, crop_dev, resample_dev, resample_len, max_src_rows, max_src_w, crop_tmp_dev, c));
-  return augment_gathered(x_dev, mask_dev, bg_dev, batch, h, w, c, geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w,
-                          blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, (cudaStream_t)stream, &cp);
-}
-
-static int occlusion_checked(const uint8_t* mask_dev, int batch, int h, int w, const uint32_t* bank_dev, int n_bank, const int32_t* cand_dev,
-                             int n_cand, int realistic, double max_occl, int square, double min_kept, const uint8_t* row_cell_dev,
-                             const uint8_t* col_cell_dev, int low_h, int low_w, uint8_t* mask_out_dev, int32_t* fallbacks_dev, cudaStream_t s,
-                             const int32_t* idx_dev, long long n_images) {
-  AAE_REQUIRE(mask_dev && cand_dev && mask_out_dev && fallbacks_dev, "null argument");
-  AAE_REQUIRE(batch >= 1 && h >= 1 && w >= 1 && n_cand >= 1, "bad geometry / candidate count");
-  AAE_REQUIRE(!realistic || (bank_dev && n_bank >= 1), "realistic occlusion needs an occluder bank");
-  AAE_REQUIRE(!square || (row_cell_dev && col_cell_dev && low_h >= 1 && low_w >= 1), "square occlusion needs the dropout cell maps");
-  if (w % 32 != 0) {
-    set_error("occlusion: mask width %d is not a multiple of 32 (rows are packed into 32-bit words)", w);
-    return AAE_ERR_UNSUPPORTED;
-  }
-  if (square && low_h * low_w > 32) {
-    set_error("occlusion: %d x %d dropout cells do not fit the 32 keep bits of a candidate", low_h, low_w);
-    return AAE_ERR_UNSUPPORTED;
-  }
-  const size_t smem = occlusion_smem_bytes(h, w, square ? low_w : 0);
-  if (smem > 48 * 1024) {
-    set_error("occlusion: a %d x %d mask needs %zu bytes of shared memory (48 KB supported)", h, w, smem);
-    return AAE_ERR_UNSUPPORTED;
-  }
-  return launch_occlusion(mask_dev, batch, h, w, bank_dev, n_bank, cand_dev, n_cand, realistic, max_occl, square, min_kept,
-                          row_cell_dev, col_cell_dev, low_w, mask_out_dev, fallbacks_dev, s, idx_dev, n_images);
-}
-
-extern "C" int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, int w, const uint32_t* bank_dev, int n_bank,
-                                     const int32_t* cand_dev, int n_cand, int realistic, double max_occl, int square, double min_kept,
-                                     const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_h, int low_w,
-                                     uint8_t* mask_out_dev, int32_t* fallbacks_dev, void* stream) {
-  return occlusion_checked(mask_dev, batch, h, w, bank_dev, n_bank, cand_dev, n_cand, realistic, max_occl, square, min_kept,
-                           row_cell_dev, col_cell_dev, low_h, low_w, mask_out_dev, fallbacks_dev, (cudaStream_t)stream, nullptr, 0);
-}
-
-static int augment_indexed(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
-                                         const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
-                                         const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
-                                         const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
-                                         const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
-                                         const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
-                                         float* out_f32_dev, float* y_out_dev, cudaStream_t s, const AugCrop* crop) {
-  AAE_REQUIRE(x_stack_dev && bg_stack_dev && idx_dev && idx_bg_dev && (mask_stack_dev || mask_batch_dev), "null argument");
-  AAE_REQUIRE(!y_out_dev || (y_stack_dev && y_to_float_dev), "y_out_dev needs y_stack_dev and y_to_float_dev");
-  AAE_REQUIRE(n_images >= 1 && n_bg >= 1, "empty image stack (%lld images, %lld backgrounds)", (long long)n_images, (long long)n_bg);
-  AAE_REQUIRE(geom_dev && lut_dev && bilinear_tab_dev && row_cell_dev && col_cell_dev && tmp_dev, "null argument");
-  AAE_REQUIRE(out_u8_dev || out_f32_dev, "no output requested");
-  AAE_REQUIRE(!out_f32_dev || u8_to_float_dev, "out_f32_dev needs u8_to_float_dev");
-  AAE_REQUIRE(batch >= 1 && h >= 1 && w >= 1 && low_w >= 1, "bad geometry");
-  if (blur_kernel_q8) {
-    int sum = 0;
-    for (int i = 0; i < 5; ++i) sum += blur_kernel_q8[i];
-    AAE_REQUIRE(sum == 256, "blur kernel must sum to 256 (8 fractional bits), got %d", sum);
-  }
-  AugIndex ix;
-  ix.idx = idx_dev;
-  ix.idx_bg = idx_bg_dev;
-  ix.n_images = n_images;
-  ix.n_bg = n_bg;
-  ix.mask_gathered = mask_batch_dev != nullptr;
-  ix.y = y_stack_dev;
-  ix.y_to_float = y_to_float_dev;
-  ix.y_out = y_out_dev;
-  return launch_augment(x_stack_dev, mask_batch_dev ? mask_batch_dev : mask_stack_dev, bg_stack_dev, batch, h, w, c, geom_dev, lut_dev,
-                        bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w, blur_kernel_q8, u8_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev,
-                        s, ix, crop);
-}
-
-extern "C" int aae_augment_batch_indexed(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
-                                         const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
-                                         const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
-                                         const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
-                                         const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
-                                         const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
-                                         float* out_f32_dev, float* y_out_dev, void* stream) {
-  return augment_indexed(x_stack_dev, mask_stack_dev, bg_stack_dev, y_stack_dev, n_images, n_bg, idx_dev, idx_bg_dev, mask_batch_dev, batch, h, w, c,
-                         geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w, blur_kernel_q8, u8_to_float_dev,
-                         y_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, y_out_dev, (cudaStream_t)stream, nullptr);
-}
-
-extern "C" int aae_augment_batch_indexed_crop(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
-                                         const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
-                                         const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
-                                         const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
-                                         const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
-                                         const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
-                                         float* out_f32_dev, float* y_out_dev, const int32_t* crop_dev,
-                                              const int32_t* resample_dev, int64_t resample_len, int max_src_rows, int max_src_w,
-                                              uint8_t* crop_tmp_dev, void* stream) {
-  AugCrop cp;
-  AAE_TRY(crop_pad_checked(cp, crop_dev, resample_dev, resample_len, max_src_rows, max_src_w, crop_tmp_dev, c));
-  return augment_indexed(x_stack_dev, mask_stack_dev, bg_stack_dev, y_stack_dev, n_images, n_bg, idx_dev, idx_bg_dev, mask_batch_dev, batch, h, w, c,
-                         geom_dev, lut_dev, bilinear_tab_dev, row_cell_dev, col_cell_dev, low_w, blur_kernel_q8, u8_to_float_dev,
-                         y_to_float_dev, tmp_dev, out_u8_dev, out_f32_dev, y_out_dev, (cudaStream_t)stream, &cp);
-}
-
-extern "C" int aae_augment_occlusion_indexed(const uint8_t* mask_stack_dev, int64_t n_images, const int32_t* idx_dev, int batch, int h, int w,
-                                             const uint32_t* bank_dev, int n_bank, const int32_t* cand_dev, int n_cand, int realistic,
-                                             double max_occl, int square, double min_kept, const uint8_t* row_cell_dev,
-                                             const uint8_t* col_cell_dev, int low_h, int low_w, uint8_t* mask_out_dev, int32_t* fallbacks_dev,
-                                             void* stream) {
-  AAE_REQUIRE(mask_stack_dev && idx_dev, "null argument");
-  AAE_REQUIRE(n_images >= 1, "empty mask stack");
-  return occlusion_checked(mask_stack_dev, batch, h, w, bank_dev, n_bank, cand_dev, n_cand, realistic, max_occl, square, min_kept,
-                           row_cell_dev, col_cell_dev, low_h, low_w, mask_out_dev, fallbacks_dev, (cudaStream_t)stream, idx_dev, n_images);
+  return launch_occlusion(*a, (cudaStream_t)stream);
 }
 
 // ============================================================================ decoder

@@ -188,38 +188,11 @@ int launch_conv_small_n(const IGemmParams& p, cudaStream_t stream);
 // p.K = number of pixels, p.Bm = dY [pixels, N<=3]; partial: [chunks, taps*SC*N]
 int launch_wgrad_small_n(const IGemmParams& p, int chunks, float* partial, cudaStream_t stream);
 
-// ---- training input pipeline (augment.cu) --------------------------------------------------
-// Resident-stack form of the input kernels (aae_augment_batch_indexed / aae_augment_occlusion_indexed): image b of the batch is
-// row idx[b] of the x / mask / y stacks and row idx_bg[b] of the background stack.  An image whose idx[b] or idx_bg[b] is outside its
-// stack is pasted from zeros and its target is y_to_float[0].  The default (idx == nullptr) is the gathered form: row b of every
-// input.
-struct AugIndex {
-  const int32_t* idx = nullptr;
-  const int32_t* idx_bg = nullptr;
-  long long n_images = 0, n_bg = 0;
-  bool mask_gathered = false;       // the mask is already [B][H][W] (an occlusion output), not a stack read through idx
-  const uint8_t* y = nullptr;       // target stack; y_out[b] = y_to_float[y[idx[b]]]
-  const float* y_to_float = nullptr;
-  float* y_out = nullptr;
-};
-// CropAndPad pass in front of the geometry pass (aae_augment_batch_crop): per-image table [B][8], resampling blocks, the bound on
-// staged source rows / row width the launch's shared memory is sized for, and its uint8 [B][H][W][C] output
-struct AugCrop {
-  const int32_t* table = nullptr;
-  const int32_t* resample = nullptr;
-  long long resample_len = 0;
-  int max_rows = 0, max_w = 0;
-  uint8_t* out = nullptr;
-};
+// ---- training input pipeline (augment.cu, occlusion.cu): launchers of arguments aae_augment / aae_occlusion have checked ----
 size_t crop_pad_smem_bytes(int max_rows, int max_w, int C);
-int launch_augment(const uint8_t* x, const uint8_t* mask, const uint8_t* bg, int B, int H, int W, int C, const int32_t* geom, const uint8_t* lut,
-                   const unsigned short* tab, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, const int32_t* blur_q8, const float* to_float,
-                   uint8_t* tmp, uint8_t* out_u8, float* out_f32, cudaStream_t s, const AugIndex& ix = AugIndex(), const AugCrop* crop = nullptr);
-// occlusion-mask augmentations (occlusion.cu); idx (optional, n_images rows): image b's mask is row idx[b] of the mask stack
+int launch_augment(const aae_augment_args& a, cudaStream_t s);
 size_t occlusion_smem_bytes(int H, int W, int low_w);
-int launch_occlusion(const uint8_t* mask, int B, int H, int W, const uint32_t* bank, int n_bank, const int32_t* cand, int K, int realistic,
-                     double max_occl, int square, double min_kept, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, uint8_t* out,
-                     int32_t* fallbacks, cudaStream_t s, const int32_t* idx = nullptr, long long n_images = 0);
+int launch_occlusion(const aae_occlusion_args& a, cudaStream_t s);
 
 // ---- latent terms of the loss (latent.cu): sigma head activation, sampled z, KL and norm terms, their backward ----------
 // Every tensor is [B, J] row-major (dcat [B, 2J]); a null pointer leaves that part out.  Forward: sigma / sz from pre and z,

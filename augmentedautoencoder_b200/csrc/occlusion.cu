@@ -177,11 +177,10 @@ __global__ void __launch_bounds__(OCCL_THREADS) occlusion_kernel(const uint8_t* 
 
 size_t occlusion_smem_bytes(int H, int W, int low_w) { return (size_t)(2 * H + low_w) * (W / 32) * sizeof(uint32_t); }
 
-int launch_occlusion(const uint8_t* mask, int B, int H, int W, const uint32_t* bank, int n_bank, const int32_t* cand, int K, int realistic,
-                     double max_occl, int square, double min_kept, const uint8_t* row_cell, const uint8_t* col_cell, int low_w, uint8_t* out,
-                     int32_t* fallbacks, cudaStream_t s, const int32_t* idx, long long n_images) {
-  occlusion_kernel<<<B, OCCL_THREADS, occlusion_smem_bytes(H, W, square ? low_w : 0), s>>>(
-      mask, H, W, bank, n_bank, cand, K, realistic, max_occl, square, min_kept, row_cell, col_cell, low_w, out, fallbacks, idx, n_images);
+int launch_occlusion(const aae_occlusion_args& a, cudaStream_t s) {
+  occlusion_kernel<<<a.batch, OCCL_THREADS, occlusion_smem_bytes(a.h, a.w, a.square ? a.low_w : 0), s>>>(
+      a.mask, a.h, a.w, a.bank, a.n_bank, a.cand, a.n_cand, a.realistic, a.max_occl, a.square, a.min_kept, a.row_cell, a.col_cell,
+      a.low_w, a.mask_out, a.fallbacks, a.idx, a.n_images);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }

@@ -250,94 +250,116 @@ AAE_API int aae_bootstrap_l2_loss(const float* x_dev, const float* target_dev, i
 
 /* ---------------------------------------------------------------- Training input pipeline ---
  * Dataset.batch on the device (auto_pose/ae/dataset.py:456-495): x[mask] = bg[mask], then the imgaug chain of the training
- * cfg (auto_pose/ae/cfg/train_template.cfg:26-37) with every random draw made by the caller:
- *   geom_dev   [B][4 + 2W + 2H] int32 per image: flags (1 affine, 2 coarse dropout, 4 blur), dropout keep bits (low, high
- *              32 bits over the low_h x low_w cells, row-major), 0, then cv2.warpAffine's fixed-point tables adelta[W],
- *              bdelta[W], X0[H], Y0[H] (10 fractional bits, rounding offset included)
- *   lut_dev    [B][C][256] uint8: the composed Add / Invert / Multiply / Multiply / ContrastNormalization table
- *   bilinear_tab_dev [1024][4] uint16: OpenCV's INTER_LINEAR weight table (rows sum to 32768);  row_cell_dev [H] / col_cell_dev [W]: cv2.resize
- *              INTER_NEAREST index maps of the dropout mask;  blur_kernel_q8: 5 host ints summing to 256 (NULL: no blur);
- *   u8_to_float_dev [256]: value / 255.  tmp_dev: [B,H,W,C] uint8 scratch.  out_u8_dev / out_f32_dev: either may be NULL. */
-AAE_API int aae_augment_batch(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
-                              const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
-                              const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
-                              const float* u8_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev, void* stream);
+ * cfg (auto_pose/ae/cfg/train_template.cfg:26-37) with every random draw made by the caller, and before it the occlusion
+ * switches on the masks.  Both calls take their arguments in a struct whose first field is struct_size = sizeof of the
+ * struct; another value is refused with AAE_ERR_INVALID_ARG, so a binding whose layout differs from this header fails
+ * instead of passing misplaced fields.  Every pointer is a device pointer except blur_kernel_q8.  Every argument is checked
+ * on the host before anything is launched; every launch goes to `stream`, with no allocation and no synchronisation.
+ *
+ * Where image b comes from: idx and idx_bg are both NULL or both set (anything else: AAE_ERR_INVALID_ARG).
+ *   both NULL  image b is row b of x, mask, bg and y (a gathered batch); n_images and n_bg are unused.
+ *   both set   image b is row idx[b] of the x, mask and y stacks and row idx_bg[b] of the bg stack, for a training set
+ *              resident on the device (Dataset.load_training_images(device=...)); n_images, n_bg >= 1 are the stack rows.
+ *              An image whose idx[b] OR idx_bg[b] is outside its stack is pasted as all zeros (its crop and pad, warp and
+ *              value tables still apply), and its target is y_to_float[0].  aae_occlusion reads a mask row outside the stack
+ *              as a mask without object pixels. */
+typedef struct {
+  int32_t struct_size;                 /* sizeof(aae_augment_args)                                                 */
+  /* geometry */
+  int32_t batch, h, w, c;              /* B images of H x W x C, C in 1..4                                         */
+  int32_t low_w;                       /* columns of the CoarseDropout cell grid (>= 1)                            */
+  /* sources: masks nonzero = BACKGROUND (the reference's mask_x) */
+  const uint8_t* x;                    /* [rows][H][W][C] object images                                            */
+  const uint8_t* mask;                 /* [rows][H][W]; may be NULL when mask_batch is set                         */
+  const uint8_t* bg;                   /* [rows][H][W][C] backgrounds                                              */
+  const uint8_t* y;                    /* [rows][H][W][C] reconstruction targets; read only for y_out              */
+  const int32_t* idx;                  /* [B] rows of x, mask and y, or NULL                                       */
+  const int32_t* idx_bg;               /* [B] rows of bg, or NULL                                                  */
+  int64_t n_images, n_bg;              /* rows of the x / mask / y stacks and of the bg stack (with idx)           */
+  const uint8_t* mask_batch;           /* optional [B][H][W]: row b is image b's mask (an aae_occlusion output)    */
+  /* per-batch draws */
+  const int32_t* geom;                 /* [B][4 + 2W + 2H] per image: flags (1 affine, 2 coarse dropout, 4 blur, 8 read the
+                                          CropAndPad output), dropout keep bits (low, high 32 bits over the CoarseDropout
+                                          cells, row-major), 0, then cv2.warpAffine's fixed-point tables adelta[W],
+                                          bdelta[W], X0[H], Y0[H] (10 fractional bits, rounding offset included)   */
+  const uint8_t* lut;                  /* [B][C][256]: the composed Add / Invert / Multiply / Multiply /
+                                          ContrastNormalization table                                              */
+  const int32_t* crop;                 /* [B][8] CropAndPad per image (below), or NULL: no CropAndPad pass         */
+  /* per-Augmenter constants */
+  const uint16_t* bilinear_tab;        /* [1024][4]: OpenCV's INTER_LINEAR weight table (rows sum to 32768)        */
+  const uint8_t* row_cell;             /* [H]: cv2.resize INTER_NEAREST row map of the dropout mask                */
+  const uint8_t* col_cell;             /* [W]: the column map                                                      */
+  const int32_t* blur_kernel_q8;       /* HOST pointer to 5 ints summing to 256, or NULL: no blur                  */
+  const float* u8_to_float;            /* [256]: value / 255., required with out_f32                               */
+  const float* y_to_float;             /* [256]: y_out = y_to_float[y] (Dataset passes the float32 values of the
+                                          y / 255. its gathered path computes), required with y_out                */
+  const int32_t* resample;             /* [resample_len] CropAndPad resampling blocks (below), required with crop  */
+  int64_t resample_len;
+  int32_t max_src_rows, max_src_w;     /* bounds of the source rows one 8-row output band reads and of sw          */
+  /* scratch */
+  uint8_t* tmp;                        /* [B][H][W][C] geometry-pass output                                        */
+  uint8_t* crop_tmp;                   /* [B][H][W][C] CropAndPad output, required with crop                       */
+  /* outputs: at least one of out_u8 / out_f32 */
+  uint8_t* out_u8;                     /* optional [B][H][W][C]                                                    */
+  float* out_f32;                      /* optional [B][H][W][C] = u8_to_float[out]                                 */
+  float* y_out;                        /* optional [B][H][W][C] reconstruction target; needs y and y_to_float      */
+} aae_augment_args;
 
-/* aae_augment_batch with CropAndPad in front (the training template's optional Sometimes(0.5, CropAndPad(percent=(-0.05, 0.1))),
- * imgaug's crop-pad-resize at keep_size=True): image b, when crop_dev[b][0] != 0, is the pasted image cropped / padded and resized
- * back to H x W before the geometry pass, which then reads it for the images whose geom flags have bit 8 set (set it exactly for
- * those images).  crop_dev int32 [B][8] per image:
+/* The augmentation chain.  CropAndPad (the training template's optional Sometimes(0.5, CropAndPad(percent=(-0.05, 0.1))),
+ * imgaug's crop-pad-resize at keep_size=True), when crop is set: image b, when crop[b][0] != 0, is the pasted image cropped /
+ * padded and resized back to H x W before the geometry pass, which reads it for the images whose geom flags have bit 8 set
+ * (set it exactly for those images).  crop[b]:
  *   [0] 0 off, 1 INTER_CUBIC, 2 INTER_AREA (cv2.resize's uint8 arithmetic);  [1] sh, [2] sw: size after crop and pad;
  *   [3] top, [4] left: signed pixels (negative = crop, positive = pad; source pixel (qy, qx) is pasted (qy - top, qx - left),
- *       pad_cval outside the image);  [5] pad_cval (0..255, all channels);  [6], [7]: offsets into resample_dev of the row
+ *       pad_cval outside the image);  [5] pad_cval (0..255, all channels);  [6], [7]: offsets into resample of the row
  *       block (H entries) and the column block (W entries).
- * resample_dev int32 [resample_len]: blocks of [dst][8] = 4 source indices (non-decreasing; in range of sh / sw) then 4 weights:
- *   cubic: fixed-point ints with 11 fractional bits; area: float32 bit patterns in OpenCV's summation order (unused taps weight 0).
- * max_src_rows / max_src_w bound the source rows one 8-row output band reads and sw; max_src_rows * max_src_w * c above 48 KB:
- * AAE_ERR_UNSUPPORTED.  An entry that breaks these bounds or its table's range writes zeros.  crop_tmp_dev: uint8 [B][H][W][C]
- * scratch of the pass.  Same stream rules as every input-pipeline call: every launch on `stream`, no allocation, no
- * synchronisation. */
-AAE_API int aae_augment_batch_crop(const uint8_t* x_dev, const uint8_t* mask_dev, const uint8_t* bg_dev, int batch, int h, int w, int c,
-                                   const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
-                                   const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
-                                   const float* u8_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev, float* out_f32_dev,
-                                   const int32_t* crop_dev, const int32_t* resample_dev, int64_t resample_len, int max_src_rows,
-                                   int max_src_w, uint8_t* crop_tmp_dev, void* stream);
+ * resample: blocks of [dst][8] = 4 source indices (non-decreasing; in range of sh / sw) then 4 weights: cubic: fixed-point
+ * ints with 11 fractional bits; area: float32 bit patterns in OpenCV's summation order (unused taps weight 0).
+ * max_src_rows * max_src_w * c above 48 KB: AAE_ERR_UNSUPPORTED.  A crop entry that breaks these bounds or its table's range
+ * writes zeros. */
+AAE_API int aae_augment(const aae_augment_args* a, void* stream);
 
-/* The occlusion switches of the training cfg, applied to the masks before aae_augment_batch (auto_pose/ae/dataset.py:421-454,
- * called at dataset.py:468-471).  mask_dev / mask_out_dev: uint8 [B][H][W], nonzero = BACKGROUND (the reference's mask_x);
- * mask_out_dev receives 0 / 1.  cand_dev: int32 [B][1 + 3K] per image, every draw made by the caller:
- *   [0]           occluder index into bank_dev (outside [0, n_bank): an occluder without pixels)
+/* The occlusion switches of the training cfg, applied to the masks before aae_augment (auto_pose/ae/dataset.py:421-454, called
+ * at dataset.py:468-471).  Image b's mask is row b of mask, or row idx[b] when idx is set (n_images >= 1).  Masks are uint8,
+ * nonzero = BACKGROUND; mask_out receives 0 / 1.
+ * cand: int32 [B][1 + 3K] per image, every draw made by the caller, K = n_cand:
+ *   [0]           occluder index into bank (outside [0, n_bank): an occluder without pixels)
  *   [1, K + 1)    column shifts tx,  [K + 1, 2K + 1) row shifts ty  (REALISTIC_OCCLUSION candidates, in draw order)
  *   [2K + 1, 3K + 1)  keep bits of the low_h x low_w dropout cells, row-major (SQUARE_OCCLUSION candidates; all cells set
  *                 when the Sometimes draw did not fire)
- * bank_dev: uint32 [n_bank][H][W/32] occluders, bit j of word w of a row = column 32 w + j.  row_cell_dev [H] / col_cell_dev
- * [W]: cv2.resize INTER_NEAREST index maps of the dropout cells.  realistic: the occluder shifted by (tx, ty) with zero fill
- * removes the object pixels it covers; the first candidate with 0 < removed / object < max_occl (double) is taken.  square:
- * the first candidate with NOT (kept / object < min_kept) (double, min_kept = 1 - SQUARE_OCCLUSION, object = the count of the
- * incoming mask) is taken.  An image whose K candidates of a step all fail keeps its mask from before that step and adds 1 to
- * fallbacks_dev[0] (realistic) or [1] (square); the reference re-draws without bound instead.  Either step may be off
- * (realistic = 0 / square = 0; its pointers may then be NULL).  W % 32 != 0, low_h * low_w > 32 or more than 48 KB of
- * shared memory per image return AAE_ERR_UNSUPPORTED. */
-AAE_API int aae_augment_occlusion(const uint8_t* mask_dev, int batch, int h, int w, const uint32_t* bank_dev, int n_bank,
-                                  const int32_t* cand_dev, int n_cand, int realistic, double max_occl, int square, double min_kept,
-                                  const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_h, int low_w,
-                                  uint8_t* mask_out_dev, int32_t* fallbacks_dev, void* stream);
+ * realistic: the occluder shifted by (tx, ty) with zero fill removes the object pixels it covers; the first candidate with
+ * 0 < removed / object < max_occl (double) is taken.  square: the first candidate with NOT (kept / object < min_kept) (double,
+ * min_kept = 1 - SQUARE_OCCLUSION, object = the count of the incoming mask) is taken.  An image whose K candidates of a step all
+ * fail keeps its mask from before that step and adds 1 to fallbacks[0] (realistic) or [1] (square); the reference re-draws
+ * without bound instead.  Either step may be off (0); its fields are then unused.  W % 32 != 0, low_h * low_w > 32 or more
+ * than 48 KB of shared memory per image: AAE_ERR_UNSUPPORTED. */
+typedef struct {
+  int32_t struct_size;                 /* sizeof(aae_occlusion_args)                                               */
+  /* geometry */
+  int32_t batch, h, w;                 /* B masks of H x W, W % 32 == 0                                            */
+  /* switches */
+  int32_t realistic, square;           /* REALISTIC_OCCLUSION / SQUARE_OCCLUSION step on (1) or off (0)            */
+  double max_occl;                     /* realistic: the switch's max_occl                                         */
+  double min_kept;                     /* square: 1 - the switch's max_occl                                        */
+  /* sources */
+  const uint8_t* mask;                 /* [rows][H][W]                                                             */
+  const int32_t* idx;                  /* [B] rows of mask, or NULL                                                */
+  int64_t n_images;                    /* rows of the mask stack (with idx)                                        */
+  /* per-batch draws */
+  const int32_t* cand;                 /* [B][1 + 3 n_cand] (above)                                                */
+  int32_t n_cand;                      /* K >= 1                                                                   */
+  /* per-Occlusion constants */
+  int32_t n_bank;                      /* occluders in bank (>= 1 with realistic)                                  */
+  const uint32_t* bank;                /* [n_bank][H][W/32] occluders, bit j of word w of a row = column 32 w + j  */
+  const uint8_t* row_cell;             /* [H]: cv2.resize INTER_NEAREST row map of the dropout cells (square)      */
+  const uint8_t* col_cell;             /* [W]: the column map (square)                                             */
+  int32_t low_h, low_w;                /* dropout cell grid (square)                                               */
+  /* outputs */
+  uint8_t* mask_out;                   /* [B][H][W]                                                                */
+  int32_t* fallbacks;                  /* [2]: realistic, square                                                   */
+} aae_occlusion_args;
 
-/* Indexed forms of the two calls above, for a training set resident on the device (Dataset.load_training_images(device=...)):
- * nothing of the batch is gathered.  x_stack_dev / y_stack_dev: uint8 [n_images][H][W][C], mask_stack_dev: uint8 [n_images][H][W]
- * (nonzero = background), bg_stack_dev: uint8 [n_bg][H][W][C].  Image b of the batch is row idx_dev[b] of the x, mask and y stacks
- * and row idx_bg_dev[b] of the background stack (int32 [batch] each, on the device).  Indices outside their stack: an image b
- * whose idx_dev[b] OR idx_bg_dev[b] is outside is pasted and warped as all zeros (its value tables still apply), and its target
- * is y_to_float_dev[0]; aae_augment_occlusion_indexed reads a mask row outside the stack as a mask without object pixels.
- *   aae_augment_occlusion_indexed: aae_augment_occlusion on the masks mask_stack_dev[idx_dev[b]]; mask_out_dev [batch][H][W].
- *   aae_augment_batch_indexed: aae_augment_batch on x_stack_dev[idx_dev[b]], background bg_stack_dev[idx_bg_dev[b]] and mask
- *     mask_stack_dev[idx_dev[b]] -- or, when mask_batch_dev is not NULL, row b of mask_batch_dev [batch][H][W] (an occlusion output;
- *     mask_stack_dev may then be NULL).  y_out_dev (optional, float32 [batch][H][W][C]) receives the reconstruction target
- *     y_to_float_dev[y_stack_dev[idx_dev[b]]], 256 floats chosen by the caller (Dataset passes the float32 values of y / 255. its gathered path computes).
- * Same stream rules as every input-pipeline call: every launch on `stream`, no allocation, no synchronisation. */
-AAE_API int aae_augment_batch_indexed(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
-                                      const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
-                                      const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
-                                      const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
-                                      const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
-                                      const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
-                                      float* out_f32_dev, float* y_out_dev, void* stream);
-/* aae_augment_batch_indexed with the CropAndPad pass of aae_augment_batch_crop (same crop arguments).  An image outside its
- * stack is pasted as zeros, and its crop and pad (pad_cval) still apply. */
-AAE_API int aae_augment_batch_indexed_crop(const uint8_t* x_stack_dev, const uint8_t* mask_stack_dev, const uint8_t* bg_stack_dev,
-                                           const uint8_t* y_stack_dev, int64_t n_images, int64_t n_bg, const int32_t* idx_dev,
-                                           const int32_t* idx_bg_dev, const uint8_t* mask_batch_dev, int batch, int h, int w, int c,
-                                           const int32_t* geom_dev, const uint8_t* lut_dev, const uint16_t* bilinear_tab_dev,
-                                           const uint8_t* row_cell_dev, const uint8_t* col_cell_dev, int low_w, const int32_t* blur_kernel_q8,
-                                           const float* u8_to_float_dev, const float* y_to_float_dev, uint8_t* tmp_dev, uint8_t* out_u8_dev,
-                                           float* out_f32_dev, float* y_out_dev, const int32_t* crop_dev, const int32_t* resample_dev,
-                                           int64_t resample_len, int max_src_rows, int max_src_w, uint8_t* crop_tmp_dev, void* stream);
-AAE_API int aae_augment_occlusion_indexed(const uint8_t* mask_stack_dev, int64_t n_images, const int32_t* idx_dev, int batch, int h, int w,
-                                          const uint32_t* bank_dev, int n_bank, const int32_t* cand_dev, int n_cand, int realistic,
-                                          double max_occl, int square, double min_kept, const uint8_t* row_cell_dev,
-                                          const uint8_t* col_cell_dev, int low_h, int low_w, uint8_t* mask_out_dev, int32_t* fallbacks_dev,
-                                          void* stream);
+AAE_API int aae_occlusion(const aae_occlusion_args* a, void* stream);
 
 /* ---------------------------------------------------------------- Training step ------------
  * Replaces sess.run(train_op): encoder fwd, decoder fwd, bootstrapped L2, backward, optimizer update

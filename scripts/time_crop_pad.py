@@ -2,7 +2,7 @@
 Sometimes(0.5, CropAndPad(percent=(-0.05, 0.1))) line, alternated in rounds (medians reported):
 
   batch        Dataset.batch_device(64) and Dataset.batch_resident(64), device time between CUDA events
-  kernel       the crop-pad pass: aae_augment_batch_crop minus aae_augment_batch on the same draws (events, half the images fired)
+  kernel       the crop-pad pass: aae_augment with the crop table minus without it, on the same draws (events, half the images fired)
   steps        the split and single-pass fp16 trainers through the started queue (Session.run on the device), per step
 
 Synthetic data; the card's name and power limit are read in the same run.  Writes nothing unless --out is given."""
@@ -59,12 +59,13 @@ def kernel_only(ds, dev, launches=200):
     gd, ld, cd = (torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in (geom, lut, aug.pack_crop(P)))
     tmp, ct, of = torch.empty_like(x), torch.empty_like(x), torch.empty(x.shape, dtype=torch.float32, device=dev)
     stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    args = [_lib.ptr(x), _lib.ptr(m), _lib.ptr(bg), B, 128, 128, 3, _lib.ptr(gd), _lib.ptr(ld), _lib.ptr(k["tab"]), _lib.ptr(k["rows"]),
-            _lib.ptr(k["cols"]), aug.low[1], _lib.ptr(k["taps"]) if k["taps"] is not None else None, _lib.ptr(k["to_float"]), _lib.ptr(tmp),
-            None, _lib.ptr(of)]
-    crop = [_lib.ptr(cd), _lib.ptr(k["resample"]), int(k["resample"].numel()), aug.crop["max_rows"], aug.crop["max_w"], _lib.ptr(ct)]
-    calls = {"without": lambda: _lib.check(_lib.lib().aae_augment_batch(*args, stream)),
-             "with": lambda: _lib.check(_lib.lib().aae_augment_batch_crop(*args, *crop, stream))}
+    plain = _lib.AugmentArgs(batch=B, h=128, w=128, c=3, low_w=aug.low[1], x=x, mask=m, bg=bg, geom=gd, lut=ld, bilinear_tab=k["tab"],
+                             row_cell=k["rows"], col_cell=k["cols"], blur_kernel_q8=k["taps"], u8_to_float=k["to_float"], tmp=tmp,
+                             out_f32=of)
+    crop = plain.copy().set(crop=cd, resample=k["resample"], resample_len=int(k["resample"].numel()), max_src_rows=aug.crop["max_rows"],
+                            max_src_w=aug.crop["max_w"], crop_tmp=ct)
+    calls = {"without": lambda: _lib.check(_lib.lib().aae_augment(C.byref(plain), stream)),
+             "with": lambda: _lib.check(_lib.lib().aae_augment(C.byref(crop), stream))}
     res = {n: [] for n in calls}
     for r in range(ROUNDS + 1):
         for n, fn in calls.items():

@@ -1,6 +1,6 @@
 """Cost of the occlusion switches in the device input pipeline at batch 64: Dataset.batch_device with both switches off,
 REALISTIC_OCCLUSION only, and both (alternated in rounds, host clock around synchronised batches), the
-aae_augment_occlusion kernel alone (CUDA events), and the host's candidate draws + packing.  Synthetic data; writes nothing."""
+aae_occlusion kernel alone (CUDA events), and the host's candidate draws + packing.  Synthetic data; writes nothing."""
 import ctypes as C
 import os
 import subprocess
@@ -89,10 +89,12 @@ def main():
         cand = torch.from_numpy(occl.pack(occl.sample(B, N_BANK))).to(dev)
         stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
+        args = _lib.OcclusionArgs(batch=B, h=H, w=H, realistic=1, max_occl=R, square=int(S != 0), min_kept=1.0 - S, mask=mask, cand=cand,
+                                  n_cand=occl.K, n_bank=N_BANK, bank=st["bank"], row_cell=st["rows"], col_cell=st["cols"],
+                                  low_h=occl.low[0], low_w=occl.low[1], mask_out=out, fallbacks=st["fallbacks"])
+
         def launch():
-            _lib.check(_lib.lib().aae_augment_occlusion(
-                _lib.ptr(mask), B, H, H, _lib.ptr(st["bank"]), N_BANK, _lib.ptr(cand), occl.K, 1, R, int(S != 0), 1.0 - S,
-                _lib.ptr(st["rows"]), _lib.ptr(st["cols"]), occl.low[0], occl.low[1], _lib.ptr(out), _lib.ptr(st["fallbacks"]), stream))
+            _lib.check(_lib.lib().aae_occlusion(C.byref(args), stream))
 
         for _ in range(10):
             launch()
@@ -104,7 +106,7 @@ def main():
             ev[1].record()
             ev[1].synchronize()
             res.append(ev[0].elapsed_time(ev[1]) / 200 * 1e3)
-        print("aae_augment_occlusion %-9s %.1f us per batch of %d (median of %d x 200 launches)" % (label, np.median(res), B, rounds))
+        print("aae_occlusion %-9s %.1f us per batch of %d (median of %d x 200 launches)" % (label, np.median(res), B, rounds))
     occl.fallbacks()
 
     # host side: candidate draws + packing

@@ -1,4 +1,4 @@
-"""Occlusion-mask augmentations on the device (aae_augment_occlusion) against the CPU restatement, which
+"""Occlusion-mask augmentations on the device (aae_occlusion) against the CPU restatement, which
 tests/test_occlusion_cpu.py pins to the reference's own output and to OpenCV."""
 import numpy as np
 import pytest

@@ -463,7 +463,7 @@ def test_set_weights_then_forward_on_the_side_stream(sess, delay, prec):
 
 
 # ------------------------------------------------------------------------------------------------ input pipeline
-def test_augment_occlusion_and_crop_extraction(sess, delay, tmp_path):
+def test_augment_args_occlusion_args_and_crop_extraction(sess, delay, tmp_path):
     from tests.test_gpu_g_occlusion import _bank, _objects
     from tests.test_gpu_z_augment import _inputs
     lib, B = _lib.lib(), 24
@@ -479,13 +479,13 @@ def test_augment_occlusion_and_crop_extraction(sess, delay, tmp_path):
 
     def augment(xd, md, bd, gd, ld):
         tmp, ou, of = poisoned(xd.shape, torch.uint8), poisoned(xd.shape, torch.uint8), poisoned(xd.shape, torch.float32)
-        ok(lib.aae_augment_batch(_lib.ptr(xd), _lib.ptr(md), _lib.ptr(bd), B, 128, 128, 3, _lib.ptr(gd), _lib.ptr(ld), _lib.ptr(k["tab"]),
-                                 _lib.ptr(k["rows"]), _lib.ptr(k["cols"]), aug.low[1], _lib.ptr(taps), _lib.ptr(k["to_float"]), _lib.ptr(tmp),
-                                 _lib.ptr(ou), _lib.ptr(of), S()))
+        ok(lib.aae_augment(C.byref(_lib.AugmentArgs(
+            batch=B, h=128, w=128, c=3, low_w=aug.low[1], x=xd, mask=md, bg=bd, geom=gd, lut=ld, bilinear_tab=k["tab"], row_cell=k["rows"],
+            col_cell=k["cols"], blur_kernel_q8=taps, u8_to_float=k["to_float"], tmp=tmp, out_u8=ou, out_f32=of)), S()))
         return ou, of
     inputs = [dev(x), dev(mask.astype(np.uint8)), dev(bg), dev(geom.astype(np.int32)), dev(lut.astype(np.uint8))]
     want = aug.augment_device(inputs[0], inputs[1], inputs[2], params=P, want_u8=True)
-    ou, of = run_on_side_stream(augment, inputs, delay, "augment_batch")
+    ou, of = run_on_side_stream(augment, inputs, delay, "augment")
     assert np.array_equal(ou, want[1].cpu().numpy()) and np.array_equal(of, want[0].cpu().numpy())
 
     rng = np.random.RandomState(0)
@@ -498,12 +498,14 @@ def test_augment_occlusion_and_crop_extraction(sess, delay, tmp_path):
 
     def occlude(md, cand, bk):
         out, fb = poisoned(md.shape, torch.uint8), torch.zeros(2, dtype=torch.int32, device="cuda")
-        ok(lib.aae_augment_occlusion(_lib.ptr(md), B, 128, 128, _lib.ptr(bk), len(words), _lib.ptr(cand), occl.K, 1, 0.4, 1, 1.0 - 0.2,
-                                     _lib.ptr(st["rows"]), _lib.ptr(st["cols"]), occl.low[0], occl.low[1], _lib.ptr(out), _lib.ptr(fb), S()))
+        ok(lib.aae_occlusion(C.byref(_lib.OcclusionArgs(
+            batch=B, h=128, w=128, realistic=1, max_occl=0.4, square=1, min_kept=1.0 - 0.2, mask=md, cand=cand, n_cand=occl.K,
+            n_bank=len(words), bank=bk, row_cell=st["rows"], col_cell=st["cols"], low_h=occl.low[0], low_w=occl.low[1], mask_out=out,
+            fallbacks=fb)), S()))
         return out, fb
     md = dev(masks.astype(np.uint8))
     want_o = occl.apply_device(md, words, params=PO).cpu().numpy()
-    out, _ = run_on_side_stream(occlude, [md, dev(occl.pack(PO)), bank], delay, "augment_occlusion")
+    out, _ = run_on_side_stream(occlude, [md, dev(occl.pack(PO)), bank], delay, "occlusion")
     assert np.array_equal(out, want_o) and 0 < out.mean() < 1
 
     frame = dev(np.random.RandomState(2).randint(0, 256, (480, 640, 3), dtype=np.uint8))

@@ -1,6 +1,6 @@
 """The training set resident on the device, the started Queue and ae_train (augmentedautoencoder_b200/ae/ae_train.py).
 
-  * Dataset.batch_resident (aae_augment_batch_indexed / aae_augment_occlusion_indexed) returns batch_device's (x, y) bit for bit,
+  * Dataset.batch_resident (aae_augment / aae_occlusion with idx set) returns batch_device's (x, y) bit for bit,
     with the same occlusion fallback counts, from the same seeds;
   * after Queue.start the k-th pulled batch is the k-th synchronous one; a slot is not rewritten before the run that read it has
     finished on the consumer's stream, even when that stream is held back; stop() joins the producer;

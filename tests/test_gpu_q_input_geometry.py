@@ -1,4 +1,4 @@
-"""The training input kernels (aae_augment_batch, aae_augment_occlusion and their indexed forms) against the CPU restatement at
+"""The training input kernels (aae_augment and aae_occlusion, gathered and indexed) against the CPU restatement at
 the cfg geometries beyond the template (tests/geometry_table.py): px64 (64 x 64 x 3), gray (128 x 128 x 1) and rect (64 x 128 x 3),
 where tests/test_input_geometry_cpu.py pins the restatement to OpenCV.  Every comparison is bit for bit: the pipelines are
 integer, and the float outputs are table look-ups.
@@ -104,7 +104,7 @@ def _y_target(y):
     return (torch.arange(256, dtype=torch.float32, device=DEV) / 255.0).cpu().numpy()[y]
 
 
-# ---- aae_augment_batch --------------------------------------------------------------------------------------------------------------
+# ---- aae_augment --------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("sigma", SIGMAS)
 @pytest.mark.parametrize("geom", GEOMS)
 def test_augment_batch_matches_the_restatement(geom, sigma):
@@ -124,7 +124,7 @@ def test_augment_batch_matches_the_restatement(geom, sigma):
     assert np.array_equal(got_f.cpu().numpy(), (want / 255.).astype(np.float32))
 
 
-# ---- aae_augment_occlusion at 64 x 64 -----------------------------------------------------------------------------------------------
+# ---- aae_occlusion at 64 x 64 -------------------------------------------------------------------------------------------------------
 FAR = [(1, 1), (1, -1), (-1, 1), (-1, -1)]                    # signs of (tx, ty) of the arranged accepts
 LATE = [0, 9, 20, A.OCCLUSION_CANDIDATES - 1]                # ... and the candidate they sit at
 

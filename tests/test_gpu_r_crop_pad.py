@@ -1,7 +1,8 @@
-"""CropAndPad on the device (aae_augment_batch_crop / aae_augment_batch_indexed_crop) against the CPU restatement, which
+"""CropAndPad on the device (aae_augment with a crop table, gathered and indexed) against the CPU restatement, which
 tests/test_crop_pad_cpu.py pins to OpenCV: forced firing patterns at every input geometry, the gathered, resident and queued
 batches bit for bit, ae_train from a cfg with the template's CropAndPad line uncommented, and the stream contract."""
 import configparser
+import ctypes as C
 import gc
 import os
 
@@ -196,7 +197,7 @@ def test_ae_train_with_crop_and_pad_uncommented(sess, golden_dir, tmp_path, monk
         m.close()
 
 
-def test_crop_entry_points_on_a_side_stream(sess, delay):
+def test_augment_with_a_crop_table_on_a_side_stream(sess, delay):
     lib, B = _lib.lib(), 24
     rng = np.random.RandomState(0)
     x, mask, bg = _inputs(rng, B, 128, 128, 3)
@@ -207,17 +208,18 @@ def test_crop_entry_points_on_a_side_stream(sess, delay):
     crop = aug.pack_crop(P)
     k = aug._constants(DEV)
     rs, taps = k["resample"], k["taps"]
-    cargs = lambda cd, ct: [_lib.ptr(cd), _lib.ptr(rs), int(rs.numel()), aug.crop["max_rows"], aug.crop["max_w"], _lib.ptr(ct)]   # noqa: E731
+    const = dict(batch=B, h=128, w=128, c=3, low_w=aug.low[1], bilinear_tab=k["tab"], row_cell=k["rows"], col_cell=k["cols"],
+                 blur_kernel_q8=taps, u8_to_float=k["to_float"], resample=rs, resample_len=int(rs.numel()),
+                 max_src_rows=aug.crop["max_rows"], max_src_w=aug.crop["max_w"])
 
     def gathered(xd, md, bd, gd, ld, cd):
         tmp, ct, of = poisoned(xd.shape, torch.uint8), poisoned(xd.shape, torch.uint8), poisoned(xd.shape, torch.float32)
-        ok(lib.aae_augment_batch_crop(_lib.ptr(xd), _lib.ptr(md), _lib.ptr(bd), B, 128, 128, 3, _lib.ptr(gd), _lib.ptr(ld), _lib.ptr(k["tab"]),
-                                      _lib.ptr(k["rows"]), _lib.ptr(k["cols"]), aug.low[1], _lib.ptr(taps), _lib.ptr(k["to_float"]),
-                                      _lib.ptr(tmp), None, _lib.ptr(of), *cargs(cd, ct), S()))
+        ok(lib.aae_augment(C.byref(_lib.AugmentArgs(x=xd, mask=md, bg=bd, geom=gd, lut=ld, crop=cd, tmp=tmp, crop_tmp=ct, out_f32=of,
+                                                    **const)), S()))
         return of
     inputs = [dev(x), dev(mask.astype(np.uint8)), dev(bg), dev(geom), dev(lut), dev(crop)]
     want = aug.augment_device(inputs[0], inputs[1], inputs[2], params=P)
-    of = run_on_side_stream(gathered, inputs, delay, "augment_batch_crop")[0]
+    of = run_on_side_stream(gathered, inputs, delay, "augment crop-pad")[0]
     assert np.array_equal(of, want.cpu().numpy())
     returns_before_the_device(lambda: gathered(*inputs), delay)
 
@@ -226,19 +228,18 @@ def test_crop_entry_points_on_a_side_stream(sess, delay):
     def indexed(xd, md, bd, yd, id_, gd, ld, cd):
         tmp, ct = poisoned(xd.shape, torch.uint8), poisoned(xd.shape, torch.uint8)
         of, yo = poisoned(xd.shape, torch.float32), poisoned(xd.shape, torch.float32)
-        ok(lib.aae_augment_batch_indexed_crop(
-            _lib.ptr(xd), _lib.ptr(md), _lib.ptr(bd), _lib.ptr(yd), B, B, _lib.ptr(id_), _lib.ptr(id_), None, B, 128, 128, 3, _lib.ptr(gd),
-            _lib.ptr(ld), _lib.ptr(k["tab"]), _lib.ptr(k["rows"]), _lib.ptr(k["cols"]), aug.low[1], _lib.ptr(taps), _lib.ptr(k["to_float"]),
-            _lib.ptr(k["y_to_float"]), _lib.ptr(tmp), None, _lib.ptr(of), _lib.ptr(yo), *cargs(cd, ct), S()))
+        ok(lib.aae_augment(C.byref(_lib.AugmentArgs(
+            x=xd, mask=md, bg=bd, y=yd, idx=id_, idx_bg=id_, n_images=B, n_bg=B, geom=gd, lut=ld, crop=cd, y_to_float=k["y_to_float"],
+            tmp=tmp, crop_tmp=ct, out_f32=of, y_out=yo, **const)), S()))
         return of, yo
     ins = [dev(x), dev(mask.astype(np.uint8)), dev(bg), dev(x), dev(idx), dev(geom), dev(lut), dev(crop)]
-    of, yo = run_on_side_stream(indexed, ins, delay, "augment_batch_indexed_crop")
+    of, yo = run_on_side_stream(indexed, ins, delay, "augment indexed crop-pad")
     want = CP.augment_batch(x[idx], mask[idx], bg[idx], P, aug.sigma, low=aug.low)
     assert np.array_equal(of, (want / 255.).astype(np.float32))
     returns_before_the_device(lambda: indexed(*ins), delay)
 
 
-def test_a_geometry_whose_rows_do_not_fit_is_refused(monkeypatch):
+def test_augment_refuses_a_geometry_whose_rows_do_not_fit(monkeypatch):
     """Below four area taps (ratio < 3) the staged rows of a 128-wide crop stay under 48 KB, so the limit is lowered to reach
     the construction check; the library's own check takes a bound above it."""
     with monkeypatch.context() as m:
@@ -248,8 +249,8 @@ def test_a_geometry_whose_rows_do_not_fit_is_refused(monkeypatch):
     aug = A.Augmenter(CROP_CODE, seed=0)
     x = torch.zeros((2, 128, 128, 3), dtype=torch.uint8, device=DEV)
     k = aug._constants(DEV)
-    st = _lib.lib().aae_augment_batch_crop(
-        _lib.ptr(x), _lib.ptr(x[..., 0]), _lib.ptr(x), 2, 128, 128, 3, _lib.ptr(x), _lib.ptr(x), _lib.ptr(k["tab"]), _lib.ptr(k["rows"]),
-        _lib.ptr(k["cols"]), aug.low[1], None, _lib.ptr(k["to_float"]), _lib.ptr(x), _lib.ptr(x), None, _lib.ptr(x), _lib.ptr(k["resample"]),
-        int(k["resample"].numel()), 200, 154, _lib.ptr(x), S())
+    st = _lib.lib().aae_augment(C.byref(_lib.AugmentArgs(
+        batch=2, h=128, w=128, c=3, low_w=aug.low[1], x=x, mask=x[..., 0], bg=x, geom=x, lut=x, crop=x, bilinear_tab=k["tab"],
+        row_cell=k["rows"], col_cell=k["cols"], u8_to_float=k["to_float"], resample=k["resample"], resample_len=int(k["resample"].numel()),
+        max_src_rows=200, max_src_w=154, tmp=x, crop_tmp=x, out_u8=x)), S())
     assert st == -3 and b"shared memory" in _lib.lib().aae_last_error_string()

@@ -1,4 +1,4 @@
-"""Device training-input pipeline (aae_augment_batch) against the CPU restatement, which tests/test_augment_cpu.py pins to OpenCV."""
+"""Device training-input pipeline (aae_augment) against the CPU restatement, which tests/test_augment_cpu.py pins to OpenCV."""
 import numpy as np
 import pytest
 import torch
