@@ -133,7 +133,7 @@ _SIGS = {
     "aae_trainer_set_global_step": (_I, [_P, _L]),
     "aae_trainer_set_latent_terms": (_I, [_P, _F, _F]),
     "aae_trainer_set_latent_noise": (_I, [_P, _F]),
-    "aae_extract_square_patches": (_I, [_P, _I, _I, _P, _I, _F, _I, _P, _P]),
+    "aae_extract_square_patches": (_I, [_P, _I, _I, _P, _I, _I, _P, _P]),
     "aae_augment": (_I, [C.POINTER(AugmentArgs), _P]),
     "aae_occlusion": (_I, [C.POINTER(OcclusionArgs), _P]),
 }

@@ -309,7 +309,7 @@ struct aae_trainer {
 };
 
 // ============================================================================ misc
-extern "C" int aae_version(void) { return 101; }
+extern "C" int aae_version(void) { return 102; }
 extern "C" int64_t aae_launch_count(void) { return (int64_t)g_launches.load(); }
 extern "C" const char* aae_last_error_string(void) { return g_err; }
 

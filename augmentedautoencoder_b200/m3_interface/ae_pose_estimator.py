@@ -20,6 +20,24 @@ from ..ae.session import Session
 from .m3_interfaces import PoseEstimate, PoseEstInterface
 
 
+def square_patch_boxes(boxes_xywh, pad_factor):
+    """int32 [n, 5] table of (x, y, w, h, size) per box, with the reference's own expressions (ae_pose_estimator.py:108-109):
+    ``np.array(bb_xywh).astype(np.int32)`` on the float64 box and ``int(np.maximum(h, w) * pad_factor)``, a float64 product
+    with the Python float ``pad_factor``.  Neither goes through float32: a box side such as 21.999999999999996 rounds up to
+    22 in float32, and float32(1.3) is below 1.3.  Raises ValueError for a box whose square would be smaller than its
+    longest side (a pad factor below 1), where the reference pastes outside its square."""
+    b = np.asarray(boxes_xywh, dtype=np.float64).reshape(-1, 4).astype(np.int32)
+    pad_factor = float(pad_factor)
+    longest = np.maximum(b[:, 3], b[:, 2])
+    size = (longest * pad_factor).astype(np.int64)          # int() of each float64 product: truncation toward zero
+    bad = np.flatnonzero(size < longest)
+    if len(bad):
+        raise ValueError("pad factor %r makes a %d px square for the box %s (x, y, w, h = %s), smaller than its longest side"
+                         % (pad_factor, size[bad[0]], np.asarray(boxes_xywh, dtype=np.float64).reshape(-1, 4)[bad[0]].tolist(),
+                            b[bad[0]].tolist()))
+    return np.ascontiguousarray(np.concatenate([b, size[:, None].astype(np.int32)], axis=1))
+
+
 class AePoseEstimator(PoseEstInterface):
 
     def __init__(self, test_config_path, devices=None, precision=None):
@@ -79,8 +97,7 @@ class AePoseEstimator(PoseEstInterface):
     def extract_square_patch(self, scene_img, bb_xywh, pad_factor, resize=(128, 128), interpolation=cv2.INTER_NEAREST, black_borders=False):
         """Square, zero-padded patch around a detection, bbox content centred (ae_pose_estimator.py:106-131; ``process``
         always uses black_borders=True).  The reference's other branch slices with float indices and cannot run."""
-        x, y, w, h = np.array(bb_xywh).astype(np.int32)
-        size = int(np.maximum(h, w) * pad_factor)
+        x, y, w, h, size = (int(v) for v in square_patch_boxes(bb_xywh, pad_factor)[0])
         scene_crop = np.zeros((size, size, 3), dtype=np.uint8)
         if not black_borders:
             raise NotImplementedError("black_borders=False is broken upstream (float slice indices, ae_pose_estimator.py:118-127)")
@@ -89,15 +106,18 @@ class AePoseEstimator(PoseEstInterface):
 
     def extract_square_patches_device(self, frame_dev, boxes_xywh, pad_factor, patch_size):
         """All crops of a frame in one launch (aae_extract_square_patches): the same pixels as ``extract_square_patch(...,
-        interpolation=cv2.INTER_LINEAR, black_borders=True)`` per box, bit for bit.  frame_dev: CUDA uint8 [H,W,3]."""
+        interpolation=cv2.INTER_LINEAR, black_borders=True)`` per box, bit for bit.  frame_dev: CUDA uint8 [H,W,3].  The
+        box integers and square sizes are computed here (``square_patch_boxes``), the pixels on the device.  A box past the
+        frame's right or bottom edge, which the reference refuses, is cropped from the frame padded with black."""
         if patch_size[0] != patch_size[1]:
             raise NotImplementedError("non-square patches")
-        n, ps = len(boxes_xywh), int(patch_size[0])
+        table = square_patch_boxes(boxes_xywh, pad_factor)
+        n, ps = len(table), int(patch_size[0])
         dev = frame_dev.device
-        boxes = torch.tensor(np.asarray(boxes_xywh, dtype=np.float32).reshape(n, 4)).to(dev)
+        boxes = torch.from_numpy(table).to(dev)
         out = torch.empty((n, ps, ps, 3), dtype=torch.uint8, device=dev)
         _lib.check(_lib.lib().aae_extract_square_patches(_lib.ptr(frame_dev), frame_dev.shape[0], frame_dev.shape[1], _lib.ptr(boxes), n,
-                                                         float(pad_factor), ps, _lib.ptr(out), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+                                                         ps, _lib.ptr(out), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
                    "extract_square_patches")
         return out
 

@@ -461,10 +461,13 @@ AAE_API int aae_trainer_profile(aae_trainer* h, int enable, float* phase_ms_out,
 /* ---------------------------------------------------------------- Crop extraction ----------
  * Batched AePoseEstimator.extract_square_patch(black_borders=True) + cv2.resize(INTER_LINEAR)
  * (auto_pose/m3_interface/ae_pose_estimator.py:106-131,157-162): one launch for all detections of a frame, bit-exact
- * with OpenCV's 8-bit fixed-point path.  image_dev: BGR uint8 [img_h, img_w, 3]; boxes_xywh_dev: [n,4] float32 pixel
- * boxes (truncated to int like the reference); out_dev: NHWC uint8 [n, out_size, out_size, 3]. */
-AAE_API int aae_extract_square_patches(const uint8_t* image_dev, int img_h, int img_w, const float* boxes_xywh_dev,
-                                       int n_boxes, float pad_factor, int out_size, uint8_t* out_dev, void* stream);
+ * with OpenCV's 8-bit fixed-point path.  image_dev: BGR uint8 [img_h, img_w, 3]; boxes_xywhs_dev: int32 [n, 5] rows
+ * (x, y, w, h, size): the box truncated to int and the square's side, computed by the caller as the reference does, from
+ * the float64 box and the float64 pad factor (int(max(h, w) * pad_factor)); out_dev: NHWC uint8 [n, out_size, out_size, 3].
+ * Pixels of the box outside the frame read as black.  A row with w <= 0, h <= 0, size <= 0 or size < max(w, h) gives a black
+ * crop.  out_size in [1, 1024]. */
+AAE_API int aae_extract_square_patches(const uint8_t* image_dev, int img_h, int img_w, const int32_t* boxes_xywhs_dev,
+                                       int n_boxes, int out_size, uint8_t* out_dev, void* stream);
 
 #ifdef __cplusplus
 }

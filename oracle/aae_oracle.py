@@ -205,27 +205,28 @@ def _check_device(dtype: torch.dtype, device: str) -> None:
 
 
 def encoder_layers(x: np.ndarray, params: Dict[str, np.ndarray], strides=STRIDES,
-                   dtype: torch.dtype = torch.float32) -> List[torch.Tensor]:
+                   dtype: torch.dtype = torch.float32, device: str = "cpu") -> List[torch.Tensor]:
     """All intermediate activations of the encoder: [conv1, conv2, ..., flatten, z]
-    (auto_pose/ae/encoder.py:37-68)."""
-    h = _t(x, dtype)
+    (auto_pose/ae/encoder.py:37-68).  device="cuda" evaluates float64 on the GPU."""
+    _check_device(dtype, device)
+    h = _t(x, dtype, device)
     outs: List[torch.Tensor] = []
     for i, s in enumerate(strides):
         name = "conv2d" if i == 0 else f"conv2d_{i}"
-        h = conv2d_same(h, _t(params[f"{name}/kernel"], dtype), _t(params[f"{name}/bias"], dtype), s, "relu")
+        h = conv2d_same(h, _t(params[f"{name}/kernel"], dtype, device), _t(params[f"{name}/bias"], dtype, device), s, "relu")
         outs.append(h)
     flat = h.reshape(h.shape[0], -1)  # tf.layers.flatten on NHWC: (h, w, c) order
     outs.append(flat)
-    z = flat @ _t(params["dense/kernel"], dtype) + _t(params["dense/bias"], dtype)
+    z = flat @ _t(params["dense/kernel"], dtype, device) + _t(params["dense/bias"], dtype, device)
     outs.append(z)
     return outs
 
 
 def encoder_forward(x: np.ndarray, params: Dict[str, np.ndarray], strides=STRIDES,
-                    dtype: torch.dtype = torch.float32) -> np.ndarray:
+                    dtype: torch.dtype = torch.float32, device: str = "cpu") -> np.ndarray:
     """crop batch (float NHWC in [0,1]) -> z [B, latent]."""
     with torch.no_grad():
-        return encoder_layers(x, params, strides, dtype)[-1].numpy()
+        return encoder_layers(x, params, strides, dtype, device)[-1].cpu().numpy()
 
 
 def l2_normalize(z: np.ndarray, eps: float = 1e-12) -> np.ndarray:
@@ -256,10 +257,11 @@ def select_indices(cos: np.ndarray, top_n: int = 1, upright: bool = False, num_c
 
 def nearest_rotation_idcs(x: np.ndarray, enc_params: Dict[str, np.ndarray], codebook: np.ndarray,
                           top_n: int = 1, upright: bool = False, num_cyclo: int = NUM_CYCLO,
-                          dtype: torch.dtype = torch.float32, return_cos: bool = False):
-    """Codebook.nearest_rotation(..., return_idcs=True) end to end (auto_pose/ae/codebook.py:55-73)."""
+                          dtype: torch.dtype = torch.float32, return_cos: bool = False, device: str = "cpu"):
+    """Codebook.nearest_rotation(..., return_idcs=True) end to end (auto_pose/ae/codebook.py:55-73).  device="cuda" runs
+    the float64 encoder on the GPU; the cosines and the selection stay on the host."""
     xf = preprocess(x)
-    z = encoder_forward(xf, enc_params, dtype=dtype)
+    z = encoder_forward(xf, enc_params, dtype=dtype, device=device)
     cb = codebook.astype(np.float64 if dtype == torch.float64 else np.float32)
     cos = cos_similarity(z, cb)
     idcs = select_indices(cos, top_n, upright, num_cyclo)

@@ -113,6 +113,27 @@ pose_visualization = False
 """
 
 
+def make_workspace(ws, objects, n):
+    """A throw-away AE_WORKSPACE_PATH with one experiment per object under group grp: its train cfg and a checkpoint of
+    random encoder weights, an n-row codebook and rendered boxes.  objects: {name: (seed, train cfg text)}.  Returns
+    {name: (encoder params, codebook, boxes)}."""
+    objs = {}
+    for name, (seed, cfg) in objects.items():
+        d = ws / "experiments" / "grp" / name
+        (d / "checkpoints").mkdir(parents=True)
+        (d / (name + ".cfg")).write_text(cfg)
+        p = O.make_encoder_params(40 + seed, bias_scale=0.02)
+        E = O.make_codebook(60 + seed, n=n)
+        rng = np.random.RandomState(seed)
+        bbs = np.stack([rng.randint(200, 400, n), rng.randint(100, 300, n), rng.randint(60, 200, n), rng.randint(60, 200, n)], 1).astype(np.int32)
+        ckpt = {name + "/" + k: v for k, v in p.items()}
+        ckpt[name + "/embedding_normalized"] = E
+        ckpt[name + "/embed_obj_bbs_var"] = bbs
+        np.savez(d / "checkpoints" / "chkpt-30000.npz", **ckpt)
+        objs[name] = (p, E, bbs)
+    return objs
+
+
 def test_pose_estimator_process_end_to_end(tmp_path, monkeypatch):
     """Two object classes, five detections (one of an unknown class), one frame: every detection must get exactly the pose
     the reference algorithm yields (crop -> encoder -> codebook NN -> pose lift), restated with the CPU oracle."""
@@ -125,20 +146,7 @@ def test_pose_estimator_process_end_to_end(tmp_path, monkeypatch):
     monkeypatch.setenv("AE_WORKSPACE_PATH", str(ws))
     ds = Dataset(None, min_n_views=162, num_cyclo=36, radius=700)
     n = ds.embedding_size
-    objs = {}
-    for name, seed in (("obj_a", 1), ("obj_b", 2)):
-        d = ws / "experiments" / "grp" / name
-        (d / "checkpoints").mkdir(parents=True)
-        (d / (name + ".cfg")).write_text(TRAIN_CFG)
-        p = O.make_encoder_params(40 + seed, bias_scale=0.02)
-        E = O.make_codebook(60 + seed, n=n)
-        rng = np.random.RandomState(seed)
-        bbs = np.stack([rng.randint(200, 400, n), rng.randint(100, 300, n), rng.randint(60, 200, n), rng.randint(60, 200, n)], 1).astype(np.int32)
-        ckpt = {name + "/" + k: v for k, v in p.items()}
-        ckpt[name + "/embedding_normalized"] = E
-        ckpt[name + "/embed_obj_bbs_var"] = bbs
-        np.savez(d / "checkpoints" / "chkpt-30000.npz", **ckpt)
-        objs[name] = (p, E, bbs)
+    objs = make_workspace(ws, {"obj_a": (1, TRAIN_CFG), "obj_b": (2, TRAIN_CFG)}, n)
     cfg_path = tmp_path / "m3.cfg"
     cfg_path.write_text(M3_CFG)
     est = AePoseEstimator(str(cfg_path))

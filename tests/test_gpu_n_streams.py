@@ -23,6 +23,7 @@ import torch
 
 from augmentedautoencoder_b200 import _lib
 from augmentedautoencoder_b200.ae import augment as A
+from augmentedautoencoder_b200.m3_interface.ae_pose_estimator import square_patch_boxes
 from oracle import aae_oracle as O
 from tests.test_augment_cpu import TEMPLATE_CODE
 from tests.test_gpu_a_parity import _codebook, _enc, sess  # noqa: F401
@@ -463,7 +464,9 @@ def test_set_weights_then_forward_on_the_side_stream(sess, delay, prec):
 
 
 # ------------------------------------------------------------------------------------------------ input pipeline
-def test_augment_args_occlusion_args_and_crop_extraction(sess, delay, tmp_path):
+def test_augment_args_occlusion_args_and_crop_table_extraction(sess, delay, tmp_path):
+    """aae_augment, aae_occlusion and aae_extract_square_patches, the last with its int32 (x, y, w, h, size) box table, on a
+    caller's side stream."""
     from tests.test_gpu_g_occlusion import _bank, _objects
     from tests.test_gpu_z_augment import _inputs
     lib, B = _lib.lib(), 24
@@ -509,11 +512,11 @@ def test_augment_args_occlusion_args_and_crop_extraction(sess, delay, tmp_path):
     assert np.array_equal(out, want_o) and 0 < out.mean() < 1
 
     frame = dev(np.random.RandomState(2).randint(0, 256, (480, 640, 3), dtype=np.uint8))
-    boxes = dev(np.array([[100, 120, 80, 60], [-10, -20, 90, 120], [600, 440, 70, 70], [300, 200, 200, 150], [0, 0, 640, 480]], np.float32))
+    boxes = dev(square_patch_boxes([[100, 120, 80, 60], [-10, -20, 90, 120], [600, 440, 70, 70], [300, 200, 200, 150], [0, 0, 640, 480]], 1.2))
 
     def extract(fr, bx):
         out = poisoned((5, 128, 128, 3), torch.uint8)
-        ok(lib.aae_extract_square_patches(_lib.ptr(fr), 480, 640, _lib.ptr(bx), 5, 1.2, 128, _lib.ptr(out), S()))
+        ok(lib.aae_extract_square_patches(_lib.ptr(fr), 480, 640, _lib.ptr(bx), 5, 128, _lib.ptr(out), S()))
         return out
     patches = run_on_side_stream(extract, [frame, boxes], delay, "extract_square_patches")[0]
     assert patches.std() > 10
