@@ -215,7 +215,9 @@ class ObjectRouter:
         missing = [c for c in self.mine if c not in self.codebooks]
         if missing:
             raise ValueError("rank %d owns classes %s but has no codebook for them" % (self.rank, missing))
-        self._stage = None
+        self._stage = None           # pinned staging buffer of route_host
+        self._copy = {}              # device index -> the stream route_host uploads on
+        self._uploaded = None        # event behind the last upload from the stage
 
     def _run_class(self, cls, crops_dev):
         return self.codebooks[cls].nearest_idx_device(crops_dev, k=1)
@@ -245,23 +247,43 @@ class ObjectRouter:
         return scores, idx
 
     def route(self, crops_dev, class_ids):
-        """crops_dev [B,H,W,C] already on this rank's device.  Returns (scores [B], idx [B]) complete on every rank."""
+        """crops_dev [B,H,W,C] already on this rank's device.  Returns (scores [B], idx [B]) complete on every rank.
+
+        On a CUDA device the call is asynchronous: all of its work, the upload of the batch positions included, is queued on
+        the current stream, and it returns without waiting for the device."""
+        dev = crops_dev.device
+        plan = self.plan(class_ids)
         parts = []
-        for cls, sel in self.plan(class_ids):
-            pos = torch.from_numpy(sel).to(crops_dev.device)
-            s, i = self._run_class(cls, crops_dev.index_select(0, pos).contiguous())
-            parts.append((pos, s, i))
-        return self._exchange(len(class_ids), parts, crops_dev.device)
+        if plan:
+            order = torch.from_numpy(np.concatenate([sel for _, sel in plan]))
+            # from pinned memory the copy does not make the host wait; torch keeps the pinned block until the copy has run
+            pos_all = order.to(dev) if dev.type == "cpu" else order.pin_memory().to(dev, non_blocking=True)
+            a = 0
+            for cls, sel in plan:
+                pos = pos_all[a:a + len(sel)]
+                s, i = self._run_class(cls, crops_dev.index_select(0, pos).contiguous())
+                parts.append((pos, s, i))
+                a += len(sel)
+        return self._exchange(len(class_ids), parts, dev)
 
     def route_host(self, crops_host, class_ids, device):
         """crops_host: the mixed batch in HOST memory (numpy array or torch CPU tensor [B,H,W,C], uint8 or float32; ideally pinned).  This rank gathers the
         crops of its own classes into a pinned staging buffer and uploads only those (1/world of the batch on average) --
-        not the whole batch on every rank.  Same return value as ``route``."""
+        not the whole batch on every rank.  Same return value as ``route``.
+
+        On a CUDA device the call is asynchronous, like ``route``.  The staged crops and their positions are uploaded on a
+        copy stream the router owns, and the current stream waits for that upload before it encodes them.  The next call
+        refills the same staging buffer, so it first waits until this upload has executed: one host-to-device copy, which
+        does not queue behind the compute stream.  Calls may therefore be pipelined, and each one returns the results of
+        its own batch.  The caller may reuse `crops_host` as soon as the call returns."""
         plan = self.plan(class_ids)
         n_own = sum(len(sel) for _, sel in plan)
         parts = []
         if n_own:
             src = crops_host.numpy() if isinstance(crops_host, torch.Tensor) else np.ascontiguousarray(crops_host)
+            if self._uploaded is not None:
+                self._uploaded.synchronize()         # the last upload has read the stage
+                self._uploaded = None
             if self._stage is None or self._stage.shape[0] < n_own or tuple(self._stage.shape[1:]) != tuple(src.shape[1:]) or \
                     self._stage.numpy().dtype != src.dtype:
                 cap = max(n_own, -(-len(class_ids) // max(1, self.world)) * 2)
@@ -274,11 +296,30 @@ class ObjectRouter:
             dst = self._stage.numpy()
             for j, i in enumerate(order_np):
                 dst[j] = src[i]
-            own_dev = self._stage[:n_own].to(device, non_blocking=True)
-            pos_dev = order.to(device, non_blocking=True)
+            if device.type == "cpu":
+                own_dev, pos_dev = self._stage[:n_own].to(device), order.to(device)
+            else:
+                own_dev, pos_dev = self._upload(self._stage[:n_own], order, device)
             a = 0
             for cls, sel in plan:
                 s, i = self._run_class(cls, own_dev[a:a + len(sel)])
                 parts.append((pos_dev[a:a + len(sel)], s, i))
                 a += len(sel)
         return self._exchange(len(class_ids), parts, device)
+
+    def _upload(self, crops, order, device):
+        """Pinned crops and host positions -> device copies that the current stream may use.  The copies run on the router's
+        copy stream, and ``self._uploaded`` is recorded behind them."""
+        compute = torch.cuda.current_stream(device)
+        copy = self._copy.get(compute.device_index)
+        if copy is None:
+            copy = self._copy[compute.device_index] = torch.cuda.Stream(device=compute.device)
+        with torch.cuda.stream(copy):
+            own = crops.to(compute.device, non_blocking=True)
+            pos = order.pin_memory().to(compute.device, non_blocking=True)
+            self._uploaded = torch.cuda.Event()
+            self._uploaded.record(copy)
+        compute.wait_event(self._uploaded)
+        own.record_stream(compute)                   # allocated on the copy stream, used and freed on the current one
+        pos.record_stream(compute)
+        return own, pos

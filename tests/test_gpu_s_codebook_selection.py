@@ -8,6 +8,8 @@ within the precision's bar of its row's float64 cosine; a position may differ fr
 float64 cosines are closer than the precision resolves; rows with identical content come out lowest index first and in
 ascending order; positions past the eligible rows are exactly (-inf, -1)."""
 import configparser
+import contextlib
+import gc
 
 import numpy as np
 import pytest
@@ -23,6 +25,7 @@ BAR = {0: 2e-6, 1: 2e-6, 2: 2.0 ** -9}     # |returned score - float64 cosine of
 RES = {0: 2e-7, 1: 2e-7, 2: 2.0 ** -8}     # float64 gap below which two rows may trade places
 MAX_BATCH = 300                              # three launches of the fused kernel (128 queries each), the last one ragged
 KS = (1, 2, 7, 8, 9, 16, 64)                 # the fused kernel takes k <= 8, the cosine-matrix route the rest
+FINE_ROWS, FINE_CYCLO = 368928, 144          # bench.py's fine codebook (configs[4]): an upright row every 144 rows
 
 
 class Book:
@@ -54,12 +57,14 @@ class Book:
             self._cos[zkey] = zq @ self.E64.T
         cos = self._cos[zkey]
         elig = self.elig(upright)
-        order = torch.sort(torch.where(elig, -cos, torch.full_like(cos, float("inf"))), dim=1, stable=True).indices
+        # 32 queries at a time: the sort's temporaries stay small beside the cosines of a large table
+        order = torch.cat([torch.sort(torch.where(elig, -c, torch.full_like(c, float("inf"))), dim=1, stable=True).indices[:, :depth]
+                           for c in cos.split(32)])
         rank, seen = np.full(self.n, -1), {}
         for r in np.nonzero(elig.cpu().numpy())[0]:
             rank[r] = seen.get(self.cls[r], 0)
             seen[self.cls[r]] = rank[r] + 1
-        self._refs[key] = dict(cos=cos, order=order[:, :depth].contiguous(), elig=elig, n_elig=int(elig.sum()),
+        self._refs[key] = dict(cos=cos, order=order, elig=elig, n_elig=int(elig.sum()),
                                rank=torch.from_numpy(rank).cuda(), cls=torch.from_numpy(self.cls).cuda())
         return self._refs[key]
 
@@ -120,53 +125,95 @@ def lab(sess):
                 book.cbs[prec] = _codebook(self.enc, book.E, num_cyclo=book.num_cyclo, max_batch=MAX_BATCH, precision=prec)
             return book.cbs[prec]
 
+        def drop(self, key):
+            """Close a table's handles and forget its references."""
+            for cb in self.books.pop(key).cbs.values():
+                cb.close()
+
     lab = Lab()
     yield lab
-    for b in lab.books.values():
-        for cb in b.cbs.values():
-            cb.close()
+    for key in list(lab.books):
+        lab.drop(key)
+    _release()
+
+
+def _release():
+    gc.collect()
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()
+
+
+@pytest.fixture(autouse=True)
+def _give_back_cached_memory():
+    """Before and after each test, the memory torch holds cached but unused goes back to the device: the codebook handles
+    allocate outside torch's cache, and the fine codebook's references take several GB."""
+    _release()
+    yield
+    _release()
+
+
+@contextlib.contextmanager
+def _fine_book(lab):
+    """The fine codebook for one test.  With its float64 references and handles it takes several GB, more than the module
+    keeps for all its other tables, so it is dropped when the test ends."""
+    try:
+        yield lab.book("fine", lambda: O.make_codebook(11, n=FINE_ROWS, num_cyclo=FINE_CYCLO), FINE_CYCLO)
+    finally:
+        lab.drop("fine")
 
 
 def _random_book(lab, n):
     return lab.book(("random", n), lambda: O.make_codebook(7, n=n))
 
 
-def _queries(E, seed=99):
+def _table(lab, n):
+    """the table of n rows for a with block: the fine codebook, or a random one kept for the module"""
+    return _fine_book(lab) if n == FINE_ROWS else contextlib.nullcontext(_random_book(lab, n))
+
+
+def _queries(E, num_cyclo=36, seed=99):
     rng = np.random.RandomState(seed)
     z = (rng.standard_normal((MAX_BATCH, 128)) * rng.uniform(0.1, 30, (MAX_BATCH, 1))).astype(np.float32)
     n = E.shape[0]
-    z[:8] = E[(np.arange(8) * 36 + 35) % n] * 1.7      # a cyclo end-point row (a copy of row v*36 when n % 36 == 0) on top
+    # a cyclo end-point row (a copy of row v*num_cyclo when n % num_cyclo == 0) on top
+    z[:8] = E[(np.arange(8) * num_cyclo + num_cyclo - 1) % n] * 1.7
     z[8] = 0                                             # every cosine 0
     return z
 
 
+def _print_peak(what):
+    print("%s: peak torch device memory %.2f GB" % (what, torch.cuda.max_memory_allocated() / 2 ** 30))
+
+
 # --------------------------------------------------------------------------------------- k on both sides of the fused limit
-@pytest.mark.parametrize("n_rows", [337, 36 * 40, O.N_CODEBOOK])
+@pytest.mark.parametrize("n_rows", [337, 36 * 40, O.N_CODEBOOK, FINE_ROWS])
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_topk_on_both_sides_of_the_fused_kernel_limit(lab, precision, n_rows):
-    book = _random_book(lab, n_rows)
-    cb = lab.cb(book, precision)
-    z = _queries(book.E)
-    zd = torch.from_numpy(z).cuda()
-    ks = KS + ((n_rows,) if n_rows < 1000 else ())
-    for upright in (False, True):
-        ref = book.ref(z, upright, max(ks))
-        for B in (1, 129, MAX_BATCH):
-            got = {}
-            for k in ks:
-                what = "prec %d n %d upright %d B %d k %d" % (precision, n_rows, upright, B, k)
-                s, i = cb.match_device(zd[:B], k=k, upright=upright)
-                s2, i2 = cb.match_device(zd[:B], k=k, upright=upright)
-                assert torch.equal(s, s2) and torch.equal(i, i2), (what, "two calls differ")
-                _check(s, i, ref, k, precision, what)
-                got[k] = i
-            for k in (9, 16):
-                _same_rows(got[k][:, :8], got[8], ref, precision, "prefix of k=%d vs k=8, prec %d n %d B %d" % (k, precision, n_rows, B))
-            if B > 8:                                    # the zero latent: every cosine 0, so the lowest eligible rows in order
+    torch.cuda.reset_peak_memory_stats()
+    with _table(lab, n_rows) as book:
+        cb = lab.cb(book, precision)
+        z = _queries(book.E, book.num_cyclo)
+        zd = torch.from_numpy(z).cuda()
+        ks = KS + ((n_rows,) if n_rows < 1000 else ())
+        for upright in (False, True):
+            ref = book.ref(z, upright, max(ks))
+            for B in (1, 129, MAX_BATCH):
+                got = {}
                 for k in ks:
-                    want = torch.nonzero(ref["elig"])[:k, 0]
-                    _, i = cb.match_device(zd[8:9], k=k, upright=upright)
-                    assert torch.equal(i[0, :len(want)].long(), want), ("zero latent", precision, n_rows, upright, k)
+                    what = "prec %d n %d upright %d B %d k %d" % (precision, n_rows, upright, B, k)
+                    s, i = cb.match_device(zd[:B], k=k, upright=upright)
+                    s2, i2 = cb.match_device(zd[:B], k=k, upright=upright)
+                    assert torch.equal(s, s2) and torch.equal(i, i2), (what, "two calls differ")
+                    _check(s, i, ref, k, precision, what)
+                    got[k] = i
+                for k in (9, 16):
+                    _same_rows(got[k][:, :8], got[8], ref, precision, "prefix of k=%d vs k=8, prec %d n %d B %d" % (k, precision, n_rows, B))
+                if B > 8:                                    # the zero latent: every cosine 0, so the lowest eligible rows in order
+                    for k in ks:
+                        want = torch.nonzero(ref["elig"])[:k, 0]
+                        _, i = cb.match_device(zd[8:9], k=k, upright=upright)
+                        assert torch.equal(i[0, :len(want)].long(), want), ("zero latent", precision, n_rows, upright, k)
+    _print_peak("prec %d n %d" % (precision, n_rows))
 
 
 # --------------------------------------------------------------------------------------- tie patterns
@@ -235,23 +282,26 @@ def test_codebook_of_equal_rows_answers_the_lowest_indices(lab, precision):
 # --------------------------------------------------------------------------------------- upright layouts
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_upright_layouts(lab, precision):
-    """num_cyclo 1 (every row upright), 36, 72 and 100 (whole 64-row fp32 tiles without an upright row), tables that are not a
-    multiple of num_cyclo, and k above the number of upright rows."""
+    """num_cyclo 1 (every row upright), 36, 72 and 100 (whole 64-row fp32 tiles without an upright row), 144 on the fine
+    codebook (upright rows further apart than the fused kernel's 128-row tile), tables that are not a multiple of num_cyclo,
+    and k above the number of upright rows."""
+    torch.cuda.reset_peak_memory_stats()
     rng = np.random.RandomState(17)
     z = (rng.standard_normal((64, 128)) * rng.uniform(0.1, 30, (64, 1))).astype(np.float32)
     zd = torch.from_numpy(z).cuda()
-    cases = [(337, nc) for nc in (1, 36, 72, 100)] + [(O.N_CODEBOOK, nc) for nc in (72, 100)]
+    cases = [(337, nc) for nc in (1, 36, 72, 100)] + [(O.N_CODEBOOK, nc) for nc in (72, 100)] + [(FINE_ROWS, FINE_CYCLO)]
     for n, nc in cases:
-        base = _random_book(lab, n)
-        book = lab.book(("cyclo", n, nc), lambda: base.E, nc)
-        cb = lab.cb(book, precision)
-        n_up = -(-n // nc)
-        ks = (1, 2, 7, 8, 9, 16) + ((min(n_up + 3, n),) if n < 1000 else ())
-        ref = book.ref(z, True, max(ks))
-        assert ref["n_elig"] == n_up
-        for k in ks:
-            s, i = cb.match_device(zd, k=k, upright=True)
-            _check(s, i, ref, k, precision, "prec %d n %d num_cyclo %d k %d" % (precision, n, nc, k))
+        with _table(lab, n) as base:
+            book = base if base.num_cyclo == nc else lab.book(("cyclo", n, nc), lambda: base.E, nc)
+            cb = lab.cb(book, precision)
+            n_up = -(-n // nc)
+            ks = (1, 2, 7, 8, 9, 16) + ((min(n_up + 3, n),) if n < 1000 else ())
+            ref = book.ref(z, True, max(ks))
+            assert ref["n_elig"] == n_up
+            for k in ks:
+                s, i = cb.match_device(zd, k=k, upright=True)
+                _check(s, i, ref, k, precision, "prec %d n %d num_cyclo %d k %d" % (precision, n, nc, k))
+    _print_peak("upright layouts, prec %d" % precision)
 
 
 # --------------------------------------------------------------------------------------- shards
