@@ -824,6 +824,12 @@ extern "C" int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decode
   for (int i = 0; i < L; ++i)
     if (st[i] != 2) { set_error("decoder: only stride-2 (x2 nearest-neighbour) stages are supported"); status = AAE_ERR_UNSUPPORTED; }
   if (cfg->in_h != cfg->in_w) { set_error("decoder: square crops only"); status = AAE_ERR_UNSUPPORTED; }
+  // every stage doubles its map, so the output is dims[0] << L: the reference's fractional resizes at other sizes are not built
+  if (status == AAE_OK && cfg->in_h != dims[0] << L) {
+    set_error("decoder: H = %d is not a multiple of 2^L = %d (the x2 stages would build a %d x %d image)", cfg->in_h, 1 << L,
+              dims[0] << L, dims[0] << L);
+    status = AAE_ERR_UNSUPPORTED;
+  }
   if (status == AAE_OK) {
     h->h0 = h->w0 = dims[0]; h->f0 = nf[0];
     const size_t dense_out = (size_t)h->h0 * h->w0 * h->f0;
@@ -1096,6 +1102,12 @@ static int trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_rati
                           aae_trainer** out) {
   AAE_REQUIRE((enc->tc == nullptr) == (dec->tc == nullptr), "encoder and decoder must use the same aae_precision for training");
   AAE_REQUIRE(enc->cfg.max_batch == dec->cfg.max_batch && enc->cfg.in_h == dec->cfg.in_h, "encoder/decoder geometry mismatch");
+  const long long numel = (long long)enc->cfg.in_h * enc->cfg.in_w * enc->cfg.in_c;
+  if (numel > AAE_BOOTSTRAP_MAX_NUMEL) {
+    set_error("trainer: a %d x %d x %d crop is %lld values; the bootstrapped L2 loss holds at most AAE_BOOTSTRAP_MAX_NUMEL = %d per "
+              "sample", enc->cfg.in_h, enc->cfg.in_w, enc->cfg.in_c, numel, AAE_BOOTSTRAP_MAX_NUMEL);
+    return AAE_ERR_UNSUPPORTED;
+  }
   DeviceGuard g(enc->device);
   aae_trainer* h = new (std::nothrow) aae_trainer();
   AAE_REQUIRE(h != nullptr, "host allocation failed");

@@ -167,8 +167,9 @@ int launch_mask_loss(const float* xmask, const float* y, int B, int pixels, int 
 
 int launch_bootstrap_l2(const float* x, const float* y, int B, int numel, int k, float* sample_sums, float* loss_out,
                         float* grad_out, cudaStream_t stream) {
+  AAE_REQUIRE(numel <= AAE_BOOTSTRAP_MAX_NUMEL, "bootstrap_l2: numel=%d per sample exceeds the shared-memory row buffer (%d floats)",
+              numel, AAE_BOOTSTRAP_MAX_NUMEL);
   const size_t smem = (size_t)numel * sizeof(unsigned);
-  AAE_REQUIRE(smem <= 200 * 1024, "bootstrap_l2: numel=%d per sample exceeds the shared-memory row buffer (51200 floats)", numel);
   AAE_REQUIRE(k >= 1 && k <= numel, "bootstrap_l2: k=%d out of range", k);
   AAE_CUDA_OK(cudaFuncSetAttribute(bootstrap_l2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const float inv_bk = 1.0f / ((float)B * (float)k);

@@ -480,7 +480,11 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
       T.in_h = ih; T.in_w = iw; T.in_c = ic;
       T.out_h = ih / 2; T.out_w = iw / 2; T.out_c = cfg->filters[l];
       T.taps = 25;
-      if (!pow2(T.out_w) || !pow2(T.out_h) || T.out_w > 128) { set_error("AAE_PREC_TC_SPLIT: output dims must be powers of two <= 128"); st = AAE_ERR_UNSUPPORTED; break; }
+      if (!pow2(T.out_w) || !pow2(T.out_h) || T.out_w > 128) {
+        set_error("AAE_PREC_TC_SPLIT: layer %d output %d x %d unsupported (needs powers of two <= 128)", l, T.out_h, T.out_w);
+        st = AAE_ERR_UNSUPPORTED;
+        break;
+      }
       T.BW = T.out_w;
       T.BH = std::min(T.out_h, 128 / T.BW);
       T.BB = 128 / (T.BW * T.BH);

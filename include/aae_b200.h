@@ -214,7 +214,10 @@ AAE_API int aae_codebook_profile(aae_codebook* h, int enable, float* stage_ms_ou
 
 /* ---------------------------------------------------------------- Decoder + loss -----------
  * Replaces Decoder.x: dense latent->8*8*512 + ReLU, 3x [NN-resize x2, conv5x5 s1 + ReLU],
- * NN-resize x2, conv5x5 -> C + sigmoid (auto_pose/ae/decoder.py:36-84). */
+ * NN-resize x2, conv5x5 -> C + sigmoid (auto_pose/ae/decoder.py:36-84).
+ * Every stage doubles the map exactly, so the first map is h0 = H / 2^L and H must equal h0 * 2^L: a crop size that is not a
+ * multiple of 2^L (the reference resizes by fractional factors there, 6 -> 12 -> 25 -> 50 -> 100 at H = 100) is refused with
+ * AAE_ERR_UNSUPPORTED on every precision, naming H and 2^L.  So are H != W and any stride other than 2. */
 AAE_API int aae_decoder_create(int device, const aae_net_cfg* cfg, aae_decoder** out);
 AAE_API int aae_decoder_destroy(aae_decoder* h);
 /* layer 0 = dense_1 [latent, h0*w0*f0]; layers 1..num_layers = the convs in forward order; num_layers + 1 = the mask head
@@ -244,7 +247,11 @@ AAE_API int aae_mask_loss(const float* mask_dev, const float* target_dev, int ba
                           float* loss_inout_dev, float* grad_out_dev, void* stream);
 /* Bootstrapped L2 (LOSS: L2, BOOTSTRAP_RATIO r): per-sample top-k of the flattened squared error,
  * k = numel/r, mean over the [B,k] survivors (auto_pose/ae/decoder.py:90-101).
- * grad_out_dev (optional, [B,numel]) receives dLoss/dx. */
+ * grad_out_dev (optional, [B,numel]) receives dLoss/dx.  One CTA holds one sample's squared errors in shared memory, so
+ * numel_per_sample is at most AAE_BOOTSTRAP_MAX_NUMEL (H * W * C = 51 200, e.g. 128 x 128 x 3 = 49 152 fits and
+ * 144 x 144 x 3 does not); a larger sample returns AAE_ERR_INVALID_ARG, and aae_trainer_create* refuses a geometry above
+ * it with AAE_ERR_UNSUPPORTED. */
+#define AAE_BOOTSTRAP_MAX_NUMEL 51200
 AAE_API int aae_bootstrap_l2_loss(const float* x_dev, const float* target_dev, int batch, int numel_per_sample,
                                   int bootstrap_ratio, float* loss_out_dev, float* grad_out_dev, void* stream);
 
@@ -369,7 +376,9 @@ AAE_API int aae_occlusion(const aae_occlusion_args* a, void* stream);
  * runs the forward pass, the data gradients and the weight gradients of all convs with Cin >= 128
  * as wgmma GEMMs (split-fp16 x3, gradients re-scaled per tensor and per step by a power of two),
  * the two dense layers and conv1's weight gradient as fp32 kernels; parameters, optimizer slots and
- * the gradients returned by aae_trainer_get_grads are fp32 in the reference layouts either way. */
+ * the gradients returned by aae_trainer_get_grads are fp32 in the reference layouts either way.
+ * The step's loss is aae_bootstrap_l2_loss over one crop per CTA: a crop of more than AAE_BOOTSTRAP_MAX_NUMEL values
+ * (H * W * C) is refused here with AAE_ERR_UNSUPPORTED, naming the limit, on every aae_trainer_create* entry point. */
 AAE_API int aae_trainer_create(aae_encoder* enc, aae_decoder* dec, int bootstrap_ratio, float learning_rate,
                                float beta1, float beta2, float epsilon, aae_trainer** out);
 /* The same trainer with the GEMM arithmetic chosen apart from the handles' precision.

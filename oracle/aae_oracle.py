@@ -70,7 +70,8 @@ def make_encoder_params(seed: int = 42, num_filters=NUM_FILTER, ksize=KSIZE, lat
                         in_w: Optional[int] = None) -> Dict[str, np.ndarray]:
     """Variable names / layouts of auto_pose/ae/encoder.py:43-66 (conv kernels HWIO, dense [in,out]).
     TF zero-initialises biases; ``bias_scale`` > 0 draws small random biases so that parity tests
-    actually exercise the bias path.  ``in_w``: crop width when it differs from the height ``in_hw``."""
+    actually exercise the bias path.  ``in_w``: crop width when it differs from the height ``in_hw``.  Each conv's output is
+    ceil(in / stride) per axis, as TF's SAME padding makes it (127 -> 64 -> 32 -> 16 -> 8)."""
     rng = np.random.RandomState(seed)
     p: Dict[str, np.ndarray] = {}
     cin, hh, ww = in_ch, in_hw, in_hw if in_w is None else in_w
@@ -78,7 +79,7 @@ def make_encoder_params(seed: int = 42, num_filters=NUM_FILTER, ksize=KSIZE, lat
         name = "conv2d" if i == 0 else f"conv2d_{i}"
         p[f"{name}/kernel"] = glorot_uniform(rng, (ksize, ksize, cin, f))
         p[f"{name}/bias"] = (bias_scale * rng.standard_normal(f)).astype(np.float32)
-        cin, hh, ww = f, hh // s, ww // s
+        cin, hh, ww = f, -(-hh // s), -(-ww // s)
     p["dense/kernel"] = glorot_uniform(rng, (hh * ww * cin, latent))
     p["dense/bias"] = (bias_scale * rng.standard_normal(latent)).astype(np.float32)
     return p
@@ -113,14 +114,15 @@ def make_crops_u8(seed: int, batch: int, hw: int = H, ch: int = C, structured: b
     """Synthetic BGR crops, NHWC uint8 (auto_pose/ae/ae_factory.py:133 placeholder shape).  structured=True draws a
     different coarse random pattern per crop (8x8 blocks + pixel noise) so that the latents -- and therefore the
     matched codebook rows -- differ from crop to crop; structured=False is i.i.d. U{0..255} (every crop then encodes
-    to almost the same latent).  ``w``: crop width when it differs from the height ``hw``."""
+    to almost the same latent).  ``w``: crop width when it differs from the height ``hw``.  A size that the cell count does
+    not divide takes ceil(size / cells) pixels per cell, the last cell cut short."""
     rng = np.random.RandomState(seed)
     w = hw if w is None else w
     if not structured:
         return rng.randint(0, 256, size=(batch, hw, w, ch), dtype=np.uint8)
     cells, cells_w = max(hw // 16, 1), max(w // 16, 1)
     coarse = rng.randint(0, 256, size=(batch, cells, cells_w, ch)).astype(np.int32)
-    img = np.repeat(np.repeat(coarse, hw // cells, axis=1), w // cells_w, axis=2)
+    img = np.repeat(np.repeat(coarse, -(-hw // cells), axis=1), -(-w // cells_w), axis=2)[:, :hw, :w]
     img = img + rng.randint(-40, 41, size=(batch, hw, w, ch))
     return np.clip(img, 0, 255).astype(np.uint8)
 

@@ -28,6 +28,14 @@ ROWS = {
     "rect": dict(h=64),
     "refused_stride": dict(strides=(2, 2, 1, 2)),
     "refused_k3": dict(k=3),
+    # crop sizes that are not powers of two: odd maps, TF's symmetric (2, 2) SAME padding of odd inputs, images that straddle
+    # 128-row tiles
+    "px112": dict(h=112, w=112),                          # maps 56/28/14/7
+    "px80": dict(h=80, w=80),                             # 40/20/10/5
+    "px96": dict(h=96, w=96),                             # 48/24/12/6
+    "px127": dict(h=127, w=127),                          # 64/32/16/8, conv1 padded (2, 2)
+    "h127": dict(h=127),                                  # 127 x 128: conv1 padded (2, 2) in height, (1, 2) in width
+    "px100": dict(h=100, w=100),                          # 50/25/13/7, pads (1, 2), (1, 2), (2, 2), (2, 2)
 }
 
 # Where each module settles with the automatic precision: (encoder, codebook match, decoder, encoder and decoder once the
@@ -49,7 +57,19 @@ LANDING = {
     "rect": (SPLIT, SPLIT, None, None, True),             # the decoder takes square crops only
     "refused_stride": (FP32, FP32, None, None, False),    # the decoder takes stride-2 stages only
     "refused_k3": (FP32, FP32, FP32, FP32, False),
+    "px112": (FP32, FP32, FP32, FP32, False),             # the tensor cores take power-of-two maps only
+    "px80": (FP32, FP32, FP32, FP32, False),
+    "px96": (FP32, FP32, FP32, FP32, False),
+    "px127": (SPLIT, SPLIT, None, None, False),           # fp32 conv1; the decoder's x2 stages cannot build 127 from 8
+    "h127": (SPLIT, SPLIT, None, None, False),            # fp32 conv1 (odd height); the decoder takes square crops only
+    "px100": (FP32, FP32, None, None, False),             # 100 is not a multiple of 2^4
 }
+
+# rows whose training check also runs at this batch: the fp32 trainer orders a stride-2 dgrad parity-major only when
+# (B * PH * PW / 4) % 128 == 0, which at B = 32 holds for 56 x 56, 28 x 28, 40 x 40, 20 x 20 and every px96 map but not for
+# 14 x 14 or 10 x 10, so one step takes both orderings
+PARITY_BATCH = 32
+PARITY_ROWS = ("px112", "px80", "px96")
 
 
 def row(rid, **change):
@@ -62,7 +82,7 @@ def row(rid, **change):
 
 
 def tc_conv1(r):
-    return r["w"] == 128 and r["c"] == 3 and r["nf"][0] == 128 and r["k"] == 5 and r["strides"][0] == 2
+    return r["w"] == 128 and r["h"] % 2 == 0 and r["c"] == 3 and r["nf"][0] == 128 and r["k"] == 5 and r["strides"][0] == 2
 
 
 def params(r, bias_scale=0.05):

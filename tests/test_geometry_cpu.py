@@ -7,7 +7,7 @@ import torch
 
 from oracle import aae_oracle as O
 from oracle import mask_oracle as MO
-from tests.geometry_table import ROWS, dec_weights, decoder, encoder, params, row
+from tests.geometry_table import ROWS, T, dec_weights, decoder, encoder, params, row
 
 
 def _shapes(mod):
@@ -35,6 +35,106 @@ def test_oracle_defaults_are_unchanged():
     assert a.keys() == b.keys() and all(np.array_equal(a[k], b[k]) for k in a)
     assert np.array_equal(O.make_crops_u8(3, 2), O.make_crops_u8(3, 2, w=O.W))
     assert O.make_crops_u8(3, 2, hw=16, w=32).shape == (2, 16, 32, 3)
+
+
+# the rows that were in the table before crop sizes other than powers of two
+POW2_ROWS = [rid for rid in ROWS if rid not in ("px112", "px80", "px96", "px127", "h127", "px100")]
+
+
+@pytest.mark.parametrize("rid", ["template"] + POW2_ROWS)
+def test_encoder_params_at_power_of_two_sizes_are_unchanged(rid):
+    """make_encoder_params takes TF SAME's ceil(in / stride) per map; at the template and every power-of-two row that equals the
+    floor it took before, so the dense kernel keeps its shape and every draw its value"""
+    r = dict(T, L=len(T["nf"]), id=rid) if rid == "template" else row(rid)
+    h, w = r["h"], r["w"]
+    for s in r["strides"]:
+        assert -(-h // s) == h // s and -(-w // s) == w // s, (rid, h, w, s)
+        h, w = h // s, w // s
+    ep, _, _ = params(r)
+    assert ep["dense/kernel"].shape == (h * w * r["nf"][-1], r["latent"])
+
+
+@pytest.mark.parametrize("rid,maps", [("px112", (56, 28, 14, 7)), ("px80", (40, 20, 10, 5)), ("px96", (48, 24, 12, 6)),
+                                      ("px127", (64, 32, 16, 8)), ("h127", (64, 32, 16, 8)), ("px100", (50, 25, 13, 7))])
+def test_encoder_params_take_the_ceiling_of_each_map(rid, maps):
+    """the dense kernel of the rows whose maps SAME padding rounds up: ceil(in / 2) per conv, 8 x 8 at 127 (the floor gave 7 x 7);
+    the oracle's forward on a crop of the row's size produces those maps and feeds that kernel (127 x 128 has the same maps in
+    both directions)"""
+    r = row(rid)
+    ep, _, _ = params(r)
+    assert ep["dense/kernel"].shape == (maps[-1] * maps[-1] * r["nf"][-1], r["latent"])
+    x = O.preprocess(O.make_crops_u8(5, 1, hw=r["h"], ch=r["c"], w=r["w"]))
+    outs = O.encoder_layers(x, ep, strides=r["strides"], dtype=torch.float64)
+    assert [tuple(o.shape[1:3]) for o in outs[:r["L"]]] == [(m, m) for m in maps], rid
+    assert outs[-1].shape == (1, r["latent"])
+
+
+def _old_crops_u8(seed, batch, hw, ch, w):
+    """make_crops_u8 as it was while every crop size was a multiple of its cell count"""
+    rng = np.random.RandomState(seed)
+    cells, cells_w = max(hw // 16, 1), max(w // 16, 1)
+    coarse = rng.randint(0, 256, size=(batch, cells, cells_w, ch)).astype(np.int32)
+    img = np.repeat(np.repeat(coarse, hw // cells, axis=1), w // cells_w, axis=2)
+    img = img + rng.randint(-40, 41, size=(batch, hw, w, ch))
+    return np.clip(img, 0, 255).astype(np.uint8)
+
+
+@pytest.mark.parametrize("hw,w,ch", [(128, 128, 3), (128, 128, 1), (64, 64, 3), (64, 128, 3), (32, 32, 3), (16, 32, 3),
+                                     (16, 16, 3), (16, 16, 1)])
+def test_crops_at_sizes_in_use_are_unchanged(hw, w, ch):
+    """make_crops_u8 draws the same bytes as before at every size the suite used before odd sizes"""
+    assert np.array_equal(O.make_crops_u8(9, 3, hw=hw, ch=ch, w=w), _old_crops_u8(9, 3, hw, ch, w))
+
+
+@pytest.mark.parametrize("hw,w", [(100, 100), (127, 127), (127, 128), (80, 80), (112, 112), (96, 96), (25, 25)])
+def test_crops_at_any_size(hw, w):
+    """at a size its cell count does not divide, each cell is ceil(size / cells) pixels and the last one is cut short: the coarse
+    pattern is constant over each cell up to the +-40 noise"""
+    x = O.make_crops_u8(9, 2, hw=hw, w=w)
+    assert x.shape == (2, hw, w, 3) and x.dtype == np.uint8
+    cells, cells_w = max(hw // 16, 1), max(w // 16, 1)
+    ph, pw = -(-hw // cells), -(-w // cells_w)
+    coarse = np.random.RandomState(9).randint(0, 256, size=(2, cells, cells_w, 3))
+    want = np.repeat(np.repeat(coarse, ph, axis=1), pw, axis=2)[:, :hw, :w]
+    d = x.astype(int) - want
+    assert np.all((d >= -40) & (d <= 40) | (x == 0) | (x == 255))
+
+
+# TF SAME padding of a k = 5, stride-2 conv, derived by hand from out = ceil(in / 2), total = max((out - 1) * 2 + 5 - in, 0),
+# before = total // 2, after = total - before
+SAME_K5_S2 = {128: (1, 2), 127: (2, 2), 112: (1, 2), 100: (1, 2), 25: (2, 2), 14: (1, 2), 13: (2, 2), 7: (2, 2)}
+
+
+@pytest.mark.parametrize("size", list(SAME_K5_S2))
+def test_same_padding_known_answers(size):
+    """_same_pads, conv2d_same and conv2d_same_loops against the literal table.  The input's pixels are 1 + their flat index and
+    output channel 5 dy + dx of the kernel is the one-hot tap (dy, dx), so each output is one known input pixel or 0; the height
+    takes the row's size and the width another row's, so that a swapped pad_t / pad_l shows."""
+    sizes = list(SAME_K5_S2)
+    ih, iw = size, sizes[(sizes.index(size) + 1) % len(sizes)]
+    (pt, pb), (pl, pr) = SAME_K5_S2[ih], SAME_K5_S2[iw]
+    assert O._same_pads(ih, 5, 2) == (pt, pb) and O._same_pads(iw, 5, 2) == (pl, pr)
+    oh, ow = (ih + pt + pb - 5) // 2 + 1, (iw + pl + pr - 5) // 2 + 1
+    assert (oh, ow) == (-(-ih // 2), -(-iw // 2))
+    x = (1.0 + np.arange(ih * iw, dtype=np.float64)).reshape(1, ih, iw, 1)
+    k = np.zeros((5, 5, 1, 25))
+    for t in range(25):
+        k[t // 5, t % 5, 0, t] = 1.0
+    want = np.zeros((1, oh, ow, 25))
+    for t in range(25):
+        dy, dx = divmod(t, 5)
+        for r in range(oh):
+            iy = 2 * r + dy - pt
+            for c in range(ow):
+                ix = 2 * c + dx - pl
+                if 0 <= iy < ih and 0 <= ix < iw:
+                    want[0, r, c, t] = x[0, iy, ix, 0]
+    # the bottom / right pad is what the last output row / column reads past the image
+    assert np.all(want[0, -1, :, 5 * (5 - pb):] == 0) and np.any(want[0, -1, :, :5 * (5 - pb)] != 0)
+    assert np.all(want[0, :, -1, [5 * dy + dx for dy in range(5) for dx in range(5 - pr, 5)]] == 0)
+    got = O.conv2d_same(torch.from_numpy(x), torch.from_numpy(k), torch.zeros(25, dtype=torch.float64), 2, None).numpy()
+    assert np.array_equal(got, want), size
+    assert np.array_equal(O.conv2d_same_loops(x, k, np.zeros(25), 2), want), size
 
 
 def _loop_encoder(x, p, strides):
@@ -65,6 +165,9 @@ SMALL = {
     "gray": (16, 16, 1, (4, 8), (2, 2), 5),
     "k3": (16, 16, 3, (4, 8), (2, 2), 3),
     "stride1": (16, 16, 3, (4, 4, 8), (2, 1, 2), 5),
+    # odd sizes: TF's symmetric (2, 2) padding of odd inputs, and (1, 2) / (2, 2) on the two axes of one conv
+    "13x16": (13, 16, 3, (4, 8), (2, 2), 5),
+    "15x15": (15, 15, 3, (4, 8, 8), (2, 2, 2), 5),
 }
 
 

@@ -13,7 +13,13 @@ Branches only these rows reach: the fp32 conv1 writing conv2's (hi, lo) space-to
 with a 4-pixel-wide output and their per-tap boxes (five_layer, px64, and the decoder's first layers there), N tiles narrower
 than 128 on a conv (cout64) and on the dense layer (latent32/64/96), a zero-filled last N tile (wide_last, Cout 480), other dense
 flat sizes and split counts, the tensor-core conv1 at 64 rows with BB = 4 (rect), the decoder at h0 = 4 and 32, a 1-channel
-output conv and the mask head on every decoder, the fp32 match at latent 32/64/256, and every automatic fallback."""
+output conv and the mask head on every decoder, the fp32 match at latent 32/64/256, and every automatic fallback.
+
+Crop sizes that are not powers of two (px112, px80, px96, px127, h127, px100) reach odd maps (7 x 7, 5 x 5, 25 x 25), TF's
+symmetric (2, 2) SAME padding of odd inputs, images that straddle 128-row tiles, and the fp32 kernels the tensor cores leave
+them: the generic conv1 weight gradient, stride-2 dgrad on odd maps in both orderings (PARITY_BATCH), decoders whose first map
+is 5, 6 or 7 pixels wide, and the fp32 conv1 with pad (2, 2) (pad_t = 2 and pad_l = 1 at 127 x 128) writing the split
+encoder's conv2 input.  The decoder refuses a crop that is not a multiple of 2^L."""
 import gc
 
 import numpy as np
@@ -22,8 +28,8 @@ import torch
 
 from oracle import aae_oracle as O
 from oracle import mask_oracle as MO
-from tests.geometry_table import (FP16, FP32, LANDING, MAXB, RAGGED, ROWS, SPLIT, dec_weights, decoder, encoder, output_conv, params,
-                                  row, tc_conv1)
+from tests.geometry_table import (FP16, FP32, LANDING, MAXB, PARITY_BATCH, PARITY_ROWS, RAGGED, ROWS, SPLIT, T, dec_weights, decoder,
+                                  encoder, output_conv, params, row, tc_conv1)
 from tests.test_gpu_a_parity import COS_TOL, _codebook, sess  # noqa: F401
 from tests.test_gpu_d_fp16 import _conv_bound_check, _dense_bound_check
 from tests.test_gpu_e_fp16_train import U, _apply, _check_grads, _cond
@@ -209,7 +215,7 @@ def test_where_each_module_lands(sess, rid):
         with pytest.raises(_lib.AaeError, match="unsupported|needs|expected|FP16"):
             e.handle(sess.device)
         assert e.precision == prec
-    if LANDING[rid][2] == FP32 and LANDING[rid][0] == SPLIT or rid == "refused_k3":
+    if LANDING[rid][2] == FP32:
         d = decoder(r, encoder(r), precision=SPLIT)
         with pytest.raises(_lib.AaeError, match="decoder"):
             d.handle(sess.device)
@@ -263,11 +269,12 @@ def test_encoder_layers_and_latent_match_float64(sess, rid):
 
 
 # ------------------------------------------------------------------------------------------------------------ codebook
-@pytest.mark.parametrize("rid", ["latent32", "latent64", "latent256"])
+@pytest.mark.parametrize("rid", ["latent32", "latent64", "latent256", "px127", "px100"])
 def test_codebook_match_at_other_latents(sess, rid):
-    """nearest_idx_device end to end (encoder + the fp32 match the automatic precision picks at latent != 128), k = 8 and upright:
-    scores within 1e-5 of the float64 cosine of the returned row, and an index other than float64's argmax only where float64
-    puts the two within 2e-6."""
+    """nearest_idx_device end to end (encoder + the fp32 match the automatic precision picks at latent != 128; at 127 px the split
+    encoder with its fp32 conv1 and the tensor-core match, at 100 px the fp32 encoder and match), k = 8 and upright: scores
+    within 1e-5 of the float64 cosine of the returned row, and an index other than float64's argmax only where float64 puts the
+    two within 2e-6."""
     r = row(rid)
     ep, _, _ = params(r)
     E = O.make_codebook(5, n=36 * 300, j=r["latent"])
@@ -336,6 +343,21 @@ def test_decoder_forward_matches_float64(sess, rid):
         _free()
 
 
+@pytest.mark.parametrize("rid,L", [("px100", 4), ("px127", 4), ("px112", 5)])
+def test_decoder_refuses_a_crop_that_is_not_a_multiple_of_2_to_the_L(sess, rid, L):
+    """Every stage doubles its map, so H = 100 would give 6 -> ... -> 96 and H = 127 (or 112 with five convs) 7 -> ... -> 112: the
+    handle is refused when it is created, on every precision, naming H and 2^L; the automatic precision ends on fp32 and raises."""
+    from augmentedautoencoder_b200 import _lib
+    r = row(rid) if L == 4 else row(rid, nf=(128, 256, 512, 512, 512), strides=(2,) * 5, L=5)
+    msg = r"H = %d is not a multiple of 2\^L = %d" % (r["h"], 2 ** L)
+    for prec in (FP32, SPLIT, None):
+        d = decoder(r, encoder(r), precision=prec)
+        with pytest.raises(_lib.AaeError, match=msg):
+            d.handle(sess.device)
+        assert d.precision == (FP32 if prec is None else prec)
+        d.close()
+
+
 # ------------------------------------------------------------------------------------------------------------ training
 def _reference(r, x, y, ep, dp, head, bootstrap=4):
     if head is None:
@@ -353,7 +375,8 @@ def _rel(a, b):
 
 @pytest.mark.parametrize("rid", IDS)
 def test_training_step_matches_float64(sess, rid):
-    """The loss and every gradient at batch 1 and a ragged batch, on whichever trainer the row settles on, within 3e-4 relative L2,
+    """The loss and every gradient at batch 1 and a ragged batch (and PARITY_BATCH on PARITY_ROWS, where one step takes both
+    orderings of the fp32 trainer's stride-2 dgrad), on whichever trainer the row settles on, within 3e-4 relative L2,
     on weights that leave a quarter of every ReLU layer dead with every pre-activation clear of zero.  Where the split trainer
     runs, five Adam steps follow the fp32 trainer: losses within 5e-5, and each variable's five-step update within 0.1 relative L2
     of the fp32 trainer's (Adam's normalised step turns the 3e-5 gradient differences of components near zero into differences
@@ -365,7 +388,7 @@ def test_training_step_matches_float64(sess, rid):
     peak = _Peak(rid + " training")
     enc, dec, top = _pair(r, ep, dp, head)
     worst = 0.0
-    for B in (1, RAGGED):
+    for B in (1, RAGGED) + ((PARITY_BATCH,) if rid in PARITY_ROWS else ()):
         x = np.random.RandomState(8).rand(B, r["h"], r["w"], r["c"]).astype(np.float32)
         y = np.random.RandomState(4).rand(B, r["h"], r["w"], r["c"]).astype(np.float32)
         margin, shares = _check_relu_paths(r, x, ep, dp)
@@ -515,5 +538,60 @@ def test_fp16_trainer_meets_the_rounding_bound(sess, rid):
         _check_grads(grads, g64, bounds, tag)
         del A
     peak.report()
+    top.close(); enc.close(); dec.close()
+    _free()
+
+
+# ------------------------------------------------------------------------------------------------------------ loss limit
+def test_bootstrapped_l2_at_its_shared_memory_limit(sess):
+    """aae_bootstrap_l2_loss at exactly AAE_BOOTSTRAP_MAX_NUMEL = 51 200 values per sample (the whole dynamic shared-memory row
+    buffer), ratio 4, with squared errors on a few hundred exact levels so that every cut splits a tie: the selected set equals a
+    stable float64 top-k (lowest index first among ties) element for element, and the loss and the gradient on that set match.
+    One value more is refused before anything is launched."""
+    from augmentedautoencoder_b200 import _lib
+    from augmentedautoencoder_b200.ae.decoder import Decoder
+    B, numel, ratio = 6, 51200, 4
+    k = numel // ratio
+    rng = np.random.RandomState(22)
+    q = rng.randint(1, 301, (B, numel))                    # |x - t| = q 2^-10 and its square are exact in fp32
+    t = np.full((B, numel), 0.5)
+    x = t + np.where(rng.rand(B, numel) < 0.5, -1.0, 1.0) * q * 2.0 ** -10
+    shape = (B, 160, 160, 2)
+    loss, grad = Decoder.loss_device(torch.from_numpy(x.astype(np.float32).reshape(shape)).cuda(),
+                                     torch.from_numpy(t.astype(np.float32).reshape(shape)).cuda(), ratio, with_grad=True)
+    grad = grad.reshape(B, numel).cpu().numpy()
+    l2 = (x - t) ** 2
+    order = np.argsort(-l2, axis=1, kind="stable")[:, :k]
+    want = np.zeros((B, numel), bool)
+    np.put_along_axis(want, order, True, axis=1)
+    thr = np.take_along_axis(l2, order[:, -1:], axis=1)
+    at_thr = l2 == thr
+    assert np.all(np.sum(at_thr & want, axis=1) > 0) and np.all(np.sum(at_thr & ~want, axis=1) > 0)   # every cut splits a tie
+    bad_rows = np.nonzero(np.any((grad != 0) != want, axis=1))[0]
+    assert not len(bad_rows), ("selection differs in rows", bad_rows)
+    loss64 = float(np.take_along_axis(l2, order, axis=1).mean())
+    assert abs(float(loss) - loss64) < 1e-6, (float(loss), loss64)
+    g64 = 2.0 * (x - t) / (B * k)
+    assert np.allclose(grad[want], g64[want], rtol=1e-6, atol=0.0)
+    over = torch.zeros((1, numel + 1), device="cuda")
+    with pytest.raises(_lib.AaeError, match="51200"):
+        Decoder.loss_device(over, over, ratio)
+
+
+@pytest.mark.parametrize("precision", [None, FP32])
+def test_trainer_refuses_a_crop_above_the_loss_limit(sess, precision):
+    """A 144 x 144 x 3 crop (62 208 values) is more than the bootstrapped L2 loss holds per sample: the encoder and decoder are
+    created (on fp32: 72 and 9 are no powers of two), and the trainer is refused when it is created, naming the limit, instead of
+    failing at its first step."""
+    from augmentedautoencoder_b200 import _lib
+    from augmentedautoencoder_b200.ae.ae import AE
+    from augmentedautoencoder_b200.ae.ae_factory import TrainOp
+    r = dict(T, h=144, w=144, L=len(T["nf"]), id="px144")
+    enc = encoder(r, precision, is_training=True)
+    dec = decoder(r, enc, precision)
+    top = TrainOp(AE(enc, dec, 0, 0), 2e-4)
+    with pytest.raises(_lib.AaeError, match="144 x 144 x 3 crop is 62208 values.*AAE_BOOTSTRAP_MAX_NUMEL = 51200"):
+        top.trainer(sess.device)
+    assert (enc.precision, dec.precision) == (FP32, FP32)
     top.close(); enc.close(); dec.close()
     _free()
