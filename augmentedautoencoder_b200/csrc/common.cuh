@@ -7,6 +7,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/aae_b200.h"
@@ -70,8 +71,87 @@ inline int creation_fence(const char* what) {
   return AAE_ERR_CUDA;
 }
 
+// The one owner of a device allocation: move-only, freed by its destructor, which must run with the allocating device
+// current (creators declare their DeviceGuard before their owners; destroyers hold one).  Aliases are raw pointers (get()).
+// Each way of allocating is named for the callers it serves.
+template <typename T>
+class DevArray {
+ public:
+  DevArray() = default;
+  DevArray(const DevArray&) = delete;
+  DevArray& operator=(const DevArray&) = delete;
+  DevArray(DevArray&& o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+  DevArray& operator=(DevArray&& o) noexcept {
+    if (this != &o) { reset(); p_ = o.p_; n_ = o.n_; o.p_ = nullptr; o.n_ = 0; }
+    return *this;
+  }
+  ~DevArray() { reset(); }
+
+  T* get() const { return p_; }
+  size_t size() const { return n_; }   // elements; 0 until an allocation has succeeded
+  void reset() {
+    if (p_) cudaFree(p_);
+    p_ = nullptr;
+    n_ = 0;
+  }
+
+  // Handle buffers: masters, workspaces, scratch that appears on first use.  Not filled; n = 0 leaves the array empty.  The
+  // error names the size in floats.
+  int alloc(size_t n) {
+    reset();
+    if (n == 0) return AAE_OK;
+    const cudaError_t e = replace(n);
+    if (e != cudaSuccess) {
+      set_error("cudaMalloc(%zu floats) failed: %s", n * sizeof(T) / sizeof(float), cudaGetErrorString(e));
+      return e == cudaErrorMemoryAllocation ? AAE_ERR_OOM : AAE_ERR_CUDA;
+    }
+    n_ = n;
+    return AAE_OK;
+  }
+  // Tensor-core plans, built inside a creator: zero-filled on the legacy stream, which creation_fence orders.
+  int alloc_zeroed(size_t n) {
+    const cudaError_t e = replace(n);
+    if (e != cudaSuccess) {
+      set_error("cudaMalloc(%zu) failed: %s", n * sizeof(T), cudaGetErrorString(e));
+      return AAE_ERR_OOM;
+    }
+    cudaMemset(p_, 0, n * sizeof(T));
+    n_ = n;
+    return AAE_OK;
+  }
+  // Scratch a stream call grows on its first use at a larger size: zero-filled on that call's stream.  Freeing the old buffer
+  // waits for the device, so the call that grows is not asynchronous; every later call at that size is.
+  int grow(size_t n, cudaStream_t s) {
+    const cudaError_t e = replace(n);
+    if (e != cudaSuccess) {
+      set_error("cudaMalloc(%zu) failed: %s", n * sizeof(T), cudaGetErrorString(e));
+      return AAE_ERR_OOM;
+    }
+    AAE_CUDA_OK(cudaMemsetAsync(p_, 0, n * sizeof(T), s));
+    n_ = n;
+    return AAE_OK;
+  }
+
+ private:
+  cudaError_t replace(size_t n) {
+    reset();
+    void* q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, n * sizeof(T));
+    if (e == cudaSuccess) p_ = static_cast<T*>(q);
+    return e;
+  }
+  T* p_ = nullptr;
+  size_t n_ = 0;
+};
+static_assert(!std::is_copy_constructible<DevArray<float>>::value, "an owner is never copied");
+static_assert(std::is_nothrow_move_constructible<DevArray<float>>::value, "std::vector moves its owners instead of copying them");
+
 // Optional per-stage device timing (cudaEvents on the launching stream), read back by bench.py for the roofline lines.
 struct StageTimer {
+  StageTimer() = default;
+  StageTimer(const StageTimer&) = delete;
+  StageTimer& operator=(const StageTimer&) = delete;
+  ~StageTimer() { for (auto e : ev) cudaEventDestroy(e); }
   bool enabled = false;
   std::vector<cudaEvent_t> ev;   // stage i is bracketed by ev[i], ev[i+1]
   int used = 0;
@@ -89,7 +169,6 @@ struct StageTimer {
     }
     return n;
   }
-  void release() { for (auto e : ev) cudaEventDestroy(e); ev.clear(); used = 0; }
 };
 
 // ---- generic implicit-GEMM (SIMT fp32) -----------------------------------------------------

@@ -514,7 +514,7 @@ struct TcConv1 {
   // uint8 kernel: weights with 1/255 folded in, 5 x 16 slot order; output tensor maps over conv2's input
   TcPlanes w8;
   TcMaps tm8, tm_out32;           // output maps: one box = a warp's 32 slots x 32 channels
-  TcPlanes bound;                 // the output the maps were encoded for (not owned)
+  TcView bound;                   // the output the maps were encoded for
   long long slots = 0;            // 256-byte output slots the tensor maps cover ((b, oh/2, ow/2, parity) positions)
 };
 
@@ -524,9 +524,10 @@ bool tc_conv1_supported(const aae_net_cfg* cfg) {
          ow == 64 && (oh % 2) == 0 && cfg->in_w == 128 && (cfg->in_h % 2 == 0);   // staging is laid out for 128-pixel-wide crops
 }
 
-int tc_conv1_create(int device, const aae_net_cfg* cfg, TcConv1** out) {
-  *out = nullptr;
-  TcConv1* h = new TcConv1();
+void TcDelete::operator()(TcConv1* h) const { delete h; }
+
+int tc_conv1_create(int device, const aae_net_cfg* cfg, TcOwner<TcConv1>* out) {
+  TcOwner<TcConv1> h(new TcConv1());
   h->N = cfg->filters[0];
   h->planes = tc_planes(cfg->precision);
   cudaDeviceProp prop;
@@ -535,33 +536,24 @@ int tc_conv1_create(int device, const aae_net_cfg* cfg, TcConv1** out) {
   const uint64_t dims[2] = {128, (uint64_t)h->N};
   const uint64_t strides[1] = {256};
   const uint32_t box[2] = {64, (uint32_t)h->N};
-  int st = h->w.alloc((size_t)h->N * 128, h->planes);
-  if (st == AAE_OK) st = h->w.encode(h->tm, 2, dims, strides, box);
-  if (st == AAE_OK) st = h->w8.alloc((size_t)h->N * 128, h->planes);
-  if (st == AAE_OK) st = h->w8.encode(h->tm8, 2, dims, strides, box);
-  if (st == AAE_OK)
-    st = with_planes(h->planes, [](auto P) {
-      return cudaFuncSetAttribute(tc_conv1_u8_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, U8_SMEM_TOTAL) == cudaSuccess ? AAE_OK : AAE_ERR_CUDA;
-    });
-  if (st != AAE_OK) { tc_conv1_destroy(h); return st; }
-  *out = h;
+  AAE_TRY(h->w.alloc((size_t)h->N * 128, h->planes));
+  AAE_TRY(h->w.view().encode(h->tm, 2, dims, strides, box));
+  AAE_TRY(h->w8.alloc((size_t)h->N * 128, h->planes));
+  AAE_TRY(h->w8.view().encode(h->tm8, 2, dims, strides, box));
+  AAE_TRY(with_planes(h->planes, [](auto P) {
+    return cudaFuncSetAttribute(tc_conv1_u8_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, U8_SMEM_TOTAL) == cudaSuccess ? AAE_OK : AAE_ERR_CUDA;
+  }));
+  *out = std::move(h);
   return AAE_OK;
-}
-
-void tc_conv1_destroy(TcConv1* h) {
-  if (!h) return;
-  h->w.release();
-  h->w8.release();
-  delete h;
 }
 
 int tc_conv1_pack(TcConv1* h, const float* w_dev, int K, float w_scale, unsigned* range_flag, unsigned range_bit, cudaStream_t s) {
   const unsigned grid = (unsigned)ceil_div(h->N * 128, 256);
-  with_planes(h->planes, [&](auto P) { pack_conv1_weights_kernel<P><<<grid, 256, 0, s>>>(w_dev, K, h->N, w_scale, h->w.hi, h->w.lo, range_flag, range_bit); });
+  with_planes(h->planes, [&](auto P) { pack_conv1_weights_kernel<P><<<grid, 256, 0, s>>>(w_dev, K, h->N, w_scale, h->w.hi.get(), h->w.lo.get(), range_flag, range_bit); });
   AAE_LAUNCH_OK();
   AAE_REQUIRE(K == 75, "tc conv1 (uint8 kernel): K = %d, expected 75", K);
   with_planes(h->planes, [&](auto P) {
-    pack_conv1_u8_weights_kernel<P><<<grid, 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8.hi, h->w8.lo, range_flag, range_bit);
+    pack_conv1_u8_weights_kernel<P><<<grid, 256, 0, s>>>(w_dev, h->N, w_scale * 256.f / 255.f, h->w8.hi.get(), h->w8.lo.get(), range_flag, range_bit);
   });
   AAE_LAUNCH_OK();
   return AAE_OK;
@@ -587,7 +579,7 @@ int tc_conv1_forward(TcConv1* h, const aae_net_cfg* cfg, const void* crops, int 
     // output tensor maps: [slot][128 channels] views of conv2's (hi, lo) input; the buffers hold max_batch crops, this call
     // may be shorter -- the maps cover exactly the slots this call writes
     const long long slots = (long long)p.num_tiles * 128;
-    const TcPlanes out{out_hi, out_lo};
+    const TcView out{out_hi, out_lo};
     if (h->bound.hi != out.hi || h->bound.lo != out.lo || h->slots != slots) {
       const uint64_t dims[2] = {128, (uint64_t)slots};
       const uint64_t strides[1] = {256};

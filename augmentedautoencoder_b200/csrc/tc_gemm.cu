@@ -320,43 +320,14 @@ __global__ void __launch_bounds__(256) splitk_forward_finish_kernel(const float*
   }
 }
 
-int dev_alloc(void** p, size_t bytes) { return tc_dev_alloc(p, bytes); }
-
-// Scratch that grows inside a stream call (first use at a larger size): zero-filled on the caller's stream.  tc_dev_alloc fills
-// on the legacy stream, which is ordered for creators only (creation_fence).  Growing frees the old buffer, and cudaFree
-// waits for the device, so the call that grows is not asynchronous; every later call at that size is.
-int scratch_grow(void** p, size_t bytes, cudaStream_t s) {
-  cudaFree(*p);
-  *p = nullptr;
-  cudaError_t e = cudaMalloc(p, bytes);
-  if (e != cudaSuccess) { *p = nullptr; set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return AAE_ERR_OOM; }
-  AAE_CUDA_OK(cudaMemsetAsync(*p, 0, bytes, s));
-  return AAE_OK;
-}
-
 bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
 }  // namespace
 
-int tc_dev_alloc(void** p, size_t bytes) {
-  cudaError_t e = cudaMalloc(p, bytes);
-  if (e != cudaSuccess) { *p = nullptr; set_error("cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e)); return AAE_ERR_OOM; }
-  cudaMemset(*p, 0, bytes);
-  return AAE_OK;
-}
+void TcDelete::operator()(TcEncoder* h) const { delete h; }
+void TcDelete::operator()(TcDecoder* h) const { delete h; }
 
-int TcPlanes::alloc(size_t n, int planes) {
-  AAE_TRY(tc_dev_alloc((void**)&hi, n * sizeof(__half)));
-  return planes == 2 ? tc_dev_alloc((void**)&lo, n * sizeof(__half)) : AAE_OK;
-}
-
-void TcPlanes::release() {
-  cudaFree(hi);
-  cudaFree(lo);
-  hi = lo = nullptr;
-}
-
-int TcPlanes::encode(TcMaps& m, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes) const {
+int TcView::encode(TcMaps& m, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes) const {
   AAE_TRY(make_tmap_f16(&m.hi, hi, rank, dims, strides_bytes, box, swizzle_bytes));
   if (lo == nullptr) {
     m.lo = m.hi;
@@ -422,33 +393,32 @@ int tc_plan_groups(TcLayer& T, int planes, const uint64_t* dims, const uint64_t*
   g.units_per_split = g.groups * g.chunks_per_tap;
   if (!halo) return AAE_OK;
   const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)(T.BH + 2), (uint32_t)T.BB};
-  return T.in.encode(T.tm_halo, 4, dims, strides_bytes, box);
+  return T.in.view().encode(T.tm_halo, 4, dims, strides_bytes, box);
 }
 
-int tc_launch_layer(const TcLayer& T, dim3 tiles, cudaStream_t s, int planes) {
+int tc_launch_layer(const TcLayer& T, const TcGemmParams& gp, dim3 tiles, cudaStream_t s, int planes) {
   const long long count = (long long)tiles.x * tiles.y * tiles.z;
   AAE_REQUIRE(count <= INT_MAX, "tc_gemm: %lld tiles exceed the kernel's int tile index", count);
-  AAE_REQUIRE(T.gp.a_slots >= 2 && T.gp.a_slots <= TC_A_SLOTS_MAX && (T.gp.a_slots & (T.gp.a_slots - 1)) == 0 &&
-              T.gp.a_slots * planes * T.gp.a_rows * TC_KCH * 2 <= TC_A_RING_BYTES, "tc_gemm: layer without a tap-group plan");
+  AAE_REQUIRE(gp.a_slots >= 2 && gp.a_slots <= TC_A_SLOTS_MAX && (gp.a_slots & (gp.a_slots - 1)) == 0 &&
+              gp.a_slots * planes * gp.a_rows * TC_KCH * 2 <= TC_A_RING_BYTES, "tc_gemm: layer without a tap-group plan");
   int device = 0, sms = 0;
   AAE_CUDA_OK(cudaGetDevice(&device));
   AAE_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
   const TcTiles g{(int)tiles.y, (int)tiles.x, (int)count};
   const unsigned ctas = (unsigned)std::min<long long>(count, sms);
-  const TcMaps& a = T.gp.a_rows == 128 ? T.tm_a : T.tm_halo;
+  const TcMaps& a = gp.a_rows == 128 ? T.tm_a : T.tm_halo;
   return with_planes(planes, [&](auto P) {
     constexpr int W_STAGES = P == 1 ? TC_W_STAGES_FP16 : TC_W_STAGES_SPLIT;
     using S = TcSmem<TC_N_TILE, W_STAGES, P>;
     auto kern = tc_gemm_kernel<TC_N_TILE, W_STAGES, P>;
     AAE_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-    kern<<<ctas, TC_THREADS, S::TOTAL, s>>>(a.hi, a.lo, T.tm_w.hi, T.tm_w.lo, T.gp, g);
+    kern<<<ctas, TC_THREADS, S::TOTAL, s>>>(a.hi, a.lo, T.tm_w.hi, T.tm_w.lo, gp, g);
     AAE_LAUNCH_OK();
     return AAE_OK;
   });
 }
 
-int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
-  *out = nullptr;
+int tc_encoder_create(int device, const aae_net_cfg* cfg, TcOwner<TcEncoder>* out) {
   const int L = cfg->num_layers;
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   if (L < 2) {
@@ -460,30 +430,27 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
     set_error("AAE_PREC_TC_FP16: the first layer needs the tensor-core conv1 (128 x 128 x 3 crops, 128 filters, k = 5, stride 2)");
     return AAE_ERR_UNSUPPORTED;
   }
-  TcEncoder* h = new TcEncoder();
+  TcOwner<TcEncoder> h(new TcEncoder());
   h->device = device;
   h->cfg = *cfg;
   h->planes = planes;
   int ih = (cfg->in_h + cfg->strides[0] - 1) / cfg->strides[0], iw = (cfg->in_w + cfg->strides[0] - 1) / cfg->strides[0], ic = cfg->filters[0];
   const int B = cfg->max_batch;
-  int st = AAE_OK;
-  for (int l = 1; l <= L && st == AAE_OK; ++l) {
+  for (int l = 1; l <= L; ++l) {
     TcLayer T;
     memset(&T.gp, 0, sizeof(T.gp));
     const bool dense = (l == L);
     if (!dense) {
       if (cfg->strides[l] != 2 || cfg->kernel_size != 5 || (ih & 1) || (iw & 1) || ic % 64 != 0 || cfg->filters[l] % 32 != 0) {
         set_error("AAE_PREC_TC_SPLIT: layer %d unsupported (needs k=5, stride 2, even dims, Cin %% 64 == 0, Cout %% 32 == 0)", l);
-        st = AAE_ERR_UNSUPPORTED;
-        break;
+        return AAE_ERR_UNSUPPORTED;
       }
       T.in_h = ih; T.in_w = iw; T.in_c = ic;
       T.out_h = ih / 2; T.out_w = iw / 2; T.out_c = cfg->filters[l];
       T.taps = 25;
       if (!pow2(T.out_w) || !pow2(T.out_h) || T.out_w > 128) {
         set_error("AAE_PREC_TC_SPLIT: layer %d output %d x %d unsupported (needs powers of two <= 128)", l, T.out_h, T.out_w);
-        st = AAE_ERR_UNSUPPORTED;
-        break;
+        return AAE_ERR_UNSUPPORTED;
       }
       T.BW = T.out_w;
       T.BH = std::min(T.out_h, 128 / T.BW);
@@ -493,15 +460,15 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
       T.out_h = T.out_w = 1; T.out_c = cfg->latent;
       T.taps = 1; T.BW = 1; T.BH = 1; T.BB = 128;
       h->flat = T.in_c;
-      if (T.in_c % 64 != 0 || T.out_c % 32 != 0) { set_error("AAE_PREC_TC_SPLIT: dense layer needs flat %% 64 == 0 and latent %% 32 == 0"); st = AAE_ERR_UNSUPPORTED; break; }
+      if (T.in_c % 64 != 0 || T.out_c % 32 != 0) { set_error("AAE_PREC_TC_SPLIT: dense layer needs flat %% 64 == 0 and latent %% 32 == 0"); return AAE_ERR_UNSUPPORTED; }
     }
     // batch dimension padded to a whole number of TMA boxes, so a tile never addresses rows outside the tensor map
     const int B_pad = (int)ceil_div(B, T.BB) * T.BB;
     // weight rows padded to whole N tiles (zero-filled; pack_weights_kernel writes rows < out_c only): the producer arms every W
     // stage for TC_N_TILE rows, so a box of fewer rows (out_c < 128) would never complete the stage's barrier
     const int w_rows = (int)ceil_div(T.out_c, TC_N_TILE) * TC_N_TILE;
-    if ((st = T.in.alloc((size_t)B_pad * T.in_h * T.in_w * T.in_c, planes)) != AAE_OK) break;
-    if ((st = T.w.alloc((size_t)w_rows * T.taps * T.in_c, planes)) != AAE_OK) break;
+    AAE_TRY(T.in.alloc((size_t)B_pad * T.in_h * T.in_w * T.in_c, planes));
+    AAE_TRY(T.w.alloc((size_t)w_rows * T.taps * T.in_c, planes));
     // ---- tensor maps ----
     uint64_t a_dims[4], a_strides[3];
     if (!dense) {
@@ -516,14 +483,14 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
     }
     {
       const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};   // dense: [64, 1, 1, 128]
-      if ((st = T.in.encode(T.tm_a, 4, a_dims, a_strides, box)) != AAE_OK) break;
+      AAE_TRY(T.in.view().encode(T.tm_a, 4, a_dims, a_strides, box));
     }
     {
       const uint64_t K = (uint64_t)T.taps * T.in_c;
       const uint64_t dims[2] = {K, (uint64_t)w_rows};
       const uint64_t strides[1] = {K * 2};
       const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)TC_N_TILE};
-      if ((st = T.w.encode(T.tm_w, 2, dims, strides, box)) != AAE_OK) break;
+      AAE_TRY(T.w.view().encode(T.tm_w, 2, dims, strides, box));
     }
     // ---- static GEMM parameters ----
     TcGemmParams& g = T.gp;
@@ -538,63 +505,49 @@ int tc_encoder_create(int device, const aae_net_cfg* cfg, TcEncoder** out) {
       g.tap_ch[t] = ((((kh + 1) & 1) << 1) | ((kw + 1) & 1)) * T.in_c;
     }
     // 5 x 5 stride 2: taps of one kw and one row parity (kh in {0, 2, 4} or {1, 3}) share a halo box -> 10 groups
-    if ((st = tc_plan_groups(T, planes, a_dims, a_strides)) != AAE_OK) break;
+    AAE_TRY(tc_plan_groups(T, planes, a_dims, a_strides));
     g.unscale = 1.f / (ACT_SCALE * W_SCALE);
     g.out_scale = ACT_SCALE;
     g.relu = dense ? 0 : 1;
-    h->layers.push_back(T);
     if (!dense) { ih = T.out_h; iw = T.out_w; ic = T.out_c; }
+    h->layers.push_back(std::move(T));
   }
-  if (st == AAE_OK) {
-    // wire outputs: layer i writes the input buffers of layer i+1; the last conv writes plain NHWC (the flatten order)
-    for (size_t i = 0; i + 1 < h->layers.size(); ++i) {
-      TcGemmParams& g = h->layers[i].gp;
-      g.out_hi = h->layers[i + 1].in.hi;
-      g.out_lo = h->layers[i + 1].in.lo;
-      g.out_mode = (i + 2 == h->layers.size()) ? OUT_PLAIN_SPLIT : OUT_S2D_SPLIT;
-    }
-    TcLayer& D = h->layers.back();
-    const int total = D.gp.groups * D.gp.chunks_per_tap;     // one tap: units are chunks
-    h->dense_splits = std::min(total, 66);
-    D.gp.units_per_split = (total + h->dense_splits - 1) / h->dense_splits;
-    h->dense_splits = (total + D.gp.units_per_split - 1) / D.gp.units_per_split;
-    D.gp.out_mode = OUT_F32;
-    st = dev_alloc((void**)&h->partials, (size_t)h->dense_splits * (B + 128) * cfg->latent * sizeof(float));
-    D.gp.out_f32 = h->partials;
+  // wire outputs: layer i writes the input buffers of layer i+1; the last conv writes plain NHWC (the flatten order)
+  for (size_t i = 0; i + 1 < h->layers.size(); ++i) {
+    TcGemmParams& g = h->layers[i].gp;
+    g.out_hi = h->layers[i + 1].in.hi.get();
+    g.out_lo = h->layers[i + 1].in.lo.get();
+    g.out_mode = (i + 2 == h->layers.size()) ? OUT_PLAIN_SPLIT : OUT_S2D_SPLIT;
   }
-  if (st == AAE_OK) st = dev_alloc((void**)&h->range_flag, sizeof(unsigned));
-  if (st == AAE_OK)
-    for (size_t i = 0; i + 1 < h->layers.size(); ++i) {   // layers[i] writes the activation of conv layer i + 1 (0-based); the dense layer writes fp32
-      h->layers[i].gp.range_flag = h->range_flag;
-      h->layers[i].gp.range_bit = 1u << (i + 1);
-    }
-  if (st == AAE_OK && tc_conv1_supported(cfg)) st = tc_conv1_create(device, cfg, &h->conv1);
-  if (st != AAE_OK) { tc_encoder_destroy(h); return st; }
-  *out = h;
+  TcLayer& D = h->layers.back();
+  const int total = D.gp.groups * D.gp.chunks_per_tap;     // one tap: units are chunks
+  h->dense_splits = std::min(total, 66);
+  D.gp.units_per_split = (total + h->dense_splits - 1) / h->dense_splits;
+  h->dense_splits = (total + D.gp.units_per_split - 1) / D.gp.units_per_split;
+  D.gp.out_mode = OUT_F32;
+  AAE_TRY(h->partials.alloc_zeroed((size_t)h->dense_splits * (B + 128) * cfg->latent));
+  D.gp.out_f32 = h->partials.get();
+  AAE_TRY(h->own_range_flag.alloc_zeroed(1));
+  h->range_flag = h->own_range_flag.get();
+  for (size_t i = 0; i + 1 < h->layers.size(); ++i) {   // layers[i] writes the activation of conv layer i + 1 (0-based); the dense layer writes fp32
+    h->layers[i].gp.range_flag = h->range_flag;
+    h->layers[i].gp.range_bit = 1u << (i + 1);
+  }
+  if (tc_conv1_supported(cfg)) AAE_TRY(tc_conv1_create(device, cfg, &h->conv1));
+  *out = std::move(h);
   return AAE_OK;
-}
-
-void tc_encoder_destroy(TcEncoder* h) {
-  if (!h) return;
-  for (auto& T : h->layers) { T.in.release(); T.w.release(); }
-  cudaFree(h->partials);
-  cudaFree(h->fwd_partials);
-  cudaFree(h->dbg);
-  if (h->owns_range_flag) cudaFree(h->range_flag);
-  tc_conv1_destroy(h->conv1);
-  delete h;
 }
 
 int tc_encoder_pack_weights(TcEncoder* h, int layer, const float* w_dev, cudaStream_t s) {
   if (layer == 0) {
-    if (h->conv1) return tc_conv1_pack(h->conv1, w_dev, h->cfg.kernel_size * h->cfg.kernel_size * h->cfg.in_c, W_SCALE, h->range_flag, 1u << 16, s);
+    if (h->conv1) return tc_conv1_pack(h->conv1.get(), w_dev, h->cfg.kernel_size * h->cfg.kernel_size * h->cfg.in_c, W_SCALE, h->range_flag, 1u << 16, s);
     return AAE_OK;  // conv1 on the fp32 SIMT kernel
   }
   AAE_REQUIRE(layer >= 1 && layer <= (int)h->layers.size(), "tc pack: layer %d out of range", layer);
   TcLayer& T = h->layers[layer - 1];
   dim3 grid((unsigned)ceil_div(T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), (unsigned)T.taps), block(32, 8);
   with_planes(h->planes, [&](auto P) {
-    pack_weights_kernel<P><<<grid, block, 0, s>>>(w_dev, T.taps, T.in_c, T.out_c, W_SCALE, T.w.hi, T.w.lo, h->range_flag, 1u << (16 + layer));
+    pack_weights_kernel<P><<<grid, block, 0, s>>>(w_dev, T.taps, T.in_c, T.out_c, W_SCALE, T.w.hi.get(), T.w.lo.get(), h->range_flag, 1u << (16 + layer));
   });
   AAE_LAUNCH_OK();
   return AAE_OK;
@@ -604,16 +557,14 @@ unsigned* tc_encoder_range_flag(TcEncoder* h) { return h->range_flag; }
 unsigned* tc_decoder_range_flag(TcDecoder* h) { return h->range_flag; }
 
 void tc_encoder_share_range_flag(TcEncoder* h, unsigned* flag) {
-  if (h->owns_range_flag) cudaFree(h->range_flag);
+  h->own_range_flag.reset();
   h->range_flag = flag;
-  h->owns_range_flag = false;
   for (size_t i = 0; i + 1 < h->layers.size(); ++i) h->layers[i].gp.range_flag = flag;   // the dense layer writes fp32: no guard
 }
 
 void tc_decoder_share_range_flag(TcDecoder* h, unsigned* flag) {
-  if (h->owns_range_flag) cudaFree(h->range_flag);
+  h->own_range_flag.reset();
   h->range_flag = flag;
-  h->owns_range_flag = false;
   for (size_t i = 0; i + 1 < h->layers.size(); ++i) h->layers[i].gp.range_flag = flag;
 }
 
@@ -623,7 +574,8 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
   timer->reset();
   timer->mark(s);
   if (h->conv1) {
-    AAE_TRY(tc_conv1_forward(h->conv1, &cfg, crops, src_u8, B, b0, ACT_SCALE, W_SCALE, h->layers[0].in.hi, h->layers[0].in.lo, h->range_flag, s));
+    AAE_TRY(tc_conv1_forward(h->conv1.get(), &cfg, crops, src_u8, B, b0, ACT_SCALE, W_SCALE, h->layers[0].in.hi.get(), h->layers[0].in.lo.get(),
+                             h->range_flag, s));
   } else {  // conv1 (Cin = 3, K = 75): fp32 SIMT implicit GEMM, epilogue writes conv2's space-to-depth (hi, lo) input directly
     IGemmParams p;
     memset(&p, 0, sizeof(p));
@@ -636,7 +588,7 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
     p.Bm = w0; p.N = cfg.filters[0]; p.bias = b0; p.act = ACT_RELU;
     p.M = B * p.PH * p.PW; p.K = p.KH * p.KW * p.SC;
     p.k_per_split = (int)ceil_div(p.K, 16) * 16;
-    p.split_hi = h->layers[0].in.hi; p.split_lo = h->layers[0].in.lo; p.split_scale = ACT_SCALE; p.split_s2d = 1;
+    p.split_hi = h->layers[0].in.hi.get(); p.split_lo = h->layers[0].in.lo.get(); p.split_scale = ACT_SCALE; p.split_s2d = 1;
     p.range_flag = h->range_flag; p.range_bit = 1u;   // bit 0: conv1's activation, as on the tensor-core conv1
     AAE_TRY(launch_igemm(p, GATHER_FWD, s));
   }
@@ -654,35 +606,31 @@ int tc_encoder_forward(TcEncoder* h, const void* crops, int src_u8, int B, const
       if (tiles * 2 <= 132) {
         splits = std::min(132 / tiles, std::max(1, total_iters / 24));
         const size_t per_split = (size_t)T.gp.M * T.gp.N;
-        if (per_split * (size_t)splits > h->fwd_partial_floats) {
+        if (per_split * (size_t)splits > h->fwd_partials.size()) {
           const size_t want = std::min<size_t>(per_split * (size_t)splits, (size_t)32 << 20);     // at most 128 MB of partials
-          if (want > h->fwd_partial_floats) {
-            h->fwd_partial_floats = 0;
-            AAE_TRY(scratch_grow((void**)&h->fwd_partials, want * sizeof(float), s));
-            h->fwd_partial_floats = want;
-          }
-          splits = (int)std::min<size_t>((size_t)splits, h->fwd_partial_floats / per_split);
+          if (want > h->fwd_partials.size()) AAE_TRY(h->fwd_partials.grow(want, s));
+          splits = (int)std::min<size_t>((size_t)splits, h->fwd_partials.size() / per_split);
         }
         splits = std::max(splits, 1);
       }
     }
     if (splits > 1) {
-      TcLayer S = T;                                   // same operands and maps, partial sums out
+      TcGemmParams S = T.gp;                           // same operands and maps, partial sums out
       const int total_units = T.gp.groups * T.gp.chunks_per_tap;   // K is cut on (tap group, chunk) boundaries
-      S.gp.units_per_split = (int)ceil_div(total_units, splits);
-      splits = (int)ceil_div(total_units, S.gp.units_per_split);
-      S.gp.out_mode = OUT_F32;
-      S.gp.out_f32 = h->fwd_partials;
+      S.units_per_split = (int)ceil_div(total_units, splits);
+      splits = (int)ceil_div(total_units, S.units_per_split);
+      S.out_mode = OUT_F32;
+      S.out_f32 = h->fwd_partials.get();
       grid.z = (unsigned)splits;
-      AAE_TRY(tc_launch_layer(S, grid, s, h->planes));
+      AAE_TRY(tc_launch_layer(T, S, grid, s, h->planes));
       const long long groups = (long long)T.gp.M * (T.gp.N >> 3);
       const unsigned fin_grid = (unsigned)std::min<long long>(132 * 8, ceil_div(groups, 256));
-      with_planes(h->planes, [&](auto P) { splitk_forward_finish_kernel<P><<<fin_grid, 256, 0, s>>>(h->fwd_partials, splits, T.gp); });
+      with_planes(h->planes, [&](auto P) { splitk_forward_finish_kernel<P><<<fin_grid, 256, 0, s>>>(h->fwd_partials.get(), splits, T.gp); });
       AAE_LAUNCH_OK();
     } else {
-      AAE_TRY(tc_launch_layer(T, grid, s, h->planes));
+      AAE_TRY(tc_launch_layer(T, T.gp, grid, s, h->planes));
     }
-    if (dense) AAE_TRY(launch_splitk_reduce(h->partials, h->dense_splits, (int64_t)B * cfg.latent, cfg.latent, dense_b, ACT_NONE, z_out, s));
+    if (dense) AAE_TRY(launch_splitk_reduce(h->partials.get(), h->dense_splits, (int64_t)B * cfg.latent, cfg.latent, dense_b, ACT_NONE, z_out, s));
     timer->mark(s);
   }
   return AAE_OK;
@@ -702,17 +650,13 @@ int tc_encoder_activation(TcEncoder* h, int layer, int B, const float** ptr, int
   if (plain) { const TcLayer& P = h->layers[layer - 1]; H = P.out_h; W = P.out_w; C = P.out_c; }
   else { H = T.in_h; W = T.in_w; C = T.in_c; }
   const size_t n = (size_t)B * H * W * C;
-  if (h->dbg_floats < n) {
-    h->dbg_floats = 0;
-    AAE_TRY(scratch_grow((void**)&h->dbg, n * sizeof(float), s));
-    h->dbg_floats = n;
-  }
+  if (h->dbg.size() < n) AAE_TRY(h->dbg.grow(n, s));
   with_planes(h->planes, [&](auto P) {
-    unpack_act_kernel<P><<<1024, 256, 0, s>>>(T.in.hi, T.in.lo, B, H, W, C, plain ? 0 : 1, 1.f / ACT_SCALE, h->dbg);
+    unpack_act_kernel<P><<<1024, 256, 0, s>>>(T.in.hi.get(), T.in.lo.get(), B, H, W, C, plain ? 0 : 1, 1.f / ACT_SCALE, h->dbg.get());
   });
   AAE_LAUNCH_OK();
   AAE_CUDA_OK(cudaStreamSynchronize(s));
-  *ptr = h->dbg;
+  *ptr = h->dbg.get();
   *count = (int64_t)n;
   return AAE_OK;
 }
@@ -797,24 +741,23 @@ int tc_layer_setup_plain(TcLayer& T, int B, int planes) {
     const uint64_t dims[4] = {(uint64_t)T.in_c, (uint64_t)T.in_w, (uint64_t)T.in_h, (uint64_t)B_pad};
     const uint64_t strides[3] = {(uint64_t)T.in_c * 2, (uint64_t)T.in_w * T.in_c * 2, (uint64_t)T.in_h * T.in_w * T.in_c * 2};
     const uint32_t box[4] = {(uint32_t)TC_KCH, (uint32_t)T.BW, (uint32_t)T.BH, (uint32_t)T.BB};
-    AAE_TRY(T.in.encode(T.tm_a, 4, dims, strides, box));
+    AAE_TRY(T.in.view().encode(T.tm_a, 4, dims, strides, box));
     AAE_TRY(tc_plan_groups(T, planes, dims, strides));   // 3 x 3 taps: one group per column offset dj
   }
   const uint64_t dims[2] = {K, (uint64_t)rows};
   const uint64_t strides[1] = {K * 2};
   const uint32_t box[2] = {(uint32_t)TC_KCH, (uint32_t)TC_N_TILE};
-  return T.w.encode(T.tm_w, 2, dims, strides, box);
+  return T.w.view().encode(T.tm_w, 2, dims, strides, box);
 }
 
-int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcDecoder** out) {
-  *out = nullptr;
+int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcOwner<TcDecoder>* out) {
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   const int L = cfg->num_layers;
   if (cfg->kernel_size != 5 || cfg->in_h != cfg->in_w) {
     set_error("AAE_PREC_TC_SPLIT decoder: kernel 5 and square crops required (kernel %d, %d x %d crops)", cfg->kernel_size, cfg->in_h, cfg->in_w);
     return AAE_ERR_UNSUPPORTED;
   }
-  TcDecoder* h = new TcDecoder();
+  TcOwner<TcDecoder> h(new TcDecoder());
   h->device = device;
   h->cfg = *cfg;
   h->planes = tc_planes(cfg->precision);
@@ -823,8 +766,7 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcDeco
   for (int i = 0; i < L; ++i) h0 /= 2;
   std::vector<int> nf(L);
   for (int i = 0; i < L; ++i) nf[i] = cfg->filters[L - 1 - i];
-  int st = AAE_OK;
-  for (int l = 0; l <= L && st == AAE_OK; ++l) {
+  for (int l = 0; l <= L; ++l) {
     TcLayer T;
     memset(&T.gp, 0, sizeof(T.gp));
     TcGemmParams& g = T.gp;
@@ -832,7 +774,7 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcDeco
       T.in_h = T.in_w = 1; T.in_c = cfg->latent; T.out_h = T.out_w = 1; T.out_c = h0 * h0 * nf[0];
       T.taps = 1; T.BW = 1; T.BH = 1; T.BB = 128;
       g.N = T.out_c; g.OH = g.OW = 1; g.relu = 1; g.out_mode = OUT_PLAIN_SPLIT;
-      if (cfg->latent % 64 != 0 || T.out_c % 128 != 0) { set_error("tc decoder: latent %% 64 and dense width %% 128 required"); st = AAE_ERR_UNSUPPORTED; break; }
+      if (cfg->latent % 64 != 0 || T.out_c % 128 != 0) { set_error("tc decoder: latent %% 64 and dense width %% 128 required"); return AAE_ERR_UNSUPPORTED; }
     } else {                                        // sub-pixel conv on the (h x w x C) low-resolution activation
       const int hh = h0 << (l - 1);
       T.in_h = T.in_w = hh; T.in_c = nf[l - 1];
@@ -840,7 +782,8 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcDeco
       T.out_h = T.out_w = 2 * hh; T.out_c = cout;
       T.taps = 9;
       if (hh > 128 || (hh & (hh - 1)) || T.in_c % 64 != 0 || (l < L && cout % 64 != 0)) {
-        set_error("tc decoder: layer %d unsupported (power-of-two size <= 128, Cin %% 64, Cout %% 64)", l); st = AAE_ERR_UNSUPPORTED; break;
+        set_error("tc decoder: layer %d unsupported (power-of-two size <= 128, Cin %% 64, Cout %% 64)", l);
+        return AAE_ERR_UNSUPPORTED;
       }
       T.BW = hh; T.BH = std::min(hh, 128 / T.BW); T.BB = 128 / (T.BW * T.BH);
       g.OH = g.OW = hh;
@@ -848,14 +791,13 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcDeco
       else {                                        // 1x1 GEMM into P, neighbourhood sum in outlayer_gather_kernel
         if (cfg->in_c > 3) {
           set_error("tc decoder: %d output channels, the tensor-core output layer takes at most 3 (AAE_PREC_FP32_SIMT takes any count)", cfg->in_c);
-          st = AAE_ERR_UNSUPPORTED; break;
+          return AAE_ERR_UNSUPPORTED;
         }
         // 9 taps x 4 parities x Cout columns: 128 for x alone, 256 with the mask head (one pass over the activation either way)
         T.taps = 1; g.N = (int)ceil_div(36 * cout, 128) * 128; g.relu = 0; g.out_mode = OUT_F32;
         h->out_x = cfg->in_c;
-        st = dev_alloc((void**)&h->out_p, (size_t)ceil_div((int64_t)B * hh * hh, 128) * 128 * g.N * sizeof(float));
-        if (st == AAE_OK && mask_head) st = dev_alloc((void**)&h->cat_tmp, (size_t)25 * T.in_c * cout * sizeof(float));
-        if (st != AAE_OK) break;
+        AAE_TRY(h->out_p.alloc_zeroed((size_t)ceil_div((int64_t)B * hh * hh, 128) * 128 * g.N));
+        if (mask_head) AAE_TRY(h->cat_tmp.alloc_zeroed((size_t)25 * T.in_c * cout));
       }
     }
     g.BW = T.BW; g.BH = T.BH; g.taps = T.taps; g.chunks_per_tap = T.in_c / TC_KCH;
@@ -866,37 +808,24 @@ int tc_decoder_create(int device, const aae_net_cfg* cfg, bool mask_head, TcDeco
     }
     g.unscale = 1.f / (ACT_SCALE * W_SCALE);
     g.out_scale = ACT_SCALE;
-    if ((st = tc_layer_setup_plain(T, B, h->planes)) != AAE_OK) { h->layers.push_back(T); break; }
-    h->layers.push_back(T);
-    float* bz = nullptr;
-    if (l > 0 && l < L) st = dev_alloc((void**)&bz, (size_t)g.N * sizeof(float));
-    h->bias_dev.push_back(bz);
+    AAE_TRY(tc_layer_setup_plain(T, B, h->planes));
     h->wm_floats = std::max(h->wm_floats, (size_t)9 * T.in_c * 4 * T.out_c);
+    DevArray<float> bias4;
+    if (l > 0 && l < L) AAE_TRY(bias4.alloc_zeroed(g.N));
+    h->layers.push_back(std::move(T));
+    h->bias_dev.push_back(std::move(bias4));
   }
-  if (st == AAE_OK) st = dev_alloc((void**)&h->wm_tmp, h->wm_floats * sizeof(float));
-  if (st == AAE_OK) st = dev_alloc((void**)&h->range_flag, sizeof(unsigned));
-  if (st == AAE_OK) {
-    for (size_t i = 0; i + 1 < h->layers.size(); ++i) {
-      h->layers[i].gp.out_hi = h->layers[i + 1].in.hi;
-      h->layers[i].gp.out_lo = h->layers[i + 1].in.lo;
-      h->layers[i].gp.range_flag = h->range_flag;       // bit i: the activation written by layer i (0 = dense_1)
-      h->layers[i].gp.range_bit = 1u << i;
-    }
+  AAE_TRY(h->wm_tmp.alloc_zeroed(h->wm_floats));
+  AAE_TRY(h->own_range_flag.alloc_zeroed(1));
+  h->range_flag = h->own_range_flag.get();
+  for (size_t i = 0; i + 1 < h->layers.size(); ++i) {
+    h->layers[i].gp.out_hi = h->layers[i + 1].in.hi.get();
+    h->layers[i].gp.out_lo = h->layers[i + 1].in.lo.get();
+    h->layers[i].gp.range_flag = h->range_flag;       // bit i: the activation written by layer i (0 = dense_1)
+    h->layers[i].gp.range_bit = 1u << i;
   }
-  if (st != AAE_OK) { tc_decoder_destroy(h); return st; }
-  *out = h;
+  *out = std::move(h);
   return AAE_OK;
-}
-
-void tc_decoder_destroy(TcDecoder* h) {
-  if (!h) return;
-  for (auto& T : h->layers) { T.in.release(); T.w.release(); }
-  for (auto b : h->bias_dev) cudaFree(b);
-  cudaFree(h->wm_tmp);
-  cudaFree(h->out_p);
-  cudaFree(h->cat_tmp);
-  if (h->owns_range_flag) cudaFree(h->range_flag);
-  delete h;
 }
 
 // layer 0: dense_1 kernel [latent, h0*w0*f0]; layers 1..L: conv kernels HWIO [5,5,cin,cout]; biases in the reference layout
@@ -908,7 +837,7 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
     if (w_dev) {
       dim3 grid((unsigned)ceil_div(T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), 1);
       with_planes(h->planes, [&](auto P) {
-        pack_weights_kernel<P><<<grid, block, 0, s>>>(w_dev, 1, T.in_c, T.out_c, W_SCALE, T.w.hi, T.w.lo, h->range_flag, 1u << 16);
+        pack_weights_kernel<P><<<grid, block, 0, s>>>(w_dev, 1, T.in_c, T.out_c, W_SCALE, T.w.hi.get(), T.w.lo.get(), h->range_flag, 1u << 16);
       });
       AAE_LAUNCH_OK();
     }
@@ -917,18 +846,18 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
   }
   const bool out_layer = layer + 1 == (int)h->layers.size();
   if (w_dev) {
-    if (out_layer && h->cat_tmp) {      // join the output conv [5,5,Cin,C] and the mask head [5,5,Cin,1] along Cout
+    if (out_layer && h->cat_tmp.get()) {      // join the output conv [5,5,Cin,C] and the mask head [5,5,Cin,1] along Cout
       AAE_REQUIRE(h->mask_w != nullptr, "tc decoder: the mask head's weights are not set");
-      AAE_TRY(launch_copy_channels(w_dev, h->out_x, 0, h->cat_tmp, T.out_c, 0, h->out_x, 25LL * T.in_c, s));
-      AAE_TRY(launch_copy_channels(h->mask_w, 1, 0, h->cat_tmp, T.out_c, h->out_x, 1, 25LL * T.in_c, s));
-      w_dev = h->cat_tmp;
+      AAE_TRY(launch_copy_channels(w_dev, h->out_x, 0, h->cat_tmp.get(), T.out_c, 0, h->out_x, 25LL * T.in_c, s));
+      AAE_TRY(launch_copy_channels(h->mask_w, 1, 0, h->cat_tmp.get(), T.out_c, h->out_x, 1, 25LL * T.in_c, s));
+      w_dev = h->cat_tmp.get();
     }
-    AAE_TRY(launch_merge_subpixel_weights(w_dev, T.in_c, T.out_c, h->wm_tmp, s));
+    AAE_TRY(launch_merge_subpixel_weights(w_dev, T.in_c, T.out_c, h->wm_tmp.get(), s));
     const unsigned bit = 1u << (16 + layer);
     dim3 grid((unsigned)ceil_div(4 * T.out_c, 32), (unsigned)ceil_div(T.in_c, 32), 9);
     with_planes(h->planes, [&](auto P) {
-      if (out_layer) pack_out_sep_kernel<P><<<64, 256, 0, s>>>(h->wm_tmp, T.in_c, 4 * T.out_c, T.gp.N, W_SCALE, T.w.hi, T.w.lo, h->range_flag, bit);
-      else pack_weights_kernel<P><<<grid, block, 0, s>>>(h->wm_tmp, 9, T.in_c, 4 * T.out_c, W_SCALE, T.w.hi, T.w.lo, h->range_flag, bit);
+      if (out_layer) pack_out_sep_kernel<P><<<64, 256, 0, s>>>(h->wm_tmp.get(), T.in_c, 4 * T.out_c, T.gp.N, W_SCALE, T.w.hi.get(), T.w.lo.get(), h->range_flag, bit);
+      else pack_weights_kernel<P><<<grid, block, 0, s>>>(h->wm_tmp.get(), 9, T.in_c, 4 * T.out_c, W_SCALE, T.w.hi.get(), T.w.lo.get(), h->range_flag, bit);
     });
     AAE_LAUNCH_OK();
   }
@@ -937,14 +866,14 @@ int tc_decoder_pack_weights(TcDecoder* h, int layer, const float* w_dev, const f
     return AAE_OK;
   }
   if (b_dev) {
-    tile_bias_kernel<<<(unsigned)ceil_div(T.gp.N, 128), 128, 0, s>>>(b_dev, T.out_c, h->bias_dev[layer]);
+    tile_bias_kernel<<<(unsigned)ceil_div(T.gp.N, 128), 128, 0, s>>>(b_dev, T.out_c, h->bias_dev[layer].get());
     AAE_LAUNCH_OK();
-    T.gp.bias = h->bias_dev[layer];
+    T.gp.bias = h->bias_dev[layer].get();
   }
   return AAE_OK;
 }
 
-const float* tc_decoder_merged_weights(const TcDecoder* h) { return h->wm_tmp; }
+const float* tc_decoder_merged_weights(const TcDecoder* h) { return h->wm_tmp.get(); }
 
 void tc_decoder_set_mask_head(TcDecoder* h, const float* w_dev, const float* b_dev) {
   h->mask_w = w_dev;
@@ -956,20 +885,20 @@ int tc_decoder_forward(TcDecoder* h, const float* z_dev, int B, float* x_out, fl
   TcLayer& D = h->layers[0];
   const unsigned grid = (unsigned)std::min<int64_t>(1024, ceil_div((int64_t)B * D.in_c, 256));
   with_planes(h->planes, [&](auto P) {
-    split_scale_kernel<P><<<grid, 256, 0, s>>>(z_dev, (long long)B * D.in_c, ACT_SCALE, D.in.hi, D.in.lo, h->range_flag, 1u << 15);
+    split_scale_kernel<P><<<grid, 256, 0, s>>>(z_dev, (long long)B * D.in_c, ACT_SCALE, D.in.hi.get(), D.in.lo.get(), h->range_flag, 1u << 15);
   });
   AAE_LAUNCH_OK();
   for (size_t i = 0; i < h->layers.size(); ++i) {
     TcLayer& T = h->layers[i];
     T.gp.M = i == 0 ? B : B * T.in_h * T.in_w;
     const bool last = i + 1 == h->layers.size();
-    if (last) T.gp.out_f32 = h->out_p;
+    if (last) T.gp.out_f32 = h->out_p.get();
     dim3 grid((unsigned)ceil_div(T.gp.M, 128), (unsigned)ceil_div(T.gp.N, TC_N_TILE), 1u);
-    AAE_TRY(tc_launch_layer(T, grid, s, h->planes));
+    AAE_TRY(tc_launch_layer(T, T.gp, grid, s, h->planes));
     if (last) {
       const long long total = (long long)T.gp.M * 4 * T.out_c;
       outlayer_gather_kernel<<<(unsigned)std::min<long long>(132 * 16, ceil_div(total, 256)), 256, 0, s>>>(
-          h->out_p, T.gp.N, h->out_bias, h->mask_b, B, T.in_h, T.in_w, h->out_x, T.out_c - h->out_x, x_out, mask_out);
+          h->out_p.get(), T.gp.N, h->out_bias, h->mask_b, B, T.in_h, T.in_w, h->out_x, T.out_c - h->out_x, x_out, mask_out);
       AAE_LAUNCH_OK();
     }
   }

@@ -344,10 +344,12 @@ struct TcCodebook {
   TcPlanes e;
   TcMaps tm, tm_up;
   bool have_up = false;
-  unsigned long long* best = nullptr;
-  unsigned long long* lists = nullptr;   // [grid][max_batch][8] packed keys of the per-CTA top-k lists (k > 1)
-  unsigned int* counter = nullptr;
+  DevArray<unsigned long long> best;
+  DevArray<unsigned long long> lists;    // [grid][max_batch][8] packed keys of the per-CTA top-k lists (k > 1)
+  DevArray<unsigned int> counter;
 };
+
+void TcDelete::operator()(TcCodebook* h) const { delete h; }
 
 constexpr int MT_KMAX = 8;
 
@@ -368,14 +370,13 @@ int tc_launch_floor_probe(int device, int with_tmem, cudaStream_t s) {
 }
 
 int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int64_t row_offset, int latent, int num_cyclo, int max_batch,
-                       int planes, TcCodebook** out) {
-  *out = nullptr;
+                       int planes, TcOwner<TcCodebook>* out) {
   AAE_REQUIRE(aae_device_supported(device), "AAE_PREC_TC_SPLIT needs a compute-capability 9.0 device (wgmma/TMA)");
   if (latent != 128) {
     set_error("AAE_PREC_TC_SPLIT codebook match is built for latent = 128 (got %d)", latent);
     return AAE_ERR_UNSUPPORTED;
   }
-  TcCodebook* h = new TcCodebook();
+  TcOwner<TcCodebook> h(new TcCodebook());
   h->device = device;
   h->planes = planes;
   h->n_rows = n_rows;
@@ -390,48 +391,42 @@ int tc_codebook_create(int device, const float* E_dev, int64_t n_rows, int64_t r
   cudaGetDeviceProperties(&prop, device);
   h->sm_count = std::min(prop.multiProcessorCount, MT_MAX_GRID);
   const int cap_b = std::min(MT_BATCH, std::max(1, max_batch));
-  if (int st = h->e.alloc((size_t)h->n_pad * 128, planes)) { tc_codebook_destroy(h); return st; }
-  cudaError_t e = cudaMalloc(&h->best, 256 * sizeof(unsigned long long));
-  if (e == cudaSuccess) e = cudaMalloc(&h->lists, (size_t)h->sm_count * cap_b * MT_KMAX * sizeof(unsigned long long));
-  if (e == cudaSuccess) e = cudaMalloc(&h->counter, sizeof(unsigned int));
-  if (e != cudaSuccess) { set_error("tc codebook alloc failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_OOM; }
-  cudaMemset(h->best, 0, 256 * sizeof(unsigned long long));
-  cudaMemset(h->counter, 0, sizeof(unsigned int));
-  with_planes(planes, [&](auto P) { pack_codebook_kernel<P><<<1024, 256>>>(E_dev, n_rows, h->n_pad, h->e.hi, h->e.lo); });
+  AAE_TRY(h->e.alloc((size_t)h->n_pad * 128, planes));
+  // the match kernels' scratch: best and counter start at zero, lists is written before it is read.  Any failure here is
+  // reported as AAE_ERR_OOM under one message (a failed cudaMalloc leaves its error as the thread's last error).
+  if (h->best.alloc_zeroed(256) != AAE_OK || h->lists.alloc((size_t)h->sm_count * cap_b * MT_KMAX) != AAE_OK ||
+      h->counter.alloc_zeroed(1) != AAE_OK) {
+    set_error("tc codebook alloc failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return AAE_ERR_OOM;
+  }
+  const TcView e = h->e.view();
+  with_planes(planes, [&](auto P) { pack_codebook_kernel<P><<<1024, 256>>>(E_dev, n_rows, h->n_pad, e.hi, e.lo); });
   g_launches.fetch_add(1);
-  e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) { set_error("pack_codebook failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_CUDA; }
+  const cudaError_t sync = cudaDeviceSynchronize();
+  if (sync != cudaSuccess) { set_error("pack_codebook failed: %s", cudaGetErrorString(sync)); return AAE_ERR_CUDA; }
   const uint64_t dims[2] = {128, (uint64_t)h->n_pad};
   const uint64_t strides[1] = {256};
   const uint32_t box[2] = {64, MT_ROWS};
-  int st = h->e.encode(h->tm, 2, dims, strides, box);
-  if (st == AAE_OK && h->num_cyclo > 1 && h->n_up > 0) {
+  AAE_TRY(e.encode(h->tm, 2, dims, strides, box));
+  if (h->num_cyclo > 1 && h->n_up > 0) {
     // `upright` view (codebook.py:66 cos[::num_cyclo]): the same memory from the shard's first upright row on, with a row
     // stride of num_cyclo rows; boxes past the last such row are zero-filled by TMA and masked by the kernel
-    TcPlanes view = h->e;                               // (a view: no ownership, never released)
-    view.hi += h->up_first * 128;
-    if (view.lo) view.lo += h->up_first * 128;
+    TcView up = e;
+    up.hi += h->up_first * 128;
+    if (up.lo) up.lo += h->up_first * 128;
     const uint64_t dims_u[2] = {128, (uint64_t)h->n_up};
     const uint64_t strides_u[1] = {(uint64_t)256 * (uint64_t)h->num_cyclo};
-    st = view.encode(h->tm_up, 2, dims_u, strides_u, box);
-    h->have_up = st == AAE_OK;
+    AAE_TRY(up.encode(h->tm_up, 2, dims_u, strides_u, box));
+    h->have_up = true;
   }
-  if (st != AAE_OK) { tc_codebook_destroy(h); return st; }
   auto attr = [&](const void* fn) { return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, MT_SMEM_TOTAL); };
-  e = with_planes(planes, [&](auto P) {
+  const cudaError_t a = with_planes(planes, [&](auto P) {
     const cudaError_t e1 = attr((const void*)tc_match_kernel<1, P>);
     return e1 == cudaSuccess ? attr((const void*)tc_match_kernel<MT_KMAX, P>) : e1;
   });
-  if (e != cudaSuccess) { set_error("cudaFuncSetAttribute(match kernels) failed: %s", cudaGetErrorString(e)); tc_codebook_destroy(h); return AAE_ERR_CUDA; }
-  *out = h;
+  if (a != cudaSuccess) { set_error("cudaFuncSetAttribute(match kernels) failed: %s", cudaGetErrorString(a)); return AAE_ERR_CUDA; }
+  *out = std::move(h);
   return AAE_OK;
-}
-
-void tc_codebook_destroy(TcCodebook* h) {
-  if (!h) return;
-  h->e.release();
-  cudaFree(h->best); cudaFree(h->lists); cudaFree(h->counter);
-  delete h;
 }
 
 bool tc_codebook_has_upright(const TcCodebook* h) { return h->num_cyclo == 1 || h->have_up; }
@@ -457,7 +452,8 @@ int tc_codebook_match(TcCodebook* h, const float* z_dev, int B, int64_t row_offs
     int32_t* io = idx_out + (size_t)a * k;
     with_planes(h->planes, [&](auto P) {
       auto kern = k == 1 ? tc_match_kernel<1, P> : tc_match_kernel<MT_KMAX, P>;
-      kern<<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(tm.hi, tm.lo, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best, h->lists, h->counter, so, io);
+      kern<<<grid, MT_THREADS, MT_SMEM_TOTAL, s>>>(tm.hi, tm.lo, z, nb, n_rows, n_tiles, idx_mul, (long long)row_offset, k, h->best.get(),
+                                                 h->lists.get(), h->counter.get(), so, io);
     });
     AAE_LAUNCH_OK();
   }

@@ -84,15 +84,25 @@ struct TcMaps {
   CUtensorMap hi, lo;
 };
 
-// An fp16 operand tensor in the plan's format: hi always, lo only for (hi, lo) split operands (planes = 2).
-struct TcPlanes {
+// The planes of an fp16 operand tensor in the plan's format, as the kernels and tensor maps take them: hi always, lo only for
+// (hi, lo) split operands (null otherwise).  Owns nothing.
+struct TcView {
   __half* hi = nullptr;
   __half* lo = nullptr;
-  // n zero-filled elements per plane
-  int alloc(size_t n, int planes);
-  void release();
   // the same map for each plane that exists (make_tmap_f16 arguments)
   int encode(TcMaps& m, int rank, const uint64_t* dims, const uint64_t* strides_bytes, const uint32_t* box, int swizzle_bytes = 128) const;
+};
+static_assert(std::is_trivially_copyable<TcView>::value, "a view is copied freely");
+
+// The owner of an operand's planes.
+struct TcPlanes {
+  DevArray<__half> hi, lo;
+  // n zero-filled elements per plane (planes = 2: hi and lo, 1: hi only)
+  int alloc(size_t n, int planes) {
+    AAE_TRY(hi.alloc_zeroed(n));
+    return planes == 2 ? lo.alloc_zeroed(n) : AAE_OK;
+  }
+  TcView view() const { return {hi.get(), lo.get()}; }
 };
 
 // Runs f(std::integral_constant<int, P>{}) with P = planes (1 or 2): the one place a plan's run-time plane count becomes a kernel's
@@ -117,40 +127,38 @@ struct TcLayer {
 struct TcEncoder {
   int device;
   aae_net_cfg cfg;
-  unsigned* range_flag = nullptr;   // device word, see above
-  bool owns_range_flag = true;      // false once tc_encoder_share_range_flag pointed it at another plan's word
+  DevArray<unsigned> own_range_flag;  // the plan's own guard word, until tc_encoder_share_range_flag drops it
+  unsigned* range_flag = nullptr;     // the device word the kernels write, see above
   std::vector<TcLayer> layers;   // conv layers 1..L-1 followed by the dense layer
   int flat;
-  float* partials = nullptr;     // dense split-K partials [splits, max_batch, latent]
-  float* fwd_partials = nullptr; // conv split-K partials of small-batch forwards [splits, M, N] (allocated on first use)
-  size_t fwd_partial_floats = 0;
+  DevArray<float> partials;      // dense split-K partials [splits, max_batch, latent]
+  DevArray<float> fwd_partials;  // conv split-K partials of small-batch forwards [splits, M, N] (allocated on first use)
   int dense_splits = 1;
-  TcConv1* conv1 = nullptr;      // tensor-core first layer (when the geometry allows), else the fp32 SIMT kernel
+  TcOwner<TcConv1> conv1;        // tensor-core first layer (when the geometry allows), else the fp32 SIMT kernel
   int planes = 2;                // fp16 planes per operand: 2 = (hi, lo) (AAE_PREC_TC_SPLIT), 1 = hi only (AAE_PREC_TC_FP16)
-  float* dbg = nullptr;          // fp32 view of an activation (tests)
-  size_t dbg_floats = 0;
+  DevArray<float> dbg;           // fp32 view of an activation (tests)
 };
 
 
 struct TcDecoder {
   int device;
   aae_net_cfg cfg;
+  DevArray<unsigned> own_range_flag;   // see TcEncoder
   unsigned* range_flag = nullptr;
-  bool owns_range_flag = true;
   std::vector<TcLayer> layers;     // [0] dense_1, [1..L-1] sub-pixel convs, [L] sub-pixel output layer
-  std::vector<float*> bias_dev;    // per sub-pixel conv: bias tiled 4x in GEMM-column order (nullptr for dense_1 and the output layer)
-  float* wm_tmp = nullptr;         // fp32 merged-weight scratch
+  std::vector<DevArray<float>> bias_dev;   // per sub-pixel conv: bias tiled 4x in GEMM-column order (empty for dense_1 and the output layer)
+  DevArray<float> wm_tmp;          // fp32 merged-weight scratch
   // Output layer (Cout <= 3, so that 36 * Cout <= 128) in "tap-separable" form.  P[pixel, (tap, cls, co)] = X[pixel, :] . Wm[tap, :, (cls, co)]
   // is ONE 1x1 GEMM (K = Cin, N = 128) that reads the activation once instead of once per tap; the 3x3 neighbourhood sum,
   // bias, sigmoid and depth-to-space scatter happen in a small gather kernel over P.
   // With the mask head (AUXILIARY_MASK) the head and the output conv read the same input and both end in a sigmoid: they are
   // one output layer of Cout = C + 1 channels (N = 256), channel C being the mask.
-  float* out_p = nullptr;          // [B*h*w (padded to 128 rows)][N] fp32
+  DevArray<float> out_p;           // [B*h*w (padded to 128 rows)][N] fp32
   const float* out_bias = nullptr; // the caller's bias [C] (device)
   int out_x = 0;                   // C: output-layer channels of x (the layer's out_c is C + 1 with the mask head)
   const float* mask_w = nullptr;   // mask head kernel [5,5,Cin,1] and bias [1] (device masters; null without the head)
   const float* mask_b = nullptr;
-  float* cat_tmp = nullptr;        // [5,5,Cin,C+1]: the output conv's kernel joined with the head's along Cout
+  DevArray<float> cat_tmp;         // [5,5,Cin,C+1]: the output conv's kernel joined with the head's along Cout
   size_t wm_floats = 0;
   int planes = 2;                  // fp16 planes per operand: 2 = (hi, lo); 1 = hi only (the single-pass trainer's private plan)
 };
@@ -381,10 +389,9 @@ struct TcTiles {
   int n, m, count;
 };
 
-// launches tc_gemm_kernel over tiles = (M tiles, N tiles, K splits) with min(SM count, tiles) persistent CTAs; planes = 1 runs
-// the single-pass (hi-only) instantiation
-int tc_launch_layer(const TcLayer& T, dim3 tiles, cudaStream_t s, int planes);
-int tc_dev_alloc(void** p, size_t bytes);
+// launches tc_gemm_kernel on T's tensor maps with parameters gp (T.gp, or a split-K variant of it) over tiles = (M tiles,
+// N tiles, K splits) with min(SM count, tiles) persistent CTAs; planes = 1 runs the single-pass (hi-only) instantiation
+int tc_launch_layer(const TcLayer& T, const TcGemmParams& gp, dim3 tiles, cudaStream_t s, int planes);
 // Tensor maps + packed-weight storage of a layer whose A operand is a PLAIN NHWC tensor [B_pad, in_h, in_w, in_c] in `planes`
 // planes (taps = unit-stride boxes): allocates T.in, fills tm_a, allocates T.w [ceil(N / TC_N_TILE) * TC_N_TILE][taps * in_c]
 // and fills tm_w.  T.{in_h,in_w,in_c,taps,BW,BH,BB,gp.N} must be set.

@@ -466,7 +466,7 @@ struct TcUnit {
   bool sep;                 // decoder output layer in tap-separable form: G is the im2col [pixel][(tap, cls, co)] of the loss gradient
   TcLayer dg;               // dgrad GEMM: A = G (dg.in is the G buffer), B = re-packed weights
   int nd;                   // dgrad output columns (decoder: cin, encoder: 4*cin)
-  TcPlanes x;               // the layer's forward input (owned by the encoder / decoder plan, or the plan's c1_x)
+  TcView x;                 // the layer's forward input (held by the encoder / decoder plan, or the plan's c1_x)
   const __half* mask_hi;    // forward activation whose ReLU masks this unit's dgrad result (same layout as the result)
   TcMaps tm_x, tm_g;        // wgrad operand maps (64-channel x 32-pixel boxes)
   TcWgradParams wp;
@@ -480,13 +480,10 @@ struct TcTrainPlan {
   TcDecoder* dec;
   std::vector<TcUnit> units;      // backward order: decoder L..1, encoder L-1..1
   int n_dec;                      // number of decoder units
-  unsigned* amax = nullptr;       // one slot per unit (largest |G|, fp32 bits)
-  float* raw = nullptr;           // fp32 dgrad result of the current unit
-  size_t raw_floats = 0;
-  float* partials = nullptr;      // split-K partials of the wgrad GEMMs
-  size_t partial_floats = 0;
-  float* wm = nullptr;            // fp32 merged sub-pixel weights / padded merged gradient scratch
-  size_t wm_floats = 0;
+  DevArray<unsigned> amax;        // one slot per unit (largest |G|, fp32 bits)
+  DevArray<float> raw;            // fp32 dgrad result of the current unit
+  DevArray<float> partials;       // split-K partials of the wgrad GEMMs
+  DevArray<float> wm;             // fp32 merged sub-pixel weights / padded merged gradient scratch
   // conv1 (Cin = 3): wgrad-only unit appended after the encoder units (index c1): X = im2col of the input image
   int c1 = -1;
   TcPlanes c1_x;
@@ -504,7 +501,7 @@ static int make_wgrad_maps(TcUnit& U, int x_c_total, int x_bpad, int g_bpad) {
     const uint64_t dims[4] = {(uint64_t)U.gN, (uint64_t)U.gw, (uint64_t)U.gh, (uint64_t)g_bpad};
     const uint64_t str[3] = {(uint64_t)U.gN * 2, (uint64_t)U.gw * U.gN * 2, (uint64_t)U.gh * U.gw * U.gN * 2};
     const uint32_t box[4] = {64, (uint32_t)bw, (uint32_t)bh, 1};
-    AAE_TRY(U.dg.in.encode(U.tm_g, 4, dims, str, box));
+    AAE_TRY(U.dg.in.view().encode(U.tm_g, 4, dims, str, box));
   }
   TcWgradParams& w = U.wp;
   memset(&w, 0, sizeof(w));
@@ -521,8 +518,9 @@ static int make_wgrad_maps(TcUnit& U, int x_c_total, int x_bpad, int g_bpad) {
   return AAE_OK;
 }
 
-int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan** out) {
-  *out = nullptr;
+void TcDelete::operator()(TcTrainPlan* h) const { delete h; }
+
+int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcOwner<TcTrainPlan>* out) {
   AAE_REQUIRE(enc && dec, "tensor-core trainer: needs the tensor-core encoder and decoder plans");
   if (!enc->conv1) {
     set_error("tensor-core trainer: conv1 runs on the fp32 kernel for this geometry (the trainer needs the tensor-core conv1: "
@@ -530,14 +528,14 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     return AAE_ERR_UNSUPPORTED;
   }
   AAE_REQUIRE(enc->planes == dec->planes, "tensor-core trainer: the encoder and decoder plans use different operand planes");
-  TcTrainPlan* h = new TcTrainPlan();
+  TcOwner<TcTrainPlan> h(new TcTrainPlan());
   h->device = enc->device; h->max_batch = max_batch; h->enc = enc; h->dec = dec; h->planes = enc->planes;
   const int B = max_batch;
-  int st = AAE_OK;
   const int Ld = (int)dec->layers.size() - 1;       // decoder conv layers 1..Ld
   const int Le = (int)enc->layers.size() - 1;       // encoder TC conv layers (conv2..): enc->layers[0..Le-1]
   size_t raw_max = 0, part_max = 0, wm_max = 0;
-  auto add_unit = [&](TcUnit& U, const TcLayer& F, int x_c_total) -> int {
+  // x: the layer's forward input, x_bb its TMA box batch; taps: the forward GEMM's tap tables (null: one tap at offset 0)
+  auto add_unit = [&](TcUnit& U, TcView x, int x_bb, const TcGemmParams* taps, int x_c_total) -> int {
     TcLayer& T = U.dg;
     memset(&T.gp, 0, sizeof(T.gp));
     T.in_h = U.gh; T.in_w = U.gw; T.in_c = U.gN;
@@ -560,15 +558,15 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     g.unscale = 1.f / W_SCALE;
     g.out_mode = OUT_F32;
     AAE_TRY(tc_layer_setup_plain(T, B, h->planes));
-    U.x = F.in;
-    const int x_bpad = (int)ceil_div(B, F.BB) * F.BB, g_bpad = (int)ceil_div(B, T.BB) * T.BB;
+    U.x = x;
+    const int x_bpad = (int)ceil_div(B, x_bb) * x_bb, g_bpad = (int)ceil_div(B, T.BB) * T.BB;
     AAE_TRY(make_wgrad_maps(U, x_c_total, x_bpad, g_bpad));
-    for (int t = 0; t < U.taps_w; ++t) { U.wp.tap_di[t] = F.gp.tap_di[t]; U.wp.tap_dj[t] = F.gp.tap_dj[t]; U.wp.tap_ch[t] = F.gp.tap_ch[t]; }
+    for (int t = 0; taps && t < U.taps_w; ++t) { U.wp.tap_di[t] = taps->tap_di[t]; U.wp.tap_dj[t] = taps->tap_dj[t]; U.wp.tap_ch[t] = taps->tap_ch[t]; }
     raw_max = std::max(raw_max, (size_t)B * U.gh * U.gw * U.nd);
     wm_max = std::max(wm_max, (size_t)U.taps_w * U.cin * U.gN);
     return AAE_OK;
   };
-  for (int l = Ld; l >= 1 && st == AAE_OK; --l) {          // decoder units
+  for (int l = Ld; l >= 1; --l) {                          // decoder units
     const TcLayer& F = dec->layers[l];
     TcUnit U;
     U.enc = false; U.cin = F.in_c; U.cout = F.out_c; U.cx = l == Ld ? dec->out_x : F.out_c;
@@ -576,65 +574,51 @@ int tc_train_create(TcEncoder* enc, TcDecoder* dec, int max_batch, TcTrainPlan**
     U.sep = l == Ld;
     U.gN = U.sep ? F.gp.N : 4 * F.out_c;           // the tap-separable layer's G has the forward GEMM's 128 or 256 columns
     U.taps_w = U.sep ? 1 : 9; U.dg_taps = U.sep ? 1 : 9; U.nd = F.in_c;
-    U.mask_hi = F.in.hi;                                   // dgrad result = gradient wrt this layer's input activation
-    h->units.push_back(U);
-    st = add_unit(h->units.back(), F, F.in_c);
+    U.mask_hi = F.in.hi.get();                             // dgrad result = gradient wrt this layer's input activation
+    h->units.push_back(std::move(U));
+    AAE_TRY(add_unit(h->units.back(), F.in.view(), F.BB, &F.gp, F.in_c));
   }
   h->n_dec = (int)h->units.size();
-  for (int i = Le - 1; i >= 0 && st == AAE_OK; --i) {      // encoder units (enc->layers[i] = conv i+2)
+  for (int i = Le - 1; i >= 0; --i) {                      // encoder units (enc->layers[i] = conv i+2)
     const TcLayer& F = enc->layers[i];
     TcUnit U;
     U.enc = true; U.cin = F.in_c; U.cout = F.out_c; U.cx = F.out_c;
     U.gh = F.out_h; U.gw = F.out_w; U.gN = F.out_c;
     U.taps_w = 25; U.dg_taps = 9; U.sep = false; U.nd = 4 * F.in_c;
-    U.mask_hi = F.in.hi;                                   // space-to-depth activation, same layout as the dgrad result
-    h->units.push_back(U);
-    st = add_unit(h->units.back(), F, 4 * F.in_c);
+    U.mask_hi = F.in.hi.get();                             // space-to-depth activation, same layout as the dgrad result
+    h->units.push_back(std::move(U));
+    AAE_TRY(add_unit(h->units.back(), F.in.view(), F.BB, &F.gp, 4 * F.in_c));
   }
-  if (st == AAE_OK) {
-    // dW1[75, 128] = sum over pixels of im2col(x)[pixel, :75]^T G1[pixel, :]: the same 1x1 wgrad GEMM as the tap-separable output layer
+  {
+    // dW1[75, 128] = sum over pixels of im2col(x)[pixel, :75]^T G1[pixel, :]: the same 1x1 wgrad GEMM as the tap-separable output
+    // layer, with X = the im2col c1_x (one image per TMA box)
     const TcLayer& F2 = enc->layers[0];                    // conv2: in_h x in_w x in_c are the dims of conv1's output (stored space-to-depth)
-    st = h->c1_x.alloc((size_t)B * F2.in_h * F2.in_w * 128, h->planes);
-    if (st == AAE_OK) {
-      TcLayer Fx;                                          // stands for "the layer whose input is X": only in, BB and the tap tables are read
-      memset(&Fx.gp, 0, sizeof(Fx.gp));
-      Fx.in = h->c1_x; Fx.BB = 1;
-      TcUnit U;
-      U.enc = true; U.cin = 128; U.cout = F2.in_c; U.cx = F2.in_c;
-      U.gh = F2.in_h; U.gw = F2.in_w; U.gN = F2.in_c;
-      U.taps_w = 1; U.dg_taps = 1; U.sep = false; U.nd = 128;   // (no dgrad is ever run for this unit: the input image needs no gradient)
-      U.mask_hi = nullptr;
-      h->units.push_back(U);
-      st = add_unit(h->units.back(), Fx, 128);
-      if (st == AAE_OK) h->c1 = (int)h->units.size() - 1;
-    }
+    AAE_TRY(h->c1_x.alloc((size_t)B * F2.in_h * F2.in_w * 128, h->planes));
+    TcUnit U;
+    U.enc = true; U.cin = 128; U.cout = F2.in_c; U.cx = F2.in_c;
+    U.gh = F2.in_h; U.gw = F2.in_w; U.gN = F2.in_c;
+    U.taps_w = 1; U.dg_taps = 1; U.sep = false; U.nd = 128;   // (no dgrad is ever run for this unit: the input image needs no gradient)
+    U.mask_hi = nullptr;
+    h->units.push_back(std::move(U));
+    AAE_TRY(add_unit(h->units.back(), h->c1_x.view(), 1, nullptr, 128));
+    h->c1 = (int)h->units.size() - 1;
   }
   part_max = (size_t)40 << 20;   // 160 MB of fp32 partials; wgrad split counts are clamped to fit
-  if (st == AAE_OK) st = tc_dev_alloc((void**)&h->amax, 64 * sizeof(unsigned));
-  if (st == AAE_OK) st = tc_dev_alloc((void**)&h->raw, raw_max * sizeof(float));
-  if (st == AAE_OK) st = tc_dev_alloc((void**)&h->partials, part_max * sizeof(float));
-  if (st == AAE_OK) st = tc_dev_alloc((void**)&h->wm, wm_max * sizeof(float));
-  h->raw_floats = raw_max; h->partial_floats = part_max; h->wm_floats = wm_max;
-  if (st != AAE_OK) { tc_train_destroy(h); return st; }
-  *out = h;
+  AAE_TRY(h->amax.alloc_zeroed(64));
+  AAE_TRY(h->raw.alloc_zeroed(raw_max));
+  AAE_TRY(h->partials.alloc_zeroed(part_max));
+  AAE_TRY(h->wm.alloc_zeroed(wm_max));
+  *out = std::move(h);
   return AAE_OK;
-}
-
-void tc_train_destroy(TcTrainPlan* h) {
-  if (!h) return;
-  for (auto& U : h->units) { U.dg.in.release(); U.dg.w.release(); }
-  cudaFree(h->amax); cudaFree(h->raw); cudaFree(h->partials); cudaFree(h->wm);
-  h->c1_x.release();
-  delete h;
 }
 
 int tc_train_num_units(const TcTrainPlan* h) { return (int)h->units.size() - 1; }   // conv units with a dgrad: all but conv1's
 int tc_train_conv1_unit(const TcTrainPlan* h) { return h->c1; }
 int tc_train_num_decoder_units(const TcTrainPlan* h) { return h->n_dec; }
-float* tc_train_raw(TcTrainPlan* h) { return h->raw; }
+float* tc_train_raw(TcTrainPlan* h) { return h->raw.get(); }
 
 int tc_train_begin_step(TcTrainPlan* h, cudaStream_t s) {
-  AAE_CUDA_OK(cudaMemsetAsync(h->amax, 0, 64 * sizeof(unsigned), s));
+  AAE_CUDA_OK(cudaMemsetAsync(h->amax.get(), 0, 64 * sizeof(unsigned), s));
   return AAE_OK;
 }
 
@@ -644,12 +628,12 @@ int tc_train_pack_weights(TcTrainPlan* h, int u, const float* w_dev, cudaStream_
   TcUnit& U = h->units[u];
   if (U.enc) {
     const unsigned grid = ew_grid(4LL * U.cin * 9 * U.cout / 8);
-    with_planes(h->planes, [&](auto P) { pack_enc_dgrad_kernel<P><<<grid, 256, 0, s>>>(w_dev, U.cin, U.cout, W_SCALE, U.dg.w.hi, U.dg.w.lo); });
+    with_planes(h->planes, [&](auto P) { pack_enc_dgrad_kernel<P><<<grid, 256, 0, s>>>(w_dev, U.cin, U.cout, W_SCALE, U.dg.w.hi.get(), U.dg.w.lo.get()); });
     AAE_LAUNCH_OK();
     return AAE_OK;
   }
-  AAE_TRY(launch_merge_subpixel_weights(w_dev, U.cin, U.cout, h->wm, s));
-  return tc_train_pack_weights_merged(h, u, h->wm, s);
+  AAE_TRY(launch_merge_subpixel_weights(w_dev, U.cin, U.cout, h->wm.get(), s));
+  return tc_train_pack_weights_merged(h, u, h->wm.get(), s);
 }
 
 // decoder unit: dgrad operand from the already merged sub-pixel weights Wm [9][cin][4*cout] (device pointer)
@@ -658,8 +642,8 @@ int tc_train_pack_weights_merged(TcTrainPlan* h, int u, const float* wm_dev, cud
   TcUnit& U = h->units[u];
   const unsigned sep_grid = ew_grid((long long)U.cin * U.gN), grid = ew_grid((long long)U.cin * 9 * U.gN);
   with_planes(h->planes, [&](auto P) {
-    if (U.sep) pack_dec_dgrad_sep_kernel<P><<<sep_grid, 256, 0, s>>>(wm_dev, U.cin, 4 * U.cout, U.gN, W_SCALE, U.dg.w.hi, U.dg.w.lo);
-    else pack_dec_dgrad_kernel<P><<<grid, 256, 0, s>>>(wm_dev, U.cin, U.gN, W_SCALE, U.dg.w.hi, U.dg.w.lo);
+    if (U.sep) pack_dec_dgrad_sep_kernel<P><<<sep_grid, 256, 0, s>>>(wm_dev, U.cin, 4 * U.cout, U.gN, W_SCALE, U.dg.w.hi.get(), U.dg.w.lo.get());
+    else pack_dec_dgrad_kernel<P><<<grid, 256, 0, s>>>(wm_dev, U.cin, U.gN, W_SCALE, U.dg.w.hi.get(), U.dg.w.lo.get());
   });
   AAE_LAUNCH_OK();
   return AAE_OK;
@@ -671,16 +655,16 @@ int tc_train_set_loss_grad(TcTrainPlan* h, const float* g_dev, const float* gm_d
   const int c = U.cx, cm = U.cout - U.cx;
   AAE_REQUIRE((gm_dev != nullptr) == (cm == 1), "tc trainer: the mask gradient is required exactly with the mask head");
   const long long n = (long long)B * U.gh * U.gw * 4 * c;
-  amax_scalar_kernel<<<ew_grid(n), 256, 0, s>>>(g_dev, n, h->amax + 0);
+  amax_scalar_kernel<<<ew_grid(n), 256, 0, s>>>(g_dev, n, h->amax.get());
   AAE_LAUNCH_OK();
   if (gm_dev) {      // one scale for the whole G of the joined layer
     const long long nm = (long long)B * U.gh * U.gw * 4;
-    amax_scalar_kernel<<<ew_grid(nm), 256, 0, s>>>(gm_dev, nm, h->amax + 0);
+    amax_scalar_kernel<<<ew_grid(nm), 256, 0, s>>>(gm_dev, nm, h->amax.get());
     AAE_LAUNCH_OK();
   }
   const unsigned grid = ew_grid((long long)B * U.gh * U.gw * 9);
   with_planes(h->planes, [&](auto P) {
-    pack_loss_grad_sep_kernel<P><<<grid, 256, 0, s>>>(g_dev, gm_dev, B, U.gh, U.gw, c, cm, U.gN, h->amax + 0, U.dg.in.hi, U.dg.in.lo);
+    pack_loss_grad_sep_kernel<P><<<grid, 256, 0, s>>>(g_dev, gm_dev, B, U.gh, U.gw, c, cm, U.gN, h->amax.get(), U.dg.in.hi.get(), U.dg.in.lo.get());
   });
   AAE_LAUNCH_OK();
   return AAE_OK;
@@ -690,11 +674,11 @@ int tc_train_set_loss_grad(TcTrainPlan* h, const float* g_dev, const float* gm_d
 int tc_train_set_unit_grad(TcTrainPlan* h, int u, const float* g_dev, int B, cudaStream_t s) {
   TcUnit& U = h->units[u];
   const long long groups = (long long)B * U.gh * U.gw * U.gN / 8;
-  amax_kernel<<<ew_grid(groups), 256, 0, s>>>(g_dev, nullptr, groups, h->amax + u);
+  amax_kernel<<<ew_grid(groups), 256, 0, s>>>(g_dev, nullptr, groups, h->amax.get() + u);
   AAE_LAUNCH_OK();
   with_planes(h->planes, [&](auto P) {
-    finish_kernel<P><<<ew_grid(groups), 256, 0, s>>>(const_cast<float*>(g_dev), nullptr, groups, REMAP_SAME, U.gh, U.gw, U.gN, h->amax + u,
-                                                     U.dg.in.hi, U.dg.in.lo, 0, nullptr, 1);
+    finish_kernel<P><<<ew_grid(groups), 256, 0, s>>>(const_cast<float*>(g_dev), nullptr, groups, REMAP_SAME, U.gh, U.gw, U.gN, h->amax.get() + u,
+                                                     U.dg.in.hi.get(), U.dg.in.lo.get(), 0, nullptr, 1);
   });
   AAE_LAUNCH_OK();
   return AAE_OK;
@@ -709,20 +693,20 @@ int tc_train_unit_wgrad(TcTrainPlan* h, int u, int B, float* dw_out, cudaStream_
   const long long mn = (long long)w.ep.M * w.ep.N;
   int splits = (int)std::max<long long>(1, (396 + (long long)m_tiles * n_tiles / 2) / ((long long)m_tiles * n_tiles));
   splits = std::min(splits, std::max(1, w.total_chunks / 16));
-  splits = (int)std::min<long long>(splits, (long long)(h->partial_floats / (size_t)mn));
+  splits = (int)std::min<long long>(splits, (long long)(h->partials.size() / (size_t)mn));
   AAE_REQUIRE(splits >= 1, "tc trainer: wgrad partial scratch too small");
   w.chunks_per_split = (int)ceil_div(w.total_chunks, splits);
   splits = (int)ceil_div(w.total_chunks, w.chunks_per_split);
-  w.ep.amax_bits = h->amax + u;
-  w.ep.out_f32 = h->partials;
+  w.ep.amax_bits = h->amax.get() + u;
+  w.ep.out_f32 = h->partials.get();
   dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)splits);
   AAE_TRY(with_planes(h->planes, [&](auto P) {
     return U.wg_n_tile == 128 ? launch_wgrad<128, P>(U.tm_x, U.tm_g, w, grid, s) : launch_wgrad<64, P>(U.tm_x, U.tm_g, w, grid, s);
   }));
-  if (!U.sep) return launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, dw_out, s);
-  AAE_REQUIRE((size_t)mn <= h->wm_floats, "tc trainer: merged-gradient scratch too small");
-  AAE_TRY(launch_splitk_reduce(h->partials, splits, mn, w.ep.N, nullptr, ACT_NONE, h->wm, s));
-  rearrange_sep_wgrad_kernel<<<ew_grid(9LL * U.cin * 4 * U.cout), 256, 0, s>>>(h->wm, U.cin, 4 * U.cout, U.gN, dw_out);
+  if (!U.sep) return launch_splitk_reduce(h->partials.get(), splits, mn, w.ep.N, nullptr, ACT_NONE, dw_out, s);
+  AAE_REQUIRE((size_t)mn <= h->wm.size(), "tc trainer: merged-gradient scratch too small");
+  AAE_TRY(launch_splitk_reduce(h->partials.get(), splits, mn, w.ep.N, nullptr, ACT_NONE, h->wm.get(), s));
+  rearrange_sep_wgrad_kernel<<<ew_grid(9LL * U.cin * 4 * U.cout), 256, 0, s>>>(h->wm.get(), U.cin, 4 * U.cout, U.gN, dw_out);
   AAE_LAUNCH_OK();
   return AAE_OK;
 }
@@ -734,13 +718,13 @@ int tc_train_conv1_wgrad(TcTrainPlan* h, const float* x_dev, int B, float* dw_ou
   const long long pixels = (long long)B * U.gh * U.gw;
   const int pad_t = std::max((U.gh - 1) * 2 + 5 - cfg.in_h, 0) / 2, pad_l = std::max((U.gw - 1) * 2 + 5 - cfg.in_w, 0) / 2;
   with_planes(h->planes, [&](auto P) {
-    conv1_im2col_kernel<P><<<ew_grid(pixels * 16), 256, 0, s>>>(x_dev, pixels, cfg.in_h, cfg.in_w, U.gh, U.gw, pad_t, pad_l, ACT_SCALE, h->c1_x.hi,
-                                                                h->c1_x.lo);
+    conv1_im2col_kernel<P><<<ew_grid(pixels * 16), 256, 0, s>>>(x_dev, pixels, cfg.in_h, cfg.in_w, U.gh, U.gw, pad_t, pad_l, ACT_SCALE,
+                                                                h->c1_x.hi.get(), h->c1_x.lo.get());
   });
   AAE_LAUNCH_OK();
-  AAE_REQUIRE((size_t)128 * U.gN <= h->wm_floats, "tc trainer: scratch too small for the conv1 wgrad");
-  AAE_TRY(tc_train_unit_wgrad(h, h->c1, B, h->wm, s));         // [128 im2col columns][cout]; rows 75.. are zero
-  AAE_CUDA_OK(cudaMemcpyAsync(dw_out, h->wm, (size_t)75 * U.gN * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  AAE_REQUIRE((size_t)128 * U.gN <= h->wm.size(), "tc trainer: scratch too small for the conv1 wgrad");
+  AAE_TRY(tc_train_unit_wgrad(h, h->c1, B, h->wm.get(), s));   // [128 im2col columns][cout]; rows 75.. are zero
+  AAE_CUDA_OK(cudaMemcpyAsync(dw_out, h->wm.get(), (size_t)75 * U.gN * sizeof(float), cudaMemcpyDeviceToDevice, s));
   return AAE_OK;
 }
 
@@ -749,7 +733,7 @@ int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s) {
   TcUnit& U = h->units[u];
   TcLayer& T = U.dg;
   T.gp.M = B * U.gh * U.gw;
-  T.gp.amax_bits = h->amax + u;
+  T.gp.amax_bits = h->amax.get() + u;
   const int m_tiles = (int)ceil_div(T.gp.M, 128), n_tiles = U.nd / TC_N_TILE;
   const int total_iters = T.gp.taps * T.gp.chunks_per_tap, total_units = T.gp.groups * T.gp.chunks_per_tap;
   // few output tiles and a long K (the 8x8 layers): split K so that the grid covers the SMs, fold the partials afterwards;
@@ -757,13 +741,13 @@ int tc_train_unit_dgrad(TcTrainPlan* h, int u, int B, cudaStream_t s) {
   int splits = std::max(1, 132 / std::max(1, m_tiles * n_tiles));
   splits = std::min(splits, std::max(1, total_iters / 64));
   const long long mn = (long long)T.gp.M * U.nd;
-  if ((size_t)splits * (size_t)mn > h->partial_floats) splits = 1;
+  if ((size_t)splits * (size_t)mn > h->partials.size()) splits = 1;
   T.gp.units_per_split = (int)ceil_div(total_units, splits);
   splits = (int)ceil_div(total_units, T.gp.units_per_split);
-  T.gp.out_f32 = splits > 1 ? h->partials : h->raw;
+  T.gp.out_f32 = splits > 1 ? h->partials.get() : h->raw.get();
   dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)splits);
-  AAE_TRY(tc_launch_layer(T, grid, s, h->planes));
-  if (splits > 1) AAE_TRY(launch_splitk_reduce(h->partials, splits, mn, U.nd, nullptr, ACT_NONE, h->raw, s));
+  AAE_TRY(tc_launch_layer(T, T.gp, grid, s, h->planes));
+  if (splits > 1) AAE_TRY(launch_splitk_reduce(h->partials.get(), splits, mn, U.nd, nullptr, ACT_NONE, h->raw.get(), s));
   return AAE_OK;
 }
 
@@ -778,8 +762,8 @@ int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, fl
   if (next >= 0) {
     TcUnit& Nx = h->units[next];
     AAE_REQUIRE((long long)Nx.gh * Nx.gw * Nx.gN == (long long)U.gh * U.gw * U.nd, "tc trainer: unit %d does not feed unit %d", u, next);
-    hi = Nx.dg.in.hi; lo = Nx.dg.in.lo; slot = h->amax + next;
-    amax_kernel<<<ew_grid(groups), 256, 0, s>>>(h->raw, U.mask_hi, groups, slot);
+    hi = Nx.dg.in.hi.get(); lo = Nx.dg.in.lo.get(); slot = h->amax.get() + next;
+    amax_kernel<<<ew_grid(groups), 256, 0, s>>>(h->raw.get(), U.mask_hi, groups, slot);
     AAE_LAUNCH_OK();
   }
   const int mode = U.enc ? REMAP_S2D_TO_PLAIN : (next >= 0 ? REMAP_PLAIN_TO_S2D : REMAP_SAME);
@@ -791,11 +775,11 @@ int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, fl
   float* colsum = nullptr;
   if (db_out) {
     AAE_REQUIRE(gpr <= 256 && 256 % gpr == 0, "tc trainer: %d columns unsupported by the fused bias gradient", U.nd);
-    AAE_REQUIRE((size_t)grid * U.nd <= h->partial_floats, "tc trainer: column-sum scratch too small");
-    colsum = h->partials;
+    AAE_REQUIRE((size_t)grid * U.nd <= h->partials.size(), "tc trainer: column-sum scratch too small");
+    colsum = h->partials.get();
   }
   with_planes(h->planes, [&](auto P) {
-    finish_kernel<P><<<grid, 256, 0, s>>>(h->raw, U.mask_hi, groups, mode, U.gh, U.gw, C, slot, hi, lo, keep_masked ? 1 : 0, colsum, std::max(gpr, 1));
+    finish_kernel<P><<<grid, 256, 0, s>>>(h->raw.get(), U.mask_hi, groups, mode, U.gh, U.gw, C, slot, hi, lo, keep_masked ? 1 : 0, colsum, std::max(gpr, 1));
   });
   AAE_LAUNCH_OK();
   if (db_out) {
@@ -809,7 +793,7 @@ int tc_train_finish(TcTrainPlan* h, int u, int next, int B, bool keep_masked, fl
 int tc_train_unpack_flat(TcTrainPlan* h, int B, float* out, cudaStream_t s) {
   const TcLayer& D = h->enc->layers.back();
   const long long n = (long long)B * D.in_c;
-  with_planes(h->planes, [&](auto P) { unpack_plain_kernel<P><<<ew_grid(n), 256, 0, s>>>(D.in.hi, D.in.lo, n, 1.f / ACT_SCALE, out); });
+  with_planes(h->planes, [&](auto P) { unpack_plain_kernel<P><<<ew_grid(n), 256, 0, s>>>(D.in.hi.get(), D.in.lo.get(), n, 1.f / ACT_SCALE, out); });
   AAE_LAUNCH_OK();
   return AAE_OK;
 }

@@ -26,8 +26,9 @@ LAUNCH_ALLOW = {
 # (file, function) -> why it may call one of LEGACY_CALLS
 CALL_ALLOW = {
     ("common.cuh", "creation_fence"): "the device-wide wait every creator ends with",
-    ("capi.cu", "DevBuf::alloc"): "allocation, by creators and by scratch that appears on first use; no fill",
-    ("capi.cu", "DevBuf::release"): "destroyers, and alloc() replacing a buffer",
+    ("common.cuh", "DevArray::replace"): "the one cudaMalloc: by creators, and by scratch that appears or grows on first use",
+    ("common.cuh", "DevArray::reset"): "the one cudaFree: owners going away or being replaced",
+    ("common.cuh", "DevArray::alloc_zeroed"): "zero-filled allocation for creators only (they end in creation_fence)",
     ("capi.cu", "aae_encoder_create"): "creator: zero masters; ends in creation_fence",
     ("capi.cu", "aae_encoder_enable_sigma_head"): "creator: zero head; ends in creation_fence",
     ("capi.cu", "aae_codebook_create"): "creator: uploads the embedding; ends in creation_fence",
@@ -36,16 +37,7 @@ CALL_ALLOW = {
     ("capi.cu", "fill_slot"): "trainer creation: initial optimizer slots; trainer_create ends in creation_fence",
     ("capi.cu", "make_pg"): "trainer creation: zero gradients; trainer_create ends in creation_fence",
     ("capi.cu", "aae_encoder_activation"): "takes no stream: waits for the device, documented in the header",
-    ("tc_gemm.cu", "tc_dev_alloc"): "zero-filled allocation for creators only (they end in creation_fence)",
-    ("tc_gemm.cu", "scratch_grow"): "scratch growing on first use at a size: fill on the caller's stream; documented not asynchronous",
-    ("tc_gemm.cu", "TcPlanes::release"): "destroyer",
-    ("tc_gemm.cu", "tc_encoder_destroy"): "destroyer",
-    ("tc_gemm.cu", "tc_decoder_destroy"): "destroyer",
-    ("tc_gemm.cu", "tc_encoder_share_range_flag"): "trainer creation: drops the private plan's own guard word",
-    ("tc_gemm.cu", "tc_decoder_share_range_flag"): "trainer creation: drops the private plan's own guard word",
-    ("tc_train.cu", "tc_train_destroy"): "destroyer",
-    ("tc_match.cu", "tc_codebook_create"): "creator: allocates, fills and waits for the device",
-    ("tc_match.cu", "tc_codebook_destroy"): "destroyer",
+    ("tc_match.cu", "tc_codebook_create"): "creator: packs the codebook and waits for the device",
 }
 
 
